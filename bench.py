@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- the headline measurement of BASELINE.json.
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload NAME]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload NAME] [--dump-outputs DIR]
 
 A "step" is one pass of the hot path over one batch of synthetic input: the NF4
 ``Linear4bit`` forward (fused 4-bit dequant GEMM) at a Llama-3-8B linear shape with
@@ -29,6 +29,10 @@ The default line also carries
 ``--workload blockwise_c1`` / ``int8_c3`` / ``sharded70b`` / ``llama8b`` print those as stand-alone lines;
 ``--workload optim_f4`` times the optimizer updates of SURVEY.md section 8 row f-4 (not a BASELINE config).
 ``--no-secondary`` skips them.
+
+``--dump-outputs DIR`` (the c2_* workloads; others reject it) writes, after the timed steps, what the last timed step returned:
+DIR/y_rows.npy (float32, 256 seeded rows of the [M, N] output) and DIR/y_row_index.npy (float64, their indices).
+The inputs depend only on the arguments (seeded), so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -53,7 +57,7 @@ WORKLOADS = {
     "c2_4096x4096_m1": (4096, 4096, 1, "nf4", False),
 }
 DEFAULT_WORKLOAD = "c2_4096x4096_m4096"
-L2_BYTES = 126 * 1024 * 1024
+L2_BYTES = 50 * 1024 * 1024  # H100 SXM
 
 
 def parse_args():
@@ -66,6 +70,8 @@ def parse_args():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-secondary", action="store_true")
     ap.add_argument("--layers", type=int, default=32, help="llama8b workload: number of decoder layers")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write a seeded sample of the last timed step's output to DIR/*.npy")
     return ap.parse_args()
 
 
@@ -292,6 +298,20 @@ def secondary_results(dev, args, N, K, M, qt, nested, with_cpu):
     return ref_cuda, sec
 
 
+# ------------------------------------------------------------------------------------------ output dump
+def dump_outputs(out_dir, y, rows=256):
+    """The last timed step's output, a fixed seeded sample of its rows, as float32 (and the row indices)."""
+    import numpy as np
+    import torch
+
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    idx = np.sort(np.random.default_rng(0).choice(y.shape[0], size=min(rows, y.shape[0]), replace=False))
+    sample = y[torch.from_numpy(idx).to(y.device)].float().cpu().numpy()
+    np.save(d / "y_rows.npy", sample)
+    np.save(d / "y_row_index.npy", idx.astype(np.float64))
+
+
 # ------------------------------------------------------------------------------------------ main
 def _protect_stdout():
     """Native libraries (NCCL's version banner, cuBLAS warnings) write to file descriptor 1; the
@@ -305,6 +325,8 @@ def _protect_stdout():
 
 def main():
     args = parse_args()
+    if args.dump_outputs and (args.workload not in WORKLOADS or args.impl != "ours"):
+        raise SystemExit(f"--dump-outputs is supported for --impl ours on the {', '.join(WORKLOADS)} workloads only")
     _protect_stdout()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -404,7 +426,7 @@ def main():
     # replay's stream, barrier + synchronize on both sides): the K launches run back to back on the device and the
     # per-rank Python / ctypes launch path (5-10 us of jitter per step, which the 8-GPU max-over-ranks time of a
     # 3 ms region otherwise pays) stays outside.  Falls back to an eager loop if capture is not possible.
-    graph, side = None, torch.cuda.Stream()
+    graph, side, last = None, torch.cuda.Stream(), None
     try:
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
@@ -414,7 +436,7 @@ def main():
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph, stream=side):
             for i in range(args.steps):
-                step(i)
+                last = step(i)
         graph.replay()  # one untimed replay: graph upload + allocator warm-up
     except Exception as exc:  # noqa: BLE001
         print(f"[bench] CUDA-graph capture of the timed steps failed ({exc!r}); timing an eager loop", file=sys.stderr)
@@ -428,7 +450,7 @@ def main():
             graph.replay()
         else:
             for i in range(args.steps):
-                step(i)
+                last = step(i)
         e_end.record()
         barrier()
         t_wall = time.perf_counter() - t_wall
@@ -446,6 +468,8 @@ def main():
             print(f"[bench] clock-sampling continuation stopped: {exc!r}", file=sys.stderr)
         clock_extra_steps = j
     total_ms = e_start.elapsed_time(e_end)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
     kernel_ms = total_ms / args.steps  # one kernel per step, launched back to back: the average launch duration
     t = torch.tensor([total_ms], device=dev, dtype=torch.float64)
     if dist is not None:
@@ -533,17 +557,9 @@ def main():
         peak = peaks["bf16_tflops_sustained"] if long_loop else peaks["bf16_tflops"]
         peak_src = "MEASURED_PEAKS.json " + ("bf16_tflops_sustained" if long_loop else "bf16_tflops (burst)")
     else:
-        peak, peak_src = 1590.0, "fallback (B200_PROFILING.md)"
+        peak, peak_src = 989.0, "H100 SXM data sheet, dense bf16 (not a measured peak)"
     achieved = flops / (kernel_ms * 1e-3) / 1e12
-    traffic, traffic_src, kernel_name = None, None, "gemm4_pair_kernel<bf16, NF4> (cta_group::2)" if M >= 512 else "gemm4_tc_kernel<bf16, NF4>"
-    try:
-        prof = json.loads((ROOT / "profiles" / "summary.json").read_text())
-        ent = prof.get(args.workload, {})
-        traffic = ent.get("dram_bytes_per_launch")
-        traffic_src = ent.get("source")
-        kernel_name = ent.get("kernel", kernel_name)
-    except Exception:
-        pass
+    traffic, traffic_src, kernel_name = None, None, "gemm4_tc_kernel<bf16, NF4> (wgmma)"
     roofline = {"bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
                 "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src, "kernel": kernel_name,
                 "kernel_ms": kernel_ms}
@@ -570,7 +586,7 @@ def main():
         "config": {"workload": args.workload, "N": N, "K": K, "M_per_gpu": M, "global_tokens": M * world,
                    "quant_type": qt, "blocksize": 64, "double_quant": nested,
                    "parallelism": f"token-sharded replicas x{world} (no data-path collective)",
-                   "l2": f"rotating {R} buffer sets ({R * layer_bytes / 2**20:.0f} MiB > 126 MiB L2)"},
+                   "l2": f"rotating {R} buffer sets ({R * layer_bytes / 2**20:.0f} MiB > {L2_BYTES >> 20} MiB L2)"},
         "tokens_per_s": world * M * args.steps / (total_ms_max * 1e-3),
         "e2e": {"value": e2e_value, "unit": "TFLOPS", "h2d_bytes_per_step": 2 * M * K, "d2h_bytes_per_step": 2 * M * N,
                 "api": "bitsandbytes_b200.nn.Linear4bit.forward on pinned-host activations, 3-stage stream pipeline"},

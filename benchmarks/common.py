@@ -5,7 +5,7 @@ import json
 from pathlib import Path
 
 ROOT = Path(__file__).resolve().parent.parent
-L2_BYTES = 126 * 1024 * 1024
+L2_BYTES = 50 * 1024 * 1024  # H100 SXM
 
 
 def peaks():
@@ -19,7 +19,7 @@ def hbm_peak():
     p = peaks()
     if "hbm_gbs" in p:
         return float(p["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs"
-    return 7700.0, "B200_PROFILING.md fallback (nominal HBM3e)"
+    return 3350.0, "H100 SXM data sheet HBM3 bandwidth (not a measured peak)"
 
 
 def bf16_peak(sustained=False):
@@ -27,7 +27,7 @@ def bf16_peak(sustained=False):
     key = "bf16_tflops_sustained" if sustained else "bf16_tflops"
     if key in p:
         return float(p[key]), f"MEASURED_PEAKS.json {key}" + ("" if sustained else " (burst)")
-    return 1590.0, "fallback (B200_PROFILING.md)"
+    return 989.0, "H100 SXM data sheet, dense bf16 (not a measured peak)"
 
 
 def sets_for(bytes_per_set: int, minimum: int = 2) -> int:

@@ -10,8 +10,8 @@ prints as its own line (``--workload NAME``) and also folds into the default lin
 Every figure is device-timed (CUDA events around a CUDA-graph replay of back-to-back launches over rotating
 buffer sets larger than L2; see common.time_us).  ``ref_cuda`` numbers are the REFERENCE's own CUDA library,
 built from its sources into oracle/_ref (same C ABI), driven on the same buffers in the same process along
-the route the reference takes on sm_100 (reference backends/cuda/ops.py:617-623: fused kernel for M <= 4,
-dequantize + cuBLAS otherwise).  This is top-level bench code; the product package never imports oracle/.
+the route the reference takes on this GPU (reference_uses_fused: its sm_90 rule, fused kernel or dequantize +
+cuBLAS).  This is top-level bench code; the product package never imports oracle/.
 """
 from __future__ import annotations
 
@@ -46,14 +46,46 @@ def _p(t):
 
 
 def reference_uses_fused(M, N, K):
-    """reference backends/cuda/ops.py:_gemm_4bit_use_custom_cuda on sm_100, 148 SMs"""
+    """Whether the reference takes its fused kernel (True) or dequantise + cuBLAS (False) for a 16-bit GEMM on this
+    device: its backends/cuda/ops.py:_gemm_4bit_use_custom_cuda for sm_90 (the H100 branch, ops.py:600-603,
+    629-680, 745-755), with the SM count read from the device, and its M <= 1536 cap (ops.py:926)."""
+    import torch
+
     if M <= 4:
         return True
+    if M > 1536:
+        return False
+    num_sms = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
     n_blocks = (N + 63) // 64
-    if n_blocks >= 148 * 3:
+    if N * K < 4 * 1024 * 1024:  # small weights
+        if K * 2 < N:
+            return M <= (512 if n_blocks * 3 < num_sms else 320)
+        if n_blocks * 4 <= num_sms:
+            return M <= 32
+        if n_blocks * 2 <= num_sms:
+            return M <= 16
+        return False
+    if M > 512:
+        return False
+    if M < 8:
+        if M >= 6 and n_blocks >= 36:
+            lt_75 = n_blocks * 4 < num_sms * 3
+            lt_60 = n_blocks * 5 < num_sms * 3
+            if K > N and lt_75:
+                return False
+            if K == N and lt_75 and not lt_60:
+                return False
+        return True
+    if n_blocks >= num_sms * 3:
+        return M <= 64
+    if n_blocks >= num_sms * 2:
+        return M <= 48
+    if n_blocks >= num_sms:
         return M <= 32
-    if n_blocks >= 148:
-        return False if K >= N else M <= 8
+    if n_blocks >= num_sms // 2:
+        if K >= N and n_blocks * 4 < num_sms * 3:
+            return False
+        return M <= 16
     return False
 
 
@@ -234,7 +266,7 @@ def measure_int8_c3(dev, steps=40):
     layer.load_state_dict(lin.state_dict())
     layer = layer.to(dev).eval()  # quantises the weight to int8 + SCB on the move to the device
     outlier_cols = torch.randint(0, K, (5,), generator=torch.Generator().manual_seed(1)).tolist()
-    sets = 3  # activations 32 MiB + outputs 86 MiB per set: 3 sets exceed the 126 MiB L2
+    sets = 3  # activations 32 MiB + outputs 86 MiB per set: 3 sets exceed the 50 MiB L2
     xs = []
     for _ in range(sets):
         x = torch.randn(M, K, device=dev, dtype=torch.float16)
@@ -286,7 +318,7 @@ def run_blockwise_c1(args, rank, world, local_rank, cpu_baseline=None):
             "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": head["us"] * 1e-3, "higher_is_better": True,
             "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic (randn, seed 0)",
             "config": {"workload": "blockwise_c1", "elements": 4 * 1024 * 1024, "blocksizes": [4096, 256],
-                       "l2": "rotating buffer sets larger than the 126 MiB L2"},
+                       "l2": "rotating buffer sets larger than the 50 MiB L2"},
             "results": r["results"],
             "roofline": {"bound": "hbm", "achieved": head["gb_per_s"], "peak": r["peak_gb_per_s"], "unit": "GB/s",
                          "frac": head["gb_per_s"] / r["peak_gb_per_s"], "traffic": None, "peak_source": r["peak_source"],

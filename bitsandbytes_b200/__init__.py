@@ -1,4 +1,4 @@
-"""bitsandbytes_b200 -- a B200-native (sm_100a) implementation of the bitsandbytes
+"""bitsandbytes_b200 -- an H100-native (sm_90a) implementation of the bitsandbytes
 quantized-linear hot path: NF4/FP4 4-bit dequant-fused GEMM, LLM.int8() and blockwise
 quantize/dequantize, behind the ``bnb.functional`` / ``bnb.nn`` API surface.
 

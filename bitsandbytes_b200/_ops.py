@@ -6,7 +6,7 @@ ours: one table drives the definitions, and the shape functions ("fake" kernels)
 written once per op below.  The optimizer ops (:409-510) are SURVEY.md section 8 row f-4.
 
 The only device with kernels is CUDA (``backends/cuda.py``): the reference's
-cpu/default/triton/xpu/mps/hpu fan-out collapses to the single sm_100a path and there is
+cpu/default/triton/xpu/mps/hpu fan-out collapses to the single sm_90a path and there is
 no CPU fallback -- calling an op on a CPU tensor raises NotImplementedError from the
 dispatcher.
 """

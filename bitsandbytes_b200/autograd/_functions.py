@@ -2,7 +2,7 @@
 
 Same contract as the reference's ``bitsandbytes/autograd/_functions.py`` (MatmulLtState
 :57-98, MatMul8bitLt :101-242, MatMul4Bit :300-386, matmul :389-404, matmul_4bit :407-491).
-Forward paths run the sm_100a kernels; the backward formulas are the reference's
+Forward paths run the sm_90a kernels; the backward formulas are the reference's
 (grad_A = grad_out . dequant(W); the int8 weight-gradient path uses int8_double_quant).
 The CPU/XPU-only ``MatMul8bitFp`` of the reference is not provided.
 """

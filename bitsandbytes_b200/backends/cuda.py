@@ -1,15 +1,15 @@
-"""Host side of the sm_100a kernels: argument checking, output allocation, the ctypes call.
+"""Host side of the sm_90a kernels: argument checking, output allocation, the ctypes call.
 
 Plays the role of the reference's ``bitsandbytes/backends/cuda/ops.py`` (:78-982) for the
 hot path, with three structural differences:
 
 * no per-architecture heuristic (reference :583-811) and no dequantize + cuBLAS fallback
-  (:904-916): ``gemm_4bit`` always runs a fused kernel -- tcgen05 for 16-bit activations,
+  (:904-916): ``gemm_4bit`` always runs a fused kernel -- wgmma for 16-bit activations,
   CUDA cores for fp32 / odd shapes; the choice is made inside the library;
 * ``int8_vectorwise_quant`` finds outlier columns inside the quantisation kernel instead
   of three torch kernels and a host sync (reference :230-236); the data-dependent
   ``outlier_cols`` tensor still has to be materialised (``nonzero``), once;
-* ``int8_scaled_mm`` / ``int8_mixed_scaled_mm`` use the int8 tcgen05 GEMM with the
+* ``int8_scaled_mm`` / ``int8_mixed_scaled_mm`` use the int8 wgmma GEMM with the
   dequantisation fused into its epilogue (the reference chains cuBLASLt -> int32 in HBM ->
   an elementwise kernel, backends/default/ops.py:64-119).
 
@@ -220,7 +220,7 @@ def gemm_4bit_multi_out(A, B, shapeB, absmax, blocksize: int, quant_type: str, b
                         absmax_offset, out_ptrs, ldc: int) -> bool:
     """Fused GEMM + all-gather: every output element is stored to each raw device address in
     ``out_ptrs`` (local buffer first, then the peers' -- symmetric memory / CUDA IPC mappings), row
-    stride ``ldc`` elements.  Returns False when the shape does not take the tcgen05 kernel (the caller
+    stride ``ldc`` elements.  Returns False when the shape does not take the wgmma kernel (the caller
     falls back to a local output + a collective)."""
     N, K = shapeB
     M = A.numel() // K
@@ -469,7 +469,7 @@ def _int8_scaled_mm(A, B, row_stats, col_stats, bias=None, dtype=None):
 
 def _fused_mixed_mm(A, CA, CB, SCA, SCB, outlier_cols, bias):
     """The whole LLM.int8() decomposition in two launches: one gathers subA and dequantises the outlier weight
-    columns into [N, jpad], the other is the int8 tcgen05 GEMM whose epilogue adds the outlier term.
+    columns into [N, jpad], the other is the int8 wgmma GEMM whose epilogue adds the outlier term.
     Returns (out, subA) or None when the shape is not served (K % 16, > 64 outlier columns, dtype)."""
     dtype = A.dtype
     if dtype not in (torch.float16, torch.bfloat16) or CA.dtype != torch.int8 or CB.dtype != torch.int8:

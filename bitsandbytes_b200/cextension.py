@@ -3,7 +3,7 @@
 Mirrors the role of the reference's ``bitsandbytes/cextension.py`` (reference
 cextension.py:22-80 library selection, :90-115 ``BNBNativeLibrary``, :392-405 deferred
 error on load failure) with the multi-backend selection collapsed to the single
-sm_100a build: ``libbitsandbytes_b200.so`` next to this file.
+sm_90a build: ``libbitsandbytes_b200.so`` next to this file.
 
 There is no CPU fallback and no mock that silently succeeds: if the library is missing
 or a symbol cannot be resolved, the first native call raises ``RuntimeError`` naming the
@@ -50,7 +50,7 @@ def _signatures():
     sig["cdequant_mm_int32_fp16"] = ([_VOIDP] * 5 + [_I32, _I32, _VOIDP], None)
     # (A, out, rowStats, threshold, rows, cols, stream)
     sig["cint8_vector_quant"] = ([_VOIDP] * 3 + [ct.c_float, _I32, _I32, _VOIDP], None)
-    # ---- B200-native additions
+    # ---- native additions
     sig["cbnb_b200_last_error"] = ([], _I32)
     sig["cbnb_b200_last_error_message"] = ([], ct.c_char_p)
     sig["cbnb_b200_build_info"] = ([], ct.c_char_p)

@@ -1,4 +1,4 @@
-// blockwise.cu -- blockwise quantize / dequantize for sm_100a (HBM-roofline kernels).
+// blockwise.cu -- blockwise quantize / dequantize for sm_90a (HBM-roofline kernels).
 //
 // Replaces the reference's kQuantizeBlockwise / kQuantizeBlockwiseSmall /
 // kDequantizeBlockwise (reference csrc/kernels.cu:269-529, launchers csrc/ops.cu:36-94).

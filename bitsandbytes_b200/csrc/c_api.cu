@@ -3,7 +3,7 @@
 // Mirrors the shape of the reference's csrc/pythonInterface.cpp (un-mangled wrappers over
 // templated launchers); see include/bitsandbytes_b200.h for the per-symbol citations.
 #include "common.cuh"
-#include "sm100_ptx.cuh"
+#include "hopper_ptx.cuh"
 
 #include <cstdio>
 #include <cstdlib>
@@ -45,12 +45,7 @@ template <typename T>
 bool launch_gemm4_tc(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
                      const float* absmax_code, const float* absmax_offset, T* out, const T* bias, int M, int N, int K,
                      int ldc, int blocksize, int quant_type, cudaStream_t stream, void* const* peers = nullptr,
-                     int n_peers = 0);
-template <typename T>
-bool launch_gemm4_pair(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
-                       const float* absmax_code, const float* absmax_offset, T* out, const T* bias, int M, int N, int K,
-                       int ldc, int blocksize, int quant_type, cudaStream_t stream, void* const* peers, int n_peers,
-                       int mt_override, int force_splits, long long* trace);
+                     int n_peers = 0, int mt_override = 0, int force_splits = 0);
 void launch_int8_vector_quant(const void* A, int8_t* out, float* rowStats, int* col_flags, float threshold, int rows,
                               int cols, int dtype, cudaStream_t stream);
 void launch_dequant_mm_int32_fp16(const int* A, const float* rowStats, const float* colStats, __half* out,
@@ -92,10 +87,10 @@ void set_last_error_msg(const char* msg) {
 int device_sm_count() {
     static int cached[64] = {0};
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return kNumSMsB200;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return kNumSMsH100;
     if (cached[dev] == 0) {
         int v = 0;
-        if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = kNumSMsB200;
+        if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = kNumSMsH100;
         cached[dev] = v;
     }
     return cached[dev];
@@ -145,12 +140,12 @@ bool encode_tmap_2d(CUtensorMap* out, const void* base, int elem_bytes, int swiz
 }
 
 // ---------------------------------------------------------------- 4-bit GEMM dispatch
-// path: 0 = CUDA-core GEMV, 1 = tcgen05 GEMM, 2 = CUDA-core generic, 3 = mma.sync decode kernel (M <= 8)
+// path: 0 = CUDA-core GEMV, 1 = wgmma GEMM, 2 = CUDA-core generic, 3 = mma.sync decode kernel (M <= 8)
 static int simt_max_m() {
     static int v = -2;
     if (v == -2) {
         const char* e = getenv("BNB_B200_SIMT_MAX_M");
-        v = e ? atoi(e) : 1;  // measured on B200: the CUDA-core GEMV wins only at M == 1 (9.8 vs 14.5 us at 4096^2)
+        v = e ? atoi(e) : 1;  // the CUDA-core GEMV serves a single token
     }
     return v;
 }
@@ -182,8 +177,8 @@ static int choose_path(int M, int N, int K, int blocksize, int dtype) {
     }
     if (!tc_shape_ok(M, N, K, blocksize, dtype)) return 2;
     if (M <= simt_max_m()) return 0;
-    // 5..8 tokens against a large weight: the tcgen05 kernel (decode cost independent of M) is level with or ahead
-    // of the mma.sync decode kernel (measured on B200, 14336 x 4096: 24.8 us against 29.2 at M = 8)
+    // 5..8 tokens against a large weight: the tensor-core GEMM (decode cost independent of M) takes over from the
+    // mma.sync decode kernel
     if (M <= mma_max_m() && (M <= 4 || (long long)N * K <= 2LL * 4096 * 4096)) return 3;
     return 1;
 }
@@ -328,10 +323,10 @@ void cbnb_b200_gemm_4bit_strided(const void* A, const uint8_t* B, const float* a
         set_last_error_msg("gemm_4bit_strided: bad dtype");
 }
 
-// Fused all-gather: the tcgen05 kernel's epilogue stores every output element to outs[0..n_outs)
+// Fused all-gather: the tensor-core kernel's epilogue stores every output element to outs[0..n_outs)
 // (outs[0] = the local buffer, the rest = the same location in the peer GPUs' buffers, mapped into
 // this process -- CUDA IPC / symmetric memory).  Returns 0, or 100 when the shape does not take
-// the tcgen05 path (the caller then falls back to local output + a collective).
+// the tensor-core path (the caller then falls back to local output + a collective).
 int cbnb_b200_gemm_4bit_multi_out(const void* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
                                   const float* absmax_code, const float* absmax_offset, void* const* outs, int n_outs,
                                   const void* bias, int M, int N, int K, int ldc, int blocksize, int quant_type,
@@ -354,24 +349,24 @@ int cbnb_b200_gemm_4bit_multi_out(const void* A, const uint8_t* B, const float* 
     return ok ? 0 : 100;
 }
 
-// Developer / test entry: the CTA-pair kernel of gemm4_pair.cu with an explicit token tile (mt = 128 | 256 |
-// 384, 0 = automatic), a forced K split (0 = the production rule, s = every tile split s ways, 100 + s = only
-// the partial last wave) and an optional event trace (device buffer of 2 * 10 * 256 + 4 * 1024 int64: clock values of
-// cluster 0, then {start ns, end ns, SM, prologue cycles} per cluster; NULL = the production build).  Returns 0, or 100 when the shape is not served by that kernel.
+// Developer / test entry: the tensor-core kernel of gemm4_tc.cu with an explicit token tile (mt = 16 | 32 | 64 |
+// 128, 0 = automatic) and a forced K split per tile (0 = the production rule).  `trace` must be NULL.  Returns 0, or
+// 100 when the shape or the options are not served by that kernel.
 int cbnb_b200_gemm_4bit_pair(const void* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
                              const float* absmax_code, const float* absmax_offset, void* out, const void* bias, int M,
                              int N, int K, int ldc, int blocksize, int quant_type, int dtype, int mt, int force_splits,
                              long long* trace, cudaStream_t stream) {
     if (M <= 0 || N <= 0) return 0;
+    if (trace != nullptr || force_splits < 0) return 100;
     bool ok = false;
     if (dtype == 1)
-        ok = launch_gemm4_pair<__half>((const __half*)A, B, absmax, absmax_8bit, absmax_code, absmax_offset,
-                                       (__half*)out, (const __half*)bias, M, N, K, ldc, blocksize, quant_type, stream,
-                                       nullptr, 0, mt, force_splits, trace);
+        ok = launch_gemm4_tc<__half>((const __half*)A, B, absmax, absmax_8bit, absmax_code, absmax_offset,
+                                     (__half*)out, (const __half*)bias, M, N, K, ldc, blocksize, quant_type, stream,
+                                     nullptr, 0, mt, force_splits);
     else if (dtype == 2)
-        ok = launch_gemm4_pair<__nv_bfloat16>((const __nv_bfloat16*)A, B, absmax, absmax_8bit, absmax_code,
-                                              absmax_offset, (__nv_bfloat16*)out, (const __nv_bfloat16*)bias, M, N, K,
-                                              ldc, blocksize, quant_type, stream, nullptr, 0, mt, force_splits, trace);
+        ok = launch_gemm4_tc<__nv_bfloat16>((const __nv_bfloat16*)A, B, absmax, absmax_8bit, absmax_code,
+                                            absmax_offset, (__nv_bfloat16*)out, (const __nv_bfloat16*)bias, M, N, K,
+                                            ldc, blocksize, quant_type, stream, nullptr, 0, mt, force_splits);
     return ok ? 0 : 100;
 }
 
@@ -496,7 +491,7 @@ int cbnb_b200_last_error(void) {
 const char* cbnb_b200_last_error_message(void) { return g_err_msg; }
 
 const char* cbnb_b200_build_info(void) {
-    return "bitsandbytes_b200: sm_100a; tcgen05 kind::f16 (A from TMEM) + kind::i8; TMA 128B-swizzle; CUDA " BNB200_STR(
+    return "bitsandbytes_b200: sm_90a; wgmma f16/bf16 (A from registers) + s8; TMA 128B-swizzle; CUDA " BNB200_STR(
         __CUDACC_VER_MAJOR__) "." BNB200_STR(__CUDACC_VER_MINOR__);
 }
 

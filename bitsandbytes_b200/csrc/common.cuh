@@ -1,4 +1,4 @@
-// common.cuh -- shared device helpers for the sm_100a kernels.
+// common.cuh -- shared device helpers for the sm_90a kernels.
 //
 // Numeric contract notes (see DESIGN.md "Numerics"):
 //  * The reference CUDA library is compiled with --use_fast_math
@@ -20,7 +20,7 @@ enum QuantType : int { kGeneral8bit = 0, kFP4 = 1, kNF4 = 2 };
 // kernel-internal variant of kGeneral8bit: the same codes through the cheaper search (blockwise.cu)
 constexpr int kGeneral8bitFast = 3;
 
-constexpr int kNumSMsB200 = 148;
+constexpr int kNumSMsH100 = 132;  // H100 SXM; the launchers ask the device
 
 // ---------------------------------------------------------------- PTX-exact fp32 ops
 __device__ __forceinline__ float mul_ftz(float a, float b) {

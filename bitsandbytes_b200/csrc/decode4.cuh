@@ -1,4 +1,4 @@
-// decode4.cuh -- register-resident 4-bit -> 16-bit decode shared by the tcgen05 GEMM and the
+// decode4.cuh -- register-resident 4-bit -> 16-bit decode shared by the wgmma GEMM and the
 // CUDA-core GEMV, plus the (optionally double-quantised) scale fetch.
 #pragma once
 
@@ -22,7 +22,7 @@ struct ScaleSrc {
 
 // NOTE on the nested (double-quant) scale: the reference has two behaviours.  Its fused
 // kernels write `code[q] * absmax2 + offset`, which nvcc contracts to one fma
-// (gemm_4bit_sm80.cu:292-297); its dequantize + F.linear path -- the one B200 takes for
+// (gemm_4bit_sm80.cu:292-297); its dequantize + F.linear path -- the one the reference takes for
 // M > 4 (backends/cuda/ops.py:617-623, 904-916) and the one F.dequantize_4bit exposes --
 // rounds the product and the sum separately.  We follow the second (mul, then add), so the
 // fused GEMM sees exactly the weights F.dequantize_4bit returns.

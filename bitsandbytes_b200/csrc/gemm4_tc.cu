@@ -1,44 +1,36 @@
-// gemm4_tc.cu -- NF4/FP4 dequant-fused GEMM on tcgen05 tensor cores (sm_100a).
+// gemm4_tc.cu -- NF4/FP4 dequant-fused GEMM on Hopper warpgroup tensor cores (wgmma, sm_90a).
 //
 // Replaces the reference's mma.sync kernel gemm_4bit_sm80_m16n8k16 (reference
-// csrc/gemm_4bit_sm80.cu:127-457) and, on B200, the dequantize + cuBLAS fallback the
-// reference actually takes for M > 4 (reference bitsandbytes/backends/cuda/ops.py:617-623,
-// 904-916).  Contract (reference _ops.py:239-295, gemm_4bit_mma.cuh:99-101):
+// csrc/gemm_4bit_sm80.cu:127-457) and the dequantize + cuBLAS fallback the reference takes for
+// M > 4 (reference bitsandbytes/backends/cuda/ops.py:617-623, 904-916).  Contract (reference
+// _ops.py:239-295, gemm_4bit_mma.cuh:99-101):
 //
 //     out[m, n] = T( sum_k X[m, k] * W_T[n, k]  (fp32 accumulate)  + bias[n] )
 //     W_T[n, k] = rn_T( value(code[n, k]) * scale[(n*K + k) / blocksize] )      (one rounding)
 //     scale[i]  = absmax[i]                                       (plain)
 //               = absmax_code[absmax_8bit[i]] * absmax[i >> 8] + offset   (double quant)
 //
-// B200-first design ("swap-AB, weights through TMEM"):
-//   * The tensor-core M dimension (128 TMEM lanes) carries the OUTPUT FEATURES n; the
-//     tokens m are the UMMA N dimension (16..256).  A CTA owns out[m0:m0+MT, n0:n0+128].
-//   * A pipeline stage is 128 k-elements.  The TMA producer stages, per stage, the packed
-//     codes of the CTA's 128 rows (128 x 64 B, 64-byte swizzle, 8 KB) and the activation tile
-//     X[m0:m0+MT, k0:k0+128] (two 128-byte-swizzled sub-tiles).
-//   * This one-CTA kernel serves M < 512 (with split-K when the grid would not fill the machine); larger
-//     token counts go to the CTA-pair kernel of gemm4_pair.cu.  The cluster-multicast, cta_group::2, all-16-warp
-//     and persistent variants that round 1 kept here behind environment switches were measured slower
-//     (DESIGN.md section 3.1) and are gone.
-//   * 16 decode warps (two groups that alternate stages) expand the codes in REGISTERS with
-//     the exact reference rounding -- a per-block 16-entry table built with 16 FMUL + 8
-//     cvt.rn.bf16x2 and looked up with PRMT only -- and write the 16-bit tile straight into
-//     TENSOR MEMORY with tcgen05.st.  tcgen05.mma consumes it as the A operand ([tmem] form):
-//     the decoded weights never pass through shared memory, whose bandwidth is what limits an
-//     SS-mode Blackwell GEMM.  The activation tile is the K-major B operand (smem descriptor).
-//   * One elected thread issues eight tcgen05.mma (128 x MT x 16) per stage behind ONE
-//     mbarrier wait and releases the stage with ONE tcgen05.commit (multicast to the
-//     cluster): synchronisation on the issuing thread was the first bottleneck found.
-//   * Accumulators (128 lanes x MT fp32 columns) live in TMEM; the decode warps become the
-//     epilogue warps: tcgen05.ld -> +bias -> rn_T -> global, or -- for split-K, which fills
-//     the 148 SMs when M is small -- fp32 partials to an L2-resident workspace with a
-//     last-arriver reduction in deterministic split order.
+// Design ("swap-AB, weights through registers"):
+//   * The wgmma M dimension (64 rows per warpgroup, two warpgroups) carries the OUTPUT FEATURES n;
+//     the tokens m are the wgmma N dimension (MT = 16..128).  A CTA owns out[m0:m0+MT, n0:n0+128].
+//   * A pipeline stage is 128 k-elements.  One TMA producer warp stages, per stage, the packed codes
+//     of the CTA's 128 rows (128 x 64 B, 64-byte swizzle, 8 KB) and the activation tile
+//     X[m0:m0+MT, k0:k0+128] (two 128-byte-swizzled sub-tiles), the K-major B operand of wgmma.
+//   * Every consumer thread decodes the codes of its two rows straight into the register fragment of
+//     wgmma's A operand, with the exact reference rounding -- a per-block 16-entry table built with
+//     16 FMUL + 8 cvt.rn and looked up with PRMT only.  The decoded weights never pass through shared
+//     memory, whose bandwidth is then left to the activation operand.
+//   * Two A-fragment register sets alternate between stages, so the decode of stage i+1 overlaps the
+//     wgmma of stage i (wgmma.wait_group 1 before a set is overwritten).
+//   * Accumulators live in registers; the epilogue adds the bias, rounds to T and stores, or -- for
+//     split-K, which fills the 132 SMs when the tile grid is small -- writes fp32 partials to an
+//     L2-resident workspace with a last-arriver reduction in deterministic split order.
 //
-// Warp roles (576 threads): warp 0 TMA producer, warp 1 MMA issuer + TMEM allocator,
-// warps 2..17 decode / epilogue (TMEM lane quarter = warp_id % 4).
+// Warp roles (288 threads): warps 0..7 = two consumer warpgroups (decode + wgmma + epilogue),
+// warp 8 = TMA producer.
 #include "common.cuh"
 #include "decode4.cuh"
-#include "sm100_ptx.cuh"
+#include "hopper_ptx.cuh"
 
 #include <cstdlib>
 #include <mutex>
@@ -48,11 +40,10 @@ namespace bnb200 {
 
 namespace {
 
-constexpr int kBK = 128;         // pipeline stage: 128 k-elements = two 128-byte swizzle atoms of X per row
-constexpr int kTileN = 128;      // output features per CTA (TMEM lanes)
-constexpr int kDecodeWarps = 16;  // two groups of 8: group g decodes the stages i with i % 2 == g
-constexpr int kThreads = 32 * (2 + kDecodeWarps);
-constexpr int kScaleDepth = 4;   // decode-side register ring for the per-block scales (stages of one group)
+constexpr int kBK = 128;           // pipeline stage: 128 k-elements = two 128-byte swizzle atoms of X per row
+constexpr int kTileN = 128;        // output features per CTA (two warpgroups of 64)
+constexpr int kConsumers = 256;    // threads of the two consumer warpgroups
+constexpr int kThreads = kConsumers + 32;
 
 struct Gemm4Params {
     const uint8_t* B;            // packed codes [N, K/2]
@@ -64,8 +55,8 @@ struct Gemm4Params {
     void* out;                   // T[M, ldc]
     void* peer_out[7];           // further copies of the output tile (peer GPUs' gather buffers, same ldc): the
     int n_peers;                 //   epilogue stores every element to all of them (fused all-gather)
-    float* ws_partial;           // split-K partials [tiles][splits][128][MT]
-    int* ws_counter;             // one per output tile, zero on entry, reset on exit
+    float* ws_partial;           // split-K partials [tiles][splits][MT][128]
+    int* ws_counter;             // two per output tile, zero on entry, reset on exit
     int M, N, K, ldc;
     int log2_bs;
     int kblocks_total;           // number of 128-wide stages = ceil(K / 128)
@@ -74,28 +65,37 @@ struct Gemm4Params {
     int splits;                  // K splits per tile (1 = none)
 };
 
-template <typename T> struct TcFmt;
-template <> struct TcFmt<__nv_bfloat16> { static constexpr uint32_t kFmt = 1; };
-template <> struct TcFmt<__half> { static constexpr uint32_t kFmt = 0; };
+// one k16 step of a 64-row warpgroup tile: D[64 x MT] += A[64 x 16] (registers) * X[MT x 16]^T (descriptor)
+template <typename T, int MT>
+__device__ __forceinline__ void wgmma_step(float (&d)[MT / 2], const uint32_t (&a)[4], uint64_t b_desc) {
+    constexpr bool bf = std::is_same<T, __nv_bfloat16>::value;
+    if constexpr (MT == 16) {
+        if constexpr (bf) ptx::wgmma_m64n16k16_bf16_rs(d, a, b_desc); else ptx::wgmma_m64n16k16_f16_rs(d, a, b_desc);
+    } else if constexpr (MT == 32) {
+        if constexpr (bf) ptx::wgmma_m64n32k16_bf16_rs(d, a, b_desc); else ptx::wgmma_m64n32k16_f16_rs(d, a, b_desc);
+    } else if constexpr (MT == 64) {
+        if constexpr (bf) ptx::wgmma_m64n64k16_bf16_rs(d, a, b_desc); else ptx::wgmma_m64n64k16_f16_rs(d, a, b_desc);
+    } else {
+        static_assert(MT == 128, "token tile");
+        if constexpr (bf) ptx::wgmma_m64n128k16_bf16_rs(d, a, b_desc); else ptx::wgmma_m64n128k16_f16_rs(d, a, b_desc);
+    }
+}
 
-
-
-// Pipeline stage = 128 k-elements: two 64-wide (128-byte, swizzle-atom) activation sub-tiles in
-// shared memory and 64 TMEM columns of decoded weights.  One `full` and one `empty` mbarrier per
-// stage keep the synchronisation cost on the single MMA-issuing thread at one wait + one commit
-// per eight tcgen05.mma (it was the bottleneck with 64-wide stages and separate barriers).
-//
+// Pipeline stage = 128 k-elements: two 64-wide (128-byte, swizzle-atom) activation sub-tiles and the
+// packed codes of 128 rows.  Ring depth: as many stages as fit next to each other in 200 KB.
 template <int MT> struct StageCfg {
-    static constexpr int kXRows = MT;                            // token rows staged by this CTA
-    static constexpr int kStages = MT == 256 ? 3 : 4;            // smem: kStages * (kXRows * 256 + 8192) B <= 216 KB
-    static constexpr int kXSubBytes = kXRows * 128;              // one 64-wide sub-tile
+    static constexpr int kXSubBytes = MT * 128;                  // one 64-wide sub-tile
     static constexpr int kXStageBytes = 2 * kXSubBytes;
     static constexpr int kWStageBytes = kTileN * 64;             // packed codes: 128 rows x 64 B (TMA, 64-B swizzle)
     static constexpr int kStageBytes = kXStageBytes + kWStageBytes;
-    static constexpr uint32_t kTmemCols = 512u;                  // D: [0, MT); W stage s: kWCol0 + 64 s
-    static constexpr uint32_t kWCol0 = 256u;
-    static_assert(kWCol0 + kStages * 64 <= kTmemCols, "TMEM budget");
+    static constexpr int kStages = (200 * 1024 / kStageBytes) > 8 ? 8 : (200 * 1024 / kStageBytes);
 };
+
+// The 16 codes of stage-row words w[4q .. 4q+3] that this thread's A fragments need (byte `t` of each,
+// t = lane % 4): wgmma k16 step 2q+u reads byte t of words 4q+2u (k 2t, 2t+1) and 4q+2u+1 (k 8+2t, 9+2t).
+__device__ __forceinline__ uint32_t gather_bytes(uint4 v, uint32_t sel) {
+    return prmt(prmt(v.x, v.y, sel), prmt(v.z, v.w, sel), 0x5410);
+}
 
 template <typename T, int QT, int MT>
 __global__ void __launch_bounds__(kThreads, 1)
@@ -105,21 +105,16 @@ __global__ void __launch_bounds__(kThreads, 1)
     constexpr int kStages = Cfg::kStages;
     constexpr int kXSubBytes = Cfg::kXSubBytes;
     constexpr int kXStageBytes = Cfg::kXStageBytes;
-    constexpr uint32_t kTmemCols = Cfg::kTmemCols;
-    constexpr uint32_t kWCol0 = Cfg::kWCol0;
+    constexpr int kWStageBytes = Cfg::kWStageBytes;
 
     // ------------------------------------------------------------------ shared memory
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    constexpr int kWStageBytes = Cfg::kWStageBytes;
     uint8_t* sx = smem;                              // [kStages][2][MT x 128 B]   activations
     uint8_t* sw = smem + kStages * kXStageBytes;     // [kStages][128 x 64 B]      packed codes
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes);
-    uint64_t* full = bars;                   // [kStages] TMA (1 arrive + X bytes) + the 8 warps of one decode group -> MMA
-    uint64_t* empty = bars + kStages;        // [kStages] MMA -> TMA producer + decode warps
-    uint64_t* w_full = bars + 2 * kStages;   // [kStages] TMA (1 arrive + W bytes) -> decode warps
-    uint64_t* acc_full = bars + 3 * kStages; // MMA -> epilogue
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3 * kStages + 1);
+    uint64_t* full = bars;                   // [kStages] TMA (1 arrive + bytes) -> consumers
+    uint64_t* empty = bars + kStages;        // [kStages] the 8 consumer warps -> TMA producer
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -131,51 +126,36 @@ __global__ void __launch_bounds__(kThreads, 1)
     const int slot0 = tile_id * splits;  // first workspace slot of this tile
     const int n0 = (tile_id % p.n_tiles) * kTileN;
     const int m0 = (tile_id / p.n_tiles) * MT;
-    // work is split in 128-wide stages
     const int per = (p.kblocks_total + splits - 1) / splits;
     const int st_begin = split * per;
     int st_end = st_begin + per;
     if (st_end > p.kblocks_total) st_end = p.kblocks_total;
     const int nst = st_end - st_begin;  // >= 1 by construction
-    const int kb64_total = p.K / 64;    // the last stage may hold a single 64-wide block
 
-    // ------------------------------------------------------------------ setup
-    if (warp == 0 && lane == 0) {
-        ptx::prefetch_tmap(&tmap_x);
-        ptx::prefetch_tmap(&tmap_w);
+    if (threadIdx.x == 0) {
         for (int s = 0; s < kStages; ++s) {
-            ptx::mbar_init(&full[s], 1 + kDecodeWarps / 2);
-            ptx::mbar_init(&empty[s], 1);
-            ptx::mbar_init(&w_full[s], 1);
+            ptx::mbar_init(&full[s], 1);
+            ptx::mbar_init(&empty[s], kConsumers / 32);
         }
-        ptx::mbar_init(acc_full, 1);
         ptx::fence_barrier_init();
     }
-    if (warp == 1) {
-        ptx::tmem_alloc<kTmemCols>(tmem_slot);
-        ptx::tmem_relinquish();
-    }
-    ptx::tc_fence_before();
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == kConsumers / 32) {
         // ================================================================== TMA producer
-        // (elect.sync instead of `lane == 0`: a region ptxas KNOWS to be single-threaded keeps TMA / MMA operands in
-        // uniform registers; with `lane == 0` every tcgen05.mma sits in an ELECT + R2UR loop, ~94 cycles each)
         if (ptx::elect_one()) {
+            ptx::prefetch_tmap(&tmap_x);
+            ptx::prefetch_tmap(&tmap_w);
             int s = 0;
             uint32_t ph = 0;
             for (int i = 0; i < nst; ++i) {
                 ptx::mbar_wait(&empty[s], ph ^ 1u);
                 const int k0 = (st_begin + i) * kBK;
+                ptx::mbar_arrive_expect_tx(&full[s], kWStageBytes + kXStageBytes);
                 // packed codes of this CTA's 128 output features: bytes [k0/2, k0/2 + 64) of rows n0..n0+127
-                ptx::mbar_arrive_expect_tx(&w_full[s], kWStageBytes);
-                ptx::tma_load_2d(sw + s * kWStageBytes, &tmap_w, &w_full[s], k0 / 2, n0);
-                ptx::mbar_arrive_expect_tx(&full[s], kXStageBytes);
+                ptx::tma_load_2d(sw + s * kWStageBytes, &tmap_w, &full[s], k0 / 2, n0);
                 uint8_t* dst = sx + s * kXStageBytes;
-                // columns past K are out of bounds for the tensor map: TMA zero-fills them
+                // rows past M, rows past N and columns past K are out of bounds for the tensor maps: TMA zero-fills
 #pragma unroll
                 for (int h = 0; h < 2; ++h) ptx::tma_load_2d(dst + h * kXSubBytes, &tmap_x, &full[s], k0 + 64 * h, m0);
                 if (++s == kStages) {
@@ -184,251 +164,195 @@ __global__ void __launch_bounds__(kThreads, 1)
                 }
             }
         }
-    } else if (warp == 1) {
-        // ================================================================== MMA issuer (one elected thread)
-        // The commit that releases stage i-1 follows the second MMA of stage i, and the barrier of stage i+1 is
-        // probed before the last MMAs of stage i (see gemm4_pair.cu): nothing but MMAs between two stages.
-        if (ptx::elect_one()) {
-            constexpr uint32_t idesc = ptx::make_idesc(/*D=F32*/ 1, TcFmt<T>::kFmt, TcFmt<T>::kFmt, /*M=*/128, /*N=*/MT);
-            int s = 0, ps = 0;
-            uint32_t ph = 0;
-            ptx::mbar_wait(&full[0], 0);
-            for (int i = 0; i < nst; ++i) {
-                ptx::tc_fence_after();
-                int ns = s + 1;
-                uint32_t nph = ph;
-                if (ns == kStages) {
-                    ns = 0;
-                    nph ^= 1u;
-                }
-                const bool more = i + 1 < nst;
-                bool ok = false;
-                const uint32_t xs = ptx::smem_u32(sx + s * kXStageBytes);
-                const uint64_t bdesc0 = ptx::make_sw128_kmajor_desc(xs);
-                const uint64_t bdesc1 = ptx::make_sw128_kmajor_desc(xs + kXSubBytes);
-                const uint32_t a_tmem = tmem_base + kWCol0 + s * 64;
+        return;
+    }
+
+    // ====================================================================== consumers
+    const int wg = warp >> 2;                 // warpgroup: feature rows [64 wg, 64 wg + 64) of the tile
+    const int g = lane >> 2, t = lane & 3;
+    const int row0 = wg * 64 + (warp & 3) * 16 + g;  // this thread's two rows: row0, row0 + 8
+    const int na = n0 + row0, nb = na + 8;
+    const bool a_ok = na < p.N, b_ok = nb < p.N;
+    const long long e_a = (long long)(a_ok ? na : 0) * p.K;
+    const long long e_b = (long long)(b_ok ? nb : 0) * p.K;
+    const ScaleSrc sc{p.absmax, p.absmax_8bit, p.absmax_code, p.absmax_offset ? __ldg(p.absmax_offset) : 0.0f};
+    const uint32_t sel = (uint32_t)t | ((uint32_t)(t + 4) << 4);
+    // 64-byte swizzle of the code rows: 16-byte chunk c of row r sits at chunk c ^ ((r >> 1) & 3)
+    const uint32_t swz_a = (uint32_t)((row0 >> 1) & 3), swz_b = (uint32_t)(((row0 + 8) >> 1) & 3);
+
+    // Scales of one stage: the 32 codes of a gathered word lie inside one quantisation block (blocks are
+    // >= 32 and aligned), so each (row, q) needs one scale.  Fetched one stage ahead.
+    float scl[2][4];
+    auto fetch = [&](int i) {
+        const long long kk = (long long)(st_begin + i) * kBK;
 #pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    // K advances by 16 elements: +8 TMEM columns for A, +32 B (2 x 16 B) inside a sub-tile
-                    ptx::mma_f16_ts(tmem_base, a_tmem + 8 * j, (j < 4 ? bdesc0 : bdesc1) + 2 * (j & 3), idesc,
-                                    (i | j) != 0 ? 1u : 0u);
-                    if (j == 1 && i > 0) ptx::tc_commit(&empty[ps]);
-                    if (j == 6 && more) ok = ptx::mbar_try_wait(&full[ns], nph);
-                }
-                if (more && !ok) ptx::mbar_wait(&full[ns], nph);
-                ps = s;
-                s = ns;
-                ph = nph;
-            }
-            ptx::tc_commit(&empty[ps]);
-            ptx::tc_commit(acc_full);
+        for (int q = 0; q < 4; ++q) {
+            const bool in_k = i < nst && kk + 32 * q < p.K;
+            scl[0][q] = (in_k && a_ok) ? sc.load((e_a + kk + 32 * q) >> p.log2_bs) : 0.f;
+            scl[1][q] = (in_k && b_ok) ? sc.load((e_b + kk + 32 * q) >> p.log2_bs) : 0.f;
         }
-        __syncwarp();
-    } else {
-        // ================================================================== decode warps
-        const int dw = warp - 2;          // 0..15
-        const int quarter = warp & 3;     // TMEM lane quarter this warp may touch
-        const int grp = dw >> 3;          // decode group: owns the stages with (stage & 1) == grp
-        const int half = (dw >> 2) & 1;   // which 64 of the stage's 128 k-elements
-        const int khalf = dw >> 2;        // epilogue: which quarter of the accumulator columns (0..3)
-        const int row = quarter * 32 + lane;
-        const int n = n0 + row;
-        const bool n_ok = n < p.N;
-        const long long e_row = (long long)(n_ok ? n : 0) * p.K;
-        ScaleSrc sc{p.absmax, p.absmax_8bit, p.absmax_code, p.absmax_offset ? __ldg(p.absmax_offset) : 0.0f};
-        const bool two_scales = p.log2_bs == 5;  // blocksize 32: two quantisation blocks per 64 codes
+    };
 
-        // The packed codes arrive by TMA (64-byte swizzle: 16-byte chunk c of row r sits at chunk
-        // c ^ ((r >> 1) & 3)); this thread owns chunks 2*half and 2*half+1 of its row.
-        const uint32_t sw_row = (uint32_t)row * 64u;
-        const uint32_t sw_c0 = (uint32_t)(((2 * half) ^ ((row >> 1) & 3)) * 16);
-        const uint32_t sw_c1 = (uint32_t)(((2 * half + 1) ^ ((row >> 1) & 3)) * 16);
+    float acc[MT / 2];
+#pragma unroll
+    for (int j = 0; j < MT / 2; ++j) acc[j] = 0.f;
 
-        // Scales are scattered 4-byte loads (one row per lane): a register ring kScaleDepth stages
-        // deep hides their latency.  The loop is unrolled by the ring depth so that slot j is a fixed
-        // register (no rotation: a move out of a load's destination would wait for the load).
-        float wsc[kScaleDepth][2];
-        auto fetch = [&](int j, int t) {
-            wsc[j][0] = wsc[j][1] = 0.f;
-            const int stage_idx = 2 * t + grp;                 // this group's t-th stage
-            const int kb = 2 * (st_begin + stage_idx) + half;  // 64-wide k-block of this warp
-            if (stage_idx < nst && n_ok && kb < kb64_total) {
-                const long long e = e_row + (long long)kb * 64;
-                wsc[j][0] = sc.load(e >> p.log2_bs);
-                if (two_scales) wsc[j][1] = sc.load((e + 32) >> p.log2_bs);
+    uint32_t afr[2][8][4];  // two A-fragment sets: [set][k16 step][reg]
+
+    // decode stage i (smem stage s) into A set `set`
+    auto decode = [&](int s, uint32_t (&a)[8][4]) {
+        const uint8_t* wt = sw + s * kWStageBytes;
+        float sc_cur[2][4];
+#pragma unroll
+        for (int r = 0; r < 2; ++r)
+#pragma unroll
+            for (int q = 0; q < 4; ++q) sc_cur[r][q] = scl[r][q];
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            const uint8_t* rowp = wt + (row0 + 8 * r) * 64;
+            const uint32_t swz = r ? swz_b : swz_a;
+            DecodeTable tab;
+            float last = 0.f;
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                const uint4 v = *reinterpret_cast<const uint4*>(rowp + (((uint32_t)q ^ swz) << 4));
+                const uint32_t word = gather_bytes(v, sel);
+                if (q == 0 || sc_cur[r][q] != last) {
+                    build_table<T, QT>(sc_cur[r][q], tab);
+                    last = sc_cur[r][q];
+                }
+                uint32_t o[4];
+                decode_word(word, tab, o);
+                // o[i]: byte i of the gathered word = word 4q+i of the row -> k16 step 2q + i/2, half i%2
+#pragma unroll
+                for (int u = 0; u < 2; ++u) {
+                    a[2 * q + u][r] = o[2 * u];          // rows g / g+8, k 2t..2t+1
+                    a[2 * q + u][2 + r] = o[2 * u + 1];  // rows g / g+8, k 8+2t..9+2t
+                }
             }
-        };
+        }
+    };
+
+    auto mma_stage = [&](int s, const uint32_t (&a)[8][4]) {
+        const uint32_t xs = ptx::smem_u32(sx + s * kXStageBytes);
+        const uint64_t d0 = ptx::make_sw128_kmajor_desc(xs);
+        const uint64_t d1 = ptx::make_sw128_kmajor_desc(xs + kXSubBytes);
+        ptx::wgmma_fence();
 #pragma unroll
-        for (int j = 0; j < kScaleDepth; ++j) fetch(j, j);
+        for (int j = 0; j < 8; ++j) wgmma_step<T, MT>(acc, a[j], (j < 4 ? d0 : d1) + 2 * (j & 3));
+        ptx::wgmma_commit();
+    };
 
-        const int cnt = (nst - grp + 1) >> 1;  // number of stages this group owns
-        for (int t0 = 0; t0 < cnt; t0 += kScaleDepth) {
+    fetch(0);
+    int prev_s = -1;
+    for (int i0 = 0; i0 < nst; i0 += 2) {
 #pragma unroll
-            for (int j = 0; j < kScaleDepth; ++j) {
-                const int t = t0 + j;
-                if (t < cnt) {
-                    const int i = 2 * t + grp;
-                    const int s = i % kStages;
-                    const uint32_t ph = (uint32_t)(i / kStages) & 1u;
-                    const float sc0 = wsc[j][0], sc1 = wsc[j][1];
-                    fetch(j, t + kScaleDepth);
-
-                    ptx::mbar_wait(&w_full[s], ph);  // this stage's codes have landed
-                    const uint8_t* wt = sw + s * kWStageBytes + sw_row;
-                    const uint4 q0 = *reinterpret_cast<const uint4*>(wt + sw_c0);
-                    const uint4 q1 = *reinterpret_cast<const uint4*>(wt + sw_c1);
-
-                    // 64 codes of row n -> 32 registers of T pairs.  (Rows past N and k-blocks past K are
-                    // zero-filled by TMA and carry scale 0: they decode to +-0.)
-                    uint32_t r[32];
-                    DecodeTable tab;
-                    build_table<T, QT>(sc0, tab);
-                    decode_word(q0.x, tab, r + 0);
-                    decode_word(q0.y, tab, r + 4);
-                    decode_word(q0.z, tab, r + 8);
-                    decode_word(q0.w, tab, r + 12);
-                    if (two_scales) build_table<T, QT>(sc1, tab);
-                    decode_word(q1.x, tab, r + 16);
-                    decode_word(q1.y, tab, r + 20);
-                    decode_word(q1.z, tab, r + 24);
-                    decode_word(q1.w, tab, r + 28);
-
-                    // w_full[s] completing implies the producer saw empty[s]; waiting on it here as well
-                    // makes this warp itself an observer of the MMA completion before it overwrites TMEM.
-                    ptx::mbar_wait(&empty[s], ph ^ 1u);
-                    ptx::tc_fence_after();
-                    const uint32_t taddr = tmem_base + (uint32_t(quarter * 32) << 16) + kWCol0 + s * 64 + half * 32;
-                    ptx::tmem_st_x32(taddr, r);
-                    ptx::tmem_wait_st();
-                    ptx::tc_fence_before();
+        for (int h = 0; h < 2; ++h) {
+            const int i = i0 + h;
+            if (i < nst) {
+                const int s = i % kStages;
+                ptx::mbar_wait(&full[s], (uint32_t)(i / kStages) & 1u);
+                decode(s, afr[h]);
+                fetch(i + 1);
+                mma_stage(s, afr[h]);
+                // the wgmma group of the previous stage has completed: its activation tile (and its A set) are free
+                ptx::wgmma_wait<1>();
+                if (prev_s >= 0) {
                     __syncwarp();
-                    if (lane == 0) ptx::mbar_arrive(&full[s]);
+                    if (lane == 0) ptx::mbar_arrive(&empty[prev_s]);
                 }
-            }
-        }
-
-        // ================================================================== epilogue
-        ptx::mbar_wait(acc_full, 0);
-        ptx::tc_fence_after();
-
-        // this warp: lanes [quarter*32, +32) (= output features), columns [khalf*MT/4, +MT/4)
-        constexpr int kColsPerWarp = MT / 4;
-        constexpr int kChunk = (kColsPerWarp >= 32) ? 32 : kColsPerWarp;  // 4 (MT=16), 8, 16, 32
-        const int col0 = khalf * kColsPerWarp;
-        const uint32_t lane_addr = tmem_base + (uint32_t(quarter * 32) << 16);
-        T* outp = reinterpret_cast<T*>(p.out);
-        float bias_v = 0.f;
-        if (p.bias != nullptr && n_ok) bias_v = DT<T>::to_f32(reinterpret_cast<const T*>(p.bias)[n]);
-
-        if (splits == 1) {
-#pragma unroll 1
-            for (int c = 0; c < kColsPerWarp; c += kChunk) {
-                uint32_t v[32];
-                if constexpr (kChunk == 32) {
-                    ptx::tmem_ld_x32(lane_addr + col0 + c, v);
-                } else {
-                    uint32_t v16[16];
-                    ptx::tmem_ld_x16(lane_addr + col0 + c, v16);  // MT=16 reads 8 columns past its half: unused
-#pragma unroll
-                    for (int t = 0; t < 16; ++t) v[t] = v16[t];
-                }
-                ptx::tmem_wait_ld();
-#pragma unroll
-                for (int t = 0; t < kChunk; ++t) {
-                    const int m = m0 + col0 + c + t;
-                    if (n_ok && m < p.M) {
-                        const T val = DT<T>::from_f32(__uint_as_float(v[t]) + bias_v);
-                        const long long idx = (long long)m * p.ldc + n;
-                        outp[idx] = val;
-                        for (int r = 0; r < p.n_peers; ++r) reinterpret_cast<T*>(p.peer_out[r])[idx] = val;
-                    }
-                }
-            }
-        } else {
-            // ---- split-K: every split CTA publishes its fp32 partial tile (layout [column m][row n], so
-            // that both the write and the later reads are 128-byte coalesced), the splits of a tile
-            // rendezvous on a counter, and EACH of them then reduces a 1/splits share of the columns
-            // (in split order: deterministic).  The launch is COOPERATIVE (all CTAs of the <= one-wave grid are
-            // resident together by contract), so the short wait cannot starve; it is bounded anyway.
-            float* ws_tile = p.ws_partial + (long long)slot0 * kTileN * MT;
-            float* my = ws_tile + (long long)split * kTileN * MT;
-#pragma unroll 1
-            for (int c = 0; c < kColsPerWarp; c += kChunk) {
-                uint32_t v[32];
-                if constexpr (kChunk == 32) {
-                    ptx::tmem_ld_x32(lane_addr + col0 + c, v);
-                } else {
-                    uint32_t v16[16];
-                    ptx::tmem_ld_x16(lane_addr + col0 + c, v16);
-#pragma unroll
-                    for (int t = 0; t < 16; ++t) v[t] = v16[t];
-                }
-                ptx::tmem_wait_ld();
-#pragma unroll
-                for (int t = 0; t < kChunk; ++t) my[(col0 + c + t) * kTileN + row] = __uint_as_float(v[t]);
-            }
-            __threadfence();
-            asm volatile("bar.sync 1, 512;" ::: "memory");
-            int* arrive = p.ws_counter + tile_id;
-            int* done = p.ws_counter + p.tiles_total + tile_id;
-            if (threadIdx.x == 64) {
-                atomicAdd(arrive, 1);
-                unsigned long long t0 = 0;
-                unsigned spins = 0;
-                while (atomicAdd(arrive, 0) < splits) {
-                    __nanosleep(64);
-                    if ((++spins & 0xFFF) == 0) {  // bounded: report + trap after 10 s instead of hanging the device
-                        unsigned long long now;
-                        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
-                        if (t0 == 0) t0 = now;
-                        else if (now - t0 > 10000000000ull) {
-                            printf("bnb200: split-K rendezvous timed out (tile %d split %d of %d)\n", tile_id, split, splits);
-                            __trap();
-                        }
-                    }
-                }
-                __threadfence();
-            }
-            asm volatile("bar.sync 1, 512;" ::: "memory");
-            {
-                const int e = threadIdx.x - 64;          // 0..511 over the 16 epilogue warps
-                const int rn = e & (kTileN - 1);         // output feature inside the tile
-                const int cg = e >> 7;                   // 0..3
-                const int nn = n0 + rn;
-                float bias_r = 0.f;
-                if (p.bias != nullptr && nn < p.N) bias_r = DT<T>::to_f32(reinterpret_cast<const T*>(p.bias)[nn]);
-                for (int c = split + splits * cg; c < MT; c += splits * 4) {
-                    const int m = m0 + c;
-                    if (m >= p.M) break;
-                    float acc = 0.f;
-                    for (int sp = 0; sp < splits; ++sp)
-                        acc += __ldcg(ws_tile + ((long long)sp * MT + c) * kTileN + rn);
-                    if (nn < p.N) {
-                        const T val = DT<T>::from_f32(acc + bias_r);
-                        const long long idx = (long long)m * p.ldc + nn;
-                        outp[idx] = val;
-                        for (int r = 0; r < p.n_peers; ++r) reinterpret_cast<T*>(p.peer_out[r])[idx] = val;
-                    }
-                }
-            }
-            asm volatile("bar.sync 1, 512;" ::: "memory");
-            if (threadIdx.x == 64) {
-                // last split out resets the tile's counters for the next launch
-                if (atomicAdd(done, 1) == splits - 1) {
-                    *arrive = 0;
-                    *done = 0;
-                    __threadfence();
-                }
+                prev_s = s;
             }
         }
     }
+    ptx::wgmma_wait<0>();
+#pragma unroll
+    for (int j = 0; j < MT / 2; ++j) ptx::fence_operand(acc[j]);
 
-    // ------------------------------------------------------------------ teardown
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        ptx::tc_fence_after();
-        ptx::tmem_dealloc_dyn(tmem_base, kTmemCols);
+    // ================================================================== epilogue
+    // acc[4j + e]: feature row row0 + 8 * (e >= 2), token column 8j + 2t + (e & 1)
+    T* outp = reinterpret_cast<T*>(p.out);
+    if (splits == 1) {
+        const T* bias = reinterpret_cast<const T*>(p.bias);
+        const float bias_a = (bias != nullptr && a_ok) ? DT<T>::to_f32(bias[na]) : 0.f;
+        const float bias_b = (bias != nullptr && b_ok) ? DT<T>::to_f32(bias[nb]) : 0.f;
+#pragma unroll
+        for (int j = 0; j < MT / 8; ++j) {
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const int m = m0 + 8 * j + 2 * t + (e & 1);
+                const bool hi = e >= 2;
+                const int n = hi ? nb : na;
+                if ((hi ? b_ok : a_ok) && m < p.M) {
+                    const T val = DT<T>::from_f32(acc[4 * j + e] + (hi ? bias_b : bias_a));
+                    const long long idx = (long long)m * p.ldc + n;
+                    outp[idx] = val;
+                    for (int r = 0; r < p.n_peers; ++r) reinterpret_cast<T*>(p.peer_out[r])[idx] = val;
+                }
+            }
+        }
+        return;
+    }
+
+    // ---- split-K: every split CTA publishes its fp32 partial tile (layout [column m][row n], so that the
+    // later reads are 128-byte coalesced), the splits of a tile rendezvous on a counter, and EACH of them then
+    // reduces a 1/splits share of the columns (in split order: deterministic).  The launch is COOPERATIVE (all
+    // CTAs of the <= one-wave grid are resident together), so the short wait cannot starve; it is bounded anyway.
+    float* ws_tile = p.ws_partial + (long long)slot0 * kTileN * MT;
+    float* my = ws_tile + (long long)split * kTileN * MT;
+#pragma unroll
+    for (int j = 0; j < MT / 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) my[(8 * j + 2 * t + (e & 1)) * kTileN + row0 + 8 * (e >> 1)] = acc[4 * j + e];
+    __threadfence();
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    int* arrive = p.ws_counter + tile_id;
+    int* done = p.ws_counter + p.tiles_total + tile_id;
+    if (threadIdx.x == 0) {
+        atomicAdd(arrive, 1);
+        unsigned long long t0 = 0;
+        unsigned spins = 0;
+        while (atomicAdd(arrive, 0) < splits) {
+            __nanosleep(64);
+            if ((++spins & 0xFFF) == 0) {  // bounded: trap after 10 s instead of hanging the device (no printf:
+                                           // a call would serialise the wgmma pipeline)
+                unsigned long long now;
+                asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
+                if (t0 == 0) t0 = now;
+                else if (now - t0 > 10000000000ull) __trap();
+            }
+        }
+        __threadfence();
+    }
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    {
+        const int e = threadIdx.x;               // 0..255 over the two consumer warpgroups
+        const int rn = e & (kTileN - 1);         // output feature inside the tile
+        const int cg = e >> 7;                   // 0..1
+        const int nn = n0 + rn;
+        float bias_r = 0.f;
+        if (p.bias != nullptr && nn < p.N) bias_r = DT<T>::to_f32(reinterpret_cast<const T*>(p.bias)[nn]);
+        for (int c = split + splits * cg; c < MT; c += splits * 2) {
+            const int m = m0 + c;
+            if (m >= p.M) break;
+            float a = 0.f;
+            for (int sp = 0; sp < splits; ++sp) a += __ldcg(ws_tile + ((long long)sp * MT + c) * kTileN + rn);
+            if (nn < p.N) {
+                const T val = DT<T>::from_f32(a + bias_r);
+                const long long idx = (long long)m * p.ldc + nn;
+                outp[idx] = val;
+                for (int r = 0; r < p.n_peers; ++r) reinterpret_cast<T*>(p.peer_out[r])[idx] = val;
+            }
+        }
+    }
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    if (threadIdx.x == 0) {
+        // last split out resets the tile's counters for the next launch
+        if (atomicAdd(done, 1) == splits - 1) {
+            *arrive = 0;
+            *done = 0;
+            __threadfence();
+        }
     }
 }
 
@@ -442,8 +366,7 @@ struct Workspace {
 
 // Split-K scratch: one FIXED-SIZE block per (device, stream), so that launches on different streams never
 // share partials or counters and the launch path never reallocates.  32 MB covers every split this
-// library launches (one-CTA kernel: <= one wave of 128 x 256 fp32 tiles = 19 MB; pair kernel: <= 148 split
-// CTAs x 128 x 384 fp32 = 29 MB).  The only allocation happens on the first split-K call of a stream; it is
+// library launches (<= one wave of 132 CTAs x 128 x 128 fp32 = 8.3 MB).  The only allocation happens on the first split-K call of a stream; it is
 // made capture-safe (relaxed capture mode around cudaMalloc) so that a CUDA-graph capture whose first
 // split-K GEMM is inside the capture still works.  The registry evicts its least recently used entry.
 constexpr size_t kWsBytes = size_t(32) << 20;
@@ -516,7 +439,7 @@ Workspace* get_workspace(cudaStream_t stream, size_t partial_bytes, size_t n_cou
 }
 
 template <typename T, int QT, int MT>
-bool launch_mt(const T* A, Gemm4Params& p, cudaStream_t stream) {
+bool launch_mt(const T* A, Gemm4Params& p, int force_splits, cudaStream_t stream) {
     using Cfg = StageCfg<MT>;
     constexpr size_t smem_bytes = 1024 /*align slack*/ + size_t(Cfg::kStages) * Cfg::kStageBytes + 256 /*barriers*/;
     // the shared-memory opt-in is PER DEVICE (one process may drive several GPUs)
@@ -544,15 +467,18 @@ bool launch_mt(const T* A, Gemm4Params& p, cudaStream_t stream) {
     // K-splitting for small problems: a uniform split so that ONE wave covers the machine.  Split CTAs exchange
     // fp32 partials through an L2-resident workspace and every split reduces its share of the columns.
     int splits = 1;
-    if (tiles * 2 <= sms) {
-        int v = sms / tiles;
-        const int max_by_k = p.kblocks_total / 2 > 0 ? p.kblocks_total / 2 : 1;  // >= two 128-wide stages per split
+    if (force_splits > 0 || tiles * 2 <= sms) {
+        int v = force_splits > 0 ? force_splits : sms / tiles;
+        // >= two 128-wide stages per split by default, >= one when the split is forced
+        const int max_by_k = force_splits > 0 ? p.kblocks_total : (p.kblocks_total / 2 > 0 ? p.kblocks_total / 2 : 1);
         if (v > max_by_k) v = max_by_k;
         if (v > 16) v = 16;
         if (v < 1) v = 1;
         const int per = (p.kblocks_total + v - 1) / v;
         splits = (p.kblocks_total + per - 1) / per;  // no empty split
     }
+    // a forced split must still be one co-resident wave (the splits of a tile wait for each other)
+    if (splits > 1 && tiles * splits > sms) return false;
     p.splits = splits;
     p.n_tiles = n_tiles;
     p.tiles_total = tiles;
@@ -595,30 +521,14 @@ bool launch_mt(const T* A, Gemm4Params& p, cudaStream_t stream) {
 
 } // namespace
 
-struct Gemm4Workspace {
-    float* partial;
-    int* counters;
-};
-bool gemm4_get_workspace(cudaStream_t stream, size_t partial_bytes, size_t n_counters, Gemm4Workspace* out) {
-    Workspace* ws = get_workspace(stream, partial_bytes, n_counters);
-    if (ws == nullptr) return false;
-    out->partial = reinterpret_cast<float*>(ws->ptr);
-    out->counters = ws->counters;
-    return true;
-}
-
-template <typename T>
-bool launch_gemm4_pair(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
-                       const float* absmax_code, const float* absmax_offset, T* out, const T* bias, int M, int N, int K,
-                       int ldc, int blocksize, int quant_type, cudaStream_t stream, void* const* peers, int n_peers,
-                       int mt_override, int force_splits, long long* trace);
-
 // Returns true if the tensor-core path handled the call.
 // `peers` / `n_peers`: up to 7 additional output bases (same ldc) that receive a copy of every element.
+// `mt_override`: token tile (16 | 32 | 64 | 128, 0 = by M); `force_splits`: K split per tile (0 = by the grid).
 template <typename T>
 bool launch_gemm4_tc(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
                      const float* absmax_code, const float* absmax_offset, T* out, const T* bias, int M, int N, int K,
-                     int ldc, int blocksize, int quant_type, cudaStream_t stream, void* const* peers, int n_peers) {
+                     int ldc, int blocksize, int quant_type, cudaStream_t stream, void* const* peers, int n_peers,
+                     int mt_override, int force_splits) {
     if (n_peers < 0 || n_peers > 7) return false;
     if (M <= 0 || N <= 0) return true;
     if (K < 64 || (K % 64) != 0) return false;
@@ -626,24 +536,14 @@ bool launch_gemm4_tc(const T* A, const uint8_t* B, const float* absmax, const ui
     if ((reinterpret_cast<uintptr_t>(A) & 15) != 0 || (reinterpret_cast<uintptr_t>(B) & 15) != 0) return false;
     if (quant_type != kNF4 && quant_type != kFP4) return false;
 
-    // Large token counts: the CTA-pair kernel (gemm4_pair.cu).  BNB_B200_PAIR_KERNEL=0 keeps the one-CTA kernel.
-    {
-        static int use_pair = -1;
-        if (use_pair < 0) {
-            const char* e = getenv("BNB_B200_PAIR_KERNEL");
-            use_pair = (e != nullptr && e[0] == '0') ? 0 : 1;
-        }
-        if (use_pair && M >= 512 &&
-            launch_gemm4_pair<T>(A, B, absmax, absmax_8bit, absmax_code, absmax_offset, out, bias, M, N, K, ldc,
-                                 blocksize, quant_type, stream, peers, n_peers, 0, 0, nullptr))
-            return true;
-    }
-
-    int MT = 256;
+    int MT = 128;
     if (M <= 16) MT = 16;
     else if (M <= 32) MT = 32;
     else if (M <= 64) MT = 64;
-    else if (M <= 128) MT = 128;
+    if (mt_override != 0) {
+        if (mt_override != 16 && mt_override != 32 && mt_override != 64 && mt_override != 128) return false;
+        MT = mt_override;
+    }
 
     Gemm4Params p{};
     p.B = B;
@@ -664,11 +564,10 @@ bool launch_gemm4_tc(const T* A, const uint8_t* B, const float* absmax, const ui
 
 #define BNB200_DISPATCH_MT(QT)                                                                                         \
     switch (MT) {                                                                                                      \
-    case 16: return launch_mt<T, QT, 16>(A, p, stream);                                                                \
-    case 32: return launch_mt<T, QT, 32>(A, p, stream);                                                                \
-    case 64: return launch_mt<T, QT, 64>(A, p, stream);                                                                \
-    case 128: return launch_mt<T, QT, 128>(A, p, stream);                                                              \
-    default: return launch_mt<T, QT, 256>(A, p, stream);                                                               \
+    case 16: return launch_mt<T, QT, 16>(A, p, force_splits, stream);                                                  \
+    case 32: return launch_mt<T, QT, 32>(A, p, force_splits, stream);                                                  \
+    case 64: return launch_mt<T, QT, 64>(A, p, force_splits, stream);                                                  \
+    default: return launch_mt<T, QT, 128>(A, p, force_splits, stream);                                                 \
     }
     if (quant_type == kNF4) {
         BNB200_DISPATCH_MT(kNF4)
@@ -680,9 +579,9 @@ bool launch_gemm4_tc(const T* A, const uint8_t* B, const float* absmax, const ui
 
 template bool launch_gemm4_tc<__nv_bfloat16>(const __nv_bfloat16*, const uint8_t*, const float*, const uint8_t*,
                                              const float*, const float*, __nv_bfloat16*, const __nv_bfloat16*, int,
-                                             int, int, int, int, int, cudaStream_t, void* const*, int);
+                                             int, int, int, int, int, cudaStream_t, void* const*, int, int, int);
 template bool launch_gemm4_tc<__half>(const __half*, const uint8_t*, const float*, const uint8_t*, const float*,
                                       const float*, __half*, const __half*, int, int, int, int, int, int,
-                                      cudaStream_t, void* const*, int);
+                                      cudaStream_t, void* const*, int, int, int);
 
 } // namespace bnb200

@@ -1,11 +1,11 @@
-// gemv4_mma.cu -- decode-time 4-bit GEMV / skinny GEMM (M <= 16 tokens) for sm_100a.
+// gemv4_mma.cu -- decode-time 4-bit GEMV / skinny GEMM (M <= 16 tokens) for sm_90a.
 //
 // The regime the reference serves with gemm_4bit_simt (reference csrc/gemm_4bit_simt.cu:109-480,
 // dispatch bitsandbytes/backends/cuda/ops.py:583-623): one to a few tokens against the whole packed
 // weight.  The roofline is the HBM stream of the codes (N*K/2 bytes); what actually limits a
 // CUDA-core kernel is the instruction count per weight (decode + widen + FFMA).  Here the multiply-
-// accumulate goes to the tensor cores through the warp-level mma.sync.m16n8k16 (a 128 x MT tcgen05
-// tile would be 87 % padding at M = 8), so the CUDA cores only decode:
+// accumulate goes to the tensor cores through the warp-level mma.sync.m16n8k16 (the wgmma kernel's
+// smallest token tile, 16, would be half padding at M = 8), so the CUDA cores only decode:
 //
 //   * a CTA owns 16 output features (the MMA's M); its 4 or 8 warps split K in 256-wide chunks and
 //     meet in shared memory at the end;

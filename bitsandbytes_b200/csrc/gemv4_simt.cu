@@ -1,9 +1,9 @@
-// gemv4_simt.cu -- fused 4-bit dequant GEMV / skinny GEMM on CUDA cores (sm_100a).
+// gemv4_simt.cu -- fused 4-bit dequant GEMV / skinny GEMM on CUDA cores (sm_90a).
 //
 // Replaces the reference's gemm_4bit_simt (reference csrc/gemm_4bit_simt.cu:109-480) and the
 // legacy kgemm_4bit_inference_naive (reference csrc/kernels.cu:1452-1567).  Two jobs:
 //   (1) fp32 activations (the tensor cores have no exact fp32 mode) and shapes the
-//       tcgen05 kernel does not take (K % 64 != 0, unaligned pointers);
+//       tensor-core kernel does not take (K % 64 != 0, unaligned pointers);
 //   (2) a simple always-correct reference for the tensor-core path in tests.
 //
 // One warp per output feature n; the 32 lanes split K in 8-element chunks (4 packed bytes,

@@ -1,4 +1,4 @@
-// int8.cu -- the LLM.int8() hot path for sm_100a.
+// int8.cu -- the LLM.int8() hot path for sm_90a.
 //
 //   int8_vector_quant   replaces reference kInt8VectorQuant (csrc/kernels.cu:1331-1385):
 //                       one read of A instead of two (the row is held in registers between
@@ -8,7 +8,7 @@
 //   int8 GEMM           lives in int8_gemm.cu.
 //   dequant_mm_int32    replaces reference kdequant_mm_int32_fp16 (csrc/kernels.cu:1396-1448).
 #include "common.cuh"
-#include "sm100_ptx.cuh"
+#include "hopper_ptx.cuh"
 
 namespace bnb200 {
 
@@ -290,7 +290,7 @@ void launch_int8_outlier_prep(const void* A, const int8_t* CB, const float* SCB,
     if (jpad <= 0 || M + N <= 0) return;
     const long long total = (long long)(M + N) * jpad;
     long long want = (total + 255) / 256;
-    const int grid = (int)(want < 148 * 16 ? want : 148 * 16);
+    const int grid = (int)(want < 132 * 16 ? want : 132 * 16);
     if (dtype == 1)
         int8_outlier_prep_kernel<__half><<<grid, 256, 0, stream>>>((const __half*)A, CB, SCB, cols, J, jpad, M, N, K,
                                                                    (__half*)subA, (__half*)subBT);
@@ -331,7 +331,7 @@ void launch_int8_zero_columns(int8_t* CA, const long long* cols, int J, int rows
     if (J <= 0 || rows <= 0) return;
     const long long total = (long long)rows * J;
     long long want = (total + 255) / 256;
-    const int grid = (int)(want < 148 * 16 ? want : 148 * 16);
+    const int grid = (int)(want < 132 * 16 ? want : 132 * 16);
     int8_zero_columns_kernel<<<grid, 256, 0, stream>>>(CA, cols, J, rows, K);
     BNB200_CHECK_LAUNCH("int8_zero_columns");
 }

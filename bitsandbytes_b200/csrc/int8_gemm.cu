@@ -1,59 +1,41 @@
-// int8_gemm.cu -- the LLM.int8() GEMM for sm_100a:  C[M,N] = A[M,K] . B[N,K]^T, int8 x int8 -> int32.
+// int8_gemm.cu -- the LLM.int8() GEMM for sm_90a:  C[M,N] = A[M,K] . B[N,K]^T, int8 x int8 -> int32.
 //
-// Replaces reference igemmlt<32,0> -> cublasLtMatmul (csrc/ops.cu:282-404) with a tcgen05 kind::i8
-// kernel: both operands TMA-staged (128-byte swizzle), int32 accumulators in TMEM, exact.  The
-// epilogue either stores int32 (cigemmlt_32 ABI) or applies the dequantisation of reference
-// kdequant_mm_int32_fp16 (csrc/kernels.cu:1396-1448),
+// Replaces reference igemmlt<32,0> -> cublasLtMatmul (csrc/ops.cu:282-404) with a wgmma s8 kernel: both
+// operands TMA-staged (128-byte swizzle), int32 accumulators in registers, exact.  The epilogue either
+// stores int32 (cigemmlt_32 ABI) or applies the dequantisation of reference kdequant_mm_int32_fp16
+// (csrc/kernels.cu:1396-1448),
 //     fp16/bf16( fma(acc * SCA[m] * SCB[n], 1/127^2, bias[n]) ),
 // in-kernel, which removes the 2 x M x N x 4-byte int32 round trip through HBM -- and, for LLM.int8()'s
 // mixed decomposition (reference backends/default/ops.py:64-100: `output.addmm(subA, subB)` after the int8
 // matmul), adds the OUTLIER term  sum_j subA[m, j] * subB[j, n]  (fp16/bf16 products, fp32 accumulation)
 // in the same epilogue, so the second pass over out[M, N] and the cuBLAS call of the reference chain are gone.
 #include "common.cuh"
-#include "sm100_ptx.cuh"
+#include "hopper_ptx.cuh"
 
 namespace bnb200 {
 
 namespace {
 
 // ======================================================================================
-// Persistent, warp-specialised kernel on 2-CTA clusters (one CTA per SM, 74 clusters):
-//   * CTA tile 128 (tokens, TMEM lanes) x 256 (features, TMEM columns), K in 128-byte k-blocks,
-//     TMA ring (128-byte swizzle) filling 192 KB of shared memory;
-//   * the two CTAs of a cluster work on vertically adjacent token tiles of the SAME feature tile
-//     and split the 256-row weight tile between them (see PAIR below);
-//   * accumulators are double-buffered (2 x 256 TMEM columns): four epilogue warps drain tile t
-//     (tcgen05.ld -> dequantise -> store) while the MMA warp already accumulates tile t+1;
-//   * static persistent schedule: cluster c processes tile pairs c, c + #clusters, ...
-// Warps: 0 = TMA producer, 1 = MMA issuer + TMEM allocator, 2..5 = epilogue.
+// Warp-specialised kernel, one 128 x 128 output tile per CTA:
+//   * CTA tile 128 tokens (two consumer warpgroups of 64 rows, the wgmma M dimension) x 128 features
+//     (the wgmma N dimension), K in 128-byte k-blocks, a TMA ring (128-byte swizzle) of up to 6 stages;
+//   * each consumer warpgroup issues four wgmma m64n128k32 per stage from shared-memory descriptors and
+//     releases the previous stage once its wgmma group has completed (wgmma.wait_group 1);
+//   * the epilogue dequantises straight from the accumulator registers.
+// Warps: 0..7 = consumers, 8 = TMA producer.
 // ======================================================================================
 constexpr int kI8BK = 128;        // int8 elements per stage = one 128-byte swizzled row
-constexpr int kI8TileM = 128;     // tokens per CTA tile (TMEM lanes)
-constexpr int kI8TileN = 256;     // output features per CTA tile (TMEM columns)
-constexpr int kI8Threads = 6 * 32;
-constexpr int kI8ABytes = kI8TileM * 128;
-constexpr int kI8Cluster = 2;
-constexpr int kI8RingBytes = 192 * 1024;
+constexpr int kI8TileM = 128;     // tokens per CTA tile
+constexpr int kI8TileN = 128;     // output features per CTA tile
+constexpr int kI8Consumers = 256;
+constexpr int kI8Threads = kI8Consumers + 32;
+constexpr int kI8StageBytes = (kI8TileM + kI8TileN) * kI8BK;
 
-// PAIR = true (default): one tcgen05.mma.cta_group::2 (M = 256) per CTA pair, issued by the leader;
-//               each CTA stages only ITS half of the weight tile and the tensor cores of both SMs
-//               read it.  Per 128-deep k-block every SM pulls 32 KB through L2 -> shared memory.
-// PAIR = false: one tcgen05.mma (cta_group::1, M = 128) per CTA; each CTA holds the whole 256-row
-//               weight tile, half of it fetched by its peer and multicast (48 KB into each SM).
-// Measured at 4096 x 11008 x 4096 (profiles/r01_int8_gemm_{pair,mc}.json): pair 135 us with 1.44 GB
-// crossing the L2 -> SM crossbar, multicast 140-151 us with 2.17 GB; tensor pipe 68 % active in both.
-// KSUB = 128-byte k sub-tiles per pipeline stage: with 2, the MMA thread pays one barrier wait and one
-// commit per eight tcgen05.mma instead of per four.
-template <bool PAIR, int KSUB> struct I8Cfg {
-    static constexpr int kASubBytes = kI8ABytes;                                   // 128 rows x 128 B
-    static constexpr int kBSubBytes = (PAIR ? kI8TileN / 2 : kI8TileN) * 128;
-    static constexpr int kABytes = KSUB * kASubBytes;
-    static constexpr int kBBytes = KSUB * kBSubBytes;
-    static constexpr int kStageBytes = kABytes + kBBytes;
-    static constexpr int kStages = kI8RingBytes / kStageBytes;  // pair: 6 x 32 KB or 3 x 64 KB; multicast: 4 x 48 KB
+template <int JMAX> struct I8Cfg {
+    // with the outlier term, 2 x 128 rows x JMAX T values of it share the 227 KB
+    static constexpr int kStages = JMAX > 0 ? 5 : 6;
 };
-
-// Every mbarrier wait in this kernel is bounded (ptx::mbar_wait_bounded: report + trap after 10 s).
 
 // EPI: 0 = int32 out, 1 = fp16 out, 2 = bf16 out (fused dequant)
 struct I8Params {
@@ -66,7 +48,7 @@ struct I8Params {
     int jpad;           // padded outlier count (multiple of 8, <= JMAX)
     int M, N, K, ldc;
     int kblocks;
-    int n_tiles, m_pairs, pair_tiles;
+    int n_tiles;
 };
 
 // 8 consecutive T -> fp32
@@ -85,342 +67,186 @@ template <int EPI> __device__ __forceinline__ void i8_unpack8(const uint4& r, fl
     }
 }
 
-// JMAX: capacity of the fused outlier term (0 = none): the thread keeps its row of subA in JMAX registers.
-template <int EPI, bool PAIR, int KSUB, int JMAX>
+// JMAX: capacity of the fused outlier term (0 = none): subA of the CTA's 128 tokens and subBT of its 128 features
+// are staged in shared memory after the main loop.
+template <int EPI, int JMAX>
 __global__ void __launch_bounds__(kI8Threads, 1)
     int8_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                         const I8Params p) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t* stages = smem;
-    using Cfg = I8Cfg<PAIR, KSUB>;
-    constexpr int kI8Stages = Cfg::kStages;
-    constexpr int kI8StageBytes = Cfg::kStageBytes;
-    float* s_scb = reinterpret_cast<float*>(smem + kI8Stages * kI8StageBytes);   // [2][256]
-    float* s_bias = s_scb + 2 * kI8TileN;                                          // [2][256]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kI8Stages * kI8StageBytes + 4096);
-    // outlier weights of 128 output features at a time: [128][JMAX] of T (row = feature), after the barriers
-    uint4* s_sub = reinterpret_cast<uint4*>(smem + kI8Stages * kI8StageBytes + 4096 + 256);
-    uint64_t* full = bars;                       // [stages] TMA -> MMA
-    uint64_t* empty = bars + kI8Stages;          // [stages] MMA of both cluster CTAs -> TMA
-    uint64_t* tmem_full = bars + 2 * kI8Stages;  // [2] MMA -> epilogue
-    uint64_t* tmem_empty = tmem_full + 2;        // [2] epilogue -> MMA
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
+    constexpr int kStages = I8Cfg<JMAX>::kStages;
+    uint8_t* stages = smem;                                                       // [stages][A 16 KB | B 16 KB]
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * kI8StageBytes);
+    uint64_t* full = bars;              // [stages] TMA -> consumers
+    uint64_t* empty = bars + kStages;   // [stages] the 8 consumer warps -> TMA
+    uint4* s_suba = reinterpret_cast<uint4*>(smem + kStages * kI8StageBytes + 256);  // [128][JMAX] of T
+    uint4* s_subb = s_suba + kI8TileM * (JMAX / 8);                                  // [128][JMAX] of T
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    constexpr uint32_t kTmemCols = 512;
-    constexpr uint16_t kMask = (uint16_t)((1u << kI8Cluster) - 1u);
+    const int n0 = (blockIdx.x % p.n_tiles) * kI8TileN;
+    const int m0 = (blockIdx.x / p.n_tiles) * kI8TileM;
 
-    if (warp == 0 && lane == 0) {
-        ptx::prefetch_tmap(&tmap_a);
-        ptx::prefetch_tmap(&tmap_b);
-        for (int s = 0; s < kI8Stages; ++s) {
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < kStages; ++s) {
             ptx::mbar_init(&full[s], 1);
-            // multicast mode: the MMA threads of both CTAs release a stage; pair mode: one commit
-            ptx::mbar_init(&empty[s], PAIR ? 1 : kI8Cluster);
-        }
-        for (int a = 0; a < 2; ++a) {
-            ptx::mbar_init(&tmem_full[a], 1);
-            // pair mode: the leader's barrier collects the epilogue warps of both CTAs
-            ptx::mbar_init(&tmem_empty[a], PAIR ? 8 : 4);
+            ptx::mbar_init(&empty[s], kI8Consumers / 32);
         }
         ptx::fence_barrier_init();
     }
-    if (warp == 1) {
-        if (PAIR) {
-            ptx::tmem_alloc_pair<kTmemCols>(tmem_slot);
-            ptx::tmem_relinquish_pair();
-        } else {
-            ptx::tmem_alloc<kTmemCols>(tmem_slot);
-            ptx::tmem_relinquish();
-        }
-    }
-    ptx::tc_fence_before();
-    ptx::cluster_sync();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t rank = ptx::cluster_ctarank();
-    const int cluster_id = blockIdx.x / kI8Cluster;
-    const int n_clusters = gridDim.x / kI8Cluster;
+    __syncthreads();
 
-    if (warp == 0) {
+    if (warp == kI8Consumers / 32) {
         // ================================================================== TMA producer
-        // (elect.sync rather than `lane == 0`: a region ptxas knows to be single-threaded keeps the TMA / MMA operands
-        // in uniform registers; with `lane == 0` every instruction is wrapped in an ELECT + R2UR loop)
         if (ptx::elect_one()) {
-            uint32_t it = 0;
-            for (int pt = cluster_id; pt < p.pair_tiles; pt += n_clusters) {
-                const int n0 = (pt % p.n_tiles) * kI8TileN;
-                const int m0 = ((pt / p.n_tiles) * kI8Cluster + (int)rank) * kI8TileM;
-                for (int i = 0; i < p.kblocks; ++i, ++it) {
-                    const int s = it % kI8Stages;
-                    const uint32_t ph = (it / kI8Stages) & 1u;
-                    ptx::mbar_wait_bounded(&empty[s], ph ^ 1u, 1, (int)it, pt);
-                    uint8_t* sa = stages + s * kI8StageBytes;
-                    if (PAIR) {
-                        // both CTAs' boxes complete on the LEADER's barrier: it waits once per stage
-                        const uint32_t lead_full = ptx::mapa_u32(ptx::smem_u32(&full[s]), 0);
-                        if (rank == 0) ptx::mbar_arrive_expect_tx(&full[s], kI8Cluster * kI8StageBytes);
-                        // (k columns past K are out of bounds for the tensor map: TMA zero-fills them)
-#pragma unroll
-                        for (int u = 0; u < KSUB; ++u) {
-                            const int kc = (i * KSUB + u) * kI8BK;
-                            ptx::tma_load_2d_pair(sa + u * Cfg::kASubBytes, &tmap_a, lead_full, kc, m0);
-                            ptx::tma_load_2d_pair(sa + Cfg::kABytes + u * Cfg::kBSubBytes, &tmap_b, lead_full, kc,
-                                                  n0 + (int)rank * (kI8TileN / kI8Cluster));
-                        }
-                    } else {
-                        ptx::mbar_arrive_expect_tx(&full[s], kI8StageBytes);
-#pragma unroll
-                        for (int u = 0; u < KSUB; ++u) {
-                            const int kc = (i * KSUB + u) * kI8BK;
-                            ptx::tma_load_2d(sa + u * Cfg::kASubBytes, &tmap_a, &full[s], kc, m0);
-                            // my half of the weight tile, to both CTAs
-                            ptx::tma_load_2d_multicast(sa + Cfg::kABytes + u * Cfg::kBSubBytes +
-                                                           rank * (Cfg::kBSubBytes / kI8Cluster),
-                                                       &tmap_b, &full[s], kc, n0 + (int)rank * (kI8TileN / kI8Cluster),
-                                                       kMask);
-                        }
-                    }
-                }
+            ptx::prefetch_tmap(&tmap_a);
+            ptx::prefetch_tmap(&tmap_b);
+            for (int i = 0; i < p.kblocks; ++i) {
+                const int s = i % kStages;
+                ptx::mbar_wait(&empty[s], ((i / kStages) & 1u) ^ 1u);
+                uint8_t* sa = stages + s * kI8StageBytes;
+                ptx::mbar_arrive_expect_tx(&full[s], kI8StageBytes);
+                // (rows past M / N and k columns past K are out of bounds for the tensor maps: TMA zero-fills them)
+                ptx::tma_load_2d(sa, &tmap_a, &full[s], i * kI8BK, m0);
+                ptx::tma_load_2d(sa + kI8TileM * kI8BK, &tmap_b, &full[s], i * kI8BK, n0);
             }
         }
-    } else if (warp == 1) {
-        // ================================================================== MMA issuer (one elected thread)
-        // kind::i8: D = S32 (2), A/B = signed int8 (1); UMMA K = 32 bytes.
-        // The barrier of stage g+1 is probed (one non-blocking try_wait) before the last MMAs of stage g, so that its
-        // latency hides under queued MMAs; only a failed probe falls back to a blocking wait.  The commit stays at
-        // the END of its stage: this kernel is bound by the L2 -> SM ingest of a 3-stage ring (ncu: 1.44 GB at
-        // 10.7 TB/s, tensor pipe 80 %), so releasing a slot two MMAs later costs more than the issue gap it hides
-        // (measured: 134 vs 125 us at 4096 x 11008 x 4096).
-        // pair mode: only the leader issues; its instructions drive both SMs.
-        if ((!PAIR || rank == 0) && ptx::elect_one()) {
-            constexpr uint32_t idesc = ptx::make_idesc(2, 1, 1, PAIR ? 2 * kI8TileM : kI8TileM, kI8TileN);
-            constexpr int kMmas = KSUB * (kI8BK / 32);  // 4 or 8 per stage
-            auto commit = [&](uint64_t* bar) {
-                if (PAIR) ptx::tc_commit_pair(bar, kMask);
-                else ptx::tc_commit_multicast(bar, kMask);
-            };
-            const int my_tiles = cluster_id < p.pair_tiles ? (p.pair_tiles - cluster_id + n_clusters - 1) / n_clusters : 0;
-            const uint32_t total = (uint32_t)my_tiles * (uint32_t)p.kblocks;  // stages this CTA pair runs
-            uint32_t g = 0, tcount = 0;
-            bool ok = false;
-            if (total > 0) ptx::mbar_wait_bounded(&full[0], 0, 3, 0, 0);
-            for (int pt = cluster_id; pt < p.pair_tiles; pt += n_clusters, ++tcount) {
-                const uint32_t acc = tcount & 1u;
-                // the epilogue has drained this accumulator (two tiles ago)
-                ptx::mbar_wait_bounded(&tmem_empty[acc], ((tcount >> 1) & 1u) ^ 1u, 2, (int)tcount, pt);
-                const uint32_t d_tmem = tmem_base + acc * kI8TileN;
-                for (int i = 0; i < p.kblocks; ++i, ++g) {
-                    const int s = g % kI8Stages;
-                    ptx::tc_fence_after();
-                    const bool more = g + 1 < total;
-                    const int ns = (g + 1) % kI8Stages;
-                    const uint32_t nph = ((g + 1) / kI8Stages) & 1u;
-                    ok = false;
-                    const uint32_t sa = ptx::smem_u32(stages + s * kI8StageBytes);
-#pragma unroll
-                    for (int q = 0; q < kMmas; ++q) {
-                        const int u = q / (kI8BK / 32), j = q % (kI8BK / 32);
-                        const uint64_t adesc = ptx::make_sw128_kmajor_desc(sa + u * Cfg::kASubBytes) + 2 * j;
-                        const uint64_t bdesc = ptx::make_sw128_kmajor_desc(sa + Cfg::kABytes + u * Cfg::kBSubBytes) + 2 * j;
-                        const uint32_t accum = (i | q) != 0 ? 1u : 0u;
-                        if (PAIR)
-                            ptx::mma_i8_ss_pair(d_tmem, adesc, bdesc, idesc, accum);
-                        else
-                            ptx::mma_i8_ss(d_tmem, adesc, bdesc, idesc, accum);
-                        if (q == kMmas - 2 && more) ok = ptx::mbar_try_wait(&full[ns], nph);
-                    }
-                    commit(&empty[s]);
-                    if (i == p.kblocks - 1) {
-                        // end of a tile: hand the accumulator to the epilogue
-                        if (PAIR) ptx::tc_commit_pair(&tmem_full[acc], kMask);
-                        else ptx::tc_commit(&tmem_full[acc]);
-                    }
-                    if (more && !ok) ptx::mbar_wait_bounded(&full[ns], nph, 3, (int)g + 1, pt);
-                }
-            }
-        }
-        __syncwarp();
-    } else {
-        // ================================================================== epilogue warps 2..5
-        const int quarter = warp & 3;  // TMEM lane quarter
-        const int et = threadIdx.x - 64;  // 0..127
-        uint32_t tcount = 0;
-        for (int pt = cluster_id; pt < p.pair_tiles; pt += n_clusters, ++tcount) {
-            const uint32_t acc = tcount & 1u;
-            const int n0 = (pt % p.n_tiles) * kI8TileN;
-            const int m0 = ((pt / p.n_tiles) * kI8Cluster + (int)rank) * kI8TileM;
-            const int m = m0 + quarter * 32 + lane;
-            const bool m_ok = m < p.M;
-            float* scb = s_scb + acc * kI8TileN;
-            float* sbias = s_bias + acc * kI8TileN;
-            if (EPI != 0) {
-                // this buffer was last read two tiles ago by these same warps (ordered by the named
-                // barrier of the previous use)
-                for (int c = et; c < kI8TileN; c += 128) {
-                    const int n = n0 + c;
-                    scb[c] = (n < p.N) ? __ldg(p.SCB + n) : 0.f;
-                    float b = 0.f;
-                    if (p.bias != nullptr && n < p.N) {
-                        if (EPI == 1)
-                            b = __half2float(reinterpret_cast<const __half*>(p.bias)[n]);
-                        else
-                            b = __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p.bias)[n]);
-                    }
-                    sbias[c] = b;
-                }
-                asm volatile("bar.sync 1, 128;" ::: "memory");
-            }
-            float sca = 0.f;
-            if (EPI != 0 && m_ok) sca = __ldg(p.SCA + m);
-            // this token's outlier activations (fp32 copies of the T values: the products below are exact)
-            float oa[JMAX > 0 ? JMAX : 1];
-            if constexpr (JMAX > 0) {
-#pragma unroll
-                for (int g = 0; g < JMAX / 8; ++g) {
-                    float t8[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-                    if (m_ok && 8 * g < p.jpad)
-                        i8_unpack8<EPI>(__ldg(reinterpret_cast<const uint4*>(
-                                            reinterpret_cast<const uint16_t*>(p.subA) + (long long)m * p.jpad + 8 * g)),
-                                        t8);
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) oa[8 * g + e] = t8[e];
-                }
-            }
-            // outlier term of tile column cc for this token: sum_j subA[m, j] * subBT[n0 + cc, j], the weights read from
-            // the staged half tile (every lane reads the same row: shared-memory broadcast, no bank conflicts)
-            auto outlier = [&](int cc) -> float {
-                float o = 0.f;
-                if constexpr (JMAX > 0) {
-                    const uint4* brow = s_sub + (cc & 127) * (JMAX / 8);
-#pragma unroll
-                    for (int g = 0; g < JMAX / 8; ++g) {
-                        if (8 * g < p.jpad) {
-                            float b8[8];
-                            i8_unpack8<EPI>(brow[g], b8);
-#pragma unroll
-                            for (int e = 0; e < 8; ++e) o = fmaf(oa[8 * g + e], b8[e], o);
-                        }
-                    }
-                }
-                return o;
-            };
-            ptx::mbar_wait_bounded(&tmem_full[acc], (tcount >> 1) & 1u, 4, (int)tcount, pt);
-            ptx::tc_fence_after();
-            const uint32_t lane_addr = tmem_base + (uint32_t(quarter * 32) << 16) + acc * kI8TileN;
-#pragma unroll 1
-            for (int c = 0; c < kI8TileN; c += 32) {
-                if constexpr (JMAX > 0) {
-                    if ((c & 127) == 0) {
-                        // stage subBT[n0 + c .. + 128) (zero rows past N): thread et owns feature row et
-                        asm volatile("bar.sync 1, 128;" ::: "memory");  // the previous half has been consumed
-                        const int nn = n0 + c + et;
-#pragma unroll
-                        for (int g = 0; g < JMAX / 8; ++g) {
-                            uint4 r = make_uint4(0, 0, 0, 0);
-                            if (nn < p.N && 8 * g < p.jpad)
-                                r = __ldg(reinterpret_cast<const uint4*>(reinterpret_cast<const uint16_t*>(p.subBT) +
-                                                                         (long long)nn * p.jpad + 8 * g));
-                            s_sub[et * (JMAX / 8) + g] = r;
-                        }
-                        asm volatile("bar.sync 1, 128;" ::: "memory");
-                    }
-                }
-                uint32_t v[32];
-                ptx::tmem_ld_x32(lane_addr + c, v);
-                ptx::tmem_wait_ld();
-                if (c + 32 == kI8TileN) {
-                    // all of this warp's TMEM reads are done: hand the accumulator back to the MMA warp
-                    ptx::tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) {
-                        if (PAIR)
-                            ptx::mbar_arrive_cluster(ptx::mapa_u32(ptx::smem_u32(&tmem_empty[acc]), 0));
-                        else
-                            ptx::mbar_arrive(&tmem_empty[acc]);
-                    }
-                }
-                if (!m_ok) continue;
-                const int n = n0 + c;
-                if (EPI == 0) {
-                    int* dst = reinterpret_cast<int*>(p.out) + (long long)m * p.ldc + n;
-                    if (n + 32 <= p.N && ((reinterpret_cast<uintptr_t>(dst) & 15) == 0)) {
-#pragma unroll
-                        for (int t = 0; t < 32; t += 4)
-                            *reinterpret_cast<uint4*>(dst + t) = make_uint4(v[t], v[t + 1], v[t + 2], v[t + 3]);
-                    } else {
-                        for (int t = 0; t < 32; ++t)
-                            if (n + t < p.N) dst[t] = (int)v[t];
-                    }
-                } else {
-                    uint32_t w[16];
-#pragma unroll
-                    for (int t = 0; t < 32; t += 2) {
-                        if (EPI == 1) {
-                            float f0 = dequant_value((int)v[t], sca, scb[c + t], sbias[c + t]);
-                            float f1 = dequant_value((int)v[t + 1], sca, scb[c + t + 1], sbias[c + t + 1]);
-                            if constexpr (JMAX > 0) {
-                                // reference: the int8 result is an fp16 tensor, then addmm adds the fp32-accumulated
-                                // outlier product and rounds once more
-                                f0 = __half2float(__float2half_rn(f0)) + outlier(c + t);
-                                f1 = __half2float(__float2half_rn(f1)) + outlier(c + t + 1);
-                            }
-                            w[t >> 1] = pack2<__half>(f0, f1);
-                        } else {
-                            // bf16 output, bit-identical to the reference chain (backends/cuda/ops.py:186-210):
-                            // the kernel result is fp16, a non-fp16 bias is added by `out.add_(bias)` on the
-                            // fp16 tensor (fp32 add, one rounding to fp16), then `.to(bfloat16)`.
-                            float f0 = __half2float(__float2half_rn(dequant_value((int)v[t], sca, scb[c + t], 0.f)));
-                            float f1 = __half2float(
-                                __float2half_rn(dequant_value((int)v[t + 1], sca, scb[c + t + 1], 0.f)));
-                            if (p.bias != nullptr) {
-                                f0 = __half2float(__float2half_rn(f0 + sbias[c + t]));
-                                f1 = __half2float(__float2half_rn(f1 + sbias[c + t + 1]));
-                            }
-                            if constexpr (JMAX > 0) {
-                                f0 = __bfloat162float(__float2bfloat16_rn(f0)) + outlier(c + t);
-                                f1 = __bfloat162float(__float2bfloat16_rn(f1)) + outlier(c + t + 1);
-                            }
-                            w[t >> 1] = pack2<__nv_bfloat16>(f0, f1);
-                        }
-                    }
-                    uint16_t* dst = reinterpret_cast<uint16_t*>(p.out) + (long long)m * p.ldc + n;
-                    if (n + 32 <= p.N && ((reinterpret_cast<uintptr_t>(dst) & 15) == 0)) {
-#pragma unroll
-                        for (int t = 0; t < 16; t += 4)
-                            *reinterpret_cast<uint4*>(dst + 2 * t) = make_uint4(w[t], w[t + 1], w[t + 2], w[t + 3]);
-                    } else {
-                        for (int t = 0; t < 32; ++t)
-                            if (n + t < p.N) dst[t] = (uint16_t)(w[t >> 1] >> (16 * (t & 1)));
-                    }
-                }
-            }
-            if (EPI != 0) asm volatile("bar.sync 1, 128;" ::: "memory");  // scale buffers free for tile t+2
-        }
+        return;
     }
 
-    ptx::tc_fence_before();
-    ptx::cluster_sync();  // no CTA exits while its peer can still multicast into / arrive on its smem
-    if (warp == 1) {
-        ptx::tc_fence_after();
-        if (PAIR)
-            ptx::tmem_dealloc_pair(tmem_base, kTmemCols);
-        else
-            ptx::tmem_dealloc_dyn(tmem_base, kTmemCols);
+    // ====================================================================== consumers
+    const int wg = warp >> 2;
+    const int g = lane >> 2, t = lane & 3;
+    int32_t acc[64];
+#pragma unroll
+    for (int j = 0; j < 64; ++j) acc[j] = 0;
+    int prev_s = -1;
+    for (int i = 0; i < p.kblocks; ++i) {
+        const int s = i % kStages;
+        ptx::mbar_wait(&full[s], (i / kStages) & 1u);
+        const uint32_t sa = ptx::smem_u32(stages + s * kI8StageBytes) + wg * 64 * kI8BK;  // this warpgroup's 64 rows
+        const uint32_t sb = ptx::smem_u32(stages + s * kI8StageBytes) + kI8TileM * kI8BK;
+        const uint64_t adesc = ptx::make_sw128_kmajor_desc(sa);
+        const uint64_t bdesc = ptx::make_sw128_kmajor_desc(sb);
+        ptx::wgmma_fence();
+#pragma unroll
+        for (int j = 0; j < kI8BK / 32; ++j) ptx::wgmma_m64n128k32_s8_ss(acc, adesc + 2 * j, bdesc + 2 * j);
+        ptx::wgmma_commit();
+        ptx::wgmma_wait<1>();  // the previous stage's wgmma group has completed: release its slot
+        if (prev_s >= 0) {
+            __syncwarp();
+            if (lane == 0) ptx::mbar_arrive(&empty[prev_s]);
+        }
+        prev_s = s;
+    }
+    ptx::wgmma_wait<0>();
+#pragma unroll
+    for (int j = 0; j < 64; ++j) ptx::fence_operand(acc[j]);
+
+    // ====================================================================== epilogue
+    // acc[4j + e]: token row rl + 8 * (e >= 2), feature column 8j + 2t + (e & 1)
+    const int rl = wg * 64 + (warp & 3) * 16 + g;
+    if constexpr (JMAX > 0) {
+        // stage the outlier operands (zero rows past M / N), thread e owns row e & 127 of one of the two
+        const int e = threadIdx.x;
+        const int r = e & 127;
+        const bool is_b = e >= 128;
+        const int gr = (is_b ? n0 : m0) + r;
+        const bool ok = gr < (is_b ? p.N : p.M);
+        const uint16_t* src = reinterpret_cast<const uint16_t*>(is_b ? p.subBT : p.subA) + (long long)(ok ? gr : 0) * p.jpad;
+        uint4* dst = (is_b ? s_subb : s_suba) + r * (JMAX / 8);
+#pragma unroll
+        for (int q = 0; q < JMAX / 8; ++q)
+            dst[q] = (ok && 8 * q < p.jpad) ? __ldg(reinterpret_cast<const uint4*>(src) + q) : make_uint4(0, 0, 0, 0);
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int m = m0 + rl + 8 * h;
+        if (m >= p.M) continue;
+        float sca = 0.f;
+        if (EPI != 0) sca = __ldg(p.SCA + m);
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+            const int n = n0 + 8 * j + 2 * t;  // this thread's two consecutive columns n, n + 1
+            const int v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+            if (EPI == 0) {
+                int* dst = reinterpret_cast<int*>(p.out) + (long long)m * p.ldc + n;
+                if (n + 1 < p.N && (reinterpret_cast<uintptr_t>(dst) & 7) == 0) {
+                    *reinterpret_cast<int2*>(dst) = make_int2(v0, v1);
+                } else {
+                    if (n < p.N) dst[0] = v0;
+                    if (n + 1 < p.N) dst[1] = v1;
+                }
+            } else {
+            // outlier term of this token and columns n, n + 1: sum_j subA[m, j] * subBT[n, j] in j order (fp32 fma)
+            float ol[2] = {0.f, 0.f};
+            if constexpr (JMAX > 0) {
+                const uint4* arow = s_suba + (rl + 8 * h) * (JMAX / 8);
+                const uint4* brow = s_subb + (8 * j + 2 * t) * (JMAX / 8);
+#pragma unroll
+                for (int q = 0; q < JMAX / 8; ++q) {
+                    if (8 * q < p.jpad) {
+                        float a8[8], b8[8], c8[8];
+                        i8_unpack8<EPI>(arow[q], a8);
+                        i8_unpack8<EPI>(brow[q], b8);
+                        i8_unpack8<EPI>(brow[JMAX / 8 + q], c8);
+#pragma unroll
+                        for (int x = 0; x < 8; ++x) {
+                            ol[0] = fmaf(a8[x], b8[x], ol[0]);
+                            ol[1] = fmaf(a8[x], c8[x], ol[1]);
+                        }
+                    }
+                }
+            }
+            float f[2];
+#pragma unroll
+            for (int u = 0; u < 2; ++u) {
+                const int nn = n + u;
+                const int v = u ? v1 : v0;
+                const float scb = nn < p.N ? __ldg(p.SCB + nn) : 0.f;
+                float b = 0.f;
+                if (p.bias != nullptr && nn < p.N) {
+                    if (EPI == 1) b = __half2float(reinterpret_cast<const __half*>(p.bias)[nn]);
+                    else b = __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p.bias)[nn]);
+                }
+                if (EPI == 1) {
+                    f[u] = dequant_value(v, sca, scb, b);
+                    // reference: the int8 result is an fp16 tensor, then addmm adds the fp32-accumulated
+                    // outlier product and rounds once more
+                    if constexpr (JMAX > 0) f[u] = __half2float(__float2half_rn(f[u])) + ol[u];
+                } else {
+                    // bf16 output, bit-identical to the reference chain (backends/cuda/ops.py:186-210): the kernel
+                    // result is fp16, a non-fp16 bias is added by `out.add_(bias)` on the fp16 tensor (fp32 add,
+                    // one rounding to fp16), then `.to(bfloat16)`.
+                    f[u] = __half2float(__float2half_rn(dequant_value(v, sca, scb, 0.f)));
+                    if (p.bias != nullptr) f[u] = __half2float(__float2half_rn(f[u] + b));
+                    if constexpr (JMAX > 0) f[u] = __bfloat162float(__float2bfloat16_rn(f[u])) + ol[u];
+                }
+            }
+            const uint32_t w = EPI == 1 ? pack2<__half>(f[0], f[1]) : pack2<__nv_bfloat16>(f[0], f[1]);
+            uint16_t* dst = reinterpret_cast<uint16_t*>(p.out) + (long long)m * p.ldc + n;
+            if (n + 1 < p.N && (reinterpret_cast<uintptr_t>(dst) & 3) == 0) {
+                *reinterpret_cast<uint32_t*>(dst) = w;
+            } else {
+                if (n < p.N) dst[0] = (uint16_t)w;
+                if (n + 1 < p.N) dst[1] = (uint16_t)(w >> 16);
+            }
+            }
+        }
     }
 }
 
-template <int EPI, bool PAIR, int KSUB, int JMAX = 0>
+template <int EPI, int JMAX = 0>
 int launch_i8(const CUtensorMap& ta, const CUtensorMap& tb, I8Params& p, cudaStream_t stream) {
-    using Cfg = I8Cfg<PAIR, KSUB>;
-    constexpr size_t smem_bytes = 1024 + size_t(Cfg::kStages) * Cfg::kStageBytes + 4096 + 256 + size_t(128) * JMAX * 2;
+    constexpr size_t smem_bytes =
+        1024 + size_t(I8Cfg<JMAX>::kStages) * kI8StageBytes + 256 + size_t(kI8TileM + kI8TileN) * JMAX * 2;
     static bool attr_set[64] = {};  // the shared-memory opt-in is per device
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 1;
-    auto kern = int8_gemm_tc_kernel<EPI, PAIR, KSUB, JMAX>;
-    p.kblocks = (p.K + KSUB * kI8BK - 1) / (KSUB * kI8BK);
+    auto kern = int8_gemm_tc_kernel<EPI, JMAX>;
+    p.kblocks = (p.K + kI8BK - 1) / kI8BK;
     if (!attr_set[dev]) {
         if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes) != cudaSuccess) {
             set_last_error("int8_gemm_tc smem attr", cudaGetLastError());
@@ -430,22 +256,11 @@ int launch_i8(const CUtensorMap& ta, const CUtensorMap& tb, I8Params& p, cudaStr
     }
     p.n_tiles = (p.N + kI8TileN - 1) / kI8TileN;
     const int m_tiles = (p.M + kI8TileM - 1) / kI8TileM;
-    p.m_pairs = (m_tiles + kI8Cluster - 1) / kI8Cluster;
-    p.pair_tiles = p.n_tiles * p.m_pairs;
-    int clusters = device_sm_count() / kI8Cluster;
-    if (clusters > p.pair_tiles) clusters = p.pair_tiles;
     cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(clusters * kI8Cluster, 1, 1);
+    cfg.gridDim = dim3(p.n_tiles * m_tiles, 1, 1);
     cfg.blockDim = dim3(kI8Threads);
     cfg.dynamicSmemBytes = smem_bytes;
     cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = kI8Cluster;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
     cudaError_t e = cudaLaunchKernelEx(&cfg, kern, ta, tb, p);
     if (e != cudaSuccess) {
         (void)cudaGetLastError();
@@ -471,8 +286,7 @@ int launch_int8_gemm(const int8_t* acts, const int8_t* weights, void* out, const
     if ((reinterpret_cast<uintptr_t>(acts) & 15) != 0 || (reinterpret_cast<uintptr_t>(weights) & 15) != 0) return 100;
     CUtensorMap ta, tb;
     if (!encode_tmap_2d(&ta, acts, 1, 128, (uint64_t)M, (uint64_t)K, (uint64_t)K, kI8TileM, kI8BK)) return 100;
-    if (!encode_tmap_2d(&tb, weights, 1, 128, (uint64_t)N, (uint64_t)K, (uint64_t)K, kI8TileN / kI8Cluster, kI8BK))
-        return 100;
+    if (!encode_tmap_2d(&tb, weights, 1, 128, (uint64_t)N, (uint64_t)K, (uint64_t)K, kI8TileN, kI8BK)) return 100;
     I8Params p{};
     p.out = out;
     p.SCA = SCA;
@@ -486,45 +300,22 @@ int launch_int8_gemm(const int8_t* acts, const int8_t* weights, void* out, const
     p.subBT = subBT;
     p.jpad = jpad;
     if (jpad > 0) {
-        // fused outlier term: the pair kernel, capacity = next of {8, 16, 32, 64}
+        // fused outlier term, capacity = next of {8, 16, 32, 64}
 #define BNB200_I8_J(E)                                                                                                 \
-        if (jpad <= 8) return launch_i8<E, true, 2, 8>(ta, tb, p, stream);                                             \
-        if (jpad <= 16) return launch_i8<E, true, 2, 16>(ta, tb, p, stream);                                           \
-        if (jpad <= 32) return launch_i8<E, true, 2, 32>(ta, tb, p, stream);                                           \
-        return launch_i8<E, true, 2, 64>(ta, tb, p, stream);
+        if (jpad <= 8) return launch_i8<E, 8>(ta, tb, p, stream);                                                      \
+        if (jpad <= 16) return launch_i8<E, 16>(ta, tb, p, stream);                                                    \
+        if (jpad <= 32) return launch_i8<E, 32>(ta, tb, p, stream);                                                    \
+        return launch_i8<E, 64>(ta, tb, p, stream);
         if (epi == 1) {
             BNB200_I8_J(1)
         }
         BNB200_I8_J(2)
 #undef BNB200_I8_J
     }
-    // BNB_B200_I8_MODE=multicast selects the cta_group::1 variant (A/B measurements); default = pair
-    static const bool pair = [] {
-        const char* e = getenv("BNB_B200_I8_MODE");
-        return !(e != nullptr && e[0] == 'm');
-    }();
-    static const int ksub = [] {
-        const char* e = getenv("BNB_B200_I8_KSUB");
-        return (e != nullptr && e[0] == '1') ? 1 : 2;
-    }();
-    if (pair && ksub == 2) {
-        switch (epi) {
-        case 0: return launch_i8<0, true, 2>(ta, tb, p, stream);
-        case 1: return launch_i8<1, true, 2>(ta, tb, p, stream);
-        default: return launch_i8<2, true, 2>(ta, tb, p, stream);
-        }
-    }
-    if (pair) {
-        switch (epi) {
-        case 0: return launch_i8<0, true, 1>(ta, tb, p, stream);
-        case 1: return launch_i8<1, true, 1>(ta, tb, p, stream);
-        default: return launch_i8<2, true, 1>(ta, tb, p, stream);
-        }
-    }
     switch (epi) {
-    case 0: return launch_i8<0, false, 1>(ta, tb, p, stream);
-    case 1: return launch_i8<1, false, 1>(ta, tb, p, stream);
-    default: return launch_i8<2, false, 1>(ta, tb, p, stream);
+    case 0: return launch_i8<0>(ta, tb, p, stream);
+    case 1: return launch_i8<1>(ta, tb, p, stream);
+    default: return launch_i8<2>(ta, tb, p, stream);
     }
 }
 

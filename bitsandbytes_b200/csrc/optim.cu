@@ -8,7 +8,7 @@
 //     the block's absmax, updated in fp32, the new absmax of the block is reduced, the parameters are updated, and
 //     the state is re-quantised with the 7-step search of the blockwise quantizer (csrc/kernels.cu:221-267; here: its
 //     bracket-table form, q8_search.cuh).
-// Both are HBM-bound element-wise kernels (12-20 bytes per element), so the B200 version is about access shape, not
+// Both are HBM-bound element-wise kernels (12-20 bytes per element), so this implementation is about access shape, not
 // about the tensor cores: a warp owns one 256-element block (lane l handles the 8 consecutive elements 8 l .. 8 l + 7
 // through 8- and 16-byte accesses: every load and store of the warp is one contiguous segment), the block's absmax is a warp-shuffle reduction (no shared-memory
 // round trip, no __syncthreads in the loop), the two code books sit in shared memory once per CTA, and the grid is

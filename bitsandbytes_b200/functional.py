@@ -7,7 +7,7 @@ gemv_4bit :1300, int8_* :1536-1673, create_dynamic_map :296, optimizer_update_32
 optimizer_update_8bit_blockwise :1169, the paged-memory helpers :25-160).  The deprecated igemm family and
 the CPU weight-repacking helpers of the reference are not provided.
 
-All tensor work is done by the ``bitsandbytes::`` ops whose only kernels are the sm_100a
+All tensor work is done by the ``bitsandbytes::`` ops whose only kernels are the sm_90a
 ones (``backends/cuda.py``); tensors must live on a CUDA device.
 """
 from __future__ import annotations

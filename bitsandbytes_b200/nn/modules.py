@@ -184,7 +184,7 @@ def fix_4bit_weight_quant_state_from_module(module: "Linear4bit"):
 
 class Linear4bit(nn.Linear):
     """QLoRA-style 4-bit linear layer.  ``module.to("cuda")`` quantises the loaded 16/32-bit
-    weights; ``forward`` runs the fused dequant-GEMM (tcgen05 on B200)."""
+    weights; ``forward`` runs the fused dequant-GEMM (wgmma on H100)."""
 
     def __init__(self, input_features, output_features, bias=True, compute_dtype=None, compress_statistics=True,
                  quant_type="fp4", quant_storage=torch.uint8, device=None):

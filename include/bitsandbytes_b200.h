@@ -1,5 +1,5 @@
 /*
- * bitsandbytes_b200.h -- the C ABI of libbitsandbytes_b200.so (sm_100a only).
+ * bitsandbytes_b200.h -- the C ABI of libbitsandbytes_b200.so (sm_90a only).
  *
  * This is the drop-in boundary: every symbol in section 1 has the SAME name,
  * argument order and argument meaning as the symbol the reference's Python layer
@@ -24,7 +24,7 @@
  * layer polls cbnb_b200_last_error() after every call and raises.  `void` entry
  * points stay `void`.
  *
- * Section 2 holds B200-only additions (stream-taking quantize, fused int8 linear,
+ * Section 2 holds native additions (stream-taking quantize, fused int8 linear,
  * sharded-linear helpers).  Section 3 lists symbols the reference loader insists on
  * (cextension.py:112-115) that are outside the hot path; they exist and fail loudly.
  */
@@ -128,14 +128,14 @@ void carange_fp32(float* A, float* B, float value, long n);
 void c_mul_fp32(float* A, float* B, float value, long n);
 
 /* =====================================================================
- * 2. B200-native additions (no reference counterpart)
+ * 2. Native additions (no reference counterpart)
  * ===================================================================== */
 
 /* 0 = no error since the last call; otherwise a code, with a message retrievable below.
  * Polling clears the flag. */
 int cbnb_b200_last_error(void);
 const char* cbnb_b200_last_error_message(void);
-/* "sm_100a tcgen05 ..." build description */
+/* "sm_90a; wgmma ..." build description */
 const char* cbnb_b200_build_info(void);
 
 /* Stream-taking quantize (the reference ABI above has none).  quant_type 0/1/2,
@@ -143,23 +143,23 @@ const char* cbnb_b200_build_info(void);
 void cbnb_b200_quantize_blockwise(const float* code, const void* A, float* absmax, unsigned char* out, int blocksize, int n, int quant_type, int dtype, bnb_stream_t stream);
 
 /* Fused all-gather for a column-sharded layer (no reference counterpart: the reference is single-device).
- * The tcgen05 kernel's epilogue stores every output element to outs[0..n_outs): outs[0] is the local
+ * The wgmma kernel's epilogue stores every output element to outs[0..n_outs): outs[0] is the local
  * [M, ldc] buffer, the others the same location in the peer GPUs' buffers mapped into this process
  * (CUDA IPC / symmetric memory), so the exchange rides on the GEMM's own stores over NVLink.
- * `outs` is a HOST array.  Returns 0, or 100 if the shape does not take the tcgen05 path. */
+ * `outs` is a HOST array.  Returns 0, or 100 if the shape does not take the wgmma path. */
 int cbnb_b200_gemm_4bit_multi_out(const void* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit, const float* absmax_code, const float* absmax_offset, void* const* outs, int n_outs, const void* bias, int M, int N, int K, int ldc, int blocksize, int quant_type, int dtype, bnb_stream_t stream);
 
 /* Which kernel a (M, N, K, blocksize, dtype) 4-bit GEMM takes: 0 = CUDA-core GEMV,
- * 1 = tcgen05 GEMM, 2 = generic CUDA-core kernel, 3 = mma.sync decode kernel (M <= 8).
+ * 1 = wgmma GEMM, 2 = generic CUDA-core kernel, 3 = mma.sync decode kernel (M <= 8).
  * For tests / bench bookkeeping. */
 int cbnb_b200_gemm_4bit_path(int M, int N, int K, int blocksize, int dtype);
 /* Force a path for the next calls on this thread (-1 = automatic). */
 void cbnb_b200_gemm_4bit_force_path(int path);
 
-/* Developer / test entry for the CTA-pair (cta_group::2) large-M kernel (csrc/gemm4_pair.cu): explicit token
- * tile mt (128 | 256 | 384; 0 = automatic), forced K split (0 = production rule; s = every tile s ways;
- * 100 + s = only the partial last wave), optional event trace (device buffer of 2*10*256 + 4*1024 int64, or NULL).
- * Returns 0, or 100 when the shape is not served by that kernel. */
+/* Developer / test entry for the wgmma 4-bit GEMM (csrc/gemm4_tc.cu): explicit token tile mt (16 | 32 | 64 | 128;
+ * 0 = by M) and forced K split per tile (0 = production rule; s = up to s ways, at least one 128-deep stage per
+ * split).  `trace` must be NULL (the name and argument list are kept for ABI stability).  Returns 0, or 100 when
+ * the shape or the options are not served (a forced split must fit one co-resident wave of CTAs). */
 int cbnb_b200_gemm_4bit_pair(const void* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit, const float* absmax_code, const float* absmax_offset, void* out, const void* bias, int M, int N, int K, int ldc, int blocksize, int quant_type, int dtype, int mt, int force_splits, long long* trace, bnb_stream_t stream);
 
 /* Strided-output variant used by the column-sharded linear: out has row stride ldc
@@ -167,7 +167,7 @@ int cbnb_b200_gemm_4bit_pair(const void* A, const uint8_t* B, const float* absma
 void cbnb_b200_gemm_4bit_strided(const void* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit, const float* absmax_code, const float* absmax_offset, void* out, const void* bias, int M, int N, int K, int ldc, int blocksize, int quant_type, int dtype, bnb_stream_t stream);
 
 /* Fused LLM.int8() linear: out[M,N] = T( (CA . CB^T) * SCA[m] * SCB[n] / 127^2 + bias[n] ),
- * int8 tcgen05 GEMM with the dequant epilogue in-kernel (no int32 round trip through HBM).
+ * int8 wgmma GEMM with the dequant epilogue in-kernel (no int32 round trip through HBM).
  * dtype 1 = fp16, 2 = bf16.  Returns 0 / 100 like cigemmlt_32. */
 int cbnb_b200_int8_scaled_mm(const int8_t* CA, const int8_t* CB, const float* SCA, const float* SCB, const void* bias, void* out, int M, int N, int K, int dtype, bnb_stream_t stream);
 

@@ -1,5 +1,5 @@
 """Import shim: makes `import bitsandbytes` resolve to bitsandbytes_b200, so that code written against the
-reference package name (Hugging Face Transformers' bitsandbytes quantizer, PEFT) runs on the B200-native
+reference package name (Hugging Face Transformers' bitsandbytes quantizer, PEFT) runs on the H100-native
 implementation unchanged.  Put this directory's parent (`shim/`) in front of PYTHONPATH; the sibling
 `bitsandbytes-0.50.2.dist-info` answers importlib.metadata's version query (Transformers requires
 bitsandbytes >= 0.46.1) with the version of the reference snapshot whose API is mirrored."""

@@ -1,5 +1,5 @@
 """Shared checker: run a quantize / dequantize implementation over the reference-generated golden
-vectors (tests/golden/reference_vectors.npz).  The GPU suite passes the C-ABI calls of the product
+vectors (tests/golden/reference_vectors_*.npz).  The GPU suite passes the C-ABI calls of the product
 library; the CPU suite passes the oracle, which validates this checker itself.
 
 quantize_fn(A_bits_or_f32: np.ndarray, dtype: str, blocksize, qt, code) -> (codes u8, absmax f32)
@@ -9,14 +9,19 @@ from pathlib import Path
 
 import numpy as np
 
-GOLDEN = Path(__file__).resolve().parent / "golden" / "reference_vectors.npz"
+GOLDEN_DIR = Path(__file__).resolve().parent / "golden"
 Q8_NAMES = ["a", "b", "c", "d", "e", "f", "g", "h"]
 Q4_NAMES = ["a", "b", "c", "d", "e", "f", "g", "h", "i"]
 OUT_DTYPES = ["fp32", "bf16", "fp16"]
 
 
 def load():
-    return np.load(GOLDEN)
+    """All arrays of the golden set (stored in parts of under 1 MB each) as one dict."""
+    out = {}
+    for part in sorted(GOLDEN_DIR.glob("reference_vectors_*.npz")):
+        with np.load(part) as z:
+            out.update({k: z[k] for k in z.files})
+    return out
 
 
 def _canon_zero(bits: np.ndarray) -> np.ndarray:
@@ -89,12 +94,12 @@ def check_gemm4(z, name, gemm_fn):
     M, N, K = (int(v) for v in z[f"{key}_shape"])
     qt = str(z[f"{key}_qt"])
     dt = str(z[f"{key}_dtype"])
-    nested = f"{key}_absmax8" in z.files
+    nested = f"{key}_absmax8" in z
     absmax = z[f"{key}_absmax2"] if nested else z[f"{key}_absmax"]
     a8 = z[f"{key}_absmax8"] if nested else None
     code2 = z[f"{key}_code2"] if nested else None
     offset = float(z[f"{key}_offset"][0]) if nested else None
-    bias = z[f"{key}_bias"] if f"{key}_bias" in z.files else None
+    bias = z[f"{key}_bias"] if f"{key}_bias" in z else None
     got = gemm_fn(z[f"{key}_x"].reshape(-1), dt, z[f"{key}_packed"], absmax, a8, code2, offset, bias, M, N, K, 64, qt)
     got = np.asarray(got, dtype=np.float64).reshape(M, N)
     y_bits = z[f"{key}_y"].reshape(-1)

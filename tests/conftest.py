@@ -10,7 +10,7 @@ if str(ROOT) not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; select with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -19,7 +19,7 @@ def pytest_collection_modifyitems(config, items):
 
     if torch.cuda.is_available():
         return
-    skip = pytest.mark.skip(reason="needs a CUDA device (B200)")
+    skip = pytest.mark.skip(reason="needs a CUDA device (H100)")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)
@@ -40,7 +40,6 @@ def _seed():
 
 @pytest.fixture(scope="session")
 def golden():
-    import numpy as np
+    from tests._golden_check import load
 
-    with np.load(ROOT / "tests" / "golden" / "reference_vectors.npz") as z:
-        return {k: z[k] for k in z.files}
+    return load()

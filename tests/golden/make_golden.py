@@ -229,9 +229,29 @@ def main():
             subprocess.run([sys.executable, __file__, "--phase", which, p], check=True)
             with np.load(p) as z:
                 merged.update({k: z[k] for k in z.files})
-    path = HERE / "reference_vectors.npz"
-    np.savez_compressed(path, **merged)
-    print(f"wrote {path} ({path.stat().st_size} bytes, {len(merged)} arrays)")
+    # parts of under 1 MB each (tests/_golden_check.load merges them), largest arrays first
+    import io
+
+    def size(d):
+        b = io.BytesIO()
+        np.savez_compressed(b, **d)
+        return b.tell()
+
+    parts, cur = [], {}
+    for k in sorted(merged, key=lambda k: -merged[k].nbytes):
+        trial = dict(cur, **{k: merged[k]})
+        if cur and size(trial) > 900_000:
+            parts.append(cur)
+            cur = {k: merged[k]}
+        else:
+            cur = trial
+    parts.append(cur)
+    for old in HERE.glob("reference_vectors_*.npz"):
+        old.unlink()
+    for i, part in enumerate(parts):
+        path = HERE / f"reference_vectors_{i}.npz"
+        np.savez_compressed(path, **part)
+        print(f"wrote {path} ({path.stat().st_size} bytes, {len(part)} arrays)")
 
 
 if __name__ == "__main__":

@@ -1,5 +1,5 @@
 """GPU tests of the public Python surface (functional / autograd / nn / parallel): the call a
-user of the reference would make, on the sm_100a kernels.  Tolerances are the reference's own
+user of the reference would make, on the sm_90a kernels.  Tolerances are the reference's own
 test bounds (cited per test)."""
 import numpy as np
 import pytest

@@ -41,8 +41,8 @@ def _inputs(n, dtype, scale=1.0):
 @pytest.mark.parametrize("qt", [None, "nf4", "fp4"])
 @pytest.mark.parametrize("n,bs", [(4096 * 3, 4096), (64 * 100, 64), (8192 + 37, 256), (1001, 128), (96, 32), (7, 64)])
 def test_dequantize_matches_oracle_and_reference(dtype, qt, n, bs):
-    if qt is None and bs < 64:
-        pytest.skip("8-bit blocksize >= 64")
+    # the reference's 8-bit kernels take blocksize >= 64: below that only the oracle is compared
+    ref_ok = not (qt is None and bs < 64)
     g = torch.Generator(device="cpu").manual_seed(n + bs)
     nbytes = n if qt is None else (n + 1) // 2
     codes = torch.randint(0, 256, (nbytes,), generator=g, dtype=torch.uint8).cuda()
@@ -57,7 +57,7 @@ def test_dequantize_matches_oracle_and_reference(dtype, qt, n, bs):
         np.testing.assert_array_equal(g_bits.view(np.uint32), want.view(np.uint32))
     else:
         np.testing.assert_array_equal(g_bits, want)
-    ref = nat.ref_cuda()
+    ref = nat.ref_cuda() if ref_ok else None
     if ref is not None:
         r = nat.dequantize(ref, codes, absmax, bs, n, qt, code, dtype)
         assert torch.equal(got.view(torch.int32 if dtype == "fp32" else torch.int16),
@@ -107,13 +107,13 @@ def _check_codes_vs_oracle(A_f32, got_codes, got_absmax, bs, qt, code):
 @pytest.mark.parametrize("n,bs", [(4096 * 5, 4096), (4096 * 4, 64), (4096 * 2 + 777, 256), (4096 + 1, 2048),
                                   (999, 128), (64 * 3, 32), (5, 64), (4096 * 3, 512), (4096 * 2, 1024)])
 def test_quantize_bit_exact(dtype, qt, n, bs):
-    if qt is None and bs < 64:
-        pytest.skip("8-bit blocksize >= 64")
+    # the reference's 8-bit kernels take blocksize >= 64: below that only the oracle is compared
+    ref_ok = not (qt is None and bs < 64)
     A = _inputs(n, dtype)
     code = _code() if qt is None else None
     got_q, got_absmax = nat.quantize(nat.lib, A, bs, qt, code, dtype)
     nat.check()
-    ref = nat.ref_cuda()
+    ref = nat.ref_cuda() if ref_ok else None
     if ref is not None:
         ref_q, ref_absmax = nat.quantize(ref, A, bs, qt, code, dtype)
         assert torch.equal(got_absmax, ref_absmax), "absmax differs from the reference CUDA kernel"

@@ -1,4 +1,4 @@
-"""GPU parity: the 4-bit dequant-fused GEMM (tcgen05 and CUDA-core paths) through the C ABI.
+"""GPU parity: the 4-bit dequant-fused GEMM (wgmma and CUDA-core paths) through the C ABI.
 
 Oracle: oracle/oracle_c.c::oracle_gemm_4bit -- exactly-rounded weights
 W_T = rn_T(value * scale), double-precision accumulation.  Tolerance (BASELINE.json
@@ -84,8 +84,6 @@ SHAPES_SMALL = [
 @pytest.mark.parametrize("path", [1, 0], ids=["tcgen05", "simt"])
 @pytest.mark.parametrize("M,N,K", SHAPES_SMALL)
 def test_bf16_nf4_vs_oracle(path, M, N, K):
-    if path == 0 and M > 64:
-        pytest.skip("SIMT path is only dispatched for small M; covered at M <= 64")
     p = make_problem(M, N, K, "nf4", "bf16")
     nat.lib.cbnb_b200_gemm_4bit_force_path(path)
     try:

@@ -194,7 +194,7 @@ def test_fp4_double_quant_at_the_c4_shard_shape(M):
         assert rel_ref.item() <= 1e-3, rel_ref.item()
 
 
-# ------------------------------------------------------------------------------------------ CTA-pair kernel (large M)
+# ------------------------------------------------------------------------------------------ tensor-core kernel, large M
 @pytest.mark.parametrize("M,N,K,qt,dtype,kw", [
     (512, 256, 128, "nf4", "bf16", {}), (600, 512, 320, "fp4", "fp16", dict(bias=True)),
     (513, 384, 192, "nf4", "bf16", dict(nested=True)), (1000, 1024, 1024, "nf4", "bf16", {}),
@@ -202,15 +202,28 @@ def test_fp4_double_quant_at_the_c4_shard_shape(M):
     (2048, 2304, 2048, "nf4", "bf16", dict(bias=True)),
 ])
 def test_pair_kernel_vs_oracle_and_one_cta_kernel(M, N, K, qt, dtype, kw):
-    """The cta_group::2 kernel (every token tile, with and without the two-way K split of the last wave) against
-    the double-precision oracle, and -- without a split, where the fp32 summation order is the same -- bit for bit
-    against the one-CTA tcgen05 kernel."""
+    """The wgmma kernel at large M (every token tile, with and without a forced K split) against the
+    double-precision oracle, and -- without a split, where the fp32 summation order is the same -- bit for bit
+    across token tiles."""
     p = make_problem(M, N, K, qt, dtype, **kw)
     y64 = exact(p) if M * N * K <= 2**31 else None
     nat.lib.cbnb_b200_gemm_4bit_force_path(1)
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    kblocks = -(-K // 128)
+
+    def splits_of(mt, sp):
+        """(splits the launcher makes of a forced sp, whether it serves them): >= one 128-deep stage per split, and
+        a split grid must be one co-resident wave (one CTA per SM)"""
+        v = min(sp, kblocks, 16)
+        per = -(-kblocks // v)
+        s = -(-kblocks // per)
+        return s, s == 1 or -(-N // 128) * -(-M // mt) * s <= sms
+
     base = None
-    for mt in (128, 256, 384):
-        for sp in (1, 2, 102):
+    ran_split = False
+    for mt in (32, 64, 128):
+        for sp in (1, 2, 3):
+            s, served = splits_of(mt, sp)
             out = torch.full((M, N), float("nan"), device="cuda", dtype=nat.DTYPE[dtype])
             rc = nat.lib.cbnb_b200_gemm_4bit_pair(
                 nat.ptr(p["x"]), nat.ptr(p["packed"]), nat.ptr(p["absmax"]), nat.ptr(p["absmax_8bit"]),
@@ -218,9 +231,11 @@ def test_pair_kernel_vs_oracle_and_one_cta_kernel(M, N, K, qt, dtype, kw):
                 nat.QT_ID[qt], nat.DTYPE_ID[dtype], mt, sp, None, nat.stream())
             torch.cuda.synchronize()
             nat.check()
-            if rc == 100 and sp == 2:
-                continue  # forcing a split of EVERY tile can exceed the fixed 32 MB split-K workspace: not served
+            if not served:
+                assert rc == 100, (mt, sp)  # the splits of a tile wait for each other: refused, not run
+                continue
             assert rc == 0, (mt, sp)
+            ran_split |= s > 1
             if y64 is not None:
                 assert_close_to_exact(out, y64, dtype, K)
             if sp == 1:
@@ -228,6 +243,9 @@ def test_pair_kernel_vs_oracle_and_one_cta_kernel(M, N, K, qt, dtype, kw):
                     base = out
                 assert torch.equal(out.view(torch.int16), base.view(torch.int16)), f"mt={mt}: token tiles disagree"
     nat.lib.cbnb_b200_gemm_4bit_force_path(-1)
+    # a split ran, unless K is one stage or even the widest token tile's grid, split in two, exceeds one wave
+    if kblocks > 1 and -(-N // 128) * -(-M // 128) * 2 <= sms:
+        assert ran_split
     if y64 is None:
         W = nat.dequantize(nat.lib, p["packed"], p["absmax"], p["bs"], N * K, qt, None, dtype).view(N, K)
         want = p["x"].float() @ W.float().t() + (p["bias"].float() if p["bias"] is not None else 0)
@@ -235,8 +253,8 @@ def test_pair_kernel_vs_oracle_and_one_cta_kernel(M, N, K, qt, dtype, kw):
 
 
 def test_pair_kernel_multi_destination_tma_stores():
-    """The fused all-gather epilogue of the pair kernel on one GPU: three destination buffers (one bulk tensor store
-    each per tile) receive this shard's columns of a wider output; nothing else is touched; M tail and N tail."""
+    """The fused all-gather epilogue of the tensor-core kernel at large M on one GPU: three destination buffers
+    receive this shard's columns of a wider output; nothing else is touched; M tail and N tail."""
     import ctypes as ct
 
     M, N, K, NF = 1100, 320, 512, 1024
@@ -254,7 +272,7 @@ def test_pair_kernel_multi_destination_tma_stores():
     for b in bufs:
         assert torch.equal(b[:, col0:col0 + N], want)
         assert (b[:, :col0] == -7.0).all() and (b[:, col0 + N:] == -7.0).all()
-    # an output whose row pitch is not a multiple of 16 bytes takes the direct-store epilogue: same result
+    # an output whose row pitch is not a multiple of 16 bytes: same result
     odd = torch.full((M, N + 3), -7.0, dtype=torch.bfloat16, device="cuda")
     nat.lib.cbnb_b200_gemm_4bit_strided(nat.ptr(p["x"]), nat.ptr(p["packed"]), nat.ptr(p["absmax"]), None, None, None,
                                         odd.data_ptr(), nat.ptr(p["bias"]), M, N, K, N + 3, p["bs"], nat.QT_ID["nf4"], 2,
@@ -279,8 +297,8 @@ def test_one_process_drives_two_devices():
         W = (torch.randn(512, 1024) / 32).to(torch.bfloat16).to(dev)
         x = torch.randn(700, 1024).to(torch.bfloat16).to(dev)
         qW, qs = F.quantize_4bit(W, quant_type="nf4")
-        y_big = bnb.matmul_4bit(x, qW.t(), qs)          # pair kernel
-        y_mid = bnb.matmul_4bit(x[:100], qW.t(), qs)    # one-CTA tcgen05 kernel
+        y_big = bnb.matmul_4bit(x, qW.t(), qs)          # wgmma kernel, 128-token tiles
+        y_mid = bnb.matmul_4bit(x[:100], qW.t(), qs)    # wgmma kernel, one token tile
         y_small = bnb.matmul_4bit(x[:24], qW.t(), qs)   # split-K
         A8 = torch.randint(-127, 128, (300, 1024), dtype=torch.int8, device=dev)
         B8 = torch.randint(-127, 128, (256, 1024), dtype=torch.int8, device=dev)

@@ -82,7 +82,7 @@ def test_reference_python_layer_runs_on_our_library(tmp_path):
     assert same(q, ref["q"]) and same(qs.absmax, ref["absmax"]) and same(F.dequantize_4bit(q, qs), ref["deq"])
     for M in (1, 8, 700):
         # The reference's Python layer picks its own route per shape (its legacy gemv symbol for one token, its
-        # dequantize + cuBLAS fallback on sm_100 for most others, reference backends/cuda/ops.py:583-623, 904-916),
+        # dequantize + cuBLAS fallback on sm_90 for most others, reference backends/cuda/ops.py:583-623, 904-916),
         # so its result and our fused GEMM's share the weights but not the fp32 summation order: the tolerance is
         # BASELINE.json's (<= 1e-3 relative for bf16 GEMM outputs); everything elementwise below is bit for bit.
         ours = bnb.matmul_4bit(ref[f"x{M}"].cuda(), q.t(), qs)

@@ -1,4 +1,4 @@
-"""GPU parity against the committed golden fixtures (tests/golden/reference_vectors.npz: outputs of the
+"""GPU parity against the committed golden fixtures (tests/golden/reference_vectors_*.npz: outputs of the
 reference's own CPU backend and pure-torch kernels on seeded inputs, edge sizes included), through the
 product's C ABI.  The checker (tests/_golden_check.py) is validated on CPU with the oracle as the
 implementation (tests/test_oracle_pinned.py).  This file sorts last on purpose: it was added after the
@@ -13,7 +13,7 @@ pytestmark = pytest.mark.gpu
 
 
 # ---------------------------------------------------------------------------- golden vectors
-# The reference-generated fixtures (tests/golden/reference_vectors.npz: the reference's own CPU
+# The reference-generated fixtures (tests/golden/reference_vectors_*.npz: the reference's own CPU
 # backend and pure-torch kernels on seeded inputs, edge sizes included) through the product's C ABI.
 def _gpu_quantize(A, dtype, bs, qt, code):
     if dtype == "fp32":
@@ -64,8 +64,8 @@ def _gpu_gemm4(x_bits, dt, packed, absmax, a8, code2, offset, bias_bits, M, N, K
 @pytest.mark.parametrize("path", [-1, 1], ids=["auto", "tcgen05"])
 @pytest.mark.parametrize("name", ["plain", "nested", "fp16"])
 def test_golden_vectors_gemm4(name, path):
-    """The reference's public API on its CPU backend (tests/golden/reference_vectors.npz) vs the product kernels
-    (the decode kernel by default at these M; the tcgen05 kernel when forced)."""
+    """The reference's public API on its CPU backend (tests/golden/reference_vectors_*.npz) vs the product kernels
+    (the decode kernel by default at these M; the wgmma kernel when forced)."""
     from tests import _golden_check as gc
 
     nat.lib.cbnb_b200_gemm_4bit_force_path(path)
@@ -77,7 +77,7 @@ def test_golden_vectors_gemm4(name, path):
 
 # ---------------------------------------------------------------------------- golden vectors
 def test_golden_vectors_int8_gemm_and_dequant():
-    """tests/golden/reference_vectors.npz (the reference's int8_linear_matmul / int8_mm_dequant on CPU) through the
+    """tests/golden/reference_vectors_*.npz (the reference's int8_linear_matmul / int8_mm_dequant on CPU) through the
     C ABI: the int8 GEMM exactly, the dequantisation within one fp16 ulp (the reference's torch kernel multiplies
     in a different order)."""
     from tests import _golden_check as gc

@@ -39,7 +39,7 @@ def test_library_loads_and_exports_every_declared_symbol():
         if n.startswith(("cigemmlt_8",)):
             continue
         assert n in table, f"{n} has no ctypes signature in cextension.py"
-    assert "sm_100a" in cextension.lib.build_info()
+    assert "sm_90a" in cextension.lib.build_info()
 
 
 def test_reference_abi_names_present():
@@ -81,7 +81,7 @@ def test_entry_points_validate_arguments_before_touching_the_device():
     assert path(1, 4096, 4096, 64, 2) == 0      # CUDA-core GEMV
     assert path(4, 4096, 4096, 64, 2) == 3      # mma.sync decode kernel
     assert path(8, 4096, 4096, 64, 1) == 3
-    assert path(9, 4096, 4096, 64, 2) == 1      # tcgen05
+    assert path(9, 4096, 4096, 64, 2) == 1      # wgmma GEMM
     assert path(4096, 4096, 4096, 64, 2) == 1
     assert path(4, 4096, 4096, 64, 0) == 2      # fp32 activations: generic CUDA-core kernel
     assert path(4, 4096, 4000, 64, 2) == 2      # K % 64 != 0
