@@ -125,9 +125,11 @@ bool encode_tmap_2d(CUtensorMap* out, const void* base, int elem_bytes, int swiz
     cuuint64_t gstride[1] = {row_stride_bytes};
     cuuint32_t box[2] = {box_cols, box_rows};
     cuuint32_t estr[2] = {1, 1};
-    CUresult r = fn(out, dt, 2, const_cast<void*>(base), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                    swizzle_bytes == 0 ? CU_TENSOR_MAP_SWIZZLE_NONE
-                                       : (swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B),
+    const CUtensorMapSwizzle swz = swizzle_bytes == 0    ? CU_TENSOR_MAP_SWIZZLE_NONE
+                                   : swizzle_bytes == 32 ? CU_TENSOR_MAP_SWIZZLE_32B
+                                   : swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
+                                                         : CU_TENSOR_MAP_SWIZZLE_128B;
+    CUresult r = fn(out, dt, 2, const_cast<void*>(base), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swz,
                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) {
@@ -350,8 +352,8 @@ int cbnb_b200_gemm_4bit_multi_out(const void* A, const uint8_t* B, const float* 
 }
 
 // Developer / test entry: the tensor-core kernel of gemm4_tc.cu with an explicit token tile (mt = 16 | 32 | 64 |
-// 128, 0 = automatic) and a forced K split per tile (0 = the production rule).  `trace` must be NULL.  Returns 0, or
-// 100 when the shape or the options are not served by that kernel.
+// 128 | 256, 0 = automatic) and a forced K split per tile (0 = the production rule).  `trace` must be NULL.  Returns
+// 0, or 100 when the shape or the options are not served by that kernel.
 int cbnb_b200_gemm_4bit_pair(const void* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
                              const float* absmax_code, const float* absmax_offset, void* out, const void* bias, int M,
                              int N, int K, int ldc, int blocksize, int quant_type, int dtype, int mt, int force_splits,

@@ -11,12 +11,17 @@ struct ScaleSrc {
     const uint8_t* absmax_8bit;
     const float* absmax_code;
     float offset;
-    __device__ __forceinline__ float load(long long idx) const {
-        if (absmax_8bit != nullptr) {
+    // DQ: double quant, known at compile time (the kernel then carries only one of the two chains)
+    template <bool DQ> __device__ __forceinline__ float load_as(long long idx) const {
+        if constexpr (DQ) {
             const float c = __ldg(absmax_code + __ldg(absmax_8bit + idx));
             return __fadd_rn(mul_ftz(c, __ldg(absmax + (idx >> 8))), offset);
+        } else {
+            return __ldg(absmax + idx);
         }
-        return __ldg(absmax + idx);
+    }
+    __device__ __forceinline__ float load(long long idx) const {
+        return absmax_8bit != nullptr ? load_as<true>(idx) : load_as<false>(idx);
     }
 };
 

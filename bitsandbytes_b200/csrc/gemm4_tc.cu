@@ -12,22 +12,25 @@
 //
 // Design ("swap-AB, weights through registers"):
 //   * The wgmma M dimension (64 rows per warpgroup, two warpgroups) carries the OUTPUT FEATURES n;
-//     the tokens m are the wgmma N dimension (MT = 16..128).  A CTA owns out[m0:m0+MT, n0:n0+128].
-//   * A pipeline stage is 128 k-elements.  One TMA producer warp stages, per stage, the packed codes
-//     of the CTA's 128 rows (128 x 64 B, 64-byte swizzle, 8 KB) and the activation tile
-//     X[m0:m0+MT, k0:k0+128] (two 128-byte-swizzled sub-tiles), the K-major B operand of wgmma.
-//   * Every consumer thread decodes the codes of its two rows straight into the register fragment of
-//     wgmma's A operand, with the exact reference rounding -- a per-block 16-entry table built with
-//     16 FMUL + 8 cvt.rn and looked up with PRMT only.  The decoded weights never pass through shared
-//     memory, whose bandwidth is then left to the activation operand.
+//     the tokens m are the wgmma N dimension (MT = 16..256).  A CTA owns out[m0:m0+MT, n0:n0+128].
+//   * A pipeline stage is BK k-elements (128; 64 at MT = 256).  Thread 0 stages with TMA, per stage,
+//     the packed codes of the CTA's 128 rows (128 x BK/2 bytes, BK/2-byte swizzle) and the activation tile
+//     X[m0:m0+MT, k0:k0+BK] (BK/64 128-byte-swizzled sub-tiles), the K-major B operand of wgmma.
+//   * Every consumer thread reads the codes of its two rows for the whole stage (ld.shared, 16 bytes per
+//     32 codes) and decodes them straight into the register fragment of wgmma's A operand, with the exact
+//     reference rounding -- a per-block 16-entry table built with 16 FMUL + 8 cvt.rn, once per (row,
+//     quantisation block) in the stage, and looked up with PRMT only.  The decoded weights never pass
+//     through shared memory, whose bandwidth is then left to the activation operand.
 //   * Two A-fragment register sets alternate between stages, so the decode of stage i+1 overlaps the
 //     wgmma of stage i (wgmma.wait_group 1 before a set is overwritten).
-//   * Accumulators live in registers; the epilogue adds the bias, rounds to T and stores, or -- for
-//     split-K, which fills the 132 SMs when the tile grid is small -- writes fp32 partials to an
-//     L2-resident workspace with a last-arriver reduction in deterministic split order.
+//   * Accumulators live in registers; the epilogue adds the bias, rounds to T, stages the tile in shared
+//     memory and stores it in 16-byte row pieces, or -- for split-K, which fills the 132 SMs when the tile
+//     grid is small -- writes fp32 partials to an L2-resident workspace with a last-arriver reduction in
+//     deterministic split order.
 //
-// Warp roles (288 threads): warps 0..7 = two consumer warpgroups (decode + wgmma + epilogue),
-// warp 8 = TMA producer.
+// 256 threads = two warpgroups (decode + wgmma + epilogue); thread 0 also issues the TMA loads.  There is no
+// producer warp: a ninth warp puts three warps on one SM sub-partition, whose 16K registers then cap every thread
+// at 168 -- too few for the 256-token tile (128 accumulators, two A-fragment sets, the decode state).
 #include "common.cuh"
 #include "decode4.cuh"
 #include "hopper_ptx.cuh"
@@ -40,10 +43,9 @@ namespace bnb200 {
 
 namespace {
 
-constexpr int kBK = 128;           // pipeline stage: 128 k-elements = two 128-byte swizzle atoms of X per row
 constexpr int kTileN = 128;        // output features per CTA (two warpgroups of 64)
 constexpr int kConsumers = 256;    // threads of the two consumer warpgroups
-constexpr int kThreads = kConsumers + 32;
+constexpr int kThreads = kConsumers;
 
 struct Gemm4Params {
     const uint8_t* B;            // packed codes [N, K/2]
@@ -55,11 +57,13 @@ struct Gemm4Params {
     void* out;                   // T[M, ldc]
     void* peer_out[7];           // further copies of the output tile (peer GPUs' gather buffers, same ldc): the
     int n_peers;                 //   epilogue stores every element to all of them (fused all-gather)
+    int out_vec;                 // every output base is 16-byte aligned and ldc % 8 == 0: 16-byte stores
     float* ws_partial;           // split-K partials [tiles][splits][MT][128]
     int* ws_counter;             // two per output tile, zero on entry, reset on exit
     int M, N, K, ldc;
     int log2_bs;
-    int kblocks_total;           // number of 128-wide stages = ceil(K / 128)
+    int scale_mask;              // a new quantisation block can start only at 32-code chunks q with (q & mask) == 0
+    int kblocks_total;           // number of stages = ceil(K / BK)
     int n_tiles;                 // N tiles of 128 (tile = m_tile * n_tiles + n_tile)
     int tiles_total;
     int splits;                  // K splits per tile (1 = none)
@@ -75,46 +79,64 @@ __device__ __forceinline__ void wgmma_step(float (&d)[MT / 2], const uint32_t (&
         if constexpr (bf) ptx::wgmma_m64n32k16_bf16_rs(d, a, b_desc); else ptx::wgmma_m64n32k16_f16_rs(d, a, b_desc);
     } else if constexpr (MT == 64) {
         if constexpr (bf) ptx::wgmma_m64n64k16_bf16_rs(d, a, b_desc); else ptx::wgmma_m64n64k16_f16_rs(d, a, b_desc);
-    } else {
-        static_assert(MT == 128, "token tile");
+    } else if constexpr (MT == 128) {
         if constexpr (bf) ptx::wgmma_m64n128k16_bf16_rs(d, a, b_desc); else ptx::wgmma_m64n128k16_f16_rs(d, a, b_desc);
+    } else {
+        static_assert(MT == 256, "token tile");
+        if constexpr (bf) ptx::wgmma_m64n256k16_bf16_rs(d, a, b_desc); else ptx::wgmma_m64n256k16_f16_rs(d, a, b_desc);
     }
 }
 
-// Pipeline stage = 128 k-elements: two 64-wide (128-byte, swizzle-atom) activation sub-tiles and the
-// packed codes of 128 rows.  Ring depth: as many stages as fit next to each other in 200 KB.
+// Pipeline stage = BK k-elements: BK/64 64-wide (128-byte, swizzle-atom) activation sub-tiles and the packed codes
+// of 128 rows.  Ring depth: as many stages as fit next to each other in 220 KB.  The 256-token tile takes 64-deep
+// stages: a 128-deep one (72 KB) leaves room for two stages only, and two 128-deep A-fragment sets (64 registers)
+// next to its 128 accumulators would not fit the consumers' register budget.
 template <int MT> struct StageCfg {
+    static constexpr int kBK = MT == 256 ? 64 : 128;
+    static constexpr int kSteps = kBK / 16;                      // wgmma k16 steps
+    static constexpr int kChunks = kBK / 32;                     // 16-byte (32-code) pieces of a code row
     static constexpr int kXSubBytes = MT * 128;                  // one 64-wide sub-tile
-    static constexpr int kXStageBytes = 2 * kXSubBytes;
-    static constexpr int kWStageBytes = kTileN * 64;             // packed codes: 128 rows x 64 B (TMA, 64-B swizzle)
+    static constexpr int kXStageBytes = (kBK / 64) * kXSubBytes;
+    static constexpr int kWRowBytes = kBK / 2;                   // packed codes of one row (TMA, kWRowBytes-byte swizzle)
+    static constexpr int kWStageBytes = kTileN * kWRowBytes;
     static constexpr int kStageBytes = kXStageBytes + kWStageBytes;
-    static constexpr int kStages = (200 * 1024 / kStageBytes) > 8 ? 8 : (200 * 1024 / kStageBytes);
+    static constexpr int kStages = (220 * 1024 / kStageBytes) > 8 ? 8 : (220 * 1024 / kStageBytes);
+    // epilogue staging: one output row of the tile (128 x T) plus 16 bytes, so that the fragment stores (four
+    // token rows two apart per warp instruction) fall on distinct banks
+    static constexpr int kOutPitch = kTileN * 2 + 16;
+    static_assert(MT * kOutPitch <= kStages * kStageBytes, "epilogue staging reuses the stage ring");
 };
 
-// The 16 codes of stage-row words w[4q .. 4q+3] that this thread's A fragments need (byte `t` of each,
-// t = lane % 4): wgmma k16 step 2q+u reads byte t of words 4q+2u (k 2t, 2t+1) and 4q+2u+1 (k 8+2t, 9+2t).
+// The 16 codes of a 16-byte chunk (stage-row words w[4q .. 4q+3]) that this thread's A fragments need (byte `t` of
+// each, t = lane % 4): wgmma k16 step 2q+u reads byte t of words 4q+2u (k 2t, 2t+1) and 4q+2u+1 (k 8+2t, 9+2t).
 __device__ __forceinline__ uint32_t gather_bytes(uint4 v, uint32_t sel) {
     return prmt(prmt(v.x, v.y, sel), prmt(v.z, v.w, sel), 0x5410);
 }
 
-template <typename T, int QT, int MT>
+template <typename T, int QT, int MT, bool DQ>
 __global__ void __launch_bounds__(kThreads, 1)
     gemm4_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
                     const Gemm4Params p) {
     using Cfg = StageCfg<MT>;
+    constexpr int kBK = Cfg::kBK;
+    constexpr int kSteps = Cfg::kSteps;
+    constexpr int kChunks = Cfg::kChunks;
     constexpr int kStages = Cfg::kStages;
     constexpr int kXSubBytes = Cfg::kXSubBytes;
     constexpr int kXStageBytes = Cfg::kXStageBytes;
+    constexpr int kWRowBytes = Cfg::kWRowBytes;
     constexpr int kWStageBytes = Cfg::kWStageBytes;
 
     // ------------------------------------------------------------------ shared memory
+    // aligned by an offset from the __shared__ array itself, so that the compiler keeps the shared address space
+    // (ld.shared for the codes, not generic loads)
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t* sx = smem;                              // [kStages][2][MT x 128 B]   activations
-    uint8_t* sw = smem + kStages * kXStageBytes;     // [kStages][128 x 64 B]      packed codes
+    uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
+    uint8_t* sx = smem;                              // [kStages][BK/64][MT x 128 B]   activations
+    uint8_t* sw = smem + kStages * kXStageBytes;     // [kStages][128 x BK/2 B]        packed codes
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes);
     uint64_t* full = bars;                   // [kStages] TMA (1 arrive + bytes) -> consumers
-    uint64_t* empty = bars + kStages;        // [kStages] the 8 consumer warps -> TMA producer
+    uint64_t* empty = bars + kStages;        // [kStages] the 8 warps -> thread 0 (stage free for the next load)
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -141,31 +163,25 @@ __global__ void __launch_bounds__(kThreads, 1)
     }
     __syncthreads();
 
-    if (warp == kConsumers / 32) {
-        // ================================================================== TMA producer
-        if (ptx::elect_one()) {
-            ptx::prefetch_tmap(&tmap_x);
-            ptx::prefetch_tmap(&tmap_w);
-            int s = 0;
-            uint32_t ph = 0;
-            for (int i = 0; i < nst; ++i) {
-                ptx::mbar_wait(&empty[s], ph ^ 1u);
-                const int k0 = (st_begin + i) * kBK;
-                ptx::mbar_arrive_expect_tx(&full[s], kWStageBytes + kXStageBytes);
-                // packed codes of this CTA's 128 output features: bytes [k0/2, k0/2 + 64) of rows n0..n0+127
-                ptx::tma_load_2d(sw + s * kWStageBytes, &tmap_w, &full[s], k0 / 2, n0);
-                uint8_t* dst = sx + s * kXStageBytes;
-                // rows past M, rows past N and columns past K are out of bounds for the tensor maps: TMA zero-fills
+    // stage j of this split into ring slot j % kStages, issued by thread 0; rows past M, rows past N and columns past K
+    // are out of bounds for the tensor maps: TMA zero-fills
+    const bool issuer = threadIdx.x == 0;
+    auto load_stage = [&](int j) {
+        const int slot = j % kStages;
+        const int k0 = (st_begin + j) * kBK;
+        ptx::mbar_arrive_expect_tx_if(issuer, &full[slot], kWStageBytes + kXStageBytes);
+        // packed codes of this CTA's 128 output features: bytes [k0/2, k0/2 + BK/2) of rows n0..n0+127
+        ptx::tma_load_2d_if(issuer, sw + slot * kWStageBytes, &tmap_w, &full[slot], k0 / 2, n0);
 #pragma unroll
-                for (int h = 0; h < 2; ++h) ptx::tma_load_2d(dst + h * kXSubBytes, &tmap_x, &full[s], k0 + 64 * h, m0);
-                if (++s == kStages) {
-                    s = 0;
-                    ph ^= 1u;
-                }
-            }
-        }
-        return;
+        for (int h = 0; h < kBK / 64; ++h)
+            ptx::tma_load_2d_if(issuer, sx + slot * kXStageBytes + h * kXSubBytes, &tmap_x, &full[slot], k0 + 64 * h,
+                                    m0);
+    };
+    if (issuer) {
+        ptx::prefetch_tmap(&tmap_x);
+        ptx::prefetch_tmap(&tmap_w);
     }
+    for (int j = 0; j < kStages && j < nst; ++j) load_stage(j);
 
     // ====================================================================== consumers
     const int wg = warp >> 2;                 // warpgroup: feature rows [64 wg, 64 wg + 64) of the tile
@@ -175,21 +191,25 @@ __global__ void __launch_bounds__(kThreads, 1)
     const bool a_ok = na < p.N, b_ok = nb < p.N;
     const long long e_a = (long long)(a_ok ? na : 0) * p.K;
     const long long e_b = (long long)(b_ok ? nb : 0) * p.K;
-    const ScaleSrc sc{p.absmax, p.absmax_8bit, p.absmax_code, p.absmax_offset ? __ldg(p.absmax_offset) : 0.0f};
+    const ScaleSrc sc{p.absmax, p.absmax_8bit, p.absmax_code, (DQ && p.absmax_offset) ? __ldg(p.absmax_offset) : 0.0f};
     const uint32_t sel = (uint32_t)t | ((uint32_t)(t + 4) << 4);
-    // 64-byte swizzle of the code rows: 16-byte chunk c of row r sits at chunk c ^ ((r >> 1) & 3)
-    const uint32_t swz_a = (uint32_t)((row0 >> 1) & 3), swz_b = (uint32_t)(((row0 + 8) >> 1) & 3);
+    const uint32_t smask = (uint32_t)p.scale_mask;
+    // the TMA swizzle of the code rows: 16-byte chunk c of row r sits at chunk c ^ ((r * kWRowBytes / 128) % kChunks)
+    const uint32_t swz[2] = {(uint32_t)((row0 * kWRowBytes) >> 7) & (kChunks - 1),
+                             (uint32_t)(((row0 + 8) * kWRowBytes) >> 7) & (kChunks - 1)};
 
-    // Scales of one stage: the 32 codes of a gathered word lie inside one quantisation block (blocks are
-    // >= 32 and aligned), so each (row, q) needs one scale.  Fetched one stage ahead.
-    float scl[2][4];
+    // Scales of one stage, one per (row, quantisation block): the 32 codes of a chunk lie inside one block (blocks
+    // are >= 32 and aligned), and a block can begin only at a chunk q with (q & smask) == 0.  Fetched one stage ahead.
+    float scl[2][kChunks];
     auto fetch = [&](int i) {
         const long long kk = (long long)(st_begin + i) * kBK;
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-            const bool in_k = i < nst && kk + 32 * q < p.K;
-            scl[0][q] = (in_k && a_ok) ? sc.load((e_a + kk + 32 * q) >> p.log2_bs) : 0.f;
-            scl[1][q] = (in_k && b_ok) ? sc.load((e_b + kk + 32 * q) >> p.log2_bs) : 0.f;
+        for (int q = 0; q < kChunks; ++q) {
+            if ((q & smask) == 0) {
+                const bool in_k = i < nst && kk + 32 * q < p.K;
+                scl[0][q] = (in_k && a_ok) ? sc.load_as<DQ>((e_a + kk + 32 * q) >> p.log2_bs) : 0.f;
+                scl[1][q] = (in_k && b_ok) ? sc.load_as<DQ>((e_b + kk + 32 * q) >> p.log2_bs) : 0.f;
+            }
         }
     };
 
@@ -197,32 +217,25 @@ __global__ void __launch_bounds__(kThreads, 1)
 #pragma unroll
     for (int j = 0; j < MT / 2; ++j) acc[j] = 0.f;
 
-    uint32_t afr[2][8][4];  // two A-fragment sets: [set][k16 step][reg]
+    uint32_t afr[2][kSteps][4];  // two A-fragment sets: [set][k16 step][reg]
 
-    // decode stage i (smem stage s) into A set `set`
-    auto decode = [&](int s, uint32_t (&a)[8][4]) {
+    // decode stage i (smem stage s) into A set `a`: all of the stage's code loads first, then the tables and PRMTs
+    auto decode = [&](int s, uint32_t (&a)[kSteps][4]) {
         const uint8_t* wt = sw + s * kWStageBytes;
-        float sc_cur[2][4];
+        uint4 v[2][kChunks];
 #pragma unroll
         for (int r = 0; r < 2; ++r)
 #pragma unroll
-            for (int q = 0; q < 4; ++q) sc_cur[r][q] = scl[r][q];
+            for (int q = 0; q < kChunks; ++q)
+                v[r][q] = *reinterpret_cast<const uint4*>(wt + (row0 + 8 * r) * kWRowBytes + (((uint32_t)q ^ swz[r]) << 4));
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
-            const uint8_t* rowp = wt + (row0 + 8 * r) * 64;
-            const uint32_t swz = r ? swz_b : swz_a;
             DecodeTable tab;
-            float last = 0.f;
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
-                const uint4 v = *reinterpret_cast<const uint4*>(rowp + (((uint32_t)q ^ swz) << 4));
-                const uint32_t word = gather_bytes(v, sel);
-                if (q == 0 || sc_cur[r][q] != last) {
-                    build_table<T, QT>(sc_cur[r][q], tab);
-                    last = sc_cur[r][q];
-                }
+            for (int q = 0; q < kChunks; ++q) {
+                if ((q & smask) == 0) build_table<T, QT>(scl[r][q], tab);
                 uint32_t o[4];
-                decode_word(word, tab, o);
+                decode_word(gather_bytes(v[r][q], sel), tab, o);
                 // o[i]: byte i of the gathered word = word 4q+i of the row -> k16 step 2q + i/2, half i%2
 #pragma unroll
                 for (int u = 0; u < 2; ++u) {
@@ -233,13 +246,12 @@ __global__ void __launch_bounds__(kThreads, 1)
         }
     };
 
-    auto mma_stage = [&](int s, const uint32_t (&a)[8][4]) {
+    auto mma_stage = [&](int s, const uint32_t (&a)[kSteps][4]) {
         const uint32_t xs = ptx::smem_u32(sx + s * kXStageBytes);
-        const uint64_t d0 = ptx::make_sw128_kmajor_desc(xs);
-        const uint64_t d1 = ptx::make_sw128_kmajor_desc(xs + kXSubBytes);
         ptx::wgmma_fence();
 #pragma unroll
-        for (int j = 0; j < 8; ++j) wgmma_step<T, MT>(acc, a[j], (j < 4 ? d0 : d1) + 2 * (j & 3));
+        for (int j = 0; j < kSteps; ++j)
+            wgmma_step<T, MT>(acc, a[j], ptx::make_sw128_kmajor_desc(xs + (j >> 2) * kXSubBytes) + 2 * (j & 3));
         ptx::wgmma_commit();
     };
 
@@ -262,6 +274,14 @@ __global__ void __launch_bounds__(kThreads, 1)
                     if (lane == 0) ptx::mbar_arrive(&empty[prev_s]);
                 }
                 prev_s = s;
+                // refill the slot of stage i - 2 (every warp released it one iteration ago, so the wait is short and
+                // the two warpgroups are not tied to each other stage by stage); kStages - 2 stages stay in flight.
+                // Every thread takes the same path, thread 0 alone issues (see tma_load_2d_if).
+                const int j = i - 2 + kStages;
+                if (i >= 2 && j < nst) {
+                    ptx::mbar_wait(&empty[j % kStages], (uint32_t)((i - 2) / kStages) & 1u);
+                    load_stage(j);
+                }
             }
         }
     }
@@ -276,18 +296,33 @@ __global__ void __launch_bounds__(kThreads, 1)
         const T* bias = reinterpret_cast<const T*>(p.bias);
         const float bias_a = (bias != nullptr && a_ok) ? DT<T>::to_f32(bias[na]) : 0.f;
         const float bias_b = (bias != nullptr && b_ok) ? DT<T>::to_f32(bias[nb]) : 0.f;
+        // Stage the rounded tile as [token][feature] rows in the stage ring -- free once both warpgroups' last
+        // wgmma has completed -- then store it in 16-byte row pieces: each token row of the tile is 256
+        // contiguous bytes of the output.
+        constexpr int kPitch = Cfg::kOutPitch;
+        asm volatile("bar.sync 1, 256;" ::: "memory");
 #pragma unroll
-        for (int j = 0; j < MT / 8; ++j) {
+        for (int j = 0; j < MT / 8; ++j)
 #pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const int m = m0 + 8 * j + 2 * t + (e & 1);
-                const bool hi = e >= 2;
-                const int n = hi ? nb : na;
-                if ((hi ? b_ok : a_ok) && m < p.M) {
-                    const T val = DT<T>::from_f32(acc[4 * j + e] + (hi ? bias_b : bias_a));
-                    const long long idx = (long long)m * p.ldc + n;
-                    outp[idx] = val;
-                    for (int r = 0; r < p.n_peers; ++r) reinterpret_cast<T*>(p.peer_out[r])[idx] = val;
+            for (int e = 0; e < 4; ++e)
+                *reinterpret_cast<T*>(smem + (8 * j + 2 * t + (e & 1)) * kPitch + (row0 + 8 * (e >> 1)) * 2) =
+                    DT<T>::from_f32(acc[4 * j + e] + (e >= 2 ? bias_b : bias_a));
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        for (int idx = threadIdx.x; idx < MT * (kTileN / 8); idx += kConsumers) {
+            const int c = idx / (kTileN / 8), n = n0 + 8 * (idx % (kTileN / 8));
+            const int m = m0 + c;
+            if (m >= p.M || n >= p.N) continue;
+            const uint8_t* src = smem + c * kPitch + (n - n0) * 2;
+            const long long o = (long long)m * p.ldc + n;
+            if (p.out_vec && n + 8 <= p.N) {
+                const uint4 val = *reinterpret_cast<const uint4*>(src);
+                *reinterpret_cast<uint4*>(outp + o) = val;
+                for (int r = 0; r < p.n_peers; ++r) *reinterpret_cast<uint4*>(reinterpret_cast<T*>(p.peer_out[r]) + o) = val;
+            } else {
+                for (int x = 0; x < 8 && n + x < p.N; ++x) {
+                    const T val = reinterpret_cast<const T*>(src)[x];
+                    outp[o + x] = val;
+                    for (int r = 0; r < p.n_peers; ++r) reinterpret_cast<T*>(p.peer_out[r])[o + x] = val;
                 }
             }
         }
@@ -366,7 +401,7 @@ struct Workspace {
 
 // Split-K scratch: one FIXED-SIZE block per (device, stream), so that launches on different streams never
 // share partials or counters and the launch path never reallocates.  32 MB covers every split this
-// library launches (<= one wave of 132 CTAs x 128 x 128 fp32 = 8.3 MB).  The only allocation happens on the first split-K call of a stream; it is
+// library launches (<= one wave of 132 CTAs x 128 x 256 fp32 = 17.3 MB).  The only allocation happens on the first split-K call of a stream; it is
 // made capture-safe (relaxed capture mode around cudaMalloc) so that a CUDA-graph capture whose first
 // split-K GEMM is inside the capture still works.  The registry evicts its least recently used entry.
 constexpr size_t kWsBytes = size_t(32) << 20;
@@ -438,15 +473,16 @@ Workspace* get_workspace(cudaStream_t stream, size_t partial_bytes, size_t n_cou
     return &e->ws;
 }
 
-template <typename T, int QT, int MT>
+template <typename T, int QT, int MT, bool DQ>
 bool launch_mt(const T* A, Gemm4Params& p, int force_splits, cudaStream_t stream) {
     using Cfg = StageCfg<MT>;
+    constexpr int kBK = Cfg::kBK;
     constexpr size_t smem_bytes = 1024 /*align slack*/ + size_t(Cfg::kStages) * Cfg::kStageBytes + 256 /*barriers*/;
     // the shared-memory opt-in is PER DEVICE (one process may drive several GPUs)
     static bool attr_set[64] = {};
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return false;
-    auto kern = gemm4_tc_kernel<T, QT, MT>;
+    auto kern = gemm4_tc_kernel<T, QT, MT, DQ>;
     if (!attr_set[dev]) {
         if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes) != cudaSuccess) {
             set_last_error("gemm4_tc smem attr", cudaGetLastError());
@@ -456,9 +492,17 @@ bool launch_mt(const T* A, Gemm4Params& p, int force_splits, cudaStream_t stream
     }
     CUtensorMap tmap, tmap_w;
     if (!encode_tmap_2d(&tmap, A, 2, 128, (uint64_t)p.M, (uint64_t)p.K, (uint64_t)p.K * 2, (uint32_t)MT, 64u)) return false;
-    // packed codes as a [N, K/2] byte matrix, 128 x 64-byte boxes, 64-byte swizzle
-    if (!encode_tmap_2d(&tmap_w, p.B, 1, 64, (uint64_t)p.N, (uint64_t)p.K / 2, (uint64_t)p.K / 2, (uint32_t)kTileN, 64u))
+    // packed codes as a [N, K/2] byte matrix, 128 x BK/2-byte boxes, BK/2-byte swizzle
+    if (!encode_tmap_2d(&tmap_w, p.B, 1, Cfg::kWRowBytes, (uint64_t)p.N, (uint64_t)p.K / 2, (uint64_t)p.K / 2,
+                        (uint32_t)kTileN, (uint32_t)Cfg::kWRowBytes))
         return false;
+    p.kblocks_total = (p.K + kBK - 1) / kBK;
+    // Every row starts at n * K, a multiple of the largest power of two dividing K, and every stage at a multiple of
+    // BK: a quantisation block can begin only at 32-code chunks that are multiples of min(blocksize, that, BK).
+    int gran = 1 << p.log2_bs;
+    if ((p.K & -p.K) < gran) gran = p.K & -p.K;
+    if (kBK < gran) gran = kBK;
+    p.scale_mask = gran / 32 - 1;
     const int n_tiles = (p.N + kTileN - 1) / kTileN;
     const int m_tiles = (p.M + MT - 1) / MT;
     const int sms = device_sm_count();
@@ -469,7 +513,7 @@ bool launch_mt(const T* A, Gemm4Params& p, int force_splits, cudaStream_t stream
     int splits = 1;
     if (force_splits > 0 || tiles * 2 <= sms) {
         int v = force_splits > 0 ? force_splits : sms / tiles;
-        // >= two 128-wide stages per split by default, >= one when the split is forced
+        // >= two stages per split by default, >= one when the split is forced
         const int max_by_k = force_splits > 0 ? p.kblocks_total : (p.kblocks_total / 2 > 0 ? p.kblocks_total / 2 : 1);
         if (v > max_by_k) v = max_by_k;
         if (v > 16) v = 16;
@@ -523,7 +567,7 @@ bool launch_mt(const T* A, Gemm4Params& p, int force_splits, cudaStream_t stream
 
 // Returns true if the tensor-core path handled the call.
 // `peers` / `n_peers`: up to 7 additional output bases (same ldc) that receive a copy of every element.
-// `mt_override`: token tile (16 | 32 | 64 | 128, 0 = by M); `force_splits`: K split per tile (0 = by the grid).
+// `mt_override`: token tile (16 | 32 | 64 | 128 | 256, 0 = by M); `force_splits`: K split per tile (0 = by the grid).
 template <typename T>
 bool launch_gemm4_tc(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
                      const float* absmax_code, const float* absmax_offset, T* out, const T* bias, int M, int N, int K,
@@ -536,12 +580,16 @@ bool launch_gemm4_tc(const T* A, const uint8_t* B, const float* absmax, const ui
     if ((reinterpret_cast<uintptr_t>(A) & 15) != 0 || (reinterpret_cast<uintptr_t>(B) & 15) != 0) return false;
     if (quant_type != kNF4 && quant_type != kFP4) return false;
 
+    // 256-token tiles decode each weight half as often as 128-token ones, but a grid of them that does not fill one
+    // wave leaves SMs idle (or needs a K split): they are taken when they alone fill every SM.
     int MT = 128;
     if (M <= 16) MT = 16;
     else if (M <= 32) MT = 32;
     else if (M <= 64) MT = 64;
+    else if ((long long)((M + 255) / 256) * ((N + kTileN - 1) / kTileN) >= device_sm_count()) MT = 256;
     if (mt_override != 0) {
-        if (mt_override != 16 && mt_override != 32 && mt_override != 64 && mt_override != 128) return false;
+        if (mt_override != 16 && mt_override != 32 && mt_override != 64 && mt_override != 128 && mt_override != 256)
+            return false;
         MT = mt_override;
     }
 
@@ -560,19 +608,31 @@ bool launch_gemm4_tc(const T* A, const uint8_t* B, const float* absmax, const ui
     p.K = K;
     p.ldc = ldc;
     p.log2_bs = ilog2_pow2(blocksize);
-    p.kblocks_total = (K + kBK - 1) / kBK;
+    bool vec = (ldc % 8) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0;
+    for (int r = 0; r < n_peers; ++r) vec = vec && (reinterpret_cast<uintptr_t>(peers[r]) & 15) == 0;
+    p.out_vec = vec ? 1 : 0;
 
-#define BNB200_DISPATCH_MT(QT)                                                                                         \
+#define BNB200_DISPATCH_MT(QT, DQ)                                                                                     \
     switch (MT) {                                                                                                      \
-    case 16: return launch_mt<T, QT, 16>(A, p, force_splits, stream);                                                  \
-    case 32: return launch_mt<T, QT, 32>(A, p, force_splits, stream);                                                  \
-    case 64: return launch_mt<T, QT, 64>(A, p, force_splits, stream);                                                  \
-    default: return launch_mt<T, QT, 128>(A, p, force_splits, stream);                                                 \
+    case 16: return launch_mt<T, QT, 16, DQ>(A, p, force_splits, stream);                                              \
+    case 32: return launch_mt<T, QT, 32, DQ>(A, p, force_splits, stream);                                              \
+    case 64: return launch_mt<T, QT, 64, DQ>(A, p, force_splits, stream);                                              \
+    case 128: return launch_mt<T, QT, 128, DQ>(A, p, force_splits, stream);                                            \
+    default: return launch_mt<T, QT, 256, DQ>(A, p, force_splits, stream);                                             \
     }
+    const bool dq = absmax_8bit != nullptr;
     if (quant_type == kNF4) {
-        BNB200_DISPATCH_MT(kNF4)
+        if (dq) {
+            BNB200_DISPATCH_MT(kNF4, true)
+        } else {
+            BNB200_DISPATCH_MT(kNF4, false)
+        }
     } else {
-        BNB200_DISPATCH_MT(kFP4)
+        if (dq) {
+            BNB200_DISPATCH_MT(kFP4, true)
+        } else {
+            BNB200_DISPATCH_MT(kFP4, false)
+        }
     }
 #undef BNB200_DISPATCH_MT
 }

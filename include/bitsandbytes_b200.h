@@ -156,9 +156,9 @@ int cbnb_b200_gemm_4bit_path(int M, int N, int K, int blocksize, int dtype);
 /* Force a path for the next calls on this thread (-1 = automatic). */
 void cbnb_b200_gemm_4bit_force_path(int path);
 
-/* Developer / test entry for the wgmma 4-bit GEMM (csrc/gemm4_tc.cu): explicit token tile mt (16 | 32 | 64 | 128;
- * 0 = by M) and forced K split per tile (0 = production rule; s = up to s ways, at least one 128-deep stage per
- * split).  `trace` must be NULL (the name and argument list are kept for ABI stability).  Returns 0, or 100 when
+/* Developer / test entry for the wgmma 4-bit GEMM (csrc/gemm4_tc.cu): explicit token tile mt (16 | 32 | 64 | 128 |
+ * 256; 0 = by M) and forced K split per tile (0 = production rule; s = up to s ways, at least one stage per split:
+ * 128 deep, 64 deep at mt = 256).  `trace` must be NULL (the name and argument list are kept for ABI stability).  Returns 0, or 100 when
  * the shape or the options are not served (a forced split must fit one co-resident wave of CTAs). */
 int cbnb_b200_gemm_4bit_pair(const void* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit, const float* absmax_code, const float* absmax_offset, void* out, const void* bias, int M, int N, int K, int ldc, int blocksize, int quant_type, int dtype, int mt, int force_splits, long long* trace, bnb_stream_t stream);
 
