@@ -13,7 +13,7 @@
 // Design ("swap-AB, weights through registers"):
 //   * The wgmma M dimension (64 rows per warpgroup, two warpgroups) carries the OUTPUT FEATURES n;
 //     the tokens m are the wgmma N dimension (MT = 16..256).  A CTA owns out[m0:m0+MT, n0:n0+128].
-//   * A pipeline stage is BK k-elements (128; 64 at MT = 256).  Thread 0 stages with TMA, per stage,
+//   * A pipeline stage is BK k-elements (128; 64 at MT = 256).  A producer thread stages with TMA, per stage,
 //     the packed codes of the CTA's 128 rows (128 x BK/2 bytes, BK/2-byte swizzle) and the activation tile
 //     X[m0:m0+MT, k0:k0+BK] (BK/64 128-byte-swizzled sub-tiles), the K-major B operand of wgmma.
 //   * Every consumer thread reads the codes of its two rows for the whole stage (ld.shared, 16 bytes per
@@ -28,9 +28,13 @@
 //     grid is small -- writes fp32 partials to an L2-resident workspace with a last-arriver reduction in
 //     deterministic split order.
 //
-// 256 threads = two warpgroups (decode + wgmma + epilogue); thread 0 also issues the TMA loads.  There is no
-// producer warp: a ninth warp puts three warps on one SM sub-partition, whose 16K registers then cap every thread
-// at 168 -- too few for the 256-token tile (128 accumulators, two A-fragment sets, the decode state).
+// 384 threads = a producer warpgroup (one thread issues every TMA load of the ring) and two consumer warpgroups
+// (decode + wgmma + epilogue).  Launch bounds allow 168 registers per thread; the producer gives registers back
+// (setmaxnreg.dec to 40) and the consumers take them (setmaxnreg.inc to 232), which the 256-token tile needs (128
+// accumulators, two A-fragment sets, the decode state).  The grid is persistent: min(units, SMs) CTAs, each running
+// every gridDim-th (tile, K split) unit, with the ring's slot and phase carried across units, so the producer loads
+// the next tile while the consumers run the epilogue.  (Measured on an H100: the persistent loop itself is neutral;
+// it is kept because the one-tile-per-CTA form of this kernel makes ptxas spill at MT = 256.)
 #include "common.cuh"
 #include "decode4.cuh"
 #include "hopper_ptx.cuh"
@@ -45,7 +49,12 @@ namespace {
 
 constexpr int kTileN = 128;        // output features per CTA (two warpgroups of 64)
 constexpr int kConsumers = 256;    // threads of the two consumer warpgroups
-constexpr int kThreads = kConsumers;
+constexpr int kThreads = 128 + kConsumers;  // producer warpgroup + consumers
+// per-thread registers after the hand-off: 128 x 40 + 256 x 232 <= 64K, the SM's register file
+constexpr int kProducerRegs = 40;
+constexpr int kConsumerRegs = 232;
+static_assert(128 * kProducerRegs + kConsumers * kConsumerRegs <= 65536, "register hand-off exceeds the SM");
+constexpr int kBarEpi = 1;    // named barrier of the consumers' epilogue
 
 struct Gemm4Params {
     const uint8_t* B;            // packed codes [N, K/2]
@@ -88,9 +97,10 @@ __device__ __forceinline__ void wgmma_step(float (&d)[MT / 2], const uint32_t (&
 }
 
 // Pipeline stage = BK k-elements: BK/64 64-wide (128-byte, swizzle-atom) activation sub-tiles and the packed codes
-// of 128 rows.  Ring depth: as many stages as fit next to each other in 220 KB.  The 256-token tile takes 64-deep
-// stages: a 128-deep one (72 KB) leaves room for two stages only, and two 128-deep A-fragment sets (64 registers)
-// next to its 128 accumulators would not fit the consumers' register budget.
+// of 128 rows.  The 256-token tile takes 64-deep stages: a 128-deep one (72 KB) leaves room for two stages only,
+// and two 128-deep A-fragment sets (64 registers) next to its 128 accumulators would not fit the consumers'
+// register budget.  The epilogue stages the output tile in a buffer of its own (the producer is already filling the
+// ring for the CTA's next tile), and the ring takes as many stages as fit next to it, at most 8.
 template <int MT> struct StageCfg {
     static constexpr int kBK = MT == 256 ? 64 : 128;
     static constexpr int kSteps = kBK / 16;                      // wgmma k16 steps
@@ -100,11 +110,15 @@ template <int MT> struct StageCfg {
     static constexpr int kWRowBytes = kBK / 2;                   // packed codes of one row (TMA, kWRowBytes-byte swizzle)
     static constexpr int kWStageBytes = kTileN * kWRowBytes;
     static constexpr int kStageBytes = kXStageBytes + kWStageBytes;
-    static constexpr int kStages = (220 * 1024 / kStageBytes) > 8 ? 8 : (220 * 1024 / kStageBytes);
     // epilogue staging: one output row of the tile (128 x T) plus 16 bytes, so that the fragment stores (four
     // token rows two apart per warp instruction) fall on distinct banks
     static constexpr int kOutPitch = kTileN * 2 + 16;
-    static_assert(MT * kOutPitch <= kStages * kStageBytes, "epilogue staging reuses the stage ring");
+    static constexpr int kOutBytes = MT * kOutPitch;
+    static constexpr int kSlack = 1024 + 256;                    // base alignment + barriers
+    static constexpr int kRing = (227 * 1024 - kSlack - kOutBytes) / kStageBytes;
+    static constexpr int kStages = kRing > 8 ? 8 : kRing;
+    static constexpr int kSmemBytes = kSlack + kStages * kStageBytes + kOutBytes;
+    static_assert(kStages >= 2 && kSmemBytes <= 227 * 1024, "shared memory");
 };
 
 // The 16 codes of a 16-byte chunk (stage-row words w[4q .. 4q+3]) that this thread's A fragments need (byte `t` of
@@ -134,25 +148,33 @@ __global__ void __launch_bounds__(kThreads, 1)
     uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t* sx = smem;                              // [kStages][BK/64][MT x 128 B]   activations
     uint8_t* sw = smem + kStages * kXStageBytes;     // [kStages][128 x BK/2 B]        packed codes
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes);
+    uint8_t* so = smem + kStages * Cfg::kStageBytes; // [MT][kOutPitch]                epilogue staging
+    uint64_t* bars = reinterpret_cast<uint64_t*>(so + Cfg::kOutBytes);
     uint64_t* full = bars;                   // [kStages] TMA (1 arrive + bytes) -> consumers
-    uint64_t* empty = bars + kStages;        // [kStages] the 8 warps -> thread 0 (stage free for the next load)
+    uint64_t* empty = bars + kStages;        // [kStages] the 8 consumer warps -> producer (slot free for the next load)
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
 
-    // Linear CTA id -> (tile, K-split): ids are ordered (tile, split)
+    // Work units u = (tile, K split), ordered (tile, split); tile = m_tile * n_tiles + n_tile.  A CTA runs units
+    // blockIdx.x, blockIdx.x + gridDim.x, ...; a split launch is one wave, one unit per CTA.
     const int splits = p.splits;
-    const int tile_id = blockIdx.x / splits;
-    const int split = blockIdx.x - tile_id * splits;
-    const int slot0 = tile_id * splits;  // first workspace slot of this tile
-    const int n0 = (tile_id % p.n_tiles) * kTileN;
-    const int m0 = (tile_id / p.n_tiles) * MT;
+    const int units = p.tiles_total * splits;
     const int per = (p.kblocks_total + splits - 1) / splits;
-    const int st_begin = split * per;
-    int st_end = st_begin + per;
-    if (st_end > p.kblocks_total) st_end = p.kblocks_total;
-    const int nst = st_end - st_begin;  // >= 1 by construction
+    struct Unit {
+        int tile, split, n0, m0, st_begin, nst;
+    };
+    auto unit_at = [&](int u) {
+        Unit w;
+        w.tile = u / splits;
+        w.split = u - w.tile * splits;
+        w.n0 = (w.tile % p.n_tiles) * kTileN;
+        w.m0 = (w.tile / p.n_tiles) * MT;
+        w.st_begin = w.split * per;
+        const int st_end = w.st_begin + per < p.kblocks_total ? w.st_begin + per : p.kblocks_total;
+        w.nst = st_end - w.st_begin;  // >= 1 by construction
+        return w;
+    };
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < kStages; ++s) {
@@ -163,34 +185,48 @@ __global__ void __launch_bounds__(kThreads, 1)
     }
     __syncthreads();
 
-    // stage j of this split into ring slot j % kStages, issued by thread 0; rows past M, rows past N and columns past K
-    // are out of bounds for the tensor maps: TMA zero-fills
-    const bool issuer = threadIdx.x == 0;
-    auto load_stage = [&](int j) {
-        const int slot = j % kStages;
-        const int k0 = (st_begin + j) * kBK;
-        ptx::mbar_arrive_expect_tx_if(issuer, &full[slot], kWStageBytes + kXStageBytes);
-        // packed codes of this CTA's 128 output features: bytes [k0/2, k0/2 + BK/2) of rows n0..n0+127
-        ptx::tma_load_2d_if(issuer, sw + slot * kWStageBytes, &tmap_w, &full[slot], k0 / 2, n0);
+    // The ring runs continuously over the CTA's units: its slot and phase carry from one unit to the next.
+    // ====================================================================== producer (warpgroup 0)
+    // (the role test is made provably warp-uniform, as setmaxnreg requires of the whole warpgroup)
+    if (__shfl_sync(0xffffffffu, threadIdx.x / 128, 0) == 0) {
+        ptx::setmaxnreg_dec<kProducerRegs>();
+        if (threadIdx.x == 0) {
+            ptx::prefetch_tmap(&tmap_x);
+            ptx::prefetch_tmap(&tmap_w);
+            int slot = 0;
+            uint32_t phase = 0;  // parity of the slot's current round
+            bool wrapped = false;
+            for (int u = blockIdx.x; u < units; u += gridDim.x) {
+                const Unit w = unit_at(u);
+                for (int j = 0; j < w.nst; ++j) {
+                    // the slot's previous load has been consumed by all 8 consumer warps
+                    if (wrapped) ptx::mbar_wait(&empty[slot], phase ^ 1u);
+                    const int k0 = (w.st_begin + j) * kBK;
+                    ptx::mbar_arrive_expect_tx(&full[slot], kWStageBytes + kXStageBytes);
+                    // rows past M, rows past N and columns past K are out of bounds for the tensor maps: TMA
+                    // zero-fills.  Packed codes of the tile's 128 output features: bytes [k0/2, k0/2 + BK/2).
+                    ptx::tma_load_2d(sw + slot * kWStageBytes, &tmap_w, &full[slot], k0 / 2, w.n0);
 #pragma unroll
-        for (int h = 0; h < kBK / 64; ++h)
-            ptx::tma_load_2d_if(issuer, sx + slot * kXStageBytes + h * kXSubBytes, &tmap_x, &full[slot], k0 + 64 * h,
-                                    m0);
-    };
-    if (issuer) {
-        ptx::prefetch_tmap(&tmap_x);
-        ptx::prefetch_tmap(&tmap_w);
+                    for (int h = 0; h < kBK / 64; ++h)
+                        ptx::tma_load_2d(sx + slot * kXStageBytes + h * kXSubBytes, &tmap_x, &full[slot],
+                                         k0 + 64 * h, w.m0);
+                    if (++slot == kStages) {
+                        slot = 0;
+                        phase ^= 1u;
+                        wrapped = true;
+                    }
+                }
+            }
+        }
+        return;
     }
-    for (int j = 0; j < kStages && j < nst; ++j) load_stage(j);
 
-    // ====================================================================== consumers
-    const int wg = warp >> 2;                 // warpgroup: feature rows [64 wg, 64 wg + 64) of the tile
+    // ====================================================================== consumers (warpgroups 1, 2)
+    ptx::setmaxnreg_inc<kConsumerRegs>();
+    const int ct = threadIdx.x - 128;         // consumer thread 0..255
+    const int wg = ct >> 7;                   // consumer warpgroup: feature rows [64 wg, 64 wg + 64) of the tile
     const int g = lane >> 2, t = lane & 3;
     const int row0 = wg * 64 + (warp & 3) * 16 + g;  // this thread's two rows: row0, row0 + 8
-    const int na = n0 + row0, nb = na + 8;
-    const bool a_ok = na < p.N, b_ok = nb < p.N;
-    const long long e_a = (long long)(a_ok ? na : 0) * p.K;
-    const long long e_b = (long long)(b_ok ? nb : 0) * p.K;
     const ScaleSrc sc{p.absmax, p.absmax_8bit, p.absmax_code, (DQ && p.absmax_offset) ? __ldg(p.absmax_offset) : 0.0f};
     const uint32_t sel = (uint32_t)t | ((uint32_t)(t + 4) << 4);
     const uint32_t smask = (uint32_t)p.scale_mask;
@@ -198,195 +234,205 @@ __global__ void __launch_bounds__(kThreads, 1)
     const uint32_t swz[2] = {(uint32_t)((row0 * kWRowBytes) >> 7) & (kChunks - 1),
                              (uint32_t)(((row0 + 8) * kWRowBytes) >> 7) & (kChunks - 1)};
 
-    // Scales of one stage, one per (row, quantisation block): the 32 codes of a chunk lie inside one block (blocks
-    // are >= 32 and aligned), and a block can begin only at a chunk q with (q & smask) == 0.  Fetched one stage ahead.
-    float scl[2][kChunks];
-    auto fetch = [&](int i) {
-        const long long kk = (long long)(st_begin + i) * kBK;
-#pragma unroll
-        for (int q = 0; q < kChunks; ++q) {
-            if ((q & smask) == 0) {
-                const bool in_k = i < nst && kk + 32 * q < p.K;
-                scl[0][q] = (in_k && a_ok) ? sc.load_as<DQ>((e_a + kk + 32 * q) >> p.log2_bs) : 0.f;
-                scl[1][q] = (in_k && b_ok) ? sc.load_as<DQ>((e_b + kk + 32 * q) >> p.log2_bs) : 0.f;
-            }
-        }
-    };
+    int slot = 0;
+    uint32_t phase = 0;
+    for (int u = blockIdx.x; u < units; u += gridDim.x) {
+        const Unit w = unit_at(u);
+        const int n0 = w.n0, m0 = w.m0, st_begin = w.st_begin, nst = w.nst;
+        const int na = n0 + row0, nb = na + 8;
+        const bool a_ok = na < p.N, b_ok = nb < p.N;
+        const long long e_a = (long long)(a_ok ? na : 0) * p.K;
+        const long long e_b = (long long)(b_ok ? nb : 0) * p.K;
 
-    float acc[MT / 2];
-#pragma unroll
-    for (int j = 0; j < MT / 2; ++j) acc[j] = 0.f;
-
-    uint32_t afr[2][kSteps][4];  // two A-fragment sets: [set][k16 step][reg]
-
-    // decode stage i (smem stage s) into A set `a`: all of the stage's code loads first, then the tables and PRMTs
-    auto decode = [&](int s, uint32_t (&a)[kSteps][4]) {
-        const uint8_t* wt = sw + s * kWStageBytes;
-        uint4 v[2][kChunks];
-#pragma unroll
-        for (int r = 0; r < 2; ++r)
-#pragma unroll
-            for (int q = 0; q < kChunks; ++q)
-                v[r][q] = *reinterpret_cast<const uint4*>(wt + (row0 + 8 * r) * kWRowBytes + (((uint32_t)q ^ swz[r]) << 4));
-#pragma unroll
-        for (int r = 0; r < 2; ++r) {
-            DecodeTable tab;
+        // Scales of one stage, one per (row, quantisation block): the 32 codes of a chunk lie inside one block (blocks
+        // are >= 32 and aligned), and a block can begin only at a chunk q with (q & smask) == 0.  Fetched one stage ahead.
+        float scl[2][kChunks];
+        auto fetch = [&](int i) {
+            const long long kk = (long long)(st_begin + i) * kBK;
 #pragma unroll
             for (int q = 0; q < kChunks; ++q) {
-                if ((q & smask) == 0) build_table<T, QT>(scl[r][q], tab);
-                uint32_t o[4];
-                decode_word(gather_bytes(v[r][q], sel), tab, o);
-                // o[i]: byte i of the gathered word = word 4q+i of the row -> k16 step 2q + i/2, half i%2
+                if ((q & smask) == 0) {
+                    const bool in_k = i < nst && kk + 32 * q < p.K;
+                    scl[0][q] = (in_k && a_ok) ? sc.load_as<DQ>((e_a + kk + 32 * q) >> p.log2_bs) : 0.f;
+                    scl[1][q] = (in_k && b_ok) ? sc.load_as<DQ>((e_b + kk + 32 * q) >> p.log2_bs) : 0.f;
+                }
+            }
+        };
+
+        float acc[MT / 2];
 #pragma unroll
-                for (int u = 0; u < 2; ++u) {
-                    a[2 * q + u][r] = o[2 * u];          // rows g / g+8, k 2t..2t+1
-                    a[2 * q + u][2 + r] = o[2 * u + 1];  // rows g / g+8, k 8+2t..9+2t
+        for (int j = 0; j < MT / 2; ++j) acc[j] = 0.f;
+
+        uint32_t afr[2][kSteps][4];  // two A-fragment sets: [set][k16 step][reg]
+
+        // decode stage i (smem stage s) into A set `a`: all of the stage's code loads first, then the tables and PRMTs
+        auto decode = [&](int s, uint32_t (&a)[kSteps][4]) {
+            const uint8_t* wt = sw + s * kWStageBytes;
+            uint4 v[2][kChunks];
+#pragma unroll
+            for (int r = 0; r < 2; ++r)
+#pragma unroll
+                for (int q = 0; q < kChunks; ++q)
+                    v[r][q] = *reinterpret_cast<const uint4*>(wt + (row0 + 8 * r) * kWRowBytes + (((uint32_t)q ^ swz[r]) << 4));
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                DecodeTable tab;
+#pragma unroll
+                for (int q = 0; q < kChunks; ++q) {
+                    if ((q & smask) == 0) build_table<T, QT>(scl[r][q], tab);
+                    uint32_t o[4];
+                    decode_word(gather_bytes(v[r][q], sel), tab, o);
+                    // o[i]: byte i of the gathered word = word 4q+i of the row -> k16 step 2q + i/2, half i%2
+#pragma unroll
+                    for (int u = 0; u < 2; ++u) {
+                        a[2 * q + u][r] = o[2 * u];          // rows g / g+8, k 2t..2t+1
+                        a[2 * q + u][2 + r] = o[2 * u + 1];  // rows g / g+8, k 8+2t..9+2t
+                    }
+                }
+            }
+        };
+
+        auto mma_stage = [&](int s, const uint32_t (&a)[kSteps][4]) {
+            const uint32_t xs = ptx::smem_u32(sx + s * kXStageBytes);
+            ptx::wgmma_fence();
+#pragma unroll
+            for (int j = 0; j < kSteps; ++j)
+                wgmma_step<T, MT>(acc, a[j], ptx::make_sw128_kmajor_desc(xs + (j >> 2) * kXSubBytes) + 2 * (j & 3));
+            ptx::wgmma_commit();
+        };
+
+        fetch(0);
+        int prev_s = -1;
+        for (int i0 = 0; i0 < nst; i0 += 2) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int i = i0 + h;
+                if (i < nst) {
+                    const int s = slot;
+                    ptx::mbar_wait(&full[s], phase);
+                    if (++slot == kStages) {
+                        slot = 0;
+                        phase ^= 1u;
+                    }
+                    decode(s, afr[h]);
+                    fetch(i + 1);
+                    mma_stage(s, afr[h]);
+                    // the wgmma group of the previous stage has completed: its activation tile (and its A set) are free
+                    ptx::wgmma_wait<1>();
+                    if (prev_s >= 0) {
+                        __syncwarp();
+                        if (lane == 0) ptx::mbar_arrive(&empty[prev_s]);
+                    }
+                    prev_s = s;
                 }
             }
         }
-    };
-
-    auto mma_stage = [&](int s, const uint32_t (&a)[kSteps][4]) {
-        const uint32_t xs = ptx::smem_u32(sx + s * kXStageBytes);
-        ptx::wgmma_fence();
+        ptx::wgmma_wait<0>();
 #pragma unroll
-        for (int j = 0; j < kSteps; ++j)
-            wgmma_step<T, MT>(acc, a[j], ptx::make_sw128_kmajor_desc(xs + (j >> 2) * kXSubBytes) + 2 * (j & 3));
-        ptx::wgmma_commit();
-    };
+        for (int j = 0; j < MT / 2; ++j) ptx::fence_operand(acc[j]);
+        __syncwarp();
+        if (lane == 0) ptx::mbar_arrive(&empty[prev_s]);
 
-    fetch(0);
-    int prev_s = -1;
-    for (int i0 = 0; i0 < nst; i0 += 2) {
+        // ================================================================== epilogue
+        // acc[4j + e]: feature row row0 + 8 * (e >= 2), token column 8j + 2t + (e & 1)
+        T* outp = reinterpret_cast<T*>(p.out);
+        if (splits == 1) {
+            const T* bias = reinterpret_cast<const T*>(p.bias);
+            const float bias_a = (bias != nullptr && a_ok) ? DT<T>::to_f32(bias[na]) : 0.f;
+            const float bias_b = (bias != nullptr && b_ok) ? DT<T>::to_f32(bias[nb]) : 0.f;
+            // Stage the rounded tile as [token][feature] rows -- once both warpgroups are done reading the previous
+            // unit's tile there -- then store it in 16-byte row pieces: each token row of the tile is 256 contiguous
+            // bytes of the output.
+            constexpr int kPitch = Cfg::kOutPitch;
+            ptx::bar_sync(kBarEpi, kConsumers);
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int i = i0 + h;
-            if (i < nst) {
-                const int s = i % kStages;
-                ptx::mbar_wait(&full[s], (uint32_t)(i / kStages) & 1u);
-                decode(s, afr[h]);
-                fetch(i + 1);
-                mma_stage(s, afr[h]);
-                // the wgmma group of the previous stage has completed: its activation tile (and its A set) are free
-                ptx::wgmma_wait<1>();
-                if (prev_s >= 0) {
-                    __syncwarp();
-                    if (lane == 0) ptx::mbar_arrive(&empty[prev_s]);
-                }
-                prev_s = s;
-                // refill the slot of stage i - 2 (every warp released it one iteration ago, so the wait is short and
-                // the two warpgroups are not tied to each other stage by stage); kStages - 2 stages stay in flight.
-                // Every thread takes the same path, thread 0 alone issues (see tma_load_2d_if).
-                const int j = i - 2 + kStages;
-                if (i >= 2 && j < nst) {
-                    ptx::mbar_wait(&empty[j % kStages], (uint32_t)((i - 2) / kStages) & 1u);
-                    load_stage(j);
+            for (int j = 0; j < MT / 8; ++j)
+#pragma unroll
+                for (int e = 0; e < 4; ++e)
+                    *reinterpret_cast<T*>(so + (8 * j + 2 * t + (e & 1)) * kPitch + (row0 + 8 * (e >> 1)) * 2) =
+                        DT<T>::from_f32(acc[4 * j + e] + (e >= 2 ? bias_b : bias_a));
+            ptx::bar_sync(kBarEpi, kConsumers);
+            for (int idx = ct; idx < MT * (kTileN / 8); idx += kConsumers) {
+                const int c = idx / (kTileN / 8), n = n0 + 8 * (idx % (kTileN / 8));
+                const int m = m0 + c;
+                if (m >= p.M || n >= p.N) continue;
+                const uint8_t* src = so + c * kPitch + (n - n0) * 2;
+                const long long o = (long long)m * p.ldc + n;
+                if (p.out_vec && n + 8 <= p.N) {
+                    const uint4 val = *reinterpret_cast<const uint4*>(src);
+                    *reinterpret_cast<uint4*>(outp + o) = val;
+                    for (int r = 0; r < p.n_peers; ++r) *reinterpret_cast<uint4*>(reinterpret_cast<T*>(p.peer_out[r]) + o) = val;
+                } else {
+                    for (int x = 0; x < 8 && n + x < p.N; ++x) {
+                        const T val = reinterpret_cast<const T*>(src)[x];
+                        outp[o + x] = val;
+                        for (int r = 0; r < p.n_peers; ++r) reinterpret_cast<T*>(p.peer_out[r])[o + x] = val;
+                    }
                 }
             }
+            continue;
         }
-    }
-    ptx::wgmma_wait<0>();
-#pragma unroll
-    for (int j = 0; j < MT / 2; ++j) ptx::fence_operand(acc[j]);
 
-    // ================================================================== epilogue
-    // acc[4j + e]: feature row row0 + 8 * (e >= 2), token column 8j + 2t + (e & 1)
-    T* outp = reinterpret_cast<T*>(p.out);
-    if (splits == 1) {
-        const T* bias = reinterpret_cast<const T*>(p.bias);
-        const float bias_a = (bias != nullptr && a_ok) ? DT<T>::to_f32(bias[na]) : 0.f;
-        const float bias_b = (bias != nullptr && b_ok) ? DT<T>::to_f32(bias[nb]) : 0.f;
-        // Stage the rounded tile as [token][feature] rows in the stage ring -- free once both warpgroups' last
-        // wgmma has completed -- then store it in 16-byte row pieces: each token row of the tile is 256
-        // contiguous bytes of the output.
-        constexpr int kPitch = Cfg::kOutPitch;
-        asm volatile("bar.sync 1, 256;" ::: "memory");
+        // ---- split-K: every split CTA publishes its fp32 partial tile (layout [column m][row n], so that the
+        // later reads are 128-byte coalesced), the splits of a tile rendezvous on a counter, and EACH of them then
+        // reduces a 1/splits share of the columns (in split order: deterministic).  The launch is COOPERATIVE (all
+        // CTAs of the <= one-wave grid are resident together), so the short wait cannot starve; it is bounded anyway.
+        const int split = w.split;
+        float* ws_tile = p.ws_partial + (long long)w.tile * splits * kTileN * MT;
+        float* my = ws_tile + (long long)split * kTileN * MT;
 #pragma unroll
         for (int j = 0; j < MT / 8; ++j)
 #pragma unroll
-            for (int e = 0; e < 4; ++e)
-                *reinterpret_cast<T*>(smem + (8 * j + 2 * t + (e & 1)) * kPitch + (row0 + 8 * (e >> 1)) * 2) =
-                    DT<T>::from_f32(acc[4 * j + e] + (e >= 2 ? bias_b : bias_a));
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        for (int idx = threadIdx.x; idx < MT * (kTileN / 8); idx += kConsumers) {
-            const int c = idx / (kTileN / 8), n = n0 + 8 * (idx % (kTileN / 8));
-            const int m = m0 + c;
-            if (m >= p.M || n >= p.N) continue;
-            const uint8_t* src = smem + c * kPitch + (n - n0) * 2;
-            const long long o = (long long)m * p.ldc + n;
-            if (p.out_vec && n + 8 <= p.N) {
-                const uint4 val = *reinterpret_cast<const uint4*>(src);
-                *reinterpret_cast<uint4*>(outp + o) = val;
-                for (int r = 0; r < p.n_peers; ++r) *reinterpret_cast<uint4*>(reinterpret_cast<T*>(p.peer_out[r]) + o) = val;
-            } else {
-                for (int x = 0; x < 8 && n + x < p.N; ++x) {
-                    const T val = reinterpret_cast<const T*>(src)[x];
-                    outp[o + x] = val;
-                    for (int r = 0; r < p.n_peers; ++r) reinterpret_cast<T*>(p.peer_out[r])[o + x] = val;
+            for (int e = 0; e < 4; ++e) my[(8 * j + 2 * t + (e & 1)) * kTileN + row0 + 8 * (e >> 1)] = acc[4 * j + e];
+        __threadfence();
+        ptx::bar_sync(kBarEpi, kConsumers);
+        int* arrive = p.ws_counter + w.tile;
+        int* done = p.ws_counter + p.tiles_total + w.tile;
+        if (ct == 0) {
+            atomicAdd(arrive, 1);
+            unsigned long long t0 = 0;
+            unsigned spins = 0;
+            while (atomicAdd(arrive, 0) < splits) {
+                __nanosleep(64);
+                if ((++spins & 0xFFF) == 0) {  // bounded: trap after 10 s instead of hanging the device (no printf:
+                                               // a call would serialise the wgmma pipeline)
+                    unsigned long long now;
+                    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
+                    if (t0 == 0) t0 = now;
+                    else if (now - t0 > 10000000000ull) __trap();
+                }
+            }
+            __threadfence();
+        }
+        ptx::bar_sync(kBarEpi, kConsumers);
+        {
+            const int e = ct;                        // 0..255 over the two consumer warpgroups
+            const int rn = e & (kTileN - 1);         // output feature inside the tile
+            const int cg = e >> 7;                   // 0..1
+            const int nn = n0 + rn;
+            float bias_r = 0.f;
+            if (p.bias != nullptr && nn < p.N) bias_r = DT<T>::to_f32(reinterpret_cast<const T*>(p.bias)[nn]);
+            for (int c = split + splits * cg; c < MT; c += splits * 2) {
+                const int m = m0 + c;
+                if (m >= p.M) break;
+                float a = 0.f;
+                for (int sp = 0; sp < splits; ++sp) a += __ldcg(ws_tile + ((long long)sp * MT + c) * kTileN + rn);
+                if (nn < p.N) {
+                    const T val = DT<T>::from_f32(a + bias_r);
+                    const long long idx = (long long)m * p.ldc + nn;
+                    outp[idx] = val;
+                    for (int r = 0; r < p.n_peers; ++r) reinterpret_cast<T*>(p.peer_out[r])[idx] = val;
                 }
             }
         }
-        return;
-    }
-
-    // ---- split-K: every split CTA publishes its fp32 partial tile (layout [column m][row n], so that the
-    // later reads are 128-byte coalesced), the splits of a tile rendezvous on a counter, and EACH of them then
-    // reduces a 1/splits share of the columns (in split order: deterministic).  The launch is COOPERATIVE (all
-    // CTAs of the <= one-wave grid are resident together), so the short wait cannot starve; it is bounded anyway.
-    float* ws_tile = p.ws_partial + (long long)slot0 * kTileN * MT;
-    float* my = ws_tile + (long long)split * kTileN * MT;
-#pragma unroll
-    for (int j = 0; j < MT / 8; ++j)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) my[(8 * j + 2 * t + (e & 1)) * kTileN + row0 + 8 * (e >> 1)] = acc[4 * j + e];
-    __threadfence();
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    int* arrive = p.ws_counter + tile_id;
-    int* done = p.ws_counter + p.tiles_total + tile_id;
-    if (threadIdx.x == 0) {
-        atomicAdd(arrive, 1);
-        unsigned long long t0 = 0;
-        unsigned spins = 0;
-        while (atomicAdd(arrive, 0) < splits) {
-            __nanosleep(64);
-            if ((++spins & 0xFFF) == 0) {  // bounded: trap after 10 s instead of hanging the device (no printf:
-                                           // a call would serialise the wgmma pipeline)
-                unsigned long long now;
-                asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
-                if (t0 == 0) t0 = now;
-                else if (now - t0 > 10000000000ull) __trap();
+        ptx::bar_sync(kBarEpi, kConsumers);
+        if (ct == 0) {
+            // last split out resets the tile's counters for the next launch
+            if (atomicAdd(done, 1) == splits - 1) {
+                *arrive = 0;
+                *done = 0;
+                __threadfence();
             }
-        }
-        __threadfence();
-    }
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    {
-        const int e = threadIdx.x;               // 0..255 over the two consumer warpgroups
-        const int rn = e & (kTileN - 1);         // output feature inside the tile
-        const int cg = e >> 7;                   // 0..1
-        const int nn = n0 + rn;
-        float bias_r = 0.f;
-        if (p.bias != nullptr && nn < p.N) bias_r = DT<T>::to_f32(reinterpret_cast<const T*>(p.bias)[nn]);
-        for (int c = split + splits * cg; c < MT; c += splits * 2) {
-            const int m = m0 + c;
-            if (m >= p.M) break;
-            float a = 0.f;
-            for (int sp = 0; sp < splits; ++sp) a += __ldcg(ws_tile + ((long long)sp * MT + c) * kTileN + rn);
-            if (nn < p.N) {
-                const T val = DT<T>::from_f32(a + bias_r);
-                const long long idx = (long long)m * p.ldc + nn;
-                outp[idx] = val;
-                for (int r = 0; r < p.n_peers; ++r) reinterpret_cast<T*>(p.peer_out[r])[idx] = val;
-            }
-        }
-    }
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    if (threadIdx.x == 0) {
-        // last split out resets the tile's counters for the next launch
-        if (atomicAdd(done, 1) == splits - 1) {
-            *arrive = 0;
-            *done = 0;
-            __threadfence();
         }
     }
 }
@@ -477,7 +523,7 @@ template <typename T, int QT, int MT, bool DQ>
 bool launch_mt(const T* A, Gemm4Params& p, int force_splits, cudaStream_t stream) {
     using Cfg = StageCfg<MT>;
     constexpr int kBK = Cfg::kBK;
-    constexpr size_t smem_bytes = 1024 /*align slack*/ + size_t(Cfg::kStages) * Cfg::kStageBytes + 256 /*barriers*/;
+    constexpr size_t smem_bytes = Cfg::kSmemBytes;
     // the shared-memory opt-in is PER DEVICE (one process may drive several GPUs)
     static bool attr_set[64] = {};
     int dev = 0;
@@ -537,8 +583,9 @@ bool launch_mt(const T* A, Gemm4Params& p, int force_splits, cudaStream_t stream
         p.ws_partial = reinterpret_cast<float*>(ws->ptr);
         p.ws_counter = ws->counters;
     }
+    // persistent: at most one CTA per SM, each running every gridDim-th unit (a split launch is one unit per CTA)
     cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(tiles * splits, 1, 1);
+    cfg.gridDim = dim3(tiles * splits < sms ? tiles * splits : sms, 1, 1);
     cfg.blockDim = dim3(kThreads);
     cfg.dynamicSmemBytes = smem_bytes;
     cfg.stream = stream;

@@ -87,22 +87,18 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
                  : "memory");
 }
 
-// The same two operations, executed only where `pred` holds, with the predicate inside the instruction: a branch
-// around them between two wgmma groups is a divergent path, and ptxas then serialises every wgmma of the kernel.
-__device__ __forceinline__ void mbar_arrive_expect_tx_if(bool pred, uint64_t* bar, uint32_t bytes) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\t"
-                 "@p mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n\t}" ::"r"(smem_u32(bar)),
-                 "r"(bytes), "r"((int)pred)
-                 : "memory");
+// ---------------------------------------------------------------- warp specialisation
+// Per-thread register limit of the calling warpgroup (all four warps execute it): .dec returns registers to the
+// CTA's pool, .inc takes them from it (and waits until they are there).  N: 24..256, a multiple of 8.
+template <int N> __device__ __forceinline__ void setmaxnreg_dec() {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
 }
-__device__ __forceinline__ void tma_load_2d_if(bool pred, void* smem_dst, const CUtensorMap* m, uint64_t* bar,
-                                               int c_inner, int c_outer) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %5, 0;\n\t"
-                 "@p cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes"
-                 " [%0], [%1, {%3, %4}], [%2];\n\t}" ::"r"(smem_u32(smem_dst)),
-                 "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c_inner), "r"(c_outer), "r"((int)pred)
-                 : "memory");
+template <int N> __device__ __forceinline__ void setmaxnreg_inc() {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
 }
+
+// Named barrier among `n` threads (a multiple of 32); id 0 is __syncthreads.
+__device__ __forceinline__ void bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 // ---------------------------------------------------------------- wgmma
 // A warpgroup (four consecutive warps, the first a multiple of four) issues one wgmma.mma_async together.
