@@ -2,8 +2,13 @@
 
 Same contract as the reference's ``bitsandbytes/autograd/_functions.py`` (MatmulLtState
 :57-98, MatMul8bitLt :101-242, MatMul4Bit :300-386, matmul :389-404, matmul_4bit :407-491).
-Forward paths run the sm_90a kernels; the backward formulas are the reference's
-(grad_A = grad_out . dequant(W); the int8 weight-gradient path uses int8_double_quant).
+Forward paths run the sm_90a kernels and are bit-identical to the reference.  grad_A is the
+reference's formula (grad_out . dequant(W)).  The int8 weight gradient of ``MatMul8bitLt``
+differs from the reference on purpose, because the reference's value is not the gradient:
+it dequantises the *row* codes of grad_out with its *column* statistics, and with
+``threshold > 0`` it adds the outlier columns of A twice (once in the int8 product, once from
+``subA``).  Here both operands of grad_outᵀ . A are column codes with their column statistics,
+and the outlier columns are zeroed in the int8 operand before ``subA`` adds them in full.
 The CPU/XPU-only ``MatMul8bitFp`` of the reference is not provided.
 """
 from __future__ import annotations
@@ -18,6 +23,7 @@ from warnings import warn
 import torch
 
 from .. import functional as F
+from ..backends.cuda import int8_zero_columns
 
 logger = logging.getLogger(__name__)
 
@@ -167,11 +173,19 @@ class MatMul8bitLt(torch.autograd.Function):
             grad_output = grad_output.reshape(-1, grad_output.shape[-1]).contiguous()
 
         if need_B:
-            Cgrad, _, _, SCgradt, _ = F.int8_double_quant(grad_output.to(torch.float16))
-            grad_B = torch.ops.bitsandbytes.int8_scaled_mm.default(Cgrad.t().contiguous(), CAt.t(), SCgradt, SCAt,
+            # grad_B[N, K] = grad_outputᵀ · A, contracted over the tokens: both operands are quantised per column
+            # (per output feature / per input feature), so the column codes go with the column statistics.
+            _, Cgradt, _, SCgradt, _ = F.int8_double_quant(grad_output.to(torch.float16))
+            outliers = state.threshold > 0.0 and subA is not None and subA.numel() > 0
+            if outliers:
+                # CAt zeroes only the entries >= threshold; subA carries the outlier columns whole, so the rest of
+                # those columns must leave the int8 product or it is counted twice
+                int8_zero_columns(CAt, idx)
+            grad_B = torch.ops.bitsandbytes.int8_scaled_mm.default(Cgradt.t().contiguous(), CAt.t(), SCgradt, SCAt,
                                                                    dtype=torch.float16)
-            if state.threshold > 0.0 and subA is not None and subA.numel() > 0:
-                grad_B[:, idx] += torch.matmul(grad_output.t(), subA)
+            if outliers:
+                # fp32 operands: one rounding, to the fp16 of grad_B, whatever the input dtype
+                grad_B[:, idx] += torch.matmul(grad_output.t().float(), subA.float())
 
         if need_A:
             if state.CB is None:

@@ -384,6 +384,19 @@ def int8_vectorwise_quant_flags(A: torch.Tensor, threshold: float):
     return q, row_stats, flags
 
 
+def int8_zero_columns(q: torch.Tensor, cols: torch.Tensor) -> None:
+    """q[..., cols] = 0 in place, for contiguous int8 codes and int64 column indices on q's device."""
+    if q.dtype != torch.int8 or not q.is_contiguous():
+        raise ValueError("q must be contiguous int8")
+    if cols.dtype != torch.int64 or not cols.is_contiguous():
+        raise ValueError("cols must be contiguous int64")
+    rows = q.numel() // q.shape[-1]
+    _check_sizes("int8_zero_columns", rows, q.shape[-1], cols.numel())
+    with _on_device(q):
+        lib.cbnb_b200_int8_zero_columns(q.data_ptr(), cols.data_ptr(), int(cols.numel()), rows, q.shape[-1], _stream(q))
+    lib.check("int8_zero_columns")
+
+
 @kernel("int8_vectorwise_quant")
 def _int8_vectorwise_quant(A: torch.Tensor, threshold=0.0):
     if A.dtype != torch.float16:
@@ -396,10 +409,7 @@ def _int8_vectorwise_quant(A: torch.Tensor, threshold=0.0):
         outlier_cols = torch.nonzero(flags).view(-1)  # data-dependent shape: the one unavoidable sync
         rows = q.numel() // q.shape[-1]
         if outlier_cols.numel() and rows > 1:
-            with _on_device(q):
-                lib.cbnb_b200_int8_zero_columns(q.data_ptr(), outlier_cols.data_ptr(), int(outlier_cols.numel()), rows,
-                                                q.shape[-1], _stream(q))
-            lib.check("int8_vectorwise_quant (outlier columns)")
+            int8_zero_columns(q, outlier_cols)
     return q, row_stats, outlier_cols
 
 

@@ -216,13 +216,14 @@ __global__ void __launch_bounds__(256)
 // A warp walks rows; a lane owns 8 consecutive columns (16-byte loads, 8-byte stores of the codes).
 template <typename T>
 __global__ void __launch_bounds__(256) int8_col_absmax_kernel(const T* __restrict__ A, float* __restrict__ col_stats,
-                                                              float threshold, int rows, int cols, int rows_per_cta) {
+                                                              float threshold, int rows, int cols, int rows_per_cta,
+                                                              int vec_ok) {
     const int c0 = (blockIdx.x * 32 + (threadIdx.x & 31)) * 8;  // this lane's first column
     const int r_begin = blockIdx.y * rows_per_cta + (threadIdx.x >> 5);
     const int r_end = min(rows, (blockIdx.y + 1) * rows_per_cta);
     if (c0 >= cols) return;
     float m[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-    const bool full = c0 + 8 <= cols && (cols & 7) == 0;
+    const bool full = vec_ok && c0 + 8 <= cols;
     for (int r = r_begin; r < r_end; r += 8) {
         float v[8];
         if (full) {
@@ -246,12 +247,12 @@ __global__ void __launch_bounds__(256) int8_col_absmax_kernel(const T* __restric
 template <typename T>
 __global__ void __launch_bounds__(256) int8_col_quant_kernel(const T* __restrict__ A, const float* __restrict__ col_stats,
                                                              int8_t* __restrict__ out, float threshold, int rows, int cols,
-                                                             int rows_per_cta) {
+                                                             int rows_per_cta, int vec_ok) {
     const int c0 = (blockIdx.x * 32 + (threadIdx.x & 31)) * 8;
     const int r_begin = blockIdx.y * rows_per_cta + (threadIdx.x >> 5);
     const int r_end = min(rows, (blockIdx.y + 1) * rows_per_cta);
     if (c0 >= cols) return;
-    const bool full = c0 + 8 <= cols && (cols & 7) == 0;
+    const bool full = vec_ok && c0 + 8 <= cols;
     float cs[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) cs[j] = c0 + j < cols ? col_stats[c0 + j] : 1.f;
@@ -314,9 +315,15 @@ bool launch_int8_col_quant(const void* A, int8_t* out, float* col_stats, float t
     if (slices < 1) slices = 1;
     const int rows_per_cta = (((rows + slices - 1) / slices) + 7) / 8 * 8;
     const dim3 grid(col_ctas, (rows + rows_per_cta - 1) / rows_per_cta);
+    // 16-byte loads of A and 8-byte stores of the codes: whole rows of 8-column groups and aligned bases (a contiguous
+    // view may start at any element of its storage)
+    const int vec_ok = (cols % 8 == 0) && ((reinterpret_cast<uintptr_t>(A) & 15) == 0) &&
+                       ((reinterpret_cast<uintptr_t>(out) & 7) == 0);
 #define BNB200_COLQ(T)                                                                                                 \
-    int8_col_absmax_kernel<T><<<grid, 256, 0, stream>>>((const T*)A, col_stats, threshold, rows, cols, rows_per_cta);  \
-    int8_col_quant_kernel<T><<<grid, 256, 0, stream>>>((const T*)A, col_stats, out, threshold, rows, cols, rows_per_cta)
+    int8_col_absmax_kernel<T><<<grid, 256, 0, stream>>>((const T*)A, col_stats, threshold, rows, cols, rows_per_cta,   \
+                                                        vec_ok);                                                       \
+    int8_col_quant_kernel<T><<<grid, 256, 0, stream>>>((const T*)A, col_stats, out, threshold, rows, cols, rows_per_cta, \
+                                                       vec_ok)
     if (dtype == 1) {
         BNB200_COLQ(__half);
     } else {

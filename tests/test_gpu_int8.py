@@ -67,7 +67,7 @@ def test_vector_quant_outlier_flags(dtype):
 
 
 @pytest.mark.parametrize("M,N,K", [(9, 24, 64), (128, 256, 128), (130, 300, 192), (1, 64, 4096), (300, 1000, 1024),
-                                   (4096, 512, 4096), (77, 11008, 256)])
+                                   (4096, 512, 4096), (77, 11008, 256), (5, 40, 16), (130, 129, 48)])
 def test_int8_gemm_exact(M, N, K):
     g = torch.Generator(device="cpu").manual_seed(M + N + K)
     A = torch.randint(-127, 128, (M, K), generator=g, dtype=torch.int8).cuda()
@@ -101,7 +101,7 @@ def test_int8_gemm_rejects_unaligned_k():
     assert rc == 100  # caller falls back, as for the reference's K % 4 != 0 case
 
 
-@pytest.mark.parametrize("rows,cols", [(9, 24), (64, 4096), (33, 1001), (4096, 512)])
+@pytest.mark.parametrize("rows,cols", [(9, 24), (64, 4096), (33, 1001), (4096, 512), (70000, 12)])
 @pytest.mark.parametrize("with_bias", [False, True])
 def test_mm_dequant_kernel(rows, cols, with_bias):
     g = torch.Generator(device="cpu").manual_seed(rows + cols)
@@ -126,27 +126,42 @@ def test_mm_dequant_kernel(rows, cols, with_bias):
         assert torch.equal(r.view(torch.int16), out.view(torch.int16))
 
 
-@pytest.mark.parametrize("M,N,K", [(9, 24, 64), (200, 384, 256), (4096, 1024, 512)])
+def expected_scaled_mm(C: torch.Tensor, SCA: torch.Tensor, SCB: torch.Tensor, bias, dtype) -> torch.Tensor:
+    """int8_scaled_mm's output from its exact int32 accumulators, by the pinned C restatement of the dequant formula.
+    fp16: fp16(fma(C*SCA*SCB, 1/127^2, bias)).  bf16: the fp16 result without bias, the bias added in fp32 and rounded
+    to fp16, then rounded to bf16 -- the order of the reference's unfused chain, which the fused epilogue keeps."""
+    C, SCA, SCB = C.cpu().numpy(), SCA.cpu().numpy(), SCB.cpu().numpy()
+    if dtype == torch.float16:
+        return nat.from_bits(oracle.int8_mm_dequant(C, SCA, SCB, nat.to_bits(bias) if bias is not None else None), "fp16")
+    h = oracle.widen(oracle.int8_mm_dequant(C, SCA, SCB), "fp16")
+    if bias is not None:
+        h = oracle.widen(oracle.round_to(h + oracle.widen(nat.to_bits(bias), "bf16"), "fp16"), "fp16")
+    return nat.from_bits(oracle.round_to(h, "bf16"), "bf16")
+
+
+# K = 16 / 80 / 208: a k-block of 128 bytes that is mostly past the end of K; N < 8 and N = 129: one partial column
+# pair, and a second tile with one column; M = 1: one valid row in a 128-row tile
+@pytest.mark.parametrize("M,N,K", [(9, 24, 64), (200, 384, 256), (4096, 1024, 512), (33, 5, 16), (1, 129, 80),
+                                   (130, 129, 208), (1, 7, 208)])
 @pytest.mark.parametrize("with_bias", [False, True])
-def test_fused_scaled_mm_equals_gemm_then_dequant(M, N, K, with_bias):
+@pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
+def test_fused_scaled_mm_equals_gemm_then_dequant(M, N, K, with_bias, dtype):
     g = torch.Generator(device="cpu").manual_seed(M * 5 + N)
     CA = torch.randint(-127, 128, (M, K), generator=g, dtype=torch.int8).cuda()
     CB = torch.randint(-127, 128, (N, K), generator=g, dtype=torch.int8).cuda()
     SCA = (torch.rand(M, generator=g) * 5 + 0.5).cuda()
     SCB = (torch.rand(N, generator=g) * 0.1 + 0.01).cuda()
-    bias = torch.randn(N, generator=g).half().cuda() if with_bias else None
-    out = torch.zeros(M, N, device="cuda", dtype=torch.float16)
+    bias = torch.randn(N, generator=g).to(dtype).cuda() if with_bias else None
+    out = torch.full((M, N), float("nan"), device="cuda", dtype=dtype)
     rc = nat.lib.cbnb_b200_int8_scaled_mm(CA.data_ptr(), CB.data_ptr(), SCA.data_ptr(), SCB.data_ptr(), nat.ptr(bias),
-                                          out.data_ptr(), M, N, K, 1, nat.stream())
+                                          out.data_ptr(), M, N, K, 1 if dtype == torch.float16 else 2, nat.stream())
     torch.cuda.synchronize()
     nat.check()
-    assert rc == 0
-    C = (CA.double() @ CB.double().t()).to(torch.int32)
-    want = torch.zeros_like(out)
-    nat.lib.cdequant_mm_int32_fp16(C.data_ptr(), SCA.data_ptr(), SCB.data_ptr(), want.data_ptr(), nat.ptr(bias), M, N,
-                                   nat.stream())
-    torch.cuda.synchronize()
-    assert torch.equal(out.view(torch.int16), want.view(torch.int16))
+    assert rc == 0  # the fused epilogue ran (100 would mean the shape was refused)
+    C = (CA.double() @ CB.double().t()).to(torch.int32)  # exact: |sum| < 2^53
+    want = expected_scaled_mm(C, SCA, SCB, bias, dtype)
+    assert torch.equal(out.view(torch.int16), want.view(torch.int16)), \
+        f"{int((out.view(torch.int16) != want.view(torch.int16)).sum())} of {out.numel()} outputs differ"
 
 
 # ------------------------------------------------------------------------------------------ column-wise quantisation
@@ -183,3 +198,23 @@ def test_native_column_quant_is_bit_identical_to_the_reference_formula(shape, dt
     # the row half is the kernel the forward uses
     rq, rs, oc = F.int8_vectorwise_quant(A, threshold=threshold)
     assert torch.equal(q_row, rq) and torch.equal(row_stats, rs)
+
+
+@pytest.mark.parametrize("offset", [1, 4])
+@pytest.mark.parametrize("threshold", [0.0, 3.0])
+def test_native_column_quant_of_an_unaligned_view(offset, threshold):
+    """A contiguous view that starts `offset` fp16 elements into its storage is not copied on its way to the column
+    kernels: they must not take 16-byte loads from it."""
+    import bitsandbytes_b200.functional as F
+
+    M, K = 96, 256
+    g = torch.Generator(device="cpu").manual_seed(offset + int(threshold))
+    buf = (torch.randn(M * K + 8, generator=g) * 1.5).half().cuda()
+    A = buf[offset:offset + M * K].view(M, K)
+    assert A.is_contiguous() and A.data_ptr() % 16 != 0
+    want_q, want_stats = _reference_col_quant(A, threshold)
+    _, q_col, _, col_stats, _ = F.int8_double_quant(A, threshold=threshold)
+    torch.cuda.synchronize()
+    nat.check()
+    assert torch.equal(col_stats, want_stats)
+    assert torch.equal(q_col, want_q)

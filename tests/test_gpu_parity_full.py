@@ -34,8 +34,10 @@ def _ulp16(x: torch.Tensor, dtype) -> torch.Tensor:
 
 
 # ------------------------------------------------------------------------------------------ fused outlier epilogue
+# jpad -> kernel capacity JMAX: 8 -> 8, 9 -> 16, 24 and 32 -> 32, 41 and 64 -> 64.  K = 80 and 208 end 16 bytes into
+# a k-block.
 @pytest.mark.parametrize("M,N,K,J", [(9, 24, 64, 1), (130, 300, 192, 5), (257, 1000, 1024, 8), (64, 512, 256, 9),
-                                     (300, 384, 512, 41), (128, 256, 128, 64)])
+                                     (300, 384, 512, 41), (128, 256, 128, 64), (150, 200, 80, 24), (129, 260, 208, 32)])
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
 @pytest.mark.parametrize("with_bias", [False, True])
 def test_fused_mixed_mm_equals_the_explicit_chain(M, N, K, J, dtype, with_bias):
