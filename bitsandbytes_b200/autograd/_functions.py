@@ -9,6 +9,8 @@ it dequantises the *row* codes of grad_out with its *column* statistics, and wit
 ``threshold > 0`` it adds the outlier columns of A twice (once in the int8 product, once from
 ``subA``).  Here both operands of grad_outᵀ . A are column codes with their column statistics,
 and the outlier columns are zeroed in the int8 operand before ``subA`` adds them in full.
+With ``threshold > 0``, a forward inside CUDA graph capture keeps the outlier columns on the device
+(``_int8_forward_captured``); that route serves inference only and leaves ``state.idx`` as it was.
 The CPU/XPU-only ``MatMul8bitFp`` of the reference is not provided.
 """
 from __future__ import annotations
@@ -23,7 +25,7 @@ from warnings import warn
 import torch
 
 from .. import functional as F
-from ..backends.cuda import int8_zero_columns
+from ..backends.cuda import int8_mixed_mm_flags, int8_vectorwise_quant_flags, int8_zero_columns
 
 logger = logging.getLogger(__name__)
 
@@ -91,6 +93,34 @@ class MatmulLtState:
         self.SBt = self.CBt = None
 
 
+def _quantize_weight(B, state: MatmulLtState) -> None:
+    """state.CB / state.SCB from the fp16 master weight B, when they are missing or stale."""
+    if state.has_fp16_weights or state.CB is None:
+        has_grad = getattr(B, "grad", None) is not None
+        if not B.is_contiguous() and B.shape[0] == B.stride(1):
+            B = B.contiguous()
+        if (state.is_training and not has_grad) or state.CB is None or state.SCB is None:
+            state.reset_grads()
+            state.CB, state.SCB, _ = F.int8_vectorwise_quant(B.to(torch.float16))
+
+
+_CAPTURED_TRAINING = ("MatMul8bitLt: under CUDA graph capture, LLM.int8() with threshold > 0 runs inference only "
+                      "(torch.no_grad(), or no input that requires grad): its backward needs the outlier columns, whose "
+                      "number depends on the data")
+
+
+def _int8_forward_captured(A, B, bias, state: MatmulLtState):
+    """LLM.int8() inference forward with threshold > 0 while a CUDA graph is being captured.  The outlier columns and
+    their count stay on the device (``int8_mixed_mm_flags``): no host synchronisation, and the captured graph gives the
+    eager result for whatever outlier set a replay meets.  ``state.idx`` is not updated on this route, because the
+    column list has a data-dependent length."""
+    A2 = A.reshape(-1, A.shape[-1])
+    CA, SCA, col_flags = int8_vectorwise_quant_flags(A2.to(torch.float16), state.threshold)
+    _quantize_weight(B, state)
+    out = int8_mixed_mm_flags(A2, CA, state.CB, SCA, state.SCB, col_flags, bias)
+    return out.reshape(*A.shape[:-1], state.CB.shape[0])
+
+
 def _empty_result(A, rows_if_match, shape_a, shape_b):
     if A.shape[-1] == shape_a:
         return torch.empty(A.shape[:-1] + shape_b[1:], dtype=A.dtype, device=A.device)
@@ -107,6 +137,11 @@ class MatMul8bitLt(torch.autograd.Function):
             ctx.A, ctx.B, ctx.bias = A, B, bias
             return _empty_result(A, None, B.shape[0], B.shape)
 
+        if state.threshold > 0.0 and A.is_cuda and torch.cuda.is_current_stream_capturing():
+            if any(ctx.needs_input_grad):
+                raise RuntimeError(_CAPTURED_TRAINING)
+            return _int8_forward_captured(A, B, bias, state)
+
         input_shape = A.shape
         if A.dtype != torch.float16 and not _is_compiling():
             logger.warning("MatMul8bitLt: inputs will be cast from %s to float16 during quantization", A.dtype)
@@ -121,13 +156,7 @@ class MatMul8bitLt(torch.autograd.Function):
             CAt = SCAt = None
 
         # 2. (training with fp16 master weights) quantise the weights
-        if state.has_fp16_weights or state.CB is None:
-            has_grad = getattr(B, "grad", None) is not None
-            if not B.is_contiguous() and B.shape[0] == B.stride(1):
-                B = B.contiguous()
-            if (state.is_training and not has_grad) or state.CB is None or state.SCB is None:
-                state.reset_grads()
-                state.CB, state.SCB, _ = F.int8_vectorwise_quant(B.to(torch.float16))
+        _quantize_weight(B, state)
 
         # 3. int8 GEMM + dequant (+ the outlier columns in 16-bit when threshold > 0)
         if state.threshold > 0.0:
@@ -249,6 +278,11 @@ def matmul(A, B, out=None, state: Optional[MatmulLtState] = None, threshold=0.0,
     state = state or MatmulLtState()
     if threshold > 0.0:
         state.threshold = threshold
+    # Under no_grad nothing is recorded, but MatMul8bitLt.forward cannot see that: it runs with grad disabled, and
+    # ctx.needs_input_grad mirrors requires_grad in every grad mode (True for fp16 master weights).
+    if (state.threshold > 0.0 and not torch.is_grad_enabled() and A.is_cuda and A.numel() > 0
+            and torch.cuda.is_current_stream_capturing()):
+        return _int8_forward_captured(A, B, bias, state)
     return MatMul8bitLt.apply(A, B, out, bias, state)
 
 

@@ -8,7 +8,8 @@ hot path, with three structural differences:
   CUDA cores for fp32 / odd shapes; the choice is made inside the library;
 * ``int8_vectorwise_quant`` finds outlier columns inside the quantisation kernel instead
   of three torch kernels and a host sync (reference :230-236); the data-dependent
-  ``outlier_cols`` tensor still has to be materialised (``nonzero``), once;
+  ``outlier_cols`` tensor still has to be materialised (``nonzero``), once, except on the
+  CUDA-graph route ``int8_mixed_mm_flags``, which keeps the columns and their count on the device;
 * ``int8_scaled_mm`` / ``int8_mixed_scaled_mm`` use the int8 wgmma GEMM with the
   dequantisation fused into its epilogue (the reference chains cuBLASLt -> int32 in HBM ->
   an elementwise kernel, backends/default/ops.py:64-119).
@@ -534,6 +535,78 @@ def _int8_mixed_scaled_mm(A, CA, CB, SCA, SCB, outlier_cols=None, bias=None):
     subA = torch.empty(0, device=A.device, dtype=A.dtype)  # keeps torch.compile's output arity fixed
     out = torch.ops.bitsandbytes.int8_scaled_mm.default(CA, CB, SCA, SCB, bias=bias, dtype=A.dtype)
     return out, subA
+
+
+# outlier columns the operands of the capturable route hold; the GEMM gathers any further ones from A and CB
+INT8_OUTLIER_CAPACITY = 64
+
+
+def int8_outlier_compact(col_flags: torch.Tensor):
+    """(cols, count): the flagged columns of ``col_flags`` (int32 [K]) in ascending order in ``cols[:count]`` (int32
+    [K]), and their number in ``count`` (int32 [1]), both on the device and without a host synchronisation."""
+    if col_flags.dtype != torch.int32 or col_flags.ndim != 1 or not col_flags.is_contiguous():
+        raise ValueError("col_flags must be a contiguous 1-D int32 tensor")
+    K = col_flags.numel()
+    _check_sizes("int8_outlier_compact", K)
+    cols = torch.empty(K, device=col_flags.device, dtype=torch.int32)
+    count = torch.empty(1, device=col_flags.device, dtype=torch.int32)
+    with _on_device(col_flags):
+        lib.cbnb_b200_int8_outlier_compact(col_flags.data_ptr(), K, cols.data_ptr(), count.data_ptr(), _stream(col_flags))
+    lib.check("int8_outlier_compact")
+    return cols, count
+
+
+def int8_mixed_mm_flags(A, CA, CB, SCA, SCB, col_flags, bias=None) -> torch.Tensor:
+    """LLM.int8() forward from the outlier *flags*, with no host synchronisation and no allocation whose size depends
+    on the data, so that it can be captured in a CUDA graph and replayed for any outlier set.
+
+    A: fp16 / bf16 activations [..., K]; CA / SCA: their row codes and statistics with ``col_flags`` (int32 [K]) from
+    :func:`int8_vectorwise_quant_flags`; CB / SCB: the weight codes [N, K] and statistics.  CA (contiguous) is zeroed
+    in place in the outlier columns, as the eager route does.  Returns ``out`` [..., N] of A's dtype: for up to 64
+    outlier columns bit-identical to ``int8_mixed_scaled_mm``, beyond that the same formula summed in column order.
+    The outlier column indices are not returned."""
+    dtype = A.dtype
+    if dtype not in (torch.float16, torch.bfloat16):
+        raise ValueError(f"int8_mixed_mm_flags: A must be float16 or bfloat16, got {dtype}")
+    if CA.dtype != torch.int8 or CB.dtype != torch.int8 or CB.ndim != 2:
+        raise ValueError("int8_mixed_mm_flags: CA and CB must be int8, CB of shape [N, K]")
+    if SCA.dtype != torch.float32 or SCB.dtype != torch.float32:
+        raise ValueError("int8_mixed_mm_flags: SCA and SCB must be float32")
+    if bias is not None and (bias.dtype != dtype or bias.ndim != 1):
+        raise ValueError(f"int8_mixed_mm_flags: bias must be 1-D of A's dtype {dtype}, got {bias.dtype}")
+    N, K = CB.shape
+    if K % 16 != 0:
+        raise ValueError(f"int8_mixed_mm_flags: K = {K} is not a multiple of 16")
+    if A.shape[-1] != K or CA.shape != A.shape or not CA.is_contiguous():
+        raise ValueError(f"int8_mixed_mm_flags: A {tuple(A.shape)} and contiguous CA {tuple(CA.shape)} must be [..., {K}]")
+    if col_flags.shape != (K,):
+        raise ValueError(f"int8_mixed_mm_flags: col_flags must have shape ({K},), got {tuple(col_flags.shape)}")
+    M = CA.numel() // K
+    _check_sizes("int8_mixed_mm_flags", M, N, K)
+    out = torch.empty((*A.shape[:-1], N), device=A.device, dtype=dtype)
+    if M == 0:
+        return out
+    A2 = A.reshape(M, K).contiguous()
+    CB = CB.contiguous()
+    SCA = SCA.contiguous()
+    SCB = SCB.contiguous()
+    bias = bias.contiguous() if bias is not None else None
+    cols, count = int8_outlier_compact(col_flags)
+    subA = torch.empty((M, INT8_OUTLIER_CAPACITY), device=A.device, dtype=dtype)
+    subBT = torch.empty((N, INT8_OUTLIER_CAPACITY), device=A.device, dtype=dtype)
+    with _on_device(A):
+        lib.cbnb_b200_int8_outlier_prep_dev(A2.data_ptr(), CA.data_ptr(), CB.data_ptr(), SCB.data_ptr(), cols.data_ptr(),
+                                            count.data_ptr(), M, N, K, _DTYPE_ID[dtype], subA.data_ptr(),
+                                            subBT.data_ptr(), _stream(A))
+        rc = lib.cbnb_b200_int8_mixed_mm_dev(CA.data_ptr(), CB.data_ptr(), SCA.data_ptr(), SCB.data_ptr(),
+                                             bias.data_ptr() if bias is not None else None, A2.data_ptr(),
+                                             subA.data_ptr(), subBT.data_ptr(), cols.data_ptr(), count.data_ptr(),
+                                             out.data_ptr(), M, N, K, _DTYPE_ID[dtype], _stream(A))
+    lib.check("int8_mixed_mm_flags")
+    if rc != 0:
+        raise RuntimeError(f"int8_mixed_mm_flags: the int8 GEMM does not take this shape (code {rc}): "
+                           f"A={tuple(A.shape)} CB={tuple(CB.shape)}")
+    return out
 
 
 # ------------------------------------------------------------------------------------------ optimizers (section 8 f-4)

@@ -74,6 +74,12 @@ def _signatures():
     sig["cbnb_b200_int8_col_quant"] = ([_VOIDP] * 3 + [ct.c_float] + [_I32] * 3 + [_VOIDP], _I32)
     # (CA, cols, J, rows, K, stream)
     sig["cbnb_b200_int8_zero_columns"] = ([_VOIDP] * 2 + [_I32] * 3 + [_VOIDP], None)
+    # (col_flags, K, cols, count, stream)
+    sig["cbnb_b200_int8_outlier_compact"] = ([_VOIDP, _I32, _VOIDP, _VOIDP, _VOIDP], None)
+    # (A, CA, CB, SCB, cols, count, M, N, K, dtype, subA, subBT, stream)
+    sig["cbnb_b200_int8_outlier_prep_dev"] = ([_VOIDP] * 6 + [_I32] * 4 + [_VOIDP] * 3, None)
+    # (CA, CB, SCA, SCB, bias, A, subA, subBT, cols, count, out, M, N, K, dtype, stream) -> int
+    sig["cbnb_b200_int8_mixed_mm_dev"] = ([_VOIDP] * 11 + [_I32] * 4 + [_VOIDP], _I32)
     # (A, out, rowStats, col_flags, threshold, rows, cols, dtype, stream)
     sig["cbnb_b200_int8_vector_quant_flags"] = ([_VOIDP] * 4 + [ct.c_float] + [_I32] * 3 + [_VOIDP], None)
     # (A, B, value, n)

@@ -52,9 +52,14 @@ void launch_dequant_mm_int32_fp16(const int* A, const float* rowStats, const flo
                                   const __half* bias, int numRows, int numCols, cudaStream_t stream);
 int launch_int8_gemm(const int8_t* acts, const int8_t* weights, void* out, const float* SCA, const float* SCB,
                      const void* bias, int M, int N, int K, int ldc, int epi, cudaStream_t stream,
-                     const void* subA = nullptr, const void* subBT = nullptr, int jpad = 0);
+                     const void* subA = nullptr, const void* subBT = nullptr, int jpad = 0,
+                     const int* jcount = nullptr, const int* cols = nullptr, const void* A = nullptr);
 void launch_int8_outlier_prep(const void* A, const int8_t* CB, const float* SCB, const long long* cols, int J, int jpad,
                               int M, int N, int K, int dtype, void* subA, void* subBT, cudaStream_t stream);
+void launch_int8_outlier_prep_dev(const void* A, int8_t* CA, const int8_t* CB, const float* SCB, const int* cols,
+                                  const int* count, int cap, int M, int N, int K, int dtype, void* subA, void* subBT,
+                                  cudaStream_t stream);
+void launch_int8_outlier_compact(const int* col_flags, int K, int* cols, int* count, cudaStream_t stream);
 void launch_int8_zero_columns(int8_t* CA, const long long* cols, int J, int rows, int K, cudaStream_t stream);
 bool launch_int8_col_quant(const void* A, int8_t* out, float* col_stats, float threshold, int rows, int cols, int dtype,
                            cudaStream_t stream);
@@ -452,6 +457,30 @@ void cbnb_b200_int8_outlier_prep(const void* A, const int8_t* CB, const float* S
 
 void cbnb_b200_int8_zero_columns(int8_t* CA, const long long* cols, int J, int rows, int K, cudaStream_t stream) {
     launch_int8_zero_columns(CA, cols, J, rows, K, stream);
+}
+
+// The same decomposition with the outlier columns and their count kept on the device, so that no launch depends on
+// them and the three launches can be captured in a CUDA graph: compact the flags, build the operands (64 columns,
+// zero-padded) and zero CA's outlier columns, then the GEMM, which reads the count and gathers any columns past 64.
+void cbnb_b200_int8_outlier_compact(const int* col_flags, int K, int* cols, int* count, cudaStream_t stream) {
+    launch_int8_outlier_compact(col_flags, K, cols, count, stream);
+}
+
+void cbnb_b200_int8_outlier_prep_dev(const void* A, int8_t* CA, const int8_t* CB, const float* SCB, const int* cols,
+                                     const int* count, int M, int N, int K, int dtype, void* subA, void* subBT,
+                                     cudaStream_t stream) {
+    if (dtype != 1 && dtype != 2) {
+        set_last_error_msg("int8_outlier_prep_dev: dtype must be 1 (fp16) or 2 (bf16)");
+        return;
+    }
+    launch_int8_outlier_prep_dev(A, CA, CB, SCB, cols, count, 64, M, N, K, dtype, subA, subBT, stream);
+}
+
+int cbnb_b200_int8_mixed_mm_dev(const int8_t* CA, const int8_t* CB, const float* SCA, const float* SCB, const void* bias,
+                                const void* A, const void* subA, const void* subBT, const int* cols, const int* count,
+                                void* out, int M, int N, int K, int dtype, cudaStream_t stream) {
+    if (dtype != 1 && dtype != 2) return 100;
+    return launch_int8_gemm(CA, CB, out, SCA, SCB, bias, M, N, K, N, dtype, stream, subA, subBT, 64, count, cols, A);
 }
 
 // Column-wise absmax + int8 codes of A[rows, cols] (the column half of the reference's int8_double_quant,

@@ -5,6 +5,8 @@
 //                       the absmax pass and the quantise pass) and, optionally, outlier-column
 //                       flags in the same pass (the reference finds them with 3-4 torch kernels
 //                       and a host sync, backends/cuda/ops.py:230-236).
+//   outlier compaction  the outlier flags -> the ascending column list and its count, on the device, for the
+//                       route that a CUDA graph can capture (no torch.nonzero, no host sync).
 //   int8 GEMM           lives in int8_gemm.cu.
 //   dequant_mm_int32    replaces reference kdequant_mm_int32_fp16 (csrc/kernels.cu:1396-1448).
 #include "common.cuh"
@@ -172,11 +174,24 @@ __global__ void __launch_bounds__(256)
 // and dequantises the matching weight columns, already in the [N, jpad] layout the GEMM epilogue reads,
 //     subBT[n, j] = T( (float(CB[n, cols[j]]) * SCB[n]) * (1/127) )  (reference _ops.py:118-121: fp32, then A.dtype)
 // ======================================================================================
-template <typename T>
+// With `count` set (the capturable route), the outlier count is read from device memory: the operands hold the first
+// min(count, jpad) columns, and the launch also zeroes CA[:, cols[j]] for all `count` of them (the job of
+// int8_zero_columns on the eager route).  The grid does not depend on the count.
+template <typename T, typename Idx>
 __global__ void __launch_bounds__(256)
     int8_outlier_prep_kernel(const T* __restrict__ A, const int8_t* __restrict__ CB, const float* __restrict__ SCB,
-                             const long long* __restrict__ cols, int J, int jpad, int M, int N, int K,
-                             T* __restrict__ subA, T* __restrict__ subBT) {
+                             const Idx* __restrict__ cols, const int* __restrict__ count, int J, int jpad, int M, int N,
+                             int K, T* __restrict__ subA, T* __restrict__ subBT, int8_t* __restrict__ CA) {
+    if (count != nullptr) {
+        const int all = *count;
+        J = min(all, jpad);
+        const long long zeros = (long long)M * all;
+        for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < zeros;
+             idx += (long long)gridDim.x * blockDim.x) {
+            const long long r = idx / all;
+            CA[r * K + cols[idx - r * all]] = 0;
+        }
+    }
     const long long total = (long long)(M + N) * jpad;
     for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
          idx += (long long)gridDim.x * blockDim.x) {
@@ -192,6 +207,35 @@ __global__ void __launch_bounds__(256)
             subBT[n * jpad + j] = DT<T>::from_f32(v);
         }
     }
+}
+
+// The outlier columns in ascending order (the order torch.nonzero gives) and their count, without a host round trip.
+// One CTA walks the flags in tiles of 1024 columns: a ballot per warp counts and ranks the flagged columns of the warp,
+// and the counts of the warps before it place them.
+constexpr int kCompactThreads = 1024;
+__global__ void __launch_bounds__(kCompactThreads)
+    int8_outlier_compact_kernel(const int* __restrict__ flags, int K, int* __restrict__ cols, int* __restrict__ count) {
+    __shared__ int s_warp[kCompactThreads / 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int base = 0;
+    for (int c0 = 0; c0 < K; c0 += kCompactThreads) {
+        const int c = c0 + threadIdx.x;
+        const bool f = c < K && flags[c] != 0;
+        const unsigned ballot = __ballot_sync(0xffffffffu, f);
+        if (lane == 0) s_warp[warp] = __popc(ballot);
+        __syncthreads();
+        int before = 0, total = 0;
+#pragma unroll
+        for (int w = 0; w < kCompactThreads / 32; ++w) {
+            const int n = s_warp[w];
+            before += w < warp ? n : 0;
+            total += n;
+        }
+        if (f) cols[base + before + __popc(ballot & ((1u << lane) - 1u))] = c;
+        base += total;
+        __syncthreads();  // s_warp is rewritten by the next tile
+    }
+    if (threadIdx.x == 0) *count = base;
 }
 
 // CA[:, cols[j]] = 0 for every outlier column (reference backends/cuda/ops.py:233-236, a torch index_put there)
@@ -293,13 +337,38 @@ void launch_int8_outlier_prep(const void* A, const int8_t* CB, const float* SCB,
     long long want = (total + 255) / 256;
     const int grid = (int)(want < 132 * 16 ? want : 132 * 16);
     if (dtype == 1)
-        int8_outlier_prep_kernel<__half><<<grid, 256, 0, stream>>>((const __half*)A, CB, SCB, cols, J, jpad, M, N, K,
-                                                                   (__half*)subA, (__half*)subBT);
+        int8_outlier_prep_kernel<__half, long long><<<grid, 256, 0, stream>>>(
+            (const __half*)A, CB, SCB, cols, nullptr, J, jpad, M, N, K, (__half*)subA, (__half*)subBT, nullptr);
     else
-        int8_outlier_prep_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>((const __nv_bfloat16*)A, CB, SCB, cols, J, jpad,
-                                                                          M, N, K, (__nv_bfloat16*)subA,
-                                                                          (__nv_bfloat16*)subBT);
+        int8_outlier_prep_kernel<__nv_bfloat16, long long><<<grid, 256, 0, stream>>>(
+            (const __nv_bfloat16*)A, CB, SCB, cols, nullptr, J, jpad, M, N, K, (__nv_bfloat16*)subA,
+            (__nv_bfloat16*)subBT, nullptr);
     BNB200_CHECK_LAUNCH("int8_outlier_prep");
+}
+
+// The capturable route: `count` and `cols` on the device (from launch_int8_outlier_compact), subA[M, cap] and
+// subBT[N, cap] of a fixed capacity `cap`, CA zeroed in the outlier columns.
+void launch_int8_outlier_prep_dev(const void* A, int8_t* CA, const int8_t* CB, const float* SCB, const int* cols,
+                                  const int* count, int cap, int M, int N, int K, int dtype, void* subA, void* subBT,
+                                  cudaStream_t stream) {
+    if (M + N <= 0) return;
+    // sized by the operands; the zeroing of up to M x K codes strides over the same grid
+    const long long total = (long long)(M + N) * cap;
+    const long long want = (total + 255) / 256;
+    const int grid = (int)(want < 132 * 16 ? want : 132 * 16);
+    if (dtype == 1)
+        int8_outlier_prep_kernel<__half, int><<<grid, 256, 0, stream>>>(
+            (const __half*)A, CB, SCB, cols, count, 0, cap, M, N, K, (__half*)subA, (__half*)subBT, CA);
+    else
+        int8_outlier_prep_kernel<__nv_bfloat16, int><<<grid, 256, 0, stream>>>(
+            (const __nv_bfloat16*)A, CB, SCB, cols, count, 0, cap, M, N, K, (__nv_bfloat16*)subA,
+            (__nv_bfloat16*)subBT, CA);
+    BNB200_CHECK_LAUNCH("int8_outlier_prep_dev");
+}
+
+void launch_int8_outlier_compact(const int* col_flags, int K, int* cols, int* count, cudaStream_t stream) {
+    int8_outlier_compact_kernel<<<1, kCompactThreads, 0, stream>>>(col_flags, K, cols, count);
+    BNB200_CHECK_LAUNCH("int8_outlier_compact");
 }
 
 // q_col[rows, cols] + col_stats[cols] of A[rows, cols]; dtype: 1 fp16, 2 bf16 (false: dtype not served)

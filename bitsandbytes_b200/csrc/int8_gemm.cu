@@ -49,6 +49,12 @@ struct I8Params {
     int M, N, K, ldc;
     int kblocks;
     int n_tiles;
+    // kDevJ instance: the outlier count J on the device (subA / subBT then hold min(J, JMAX) columns at a row pitch of
+    // JMAX), and what the columns past JMAX are gathered from
+    const int* jcount;
+    const int* cols;    // [J] ascending outlier columns
+    const void* A;      // T[M, K] activations
+    const int8_t* CB;   // [N, K] weight codes
 };
 
 // 8 consecutive T -> fp32
@@ -69,7 +75,10 @@ template <int EPI> __device__ __forceinline__ void i8_unpack8(const uint4& r, fl
 
 // JMAX: capacity of the fused outlier term (0 = none): subA of the CTA's 128 tokens and subBT of its 128 features
 // are staged in shared memory after the main loop.
-template <int EPI, int JMAX>
+// kDevJ (JMAX = 64): the outlier count is read from device memory, so one launch serves any J.  The first JMAX columns
+// come from subA / subBT; the rest are gathered from A and CB, JMAX at a time, into the same shared-memory buffers and
+// continue the same fp32 sum in column order.
+template <int EPI, int JMAX, bool kDevJ = false>
 __global__ void __launch_bounds__(kI8Threads, 1)
     int8_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                         const I8Params p) {
@@ -147,7 +156,81 @@ __global__ void __launch_bounds__(kI8Threads, 1)
     // ====================================================================== epilogue
     // acc[4j + e]: token row rl + 8 * (e >= 2), feature column 8j + 2t + (e & 1)
     const int rl = wg * 64 + (warp & 3) * 16 + g;
-    if constexpr (JMAX > 0) {
+    int J = 0;                   // kDevJ: the outlier count
+    float olr[kDevJ ? 64 : 1];   // kDevJ: the outlier term of this thread's outputs, (h, j, u) at 32 h + 2 j + u
+    if constexpr (kDevJ) {
+        static_assert(JMAX == 64, "the device-count instance stages 64 columns at a time");
+        J = __ldg(p.jcount);
+#pragma unroll
+        for (int i = 0; i < 64; ++i) olr[i] = 0.f;
+        // thread e stages row e & 127 of one of the two operands, as below
+        const int e = threadIdx.x;
+        const int r = e & 127;
+        const bool is_b = e >= 128;
+        const int gr = (is_b ? n0 : m0) + r;
+        const bool ok = gr < (is_b ? p.N : p.M);
+        uint4* dst = (is_b ? s_subb : s_suba) + r * (JMAX / 8);
+        for (int c0 = 0; c0 < J; c0 += JMAX) {
+            const int jc = min(J - c0, JMAX);
+            const int jpad = (jc + 7) & ~7;
+            if (c0 == 0) {
+                const uint16_t* src =
+                    reinterpret_cast<const uint16_t*>(is_b ? p.subBT : p.subA) + (long long)(ok ? gr : 0) * JMAX;
+#pragma unroll
+                for (int q = 0; q < JMAX / 8; ++q)
+                    dst[q] = (ok && 8 * q < jpad) ? __ldg(reinterpret_cast<const uint4*>(src) + q) : make_uint4(0, 0, 0, 0);
+            } else {
+                asm volatile("bar.sync 1, 256;" ::: "memory");  // every consumer is done with the previous chunk
+                // subA[m, j] = A[m, cols[j]]; subBT[n, j] = T((float(CB[n, cols[j]]) * SCB[n]) * (1/127)), as the prep
+                // kernel builds them
+                const float scb = ok && is_b ? __ldg(p.SCB + gr) : 0.f;
+                for (int q = 0; q < JMAX / 8; ++q) {
+                    uint32_t w[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+                    for (int x = 0; x < 8; ++x) {
+                        const int jj = 8 * q + x;
+                        if (ok && jj < jc) {
+                            const long long at = (long long)gr * p.K + __ldg(p.cols + c0 + jj);
+                            uint32_t bits;
+                            if (is_b) {
+                                const float v = __fmul_rn(__fmul_rn((float)p.CB[at], scb), 7.874015718698502e-3f);
+                                bits = EPI == 1 ? __half_as_ushort(__float2half_rn(v))
+                                                : __bfloat16_as_ushort(__float2bfloat16_rn(v));
+                            } else {
+                                bits = reinterpret_cast<const uint16_t*>(p.A)[at];
+                            }
+                            w[x >> 1] |= bits << (16 * (x & 1));
+                        }
+                    }
+                    dst[q] = make_uint4(w[0], w[1], w[2], w[3]);
+                }
+            }
+            asm volatile("bar.sync 1, 256;" ::: "memory");
+            // 8 columns at a time for all 64 outputs: each output still sums its columns in order.  The loop keeps the
+            // code small; unrolled over all 64 columns, as the JMAX instances are, this epilogue is ~10 k instructions
+            // and took 2.7x as long at J = 5 and 4096 tokens
+#pragma unroll 1
+            for (int q = 0; q < jpad / 8; ++q) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    float a8[8];
+                    i8_unpack8<EPI>(s_suba[(rl + 8 * h) * (JMAX / 8) + q], a8);
+#pragma unroll
+                    for (int j = 0; j < 16; ++j) {
+                        const uint4* brow = s_subb + (8 * j + 2 * t) * (JMAX / 8);
+                        float b8[8], c8[8];
+                        i8_unpack8<EPI>(brow[q], b8);
+                        i8_unpack8<EPI>(brow[JMAX / 8 + q], c8);
+#pragma unroll
+                        for (int x = 0; x < 8; ++x) {
+                            olr[32 * h + 2 * j] = fmaf(a8[x], b8[x], olr[32 * h + 2 * j]);
+                            olr[32 * h + 2 * j + 1] = fmaf(a8[x], c8[x], olr[32 * h + 2 * j + 1]);
+                        }
+                    }
+                }
+            }
+        }
+    } else if constexpr (JMAX > 0) {
         // stage the outlier operands (zero rows past M / N), thread e owns row e & 127 of one of the two
         const int e = threadIdx.x;
         const int r = e & 127;
@@ -161,6 +244,8 @@ __global__ void __launch_bounds__(kI8Threads, 1)
             dst[q] = (ok && 8 * q < p.jpad) ? __ldg(reinterpret_cast<const uint4*>(src) + q) : make_uint4(0, 0, 0, 0);
         asm volatile("bar.sync 1, 256;" ::: "memory");
     }
+    // with no outlier column at all the result is the plain int8 one: -0 + (+0) would otherwise turn a -0 into +0
+    const bool add_ol = JMAX > 0 && (!kDevJ || J > 0);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
         const int m = m0 + rl + 8 * h;
@@ -182,7 +267,10 @@ __global__ void __launch_bounds__(kI8Threads, 1)
             } else {
             // outlier term of this token and columns n, n + 1: sum_j subA[m, j] * subBT[n, j] in j order (fp32 fma)
             float ol[2] = {0.f, 0.f};
-            if constexpr (JMAX > 0) {
+            if constexpr (kDevJ) {
+                ol[0] = olr[32 * h + 2 * j];
+                ol[1] = olr[32 * h + 2 * j + 1];
+            } else if constexpr (JMAX > 0) {
                 const uint4* arow = s_suba + (rl + 8 * h) * (JMAX / 8);
                 const uint4* brow = s_subb + (8 * j + 2 * t) * (JMAX / 8);
 #pragma unroll
@@ -215,14 +303,14 @@ __global__ void __launch_bounds__(kI8Threads, 1)
                     f[u] = dequant_value(v, sca, scb, b);
                     // reference: the int8 result is an fp16 tensor, then addmm adds the fp32-accumulated
                     // outlier product and rounds once more
-                    if constexpr (JMAX > 0) f[u] = __half2float(__float2half_rn(f[u])) + ol[u];
+                    if (add_ol) f[u] = __half2float(__float2half_rn(f[u])) + ol[u];
                 } else {
                     // bf16 output, bit-identical to the reference chain (backends/cuda/ops.py:186-210): the kernel
                     // result is fp16, a non-fp16 bias is added by `out.add_(bias)` on the fp16 tensor (fp32 add,
                     // one rounding to fp16), then `.to(bfloat16)`.
                     f[u] = __half2float(__float2half_rn(dequant_value(v, sca, scb, 0.f)));
                     if (p.bias != nullptr) f[u] = __half2float(__float2half_rn(f[u] + b));
-                    if constexpr (JMAX > 0) f[u] = __bfloat162float(__float2bfloat16_rn(f[u])) + ol[u];
+                    if (add_ol) f[u] = __bfloat162float(__float2bfloat16_rn(f[u])) + ol[u];
                 }
             }
             const uint32_t w = EPI == 1 ? pack2<__half>(f[0], f[1]) : pack2<__nv_bfloat16>(f[0], f[1]);
@@ -238,14 +326,14 @@ __global__ void __launch_bounds__(kI8Threads, 1)
     }
 }
 
-template <int EPI, int JMAX = 0>
+template <int EPI, int JMAX = 0, bool kDevJ = false>
 int launch_i8(const CUtensorMap& ta, const CUtensorMap& tb, I8Params& p, cudaStream_t stream) {
     constexpr size_t smem_bytes =
         1024 + size_t(I8Cfg<JMAX>::kStages) * kI8StageBytes + 256 + size_t(kI8TileM + kI8TileN) * JMAX * 2;
     static bool attr_set[64] = {};  // the shared-memory opt-in is per device
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 1;
-    auto kern = int8_gemm_tc_kernel<EPI, JMAX>;
+    auto kern = int8_gemm_tc_kernel<EPI, JMAX, kDevJ>;
     p.kblocks = (p.K + kI8BK - 1) / kI8BK;
     if (!attr_set[dev]) {
         if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes) != cudaSuccess) {
@@ -275,14 +363,18 @@ int launch_i8(const CUtensorMap& ta, const CUtensorMap& tb, I8Params& p, cudaStr
 
 // epi: 0 int32, 1 fp16, 2 bf16.  Returns 0 ok, 100 "not implemented for this shape".
 // subA / subBT / jpad: the fused outlier term (epi 1 / 2 only; jpad a multiple of 8, <= 64), or NULL / 0.
+// jcount / cols / A: the outlier count on the device, the ascending outlier columns and the T[M, K] activations they
+// index (epi 1 / 2 only; jpad = 64 is then the row pitch of subA / subBT), or NULL.
 int launch_int8_gemm(const int8_t* acts, const int8_t* weights, void* out, const float* SCA,
                                 const float* SCB, const void* bias, int M, int N, int K, int ldc, int epi,
-                                cudaStream_t stream, const void* subA, const void* subBT, int jpad) {
+                                cudaStream_t stream, const void* subA, const void* subBT, int jpad,
+                                const int* jcount, const int* cols, const void* A) {
     if (M <= 0 || N <= 0) return 0;
     if (K <= 0 || (K % 16) != 0) return 100;
     if (jpad != 0 && (epi == 0 || jpad < 0 || jpad > 64 || (jpad % 8) != 0 || subA == nullptr || subBT == nullptr ||
                       (reinterpret_cast<uintptr_t>(subA) & 15) != 0 || (reinterpret_cast<uintptr_t>(subBT) & 15) != 0))
         return 100;
+    if (jcount != nullptr && (jpad != 64 || cols == nullptr || A == nullptr)) return 100;
     if ((reinterpret_cast<uintptr_t>(acts) & 15) != 0 || (reinterpret_cast<uintptr_t>(weights) & 15) != 0) return 100;
     CUtensorMap ta, tb;
     if (!encode_tmap_2d(&ta, acts, 1, 128, (uint64_t)M, (uint64_t)K, (uint64_t)K, kI8TileM, kI8BK)) return 100;
@@ -299,6 +391,12 @@ int launch_int8_gemm(const int8_t* acts, const int8_t* weights, void* out, const
     p.subA = subA;
     p.subBT = subBT;
     p.jpad = jpad;
+    p.jcount = jcount;
+    p.cols = cols;
+    p.A = A;
+    p.CB = weights;
+    if (jcount != nullptr)
+        return epi == 1 ? launch_i8<1, 64, true>(ta, tb, p, stream) : launch_i8<2, 64, true>(ta, tb, p, stream);
     if (jpad > 0) {
         // fused outlier term, capacity = next of {8, 16, 32, 64}
 #define BNB200_I8_J(E)                                                                                                 \

@@ -190,6 +190,23 @@ int cbnb_b200_int8_col_quant(const void* A, int8_t* out, float* col_stats, float
 /* CA[:, cols[j]] = 0 for the J outlier columns (reference backends/cuda/ops.py:233-236). */
 void cbnb_b200_int8_zero_columns(int8_t* CA, const long long* cols, int J, int rows, int K, bnb_stream_t stream);
 
+/* The same decomposition with the outlier columns and their count kept on the device: no launch depends on them, so
+ * the three calls below can be captured once in a CUDA graph and replayed for any outlier set.
+ *
+ * cols[0 .. *count) = the flagged columns of col_flags[K] in ascending order (what torch.nonzero gives), and *count.
+ * cols holds K ints.  One CTA. */
+void cbnb_b200_int8_outlier_compact(const int* col_flags, int K, int* cols, int* count, bnb_stream_t stream);
+
+/* CA[:, cols[j]] = 0 for every j < *count, and the outlier operands at a fixed capacity of 64 columns:
+ * subA[M, 64] and subBT[N, 64] as cbnb_b200_int8_outlier_prep builds them for j < min(*count, 64), zeros after. */
+void cbnb_b200_int8_outlier_prep_dev(const void* A, int8_t* CA, const int8_t* CB, const float* SCB, const int* cols, const int* count, int M, int N, int K, int dtype, void* subA, void* subBT, bnb_stream_t stream);
+
+/* cbnb_b200_int8_mixed_mm with J = *count read on the device.  The first min(J, 64) outlier columns come from
+ * subA / subBT [*, 64]; columns 64 .. J-1 are gathered from A (T[M, K]) and CB through cols, 64 at a time, and continue
+ * the same fp32 sum in column order.  For J <= 64 the result is bit-identical to cbnb_b200_int8_mixed_mm (J = 0: to
+ * cbnb_b200_int8_scaled_mm).  Returns 0 / 100. */
+int cbnb_b200_int8_mixed_mm_dev(const int8_t* CA, const int8_t* CB, const float* SCA, const float* SCB, const void* bias, const void* A, const void* subA, const void* subBT, const int* cols, const int* count, void* out, int M, int N, int K, int dtype, bnb_stream_t stream);
+
 /* Fused row quantisation + outlier-column detection without a host sync:
  * col_flags[c] = 1 if any |A[r,c]| >= threshold.  dtype 1 = fp16, 2 = bf16 (A is read as
  * that type; the reference kernel is fp16-only). */
