@@ -4,8 +4,9 @@ Plays the role of the reference's ``bitsandbytes/backends/cuda/ops.py`` (:78-982
 hot path, with three structural differences:
 
 * no per-architecture heuristic (reference :583-811) and no dequantize + cuBLAS fallback
-  (:904-916): ``gemm_4bit`` always runs a fused kernel -- wgmma for 16-bit activations,
-  CUDA cores for fp32 / odd shapes; the choice is made inside the library;
+  (:904-916): ``gemm_4bit`` always runs a fused kernel -- wgmma for 16-bit activations and,
+  when PyTorch allows TF32 for fp32 matmuls, for fp32 ones on TF32 tensor cores; CUDA cores
+  for other fp32 calls / odd shapes; the choice is made inside the library;
 * ``int8_vectorwise_quant`` finds outlier columns inside the quantisation kernel instead
   of three torch kernels and a host sync (reference :230-236); the data-dependent
   ``outlier_cols`` tensor still has to be materialised (``nonzero``), once, except on the
@@ -177,9 +178,26 @@ def _dequantize_4bit_out(A, absmax, blocksize: int, quant_type: str, shape: Sequ
 
 
 # ====================================================================================== 4-bit GEMM
+_DTYPE_ID_TF32 = 3  # fp32 activations with TF32 allowed: the library's TF32 tensor-core route
+
+
+def gemm_4bit_dtype_id(dtype: torch.dtype) -> int:
+    """The native dtype id of a 4-bit GEMM with activations of ``dtype``.  fp32 follows PyTorch's fp32 matmul
+    precision, as cuBLAS does for ``torch.matmul``: 3 (TF32 allowed) when
+    ``torch.backends.cuda.matmul.fp32_precision`` is ``"tf32"`` -- set directly, inherited from
+    ``torch.backends.fp32_precision``, or through ``allow_tf32 = True`` / ``set_float32_matmul_precision("high")`` or
+    ``("medium")`` -- and 0 (fp32 CUDA-core products) otherwise.  The setting is read on every call, so a CUDA graph
+    keeps the route in force when it was captured.  (Only ``fp32_precision`` is read: the legacy getters raise once
+    the legacy and the per-backend APIs have been mixed.)"""
+    if dtype == torch.float32 and torch.backends.cuda.matmul.fp32_precision == "tf32":
+        return _DTYPE_ID_TF32
+    return _DTYPE_ID[dtype]
+
+
 def gemm_4bit_into(A, B, shapeB, absmax, blocksize, quant_type, bias, absmax_8bit, absmax_code, absmax_offset,
                    out: torch.Tensor, ldc: int) -> None:
-    """out[:, :N] (row stride ldc) = A . dequant(B)^T + bias.  Shared by the op and the sharded linear."""
+    """out[:, :N] (row stride ldc) = A . dequant(B)^T + bias.  Shared by the op and the sharded linear.  fp32 ``A``
+    runs on TF32 tensor cores when PyTorch's fp32 matmul precision allows TF32 (:func:`gemm_4bit_dtype_id`)."""
     K = A.shape[-1]
     M = A.numel() // K if K else 0
     N = shapeB[0]
@@ -213,7 +231,7 @@ def gemm_4bit_into(A, B, shapeB, absmax, blocksize, quant_type, bias, absmax_8bi
             absmax_code.data_ptr() if absmax_code is not None else None,
             off.data_ptr() if off is not None else None,
             out.data_ptr(), bias.data_ptr() if bias is not None else None,
-            M, N, K, ldc, blocksize, _QT_ID[quant_type], _DTYPE_ID[A.dtype], _stream(A))
+            M, N, K, ldc, blocksize, _QT_ID[quant_type], gemm_4bit_dtype_id(A.dtype), _stream(A))
     lib.check("gemm_4bit")
 
 

@@ -59,6 +59,7 @@ def _signatures():
     sig["cbnb_b200_gemm_4bit_path"] = ([_I32] * 5, _I32)
     sig["cbnb_b200_gemm_4bit_force_path"] = ([_I32], None)
     # (A, B, absmax, absmax_8bit, absmax_code, absmax_offset, out, bias, M, N, K, ldc, blocksize, quant_type, dtype, stream)
+    # dtype for the 4-bit GEMM entries: 0 fp32, 1 fp16, 2 bf16, 3 fp32 with TF32 allowed
     sig["cbnb_b200_gemm_4bit_strided"] = ([_VOIDP] * 8 + [_I32] * 7 + [_VOIDP], None)
     # (A, B, absmax, absmax_8bit, absmax_code, absmax_offset, out, bias, M, N, K, ldc, blocksize, quant_type, dtype,
     #  mt, force_splits, trace, stream) -> int

@@ -125,7 +125,9 @@ bool encode_tmap_2d(CUtensorMap* out, const void* base, int elem_bytes, int swiz
         return false;
     }
     if ((reinterpret_cast<uintptr_t>(base) & 15) != 0 || (row_stride_bytes & 15) != 0) return false;
-    const CUtensorMapDataType dt = elem_bytes == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_UINT16;
+    const CUtensorMapDataType dt = elem_bytes == 1   ? CU_TENSOR_MAP_DATA_TYPE_UINT8
+                                   : elem_bytes == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                                     : CU_TENSOR_MAP_DATA_TYPE_UINT16;
     cuuint64_t gdim[2] = {cols, rows};
     cuuint64_t gstride[1] = {row_stride_bytes};
     cuuint32_t box[2] = {box_cols, box_rows};
@@ -148,6 +150,7 @@ bool encode_tmap_2d(CUtensorMap* out, const void* base, int elem_bytes, int swiz
 
 // ---------------------------------------------------------------- 4-bit GEMM dispatch
 // path: 0 = CUDA-core GEMV, 1 = wgmma GEMM, 2 = CUDA-core generic, 3 = mma.sync decode kernel (M <= 8)
+// dtype: 0 = fp32, 1 = fp16, 2 = bf16, 3 = fp32 with TF32 allowed (the caller's fp32 matmul precision is "tf32")
 static int simt_max_m() {
     static int v = -2;
     if (v == -2) {
@@ -168,6 +171,10 @@ static int mma_max_m() {
     return v;
 }
 
+// dtype 3: fp32 activations take the TF32 instance of the wgmma GEMM from this many tokens on: the measured crossover
+// against the CUDA-core kernel on an H100 (DESIGN.md section 7)
+constexpr int kTf32MinM = 4;
+
 static bool tc_shape_ok(int M, int N, int K, int blocksize, int dtype) {
     (void)M;
     (void)N;
@@ -178,6 +185,11 @@ static bool tc_shape_ok(int M, int N, int K, int blocksize, int dtype) {
 }
 
 static int choose_path(int M, int N, int K, int blocksize, int dtype) {
+    if (dtype == 3) {
+        // TF32 where the wgmma GEMM serves the shape and, unforced, from kTf32MinM tokens; otherwise the fp32 route
+        const bool tc = tc_shape_ok(M, N, K, blocksize, dtype) && (t_forced_path >= 0 ? t_forced_path == 1 : M >= kTf32MinM);
+        return tc ? 1 : choose_path(M, N, K, blocksize, 0);
+    }
     if (t_forced_path >= 0) {
         if ((t_forced_path == 1 || t_forced_path == 3) && !tc_shape_ok(M, N, K, blocksize, dtype)) return 2;
         return t_forced_path;
@@ -211,11 +223,10 @@ static void gemm_4bit_dispatch(const T* A, const uint8_t* B, const float* absmax
         }
     }
     if (path == 1) {
-        if constexpr (!std::is_same<T, float>::value) {
-            if (launch_gemm4_tc<T>(A, B, absmax, absmax_8bit, absmax_code, absmax_offset, out, bias, M, N, K, ldc,
-                                   blocksize, quant_type, stream))
-                return;
-        }
+        // (fp32 takes path 1 only as dtype 3: the TF32 instance)
+        if (launch_gemm4_tc<T>(A, B, absmax, absmax_8bit, absmax_code, absmax_offset, out, bias, M, N, K, ldc,
+                               blocksize, quant_type, stream))
+            return;
     }
     launch_gemv4_simt<T>(A, B, absmax, absmax_8bit, absmax_code, absmax_offset, nullptr, quant_type, out, bias, M, N,
                          K, ldc, blocksize, stream);
@@ -316,9 +327,9 @@ void cbnb_b200_gemm_4bit_strided(const void* A, const uint8_t* B, const float* a
                                  const float* absmax_code, const float* absmax_offset, void* out, const void* bias,
                                  int M, int N, int K, int ldc, int blocksize, int quant_type, int dtype,
                                  cudaStream_t stream) {
-    if (dtype == 0)
+    if (dtype == 0 || dtype == 3)
         gemm_4bit_dispatch<float>((const float*)A, B, absmax, absmax_8bit, absmax_code, absmax_offset, (float*)out,
-                                  (const float*)bias, M, N, K, ldc, blocksize, quant_type, 0, stream);
+                                  (const float*)bias, M, N, K, ldc, blocksize, quant_type, dtype, stream);
     else if (dtype == 1)
         gemm_4bit_dispatch<__half>((const __half*)A, B, absmax, absmax_8bit, absmax_code, absmax_offset, (__half*)out,
                                    (const __half*)bias, M, N, K, ldc, blocksize, quant_type, 1, stream);
@@ -357,8 +368,9 @@ int cbnb_b200_gemm_4bit_multi_out(const void* A, const uint8_t* B, const float* 
 }
 
 // Developer / test entry: the tensor-core kernel of gemm4_tc.cu with an explicit token tile (mt = 16 | 32 | 64 |
-// 128 | 256, 0 = automatic) and a forced K split per tile (0 = the production rule).  `trace` must be NULL.  Returns
-// 0, or 100 when the shape or the options are not served by that kernel.
+// 128 | 256, 0 = automatic; 128 at most for dtype 3, the TF32 instance) and a forced K split per tile (0 = the
+// production rule).  `trace` must be NULL.  Returns 0, or 100 when the shape or the options are not served by that
+// kernel.
 int cbnb_b200_gemm_4bit_pair(const void* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
                              const float* absmax_code, const float* absmax_offset, void* out, const void* bias, int M,
                              int N, int K, int ldc, int blocksize, int quant_type, int dtype, int mt, int force_splits,
@@ -374,6 +386,10 @@ int cbnb_b200_gemm_4bit_pair(const void* A, const uint8_t* B, const float* absma
         ok = launch_gemm4_tc<__nv_bfloat16>((const __nv_bfloat16*)A, B, absmax, absmax_8bit, absmax_code,
                                             absmax_offset, (__nv_bfloat16*)out, (const __nv_bfloat16*)bias, M, N, K,
                                             ldc, blocksize, quant_type, stream, nullptr, 0, mt, force_splits);
+    else if (dtype == 3)
+        ok = launch_gemm4_tc<float>((const float*)A, B, absmax, absmax_8bit, absmax_code, absmax_offset, (float*)out,
+                                    (const float*)bias, M, N, K, ldc, blocksize, quant_type, stream, nullptr, 0, mt,
+                                    force_splits);
     return ok ? 0 : 100;
 }
 

@@ -1,5 +1,6 @@
 // decode4.cuh -- register-resident 4-bit -> 16-bit decode shared by the wgmma GEMM and the
-// CUDA-core GEMV, plus the (optionally double-quantised) scale fetch.
+// CUDA-core GEMV, the 4-bit -> TF32 decode of the GEMM's TF32 instance, plus the (optionally
+// double-quantised) scale fetch.
 #pragma once
 
 #include "common.cuh"
@@ -92,6 +93,63 @@ __device__ __forceinline__ void decode_word(uint32_t w, const DecodeTable& t, ui
         const uint32_t hi = prmt(prmt(t.hi[0], t.hi[1], c), prmt(t.hi[2], t.hi[3], c), selm);
         o[2 * g] = prmt(lo, hi, 0x4051);      // (T[hi nibble of byte 0], T[lo nibble of byte 0])
         o[2 * g + 1] = prmt(lo, hi, 0x6273);  // byte 1
+    }
+}
+
+// ---------------------------------------------------------------- TF32 decode (fp32 activations)
+// W = rna_tf32(value(code) * scale): the fp32 product F.dequantize_4bit(..., torch.float32) returns (mul_ftz, the
+// same scale), rounded to the nearest TF32 value, ties away from zero.  A TF32 value is the top 19 bits of its fp32
+// pattern, so byte 0 of every entry is zero and the table is three byte planes: bytes 3 and 2 (the top 16 bits, as
+// in DecodeTable) and byte 1.
+struct DecodeTableTf32 {
+    uint32_t b1[4];  // b1[j] = byte 1 of entries 4j .. 4j+3
+    uint32_t b2[4];  // byte 2
+    uint32_t b3[4];  // byte 3
+};
+
+__device__ __forceinline__ uint32_t rna_tf32(float x) {
+    uint32_t r;
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+    return r;
+}
+
+template <int QT> __device__ __forceinline__ void build_table_tf32(float scale, DecodeTableTf32& t) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        uint32_t e[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) e[i] = rna_tf32(mul_ftz(code4_value<QT>(4 * j + i), scale));
+        const uint32_t ab13 = prmt(e[0], e[1], 0x7351), cd13 = prmt(e[2], e[3], 0x7351);  // (x.1, y.1, x.3, y.3)
+        const uint32_t ab2 = prmt(e[0], e[1], 0x6262), cd2 = prmt(e[2], e[3], 0x6262);    // (x.2, y.2, x.2, y.2)
+        t.b1[j] = prmt(ab13, cd13, 0x5410);
+        t.b2[j] = prmt(ab2, cd2, 0x5410);
+        t.b3[j] = prmt(ab13, cd13, 0x7632);
+    }
+}
+
+// One word of 8 codes (nibble n = code n, any order the caller chooses) -> o[n] = the TF32 bit pattern of code n.
+// Per four codes: three PRMT look-ups of three planes, two PRMT that interleave byte 1 with zero bytes, two that pair
+// bytes 2 and 3, and one PRMT per value that joins the two halves.
+__device__ __forceinline__ void decode_word_tf32(uint32_t w, const DecodeTableTf32& t, uint32_t (&o)[8]) {
+    const uint32_t c7 = w & 0x77777777u;
+    const uint32_t w1 = shr_fma(w, 0x80000000u);      // w >> 1
+    const uint32_t c7h = shr_fma(c7, 0x00010000u);    // c7 >> 16
+    const uint32_t w17 = shr_fma(w, 0x00008000u);     // w >> 17
+#pragma unroll
+    for (int g = 0; g < 2; ++g) {
+        const uint32_t c = g ? c7h : c7;
+        const uint32_t selm = sel_half(g ? w17 : w1);
+        // byte i of each: the plane's byte of code 4g + i
+        const uint32_t p1 = prmt(prmt(t.b1[0], t.b1[1], c), prmt(t.b1[2], t.b1[3], c), selm);
+        const uint32_t p2 = prmt(prmt(t.b2[0], t.b2[1], c), prmt(t.b2[2], t.b2[3], c), selm);
+        const uint32_t p3 = prmt(prmt(t.b3[0], t.b3[1], c), prmt(t.b3[2], t.b3[3], c), selm);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const uint32_t lo = prmt(p1, 0u, h ? 0x3424 : 0x1404);  // (0, p1[2h], 0, p1[2h+1])
+            const uint32_t hi = prmt(p2, p3, h ? 0x7362 : 0x5140);  // (p2[2h], p3[2h], p2[2h+1], p3[2h+1])
+            o[4 * g + 2 * h] = prmt(lo, hi, 0x5410);
+            o[4 * g + 2 * h + 1] = prmt(lo, hi, 0x7632);
+        }
     }
 }
 

@@ -35,6 +35,10 @@
 // every gridDim-th (tile, K split) unit, with the ring's slot and phase carried across units, so the producer loads
 // the next tile while the consumers run the epilogue.  (Measured on an H100: the persistent loop itself is neutral;
 // it is kept because the one-tile-per-CTA form of this kernel makes ptxas spill at MT = 256.)
+//
+// T = float is the TF32 instance (fp32 activations when the caller allows TF32): wgmma k8 steps on TF32 operands,
+// weights rna_tf32(fp32 dequantised weight) decoded by decode_word_tf32, 64-deep stages of fp32 activations, MT <= 128,
+// an fp32 epilogue that adds the bias and rounds nothing.
 #include "common.cuh"
 #include "decode4.cuh"
 #include "hopper_ptx.cuh"
@@ -79,10 +83,17 @@ struct Gemm4Params {
 };
 
 // one k16 step of a 64-row warpgroup tile: D[64 x MT] += A[64 x 16] (registers) * X[MT x 16]^T (descriptor)
+// (T = float: one k8 step with TF32 operands)
 template <typename T, int MT>
 __device__ __forceinline__ void wgmma_step(float (&d)[MT / 2], const uint32_t (&a)[4], uint64_t b_desc) {
     constexpr bool bf = std::is_same<T, __nv_bfloat16>::value;
-    if constexpr (MT == 16) {
+    if constexpr (std::is_same<T, float>::value) {
+        static_assert(MT <= 128, "TF32 token tile");
+        if constexpr (MT == 16) ptx::wgmma_m64n16k8_tf32_rs(d, a, b_desc);
+        else if constexpr (MT == 32) ptx::wgmma_m64n32k8_tf32_rs(d, a, b_desc);
+        else if constexpr (MT == 64) ptx::wgmma_m64n64k8_tf32_rs(d, a, b_desc);
+        else ptx::wgmma_m64n128k8_tf32_rs(d, a, b_desc);
+    } else if constexpr (MT == 16) {
         if constexpr (bf) ptx::wgmma_m64n16k16_bf16_rs(d, a, b_desc); else ptx::wgmma_m64n16k16_f16_rs(d, a, b_desc);
     } else if constexpr (MT == 32) {
         if constexpr (bf) ptx::wgmma_m64n32k16_bf16_rs(d, a, b_desc); else ptx::wgmma_m64n32k16_f16_rs(d, a, b_desc);
@@ -96,23 +107,27 @@ __device__ __forceinline__ void wgmma_step(float (&d)[MT / 2], const uint32_t (&
     }
 }
 
-// Pipeline stage = BK k-elements: BK/64 64-wide (128-byte, swizzle-atom) activation sub-tiles and the packed codes
-// of 128 rows.  The 256-token tile takes 64-deep stages: a 128-deep one (72 KB) leaves room for two stages only,
-// and two 128-deep A-fragment sets (64 registers) next to its 128 accumulators would not fit the consumers'
-// register budget.  The epilogue stages the output tile in a buffer of its own (the producer is already filling the
-// ring for the CTA's next tile), and the ring takes as many stages as fit next to it, at most 8.
-template <int MT> struct StageCfg {
-    static constexpr int kBK = MT == 256 ? 64 : 128;
-    static constexpr int kSteps = kBK / 16;                      // wgmma k16 steps
+// Pipeline stage = BK k-elements: BK/kSubK activation sub-tiles of 128-byte rows (the swizzle atom: 64 16-bit or 32
+// fp32 elements) and the packed codes of 128 rows.  The 256-token tile takes 64-deep stages: a 128-deep one (72 KB)
+// leaves room for two stages only, and two 128-deep A-fragment sets (64 registers) next to its 128 accumulators would
+// not fit the consumers' register budget.  The TF32 instance (T = float) takes 64-deep stages at every tile: eight k8
+// steps, so its two A-fragment sets are the 64 registers of the 16-bit kernel's 128-deep ones.  The epilogue stages
+// the output tile in a buffer of its own (the producer is already filling the ring for the CTA's next tile), and the
+// ring takes as many stages as fit next to it, at most 8.
+template <typename T, int MT> struct StageCfg {
+    static constexpr bool kTf32 = std::is_same<T, float>::value;
+    static constexpr int kBK = (MT == 256 || kTf32) ? 64 : 128;
+    static constexpr int kSteps = kBK / (kTf32 ? 8 : 16);       // wgmma k16 (k8 for TF32) steps
     static constexpr int kChunks = kBK / 32;                     // 16-byte (32-code) pieces of a code row
-    static constexpr int kXSubBytes = MT * 128;                  // one 64-wide sub-tile
-    static constexpr int kXStageBytes = (kBK / 64) * kXSubBytes;
+    static constexpr int kSubK = 128 / (int)sizeof(T);           // k-elements of one sub-tile row
+    static constexpr int kXSubBytes = MT * 128;                  // one sub-tile
+    static constexpr int kXStageBytes = (kBK / kSubK) * kXSubBytes;
     static constexpr int kWRowBytes = kBK / 2;                   // packed codes of one row (TMA, kWRowBytes-byte swizzle)
     static constexpr int kWStageBytes = kTileN * kWRowBytes;
     static constexpr int kStageBytes = kXStageBytes + kWStageBytes;
     // epilogue staging: one output row of the tile (128 x T) plus 16 bytes, so that the fragment stores (four
     // token rows two apart per warp instruction) fall on distinct banks
-    static constexpr int kOutPitch = kTileN * 2 + 16;
+    static constexpr int kOutPitch = kTileN * (int)sizeof(T) + 16;
     static constexpr int kOutBytes = MT * kOutPitch;
     static constexpr int kSlack = 1024 + 256;                    // base alignment + barriers
     static constexpr int kRing = (227 * 1024 - kSlack - kOutBytes) / kStageBytes;
@@ -127,11 +142,24 @@ __device__ __forceinline__ uint32_t gather_bytes(uint4 v, uint32_t sel) {
     return prmt(prmt(v.x, v.y, sel), prmt(v.z, v.w, sel), 0x5410);
 }
 
+// TF32: a k8 step is one word of the chunk (8 codes, word i = step 4q + i), of which thread t needs codes t and t + 4:
+// byte t/2 and byte t/2 + 2, the high nibble for even t.  `sel` gathers those two bytes of words (x, y) and of
+// (z, w); the code nibbles are then moved into one word: nibble n = 2j + h holds byte j of the h-th gathered pair,
+// that is k8 step 4q + 2h + j/2 and k t + 4 (j & 1).  `shr` = 4 for even t, 0 for odd; `mul` = 1 << (4 - shr).
+__device__ __forceinline__ uint32_t gather_nibbles(uint4 v, uint32_t sel, uint32_t shr, uint32_t mul) {
+    const uint32_t r0 = prmt(v.x, v.y, sel) >> shr;
+    const uint32_t r1 = prmt(v.z, v.w, sel) * mul;
+    uint32_t r;
+    asm("lop3.b32 %0, %1, %2, 0x0F0F0F0F, 0xE4;" : "=r"(r) : "r"(r0), "r"(r1));  // (r0 & m) | (r1 & ~m)
+    return r;
+}
+
 template <typename T, int QT, int MT, bool DQ>
 __global__ void __launch_bounds__(kThreads, 1)
     gemm4_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
                     const Gemm4Params p) {
-    using Cfg = StageCfg<MT>;
+    using Cfg = StageCfg<T, MT>;
+    constexpr bool kTf32 = Cfg::kTf32;
     constexpr int kBK = Cfg::kBK;
     constexpr int kSteps = Cfg::kSteps;
     constexpr int kChunks = Cfg::kChunks;
@@ -146,7 +174,7 @@ __global__ void __launch_bounds__(kThreads, 1)
     // (ld.shared for the codes, not generic loads)
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
-    uint8_t* sx = smem;                              // [kStages][BK/64][MT x 128 B]   activations
+    uint8_t* sx = smem;                              // [kStages][BK/kSubK][MT x 128 B] activations
     uint8_t* sw = smem + kStages * kXStageBytes;     // [kStages][128 x BK/2 B]        packed codes
     uint8_t* so = smem + kStages * Cfg::kStageBytes; // [MT][kOutPitch]                epilogue staging
     uint64_t* bars = reinterpret_cast<uint64_t*>(so + Cfg::kOutBytes);
@@ -207,9 +235,9 @@ __global__ void __launch_bounds__(kThreads, 1)
                     // zero-fills.  Packed codes of the tile's 128 output features: bytes [k0/2, k0/2 + BK/2).
                     ptx::tma_load_2d(sw + slot * kWStageBytes, &tmap_w, &full[slot], k0 / 2, w.n0);
 #pragma unroll
-                    for (int h = 0; h < kBK / 64; ++h)
+                    for (int h = 0; h < kBK / Cfg::kSubK; ++h)
                         ptx::tma_load_2d(sx + slot * kXStageBytes + h * kXSubBytes, &tmap_x, &full[slot],
-                                         k0 + 64 * h, w.m0);
+                                         k0 + Cfg::kSubK * h, w.m0);
                     if (++slot == kStages) {
                         slot = 0;
                         phase ^= 1u;
@@ -276,22 +304,40 @@ __global__ void __launch_bounds__(kThreads, 1)
                     v[r][q] = *reinterpret_cast<const uint4*>(wt + (row0 + 8 * r) * kWRowBytes + (((uint32_t)q ^ swz[r]) << 4));
 #pragma unroll
             for (int r = 0; r < 2; ++r) {
-                DecodeTable tab;
+                if constexpr (kTf32) {
+                    // gather_nibbles: bytes t/2 and t/2 + 2 of two words, the high nibble for even t
+                    const uint32_t tsel = (uint32_t)(t >> 1) * 0x1111u + 0x6420u;
+                    const uint32_t tshr = (t & 1) ? 0u : 4u;
+                    const uint32_t tmul = (t & 1) ? 16u : 1u;
+                    DecodeTableTf32 tab;
 #pragma unroll
-                for (int q = 0; q < kChunks; ++q) {
-                    if ((q & smask) == 0) build_table<T, QT>(scl[r][q], tab);
-                    uint32_t o[4];
-                    decode_word(gather_bytes(v[r][q], sel), tab, o);
-                    // o[i]: byte i of the gathered word = word 4q+i of the row -> k16 step 2q + i/2, half i%2
+                    for (int q = 0; q < kChunks; ++q) {
+                        if ((q & smask) == 0) build_table_tf32<QT>(scl[r][q], tab);
+                        uint32_t o[8];
+                        decode_word_tf32(gather_nibbles(v[r][q], tsel, tshr, tmul), tab, o);
+                        // o[n]: k8 step 4q + 2(n & 1) + n/4, k t + 4((n >> 1) & 1) -> register r (k t) or 2 + r (t + 4)
 #pragma unroll
-                    for (int u = 0; u < 2; ++u) {
-                        a[2 * q + u][r] = o[2 * u];          // rows g / g+8, k 2t..2t+1
-                        a[2 * q + u][2 + r] = o[2 * u + 1];  // rows g / g+8, k 8+2t..9+2t
+                        for (int n = 0; n < 8; ++n) a[4 * q + 2 * (n & 1) + (n >> 2)][r + 2 * ((n >> 1) & 1)] = o[n];
+                    }
+                } else {
+                    DecodeTable tab;
+#pragma unroll
+                    for (int q = 0; q < kChunks; ++q) {
+                        if ((q & smask) == 0) build_table<T, QT>(scl[r][q], tab);
+                        uint32_t o[4];
+                        decode_word(gather_bytes(v[r][q], sel), tab, o);
+                        // o[i]: byte i of the gathered word = word 4q+i of the row -> k16 step 2q + i/2, half i%2
+#pragma unroll
+                        for (int u = 0; u < 2; ++u) {
+                            a[2 * q + u][r] = o[2 * u];          // rows g / g+8, k 2t..2t+1
+                            a[2 * q + u][2 + r] = o[2 * u + 1];  // rows g / g+8, k 8+2t..9+2t
+                        }
                     }
                 }
             }
         };
 
+        // a k16 step (k8 for TF32) is 32 bytes of an activation row: four per 128-byte sub-tile row
         auto mma_stage = [&](int s, const uint32_t (&a)[kSteps][4]) {
             const uint32_t xs = ptx::smem_u32(sx + s * kXStageBytes);
             ptx::wgmma_fence();
@@ -341,29 +387,30 @@ __global__ void __launch_bounds__(kThreads, 1)
             const float bias_a = (bias != nullptr && a_ok) ? DT<T>::to_f32(bias[na]) : 0.f;
             const float bias_b = (bias != nullptr && b_ok) ? DT<T>::to_f32(bias[nb]) : 0.f;
             // Stage the rounded tile as [token][feature] rows -- once both warpgroups are done reading the previous
-            // unit's tile there -- then store it in 16-byte row pieces: each token row of the tile is 256 contiguous
-            // bytes of the output.
+            // unit's tile there -- then store it in 16-byte row pieces of kVec elements: each token row of the tile is
+            // 128 contiguous elements of the output.  (fp32: the bias is added in fp32 and nothing is rounded.)
             constexpr int kPitch = Cfg::kOutPitch;
+            constexpr int kVec = 16 / (int)sizeof(T);
             ptx::bar_sync(kBarEpi, kConsumers);
 #pragma unroll
             for (int j = 0; j < MT / 8; ++j)
 #pragma unroll
                 for (int e = 0; e < 4; ++e)
-                    *reinterpret_cast<T*>(so + (8 * j + 2 * t + (e & 1)) * kPitch + (row0 + 8 * (e >> 1)) * 2) =
+                    *reinterpret_cast<T*>(so + (8 * j + 2 * t + (e & 1)) * kPitch + (row0 + 8 * (e >> 1)) * (int)sizeof(T)) =
                         DT<T>::from_f32(acc[4 * j + e] + (e >= 2 ? bias_b : bias_a));
             ptx::bar_sync(kBarEpi, kConsumers);
-            for (int idx = ct; idx < MT * (kTileN / 8); idx += kConsumers) {
-                const int c = idx / (kTileN / 8), n = n0 + 8 * (idx % (kTileN / 8));
+            for (int idx = ct; idx < MT * (kTileN / kVec); idx += kConsumers) {
+                const int c = idx / (kTileN / kVec), n = n0 + kVec * (idx % (kTileN / kVec));
                 const int m = m0 + c;
                 if (m >= p.M || n >= p.N) continue;
-                const uint8_t* src = so + c * kPitch + (n - n0) * 2;
+                const uint8_t* src = so + c * kPitch + (n - n0) * (int)sizeof(T);
                 const long long o = (long long)m * p.ldc + n;
-                if (p.out_vec && n + 8 <= p.N) {
+                if (p.out_vec && n + kVec <= p.N) {
                     const uint4 val = *reinterpret_cast<const uint4*>(src);
                     *reinterpret_cast<uint4*>(outp + o) = val;
                     for (int r = 0; r < p.n_peers; ++r) *reinterpret_cast<uint4*>(reinterpret_cast<T*>(p.peer_out[r]) + o) = val;
                 } else {
-                    for (int x = 0; x < 8 && n + x < p.N; ++x) {
+                    for (int x = 0; x < kVec && n + x < p.N; ++x) {
                         const T val = reinterpret_cast<const T*>(src)[x];
                         outp[o + x] = val;
                         for (int r = 0; r < p.n_peers; ++r) reinterpret_cast<T*>(p.peer_out[r])[o + x] = val;
@@ -521,7 +568,7 @@ Workspace* get_workspace(cudaStream_t stream, size_t partial_bytes, size_t n_cou
 
 template <typename T, int QT, int MT, bool DQ>
 bool launch_mt(const T* A, Gemm4Params& p, int force_splits, cudaStream_t stream) {
-    using Cfg = StageCfg<MT>;
+    using Cfg = StageCfg<T, MT>;
     constexpr int kBK = Cfg::kBK;
     constexpr size_t smem_bytes = Cfg::kSmemBytes;
     // the shared-memory opt-in is PER DEVICE (one process may drive several GPUs)
@@ -537,7 +584,10 @@ bool launch_mt(const T* A, Gemm4Params& p, int force_splits, cudaStream_t stream
         attr_set[dev] = true;
     }
     CUtensorMap tmap, tmap_w;
-    if (!encode_tmap_2d(&tmap, A, 2, 128, (uint64_t)p.M, (uint64_t)p.K, (uint64_t)p.K * 2, (uint32_t)MT, 64u)) return false;
+    // activations [M, K]: MT x kSubK boxes (128-byte rows), 128-byte swizzle (fp32 for the TF32 instance)
+    if (!encode_tmap_2d(&tmap, A, (int)sizeof(T), 128, (uint64_t)p.M, (uint64_t)p.K, (uint64_t)p.K * sizeof(T),
+                        (uint32_t)MT, (uint32_t)Cfg::kSubK))
+        return false;
     // packed codes as a [N, K/2] byte matrix, 128 x BK/2-byte boxes, BK/2-byte swizzle
     if (!encode_tmap_2d(&tmap_w, p.B, 1, Cfg::kWRowBytes, (uint64_t)p.N, (uint64_t)p.K / 2, (uint64_t)p.K / 2,
                         (uint32_t)kTileN, (uint32_t)Cfg::kWRowBytes))
@@ -628,14 +678,18 @@ bool launch_gemm4_tc(const T* A, const uint8_t* B, const float* absmax, const ui
     if (quant_type != kNF4 && quant_type != kFP4) return false;
 
     // 256-token tiles decode each weight half as often as 128-token ones, but a grid of them that does not fill one
-    // wave leaves SMs idle (or needs a K split): they are taken when they alone fill every SM.
+    // wave leaves SMs idle (or needs a K split): they are taken when they alone fill every SM.  The TF32 instance stops
+    // at 128 tokens: one 64-deep fp32 stage of a 256-token tile (68 KB) next to its 132 KB of epilogue staging leaves
+    // room for a single ring stage.
+    constexpr bool tf32 = std::is_same<T, float>::value;
     int MT = 128;
     if (M <= 16) MT = 16;
     else if (M <= 32) MT = 32;
     else if (M <= 64) MT = 64;
-    else if ((long long)((M + 255) / 256) * ((N + kTileN - 1) / kTileN) >= device_sm_count()) MT = 256;
+    else if (!tf32 && (long long)((M + 255) / 256) * ((N + kTileN - 1) / kTileN) >= device_sm_count()) MT = 256;
     if (mt_override != 0) {
-        if (mt_override != 16 && mt_override != 32 && mt_override != 64 && mt_override != 128 && mt_override != 256)
+        if (mt_override != 16 && mt_override != 32 && mt_override != 64 && mt_override != 128 &&
+            (tf32 || mt_override != 256))
             return false;
         MT = mt_override;
     }
@@ -655,7 +709,7 @@ bool launch_gemm4_tc(const T* A, const uint8_t* B, const float* absmax, const ui
     p.K = K;
     p.ldc = ldc;
     p.log2_bs = ilog2_pow2(blocksize);
-    bool vec = (ldc % 8) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0;
+    bool vec = (ldc % (16 / (int)sizeof(T))) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0;
     for (int r = 0; r < n_peers; ++r) vec = vec && (reinterpret_cast<uintptr_t>(peers[r]) & 15) == 0;
     p.out_vec = vec ? 1 : 0;
 
@@ -665,7 +719,9 @@ bool launch_gemm4_tc(const T* A, const uint8_t* B, const float* absmax, const ui
     case 32: return launch_mt<T, QT, 32, DQ>(A, p, force_splits, stream);                                              \
     case 64: return launch_mt<T, QT, 64, DQ>(A, p, force_splits, stream);                                              \
     case 128: return launch_mt<T, QT, 128, DQ>(A, p, force_splits, stream);                                            \
-    default: return launch_mt<T, QT, 256, DQ>(A, p, force_splits, stream);                                             \
+    default:                                                                                                           \
+        if constexpr (tf32) return false;                                                                              \
+        else return launch_mt<T, QT, 256, DQ>(A, p, force_splits, stream);                                             \
     }
     const bool dq = absmax_8bit != nullptr;
     if (quant_type == kNF4) {
@@ -690,5 +746,9 @@ template bool launch_gemm4_tc<__nv_bfloat16>(const __nv_bfloat16*, const uint8_t
 template bool launch_gemm4_tc<__half>(const __half*, const uint8_t*, const float*, const uint8_t*, const float*,
                                       const float*, __half*, const __half*, int, int, int, int, int, int,
                                       cudaStream_t, void* const*, int, int, int);
+// fp32 activations and output, TF32 tensor cores
+template bool launch_gemm4_tc<float>(const float*, const uint8_t*, const float*, const uint8_t*, const float*,
+                                     const float*, float*, const float*, int, int, int, int, int, int, cudaStream_t,
+                                     void* const*, int, int, int);
 
 } // namespace bnb200

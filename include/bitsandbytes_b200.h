@@ -151,14 +151,17 @@ int cbnb_b200_gemm_4bit_multi_out(const void* A, const uint8_t* B, const float* 
 
 /* Which kernel a (M, N, K, blocksize, dtype) 4-bit GEMM takes: 0 = CUDA-core GEMV,
  * 1 = wgmma GEMM, 2 = generic CUDA-core kernel, 3 = mma.sync decode kernel (M <= 8).
+ * dtype for the 4-bit GEMM entries below: 0 = fp32, 1 = fp16, 2 = bf16, 3 = fp32 with TF32 allowed -- the
+ * caller's fp32 matmul precision is "tf32": from 4 tokens on (K % 64 == 0, power-of-two blocksize >= 32) the
+ * wgmma GEMM runs on TF32 tensor cores with weights rna_tf32(fp32 dequantised weight); otherwise as dtype 0.
  * For tests / bench bookkeeping. */
 int cbnb_b200_gemm_4bit_path(int M, int N, int K, int blocksize, int dtype);
 /* Force a path for the next calls on this thread (-1 = automatic). */
 void cbnb_b200_gemm_4bit_force_path(int path);
 
 /* Developer / test entry for the wgmma 4-bit GEMM (csrc/gemm4_tc.cu): explicit token tile mt (16 | 32 | 64 | 128 |
- * 256; 0 = by M) and forced K split per tile (0 = production rule; s = up to s ways, at least one stage per split:
- * 128 deep, 64 deep at mt = 256).  `trace` must be NULL (the name and argument list are kept for ABI stability).  Returns 0, or 100 when
+ * 256, at most 128 for dtype 3; 0 = by M) and forced K split per tile (0 = production rule; s = up to s ways, at
+ * least one stage per split: 128 deep, 64 deep at mt = 256 and for dtype 3).  dtype 1, 2 or 3 (TF32).  `trace` must be NULL (the name and argument list are kept for ABI stability).  Returns 0, or 100 when
  * the shape or the options are not served (a forced split must fit one co-resident wave of CTAs). */
 int cbnb_b200_gemm_4bit_pair(const void* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit, const float* absmax_code, const float* absmax_offset, void* out, const void* bias, int M, int N, int K, int ldc, int blocksize, int quant_type, int dtype, int mt, int force_splits, long long* trace, bnb_stream_t stream);
 
