@@ -28,6 +28,7 @@ from warnings import warn
 import torch
 
 from .._ops import kernel
+from .. import cextension as cext
 from ..cextension import lib
 
 _DTYPE_SUFFIX = {torch.float32: "fp32", torch.float16: "fp16", torch.bfloat16: "bf16"}
@@ -689,3 +690,105 @@ def _optimizer_update_8bit_blockwise(optimizer_name, g, p, state1, state2, beta1
     lib.check("optimizer_update_8bit_blockwise")
     if rc != 0:
         raise RuntimeError(f"optimizer_update_8bit_blockwise: native call returned {rc}")
+
+
+# ---- multi-tensor steps: one native call per descriptor-capacity chunk of a list of tensors that share every scalar
+_multi_capacity = None
+
+
+def optimizer_multi_capacity() -> int:
+    """Tensors per multi-tensor launch: the descriptors travel as a kernel parameter (at most 32764 bytes)."""
+    global _multi_capacity
+    if _multi_capacity is None:
+        _multi_capacity = int(lib.cbnb_b200_optimizer_multi_capacity())
+    return _multi_capacity
+
+
+def _optimizer_list(what, optimizer_name, supported, g, p, state1, state2, absmax1, absmax2, step, eight_bit):
+    """Validate a multi-tensor step as the single-tensor ops do and pack its descriptors (cextension.OptimTensor)."""
+    if optimizer_name not in supported:
+        raise ValueError(f"Unsupported optimizer name: {optimizer_name}. Supported optimizers: {list(supported)}")
+    k = len(p)
+    two = optimizer_name in ("adam", "ademamix", "lamb")
+    lists = {"g": g, "state1": state1, "step": step}
+    if two:
+        lists["state2"] = state2
+    if eight_bit:
+        lists["absmax1"] = absmax1
+        if two:
+            lists["absmax2"] = absmax2
+    for name, values in lists.items():
+        if values is None or len(values) != k:
+            raise ValueError(f"{what}: {name} must list one entry per parameter ({k})")
+    if k == 0:
+        return None, None
+    dtype, device = g[0].dtype, g[0].device
+    if dtype not in _DTYPE_ID:
+        raise ValueError(f"{what}: unsupported gradient dtype {dtype}. Supported dtypes: torch.float32, torch.float16, "
+                         "torch.bfloat16")
+    if device.type != "cuda":
+        raise RuntimeError(f"{what}: tensors must live on a CUDA device, got {device}")
+    descs = []
+    for i in range(k):
+        s2 = state2[i] if two else None
+        a1 = absmax1[i] if eight_bit else None
+        a2 = absmax2[i] if eight_bit and two else None
+        gi, pi = g[i], p[i]
+        if gi.dtype != dtype or pi.dtype != dtype or gi.numel() != pi.numel():
+            raise ValueError(f"{what}: every g and p must have dtype {dtype} and g and p the same number of elements "
+                             f"(entry {i}: {gi.dtype} {tuple(gi.shape)}, {pi.dtype} {tuple(pi.shape)})")
+        for t in (gi, pi, state1[i], s2, a1, a2):
+            if t is None:
+                continue
+            if not t.is_contiguous():
+                raise ValueError(f"{what}: tensors must be contiguous (entry {i})")
+            # managed ("paged") state is a CPU tensor to PyTorch that every GPU can address
+            if t.device != device and not getattr(t, "is_paged", False):
+                raise RuntimeError(f"{what}: tensors must be on one device, {device}; entry {i} has one on {t.device}")
+        descs.append(cext.OptimTensor(pi.data_ptr(), gi.data_ptr(), state1[i].data_ptr(), _optional_ptr(s2),
+                                      _optional_ptr(a1), _optional_ptr(a2), pi.numel(), int(step[i]), 0))
+    return g[0], (cext.OptimTensor * k)(*descs)
+
+
+def _launch_list(what, fn, optimizer_name, g0, descs, scalars):
+    """fn(optimizer, dtype, tensors, count, *scalars, stream) once per capacity chunk of descs."""
+    cap, k, size = optimizer_multi_capacity(), len(descs), ct.sizeof(cext.OptimTensor)
+    for lo in range(0, k, cap):
+        rc = fn(_OPTIMIZER_ID[optimizer_name], _DTYPE_ID[g0.dtype], ct.addressof(descs) + lo * size, min(cap, k - lo),
+                *scalars, _stream(g0))
+        lib.check(what)
+        if rc != 0:
+            raise RuntimeError(f"{what}: native call returned {rc}")
+
+
+def optimizer_update_32bit_multi(optimizer_name, g, p, state1, state2, beta1, beta2, beta3, alpha, eps, weight_decay, step,
+                                 lr, gnorm_scale=1.0, skip_zeros=False):
+    """In-place fp32-state steps of several parameters in one launch per capacity chunk: g, p, state1, state2 (None for
+    one-state optimizers) and step list one entry per parameter; the scalars are shared.  No trust ratio (max_unorm)."""
+    what = "optimizer_update_32bit_multi"
+    g0, descs = _optimizer_list(what, optimizer_name, _OPTIMIZER_ID, g, p, state1, state2, None, None, step, False)
+    if descs is None:
+        return
+    with _on_device(g0):
+        _launch_list(what, lib.cbnb_b200_optimizer_update_32bit_multi, optimizer_name, g0, descs,
+                     (float(beta1), float(beta2), float(beta3), float(alpha), float(eps), float(weight_decay), float(lr),
+                      float(gnorm_scale), bool(skip_zeros)))
+
+
+def optimizer_update_8bit_blockwise_multi(optimizer_name, g, p, state1, state2, beta1, beta2, beta3, alpha, eps, step, lr,
+                                          qmap1, qmap2, absmax1, absmax2, weight_decay, gnorm_scale=1.0, skip_zeros=False):
+    """In-place blockwise (256) 8-bit-state steps of several parameters in one launch per capacity chunk: g, p, state1,
+    state2, absmax1, absmax2 and step list one entry per parameter (state2 / absmax2 None for one-state optimizers);
+    the code books qmap1 / qmap2 and the scalars are shared."""
+    what = "optimizer_update_8bit_blockwise_multi"
+    g0, descs = _optimizer_list(what, optimizer_name, _OPTIMIZER_8BIT, g, p, state1, state2, absmax1, absmax2, step, True)
+    if descs is None:
+        return
+    two = optimizer_name in ("adam", "ademamix")
+    for q in (qmap1, qmap2) if two else (qmap1,):
+        if q is None or q.device != g0.device or not q.is_contiguous() or q.dtype != torch.float32 or q.numel() < 256:
+            raise ValueError(f"{what}: the code books must be contiguous fp32 [256] tensors on {g0.device}")
+    with _on_device(g0):
+        _launch_list(what, lib.cbnb_b200_optimizer_update_8bit_blockwise_multi, optimizer_name, g0, descs,
+                     (float(beta1), float(beta2), float(beta3), float(alpha), float(eps), float(weight_decay), float(lr),
+                      qmap1.data_ptr(), qmap2.data_ptr() if two else None, float(gnorm_scale), bool(skip_zeros)))

@@ -113,7 +113,22 @@ def _signatures():
     #  gnorm_scale, skip_zeros, n, stream) -> int
     sig["cbnb_b200_optimizer_update_8bit_blockwise"] = ([_I32, _I32] + [_VOIDP] * 4 + [_F] * 5 + [_I32, _F] + [_VOIDP] * 4
                                                         + [_F, _F, ct.c_bool, ct.c_longlong, _VOIDP], _I32)
+    sig["cbnb_b200_optimizer_multi_capacity"] = ([], _I32)
+    # (optimizer, dtype, tensors (bnb_b200_optim_tensor_t[count]), count, beta1, beta2, beta3, alpha, eps, weight_decay,
+    #  lr, gnorm_scale, skip_zeros, stream) -> int
+    sig["cbnb_b200_optimizer_update_32bit_multi"] = ([_I32, _I32, _VOIDP, _I32] + [_F] * 8 + [ct.c_bool, _VOIDP], _I32)
+    # (optimizer, dtype, tensors, count, beta1, beta2, beta3, alpha, eps, weight_decay, lr, q1, q2, gnorm_scale,
+    #  skip_zeros, stream) -> int
+    sig["cbnb_b200_optimizer_update_8bit_blockwise_multi"] = ([_I32, _I32, _VOIDP, _I32] + [_F] * 7 + [_VOIDP, _VOIDP, _F,
+                                                               ct.c_bool, _VOIDP], _I32)
     return sig
+
+
+class OptimTensor(ct.Structure):
+    """One entry of a multi-tensor optimizer call: bnb_b200_optim_tensor_t of include/bitsandbytes_b200.h."""
+
+    _fields_ = [("p", _VOIDP), ("g", _VOIDP), ("state1", _VOIDP), ("state2", _VOIDP), ("absmax1", _VOIDP),
+                ("absmax2", _VOIDP), ("n", ct.c_longlong), ("step", ct.c_int32), ("reserved", ct.c_int32)]
 
 
 EXPORTED_SYMBOLS = tuple(sorted(_signatures()))

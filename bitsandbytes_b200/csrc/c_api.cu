@@ -32,6 +32,13 @@ bool launch_optimizer8bit_blockwise(int opt, int dtype, void* p, const void* g, 
                                     float beta1, float beta2, float beta3, float alpha, float eps, int step, float lr,
                                     const float* q1, const float* q2, float* a1, float* a2, float wd,
                                     float gnorm_scale, bool skip_zeros, long n, cudaStream_t st);
+int optimizer_list_capacity();
+bool launch_optimizer32bit_list(int opt, int dtype, const OptimTensor* ts, int count, float beta1, float beta2,
+                                float beta3, float alpha, float eps, float wd, float lr, float gnorm_scale,
+                                bool skip_zeros, cudaStream_t st);
+bool launch_optimizer8bit_blockwise_list(int opt, int dtype, const OptimTensor* ts, int count, float beta1, float beta2,
+                                         float beta3, float alpha, float eps, float wd, float lr, const float* q1,
+                                         const float* q2, float gnorm_scale, bool skip_zeros, cudaStream_t st);
 
 template <typename T>
 void launch_gemv4_simt(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
@@ -593,6 +600,42 @@ int cbnb_b200_optimizer_update_8bit_blockwise(int optimizer, int dtype, void* p,
                                           skip_zeros, (long)n, stream)
                ? 0
                : 100;
+}
+
+// Multi-tensor steps: one launch updates `count` tensors that share every per-launch scalar (and, 8-bit, the code
+// books); each tensor brings its own pointers, size and step.  count <= cbnb_b200_optimizer_multi_capacity().
+int cbnb_b200_optimizer_multi_capacity(void) { return optimizer_list_capacity(); }
+
+static bool optimizer_list_ok(const char* what, int optimizer, int dtype, const OptimTensor* tensors, int count) {
+    char msg[160];
+    if (count < 0 || count > optimizer_list_capacity() || (count > 0 && tensors == nullptr))
+        snprintf(msg, sizeof(msg), "%s: %d tensors (at most %d per call)", what, count, optimizer_list_capacity());
+    else if (optimizer < 0 || optimizer > 5 || dtype < 0 || dtype > 2)
+        snprintf(msg, sizeof(msg), "%s: unknown optimizer id %d or dtype id %d", what, optimizer, dtype);
+    else
+        return true;
+    set_last_error_msg(msg);
+    return false;
+}
+
+int cbnb_b200_optimizer_update_32bit_multi(int optimizer, int dtype, const OptimTensor* tensors, int count, float beta1,
+                                           float beta2, float beta3, float alpha, float eps, float weight_decay,
+                                           float lr, float gnorm_scale, bool skip_zeros, cudaStream_t stream) {
+    if (!optimizer_list_ok("optimizer_update_32bit_multi", optimizer, dtype, tensors, count)) return 100;
+    launch_optimizer32bit_list(optimizer, dtype, tensors, count, beta1, beta2, beta3, alpha, eps, weight_decay, lr,
+                               gnorm_scale, skip_zeros, stream);
+    return 0;
+}
+
+int cbnb_b200_optimizer_update_8bit_blockwise_multi(int optimizer, int dtype, const OptimTensor* tensors, int count,
+                                                    float beta1, float beta2, float beta3, float alpha, float eps,
+                                                    float weight_decay, float lr, const float* quantiles1,
+                                                    const float* quantiles2, float gnorm_scale, bool skip_zeros,
+                                                    cudaStream_t stream) {
+    if (!optimizer_list_ok("optimizer_update_8bit_blockwise_multi", optimizer, dtype, tensors, count)) return 100;
+    launch_optimizer8bit_blockwise_list(optimizer, dtype, tensors, count, beta1, beta2, beta3, alpha, eps,
+                                        weight_decay, lr, quantiles1, quantiles2, gnorm_scale, skip_zeros, stream);
+    return 0;
 }
 
 #define BNB200_C32(name, id, ctype, suffix, dt)                                                                        \

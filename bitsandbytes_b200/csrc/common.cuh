@@ -213,4 +213,19 @@ void set_last_error_msg(const char* msg);
 
 int device_sm_count();
 
+// ---------------------------------------------------------------- optimizer tensor lists (optim.cu, c_api.cu)
+// One tensor of a multi-tensor optimizer step: the layout of bnb_b200_optim_tensor_t in include/bitsandbytes_b200.h.
+struct OptimTensor {
+    void* p;
+    const void* g;
+    void* state1;
+    void* state2;     // NULL for one-state optimizers
+    float* absmax1;   // 8-bit state only
+    float* absmax2;
+    long long n;      // elements of p
+    int step;         // this tensor's own step (1 on its first update)
+    int reserved;
+};
+static_assert(sizeof(OptimTensor) == 64, "bnb_b200_optim_tensor_t is 64 bytes");
+
 } // namespace bnb200

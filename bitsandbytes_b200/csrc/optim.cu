@@ -12,7 +12,7 @@
 // about the tensor cores: a warp owns one 256-element block (lane l handles the 8 consecutive elements 8 l .. 8 l + 7
 // through 8- and 16-byte accesses: every load and store of the warp is one contiguous segment), the block's absmax is a warp-shuffle reduction (no shared-memory
 // round trip, no __syncthreads in the loop), the two code books sit in shared memory once per CTA, and the grid is
-// persistent (a multiple of the SM count).  The 32-bit kernels are plain grid-stride loops.
+// persistent (a multiple of the SM count).  The 32-bit kernel hands a CTA a 4096-element chunk at a time.
 //
 // Numerics follow the reference operation by operation, including what looks accidental there, because a state
 // written by one implementation must be readable by the other:
@@ -41,6 +41,46 @@ __device__ __forceinline__ float sgnf(float v) { return (float)((0.0f < v) - (v 
 
 template <typename T> __device__ __forceinline__ T round_to(float v) { return DT<T>::from_f32(v); }
 template <typename T> __device__ __forceinline__ float widen(T v) { return DT<T>::to_f32(v); }
+
+// ---------------------------------------------------------------------------------------------------------------
+// Tensor lists
+// ---------------------------------------------------------------------------------------------------------------
+// Every update kernel takes a list of tensors by value, as a __grid_constant__ kernel parameter (CUDA >= 12.1 allows
+// 32764 bytes of parameters on sm_70+): a single-tensor call is a list of one, a multi-tensor call updates up to
+// kOptimListCap tensors in one launch, with no staging buffer to upload or keep alive.  The work items of the launch
+// -- 256-element blocks (8-bit state) or kOpt32Chunk-element chunks (32-bit state) -- are numbered across the list:
+// start[i] items come before tensor i, start[count] is the total, and a warp (8-bit) or CTA (32-bit) finds the tensor
+// of its item by binary search.  Everything but the tensor's pointers, size and step is per launch.
+constexpr int kKernelParamBytes = 32764;
+constexpr int kScalarParamBytes = 128;  // the other kernel parameters (checked below)
+constexpr int kOptimListCap = (kKernelParamBytes - kScalarParamBytes - 16) / (sizeof(OptimTensor) + sizeof(long long));
+
+struct OptimList {
+    long long start[kOptimListCap + 1];
+    OptimTensor t[kOptimListCap];
+    int count;
+};
+static_assert(sizeof(OptimList) + kScalarParamBytes <= kKernelParamBytes, "kernel parameters exceed 32764 bytes");
+
+// the per-launch scalars
+struct OptimScalars {
+    float beta1, beta2, beta3, alpha, eps, weight_decay, lr, gnorm_scale;
+    bool skip_zeros;
+};
+static_assert(sizeof(OptimScalars) + 4 * sizeof(void*) + 2 * sizeof(float) <= kScalarParamBytes, "");
+
+// the tensor of work item `item`: the last i >= lo with start[i] <= item (tensors without items are skipped)
+__device__ __forceinline__ int find_tensor(const OptimList& L, long long item, int lo) {
+    int hi = L.count - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (L.start[mid] <= item)
+            lo = mid;
+        else
+            hi = mid - 1;
+    }
+    return lo;
+}
 
 // ---------------------------------------------------------------------------------------------------------------
 // 32-bit state
@@ -165,63 +205,83 @@ template <> struct Vec4<float> { using type = float4; };
 template <> struct Vec4<__half> { using type = uint2; };
 template <> struct Vec4<__nv_bfloat16> { using type = uint2; };
 
-// VEC: four consecutive elements per thread and iteration through 8- / 16-byte accesses (every pointer 16-byte
-// aligned; the host checks), the last n % 4 elements by the first threads of CTA 0; otherwise one element per access.
-template <typename T, int OPT, bool VEC>
-__global__ void __launch_bounds__(512) optim32_kernel(const T* g, T* p, float* s1, float* s2, const float* unorm,
-                                                      float max_unorm, float param_norm, float beta1, float beta2,
-                                                      float beta3, float alpha, float eps, float weight_decay, int step,
-                                                      float lr, float gnorm_scale, bool skip_zeros, long n) {
+constexpr int kOpt32Chunk = 4096;  // elements per work item of the 32-bit kernel: two passes of a 512-thread CTA
+
+// A CTA per chunk of kOpt32Chunk elements of one tensor.  16-bit parameters whose pointers are all aligned (and, for
+// AdEMAMix, whose size is a multiple of 4: s1 + n + i is 16-byte aligned only then): four consecutive elements per
+// thread and iteration through 8- / 16-byte accesses -- there the rounding to T hides how the compiler contracts an
+// fma, and the vector path is bit-identical to the scalar one (and to the reference); fp32 already moves 128 bytes
+// per warp access.  Otherwise one element per access.  The choice is made per tensor, so a misaligned view in the list
+// does not demote the others.  max_unorm > 0 (LAMB / LARS) takes a list of one: unorm and param_norm belong to it.
+template <typename T, int OPT>
+__global__ void __launch_bounds__(512) optim32_kernel(const __grid_constant__ OptimList list, const OptimScalars s,
+                                                      const float* unorm, float max_unorm, float param_norm) {
     constexpr bool two = OPT == kAdam || OPT == kAdemamix;
     Opt32Args q;
-    q.beta1 = beta1, q.beta2 = beta2, q.beta3 = beta3, q.alpha = alpha, q.eps = eps, q.weight_decay = weight_decay;
-    q.lr = lr, q.gnorm_scale = gnorm_scale, q.step = step, q.skip_zeros = skip_zeros;
-    q.correction1 = 1.0f - powf(beta1, step);
-    q.correction2 = sqrtf(1.0f - powf(beta2, step));
-    q.step_size = -lr * q.correction2 / q.correction1;
+    q.beta1 = s.beta1, q.beta2 = s.beta2, q.beta3 = s.beta3, q.alpha = s.alpha, q.eps = s.eps;
+    q.weight_decay = s.weight_decay, q.lr = s.lr, q.gnorm_scale = s.gnorm_scale, q.skip_zeros = s.skip_zeros;
     q.update_scale = 1.0f;
     if (max_unorm > 0.0f) {
         const float us = sqrtf(unorm[0]);
-        const float cap = two ? max_unorm * param_norm : max_unorm * param_norm + eps;
+        const float cap = two ? max_unorm * param_norm : max_unorm * param_norm + s.eps;
         q.update_scale = us > cap ? cap / us : 1.0f;
     }
-    auto one = [&](long i) {
-        T pt = p[i];
-        float a = s1[i], b = two ? s2[i] : 0.f, c = OPT == kAdemamix ? s1[n + i] : 0.f;
-        opt32_element<T, OPT>(q, g[i], pt, a, b, c);
-        p[i] = pt;
-        s1[i] = a;
-        if (two) s2[i] = b;
-        if (OPT == kAdemamix) s1[n + i] = c;
-    };
-    const long tid = (long)blockIdx.x * blockDim.x + threadIdx.x, nthreads = (long)gridDim.x * blockDim.x;
-    if (!VEC) {
-        for (long i = tid; i < n; i += nthreads) one(i);
-        return;
-    }
-    using V = typename Vec4<T>::type;
-    const long n4 = n >> 2;
-    for (long v = tid; v < n4; v += nthreads) {
-        const long i = v << 2;
-        V gv4 = *reinterpret_cast<const V*>(g + i);
-        V pv4 = *reinterpret_cast<const V*>(p + i);
-        float4 a4 = *reinterpret_cast<const float4*>(s1 + i);
-        float4 b4 = two ? *reinterpret_cast<const float4*>(s2 + i) : make_float4(0.f, 0.f, 0.f, 0.f);
-        // (AdEMAMix: s1 + n + i is 16-byte aligned only when n % 4 == 0: the host sends other sizes down the scalar path)
-        float4 c4 = OPT == kAdemamix ? *reinterpret_cast<const float4*>(s1 + n + i) : make_float4(0.f, 0.f, 0.f, 0.f);
-        T* gt = reinterpret_cast<T*>(&gv4);
-        T* pt = reinterpret_cast<T*>(&pv4);
-        float* a = reinterpret_cast<float*>(&a4);
-        float* b = reinterpret_cast<float*>(&b4);
-        float* c = reinterpret_cast<float*>(&c4);
+    const long long total = list.start[list.count];
+    int ti = 0;
+    for (long long item = blockIdx.x; item < total; item += gridDim.x) {
+        ti = find_tensor(list, item, ti);
+        const OptimTensor& d = list.t[ti];
+        const T* g = static_cast<const T*>(d.g);
+        T* p = static_cast<T*>(d.p);
+        float* s1 = static_cast<float*>(d.state1);
+        float* s2 = static_cast<float*>(d.state2);
+        const long n = d.n;
+        q.step = d.step;
+        q.correction1 = 1.0f - powf(q.beta1, q.step);
+        q.correction2 = sqrtf(1.0f - powf(q.beta2, q.step));
+        q.step_size = -q.lr * q.correction2 / q.correction1;
+        const long c0 = (item - list.start[ti]) * kOpt32Chunk;
+        const long c1 = c0 + kOpt32Chunk < n ? c0 + kOpt32Chunk : n;
+        auto one = [&](long i) {
+            T pt = p[i];
+            float a = s1[i], b = two ? s2[i] : 0.f, c = OPT == kAdemamix ? s1[n + i] : 0.f;
+            opt32_element<T, OPT>(q, g[i], pt, a, b, c);
+            p[i] = pt;
+            s1[i] = a;
+            if (two) s2[i] = b;
+            if (OPT == kAdemamix) s1[n + i] = c;
+        };
+        auto al = [](const void* v, uintptr_t m) { return (reinterpret_cast<uintptr_t>(v) & m) == 0; };
+        const bool vec = sizeof(T) == 2 && al(g, sizeof(T) * 4 - 1) && al(p, sizeof(T) * 4 - 1) && al(s1, 15) &&
+                         al(s2, 15) && (OPT != kAdemamix || (n & 3) == 0);
+        if (vec) {
+            using V = typename Vec4<T>::type;
+            for (long i = c0 + 4 * threadIdx.x; i < c1; i += 4 * blockDim.x) {
+                if (i + 4 > n) {  // the last n % 4 elements
+                    for (long j = i; j < n; ++j) one(j);
+                    break;
+                }
+                V gv4 = *reinterpret_cast<const V*>(g + i);
+                V pv4 = *reinterpret_cast<const V*>(p + i);
+                float4 a4 = *reinterpret_cast<const float4*>(s1 + i);
+                float4 b4 = two ? *reinterpret_cast<const float4*>(s2 + i) : make_float4(0.f, 0.f, 0.f, 0.f);
+                float4 c4 = OPT == kAdemamix ? *reinterpret_cast<const float4*>(s1 + n + i) : make_float4(0.f, 0.f, 0.f, 0.f);
+                T* gt = reinterpret_cast<T*>(&gv4);
+                T* pt = reinterpret_cast<T*>(&pv4);
+                float* a = reinterpret_cast<float*>(&a4);
+                float* b = reinterpret_cast<float*>(&b4);
+                float* c = reinterpret_cast<float*>(&c4);
 #pragma unroll
-        for (int k = 0; k < 4; ++k) opt32_element<T, OPT>(q, gt[k], pt[k], a[k], b[k], c[k]);
-        *reinterpret_cast<V*>(p + i) = pv4;
-        *reinterpret_cast<float4*>(s1 + i) = a4;
-        if (two) *reinterpret_cast<float4*>(s2 + i) = b4;
-        if (OPT == kAdemamix) *reinterpret_cast<float4*>(s1 + n + i) = c4;
+                for (int k = 0; k < 4; ++k) opt32_element<T, OPT>(q, gt[k], pt[k], a[k], b[k], c[k]);
+                *reinterpret_cast<V*>(p + i) = pv4;
+                *reinterpret_cast<float4*>(s1 + i) = a4;
+                if (two) *reinterpret_cast<float4*>(s2 + i) = b4;
+                if (OPT == kAdemamix) *reinterpret_cast<float4*>(s1 + n + i) = c4;
+            }
+        } else {
+            for (long i = c0 + threadIdx.x; i < c1; i += blockDim.x) one(i);
+        }
     }
-    if (tid < (n & 3)) one((n4 << 2) + tid);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -304,13 +364,45 @@ __device__ __forceinline__ void store8c(unsigned char* dst, long i0, long n, boo
     }
 }
 
+// A warp per work item, i.e. per (tensor, 256-element block) of the list, and the fields of the item's tensor.  Kept
+// in registers across items these would cost registers (and occupancy) that kernel parameters do not: a warp reads
+// them from the parameter space for every item.  ONE: a list of one tensor (the single-tensor entries); the tensor
+// index is then the constant 0, so the fields and the per-step values are loop invariants, as in a kernel that takes
+// one tensor's pointers as its parameters.
+template <typename T> struct Tensor8 {
+    T* p;
+    const T* g;
+    unsigned char* state1;
+    unsigned char* state2;  // (NULL for one-state optimizers)
+    float* absmax1;
+    float* absmax2;
+    long n;
+    long long first;  // the list's number of its block 0
+    int step;
+    bool aligned;     // 16-byte p / g and 8-byte state accesses allowed
+
+    __device__ __forceinline__ void load(const OptimList& L, int i) {
+        const OptimTensor& d = L.t[i];
+        p = static_cast<T*>(d.p);
+        g = static_cast<const T*>(d.g);
+        state1 = static_cast<unsigned char*>(d.state1);
+        state2 = static_cast<unsigned char*>(d.state2);
+        absmax1 = d.absmax1;
+        absmax2 = d.absmax2;
+        n = d.n;
+        first = L.start[i];
+        step = d.step;
+        aligned = ((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g)) & 15) == 0 &&
+                  ((reinterpret_cast<uintptr_t>(state1) | reinterpret_cast<uintptr_t>(state2)) & 7) == 0;
+    }
+};
+
 // reference csrc/kernels.cu:914-1150
-template <typename T, int OPT>
-__global__ void __launch_bounds__(256) optim8_2state_kernel(T* p, const T* g, unsigned char* state1, unsigned char* state2,
-                                                            float beta1, float beta2, float beta3, float alpha, float eps,
-                                                            int step, float lr, const float* qmap1, const float* qmap2,
-                                                            float* absmax1, float* absmax2, float weight_decay,
-                                                            float gnorm_scale, bool skip_zeros, long n) {
+template <typename T, int OPT, bool ONE>
+__global__ void __launch_bounds__(256) optim8_2state_kernel(const __grid_constant__ OptimList list, const OptimScalars s,
+                                                            const float* qmap1, const float* qmap2) {
+    const float beta1 = s.beta1, beta2 = s.beta2, beta3 = s.beta3, alpha = s.alpha, eps = s.eps, lr = s.lr;
+    const float weight_decay = s.weight_decay, gnorm_scale = s.gnorm_scale;
     __shared__ float code1[256];
     __shared__ float code2[256];
     __shared__ float2 fin1[257], fin2[257];
@@ -324,16 +416,26 @@ __global__ void __launch_bounds__(256) optim8_2state_kernel(T* p, const T* g, un
     build_q8_final(code2, fin2);
     __syncthreads();
     const CodeBook cb1{code1, fin1, br1}, cb2{code2, fin2, br2};
-    const bool aligned = ((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g)) & 15) == 0 &&
-                         ((reinterpret_cast<uintptr_t>(state1) | reinterpret_cast<uintptr_t>(state2)) & 7) == 0;
-    (void)skip_zeros;  // (the reference's 2-state kernel ignores it too)
-    const float correction1 = 1.0f - __powf(beta1, step);
-    const float correction2 = sqrtf(1.0f - __powf(beta2, step));
-    const float step_size = __fdividef(-lr * correction2, correction1);
+    // (s.skip_zeros: the reference's 2-state kernel ignores it too)
     const int lane = threadIdx.x & 31;
-    const long n_blocks = (n + kOptBlock - 1) / kOptBlock;
-    const long warps = (long)gridDim.x * (blockDim.x >> 5);
-    for (long blk = (long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); blk < n_blocks; blk += warps) {
+    const long long total = list.start[list.count];
+    const long long warps = (long long)gridDim.x * (blockDim.x >> 5);
+    int ti = 0;
+    for (long long item = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); item < total; item += warps) {
+        ti = ONE ? 0 : find_tensor(list, item, ti);
+        Tensor8<T> t;
+        t.load(list, ti);
+        const float correction1 = 1.0f - __powf(beta1, t.step);
+        const float correction2 = sqrtf(1.0f - __powf(beta2, t.step));
+        const float step_size = __fdividef(-lr * correction2, correction1);
+        T* p = t.p;
+        const T* g = t.g;
+        unsigned char* state1 = t.state1;
+        unsigned char* state2 = t.state2;
+        float* absmax1 = t.absmax1;
+        float* absmax2 = t.absmax2;
+        const long n = t.n, blk = (long)(item - t.first);
+        const bool aligned = t.aligned;
         const long base = blk * kOptBlock;
         const float am1 = absmax1[blk], am2 = absmax2[blk];
         const float am3 = OPT == kAdemamix ? absmax1[(n + base) / kOptBlock] : 0.f;
@@ -404,11 +506,12 @@ __global__ void __launch_bounds__(256) optim8_2state_kernel(T* p, const T* g, un
 }
 
 // reference csrc/kernels.cu:1152-1325
-template <typename T, int OPT>
-__global__ void __launch_bounds__(256) optim8_1state_kernel(T* p, const T* g, unsigned char* state1, float beta1,
-                                                            float beta2, float eps, int step, float lr,
-                                                            const float* qmap1, float* absmax1, float weight_decay,
-                                                            float gnorm_scale, bool skip_zeros, long n) {
+template <typename T, int OPT, bool ONE>
+__global__ void __launch_bounds__(256) optim8_1state_kernel(const __grid_constant__ OptimList list, const OptimScalars s,
+                                                            const float* qmap1) {
+    const float beta1 = s.beta1, beta2 = s.beta2, eps = s.eps, lr = s.lr, weight_decay = s.weight_decay;
+    const float gnorm_scale = s.gnorm_scale;
+    const bool skip_zeros = s.skip_zeros;
     __shared__ float code1[256];
     __shared__ float2 fin1[257];
     __shared__ uint32_t br1[kQ8Cells];
@@ -418,12 +521,21 @@ __global__ void __launch_bounds__(256) optim8_1state_kernel(T* p, const T* g, un
     build_q8_final(code1, fin1);
     __syncthreads();
     const CodeBook cb1{code1, fin1, br1};
-    const bool aligned = ((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g)) & 15) == 0 &&
-                         (reinterpret_cast<uintptr_t>(state1) & 7) == 0;
     const int lane = threadIdx.x & 31;
-    const long n_blocks = (n + kOptBlock - 1) / kOptBlock;
-    const long warps = (long)gridDim.x * (blockDim.x >> 5);
-    for (long blk = (long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); blk < n_blocks; blk += warps) {
+    const long long total = list.start[list.count];
+    const long long warps = (long long)gridDim.x * (blockDim.x >> 5);
+    int ti = 0;
+    for (long long item = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); item < total; item += warps) {
+        ti = ONE ? 0 : find_tensor(list, item, ti);
+        Tensor8<T> t;
+        t.load(list, ti);
+        T* p = t.p;
+        const T* g = t.g;
+        unsigned char* state1 = t.state1;
+        float* absmax1 = t.absmax1;
+        const long n = t.n, blk = (long)(item - t.first);
+        const int step = t.step;
+        const bool aligned = t.aligned;
         const long base = blk * kOptBlock;
         const float am1 = absmax1[blk];
         const long i0 = base + lane * 8;
@@ -502,63 +614,74 @@ int grid_for(long work_items, int per_cta) {
     return ctas < 1 ? 1 : (int)ctas;
 }
 
+// the list of a launch: the tensors and the work-item prefix counts; returns the number of work items
+long long make_list(OptimList& L, const OptimTensor* ts, int count, long long per_item) {
+    long long total = 0;
+    for (int i = 0; i < count; ++i) {
+        L.t[i] = ts[i];
+        L.start[i] = total;
+        total += ts[i].n > 0 ? (ts[i].n + per_item - 1) / per_item : 0;
+    }
+    L.start[count] = total;
+    L.count = count;
+    return total;
+}
+
+// count <= kOptimListCap; unorm / max_unorm / param_norm: the LAMB / LARS trust ratio of a list of one (max_unorm = 0
+// otherwise)
 template <typename T, int OPT>
-void run32(const T* g, T* p, float* s1, float* s2, float* unorm, float max_unorm, float param_norm, float beta1,
-           float beta2, float beta3, float alpha, float eps, float weight_decay, int step, float lr, float gnorm_scale,
-           bool skip_zeros, long n, cudaStream_t stream) {
-    if (n <= 0) return;
-    const int grid = grid_for(n, 512 * 4 * 2);
+void run32(const OptimTensor* ts, int count, const OptimScalars& s, float* unorm, float max_unorm, float param_norm,
+           cudaStream_t stream) {
+    OptimList L;
+    const long long chunks = make_list(L, ts, count, kOpt32Chunk);
+    if (chunks == 0) return;
+    const int grid = grid_for(chunks, 1);
     const bool trust = max_unorm > 0.0f && OPT != kAdemamix;
+    const T* g = static_cast<const T*>(ts[0].g);
+    const float* s1 = static_cast<const float*>(ts[0].state1);
+    const float* s2 = static_cast<const float*>(ts[0].state2);
     // Lion: the parameter update comes first, the norm of the NEW state feeds the next step (reference ops.cu:124-137)
     if (trust && OPT != kLion) {
         cudaMemsetAsync(unorm, 0, sizeof(float), stream);
-        optim32_unorm_kernel<T, OPT><<<grid, 512, 0, stream>>>(g, s1, s2, unorm, beta1, beta2, eps, step, gnorm_scale, n);
+        optim32_unorm_kernel<T, OPT><<<grid, 512, 0, stream>>>(g, s1, s2, unorm, s.beta1, s.beta2, s.eps, ts[0].step,
+                                                               s.gnorm_scale, ts[0].n);
     }
-    auto al = [](const void* q, uintptr_t m) { return q == nullptr || (reinterpret_cast<uintptr_t>(q) & m) == 0; };
-    // 16-bit parameters only: there the rounding to T hides how the compiler contracts an fma, and the vector kernel is
-    // bit-identical to the scalar one (and to the reference); fp32 already moves 128 bytes per warp access
-    const bool vec = sizeof(T) == 2 && al(g, sizeof(T) * 4 - 1) && al(p, sizeof(T) * 4 - 1) && al(s1, 15) && al(s2, 15) &&
-                     (OPT != kAdemamix || (n & 3) == 0);
-    if (vec)
-        optim32_kernel<T, OPT, true><<<grid, 512, 0, stream>>>(g, p, s1, s2, unorm, max_unorm, param_norm, beta1, beta2,
-                                                               beta3, alpha, eps, weight_decay, step, lr, gnorm_scale,
-                                                               skip_zeros, n);
-    else
-        optim32_kernel<T, OPT, false><<<grid, 512, 0, stream>>>(g, p, s1, s2, unorm, max_unorm, param_norm, beta1, beta2,
-                                                                beta3, alpha, eps, weight_decay, step, lr, gnorm_scale,
-                                                                skip_zeros, n);
+    optim32_kernel<T, OPT><<<grid, 512, 0, stream>>>(L, s, unorm, max_unorm, param_norm);
     if (trust && OPT == kLion) {
         cudaMemsetAsync(unorm, 0, sizeof(float), stream);
-        optim32_unorm_kernel<T, OPT><<<grid, 512, 0, stream>>>(g, s1, s2, unorm, beta1, beta2, eps, step, gnorm_scale, n);
+        optim32_unorm_kernel<T, OPT><<<grid, 512, 0, stream>>>(g, s1, s2, unorm, s.beta1, s.beta2, s.eps, ts[0].step,
+                                                               s.gnorm_scale, ts[0].n);
     }
     BNB200_CHECK_LAUNCH("optimizer32bit");
 }
 
 template <typename T, int OPT>
-void run8(T* p, const T* g, unsigned char* state1, unsigned char* state2, float beta1, float beta2, float beta3,
-          float alpha, float eps, int step, float lr, const float* qmap1, const float* qmap2, float* absmax1,
-          float* absmax2, float weight_decay, float gnorm_scale, bool skip_zeros, long n, cudaStream_t stream) {
-    if (n <= 0) return;
-    const long n_blocks = (n + kOptBlock - 1) / kOptBlock;
+void run8(const OptimTensor* ts, int count, const OptimScalars& s, const float* qmap1, const float* qmap2,
+          cudaStream_t stream) {
+    OptimList L;
+    const long long n_blocks = make_list(L, ts, count, kOptBlock);
+    if (n_blocks == 0) return;
     const int grid = grid_for(n_blocks, 8);
-    if (OPT == kAdam || OPT == kAdemamix)
-        optim8_2state_kernel<T, OPT><<<grid, 256, 0, stream>>>(p, g, state1, state2, beta1, beta2, beta3, alpha, eps, step,
-                                                               lr, qmap1, qmap2, absmax1, absmax2, weight_decay,
-                                                               gnorm_scale, skip_zeros, n);
-    else
-        optim8_1state_kernel<T, OPT><<<grid, 256, 0, stream>>>(p, g, state1, beta1, beta2, eps, step, lr, qmap1, absmax1,
-                                                               weight_decay, gnorm_scale, skip_zeros, n);
+    if constexpr (OPT == kAdam || OPT == kAdemamix) {
+        if (count == 1)
+            optim8_2state_kernel<T, OPT, true><<<grid, 256, 0, stream>>>(L, s, qmap1, qmap2);
+        else
+            optim8_2state_kernel<T, OPT, false><<<grid, 256, 0, stream>>>(L, s, qmap1, qmap2);
+    } else {
+        if (count == 1)
+            optim8_1state_kernel<T, OPT, true><<<grid, 256, 0, stream>>>(L, s, qmap1);
+        else
+            optim8_1state_kernel<T, OPT, false><<<grid, 256, 0, stream>>>(L, s, qmap1);
+    }
     BNB200_CHECK_LAUNCH("optimizer8bit_blockwise");
 }
 
 template <typename T>
-bool dispatch32(int opt, const T* g, T* p, float* s1, float* s2, float* unorm, float max_unorm, float param_norm,
-                float beta1, float beta2, float beta3, float alpha, float eps, float wd, int step, float lr,
-                float gnorm_scale, bool skip_zeros, long n, cudaStream_t st) {
+bool dispatch32(int opt, const OptimTensor* ts, int count, const OptimScalars& s, float* unorm, float max_unorm,
+                float param_norm, cudaStream_t st) {
 #define BNB200_O32(ID)                                                                                                 \
     case ID:                                                                                                           \
-        run32<T, ID>(g, p, s1, s2, unorm, max_unorm, param_norm, beta1, beta2, beta3, alpha, eps, wd, step, lr,        \
-                     gnorm_scale, skip_zeros, n, st);                                                                  \
+        run32<T, ID>(ts, count, s, unorm, max_unorm, param_norm, st);                                                  \
         return true;
     switch (opt) {
         BNB200_O32(kAdam)
@@ -573,13 +696,11 @@ bool dispatch32(int opt, const T* g, T* p, float* s1, float* s2, float* unorm, f
 }
 
 template <typename T>
-bool dispatch8(int opt, T* p, const T* g, unsigned char* s1, unsigned char* s2, float beta1, float beta2, float beta3,
-               float alpha, float eps, int step, float lr, const float* q1, const float* q2, float* a1, float* a2,
-               float wd, float gnorm_scale, bool skip_zeros, long n, cudaStream_t st) {
+bool dispatch8(int opt, const OptimTensor* ts, int count, const OptimScalars& s, const float* q1, const float* q2,
+               cudaStream_t st) {
 #define BNB200_O8(ID)                                                                                                  \
     case ID:                                                                                                           \
-        run8<T, ID>(p, g, s1, s2, beta1, beta2, beta3, alpha, eps, step, lr, q1, q2, a1, a2, wd, gnorm_scale,          \
-                    skip_zeros, n, st);                                                                                \
+        run8<T, ID>(ts, count, s, q1, q2, st);                                                                         \
         return true;
     switch (opt) {
         BNB200_O8(kAdam)
@@ -593,44 +714,66 @@ bool dispatch8(int opt, T* p, const T* g, unsigned char* s1, unsigned char* s2, 
     return false;
 }
 
+bool list32(int opt, int dtype, const OptimTensor* ts, int count, const OptimScalars& s, float* unorm, float max_unorm,
+            float param_norm, cudaStream_t st) {
+    switch (dtype) {
+    case 0: return dispatch32<float>(opt, ts, count, s, unorm, max_unorm, param_norm, st);
+    case 1: return dispatch32<__half>(opt, ts, count, s, unorm, max_unorm, param_norm, st);
+    case 2: return dispatch32<__nv_bfloat16>(opt, ts, count, s, unorm, max_unorm, param_norm, st);
+    }
+    return false;
+}
+
+bool list8(int opt, int dtype, const OptimTensor* ts, int count, const OptimScalars& s, const float* q1, const float* q2,
+           cudaStream_t st) {
+    switch (dtype) {
+    case 0: return dispatch8<float>(opt, ts, count, s, q1, q2, st);
+    case 1: return dispatch8<__half>(opt, ts, count, s, q1, q2, st);
+    case 2: return dispatch8<__nv_bfloat16>(opt, ts, count, s, q1, q2, st);
+    }
+    return false;
+}
+
+OptimTensor one_tensor(void* p, const void* g, void* s1, void* s2, float* a1, float* a2, long n, int step) {
+    return OptimTensor{p, g, s1, s2, a1, a2, (long long)n, step, 0};
+}
+
 } // namespace
+
+int optimizer_list_capacity() { return kOptimListCap; }
 
 // dtype: 0 = fp32, 1 = fp16, 2 = bf16 (the library's convention)
 bool launch_optimizer32bit(int opt, int dtype, const void* g, void* p, float* s1, float* s2, float* unorm,
                            float max_unorm, float param_norm, float beta1, float beta2, float beta3, float alpha,
                            float eps, float wd, int step, float lr, float gnorm_scale, bool skip_zeros, long n,
                            cudaStream_t st) {
-    switch (dtype) {
-    case 0:
-        return dispatch32<float>(opt, (const float*)g, (float*)p, s1, s2, unorm, max_unorm, param_norm, beta1, beta2,
-                                 beta3, alpha, eps, wd, step, lr, gnorm_scale, skip_zeros, n, st);
-    case 1:
-        return dispatch32<__half>(opt, (const __half*)g, (__half*)p, s1, s2, unorm, max_unorm, param_norm, beta1, beta2,
-                                  beta3, alpha, eps, wd, step, lr, gnorm_scale, skip_zeros, n, st);
-    case 2:
-        return dispatch32<__nv_bfloat16>(opt, (const __nv_bfloat16*)g, (__nv_bfloat16*)p, s1, s2, unorm, max_unorm,
-                                         param_norm, beta1, beta2, beta3, alpha, eps, wd, step, lr, gnorm_scale,
-                                         skip_zeros, n, st);
-    }
-    return false;
+    const OptimTensor t = one_tensor(p, g, s1, s2, nullptr, nullptr, n, step);
+    const OptimScalars s{beta1, beta2, beta3, alpha, eps, wd, lr, gnorm_scale, skip_zeros};
+    return list32(opt, dtype, &t, 1, s, unorm, max_unorm, param_norm, st);
 }
 
 bool launch_optimizer8bit_blockwise(int opt, int dtype, void* p, const void* g, unsigned char* s1, unsigned char* s2,
                                     float beta1, float beta2, float beta3, float alpha, float eps, int step, float lr,
                                     const float* q1, const float* q2, float* a1, float* a2, float wd,
                                     float gnorm_scale, bool skip_zeros, long n, cudaStream_t st) {
-    switch (dtype) {
-    case 0:
-        return dispatch8<float>(opt, (float*)p, (const float*)g, s1, s2, beta1, beta2, beta3, alpha, eps, step, lr, q1,
-                                q2, a1, a2, wd, gnorm_scale, skip_zeros, n, st);
-    case 1:
-        return dispatch8<__half>(opt, (__half*)p, (const __half*)g, s1, s2, beta1, beta2, beta3, alpha, eps, step, lr, q1,
-                                 q2, a1, a2, wd, gnorm_scale, skip_zeros, n, st);
-    case 2:
-        return dispatch8<__nv_bfloat16>(opt, (__nv_bfloat16*)p, (const __nv_bfloat16*)g, s1, s2, beta1, beta2, beta3,
-                                        alpha, eps, step, lr, q1, q2, a1, a2, wd, gnorm_scale, skip_zeros, n, st);
-    }
-    return false;
+    const OptimTensor t = one_tensor(p, g, s1, s2, a1, a2, n, step);
+    const OptimScalars s{beta1, beta2, beta3, alpha, eps, wd, lr, gnorm_scale, skip_zeros};
+    return list8(opt, dtype, &t, 1, s, q1, q2, st);
+}
+
+// count <= optimizer_list_capacity(): one launch
+bool launch_optimizer32bit_list(int opt, int dtype, const OptimTensor* ts, int count, float beta1, float beta2,
+                                float beta3, float alpha, float eps, float wd, float lr, float gnorm_scale,
+                                bool skip_zeros, cudaStream_t st) {
+    const OptimScalars s{beta1, beta2, beta3, alpha, eps, wd, lr, gnorm_scale, skip_zeros};
+    return list32(opt, dtype, ts, count, s, nullptr, 0.0f, 0.0f, st);
+}
+
+bool launch_optimizer8bit_blockwise_list(int opt, int dtype, const OptimTensor* ts, int count, float beta1, float beta2,
+                                         float beta3, float alpha, float eps, float wd, float lr, const float* q1,
+                                         const float* q2, float gnorm_scale, bool skip_zeros, cudaStream_t st) {
+    const OptimScalars s{beta1, beta2, beta3, alpha, eps, wd, lr, gnorm_scale, skip_zeros};
+    return list8(opt, dtype, ts, count, s, q1, q2, st);
 }
 
 } // namespace bnb200

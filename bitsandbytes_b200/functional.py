@@ -14,7 +14,7 @@ from __future__ import annotations
 
 import ctypes as ct
 import itertools
-from typing import Any, Optional
+from typing import Any, Optional, Sequence
 
 import torch
 from torch import Tensor
@@ -508,6 +508,35 @@ def optimizer_update_8bit_blockwise(optimizer_name: str, g: Tensor, p: Tensor, s
     is_on_gpu_or_paged([p, g, state1, state2, qmap1, qmap2, absmax1, absmax2])
     _ops_ns.optimizer_update_8bit_blockwise(optimizer_name, g, p, state1, state2, beta1, beta2, beta3, alpha, eps, step, lr,
                                             qmap1, qmap2, absmax1, absmax2, weight_decay, gnorm_scale, skip_zeros)
+
+
+def optimizer_update_32bit_multi(optimizer_name: str, g: Sequence[Tensor], p: Sequence[Tensor], state1: Sequence[Tensor],
+                                 beta1: float, eps: float, step: Sequence[int], lr: float,
+                                 state2: Optional[Sequence[Tensor]] = None, beta2: float = 0.0, beta3: float = 0.0,
+                                 alpha: float = 0.0, weight_decay: float = 0.0, gnorm_scale: float = 1.0,
+                                 skip_zeros=False) -> None:
+    """``optimizer_update_32bit`` for several parameters at once: one kernel launch per
+    ``backends.cuda.optimizer_multi_capacity()`` parameters instead of one per parameter, with the same results bit
+    for bit.  g, p, state1, step (and state2 for adam / ademamix) list one entry per parameter; every other argument is
+    shared.  All tensors on one GPU (paged state allowed); no trust ratio (max_unorm: LAMB / LARS take the
+    single-tensor call)."""
+    _cuda_backend.optimizer_update_32bit_multi(optimizer_name, g, p, state1, state2, beta1, beta2, beta3, alpha, eps,
+                                               weight_decay, step, lr, gnorm_scale, skip_zeros)
+
+
+def optimizer_update_8bit_blockwise_multi(optimizer_name: str, g: Sequence[Tensor], p: Sequence[Tensor],
+                                          state1: Sequence[Tensor], state2: Optional[Sequence[Tensor]], beta1: float,
+                                          beta2: float, beta3: float, alpha: float, eps: float, step: Sequence[int],
+                                          lr: float, qmap1: Tensor, qmap2: Optional[Tensor], absmax1: Sequence[Tensor],
+                                          absmax2: Optional[Sequence[Tensor]], weight_decay: float = 0.0,
+                                          gnorm_scale: float = 1.0, skip_zeros=False) -> None:
+    """``optimizer_update_8bit_blockwise`` for several parameters at once: one kernel launch per
+    ``backends.cuda.optimizer_multi_capacity()`` parameters instead of one per parameter, with the same results bit
+    for bit.  g, p, state1, absmax1, step (and state2 / absmax2 for adam / ademamix) list one entry per parameter; the
+    code books and every other argument are shared."""
+    _cuda_backend.optimizer_update_8bit_blockwise_multi(optimizer_name, g, p, state1, state2, beta1, beta2, beta3, alpha,
+                                                        eps, step, lr, qmap1, qmap2, absmax1, absmax2, weight_decay,
+                                                        gnorm_scale, skip_zeros)
 
 
 class GlobalPageManager:

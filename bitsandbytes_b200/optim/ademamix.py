@@ -7,7 +7,7 @@ from typing import Optional
 import torch
 
 from .. import functional as F
-from .optimizer import Optimizer2State
+from .optimizer import Optimizer2State, _Update
 
 
 def _schedules(step, beta1, beta3, alpha, t_alpha, t_beta3):
@@ -84,21 +84,13 @@ class AdEMAMix(Optimizer2State):
         state["state1"] = self._get_state_double_buffer(p, dtype=dtype)
         state["state2"] = self.get_state_buffer(p, dtype=dtype)
 
-    @torch.no_grad()
-    def update_step(self, group, p, gindex, pindex):
+    def _update_args(self, group, p, gindex, pindex) -> _Update:
+        u = super()._update_args(group, p, gindex, pindex)
         config = self.get_config(gindex, pindex, group)
-        if not config["t_alpha"] and not config["t_beta3"]:
-            super().update_step(group, p, gindex, pindex)
-            return
-        p.data = p.data.contiguous()
-        p.grad = p.grad.contiguous()
-        state = self.state[p]
-        state["step"] += 1
-        step = state["step"]
-        beta1, beta2, beta3 = config["betas"]
-        alpha, t_alpha, t_beta3 = config["alpha"], config["t_alpha"], config["t_beta3"]
-        alpha_t, beta3_t = _schedules(step, beta1, beta3, alpha, t_alpha, t_beta3)
-        self._launch(state, p, config, beta1, beta2, beta3_t, alpha_t)
+        if config["t_alpha"] or config["t_beta3"]:  # the warm-up schedules: scalars of this parameter's step
+            u.alpha, u.beta3 = _schedules(u.state["step"], u.beta1, u.beta3, config["alpha"], config["t_alpha"],
+                                          config["t_beta3"])
+        return u
 
     def _get_state_double_buffer(self, p, dtype=torch.float32):
         if not self.is_paged or p.numel() < 1e5:

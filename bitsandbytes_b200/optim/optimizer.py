@@ -4,8 +4,10 @@ API mirror of the reference's ``bitsandbytes/optim/optimizer.py`` (GlobalOptimMa
 :117-401, Optimizer2State :403-590, Optimizer1State :593-756): same constructor arguments, state-dict keys
 (``state1``, ``state2``, ``qmap1``, ``qmap2``, ``absmax1``, ``absmax2``, ``unorm_vec``, ``step``), per-parameter
 overrides and the ``min_8bit_size`` rule, so that a checkpoint written by either implementation loads in the
-other.  The update itself is one native launch per parameter (``functional.optimizer_update_32bit`` /
-``optimizer_update_8bit_blockwise``, kernels in ``csrc/optim.cu``).
+other.  Unlike the reference, ``step()`` updates all parameters that share their launch arguments in one native call
+(``functional.optimizer_update_32bit_multi`` / ``optimizer_update_8bit_blockwise_multi``, kernels in
+``csrc/optim.cu``), with the results of one call per parameter bit for bit; ``update_step`` still updates one
+parameter.
 """
 from __future__ import annotations
 
@@ -25,6 +27,40 @@ class MockArgs:
     def __init__(self, initial_data):
         for key, value in initial_data.items():
             setattr(self, key, value)
+
+
+class _Update:
+    """One parameter's launch arguments: what ``update_step`` computes (advancing ``state["step"]``) before it launches."""
+
+    __slots__ = ("name", "p", "state", "beta1", "beta2", "beta3", "alpha", "eps", "weight_decay", "lr", "skip_zeros",
+                 "max_unorm")
+
+    def __init__(self, name, p, state, config, beta1, beta2, beta3, alpha):
+        self.name, self.p, self.state = name, p, state
+        self.beta1, self.beta2, self.beta3, self.alpha = beta1, beta2, beta3, alpha
+        self.eps, self.weight_decay, self.lr = config["eps"], config["weight_decay"], config["lr"]
+        self.skip_zeros, self.max_unorm = config["skip_zeros"], config["max_unorm"]
+
+    def per_parameter(self) -> bool:
+        """32-bit state with a trust ratio (LAMB / LARS) needs the parameter's norm and a norm pre-pass: one launch each."""
+        return self.max_unorm > 0.0 and self.state["state1"].dtype == torch.float32
+
+    def group_key(self):
+        """Parameters with equal keys share every per-launch argument of the multi-tensor call."""
+        st = self.state
+        eight = st["state1"].dtype == torch.uint8
+        return (self.p.device, self.p.dtype, eight, self.name, self.beta1, self.beta2, self.beta3, self.alpha, self.eps,
+                self.weight_decay, self.lr, self.skip_zeros,
+                id(st["qmap1"]) if eight else None, id(st.get("qmap2")) if eight else None)
+
+
+def group_updates(updates):
+    """The multi-tensor calls of one step: the updates grouped by launch arguments, in order of first appearance.  (A
+    group longer than a launch's descriptor capacity is split by the backend.)"""
+    groups = {}
+    for u in updates:
+        groups.setdefault(u.group_key(), []).append(u)
+    return list(groups.values())
 
 
 class GlobalOptimManager:
@@ -156,6 +192,18 @@ class Optimizer8bit(torch.optim.Optimizer):
             return new_group
 
         self.__setstate__({"state": state, "param_groups": [update_group(g, ng) for g, ng in zip(groups, saved_groups)]})
+        self._share_qmaps()
+
+    def _share_qmaps(self):
+        """A loaded state holds its own copy of the code books in every parameter: point the copies equal to this
+        optimizer's code books back at them, so that the parameters share one multi-tensor call again."""
+        for st in self.state.values():
+            for key, name in (("qmap1", "dynamic"), ("qmap2", "udynamic")):
+                q = st.get(key)
+                if isinstance(q, torch.Tensor) and q.is_cuda:
+                    shared = self._qmap(name, q.device)
+                    if q is not shared and torch.equal(q, shared):
+                        st[key] = shared
 
     def to_gpu(self):
         for group in self.param_groups:
@@ -187,7 +235,9 @@ class Optimizer8bit(torch.optim.Optimizer):
             self.check_overrides()
             self.to_gpu()
             self.initialized = True
+        multi = self._steps_in_groups()
         last = None
+        updates = []
         for gindex, group in enumerate(self.param_groups):
             for pindex, p in enumerate(group["params"]):
                 if p.grad is None:
@@ -195,11 +245,24 @@ class Optimizer8bit(torch.optim.Optimizer):
                 if len(self.state[p]) == 0:
                     self.init_state(group, p, gindex, pindex)
                 self.prefetch_state(p)
-                self.update_step(group, p, gindex, pindex)
+                if not multi:
+                    self.update_step(group, p, gindex, pindex)
+                else:
+                    u = self._update_args(group, p, gindex, pindex)
+                    if u.per_parameter():
+                        self._launch(u)
+                    else:
+                        updates.append(u)
                 last = p
+        for batch in group_updates(updates):
+            self._launch_multi(batch)
         if self.is_paged and last is not None:
             torch.cuda.synchronize(last.device)  # managed memory: the host may read the state right after step()
         return loss
+
+    def _steps_in_groups(self) -> bool:
+        """A subclass that replaces update_step outside this package keeps one update_step call per parameter."""
+        return type(self).update_step.__module__.split(".")[0] == __name__.split(".")[0]
 
     def get_config(self, gindex, pindex, group):
         config = {"betas": group["betas"], "eps": group["eps"], "weight_decay": group["weight_decay"], "lr": group["lr"],
@@ -216,8 +279,54 @@ class Optimizer8bit(torch.optim.Optimizer):
     def init_state(self, group, p, gindex, pindex):
         raise NotImplementedError("init_state method needs to be overridden")
 
+    @torch.no_grad()
     def update_step(self, group, p, gindex, pindex):
+        """Update one parameter: compute its launch arguments (advancing its step) and launch them."""
+        self._launch(self._update_args(group, p, gindex, pindex))
+
+    def _update_args(self, group, p, gindex, pindex) -> _Update:
         raise NotImplementedError("The update_step method needs to be overridden")
+
+    def _make_update(self, group, p, gindex, pindex):
+        """Common part of _update_args: contiguous parameter and gradient, the config, the step advanced."""
+        if not p.is_contiguous():
+            p.data = p.data.contiguous()
+        if not p.grad.is_contiguous():
+            p.grad = p.grad.contiguous()
+        state = self.state[p]
+        state["step"] += 1
+        return state, self.get_config(gindex, pindex, group)
+
+    def _launch(self, u: _Update):
+        st = u.state
+        if st["state1"].dtype == torch.float32:
+            F.optimizer_update_32bit(u.name, u.p.grad, u.p, st["state1"], u.beta1, u.eps, st["step"], u.lr, st.get("state2"),
+                                     u.beta2, u.beta3, u.alpha, u.weight_decay, 1.0,
+                                     st["unorm_vec"] if u.max_unorm > 0.0 else None, max_unorm=u.max_unorm,
+                                     skip_zeros=u.skip_zeros)
+        else:
+            F.optimizer_update_8bit_blockwise(u.name, u.p.grad, u.p, st["state1"], st.get("state2"), u.beta1, u.beta2,
+                                              u.beta3, u.alpha, u.eps, st["step"], u.lr, st["qmap1"], st.get("qmap2"),
+                                              st["absmax1"], st.get("absmax2"), u.weight_decay, gnorm_scale=1.0,
+                                              skip_zeros=u.skip_zeros)
+
+    def _launch_multi(self, batch):
+        """One multi-tensor call for updates with equal group keys."""
+        u, st = batch[0], batch[0].state
+        g = [b.p.grad for b in batch]
+        p = [b.p for b in batch]
+        s1 = [b.state["state1"] for b in batch]
+        s2 = [b.state["state2"] for b in batch] if "state2" in st else None
+        steps = [b.state["step"] for b in batch]
+        if st["state1"].dtype == torch.float32:
+            F.optimizer_update_32bit_multi(u.name, g, p, s1, u.beta1, u.eps, steps, u.lr, s2, u.beta2, u.beta3, u.alpha,
+                                           u.weight_decay, 1.0, skip_zeros=u.skip_zeros)
+        else:
+            a1 = [b.state["absmax1"] for b in batch]
+            a2 = [b.state["absmax2"] for b in batch] if s2 is not None else None
+            F.optimizer_update_8bit_blockwise_multi(u.name, g, p, s1, s2, u.beta1, u.beta2, u.beta3, u.alpha, u.eps, steps,
+                                                    u.lr, st["qmap1"], st.get("qmap2"), a1, a2, u.weight_decay,
+                                                    gnorm_scale=1.0, skip_zeros=u.skip_zeros)
 
     def get_state_buffer(self, p, dtype=torch.float32):
         if p.device.type != "cuda":
@@ -308,28 +417,11 @@ class Optimizer2State(Optimizer8bit):
         if config["max_unorm"] > 0.0:
             state["unorm_vec"] = torch.zeros((1,), device=p.device)
 
-    @torch.no_grad()
-    def update_step(self, group, p, gindex, pindex):
-        p.data = p.data.contiguous()
-        p.grad = p.grad.contiguous()
-        state = self.state[p]
-        config = self.get_config(gindex, pindex, group)
-        state["step"] += 1
+    def _update_args(self, group, p, gindex, pindex) -> _Update:
+        state, config = self._make_update(group, p, gindex, pindex)
         betas = config["betas"]
         beta3 = betas[2] if len(betas) >= 3 else 0.0
-        self._launch(state, p, config, betas[0], betas[1], beta3, config.get("alpha", 0.0))
-
-    def _launch(self, state, p, config, beta1, beta2, beta3, alpha):
-        if state["state1"].dtype == torch.float32:
-            F.optimizer_update_32bit(self.optimizer_name, p.grad, p, state["state1"], beta1, config["eps"], state["step"],
-                                     config["lr"], state["state2"], beta2, beta3, alpha, config["weight_decay"], 1.0,
-                                     state["unorm_vec"] if config["max_unorm"] > 0.0 else None,
-                                     max_unorm=config["max_unorm"], skip_zeros=config["skip_zeros"])
-        else:
-            F.optimizer_update_8bit_blockwise(self.optimizer_name, p.grad, p, state["state1"], state["state2"], beta1, beta2,
-                                              beta3, alpha, config["eps"], state["step"], config["lr"], state["qmap1"],
-                                              state["qmap2"], state["absmax1"], state["absmax2"], config["weight_decay"],
-                                              gnorm_scale=1.0, skip_zeros=config["skip_zeros"])
+        return _Update(self.optimizer_name, p, state, config, betas[0], betas[1], beta3, config.get("alpha", 0.0))
 
 
 class Optimizer1State(Optimizer8bit):
@@ -356,21 +448,6 @@ class Optimizer1State(Optimizer8bit):
         if config["max_unorm"] > 0.0:
             state["unorm_vec"] = torch.zeros((1,), device=p.device)
 
-    @torch.no_grad()
-    def update_step(self, group, p, gindex, pindex):
-        p.data = p.data.contiguous()
-        p.grad = p.grad.contiguous()
-        state = self.state[p]
-        config = self.get_config(gindex, pindex, group)
-        state["step"] += 1
-        beta1, beta2 = config["betas"][0], config["betas"][1]
-        if state["state1"].dtype == torch.float32:
-            F.optimizer_update_32bit(self.optimizer_name, p.grad, p, state["state1"], beta1, config["eps"], state["step"],
-                                     config["lr"], None, beta2, 0.0, 0.0, config["weight_decay"], 1.0,
-                                     state["unorm_vec"] if config["max_unorm"] > 0.0 else None,
-                                     max_unorm=config["max_unorm"], skip_zeros=config["skip_zeros"])
-        else:
-            F.optimizer_update_8bit_blockwise(self.optimizer_name, p.grad, p, state["state1"], None, beta1, beta2, 0.0, 0.0,
-                                              config["eps"], state["step"], config["lr"], state["qmap1"], None,
-                                              state["absmax1"], None, config["weight_decay"], gnorm_scale=1.0,
-                                              skip_zeros=config["skip_zeros"])
+    def _update_args(self, group, p, gindex, pindex) -> _Update:
+        state, config = self._make_update(group, p, gindex, pindex)
+        return _Update(self.optimizer_name, p, state, config, config["betas"][0], config["betas"][1], 0.0, 0.0)

@@ -241,6 +241,26 @@ void cadam_8bit_blockwise_grad_fp32(float* p, float* g, unsigned char* state1, u
  * 2 rmsprop, 3 adagrad, 4 lion, 5 ademamix) and dtype id (0 fp32, 1 fp16, 2 bf16).  Return 0, or 100 for an unknown id. */
 int cbnb_b200_optimizer_update_32bit(int optimizer, int dtype, const void* g, void* p, float* state1, float* state2, float* unorm, float max_unorm, float param_norm, float beta1, float beta2, float beta3, float alpha, float eps, float weight_decay, int step, float lr, float gnorm_scale, bool skip_zeros, long long n, bnb_stream_t stream);
 int cbnb_b200_optimizer_update_8bit_blockwise(int optimizer, int dtype, void* p, const void* g, unsigned char* state1, unsigned char* state2, float beta1, float beta2, float beta3, float alpha, float eps, int step, float lr, const float* quantiles1, const float* quantiles2, float* absmax1, float* absmax2, float weight_decay, float gnorm_scale, bool skip_zeros, long long n, bnb_stream_t stream);
+/* Multi-tensor steps: one kernel launch updates `count` tensors that share the optimizer, the dtype, every scalar and
+ * (8-bit) the code books; each tensor brings its pointers, element count and its own step.  The results are those of
+ * one single-tensor call per tensor, bit for bit.  state1 / state2 are float (32-bit) or unsigned char (8-bit) arrays;
+ * state2 and absmax2 are NULL for one-state optimizers; absmax1 / absmax2 are unused by the 32-bit call.  count may
+ * be 0 and at most cbnb_b200_optimizer_multi_capacity(); the 32-bit call has no trust ratio (max_unorm = 0).  Return 0,
+ * or 100 with cbnb_b200_last_error_message() set. */
+typedef struct bnb_b200_optim_tensor {
+    void* p;
+    const void* g;
+    void* state1;
+    void* state2;
+    float* absmax1;
+    float* absmax2;
+    long long n;
+    int step;
+    int reserved; /* 0 */
+} bnb_b200_optim_tensor_t;
+int cbnb_b200_optimizer_multi_capacity(void);
+int cbnb_b200_optimizer_update_32bit_multi(int optimizer, int dtype, const bnb_b200_optim_tensor_t* tensors, int count, float beta1, float beta2, float beta3, float alpha, float eps, float weight_decay, float lr, float gnorm_scale, bool skip_zeros, bnb_stream_t stream);
+int cbnb_b200_optimizer_update_8bit_blockwise_multi(int optimizer, int dtype, const bnb_b200_optim_tensor_t* tensors, int count, float beta1, float beta2, float beta3, float alpha, float eps, float weight_decay, float lr, const float* quantiles1, const float* quantiles2, float gnorm_scale, bool skip_zeros, bnb_stream_t stream);
 
 #ifdef __cplusplus
 }
