@@ -57,6 +57,7 @@ def _signatures():
     # (code, A, absmax, out, blocksize, n, quant_type, dtype, stream)
     sig["cbnb_b200_quantize_blockwise"] = ([_VOIDP] * 4 + [_I32] * 4 + [_VOIDP], None)
     sig["cbnb_b200_gemm_4bit_path"] = ([_I32] * 5, _I32)
+    sig["cbnb_b200_gemm_4bit_staged_route"] = ([_I32] * 5, _I32)
     sig["cbnb_b200_gemm_4bit_force_path"] = ([_I32], None)
     # (A, B, absmax, absmax_8bit, absmax_code, absmax_offset, out, bias, M, N, K, ldc, blocksize, quant_type, dtype, stream)
     # dtype for the 4-bit GEMM entries: 0 fp32, 1 fp16, 2 bf16, 3 fp32 with TF32 allowed
@@ -65,6 +66,13 @@ def _signatures():
     #  mt, force_splits, trace, stream) -> int
     sig["cbnb_b200_gemm_4bit_pair"] = ([_VOIDP] * 8 + [_I32] * 9 + [_VOIDP, _VOIDP], _I32)
     sig["cbnb_b200_gemm_4bit_multi_out"] = ([_VOIDP] * 7 + [_I32] + [_VOIDP] + [_I32] * 7 + [_VOIDP], _I32)
+    # (A, B, absmax, absmax_8bit, absmax_code, absmax_offset, outs, n_outs, bias, M, N, K, ldc, blocksize, quant_type,
+    #  dtype, mt, panel_rows, stream) -> int
+    sig["cbnb_b200_gemm_4bit_staged"] = ([_VOIDP] * 7 + [_I32] + [_VOIDP] + [_I32] * 9 + [_VOIDP], _I32)
+    # (B, absmax, absmax_8bit, absmax_code, absmax_offset, out, blocksize, quant_type, dtype, n0, rows, K, stream) -> int
+    sig["cbnb_b200_dequantize_4bit_panel"] = ([_VOIDP] * 6 + [_I32] * 6 + [_VOIDP], _I32)
+    # (A, W, out, bias, M, N, K, ldc, dtype, mt, stream) -> int
+    sig["cbnb_b200_gemm_decoded"] = ([_VOIDP] * 4 + [_I32] * 6 + [_VOIDP], _I32)
     # (CA, CB, SCA, SCB, bias, out, M, N, K, dtype, stream) -> int
     sig["cbnb_b200_int8_scaled_mm"] = ([_VOIDP] * 6 + [_I32] * 4 + [_VOIDP], _I32)
     # (CA, CB, SCA, SCB, bias, subA, subBT, jpad, out, M, N, K, dtype, stream) -> int

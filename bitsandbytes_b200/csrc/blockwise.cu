@@ -564,12 +564,19 @@ __global__ void __launch_bounds__(kDqThreads)
 //     coalesced 512-byte warp stores;
 //   * grid = a multiple of the SM count, several CTAs per SM: each thread has 32 B of codes + its scale in
 //     flight, i.e. > 32 KB of reads per SM, which covers the HBM latency-bandwidth product.
+// It also decodes a panel of weight rows for the staged 4-bit GEMM (gemm4_tc.cu): the scales come through
+// ScaleSrc::load_as<DQ>, the fetch of the fused GEMM (nested statistics included), and `e0` is the element index of
+// A[0] in the whole weight, so that scale indices count from the weight's start -- a panel may begin inside a
+// quantisation block.  e0 is a multiple of 64: a 64-element unit never straddles a block of >= 64 elements.
 constexpr int kD4Warps = 8;
 
-template <typename T, int QT>
+template <typename T, int QT, bool DQ>
 __global__ void __launch_bounds__(kD4Warps * 32, 4)
-    dequantize4_prmt_kernel(const uint8_t* __restrict__ A, const float* __restrict__ absmax, T* __restrict__ out,
-                            int log2_bs, long long n_units /* 64-element units */) {
+    dequantize4_prmt_kernel(const uint8_t* __restrict__ A, const float* __restrict__ absmax,
+                            const uint8_t* __restrict__ absmax_8bit, const float* __restrict__ absmax_code,
+                            const float* __restrict__ absmax_offset, T* __restrict__ out, int log2_bs,
+                            long long n_units /* 64-element units */, long long e0) {
+    const ScaleSrc sc{absmax, absmax_8bit, absmax_code, (DQ && absmax_offset) ? __ldg(absmax_offset) : 0.f};
     __shared__ __align__(128) uint8_t stage[kD4Warps][4096];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const bool two = log2_bs == 5;
@@ -583,8 +590,8 @@ __global__ void __launch_bounds__(kD4Warps * 32, 4)
             // default caching: the two halves of a 32-byte sector are fetched by consecutive instructions
             q0 = __ldg(reinterpret_cast<const uint4*>(A + u * 32));
             q1 = __ldg(reinterpret_cast<const uint4*>(A + u * 32 + 16));
-            s0 = __ldg(absmax + ((u * 64) >> log2_bs));
-            if (two) s1 = __ldg(absmax + ((u * 64 + 32) >> log2_bs));
+            s0 = sc.load_as<DQ>((e0 + u * 64) >> log2_bs);
+            if (two) s1 = sc.load_as<DQ>((e0 + u * 64 + 32) >> log2_bs);
         }
         uint32_t r[32];
         DecodeTable tab;
@@ -650,7 +657,8 @@ void launch_dequantize_blockwise(const float* code, const uint8_t* A, const floa
             const long long n_units = n / 64;
             const long long want = (n_units + kD4Warps * 32 - 1) / (kD4Warps * 32);
             const int grid = (int)(want < (long long)sms * 4 ? want : (long long)sms * 4);  // 4 resident CTAs per SM
-            dequantize4_prmt_kernel<T, QT><<<grid, kD4Warps * 32, 0, stream>>>(A, absmax, out, ilog2_pow2(blocksize), n_units);
+            dequantize4_prmt_kernel<T, QT, false><<<grid, kD4Warps * 32, 0, stream>>>(
+                A, absmax, nullptr, nullptr, nullptr, out, ilog2_pow2(blocksize), n_units, 0);
             BNB200_CHECK_LAUNCH("dequantize4_prmt");
             n_vec = 0;
             const long long first4 = n_units * 64;
@@ -678,6 +686,38 @@ void launch_dequantize_blockwise(const float* code, const uint8_t* A, const floa
         BNB200_CHECK_LAUNCH("dequantize_blockwise_generic");
     }
 }
+
+// Rows [n0, n0 + rows) of a [N, K] 4-bit weight (K a multiple of 64, codes 16-byte aligned) decoded to T into
+// out[rows, K], bit-identical to the same rows of F.dequantize_4bit.  absmax_8bit != NULL: nested statistics.
+template <typename T>
+void launch_dequantize4_panel(const uint8_t* codes, const float* absmax, const uint8_t* absmax_8bit,
+                              const float* absmax_code, const float* absmax_offset, T* out, int blocksize,
+                              int quant_type, int n0, int rows, int K, cudaStream_t stream) {
+    const long long e0 = (long long)n0 * K;
+    const long long n_units = (long long)rows * K / 64;
+    const long long want = (n_units + kD4Warps * 32 - 1) / (kD4Warps * 32);
+    const int sms = device_sm_count();
+    const int grid = (int)(want < (long long)sms * 4 ? want : (long long)sms * 4);
+    const uint8_t* A = codes + e0 / 2;
+    const int lbs = ilog2_pow2(blocksize);
+#define BNB200_PANEL(QT, DQ)                                                                                           \
+    dequantize4_prmt_kernel<T, QT, DQ><<<grid, kD4Warps * 32, 0, stream>>>(A, absmax, absmax_8bit, absmax_code,       \
+                                                                            absmax_offset, out, lbs, n_units, e0)
+    if (absmax_8bit != nullptr) {
+        if (quant_type == kNF4) BNB200_PANEL(kNF4, true);
+        else BNB200_PANEL(kFP4, true);
+    } else {
+        if (quant_type == kNF4) BNB200_PANEL(kNF4, false);
+        else BNB200_PANEL(kFP4, false);
+    }
+#undef BNB200_PANEL
+    BNB200_CHECK_LAUNCH("dequantize4_panel");
+}
+template void launch_dequantize4_panel<__half>(const uint8_t*, const float*, const uint8_t*, const float*,
+                                               const float*, __half*, int, int, int, int, int, cudaStream_t);
+template void launch_dequantize4_panel<__nv_bfloat16>(const uint8_t*, const float*, const uint8_t*, const float*,
+                                                      const float*, __nv_bfloat16*, int, int, int, int, int,
+                                                      cudaStream_t);
 
 #define INSTANTIATE(T)                                                                                                 \
     template void launch_quantize_blockwise<T, kGeneral8bit>(const float*, const T*, float*, uint8_t*, int, long long, \

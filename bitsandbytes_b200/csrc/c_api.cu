@@ -53,6 +53,20 @@ bool launch_gemm4_tc(const T* A, const uint8_t* B, const float* absmax, const ui
                      const float* absmax_code, const float* absmax_offset, T* out, const T* bias, int M, int N, int K,
                      int ldc, int blocksize, int quant_type, cudaStream_t stream, void* const* peers = nullptr,
                      int n_peers = 0, int mt_override = 0, int force_splits = 0);
+template <typename T>
+bool launch_gemm4_staged(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
+                         const float* absmax_code, const float* absmax_offset, T* out, const T* bias, int M, int N,
+                         int K, int ldc, int blocksize, int quant_type, cudaStream_t stream, void* const* peers,
+                         int n_peers, int mt_override, int panel_rows);
+template <typename T>
+bool launch_gemm_decoded(const T* A, const T* W, T* out, const T* bias, int M, int N, int K, int ldc, int mt,
+                         cudaStream_t stream);
+template <typename T>
+void launch_dequantize4_panel(const uint8_t* codes, const float* absmax, const uint8_t* absmax_8bit,
+                              const float* absmax_code, const float* absmax_offset, T* out, int blocksize,
+                              int quant_type, int n0, int rows, int K, cudaStream_t stream);
+int staged_max_panel_rows(int K, int elem_bytes);
+int staged_plan(int M, int N, int K, int sms, int* panel_rows);
 void launch_int8_vector_quant(const void* A, int8_t* out, float* rowStats, int* col_flags, float threshold, int rows,
                               int cols, int dtype, cudaStream_t stream);
 void launch_dequant_mm_int32_fp16(const int* A, const float* rowStats, const float* colStats, __half* out,
@@ -157,6 +171,7 @@ bool encode_tmap_2d(CUtensorMap* out, const void* base, int elem_bytes, int swiz
 
 // ---------------------------------------------------------------- 4-bit GEMM dispatch
 // path: 0 = CUDA-core GEMV, 1 = wgmma GEMM, 2 = CUDA-core generic, 3 = mma.sync decode kernel (M <= 8)
+// Path 1 has two forms: the fused kernel, and at large M the staged route (staged_route() below).
 // dtype: 0 = fp32, 1 = fp16, 2 = bf16, 3 = fp32 with TF32 allowed (the caller's fp32 matmul precision is "tf32")
 static int simt_max_m() {
     static int v = -2;
@@ -181,6 +196,12 @@ static int mma_max_m() {
 // dtype 3: fp32 activations take the TF32 instance of the wgmma GEMM from this many tokens on: the measured crossover
 // against the CUDA-core kernel on an H100 (DESIGN.md section 7)
 constexpr int kTf32MinM = 4;
+
+// the staged route from this many tokens on (fp16 / bf16): the fused kernel decodes every weight once per 256-token tile, the
+// staged route once per call.  The measured crossover on an H100 (tools/time_gemm4_staged.py, DESIGN.md section 7):
+// at 1024 tokens the route still loses on the 11008 x 4096 weight, from 2048 on it wins where its panels take no
+// more waves of 256-token tiles than the fused kernel's grid.
+constexpr int kStagedMinM = 2048;
 
 static bool tc_shape_ok(int M, int N, int K, int blocksize, int dtype) {
     (void)M;
@@ -209,6 +230,20 @@ static int choose_path(int M, int N, int K, int blocksize, int dtype) {
     return 1;
 }
 
+// Whether an unforced path-1 call with 16-bit activations takes the staged route (decode every weight panel once,
+// then the wgmma GEMM on shared-memory operands) instead of the fused kernel: from kStagedMinM tokens, where the
+// 256-token tiles fill every SM (the route never splits K) and its panels (each a launch of its own) take no more
+// waves than the fused kernel's persistent grid.  A forced path 1 keeps the fused kernel.
+static bool staged_route(int M, int N, int K, int blocksize, int dtype) {
+    if (t_forced_path >= 0 || (dtype != 1 && dtype != 2) || M < kStagedMinM) return false;
+    if (choose_path(M, N, K, blocksize, dtype) != 1) return false;
+    const int sms = device_sm_count();
+    const long long tiles = (long long)((M + 255) / 256) * ((N + 127) / 128);
+    int panel = 0;
+    const int staged_waves = staged_plan(M, N, K, sms, &panel);
+    return staged_waves > 0 && tiles >= sms && staged_waves <= (tiles + sms - 1) / sms;
+}
+
 template <typename T>
 static void gemm_4bit_dispatch(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
                                const float* absmax_code, const float* absmax_offset, T* out, const T* bias, int M,
@@ -219,6 +254,13 @@ static void gemm_4bit_dispatch(const T* A, const uint8_t* B, const float* absmax
         return;
     }
     const int path = choose_path(M, N, K, blocksize, dtype);
+    if (path == 1 && staged_route(M, N, K, blocksize, dtype)) {
+        if constexpr (!std::is_same<T, float>::value) {
+            if (launch_gemm4_staged<T>(A, B, absmax, absmax_8bit, absmax_code, absmax_offset, out, bias, M, N, K, ldc,
+                                       blocksize, quant_type, stream, nullptr, 0, 0, 0))
+                return;
+        }
+    }
     if (path == 3) {
         if constexpr (!std::is_same<T, float>::value) {
             if (launch_gemv4_mma<T>(A, B, absmax, absmax_8bit, absmax_code, absmax_offset, out, bias, M, N, K, ldc,
@@ -362,6 +404,18 @@ int cbnb_b200_gemm_4bit_multi_out(const void* A, const uint8_t* B, const float* 
     }
     if (M <= 0 || N <= 0) return 0;
     if (!tc_shape_ok(M, N, K, blocksize, dtype)) return 100;
+    // the route the plain call takes for this shape, so that every destination holds the same bits
+    if (staged_route(M, N, K, blocksize, dtype)) {
+        if (dtype == 1 && launch_gemm4_staged<__half>((const __half*)A, B, absmax, absmax_8bit, absmax_code,
+                                                      absmax_offset, (__half*)outs[0], (const __half*)bias, M, N, K,
+                                                      ldc, blocksize, quant_type, stream, outs + 1, n_outs - 1, 0, 0))
+            return 0;
+        if (dtype == 2 && launch_gemm4_staged<__nv_bfloat16>((const __nv_bfloat16*)A, B, absmax, absmax_8bit,
+                                                             absmax_code, absmax_offset, (__nv_bfloat16*)outs[0],
+                                                             (const __nv_bfloat16*)bias, M, N, K, ldc, blocksize,
+                                                             quant_type, stream, outs + 1, n_outs - 1, 0, 0))
+            return 0;
+    }
     bool ok = false;
     if (dtype == 1)
         ok = launch_gemm4_tc<__half>((const __half*)A, B, absmax, absmax_8bit, absmax_code, absmax_offset,
@@ -400,8 +454,68 @@ int cbnb_b200_gemm_4bit_pair(const void* A, const uint8_t* B, const float* absma
     return ok ? 0 : 100;
 }
 
+// Developer / test entry: the staged route with a chosen token tile (mt = 128 | 256, 0 = by the shape) and
+// panel (panel_rows: a multiple of 128 whose decoded rows fit the 32 MB workspace, 0 = the largest that does), every
+// element stored to outs[0..n_outs) as in cbnb_b200_gemm_4bit_multi_out.  dtype 1 or 2.  Returns 0, or 100 when the
+// route does not serve the shape or the options.
+int cbnb_b200_gemm_4bit_staged(const void* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
+                               const float* absmax_code, const float* absmax_offset, void* const* outs, int n_outs,
+                               const void* bias, int M, int N, int K, int ldc, int blocksize, int quant_type, int dtype,
+                               int mt, int panel_rows, cudaStream_t stream) {
+    if (n_outs < 1 || n_outs > 8 || outs == nullptr) return 100;
+    if (M <= 0 || N <= 0) return 0;
+    bool ok = false;
+    if (dtype == 1)
+        ok = launch_gemm4_staged<__half>((const __half*)A, B, absmax, absmax_8bit, absmax_code, absmax_offset,
+                                         (__half*)outs[0], (const __half*)bias, M, N, K, ldc, blocksize, quant_type,
+                                         stream, outs + 1, n_outs - 1, mt, panel_rows);
+    else if (dtype == 2)
+        ok = launch_gemm4_staged<__nv_bfloat16>((const __nv_bfloat16*)A, B, absmax, absmax_8bit, absmax_code,
+                                                absmax_offset, (__nv_bfloat16*)outs[0], (const __nv_bfloat16*)bias, M,
+                                                N, K, ldc, blocksize, quant_type, stream, outs + 1, n_outs - 1, mt,
+                                                panel_rows);
+    return ok ? 0 : 100;
+}
+
+// The staged route's two phases on their own, for tests and timing: rows [n0, n0 + rows) of a [N, K] 4-bit weight
+// decoded into out[rows, K] (returns 100 unless K % 64 == 0, n0 % 128 == 0, blocksize a power of two >= 32 and the
+// codes 16-byte aligned), and the staged GEMM on such a decoded weight W[N, K] (mt = 128 | 256).
+int cbnb_b200_dequantize_4bit_panel(const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
+                                    const float* absmax_code, const float* absmax_offset, void* out, int blocksize,
+                                    int quant_type, int dtype, int n0, int rows, int K, cudaStream_t stream) {
+    if (rows <= 0) return 0;
+    if (K < 64 || (K % 64) != 0 || n0 < 0 || (n0 % 128) != 0 || blocksize < 32 || (blocksize & (blocksize - 1)) != 0 ||
+        (quant_type != kNF4 && quant_type != kFP4) || (reinterpret_cast<uintptr_t>(B) & 15) != 0)
+        return 100;
+    if (dtype == 1)
+        launch_dequantize4_panel<__half>(B, absmax, absmax_8bit, absmax_code, absmax_offset, (__half*)out, blocksize,
+                                         quant_type, n0, rows, K, stream);
+    else if (dtype == 2)
+        launch_dequantize4_panel<__nv_bfloat16>(B, absmax, absmax_8bit, absmax_code, absmax_offset,
+                                                (__nv_bfloat16*)out, blocksize, quant_type, n0, rows, K, stream);
+    else
+        return 100;
+    return 0;
+}
+
+int cbnb_b200_gemm_decoded(const void* A, const void* W, void* out, const void* bias, int M, int N, int K, int ldc,
+                           int dtype, int mt, cudaStream_t stream) {
+    bool ok = false;
+    if (dtype == 1)
+        ok = launch_gemm_decoded<__half>((const __half*)A, (const __half*)W, (__half*)out, (const __half*)bias, M, N, K,
+                                         ldc, mt, stream);
+    else if (dtype == 2)
+        ok = launch_gemm_decoded<__nv_bfloat16>((const __nv_bfloat16*)A, (const __nv_bfloat16*)W, (__nv_bfloat16*)out,
+                                                (const __nv_bfloat16*)bias, M, N, K, ldc, mt, stream);
+    return ok ? 0 : 100;
+}
+
 int cbnb_b200_gemm_4bit_path(int M, int N, int K, int blocksize, int dtype) {
     return choose_path(M, N, K, blocksize, dtype);
+}
+
+int cbnb_b200_gemm_4bit_staged_route(int M, int N, int K, int blocksize, int dtype) {
+    return staged_route(M, N, K, blocksize, dtype) ? 1 : 0;
 }
 
 void cbnb_b200_gemm_4bit_force_path(int path) { t_forced_path = path; }
@@ -545,7 +659,7 @@ int cbnb_b200_last_error(void) {
 const char* cbnb_b200_last_error_message(void) { return g_err_msg; }
 
 const char* cbnb_b200_build_info(void) {
-    return "bitsandbytes_b200: sm_90a; wgmma f16/bf16 (A from registers) + s8; TMA 128B-swizzle; CUDA " BNB200_STR(
+    return "bitsandbytes_b200: sm_90a; wgmma f16/bf16 (A from registers or shared memory) + s8; TMA 128B-swizzle; CUDA " BNB200_STR(
         __CUDACC_VER_MAJOR__) "." BNB200_STR(__CUDACC_VER_MINOR__);
 }
 

@@ -39,6 +39,10 @@
 // T = float is the TF32 instance (fp32 activations when the caller allows TF32): wgmma k8 steps on TF32 operands,
 // weights rna_tf32(fp32 dequantised weight) decoded by decode_word_tf32, 64-deep stages of fp32 activations, MT <= 128,
 // an fp32 epilogue that adds the bias and rounds nothing.
+//
+// QT = kDecoded is the staged instance of the large-M route (launch_gemm4_staged, below): the weights arrive already
+// decoded, as a [N, K] panel that the producer loads like the activations, and both wgmma operands come from shared
+// memory.
 #include "common.cuh"
 #include "decode4.cuh"
 #include "hopper_ptx.cuh"
@@ -48,6 +52,12 @@
 #include <type_traits>
 
 namespace bnb200 {
+
+// blockwise.cu: rows [n0, n0 + rows) of a 4-bit weight decoded to T, bit-identical to F.dequantize_4bit
+template <typename T>
+void launch_dequantize4_panel(const uint8_t* codes, const float* absmax, const uint8_t* absmax_8bit,
+                              const float* absmax_code, const float* absmax_offset, T* out, int blocksize,
+                              int quant_type, int n0, int rows, int K, cudaStream_t stream);
 
 namespace {
 
@@ -59,6 +69,8 @@ constexpr int kProducerRegs = 40;
 constexpr int kConsumerRegs = 232;
 static_assert(128 * kProducerRegs + kConsumers * kConsumerRegs <= 65536, "register hand-off exceeds the SM");
 constexpr int kBarEpi = 1;    // named barrier of the consumers' epilogue
+// QT of the staged instance: the weights arrive already decoded to T, a [N, K] panel (launch_gemm4_staged)
+constexpr int kDecoded = -1;
 
 struct Gemm4Params {
     const uint8_t* B;            // packed codes [N, K/2]
@@ -81,6 +93,18 @@ struct Gemm4Params {
     int tiles_total;
     int splits;                  // K splits per tile (1 = none)
 };
+
+// the staged instance: D[64 x MT] += A[64 x 16] * X[MT x 16]^T with both operands from descriptors
+template <typename T, int MT>
+__device__ __forceinline__ void wgmma_step_ss(float (&d)[MT / 2], uint64_t a_desc, uint64_t b_desc) {
+    constexpr bool bf = std::is_same<T, __nv_bfloat16>::value;
+    static_assert(MT == 128 || MT == 256, "staged token tile");
+    if constexpr (MT == 128) {
+        if constexpr (bf) ptx::wgmma_m64n128k16_bf16_ss(d, a_desc, b_desc); else ptx::wgmma_m64n128k16_f16_ss(d, a_desc, b_desc);
+    } else {
+        if constexpr (bf) ptx::wgmma_m64n256k16_bf16_ss(d, a_desc, b_desc); else ptx::wgmma_m64n256k16_f16_ss(d, a_desc, b_desc);
+    }
+}
 
 // one k16 step of a 64-row warpgroup tile: D[64 x MT] += A[64 x 16] (registers) * X[MT x 16]^T (descriptor)
 // (T = float: one k8 step with TF32 operands)
@@ -114,26 +138,31 @@ __device__ __forceinline__ void wgmma_step(float (&d)[MT / 2], const uint32_t (&
 // steps, so its two A-fragment sets are the 64 registers of the 16-bit kernel's 128-deep ones.  The epilogue stages
 // the output tile in a buffer of its own (the producer is already filling the ring for the CTA's next tile), and the
 // ring takes as many stages as fit next to it, at most 8.
-template <typename T, int MT> struct StageCfg {
+// The staged instance (SS) loads a [128 x 64] tile of the decoded weight panel per stage (128-byte rows, 128-byte
+// swizzle: the K-major A operand of wgmma) and stages the epilogue in slices of 64 tokens, so that the 256-token tile
+// keeps four 48 KB stages (its whole 68 KB tile next to them leaves room for three).
+template <typename T, int MT, bool SS = false> struct StageCfg {
     static constexpr bool kTf32 = std::is_same<T, float>::value;
-    static constexpr int kBK = (MT == 256 || kTf32) ? 64 : 128;
+    static constexpr int kBK = (MT == 256 || kTf32 || SS) ? 64 : 128;
     static constexpr int kSteps = kBK / (kTf32 ? 8 : 16);       // wgmma k16 (k8 for TF32) steps
     static constexpr int kChunks = kBK / 32;                     // 16-byte (32-code) pieces of a code row
     static constexpr int kSubK = 128 / (int)sizeof(T);           // k-elements of one sub-tile row
     static constexpr int kXSubBytes = MT * 128;                  // one sub-tile
     static constexpr int kXStageBytes = (kBK / kSubK) * kXSubBytes;
-    static constexpr int kWRowBytes = kBK / 2;                   // packed codes of one row (TMA, kWRowBytes-byte swizzle)
+    static constexpr int kWRowBytes = SS ? kBK * (int)sizeof(T)  // decoded weights of one row (128 bytes)
+                                         : kBK / 2;              // packed codes of one row (TMA, kWRowBytes-byte swizzle)
     static constexpr int kWStageBytes = kTileN * kWRowBytes;
     static constexpr int kStageBytes = kXStageBytes + kWStageBytes;
     // epilogue staging: one output row of the tile (128 x T) plus 16 bytes, so that the fragment stores (four
     // token rows two apart per warp instruction) fall on distinct banks
     static constexpr int kOutPitch = kTileN * (int)sizeof(T) + 16;
-    static constexpr int kOutBytes = MT * kOutPitch;
+    static constexpr int kOutSlices = SS ? MT / 64 : 1;          // the tile is staged and stored in token slices
+    static constexpr int kOutBytes = MT / kOutSlices * kOutPitch;
     static constexpr int kSlack = 1024 + 256;                    // base alignment + barriers
     static constexpr int kRing = (227 * 1024 - kSlack - kOutBytes) / kStageBytes;
     static constexpr int kStages = kRing > 8 ? 8 : kRing;
     static constexpr int kSmemBytes = kSlack + kStages * kStageBytes + kOutBytes;
-    static_assert(kStages >= 2 && kSmemBytes <= 227 * 1024, "shared memory");
+    static_assert(kStages >= (SS ? 4 : 2) && kSmemBytes <= 227 * 1024, "shared memory");
 };
 
 // The 16 codes of a 16-byte chunk (stage-row words w[4q .. 4q+3]) that this thread's A fragments need (byte `t` of
@@ -158,7 +187,8 @@ template <typename T, int QT, int MT, bool DQ>
 __global__ void __launch_bounds__(kThreads, 1)
     gemm4_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
                     const Gemm4Params p) {
-    using Cfg = StageCfg<T, MT>;
+    constexpr bool kSS = QT == kDecoded;  // the staged instance: weights from a decoded panel, no decode here
+    using Cfg = StageCfg<T, MT, kSS>;
     constexpr bool kTf32 = Cfg::kTf32;
     constexpr int kBK = Cfg::kBK;
     constexpr int kSteps = Cfg::kSteps;
@@ -175,7 +205,7 @@ __global__ void __launch_bounds__(kThreads, 1)
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t* sx = smem;                              // [kStages][BK/kSubK][MT x 128 B] activations
-    uint8_t* sw = smem + kStages * kXStageBytes;     // [kStages][128 x BK/2 B]        packed codes
+    uint8_t* sw = smem + kStages * kXStageBytes;     // [kStages][128 x BK/2 B]        packed codes (SS: 128 x 128 B)
     uint8_t* so = smem + kStages * Cfg::kStageBytes; // [MT][kOutPitch]                epilogue staging
     uint64_t* bars = reinterpret_cast<uint64_t*>(so + Cfg::kOutBytes);
     uint64_t* full = bars;                   // [kStages] TMA (1 arrive + bytes) -> consumers
@@ -233,7 +263,7 @@ __global__ void __launch_bounds__(kThreads, 1)
                     ptx::mbar_arrive_expect_tx(&full[slot], kWStageBytes + kXStageBytes);
                     // rows past M, rows past N and columns past K are out of bounds for the tensor maps: TMA
                     // zero-fills.  Packed codes of the tile's 128 output features: bytes [k0/2, k0/2 + BK/2).
-                    ptx::tma_load_2d(sw + slot * kWStageBytes, &tmap_w, &full[slot], k0 / 2, w.n0);
+                    ptx::tma_load_2d(sw + slot * kWStageBytes, &tmap_w, &full[slot], kSS ? k0 : k0 / 2, w.n0);
 #pragma unroll
                     for (int h = 0; h < kBK / Cfg::kSubK; ++h)
                         ptx::tma_load_2d(sx + slot * kXStageBytes + h * kXSubBytes, &tmap_x, &full[slot],
@@ -341,13 +371,21 @@ __global__ void __launch_bounds__(kThreads, 1)
         auto mma_stage = [&](int s, const uint32_t (&a)[kSteps][4]) {
             const uint32_t xs = ptx::smem_u32(sx + s * kXStageBytes);
             ptx::wgmma_fence();
+            if constexpr (kSS) {
+                // this warpgroup's 64 weight rows: 8 KB into the stage's tile, a 1024-byte-aligned swizzle atom group
+                const uint64_t a_desc = ptx::make_sw128_kmajor_desc(ptx::smem_u32(sw + s * kWStageBytes + wg * 64 * 128));
 #pragma unroll
-            for (int j = 0; j < kSteps; ++j)
-                wgmma_step<T, MT>(acc, a[j], ptx::make_sw128_kmajor_desc(xs + (j >> 2) * kXSubBytes) + 2 * (j & 3));
+                for (int j = 0; j < kSteps; ++j)
+                    wgmma_step_ss<T, MT>(acc, a_desc + 2 * j, ptx::make_sw128_kmajor_desc(xs) + 2 * j);
+            } else {
+#pragma unroll
+                for (int j = 0; j < kSteps; ++j)
+                    wgmma_step<T, MT>(acc, a[j], ptx::make_sw128_kmajor_desc(xs + (j >> 2) * kXSubBytes) + 2 * (j & 3));
+            }
             ptx::wgmma_commit();
         };
 
-        fetch(0);
+        if constexpr (!kSS) fetch(0);
         int prev_s = -1;
         for (int i0 = 0; i0 < nst; i0 += 2) {
 #pragma unroll
@@ -360,8 +398,10 @@ __global__ void __launch_bounds__(kThreads, 1)
                         slot = 0;
                         phase ^= 1u;
                     }
-                    decode(s, afr[h]);
-                    fetch(i + 1);
+                    if constexpr (!kSS) {
+                        decode(s, afr[h]);
+                        fetch(i + 1);
+                    }
                     mma_stage(s, afr[h]);
                     // the wgmma group of the previous stage has completed: its activation tile (and its A set) are free
                     ptx::wgmma_wait<1>();
@@ -391,29 +431,66 @@ __global__ void __launch_bounds__(kThreads, 1)
             // 128 contiguous elements of the output.  (fp32: the bias is added in fp32 and nothing is rounded.)
             constexpr int kPitch = Cfg::kOutPitch;
             constexpr int kVec = 16 / (int)sizeof(T);
-            ptx::bar_sync(kBarEpi, kConsumers);
+            constexpr int kSliceT = MT / Cfg::kOutSlices;  // tokens per staged slice
+            if constexpr (Cfg::kOutSlices == 1) {
+                ptx::bar_sync(kBarEpi, kConsumers);
 #pragma unroll
-            for (int j = 0; j < MT / 8; ++j)
+                for (int j = 0; j < MT / 8; ++j)
 #pragma unroll
-                for (int e = 0; e < 4; ++e)
-                    *reinterpret_cast<T*>(so + (8 * j + 2 * t + (e & 1)) * kPitch + (row0 + 8 * (e >> 1)) * (int)sizeof(T)) =
-                        DT<T>::from_f32(acc[4 * j + e] + (e >= 2 ? bias_b : bias_a));
-            ptx::bar_sync(kBarEpi, kConsumers);
-            for (int idx = ct; idx < MT * (kTileN / kVec); idx += kConsumers) {
-                const int c = idx / (kTileN / kVec), n = n0 + kVec * (idx % (kTileN / kVec));
-                const int m = m0 + c;
-                if (m >= p.M || n >= p.N) continue;
-                const uint8_t* src = so + c * kPitch + (n - n0) * (int)sizeof(T);
-                const long long o = (long long)m * p.ldc + n;
-                if (p.out_vec && n + kVec <= p.N) {
-                    const uint4 val = *reinterpret_cast<const uint4*>(src);
-                    *reinterpret_cast<uint4*>(outp + o) = val;
-                    for (int r = 0; r < p.n_peers; ++r) *reinterpret_cast<uint4*>(reinterpret_cast<T*>(p.peer_out[r]) + o) = val;
-                } else {
-                    for (int x = 0; x < kVec && n + x < p.N; ++x) {
-                        const T val = reinterpret_cast<const T*>(src)[x];
-                        outp[o + x] = val;
-                        for (int r = 0; r < p.n_peers; ++r) reinterpret_cast<T*>(p.peer_out[r])[o + x] = val;
+                    for (int e = 0; e < 4; ++e)
+                        *reinterpret_cast<T*>(so + (8 * j + 2 * t + (e & 1)) * kPitch + (row0 + 8 * (e >> 1)) * (int)sizeof(T)) =
+                            DT<T>::from_f32(acc[4 * j + e] + (e >= 2 ? bias_b : bias_a));
+                ptx::bar_sync(kBarEpi, kConsumers);
+                for (int idx = ct; idx < MT * (kTileN / kVec); idx += kConsumers) {
+                    const int c = idx / (kTileN / kVec), n = n0 + kVec * (idx % (kTileN / kVec));
+                    const int m = m0 + c;
+                    if (m >= p.M || n >= p.N) continue;
+                    const uint8_t* src = so + c * kPitch + (n - n0) * (int)sizeof(T);
+                    const long long o = (long long)m * p.ldc + n;
+                    if (p.out_vec && n + kVec <= p.N) {
+                        const uint4 val = *reinterpret_cast<const uint4*>(src);
+                        *reinterpret_cast<uint4*>(outp + o) = val;
+                        for (int r = 0; r < p.n_peers; ++r) *reinterpret_cast<uint4*>(reinterpret_cast<T*>(p.peer_out[r]) + o) = val;
+                    } else {
+                        for (int x = 0; x < kVec && n + x < p.N; ++x) {
+                            const T val = reinterpret_cast<const T*>(src)[x];
+                            outp[o + x] = val;
+                            for (int r = 0; r < p.n_peers; ++r) reinterpret_cast<T*>(p.peer_out[r])[o + x] = val;
+                        }
+                    }
+                }
+            } else {
+                // the staged instance: slices of kSliceT tokens (every j unrolled, the slice test predicated, so
+                // that the accumulators stay in registers)
+                for (int sl = 0; sl < Cfg::kOutSlices; ++sl) {
+                    ptx::bar_sync(kBarEpi, kConsumers);
+#pragma unroll
+                    for (int j = 0; j < MT / 8; ++j) {
+                        if (j / (kSliceT / 8) != sl) continue;
+#pragma unroll
+                        for (int e = 0; e < 4; ++e)
+                            *reinterpret_cast<T*>(so + (8 * j - sl * kSliceT + 2 * t + (e & 1)) * kPitch +
+                                                  (row0 + 8 * (e >> 1)) * (int)sizeof(T)) =
+                                DT<T>::from_f32(acc[4 * j + e] + (e >= 2 ? bias_b : bias_a));
+                    }
+                    ptx::bar_sync(kBarEpi, kConsumers);
+                    for (int idx = ct; idx < kSliceT * (kTileN / kVec); idx += kConsumers) {
+                        const int c = idx / (kTileN / kVec), n = n0 + kVec * (idx % (kTileN / kVec));
+                        const int m = m0 + sl * kSliceT + c;
+                        if (m >= p.M || n >= p.N) continue;
+                        const uint8_t* src = so + c * kPitch + (n - n0) * (int)sizeof(T);
+                        const long long o = (long long)m * p.ldc + n;
+                        if (p.out_vec && n + kVec <= p.N) {
+                            const uint4 val = *reinterpret_cast<const uint4*>(src);
+                            *reinterpret_cast<uint4*>(outp + o) = val;
+                            for (int r = 0; r < p.n_peers; ++r) *reinterpret_cast<uint4*>(reinterpret_cast<T*>(p.peer_out[r]) + o) = val;
+                        } else {
+                            for (int x = 0; x < kVec && n + x < p.N; ++x) {
+                                const T val = reinterpret_cast<const T*>(src)[x];
+                                outp[o + x] = val;
+                                for (int r = 0; r < p.n_peers; ++r) reinterpret_cast<T*>(p.peer_out[r])[o + x] = val;
+                            }
+                        }
                     }
                 }
             }
@@ -568,7 +645,8 @@ Workspace* get_workspace(cudaStream_t stream, size_t partial_bytes, size_t n_cou
 
 template <typename T, int QT, int MT, bool DQ>
 bool launch_mt(const T* A, Gemm4Params& p, int force_splits, cudaStream_t stream) {
-    using Cfg = StageCfg<T, MT>;
+    constexpr bool kSS = QT == kDecoded;
+    using Cfg = StageCfg<T, MT, kSS>;
     constexpr int kBK = Cfg::kBK;
     constexpr size_t smem_bytes = Cfg::kSmemBytes;
     // the shared-memory opt-in is PER DEVICE (one process may drive several GPUs)
@@ -588,10 +666,17 @@ bool launch_mt(const T* A, Gemm4Params& p, int force_splits, cudaStream_t stream
     if (!encode_tmap_2d(&tmap, A, (int)sizeof(T), 128, (uint64_t)p.M, (uint64_t)p.K, (uint64_t)p.K * sizeof(T),
                         (uint32_t)MT, (uint32_t)Cfg::kSubK))
         return false;
-    // packed codes as a [N, K/2] byte matrix, 128 x BK/2-byte boxes, BK/2-byte swizzle
-    if (!encode_tmap_2d(&tmap_w, p.B, 1, Cfg::kWRowBytes, (uint64_t)p.N, (uint64_t)p.K / 2, (uint64_t)p.K / 2,
-                        (uint32_t)kTileN, (uint32_t)Cfg::kWRowBytes))
-        return false;
+    if constexpr (kSS) {
+        // the decoded panel [N, K] of T, 128 x 64 boxes (128-byte rows), 128-byte swizzle
+        if (!encode_tmap_2d(&tmap_w, p.B, (int)sizeof(T), 128, (uint64_t)p.N, (uint64_t)p.K, (uint64_t)p.K * sizeof(T),
+                            (uint32_t)kTileN, (uint32_t)kBK))
+            return false;
+    } else {
+        // packed codes as a [N, K/2] byte matrix, 128 x BK/2-byte boxes, BK/2-byte swizzle
+        if (!encode_tmap_2d(&tmap_w, p.B, 1, Cfg::kWRowBytes, (uint64_t)p.N, (uint64_t)p.K / 2, (uint64_t)p.K / 2,
+                            (uint32_t)kTileN, (uint32_t)Cfg::kWRowBytes))
+            return false;
+    }
     p.kblocks_total = (p.K + kBK - 1) / kBK;
     // Every row starts at n * K, a multiple of the largest power of two dividing K, and every stage at a multiple of
     // BK: a quantisation block can begin only at 32-code chunks that are multiples of min(blocksize, that, BK).
@@ -619,6 +704,11 @@ bool launch_mt(const T* A, Gemm4Params& p, int force_splits, cudaStream_t stream
     }
     // a forced split must still be one co-resident wave (the splits of a tile wait for each other)
     if (splits > 1 && tiles * splits > sms) return false;
+    // the staged route keeps its weight panel in the split-K workspace: it must never split
+    if (kSS && splits != 1) {
+        set_last_error_msg("gemm4_tc: the staged GEMM was asked to split K");
+        return false;
+    }
     p.splits = splits;
     p.n_tiles = n_tiles;
     p.tiles_total = tiles;
@@ -739,6 +829,128 @@ bool launch_gemm4_tc(const T* A, const uint8_t* B, const float* absmax, const ui
     }
 #undef BNB200_DISPATCH_MT
 }
+
+// ------------------------------------------------------------------ the staged route
+// At large M the fused kernel decodes every weight once per token tile (M / 256 times).  The staged route decodes
+// each weight once: it loops over panels of `panel_rows` output features (a multiple of 128), decodes the panel into
+// the stream's workspace block (dequantize4_prmt_kernel, the fused kernel's table decode and scale fetch: the same
+// bits) and runs the staged instance of gemm4_tc_kernel over all M tokens of that panel.  Both launches go on
+// `stream`, so a panel is never overwritten while the GEMM before it still reads it.  Same A values, same k16 order,
+// same instruction shape, accumulation from zero and one rounding in the same epilogue: the output is the fused
+// kernel's, bit for bit.  The panel lives in the per-stream split-K block, so the staged GEMM never splits K.
+int staged_max_panel_rows(int K, int elem_bytes) {
+    const long long rows = (long long)kWsBytes / ((long long)K * elem_bytes);
+    return rows >= kTileN ? (int)(rows / kTileN * kTileN) : 0;
+}
+
+// Each panel is a launch of its own, so the last wave of every panel's 256-token tiles runs partly empty.  The panel
+// is the one (a multiple of 128 rows that fits the workspace) whose panels take the fewest waves in all, the largest
+// of those (fewest launches).  Returns that wave count and sets *panel_rows; 0 when no panel fits.
+int staged_plan(int M, int N, int K, int sms, int* panel_rows) {
+    const int max_units = staged_max_panel_rows(K, 2) / kTileN;
+    const long long m_tiles = (M + 255) / 256;
+    const int n_units = (N + kTileN - 1) / kTileN;
+    long long best = 0;
+    for (int u = 1; u <= max_units && u <= n_units; ++u) {
+        const long long full = n_units / u, rest = n_units % u;
+        const long long waves = full * ((m_tiles * u + sms - 1) / sms) + (rest ? (m_tiles * rest + sms - 1) / sms : 0);
+        if (best == 0 || waves <= best) {
+            best = waves;
+            *panel_rows = u * kTileN;
+        }
+    }
+    return (int)best;
+}
+
+// panel_rows 0: the panel of staged_plan (DESIGN.md section 3.1)
+template <typename T>
+bool launch_gemm4_staged(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
+                         const float* absmax_code, const float* absmax_offset, T* out, const T* bias, int M, int N,
+                         int K, int ldc, int blocksize, int quant_type, cudaStream_t stream, void* const* peers,
+                         int n_peers, int mt_override, int panel_rows) {
+    static_assert(!std::is_same<T, float>::value, "the staged route has 16-bit instances only");
+    if (n_peers < 0 || n_peers > 7) return false;
+    if (M <= 0 || N <= 0) return true;
+    if (K < 64 || (K % 64) != 0) return false;
+    if (blocksize < 32 || (blocksize & (blocksize - 1)) != 0) return false;
+    if ((reinterpret_cast<uintptr_t>(A) & 15) != 0 || (reinterpret_cast<uintptr_t>(B) & 15) != 0) return false;
+    if (quant_type != kNF4 && quant_type != kFP4) return false;
+    const int max_rows = staged_max_panel_rows(K, (int)sizeof(T));
+    const int sms = device_sm_count();
+    if (panel_rows == 0) staged_plan(M, N, K, sms, &panel_rows);
+    if (panel_rows <= 0 || panel_rows % kTileN != 0 || panel_rows > max_rows) return false;
+    const int n_pad = (N + kTileN - 1) / kTileN * kTileN;
+    if (panel_rows > n_pad) panel_rows = n_pad;
+
+    // 256-token tiles where the whole weight's tiles fill the SMs (every shape the dispatcher routes here)
+    int MT = (long long)((M + 255) / 256) * (n_pad / kTileN) >= sms ? 256 : 128;
+    if (mt_override != 0) {
+        if (mt_override != 128 && mt_override != 256) return false;
+        MT = mt_override;
+    }
+    Workspace* ws = get_workspace(stream, (size_t)panel_rows * K * sizeof(T), 0);
+    if (ws == nullptr) {
+        set_last_error_msg("gemm4_tc: could not allocate the staged route's workspace");
+        return false;
+    }
+    T* panel = reinterpret_cast<T*>(ws->ptr);
+    bool vec = (ldc % (16 / (int)sizeof(T))) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0;
+    for (int r = 0; r < n_peers; ++r) vec = vec && (reinterpret_cast<uintptr_t>(peers[r]) & 15) == 0;
+    for (int n0 = 0; n0 < N; n0 += panel_rows) {
+        const int rows = N - n0 < panel_rows ? N - n0 : panel_rows;
+        launch_dequantize4_panel<T>(B, absmax, absmax_8bit, absmax_code, absmax_offset, panel, blocksize, quant_type,
+                                    n0, rows, K, stream);
+        // the panel's columns of the output: n0 is a multiple of 128, so every base keeps its 16-byte alignment
+        Gemm4Params p{};
+        p.B = reinterpret_cast<const uint8_t*>(panel);
+        p.bias = bias != nullptr ? bias + n0 : nullptr;
+        p.out = out + n0;
+        p.n_peers = n_peers;
+        for (int r = 0; r < n_peers; ++r) p.peer_out[r] = reinterpret_cast<T*>(peers[r]) + n0;
+        p.M = M;
+        p.N = rows;
+        p.K = K;
+        p.ldc = ldc;
+        p.log2_bs = ilog2_pow2(blocksize);
+        p.out_vec = vec ? 1 : 0;
+        const bool ok = MT == 256 ? launch_mt<T, kDecoded, 256, false>(A, p, 1, stream)
+                                  : launch_mt<T, kDecoded, 128, false>(A, p, 1, stream);
+        if (!ok) return false;
+    }
+    return true;
+}
+
+template bool launch_gemm4_staged<__nv_bfloat16>(const __nv_bfloat16*, const uint8_t*, const float*, const uint8_t*,
+                                                 const float*, const float*, __nv_bfloat16*, const __nv_bfloat16*,
+                                                 int, int, int, int, int, int, cudaStream_t, void* const*, int, int,
+                                                 int);
+template bool launch_gemm4_staged<__half>(const __half*, const uint8_t*, const float*, const uint8_t*, const float*,
+                                          const float*, __half*, const __half*, int, int, int, int, int, int,
+                                          cudaStream_t, void* const*, int, int, int);
+
+// The staged GEMM alone on an already decoded weight W[N, K] (no workspace): for timing the route's phases.
+template <typename T>
+bool launch_gemm_decoded(const T* A, const T* W, T* out, const T* bias, int M, int N, int K, int ldc, int mt,
+                         cudaStream_t stream) {
+    if (M <= 0 || N <= 0) return true;
+    if (K < 64 || (K % 64) != 0 || (mt != 128 && mt != 256)) return false;
+    if ((reinterpret_cast<uintptr_t>(A) & 15) != 0 || (reinterpret_cast<uintptr_t>(W) & 15) != 0) return false;
+    Gemm4Params p{};
+    p.B = reinterpret_cast<const uint8_t*>(W);
+    p.bias = bias;
+    p.out = out;
+    p.M = M;
+    p.N = N;
+    p.K = K;
+    p.ldc = ldc;
+    p.out_vec = ((ldc % (16 / (int)sizeof(T))) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0) ? 1 : 0;
+    return mt == 256 ? launch_mt<T, kDecoded, 256, false>(A, p, 1, stream)
+                     : launch_mt<T, kDecoded, 128, false>(A, p, 1, stream);
+}
+template bool launch_gemm_decoded<__nv_bfloat16>(const __nv_bfloat16*, const __nv_bfloat16*, __nv_bfloat16*,
+                                                 const __nv_bfloat16*, int, int, int, int, int, cudaStream_t);
+template bool launch_gemm_decoded<__half>(const __half*, const __half*, __half*, const __half*, int, int, int, int, int,
+                                          cudaStream_t);
 
 template bool launch_gemm4_tc<__nv_bfloat16>(const __nv_bfloat16*, const uint8_t*, const float*, const uint8_t*,
                                              const float*, const float*, __nv_bfloat16*, const __nv_bfloat16*, int,

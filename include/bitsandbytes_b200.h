@@ -156,6 +156,10 @@ int cbnb_b200_gemm_4bit_multi_out(const void* A, const uint8_t* B, const float* 
  * wgmma GEMM runs on TF32 tensor cores with weights rna_tf32(fp32 dequantised weight); otherwise as dtype 0.
  * For tests / bench bookkeeping. */
 int cbnb_b200_gemm_4bit_path(int M, int N, int K, int blocksize, int dtype);
+/* 1 when an unforced path-1 call takes the staged route (fp16 / bf16, large M: each weight panel decoded once into a
+ * per-stream workspace, then the wgmma GEMM on shared-memory operands; the same bits as the fused kernel), else 0.
+ * A forced path 1 always runs the fused kernel. */
+int cbnb_b200_gemm_4bit_staged_route(int M, int N, int K, int blocksize, int dtype);
 /* Force a path for the next calls on this thread (-1 = automatic). */
 void cbnb_b200_gemm_4bit_force_path(int path);
 
@@ -164,6 +168,16 @@ void cbnb_b200_gemm_4bit_force_path(int path);
  * least one stage per split: 128 deep, 64 deep at mt = 256 and for dtype 3).  dtype 1, 2 or 3 (TF32).  `trace` must be NULL (the name and argument list are kept for ABI stability).  Returns 0, or 100 when
  * the shape or the options are not served (a forced split must fit one co-resident wave of CTAs). */
 int cbnb_b200_gemm_4bit_pair(const void* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit, const float* absmax_code, const float* absmax_offset, void* out, const void* bias, int M, int N, int K, int ldc, int blocksize, int quant_type, int dtype, int mt, int force_splits, long long* trace, bnb_stream_t stream);
+
+/* Developer / test entries for the staged route.  _staged: the whole route with token tile mt (128 | 256,
+ * 0 = by the shape) and panel_rows output features per panel (a multiple of 128 whose decoded rows fit the 32 MB
+ * per-stream workspace, 0 = the largest such), stores to outs[0..n_outs) as _multi_out; returns 0, or 100 when not
+ * served.  _dequantize_4bit_panel: rows [n0, n0 + rows) of a [N, K] 4-bit weight decoded into out[rows, K]
+ * (n0 % 128 == 0), bit-identical to the same rows of F.dequantize_4bit.  _gemm_decoded: the staged GEMM alone,
+ * out[M, N] = A[M, K] . W[N, K]^T (+ bias) on an already decoded W.  dtype 1 = fp16, 2 = bf16. */
+int cbnb_b200_gemm_4bit_staged(const void* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit, const float* absmax_code, const float* absmax_offset, void* const* outs, int n_outs, const void* bias, int M, int N, int K, int ldc, int blocksize, int quant_type, int dtype, int mt, int panel_rows, bnb_stream_t stream);
+int cbnb_b200_dequantize_4bit_panel(const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit, const float* absmax_code, const float* absmax_offset, void* out, int blocksize, int quant_type, int dtype, int n0, int rows, int K, bnb_stream_t stream);
+int cbnb_b200_gemm_decoded(const void* A, const void* W, void* out, const void* bias, int M, int N, int K, int ldc, int dtype, int mt, bnb_stream_t stream);
 
 /* Strided-output variant used by the column-sharded linear: out has row stride ldc
  * (elements), so a shard writes its [M, N_shard] block into the gathered [M, N]. */
