@@ -705,7 +705,9 @@ def optimizer_multi_capacity() -> int:
 
 
 def _optimizer_list(what, optimizer_name, supported, g, p, state1, state2, absmax1, absmax2, step, eight_bit):
-    """Validate a multi-tensor step as the single-tensor ops do and pack its descriptors (cextension.OptimTensor)."""
+    """Validate a multi-tensor step as the single-tensor ops do and pack its descriptors (cextension.OptimTensor).
+    Returns (g[0], descriptors, capturable): capturable when the steps are CUDA tensors, the device step counters that
+    the _dev entries advance and read; their descriptors carry the counters' pointers instead of the steps."""
     if optimizer_name not in supported:
         raise ValueError(f"Unsupported optimizer name: {optimizer_name}. Supported optimizers: {list(supported)}")
     k = len(p)
@@ -721,14 +723,15 @@ def _optimizer_list(what, optimizer_name, supported, g, p, state1, state2, absma
         if values is None or len(values) != k:
             raise ValueError(f"{what}: {name} must list one entry per parameter ({k})")
     if k == 0:
-        return None, None
+        return None, None, False
     dtype, device = g[0].dtype, g[0].device
+    capturable = any(isinstance(s, torch.Tensor) and s.is_cuda for s in step)
     if dtype not in _DTYPE_ID:
         raise ValueError(f"{what}: unsupported gradient dtype {dtype}. Supported dtypes: torch.float32, torch.float16, "
                          "torch.bfloat16")
     if device.type != "cuda":
         raise RuntimeError(f"{what}: tensors must live on a CUDA device, got {device}")
-    descs = []
+    descs, step_ptrs = [], set()
     for i in range(k):
         s2 = state2[i] if two else None
         a1 = absmax1[i] if eight_bit else None
@@ -745,9 +748,33 @@ def _optimizer_list(what, optimizer_name, supported, g, p, state1, state2, absma
             # managed ("paged") state is a CPU tensor to PyTorch that every GPU can address
             if t.device != device and not getattr(t, "is_paged", False):
                 raise RuntimeError(f"{what}: tensors must be on one device, {device}; entry {i} has one on {t.device}")
-        descs.append(cext.OptimTensor(pi.data_ptr(), gi.data_ptr(), state1[i].data_ptr(), _optional_ptr(s2),
-                                      _optional_ptr(a1), _optional_ptr(a2), pi.numel(), int(step[i]), 0))
-    return g[0], (cext.OptimTensor * k)(*descs)
+        if not capturable:
+            descs.append(cext.OptimTensor(pi.data_ptr(), gi.data_ptr(), state1[i].data_ptr(), _optional_ptr(s2),
+                                          _optional_ptr(a1), _optional_ptr(a2), pi.numel(), int(step[i]), 0))
+            continue
+        si = step[i]
+        if (not isinstance(si, torch.Tensor) or si.dtype != torch.int32 or si.numel() != 1 or not si.is_contiguous()
+                or si.device != device):
+            raise ValueError(f"{what}: device steps must be contiguous one-element int32 tensors on {device} (entry {i})")
+        d = cext.OptimTensor(pi.data_ptr(), gi.data_ptr(), state1[i].data_ptr(), _optional_ptr(s2), _optional_ptr(a1),
+                             _optional_ptr(a2), pi.numel())
+        d.step_ptr = si.data_ptr()
+        step_ptrs.add(d.step_ptr)
+        descs.append(d)
+    if capturable and len(step_ptrs) != k:
+        raise ValueError(f"{what}: every parameter needs its own step counter (the call advances each once)")
+    return g[0], (cext.OptimTensor * k)(*descs), capturable
+
+
+def _device_lr(what, lr, device):
+    """(lr, lr_dev) of a capturable call: a one-element fp32 tensor on the device is read by the kernel at every launch
+    (and every replay of a CUDA graph); a number is passed by value."""
+    if not isinstance(lr, torch.Tensor):
+        return float(lr), None
+    if lr.dtype != torch.float32 or lr.numel() != 1 or lr.device != device:
+        raise ValueError(f"{what}: a tensor lr must be a one-element float32 tensor on {device}, got {lr.dtype} "
+                         f"{tuple(lr.shape)} on {lr.device}")
+    return 0.0, lr.data_ptr()
 
 
 def _launch_list(what, fn, optimizer_name, g0, descs, scalars):
@@ -764,14 +791,23 @@ def _launch_list(what, fn, optimizer_name, g0, descs, scalars):
 def optimizer_update_32bit_multi(optimizer_name, g, p, state1, state2, beta1, beta2, beta3, alpha, eps, weight_decay, step,
                                  lr, gnorm_scale=1.0, skip_zeros=False):
     """In-place fp32-state steps of several parameters in one launch per capacity chunk: g, p, state1, state2 (None for
-    one-state optimizers) and step list one entry per parameter; the scalars are shared.  No trust ratio (max_unorm)."""
+    one-state optimizers) and step list one entry per parameter; the scalars are shared.  No trust ratio (max_unorm).
+
+    Capturable route: when the steps are one-element int32 CUDA tensors, the call advances each by one on the device
+    and updates with the advanced values; lr may then also be a one-element fp32 CUDA tensor.  Nothing is read on the
+    host, so the call can be captured in a CUDA graph and replayed."""
     what = "optimizer_update_32bit_multi"
-    g0, descs = _optimizer_list(what, optimizer_name, _OPTIMIZER_ID, g, p, state1, state2, None, None, step, False)
+    g0, descs, dev = _optimizer_list(what, optimizer_name, _OPTIMIZER_ID, g, p, state1, state2, None, None, step, False)
     if descs is None:
         return
+    if dev:
+        lr_value, lr_dev = _device_lr(what, lr, g0.device)
+        fn, scalars = lib.cbnb_b200_optimizer_update_32bit_multi_dev, (float(lr_value), lr_dev)
+    else:
+        fn, scalars = lib.cbnb_b200_optimizer_update_32bit_multi, (float(lr),)
     with _on_device(g0):
-        _launch_list(what, lib.cbnb_b200_optimizer_update_32bit_multi, optimizer_name, g0, descs,
-                     (float(beta1), float(beta2), float(beta3), float(alpha), float(eps), float(weight_decay), float(lr),
+        _launch_list(what, fn, optimizer_name, g0, descs,
+                     (float(beta1), float(beta2), float(beta3), float(alpha), float(eps), float(weight_decay), *scalars,
                       float(gnorm_scale), bool(skip_zeros)))
 
 
@@ -779,16 +815,22 @@ def optimizer_update_8bit_blockwise_multi(optimizer_name, g, p, state1, state2, 
                                           qmap1, qmap2, absmax1, absmax2, weight_decay, gnorm_scale=1.0, skip_zeros=False):
     """In-place blockwise (256) 8-bit-state steps of several parameters in one launch per capacity chunk: g, p, state1,
     state2, absmax1, absmax2 and step list one entry per parameter (state2 / absmax2 None for one-state optimizers);
-    the code books qmap1 / qmap2 and the scalars are shared."""
+    the code books qmap1 / qmap2 and the scalars are shared.  Device steps (and lr) as optimizer_update_32bit_multi."""
     what = "optimizer_update_8bit_blockwise_multi"
-    g0, descs = _optimizer_list(what, optimizer_name, _OPTIMIZER_8BIT, g, p, state1, state2, absmax1, absmax2, step, True)
+    g0, descs, dev = _optimizer_list(what, optimizer_name, _OPTIMIZER_8BIT, g, p, state1, state2, absmax1, absmax2, step,
+                                     True)
     if descs is None:
         return
     two = optimizer_name in ("adam", "ademamix")
     for q in (qmap1, qmap2) if two else (qmap1,):
         if q is None or q.device != g0.device or not q.is_contiguous() or q.dtype != torch.float32 or q.numel() < 256:
             raise ValueError(f"{what}: the code books must be contiguous fp32 [256] tensors on {g0.device}")
+    if dev:
+        lr_value, lr_dev = _device_lr(what, lr, g0.device)
+        fn, scalars = lib.cbnb_b200_optimizer_update_8bit_blockwise_multi_dev, (float(lr_value), lr_dev)
+    else:
+        fn, scalars = lib.cbnb_b200_optimizer_update_8bit_blockwise_multi, (float(lr),)
     with _on_device(g0):
-        _launch_list(what, lib.cbnb_b200_optimizer_update_8bit_blockwise_multi, optimizer_name, g0, descs,
-                     (float(beta1), float(beta2), float(beta3), float(alpha), float(eps), float(weight_decay), float(lr),
+        _launch_list(what, fn, optimizer_name, g0, descs,
+                     (float(beta1), float(beta2), float(beta3), float(alpha), float(eps), float(weight_decay), *scalars,
                       qmap1.data_ptr(), qmap2.data_ptr() if two else None, float(gnorm_scale), bool(skip_zeros)))

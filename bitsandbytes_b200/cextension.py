@@ -129,14 +129,30 @@ def _signatures():
     #  skip_zeros, stream) -> int
     sig["cbnb_b200_optimizer_update_8bit_blockwise_multi"] = ([_I32, _I32, _VOIDP, _I32] + [_F] * 7 + [_VOIDP, _VOIDP, _F,
                                                                ct.c_bool, _VOIDP], _I32)
+    # the capturable forms: (optimizer, dtype, tensors (with step_ptr), count, beta1 .. lr, lr_dev, ...) -> int
+    sig["cbnb_b200_optimizer_update_32bit_multi_dev"] = ([_I32, _I32, _VOIDP, _I32] + [_F] * 7 + [_VOIDP, _F, ct.c_bool,
+                                                          _VOIDP], _I32)
+    sig["cbnb_b200_optimizer_update_8bit_blockwise_multi_dev"] = ([_I32, _I32, _VOIDP, _I32] + [_F] * 7 + [_VOIDP] * 3
+                                                                   + [_F, ct.c_bool, _VOIDP], _I32)
     return sig
 
 
 class OptimTensor(ct.Structure):
-    """One entry of a multi-tensor optimizer call: bnb_b200_optim_tensor_t of include/bitsandbytes_b200.h."""
+    """One entry of a multi-tensor optimizer call: bnb_b200_optim_tensor_t of include/bitsandbytes_b200.h.
+
+    ``step`` and ``reserved`` share their 8 bytes with ``step_ptr``, the device step counter of the capturable (_dev)
+    entries: the C union, which ctypes fields cannot overlap, is the ``step_ptr`` property."""
 
     _fields_ = [("p", _VOIDP), ("g", _VOIDP), ("state1", _VOIDP), ("state2", _VOIDP), ("absmax1", _VOIDP),
                 ("absmax2", _VOIDP), ("n", ct.c_longlong), ("step", ct.c_int32), ("reserved", ct.c_int32)]
+
+    @property
+    def step_ptr(self):
+        return _VOIDP.from_buffer(self, OptimTensor.step.offset).value
+
+    @step_ptr.setter
+    def step_ptr(self, ptr):
+        _VOIDP.from_buffer(self, OptimTensor.step.offset).value = ptr
 
 
 EXPORTED_SYMBOLS = tuple(sorted(_signatures()))

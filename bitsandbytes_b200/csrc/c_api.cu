@@ -39,6 +39,13 @@ bool launch_optimizer32bit_list(int opt, int dtype, const OptimTensor* ts, int c
 bool launch_optimizer8bit_blockwise_list(int opt, int dtype, const OptimTensor* ts, int count, float beta1, float beta2,
                                          float beta3, float alpha, float eps, float wd, float lr, const float* q1,
                                          const float* q2, float gnorm_scale, bool skip_zeros, cudaStream_t st);
+bool launch_optimizer32bit_list_dev(int opt, int dtype, const OptimTensor* ts, int count, float beta1, float beta2,
+                                    float beta3, float alpha, float eps, float wd, float lr, const float* lr_dev,
+                                    float gnorm_scale, bool skip_zeros, cudaStream_t st);
+bool launch_optimizer8bit_blockwise_list_dev(int opt, int dtype, const OptimTensor* ts, int count, float beta1,
+                                             float beta2, float beta3, float alpha, float eps, float wd, float lr,
+                                             const float* lr_dev, const float* q1, const float* q2, float gnorm_scale,
+                                             bool skip_zeros, cudaStream_t st);
 
 template <typename T>
 void launch_gemv4_simt(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
@@ -749,6 +756,47 @@ int cbnb_b200_optimizer_update_8bit_blockwise_multi(int optimizer, int dtype, co
     if (!optimizer_list_ok("optimizer_update_8bit_blockwise_multi", optimizer, dtype, tensors, count)) return 100;
     launch_optimizer8bit_blockwise_list(optimizer, dtype, tensors, count, beta1, beta2, beta3, alpha, eps,
                                         weight_decay, lr, quantiles1, quantiles2, gnorm_scale, skip_zeros, stream);
+    return 0;
+}
+
+// Capturable multi-tensor steps: each descriptor's step_ptr is the tensor's int32 step counter in device memory, which
+// the call advances before the update reads it; lr_dev, if not NULL, is read in place of lr.  A CUDA graph that
+// captured the call therefore uses the current steps and learning rate at every replay.
+static bool optimizer_steps_ok(const char* what, const OptimTensor* tensors, int count) {
+    for (int i = 0; i < count; ++i) {
+        if (tensors[i].step_ptr == nullptr) {
+            char msg[160];
+            snprintf(msg, sizeof(msg), "%s: tensor %d has no step counter (step_ptr is NULL)", what, i);
+            set_last_error_msg(msg);
+            return false;
+        }
+    }
+    return true;
+}
+
+int cbnb_b200_optimizer_update_32bit_multi_dev(int optimizer, int dtype, const OptimTensor* tensors, int count,
+                                               float beta1, float beta2, float beta3, float alpha, float eps,
+                                               float weight_decay, float lr, const float* lr_dev, float gnorm_scale,
+                                               bool skip_zeros, cudaStream_t stream) {
+    const char* what = "optimizer_update_32bit_multi_dev";
+    if (!optimizer_list_ok(what, optimizer, dtype, tensors, count) || !optimizer_steps_ok(what, tensors, count))
+        return 100;
+    launch_optimizer32bit_list_dev(optimizer, dtype, tensors, count, beta1, beta2, beta3, alpha, eps, weight_decay, lr,
+                                   lr_dev, gnorm_scale, skip_zeros, stream);
+    return 0;
+}
+
+int cbnb_b200_optimizer_update_8bit_blockwise_multi_dev(int optimizer, int dtype, const OptimTensor* tensors, int count,
+                                                        float beta1, float beta2, float beta3, float alpha, float eps,
+                                                        float weight_decay, float lr, const float* lr_dev,
+                                                        const float* quantiles1, const float* quantiles2,
+                                                        float gnorm_scale, bool skip_zeros, cudaStream_t stream) {
+    const char* what = "optimizer_update_8bit_blockwise_multi_dev";
+    if (!optimizer_list_ok(what, optimizer, dtype, tensors, count) || !optimizer_steps_ok(what, tensors, count))
+        return 100;
+    launch_optimizer8bit_blockwise_list_dev(optimizer, dtype, tensors, count, beta1, beta2, beta3, alpha, eps,
+                                            weight_decay, lr, lr_dev, quantiles1, quantiles2, gnorm_scale, skip_zeros,
+                                            stream);
     return 0;
 }
 

@@ -11,6 +11,7 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
+#include <stddef.h>
 #include <stdint.h>
 
 namespace bnb200 {
@@ -223,9 +224,15 @@ struct OptimTensor {
     float* absmax1;   // 8-bit state only
     float* absmax2;
     long long n;      // elements of p
-    int step;         // this tensor's own step (1 on its first update)
-    int reserved;
+    union {
+        struct {
+            int step;     // this tensor's own step (1 on its first update)
+            int reserved;
+        };
+        int* step_ptr;    // the capturable (_dev) entries: the step counter in device memory, advanced by the call
+    };
 };
 static_assert(sizeof(OptimTensor) == 64, "bnb_b200_optim_tensor_t is 64 bytes");
+static_assert(offsetof(OptimTensor, step) == 56 && offsetof(OptimTensor, step_ptr) == 56, "step union at offset 56");
 
 } // namespace bnb200

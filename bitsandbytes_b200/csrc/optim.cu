@@ -51,6 +51,13 @@ template <typename T> __device__ __forceinline__ float widen(T v) { return DT<T>
 // -- 256-element blocks (8-bit state) or kOpt32Chunk-element chunks (32-bit state) -- are numbered across the list:
 // start[i] items come before tensor i, start[count] is the total, and a warp (8-bit) or CTA (32-bit) finds the tensor
 // of its item by binary search.  Everything but the tensor's pointers, size and step is per launch.
+//
+// Capturable instances (DEV = true, the _dev entries): each descriptor carries a pointer to the tensor's step counter
+// in device memory instead of the step, and the learning rate may come from a device pointer (lr_dev; NULL: s.lr), so
+// a CUDA graph that captured the launch reads the current values at every replay.  The counters are advanced by
+// optim_step_increment_kernel, launched just before the update on the same stream: the update kernel cannot do it,
+// since other warps and CTAs of the tensor read the step.  The arithmetic is that of the DEV = false instances, on the
+// same values, so the results are the same bits.
 constexpr int kKernelParamBytes = 32764;
 constexpr int kScalarParamBytes = 128;  // the other kernel parameters (checked below)
 constexpr int kOptimListCap = (kKernelParamBytes - kScalarParamBytes - 16) / (sizeof(OptimTensor) + sizeof(long long));
@@ -67,7 +74,21 @@ struct OptimScalars {
     float beta1, beta2, beta3, alpha, eps, weight_decay, lr, gnorm_scale;
     bool skip_zeros;
 };
-static_assert(sizeof(OptimScalars) + 4 * sizeof(void*) + 2 * sizeof(float) <= kScalarParamBytes, "");
+static_assert(sizeof(OptimScalars) + 5 * sizeof(void*) + 2 * sizeof(float) <= kScalarParamBytes, "");
+
+// the per-launch learning rate: from device memory in the capturable instances when given
+template <bool DEV> __device__ __forceinline__ float launch_lr(const OptimScalars& s, const float* lr_dev) {
+    return DEV && lr_dev != nullptr ? *lr_dev : s.lr;
+}
+// a descriptor's step: the value (DEV = false) or the device counter it points to
+template <bool DEV> __device__ __forceinline__ int tensor_step(const OptimTensor& d) {
+    return DEV ? *d.step_ptr : d.step;
+}
+
+// ++step of every tensor of a capturable launch, before its update kernel
+__global__ void __launch_bounds__(256) optim_step_increment_kernel(const __grid_constant__ OptimList list) {
+    for (int i = threadIdx.x; i < list.count; i += blockDim.x) atomicAdd(list.t[i].step_ptr, 1);
+}
 
 // the tensor of work item `item`: the last i >= lo with start[i] <= item (tensors without items are skipped)
 __device__ __forceinline__ int find_tensor(const OptimList& L, long long item, int lo) {
@@ -213,13 +234,15 @@ constexpr int kOpt32Chunk = 4096;  // elements per work item of the 32-bit kerne
 // fma, and the vector path is bit-identical to the scalar one (and to the reference); fp32 already moves 128 bytes
 // per warp access.  Otherwise one element per access.  The choice is made per tensor, so a misaligned view in the list
 // does not demote the others.  max_unorm > 0 (LAMB / LARS) takes a list of one: unorm and param_norm belong to it.
-template <typename T, int OPT>
+template <typename T, int OPT, bool DEV>
 __global__ void __launch_bounds__(512) optim32_kernel(const __grid_constant__ OptimList list, const OptimScalars s,
-                                                      const float* unorm, float max_unorm, float param_norm) {
+                                                      const float* unorm, float max_unorm, float param_norm,
+                                                      const float* lr_dev) {
     constexpr bool two = OPT == kAdam || OPT == kAdemamix;
     Opt32Args q;
     q.beta1 = s.beta1, q.beta2 = s.beta2, q.beta3 = s.beta3, q.alpha = s.alpha, q.eps = s.eps;
-    q.weight_decay = s.weight_decay, q.lr = s.lr, q.gnorm_scale = s.gnorm_scale, q.skip_zeros = s.skip_zeros;
+    q.weight_decay = s.weight_decay, q.lr = launch_lr<DEV>(s, lr_dev), q.gnorm_scale = s.gnorm_scale;
+    q.skip_zeros = s.skip_zeros;
     q.update_scale = 1.0f;
     if (max_unorm > 0.0f) {
         const float us = sqrtf(unorm[0]);
@@ -236,7 +259,7 @@ __global__ void __launch_bounds__(512) optim32_kernel(const __grid_constant__ Op
         float* s1 = static_cast<float*>(d.state1);
         float* s2 = static_cast<float*>(d.state2);
         const long n = d.n;
-        q.step = d.step;
+        q.step = tensor_step<DEV>(d);
         q.correction1 = 1.0f - powf(q.beta1, q.step);
         q.correction2 = sqrtf(1.0f - powf(q.beta2, q.step));
         q.step_size = -q.lr * q.correction2 / q.correction1;
@@ -381,7 +404,7 @@ template <typename T> struct Tensor8 {
     int step;
     bool aligned;     // 16-byte p / g and 8-byte state accesses allowed
 
-    __device__ __forceinline__ void load(const OptimList& L, int i) {
+    template <bool DEV> __device__ __forceinline__ void load(const OptimList& L, int i) {
         const OptimTensor& d = L.t[i];
         p = static_cast<T*>(d.p);
         g = static_cast<const T*>(d.g);
@@ -391,17 +414,19 @@ template <typename T> struct Tensor8 {
         absmax2 = d.absmax2;
         n = d.n;
         first = L.start[i];
-        step = d.step;
+        step = tensor_step<DEV>(d);
         aligned = ((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g)) & 15) == 0 &&
                   ((reinterpret_cast<uintptr_t>(state1) | reinterpret_cast<uintptr_t>(state2)) & 7) == 0;
     }
 };
 
 // reference csrc/kernels.cu:914-1150
-template <typename T, int OPT, bool ONE>
+template <typename T, int OPT, bool ONE, bool DEV>
 __global__ void __launch_bounds__(256) optim8_2state_kernel(const __grid_constant__ OptimList list, const OptimScalars s,
-                                                            const float* qmap1, const float* qmap2) {
-    const float beta1 = s.beta1, beta2 = s.beta2, beta3 = s.beta3, alpha = s.alpha, eps = s.eps, lr = s.lr;
+                                                            const float* qmap1, const float* qmap2,
+                                                            const float* lr_dev) {
+    const float beta1 = s.beta1, beta2 = s.beta2, beta3 = s.beta3, alpha = s.alpha, eps = s.eps;
+    const float lr = launch_lr<DEV>(s, lr_dev);
     const float weight_decay = s.weight_decay, gnorm_scale = s.gnorm_scale;
     __shared__ float code1[256];
     __shared__ float code2[256];
@@ -424,7 +449,7 @@ __global__ void __launch_bounds__(256) optim8_2state_kernel(const __grid_constan
     for (long long item = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); item < total; item += warps) {
         ti = ONE ? 0 : find_tensor(list, item, ti);
         Tensor8<T> t;
-        t.load(list, ti);
+        t.template load<DEV>(list, ti);
         const float correction1 = 1.0f - __powf(beta1, t.step);
         const float correction2 = sqrtf(1.0f - __powf(beta2, t.step));
         const float step_size = __fdividef(-lr * correction2, correction1);
@@ -506,10 +531,11 @@ __global__ void __launch_bounds__(256) optim8_2state_kernel(const __grid_constan
 }
 
 // reference csrc/kernels.cu:1152-1325
-template <typename T, int OPT, bool ONE>
+template <typename T, int OPT, bool ONE, bool DEV>
 __global__ void __launch_bounds__(256) optim8_1state_kernel(const __grid_constant__ OptimList list, const OptimScalars s,
-                                                            const float* qmap1) {
-    const float beta1 = s.beta1, beta2 = s.beta2, eps = s.eps, lr = s.lr, weight_decay = s.weight_decay;
+                                                            const float* qmap1, const float* lr_dev) {
+    const float beta1 = s.beta1, beta2 = s.beta2, eps = s.eps, weight_decay = s.weight_decay;
+    const float lr = launch_lr<DEV>(s, lr_dev);
     const float gnorm_scale = s.gnorm_scale;
     const bool skip_zeros = s.skip_zeros;
     __shared__ float code1[256];
@@ -528,7 +554,7 @@ __global__ void __launch_bounds__(256) optim8_1state_kernel(const __grid_constan
     for (long long item = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); item < total; item += warps) {
         ti = ONE ? 0 : find_tensor(list, item, ti);
         Tensor8<T> t;
-        t.load(list, ti);
+        t.template load<DEV>(list, ti);
         T* p = t.p;
         const T* g = t.g;
         unsigned char* state1 = t.state1;
@@ -627,14 +653,24 @@ long long make_list(OptimList& L, const OptimTensor* ts, int count, long long pe
     return total;
 }
 
+// The step counters of a capturable launch (dev): advanced before the update, also those of empty tensors, as the
+// eager optimizer advances every step it updates.
+void increment_steps(const OptimList& L, bool dev, cudaStream_t stream) {
+    if (dev && L.count > 0) optim_step_increment_kernel<<<1, 256, 0, stream>>>(L);
+}
+
 // count <= kOptimListCap; unorm / max_unorm / param_norm: the LAMB / LARS trust ratio of a list of one (max_unorm = 0
-// otherwise)
+// otherwise); dev: the descriptors carry step pointers and lr_dev (if not NULL) replaces s.lr
 template <typename T, int OPT>
 void run32(const OptimTensor* ts, int count, const OptimScalars& s, float* unorm, float max_unorm, float param_norm,
-           cudaStream_t stream) {
+           bool dev, const float* lr_dev, cudaStream_t stream) {
     OptimList L;
     const long long chunks = make_list(L, ts, count, kOpt32Chunk);
-    if (chunks == 0) return;
+    increment_steps(L, dev, stream);
+    if (chunks == 0) {
+        BNB200_CHECK_LAUNCH("optimizer32bit");
+        return;
+    }
     const int grid = grid_for(chunks, 1);
     const bool trust = max_unorm > 0.0f && OPT != kAdemamix;
     const T* g = static_cast<const T*>(ts[0].g);
@@ -646,7 +682,10 @@ void run32(const OptimTensor* ts, int count, const OptimScalars& s, float* unorm
         optim32_unorm_kernel<T, OPT><<<grid, 512, 0, stream>>>(g, s1, s2, unorm, s.beta1, s.beta2, s.eps, ts[0].step,
                                                                s.gnorm_scale, ts[0].n);
     }
-    optim32_kernel<T, OPT><<<grid, 512, 0, stream>>>(L, s, unorm, max_unorm, param_norm);
+    if (dev)
+        optim32_kernel<T, OPT, true><<<grid, 512, 0, stream>>>(L, s, unorm, max_unorm, param_norm, lr_dev);
+    else
+        optim32_kernel<T, OPT, false><<<grid, 512, 0, stream>>>(L, s, unorm, max_unorm, param_norm, nullptr);
     if (trust && OPT == kLion) {
         cudaMemsetAsync(unorm, 0, sizeof(float), stream);
         optim32_unorm_kernel<T, OPT><<<grid, 512, 0, stream>>>(g, s1, s2, unorm, s.beta1, s.beta2, s.eps, ts[0].step,
@@ -655,33 +694,42 @@ void run32(const OptimTensor* ts, int count, const OptimScalars& s, float* unorm
     BNB200_CHECK_LAUNCH("optimizer32bit");
 }
 
+// dev: as run32 (the capturable instances take any count: they are not specialised for a list of one)
 template <typename T, int OPT>
-void run8(const OptimTensor* ts, int count, const OptimScalars& s, const float* qmap1, const float* qmap2,
-          cudaStream_t stream) {
+void run8(const OptimTensor* ts, int count, const OptimScalars& s, const float* qmap1, const float* qmap2, bool dev,
+          const float* lr_dev, cudaStream_t stream) {
     OptimList L;
     const long long n_blocks = make_list(L, ts, count, kOptBlock);
-    if (n_blocks == 0) return;
+    increment_steps(L, dev, stream);
+    if (n_blocks == 0) {
+        BNB200_CHECK_LAUNCH("optimizer8bit_blockwise");
+        return;
+    }
     const int grid = grid_for(n_blocks, 8);
     if constexpr (OPT == kAdam || OPT == kAdemamix) {
-        if (count == 1)
-            optim8_2state_kernel<T, OPT, true><<<grid, 256, 0, stream>>>(L, s, qmap1, qmap2);
+        if (dev)
+            optim8_2state_kernel<T, OPT, false, true><<<grid, 256, 0, stream>>>(L, s, qmap1, qmap2, lr_dev);
+        else if (count == 1)
+            optim8_2state_kernel<T, OPT, true, false><<<grid, 256, 0, stream>>>(L, s, qmap1, qmap2, nullptr);
         else
-            optim8_2state_kernel<T, OPT, false><<<grid, 256, 0, stream>>>(L, s, qmap1, qmap2);
+            optim8_2state_kernel<T, OPT, false, false><<<grid, 256, 0, stream>>>(L, s, qmap1, qmap2, nullptr);
     } else {
-        if (count == 1)
-            optim8_1state_kernel<T, OPT, true><<<grid, 256, 0, stream>>>(L, s, qmap1);
+        if (dev)
+            optim8_1state_kernel<T, OPT, false, true><<<grid, 256, 0, stream>>>(L, s, qmap1, lr_dev);
+        else if (count == 1)
+            optim8_1state_kernel<T, OPT, true, false><<<grid, 256, 0, stream>>>(L, s, qmap1, nullptr);
         else
-            optim8_1state_kernel<T, OPT, false><<<grid, 256, 0, stream>>>(L, s, qmap1);
+            optim8_1state_kernel<T, OPT, false, false><<<grid, 256, 0, stream>>>(L, s, qmap1, nullptr);
     }
     BNB200_CHECK_LAUNCH("optimizer8bit_blockwise");
 }
 
 template <typename T>
 bool dispatch32(int opt, const OptimTensor* ts, int count, const OptimScalars& s, float* unorm, float max_unorm,
-                float param_norm, cudaStream_t st) {
+                float param_norm, bool dev, const float* lr_dev, cudaStream_t st) {
 #define BNB200_O32(ID)                                                                                                 \
     case ID:                                                                                                           \
-        run32<T, ID>(ts, count, s, unorm, max_unorm, param_norm, st);                                                  \
+        run32<T, ID>(ts, count, s, unorm, max_unorm, param_norm, dev, lr_dev, st);                                     \
         return true;
     switch (opt) {
         BNB200_O32(kAdam)
@@ -697,10 +745,10 @@ bool dispatch32(int opt, const OptimTensor* ts, int count, const OptimScalars& s
 
 template <typename T>
 bool dispatch8(int opt, const OptimTensor* ts, int count, const OptimScalars& s, const float* q1, const float* q2,
-               cudaStream_t st) {
+               bool dev, const float* lr_dev, cudaStream_t st) {
 #define BNB200_O8(ID)                                                                                                  \
     case ID:                                                                                                           \
-        run8<T, ID>(ts, count, s, q1, q2, st);                                                                         \
+        run8<T, ID>(ts, count, s, q1, q2, dev, lr_dev, st);                                                            \
         return true;
     switch (opt) {
         BNB200_O8(kAdam)
@@ -715,21 +763,21 @@ bool dispatch8(int opt, const OptimTensor* ts, int count, const OptimScalars& s,
 }
 
 bool list32(int opt, int dtype, const OptimTensor* ts, int count, const OptimScalars& s, float* unorm, float max_unorm,
-            float param_norm, cudaStream_t st) {
+            float param_norm, bool dev, const float* lr_dev, cudaStream_t st) {
     switch (dtype) {
-    case 0: return dispatch32<float>(opt, ts, count, s, unorm, max_unorm, param_norm, st);
-    case 1: return dispatch32<__half>(opt, ts, count, s, unorm, max_unorm, param_norm, st);
-    case 2: return dispatch32<__nv_bfloat16>(opt, ts, count, s, unorm, max_unorm, param_norm, st);
+    case 0: return dispatch32<float>(opt, ts, count, s, unorm, max_unorm, param_norm, dev, lr_dev, st);
+    case 1: return dispatch32<__half>(opt, ts, count, s, unorm, max_unorm, param_norm, dev, lr_dev, st);
+    case 2: return dispatch32<__nv_bfloat16>(opt, ts, count, s, unorm, max_unorm, param_norm, dev, lr_dev, st);
     }
     return false;
 }
 
 bool list8(int opt, int dtype, const OptimTensor* ts, int count, const OptimScalars& s, const float* q1, const float* q2,
-           cudaStream_t st) {
+           bool dev, const float* lr_dev, cudaStream_t st) {
     switch (dtype) {
-    case 0: return dispatch8<float>(opt, ts, count, s, q1, q2, st);
-    case 1: return dispatch8<__half>(opt, ts, count, s, q1, q2, st);
-    case 2: return dispatch8<__nv_bfloat16>(opt, ts, count, s, q1, q2, st);
+    case 0: return dispatch8<float>(opt, ts, count, s, q1, q2, dev, lr_dev, st);
+    case 1: return dispatch8<__half>(opt, ts, count, s, q1, q2, dev, lr_dev, st);
+    case 2: return dispatch8<__nv_bfloat16>(opt, ts, count, s, q1, q2, dev, lr_dev, st);
     }
     return false;
 }
@@ -749,7 +797,7 @@ bool launch_optimizer32bit(int opt, int dtype, const void* g, void* p, float* s1
                            cudaStream_t st) {
     const OptimTensor t = one_tensor(p, g, s1, s2, nullptr, nullptr, n, step);
     const OptimScalars s{beta1, beta2, beta3, alpha, eps, wd, lr, gnorm_scale, skip_zeros};
-    return list32(opt, dtype, &t, 1, s, unorm, max_unorm, param_norm, st);
+    return list32(opt, dtype, &t, 1, s, unorm, max_unorm, param_norm, false, nullptr, st);
 }
 
 bool launch_optimizer8bit_blockwise(int opt, int dtype, void* p, const void* g, unsigned char* s1, unsigned char* s2,
@@ -758,7 +806,7 @@ bool launch_optimizer8bit_blockwise(int opt, int dtype, void* p, const void* g, 
                                     float gnorm_scale, bool skip_zeros, long n, cudaStream_t st) {
     const OptimTensor t = one_tensor(p, g, s1, s2, a1, a2, n, step);
     const OptimScalars s{beta1, beta2, beta3, alpha, eps, wd, lr, gnorm_scale, skip_zeros};
-    return list8(opt, dtype, &t, 1, s, q1, q2, st);
+    return list8(opt, dtype, &t, 1, s, q1, q2, false, nullptr, st);
 }
 
 // count <= optimizer_list_capacity(): one launch
@@ -766,14 +814,30 @@ bool launch_optimizer32bit_list(int opt, int dtype, const OptimTensor* ts, int c
                                 float beta3, float alpha, float eps, float wd, float lr, float gnorm_scale,
                                 bool skip_zeros, cudaStream_t st) {
     const OptimScalars s{beta1, beta2, beta3, alpha, eps, wd, lr, gnorm_scale, skip_zeros};
-    return list32(opt, dtype, ts, count, s, nullptr, 0.0f, 0.0f, st);
+    return list32(opt, dtype, ts, count, s, nullptr, 0.0f, 0.0f, false, nullptr, st);
+}
+
+// the capturable list: step pointers in the descriptors, lr_dev (NULL: lr) read by the kernel
+bool launch_optimizer32bit_list_dev(int opt, int dtype, const OptimTensor* ts, int count, float beta1, float beta2,
+                                    float beta3, float alpha, float eps, float wd, float lr, const float* lr_dev,
+                                    float gnorm_scale, bool skip_zeros, cudaStream_t st) {
+    const OptimScalars s{beta1, beta2, beta3, alpha, eps, wd, lr, gnorm_scale, skip_zeros};
+    return list32(opt, dtype, ts, count, s, nullptr, 0.0f, 0.0f, true, lr_dev, st);
 }
 
 bool launch_optimizer8bit_blockwise_list(int opt, int dtype, const OptimTensor* ts, int count, float beta1, float beta2,
                                          float beta3, float alpha, float eps, float wd, float lr, const float* q1,
                                          const float* q2, float gnorm_scale, bool skip_zeros, cudaStream_t st) {
     const OptimScalars s{beta1, beta2, beta3, alpha, eps, wd, lr, gnorm_scale, skip_zeros};
-    return list8(opt, dtype, ts, count, s, q1, q2, st);
+    return list8(opt, dtype, ts, count, s, q1, q2, false, nullptr, st);
+}
+
+bool launch_optimizer8bit_blockwise_list_dev(int opt, int dtype, const OptimTensor* ts, int count, float beta1,
+                                             float beta2, float beta3, float alpha, float eps, float wd, float lr,
+                                             const float* lr_dev, const float* q1, const float* q2, float gnorm_scale,
+                                             bool skip_zeros, cudaStream_t st) {
+    const OptimScalars s{beta1, beta2, beta3, alpha, eps, wd, lr, gnorm_scale, skip_zeros};
+    return list8(opt, dtype, ts, count, s, q1, q2, true, lr_dev, st);
 }
 
 } // namespace bnb200

@@ -14,7 +14,7 @@ from __future__ import annotations
 
 import ctypes as ct
 import itertools
-from typing import Any, Optional, Sequence
+from typing import Any, Optional, Sequence, Union
 
 import torch
 from torch import Tensor
@@ -511,7 +511,7 @@ def optimizer_update_8bit_blockwise(optimizer_name: str, g: Tensor, p: Tensor, s
 
 
 def optimizer_update_32bit_multi(optimizer_name: str, g: Sequence[Tensor], p: Sequence[Tensor], state1: Sequence[Tensor],
-                                 beta1: float, eps: float, step: Sequence[int], lr: float,
+                                 beta1: float, eps: float, step: Sequence[Union[int, Tensor]], lr: Union[float, Tensor],
                                  state2: Optional[Sequence[Tensor]] = None, beta2: float = 0.0, beta3: float = 0.0,
                                  alpha: float = 0.0, weight_decay: float = 0.0, gnorm_scale: float = 1.0,
                                  skip_zeros=False) -> None:
@@ -519,21 +519,26 @@ def optimizer_update_32bit_multi(optimizer_name: str, g: Sequence[Tensor], p: Se
     ``backends.cuda.optimizer_multi_capacity()`` parameters instead of one per parameter, with the same results bit
     for bit.  g, p, state1, step (and state2 for adam / ademamix) list one entry per parameter; every other argument is
     shared.  All tensors on one GPU (paged state allowed); no trust ratio (max_unorm: LAMB / LARS take the
-    single-tensor call)."""
+    single-tensor call).
+
+    Capturable form: when ``step`` lists one-element int32 CUDA tensors, one per parameter, the call advances each by
+    one on the GPU and updates with the advanced steps, and ``lr`` may be a one-element float32 CUDA tensor.  The call
+    then reads nothing on the host, so a CUDA graph that captured it uses the current steps and ``lr`` at every replay.
+    The results are those of the integer form given the same steps and ``lr``, bit for bit."""
     _cuda_backend.optimizer_update_32bit_multi(optimizer_name, g, p, state1, state2, beta1, beta2, beta3, alpha, eps,
                                                weight_decay, step, lr, gnorm_scale, skip_zeros)
 
 
 def optimizer_update_8bit_blockwise_multi(optimizer_name: str, g: Sequence[Tensor], p: Sequence[Tensor],
                                           state1: Sequence[Tensor], state2: Optional[Sequence[Tensor]], beta1: float,
-                                          beta2: float, beta3: float, alpha: float, eps: float, step: Sequence[int],
-                                          lr: float, qmap1: Tensor, qmap2: Optional[Tensor], absmax1: Sequence[Tensor],
+                                          beta2: float, beta3: float, alpha: float, eps: float,
+                                          step: Sequence[Union[int, Tensor]], lr: Union[float, Tensor], qmap1: Tensor, qmap2: Optional[Tensor], absmax1: Sequence[Tensor],
                                           absmax2: Optional[Sequence[Tensor]], weight_decay: float = 0.0,
                                           gnorm_scale: float = 1.0, skip_zeros=False) -> None:
     """``optimizer_update_8bit_blockwise`` for several parameters at once: one kernel launch per
     ``backends.cuda.optimizer_multi_capacity()`` parameters instead of one per parameter, with the same results bit
     for bit.  g, p, state1, absmax1, step (and state2 / absmax2 for adam / ademamix) list one entry per parameter; the
-    code books and every other argument are shared."""
+    code books and every other argument are shared.  Device steps and ``lr``: as ``optimizer_update_32bit_multi``."""
     _cuda_backend.optimizer_update_8bit_blockwise_multi(optimizer_name, g, p, state1, state2, beta1, beta2, beta3, alpha,
                                                         eps, step, lr, qmap1, qmap2, absmax1, absmax2, weight_decay,
                                                         gnorm_scale, skip_zeros)

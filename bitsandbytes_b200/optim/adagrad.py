@@ -17,22 +17,25 @@ def _check(lr, weight_decay, eps, initial_accumulator_value, lr_decay):
 
 class Adagrad(Optimizer1State):
     def __init__(self, params, lr=1e-2, lr_decay=0, weight_decay=0, initial_accumulator_value=0, eps=1e-10, optim_bits=32,
-                 args=None, min_8bit_size=4096):
+                 args=None, min_8bit_size=4096, capturable=False):
         _check(lr, weight_decay, eps, initial_accumulator_value, lr_decay)
-        super().__init__("adagrad", params, lr, (0.0, 0.0), eps, weight_decay, optim_bits, args, min_8bit_size)
+        super().__init__("adagrad", params, lr, (0.0, 0.0), eps, weight_decay, optim_bits, args, min_8bit_size,
+                         capturable=capturable)
 
 
 class Adagrad8bit(Optimizer1State):
     def __init__(self, params, lr=1e-2, lr_decay=0, weight_decay=0, initial_accumulator_value=0, eps=1e-10, optim_bits=8,
-                 args=None, min_8bit_size=4096):
+                 args=None, min_8bit_size=4096, capturable=False):
         _check(lr, weight_decay, eps, initial_accumulator_value, lr_decay)
         if optim_bits != 8:
             raise ValueError("Adagrad8bit only supports optim_bits=8 (default value for compatibility)")
-        super().__init__("adagrad", params, lr, (0.0, 0.0), eps, weight_decay, 8, args, min_8bit_size)
+        super().__init__("adagrad", params, lr, (0.0, 0.0), eps, weight_decay, 8, args, min_8bit_size,
+                         capturable=capturable)
 
 
 class Adagrad32bit(Optimizer1State):
     def __init__(self, params, lr=1e-2, lr_decay=0, weight_decay=0, initial_accumulator_value=0, eps=1e-10, optim_bits=32,
-                 args=None, min_8bit_size=4096):
+                 args=None, min_8bit_size=4096, capturable=False):
         _check(lr, weight_decay, eps, initial_accumulator_value, lr_decay)
-        super().__init__("adagrad", params, lr, (0.0, 0.0), eps, weight_decay, 32, args, min_8bit_size)
+        super().__init__("adagrad", params, lr, (0.0, 0.0), eps, weight_decay, 32, args, min_8bit_size,
+                         capturable=capturable)

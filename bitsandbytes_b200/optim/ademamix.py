@@ -7,7 +7,7 @@ from typing import Optional
 import torch
 
 from .. import functional as F
-from .optimizer import Optimizer2State, _Update
+from .optimizer import _NO_SCHEDULES, Optimizer2State, _Update
 
 
 def _schedules(step, beta1, beta3, alpha, t_alpha, t_beta3):
@@ -65,17 +65,17 @@ class _ReferenceAdEMAMix(torch.optim.Optimizer):
 class AdEMAMix(Optimizer2State):
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999, 0.9999), alpha=5.0, t_alpha: Optional[int] = None,
                  t_beta3: Optional[int] = None, eps=1e-8, weight_decay=1e-2, optim_bits=32, min_8bit_size=4096,
-                 is_paged=False):
+                 is_paged=False, capturable=False):
         super().__init__("ademamix", params=params, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay,
                          optim_bits=optim_bits, args=None, min_8bit_size=min_8bit_size, is_paged=is_paged, alpha=alpha,
-                         t_alpha=t_alpha, t_beta3=t_beta3)
+                         t_alpha=t_alpha, t_beta3=t_beta3, capturable=capturable)
 
     @torch.no_grad()
     def init_state(self, group, p, gindex, pindex):
         config = self.get_config(gindex, pindex, group)
         dtype = self._state_dtype(config, p)
         state = self.state[p]
-        state["step"] = 0
+        state["step"] = self._initial_step(p)
         if dtype == torch.uint8:
             state["qmap1"] = self._qmap("dynamic", p.device)
             state["qmap2"] = self._qmap("udynamic", p.device)
@@ -88,6 +88,8 @@ class AdEMAMix(Optimizer2State):
         u = super()._update_args(group, p, gindex, pindex)
         config = self.get_config(gindex, pindex, group)
         if config["t_alpha"] or config["t_beta3"]:  # the warm-up schedules: scalars of this parameter's step
+            if self.capturable:  # (a per-parameter override: the constructor refuses the group-wide schedules)
+                raise ValueError(_NO_SCHEDULES)
             u.alpha, u.beta3 = _schedules(u.state["step"], u.beta1, u.beta3, config["alpha"], config["t_alpha"],
                                           config["t_beta3"])
         return u
@@ -103,34 +105,40 @@ class AdEMAMix(Optimizer2State):
 
 class AdEMAMix8bit(AdEMAMix):
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999, 0.9999), alpha=5.0, t_alpha: Optional[int] = None,
-                 t_beta3: Optional[int] = None, eps=1e-8, weight_decay=1e-2, min_8bit_size=4096, is_paged=False):
+                 t_beta3: Optional[int] = None, eps=1e-8, weight_decay=1e-2, min_8bit_size=4096, is_paged=False,
+                 capturable=False):
         super().__init__(params, lr=lr, betas=betas, alpha=alpha, t_alpha=t_alpha, t_beta3=t_beta3, eps=eps,
-                         weight_decay=weight_decay, optim_bits=8, min_8bit_size=min_8bit_size, is_paged=is_paged)
+                         weight_decay=weight_decay, optim_bits=8, min_8bit_size=min_8bit_size, is_paged=is_paged,
+                         capturable=capturable)
 
 
 class PagedAdEMAMix8bit(AdEMAMix8bit):
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999, 0.9999), alpha=5.0, t_alpha: Optional[int] = None,
-                 t_beta3: Optional[int] = None, eps=1e-8, weight_decay=1e-2, min_8bit_size=4096):
+                 t_beta3: Optional[int] = None, eps=1e-8, weight_decay=1e-2, min_8bit_size=4096, capturable=False):
         super().__init__(params, lr=lr, betas=betas, alpha=alpha, t_alpha=t_alpha, t_beta3=t_beta3, eps=eps,
-                         weight_decay=weight_decay, min_8bit_size=min_8bit_size, is_paged=True)
+                         weight_decay=weight_decay, min_8bit_size=min_8bit_size, is_paged=True, capturable=capturable)
 
 
 class PagedAdEMAMix(AdEMAMix):
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999, 0.9999), alpha=5.0, t_alpha: Optional[int] = None,
-                 t_beta3: Optional[int] = None, eps=1e-8, weight_decay=1e-2, optim_bits=32, min_8bit_size=4096):
+                 t_beta3: Optional[int] = None, eps=1e-8, weight_decay=1e-2, optim_bits=32, min_8bit_size=4096,
+                 capturable=False):
         super().__init__(params, lr=lr, betas=betas, alpha=alpha, t_alpha=t_alpha, t_beta3=t_beta3, eps=eps,
-                         weight_decay=weight_decay, optim_bits=optim_bits, min_8bit_size=min_8bit_size, is_paged=True)
+                         weight_decay=weight_decay, optim_bits=optim_bits, min_8bit_size=min_8bit_size, is_paged=True,
+                         capturable=capturable)
 
 
 class AdEMAMix32bit(AdEMAMix):
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999, 0.9999), alpha=5.0, t_alpha: Optional[int] = None,
-                 t_beta3: Optional[int] = None, eps=1e-8, weight_decay=1e-2, min_8bit_size=4096, is_paged=False):
+                 t_beta3: Optional[int] = None, eps=1e-8, weight_decay=1e-2, min_8bit_size=4096, is_paged=False,
+                 capturable=False):
         super().__init__(params, lr=lr, betas=betas, alpha=alpha, t_alpha=t_alpha, t_beta3=t_beta3, eps=eps,
-                         weight_decay=weight_decay, optim_bits=32, min_8bit_size=min_8bit_size, is_paged=is_paged)
+                         weight_decay=weight_decay, optim_bits=32, min_8bit_size=min_8bit_size, is_paged=is_paged,
+                         capturable=capturable)
 
 
 class PagedAdEMAMix32bit(AdEMAMix32bit):
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999, 0.9999), alpha=5.0, t_alpha: Optional[int] = None,
-                 t_beta3: Optional[int] = None, eps=1e-8, weight_decay=1e-2, min_8bit_size=4096):
+                 t_beta3: Optional[int] = None, eps=1e-8, weight_decay=1e-2, min_8bit_size=4096, capturable=False):
         super().__init__(params, lr=lr, betas=betas, alpha=alpha, t_alpha=t_alpha, t_beta3=t_beta3, eps=eps,
-                         weight_decay=weight_decay, min_8bit_size=min_8bit_size, is_paged=True)
+                         weight_decay=weight_decay, min_8bit_size=min_8bit_size, is_paged=True, capturable=capturable)

@@ -13,26 +13,26 @@ def _need_momentum(momentum):
 
 class LARS(Optimizer1State):
     def __init__(self, params, lr, momentum=0, dampening=0, weight_decay=0, nesterov=False, optim_bits=32, args=None,
-                 min_8bit_size=4096, max_unorm=0.02):
+                 min_8bit_size=4096, max_unorm=0.02, capturable=False):
         _need_momentum(momentum)
         super().__init__("lars", params, lr, (momentum, dampening), 0.0, weight_decay, optim_bits, args, min_8bit_size,
-                         max_unorm=max_unorm)
+                         max_unorm=max_unorm, capturable=capturable)
 
 
 class LARS8bit(Optimizer1State):
     def __init__(self, params, lr, momentum=0, dampening=0, weight_decay=0, nesterov=False, args=None, min_8bit_size=4096,
-                 max_unorm=0.02):
+                 max_unorm=0.02, capturable=False):
         _need_momentum(momentum)
         super().__init__("lars", params, lr, (momentum, dampening), 0.0, weight_decay, 8, args, min_8bit_size,
-                         max_unorm=max_unorm)
+                         max_unorm=max_unorm, capturable=capturable)
 
 
 class LARS32bit(Optimizer1State):
     def __init__(self, params, lr, momentum=0, dampening=0, weight_decay=0, nesterov=False, args=None, min_8bit_size=4096,
-                 max_unorm=0.02):
+                 max_unorm=0.02, capturable=False):
         _need_momentum(momentum)
         super().__init__("lars", params, lr, (momentum, dampening), 0.0, weight_decay, 32, args, min_8bit_size,
-                         max_unorm=max_unorm)
+                         max_unorm=max_unorm, capturable=capturable)
 
 
 class PytorchLARS(Optimizer):

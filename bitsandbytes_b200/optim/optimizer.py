@@ -8,6 +8,10 @@ other.  Unlike the reference, ``step()`` updates all parameters that share their
 (``functional.optimizer_update_32bit_multi`` / ``optimizer_update_8bit_blockwise_multi``, kernels in
 ``csrc/optim.cu``), with the results of one call per parameter bit for bit; ``update_step`` still updates one
 parameter.
+
+``capturable=True`` makes ``step()`` safe to capture in a CUDA graph: every ``state["step"]`` is an int32 counter on the
+parameter's device that the kernels advance, ``group["lr"]`` may be a one-element fp32 CUDA tensor read at every launch,
+and ``step()`` reads nothing on the host.  The results are those of ``capturable=False``, bit for bit.
 """
 from __future__ import annotations
 
@@ -46,11 +50,13 @@ class _Update:
         return self.max_unorm > 0.0 and self.state["state1"].dtype == torch.float32
 
     def group_key(self):
-        """Parameters with equal keys share every per-launch argument of the multi-tensor call."""
+        """Parameters with equal keys share every per-launch argument of the multi-tensor call.  A tensor lr is keyed
+        by identity: the kernel reads it, whatever its value."""
         st = self.state
         eight = st["state1"].dtype == torch.uint8
+        lr = ("tensor", id(self.lr)) if isinstance(self.lr, torch.Tensor) else self.lr
         return (self.p.device, self.p.dtype, eight, self.name, self.beta1, self.beta2, self.beta3, self.alpha, self.eps,
-                self.weight_decay, self.lr, self.skip_zeros,
+                self.weight_decay, lr, self.skip_zeros,
                 id(st["qmap1"]) if eight else None, id(st.get("qmap2")) if eight else None)
 
 
@@ -61,6 +67,17 @@ def group_updates(updates):
     for u in updates:
         groups.setdefault(u.group_key(), []).append(u)
     return list(groups.values())
+
+
+def _capturing() -> bool:
+    """Whether the current CUDA stream is capturing a graph (impossible before CUDA is initialised)."""
+    return torch.cuda.is_initialized() and torch.cuda.is_current_stream_capturing()
+
+
+_NO_TRUST_RATIO = ("capturable=True does not support 32-bit state with max_unorm > 0 (LAMB / LARS): the trust ratio "
+                   "needs the parameter's norm on the host at every step")
+_NO_SCHEDULES = ("capturable=True does not support AdEMAMix's t_alpha / t_beta3: their schedules are computed on the "
+                 "host from the step")
 
 
 class GlobalOptimManager:
@@ -112,11 +129,12 @@ class GlobalOptimManager:
 class Optimizer8bit(torch.optim.Optimizer):
     _FSDP_WRAPPED_QUANT_STATE_KEY = "__bnb_optimizer_quant_state__"
 
-    def __init__(self, params, defaults, optim_bits=32, is_paged=False):
+    def __init__(self, params, defaults, optim_bits=32, is_paged=False, capturable=False):
         super().__init__(params, defaults)
         self.initialized = False
         self.name2qmap = {}
         self.is_paged = is_paged
+        self.capturable = bool(capturable)
         self.page_mng = F.GlobalPageManager.get_instance()
         self.mng = GlobalOptimManager.get_instance()
         # tensors of the state that must keep their dtype when a state dict is loaded
@@ -136,6 +154,8 @@ class Optimizer8bit(torch.optim.Optimizer):
         packed = {}
         for key, param_state in sd["state"].items():  # (torch hands out the live per-parameter dicts: copy, don't pop)
             plain = {k: v for k, v in param_state.items() if k not in self.non_castable_tensor_keys}
+            if isinstance(plain.get("step"), torch.Tensor):  # a capturable optimizer's counter: saved as an int
+                plain["step"] = int(plain["step"].item())
             wrapped = {k: v for k, v in param_state.items() if k in self.non_castable_tensor_keys}
             if wrapped:
                 plain[self._FSDP_WRAPPED_QUANT_STATE_KEY] = wrapped
@@ -193,6 +213,10 @@ class Optimizer8bit(torch.optim.Optimizer):
 
         self.__setstate__({"state": state, "param_groups": [update_group(g, ng) for g, ng in zip(groups, saved_groups)]})
         self._share_qmaps()
+        if self.capturable:
+            for p, st in self.state.items():
+                if "step" in st and isinstance(p, torch.Tensor):
+                    st["step"] = self._initial_step(p, int(st["step"]))
 
     def _share_qmaps(self):
         """A loaded state holds its own copy of the code books in every parameter: point the copies equal to this
@@ -227,6 +251,11 @@ class Optimizer8bit(torch.optim.Optimizer):
 
     @torch.no_grad()
     def step(self, closure=None):
+        capturing = _capturing()
+        if capturing and not self.capturable:
+            raise RuntimeError(f"{type(self).__name__}.step() is being captured in a CUDA graph, but the optimizer was "
+                               "constructed with capturable=False: every replay would repeat this step's step number "
+                               "and learning rate.  Construct it with capturable=True.")
         loss = None
         if closure is not None:
             with torch.enable_grad():
@@ -243,6 +272,9 @@ class Optimizer8bit(torch.optim.Optimizer):
                 if p.grad is None:
                     continue
                 if len(self.state[p]) == 0:
+                    if capturing:
+                        raise RuntimeError(f"{type(self).__name__}.step() would create optimizer state while a CUDA "
+                                           "graph is being captured: run one eager step() before capturing")
                     self.init_state(group, p, gindex, pindex)
                 self.prefetch_state(p)
                 if not multi:
@@ -250,6 +282,8 @@ class Optimizer8bit(torch.optim.Optimizer):
                 else:
                     u = self._update_args(group, p, gindex, pindex)
                     if u.per_parameter():
+                        if self.capturable:
+                            raise ValueError(_NO_TRUST_RATIO)
                         self._launch(u)
                     else:
                         updates.append(u)
@@ -282,7 +316,13 @@ class Optimizer8bit(torch.optim.Optimizer):
     @torch.no_grad()
     def update_step(self, group, p, gindex, pindex):
         """Update one parameter: compute its launch arguments (advancing its step) and launch them."""
-        self._launch(self._update_args(group, p, gindex, pindex))
+        u = self._update_args(group, p, gindex, pindex)
+        if not self.capturable:
+            self._launch(u)
+        elif u.per_parameter():
+            raise ValueError(_NO_TRUST_RATIO)
+        else:
+            self._launch_multi([u])  # (the call advances the device step)
 
     def _update_args(self, group, p, gindex, pindex) -> _Update:
         raise NotImplementedError("The update_step method needs to be overridden")
@@ -294,8 +334,25 @@ class Optimizer8bit(torch.optim.Optimizer):
         if not p.grad.is_contiguous():
             p.grad = p.grad.contiguous()
         state = self.state[p]
-        state["step"] += 1
+        if not self.capturable:  # (a capturable step is advanced on the device by the update call)
+            state["step"] += 1
         return state, self.get_config(gindex, pindex, group)
+
+    def _initial_step(self, p, step=0):
+        """state["step"]: an int, or for capturable=True an int32 counter on the parameter's device."""
+        return torch.tensor([step], dtype=torch.int32, device=p.device) if self.capturable else step
+
+    def _check_capturable(self):
+        """Refuse at construction what needs a host value at every step of a capturable optimizer."""
+        if not self.capturable:
+            return
+        if self.is_paged:
+            raise ValueError("capturable=True does not support paged state: its prefetch and synchronisation cannot be "
+                             "captured in a CUDA graph")
+        if self.args.optim_bits == 32 and self.args.max_unorm > 0.0:
+            raise ValueError(_NO_TRUST_RATIO)
+        if any(g.get("t_alpha") or g.get("t_beta3") for g in self.param_groups):
+            raise ValueError(_NO_SCHEDULES)
 
     def _launch(self, u: _Update):
         st = u.state
@@ -393,20 +450,21 @@ class Optimizer2State(Optimizer8bit):
 
     def __init__(self, optimizer_name, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, optim_bits=32,
                  args=None, min_8bit_size=4096, max_unorm=0.0, skip_zeros=False, is_paged=False, alpha=0.0,
-                 t_alpha: Optional[int] = None, t_beta3: Optional[int] = None):
+                 t_alpha: Optional[int] = None, t_beta3: Optional[int] = None, capturable=False):
         betas = self._validate(lr, eps, betas, weight_decay)
         defaults = dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, alpha=alpha, t_alpha=t_alpha,
                         t_beta3=t_beta3)
-        super().__init__(params, defaults, optim_bits, is_paged)
+        super().__init__(params, defaults, optim_bits, is_paged, capturable)
         self._set_args(args, optim_bits, min_8bit_size, max_unorm, skip_zeros)
         self.optimizer_name = optimizer_name
+        self._check_capturable()
 
     @torch.no_grad()
     def init_state(self, group, p, gindex, pindex):
         config = self.get_config(gindex, pindex, group)
         dtype = self._state_dtype(config, p)
         state = self.state[p]
-        state["step"] = 0
+        state["step"] = self._initial_step(p)
         state["state1"] = self.get_state_buffer(p, dtype=dtype)
         state["state2"] = self.get_state_buffer(p, dtype=dtype)
         if dtype == torch.uint8:
@@ -428,19 +486,20 @@ class Optimizer1State(Optimizer8bit):
     """One moving average per parameter: SGD with momentum / LARS / RMSprop / Adagrad / Lion."""
 
     def __init__(self, optimizer_name, params, lr=1e-3, betas=(0.9, 0.0), eps=1e-8, weight_decay=0.0, optim_bits=32,
-                 args=None, min_8bit_size=4096, max_unorm=0.0, skip_zeros=False, is_paged=False):
+                 args=None, min_8bit_size=4096, max_unorm=0.0, skip_zeros=False, is_paged=False, capturable=False):
         betas = self._validate(lr, eps, betas, weight_decay)
         defaults = dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay)
-        super().__init__(params, defaults, optim_bits, is_paged)
+        super().__init__(params, defaults, optim_bits, is_paged, capturable)
         self._set_args(args, optim_bits, min_8bit_size, max_unorm, skip_zeros)
         self.optimizer_name = optimizer_name
+        self._check_capturable()
 
     @torch.no_grad()
     def init_state(self, group, p, gindex, pindex):
         config = self.get_config(gindex, pindex, group)
         dtype = self._state_dtype(config, p)
         state = self.state[p]
-        state["step"] = 0
+        state["step"] = self._initial_step(p)
         state["state1"] = self.get_state_buffer(p, dtype=dtype)
         if dtype == torch.uint8:
             state["qmap1"] = self._qmap("dynamic", p.device)

@@ -11,20 +11,23 @@ def _check(alpha, centered):
 
 class RMSprop(Optimizer1State):
     def __init__(self, params, lr=1e-2, alpha=0.99, eps=1e-8, weight_decay=0, momentum=0, centered=False, optim_bits=32,
-                 args=None, min_8bit_size=4096):
+                 args=None, min_8bit_size=4096, capturable=False):
         _check(alpha, centered)
-        super().__init__("rmsprop", params, lr, (alpha, momentum), eps, weight_decay, optim_bits, args, min_8bit_size)
+        super().__init__("rmsprop", params, lr, (alpha, momentum), eps, weight_decay, optim_bits, args, min_8bit_size,
+                         capturable=capturable)
 
 
 class RMSprop8bit(Optimizer1State):
     def __init__(self, params, lr=1e-2, alpha=0.99, eps=1e-8, weight_decay=0, momentum=0, centered=False, args=None,
-                 min_8bit_size=4096):
+                 min_8bit_size=4096, capturable=False):
         _check(alpha, centered)
-        super().__init__("rmsprop", params, lr, (alpha, momentum), eps, weight_decay, 8, args, min_8bit_size)
+        super().__init__("rmsprop", params, lr, (alpha, momentum), eps, weight_decay, 8, args, min_8bit_size,
+                         capturable=capturable)
 
 
 class RMSprop32bit(Optimizer1State):
     def __init__(self, params, lr=1e-2, alpha=0.99, eps=1e-8, weight_decay=0, momentum=0, centered=False, args=None,
-                 min_8bit_size=4096):
+                 min_8bit_size=4096, capturable=False):
         _check(alpha, centered)
-        super().__init__("rmsprop", params, lr, (alpha, momentum), eps, weight_decay, 32, args, min_8bit_size)
+        super().__init__("rmsprop", params, lr, (alpha, momentum), eps, weight_decay, 32, args, min_8bit_size,
+                         capturable=capturable)

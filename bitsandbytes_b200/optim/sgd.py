@@ -9,18 +9,23 @@ def _need_momentum(momentum):
 
 class SGD(Optimizer1State):
     def __init__(self, params, lr, momentum=0, dampening=0, weight_decay=0, nesterov=False, optim_bits=32, args=None,
-                 min_8bit_size=4096):
+                 min_8bit_size=4096, capturable=False):
         _need_momentum(momentum)
-        super().__init__("momentum", params, lr, (momentum, dampening), 0.0, weight_decay, optim_bits, args, min_8bit_size)
+        super().__init__("momentum", params, lr, (momentum, dampening), 0.0, weight_decay, optim_bits, args,
+                         min_8bit_size, capturable=capturable)
 
 
 class SGD8bit(Optimizer1State):
-    def __init__(self, params, lr, momentum=0, dampening=0, weight_decay=0, nesterov=False, args=None, min_8bit_size=4096):
+    def __init__(self, params, lr, momentum=0, dampening=0, weight_decay=0, nesterov=False, args=None,
+                 min_8bit_size=4096, capturable=False):
         _need_momentum(momentum)
-        super().__init__("momentum", params, lr, (momentum, dampening), 0.0, weight_decay, 8, args, min_8bit_size)
+        super().__init__("momentum", params, lr, (momentum, dampening), 0.0, weight_decay, 8, args, min_8bit_size,
+                         capturable=capturable)
 
 
 class SGD32bit(Optimizer1State):
-    def __init__(self, params, lr, momentum=0, dampening=0, weight_decay=0, nesterov=False, args=None, min_8bit_size=4096):
+    def __init__(self, params, lr, momentum=0, dampening=0, weight_decay=0, nesterov=False, args=None,
+                 min_8bit_size=4096, capturable=False):
         _need_momentum(momentum)
-        super().__init__("momentum", params, lr, (momentum, dampening), 0.0, weight_decay, 32, args, min_8bit_size)
+        super().__init__("momentum", params, lr, (momentum, dampening), 0.0, weight_decay, 32, args, min_8bit_size,
+                         capturable=capturable)

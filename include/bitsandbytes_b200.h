@@ -269,12 +269,25 @@ typedef struct bnb_b200_optim_tensor {
     float* absmax1;
     float* absmax2;
     long long n;
-    int step;
-    int reserved; /* 0 */
+    union {
+        struct {
+            int step;
+            int reserved; /* 0 */
+        };
+        int* step_ptr; /* the _dev entries only: the tensor's step counter in device memory */
+    };
 } bnb_b200_optim_tensor_t;
 int cbnb_b200_optimizer_multi_capacity(void);
 int cbnb_b200_optimizer_update_32bit_multi(int optimizer, int dtype, const bnb_b200_optim_tensor_t* tensors, int count, float beta1, float beta2, float beta3, float alpha, float eps, float weight_decay, float lr, float gnorm_scale, bool skip_zeros, bnb_stream_t stream);
 int cbnb_b200_optimizer_update_8bit_blockwise_multi(int optimizer, int dtype, const bnb_b200_optim_tensor_t* tensors, int count, float beta1, float beta2, float beta3, float alpha, float eps, float weight_decay, float lr, const float* quantiles1, const float* quantiles2, float gnorm_scale, bool skip_zeros, bnb_stream_t stream);
+/* Capturable multi-tensor steps, for CUDA graphs: as the _multi entries, but each descriptor's step_ptr points to the
+ * tensor's int32 step counter in device memory, and lr_dev, if not NULL, points to an fp32 learning rate in device
+ * memory that is used instead of lr.  Per call, one kernel does ++*step_ptr for every descriptor, then the update
+ * kernel reads the counters and lr_dev, on the same stream: a captured call reads the current values at every replay.
+ * Each descriptor needs its own counter.  The results are those of the _multi entries given the advanced steps and the
+ * learning rate, bit for bit.  Return 0, or 100 with the message set (also for a NULL step_ptr). */
+int cbnb_b200_optimizer_update_32bit_multi_dev(int optimizer, int dtype, const bnb_b200_optim_tensor_t* tensors, int count, float beta1, float beta2, float beta3, float alpha, float eps, float weight_decay, float lr, const float* lr_dev, float gnorm_scale, bool skip_zeros, bnb_stream_t stream);
+int cbnb_b200_optimizer_update_8bit_blockwise_multi_dev(int optimizer, int dtype, const bnb_b200_optim_tensor_t* tensors, int count, float beta1, float beta2, float beta3, float alpha, float eps, float weight_decay, float lr, const float* lr_dev, const float* quantiles1, const float* quantiles2, float gnorm_scale, bool skip_zeros, bnb_stream_t stream);
 
 #ifdef __cplusplus
 }
