@@ -264,6 +264,99 @@ def gemm_4bit_multi_out(A, B, shapeB, absmax, blocksize: int, quant_type: str, b
     return rc == 0
 
 
+def gemm_4bit_partial(A, B, shapeB, absmax, blocksize: int, quant_type: str, absmax_8bit, absmax_code, absmax_offset,
+                      outs, ldc: int) -> bool:
+    """Partial GEMM of a row-sharded layer: ``P[m, n] = sum_k A[m, k] * dequant(B)[n, k]`` in fp32, with no bias and no
+    rounding, stored to every destination in ``outs`` at row stride ``ldc`` (elements).  A destination is an fp32
+    CUDA tensor, checked here, or a raw device address (a peer's symmetric-memory slot), which the caller vouches
+    for.  The kernel and its K split are the ones the plain GEMM takes for this shape (fp32 ``A`` follows
+    :func:`gemm_4bit_dtype_id`), so with one shard the result is the plain GEMM's accumulator.  Returns False when
+    the library does not serve the call (the caller takes another route)."""
+    N, K = shapeB
+    if A.shape[-1] != K:
+        raise RuntimeError(f"A inner dim ({A.shape[-1]}) does not match weight ({K})")
+    M = A.numel() // K if K else 0
+    _check_sizes("gemm_4bit_partial", M, N, K, ldc)
+    if A.dtype not in _DTYPE_ID:
+        raise RuntimeError(f"unsupported dtype {A.dtype}")
+    if absmax.dtype != torch.float32:
+        raise RuntimeError(f"absmax must be float32, got {absmax.dtype}")
+    if quant_type not in _QT_ID:
+        raise RuntimeError(f"quant_type must be nf4 or fp4, got {quant_type}")
+    if blocksize not in _4BIT_BLOCKSIZES:
+        raise RuntimeError(f"invalid blocksize {blocksize}")
+    if (absmax_8bit is None) != (absmax_code is None) or (absmax_8bit is None) != (absmax_offset is None):
+        raise RuntimeError("absmax_8bit, absmax_code and absmax_offset must be given together")
+    if not 1 <= len(outs) <= 8:
+        raise RuntimeError("gemm_4bit_partial: between 1 and 8 destinations")
+    if ldc < N:
+        raise RuntimeError(f"gemm_4bit_partial: ldc ({ldc}) < N ({N})")
+    need = (M - 1) * ldc + N if M > 0 else 0
+    ptrs = []
+    for o in outs:
+        if isinstance(o, torch.Tensor):
+            if o.dtype != torch.float32 or o.device != A.device:
+                raise RuntimeError(f"gemm_4bit_partial: destinations must be float32 on {A.device}, got {o.dtype} on "
+                                   f"{o.device}")
+            if o.untyped_storage().nbytes() // 4 - o.storage_offset() < need:
+                raise RuntimeError(f"gemm_4bit_partial: a destination needs {need} elements from its start")
+            ptrs.append(o.data_ptr())
+        else:
+            ptrs.append(int(o))
+    if M == 0 or N == 0:
+        return True
+    A = A.contiguous()
+    B = B.contiguous()
+    off = absmax_offset.to(dtype=torch.float32).contiguous() if absmax_offset is not None else None
+    arr = (ct.c_void_p * len(ptrs))(*ptrs)
+    with _on_device(A):
+        rc = lib.cbnb_b200_gemm_4bit_partial(
+            A.data_ptr(), B.data_ptr(), absmax.data_ptr(),
+            absmax_8bit.data_ptr() if absmax_8bit is not None else None,
+            absmax_code.data_ptr() if absmax_code is not None else None,
+            off.data_ptr() if off is not None else None,
+            ct.cast(arr, ct.c_void_p), len(ptrs), M, N, K, ldc, blocksize, _QT_ID[quant_type],
+            gemm_4bit_dtype_id(A.dtype), _stream(A))
+    lib.check("gemm_4bit_partial")
+    return rc == 0
+
+
+def reduce_partials(parts: torch.Tensor, dtype: torch.dtype, bias: Optional[torch.Tensor] = None,
+                    out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """``out = dtype((((parts[0] + parts[1]) + ...) + parts[w-1]) + bias)``: the ``[w, M, N]`` fp32 partials of a
+    row-sharded layer summed in rank order in fp32, the bias added in fp32, one rounding.  ``out`` may be a
+    ``[M, N]`` view with unit column stride and any row stride (a column slice of a wider buffer)."""
+    if parts.dtype != torch.float32 or parts.dim() != 3 or not parts.is_cuda:
+        raise RuntimeError(f"reduce_partials: parts must be a [world, M, N] float32 CUDA tensor, got {parts.dtype} "
+                           f"{tuple(parts.shape)} on {parts.device}")
+    if dtype not in _DTYPE_ID:
+        raise RuntimeError(f"reduce_partials: unsupported dtype {dtype}")
+    world, M, N = parts.shape
+    if world < 1:
+        raise RuntimeError("reduce_partials: no partials")
+    parts = parts.contiguous()
+    if bias is not None and (bias.dtype != dtype or bias.shape != (N,) or bias.device != parts.device):
+        raise RuntimeError(f"reduce_partials: bias must be {dtype} [{N}] on {parts.device}")
+    if bias is not None:
+        bias = bias.contiguous()
+    if out is None:
+        out = torch.empty((M, N), dtype=dtype, device=parts.device)
+    elif (out.dtype != dtype or out.shape != (M, N) or out.device != parts.device
+          or (M > 1 and out.stride(1) != 1) or out.stride(0) < N):
+        raise RuntimeError(f"reduce_partials: out must be {dtype} [{M}, {N}] with unit column stride on {parts.device}")
+    _check_sizes("reduce_partials", M, N, out.stride(0), world)
+    if M == 0 or N == 0:
+        return out
+    with _on_device(parts):
+        rc = lib.cbnb_b200_reduce_partials(parts.data_ptr(), world, M * N, out.data_ptr(),
+                                           bias.data_ptr() if bias is not None else None, M, N, out.stride(0),
+                                           _DTYPE_ID[dtype], _stream(parts))
+    lib.check("reduce_partials")
+    if rc != 0:
+        raise RuntimeError(f"reduce_partials: the library refused the call (code {rc})")
+    return out
+
+
 @kernel("gemm_4bit")
 def _gemm_4bit(A, B, shapeB, absmax, blocksize: int, quant_type: str, bias=None, absmax_8bit=None, absmax_code=None,
                absmax_offset=None):

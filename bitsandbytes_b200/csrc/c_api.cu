@@ -47,24 +47,29 @@ bool launch_optimizer8bit_blockwise_list_dev(int opt, int dtype, const OptimTens
                                              const float* lr_dev, const float* q1, const float* q2, float gnorm_scale,
                                              bool skip_zeros, cudaStream_t st);
 
-template <typename T>
+// PART = true: the partial instances (fp32 accumulators to every destination of a PartialOuts, no bias, no rounding)
+template <typename T, bool PART = false>
 void launch_gemv4_simt(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
                        const float* absmax_code, const float* absmax_offset, const float* lut16, int quant_type,
-                       T* out, const T* bias, int M, int N, int K, int ldc, int blocksize, cudaStream_t stream);
-template <typename T>
+                       typename OutArg<T, PART>::type out, const T* bias, int M, int N, int K, int ldc, int blocksize,
+                       cudaStream_t stream);
+template <typename T, bool PART = false>
 bool launch_gemv4_mma(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
-                      const float* absmax_code, const float* absmax_offset, T* out, const T* bias, int M, int N, int K,
-                      int ldc, int blocksize, int quant_type, cudaStream_t stream);
-template <typename T>
+                      const float* absmax_code, const float* absmax_offset, typename OutArg<T, PART>::type out,
+                      const T* bias, int M, int N, int K, int ldc, int blocksize, int quant_type, cudaStream_t stream);
+template <typename T, bool PART = false>
 bool launch_gemm4_tc(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
-                     const float* absmax_code, const float* absmax_offset, T* out, const T* bias, int M, int N, int K,
-                     int ldc, int blocksize, int quant_type, cudaStream_t stream, void* const* peers = nullptr,
-                     int n_peers = 0, int mt_override = 0, int force_splits = 0);
-template <typename T>
+                     const float* absmax_code, const float* absmax_offset, typename OutArg<T, PART>::type out,
+                     const T* bias, int M, int N, int K, int ldc, int blocksize, int quant_type, cudaStream_t stream,
+                     void* const* peers = nullptr, int n_peers = 0, int mt_override = 0, int force_splits = 0);
+template <typename T, bool PART = false>
 bool launch_gemm4_staged(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
-                         const float* absmax_code, const float* absmax_offset, T* out, const T* bias, int M, int N,
-                         int K, int ldc, int blocksize, int quant_type, cudaStream_t stream, void* const* peers,
-                         int n_peers, int mt_override, int panel_rows);
+                         const float* absmax_code, const float* absmax_offset, typename OutArg<T, PART>::type out,
+                         const T* bias, int M, int N, int K, int ldc, int blocksize, int quant_type,
+                         cudaStream_t stream, void* const* peers, int n_peers, int mt_override, int panel_rows);
+// partials.cu
+bool launch_reduce_partials(const float* parts, int world, long long part_stride, void* out, const void* bias, int M,
+                            int N, int ldc, int dtype, cudaStream_t stream);
 template <typename T>
 bool launch_gemm_decoded(const T* A, const T* W, T* out, const T* bias, int M, int N, int K, int ldc, int mt,
                          cudaStream_t stream);
@@ -251,10 +256,12 @@ static bool staged_route(int M, int N, int K, int blocksize, int dtype) {
     return staged_waves > 0 && tiles >= sms && staged_waves <= (tiles + sms - 1) / sms;
 }
 
-template <typename T>
+// PART: the partial form (cbnb_b200_gemm_4bit_partial), the same kernel choice with the partial instances
+template <typename T, bool PART = false>
 static void gemm_4bit_dispatch(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
-                               const float* absmax_code, const float* absmax_offset, T* out, const T* bias, int M,
-                               int N, int K, int ldc, int blocksize, int quant_type, int dtype, cudaStream_t stream) {
+                               const float* absmax_code, const float* absmax_offset,
+                               typename OutArg<T, PART>::type out, const T* bias, int M, int N, int K, int ldc,
+                               int blocksize, int quant_type, int dtype, cudaStream_t stream) {
     if (M <= 0 || N <= 0) return;
     if (quant_type != kFP4 && quant_type != kNF4) {
         set_last_error_msg("gemm_4bit: quant_type must be 1 (FP4) or 2 (NF4)");
@@ -263,29 +270,29 @@ static void gemm_4bit_dispatch(const T* A, const uint8_t* B, const float* absmax
     const int path = choose_path(M, N, K, blocksize, dtype);
     if (path == 1 && staged_route(M, N, K, blocksize, dtype)) {
         if constexpr (!std::is_same<T, float>::value) {
-            if (launch_gemm4_staged<T>(A, B, absmax, absmax_8bit, absmax_code, absmax_offset, out, bias, M, N, K, ldc,
-                                       blocksize, quant_type, stream, nullptr, 0, 0, 0))
+            if (launch_gemm4_staged<T, PART>(A, B, absmax, absmax_8bit, absmax_code, absmax_offset, out, bias, M, N, K,
+                                             ldc, blocksize, quant_type, stream, nullptr, 0, 0, 0))
                 return;
         }
     }
     if (path == 3) {
         if constexpr (!std::is_same<T, float>::value) {
-            if (launch_gemv4_mma<T>(A, B, absmax, absmax_8bit, absmax_code, absmax_offset, out, bias, M, N, K, ldc,
-                                    blocksize, quant_type, stream))
+            if (launch_gemv4_mma<T, PART>(A, B, absmax, absmax_8bit, absmax_code, absmax_offset, out, bias, M, N, K,
+                                          ldc, blocksize, quant_type, stream))
                 return;
-            if (launch_gemm4_tc<T>(A, B, absmax, absmax_8bit, absmax_code, absmax_offset, out, bias, M, N, K, ldc,
-                                   blocksize, quant_type, stream))
+            if (launch_gemm4_tc<T, PART>(A, B, absmax, absmax_8bit, absmax_code, absmax_offset, out, bias, M, N, K,
+                                         ldc, blocksize, quant_type, stream))
                 return;
         }
     }
     if (path == 1) {
         // (fp32 takes path 1 only as dtype 3: the TF32 instance)
-        if (launch_gemm4_tc<T>(A, B, absmax, absmax_8bit, absmax_code, absmax_offset, out, bias, M, N, K, ldc,
-                               blocksize, quant_type, stream))
+        if (launch_gemm4_tc<T, PART>(A, B, absmax, absmax_8bit, absmax_code, absmax_offset, out, bias, M, N, K, ldc,
+                                     blocksize, quant_type, stream))
             return;
     }
-    launch_gemv4_simt<T>(A, B, absmax, absmax_8bit, absmax_code, absmax_offset, nullptr, quant_type, out, bias, M, N,
-                         K, ldc, blocksize, stream);
+    launch_gemv4_simt<T, PART>(A, B, absmax, absmax_8bit, absmax_code, absmax_offset, nullptr, quant_type, out, bias,
+                               M, N, K, ldc, blocksize, stream);
 }
 
 } // namespace bnb200
@@ -433,6 +440,43 @@ int cbnb_b200_gemm_4bit_multi_out(const void* A, const uint8_t* B, const float* 
                                             absmax_offset, (__nv_bfloat16*)outs[0], (const __nv_bfloat16*)bias, M, N, K,
                                             ldc, blocksize, quant_type, stream, outs + 1, n_outs - 1);
     return ok ? 0 : 100;
+}
+
+// Partial GEMM of a row-sharded layer: outs[0..n_outs)[m, n] (row stride ldc, fp32) = the fp32 sum over k of
+// A[m, k] * W[n, k], with no bias and no rounding, computed by the kernel (and the K split) that the plain call of the
+// same shape takes.  outs is a host array of device addresses (local buffers, or peers' mapped buffers).  Returns 0,
+// 1 for a bad destination list, or 100 for a dtype the entry does not serve.
+int cbnb_b200_gemm_4bit_partial(const void* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
+                                const float* absmax_code, const float* absmax_offset, float* const* outs, int n_outs,
+                                int M, int N, int K, int ldc, int blocksize, int quant_type, int dtype,
+                                cudaStream_t stream) {
+    if (n_outs < 1 || n_outs > kMaxPartialOuts || outs == nullptr) {
+        set_last_error_msg("gemm_4bit_partial: 1 <= n_outs <= 8");
+        return 1;
+    }
+    if (dtype < 0 || dtype > 3) return 100;
+    PartialOuts po{};
+    for (int i = 0; i < n_outs; ++i) po.p[i] = outs[i];
+    po.n = n_outs;
+    if (dtype == 0 || dtype == 3)
+        gemm_4bit_dispatch<float, true>((const float*)A, B, absmax, absmax_8bit, absmax_code, absmax_offset, po,
+                                        nullptr, M, N, K, ldc, blocksize, quant_type, dtype, stream);
+    else if (dtype == 1)
+        gemm_4bit_dispatch<__half, true>((const __half*)A, B, absmax, absmax_8bit, absmax_code, absmax_offset, po,
+                                         nullptr, M, N, K, ldc, blocksize, quant_type, 1, stream);
+    else
+        gemm_4bit_dispatch<__nv_bfloat16, true>((const __nv_bfloat16*)A, B, absmax, absmax_8bit, absmax_code,
+                                                absmax_offset, po, nullptr, M, N, K, ldc, blocksize, quant_type, 2,
+                                                stream);
+    return 0;
+}
+
+// out[m, n] (row stride ldc) = T(((parts[0] + parts[1]) + ... + parts[world - 1])[m, n] + bias[n]): the partials
+// [M, N] (row stride N, one every part_stride elements) summed in rank order in fp32, the bias added in fp32, one
+// rounding.  dtype 0 or 3 = fp32, 1 = fp16, 2 = bf16.  Returns 0, or 100 for a dtype or world it does not serve.
+int cbnb_b200_reduce_partials(const float* parts, int world, long long part_stride, void* out, const void* bias, int M,
+                              int N, int ldc, int dtype, cudaStream_t stream) {
+    return launch_reduce_partials(parts, world, part_stride, out, bias, M, N, ldc, dtype, stream) ? 0 : 100;
 }
 
 // Developer / test entry: the tensor-core kernel of gemm4_tc.cu with an explicit token tile (mt = 16 | 32 | 64 |

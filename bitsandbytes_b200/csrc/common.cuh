@@ -214,6 +214,23 @@ void set_last_error_msg(const char* msg);
 
 int device_sm_count();
 
+// ---------------------------------------------------------------- partial outputs (cbnb_b200_gemm_4bit_partial)
+// The destinations of a partial 4-bit GEMM: the fp32 accumulators, with no bias and no rounding, stored to each of
+// p[0..n) at the same row stride (a row-sharded layer's slot in every rank's buffer).
+constexpr int kMaxPartialOuts = 8;
+struct PartialOuts {
+    float* p[kMaxPartialOuts];
+    int n;
+};
+// The output argument of a 4-bit GEMM kernel or launcher: T* (bias added, rounded once to T), or, for the partial
+// instances (PART), the fp32 destinations.
+template <typename T, bool PART> struct OutArg {
+    using type = T* __restrict__;
+};
+template <typename T> struct OutArg<T, true> {
+    using type = PartialOuts;
+};
+
 // ---------------------------------------------------------------- optimizer tensor lists (optim.cu, c_api.cu)
 // One tensor of a multi-tensor optimizer step: the layout of bnb_b200_optim_tensor_t in include/bitsandbytes_b200.h.
 struct OptimTensor {

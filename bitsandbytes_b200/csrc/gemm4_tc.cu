@@ -43,6 +43,10 @@
 // QT = kDecoded is the staged instance of the large-M route (launch_gemm4_staged, below): the weights arrive already
 // decoded, as a [N, K] panel that the producer loads like the activations, and both wgmma operands come from shared
 // memory.
+//
+// PART is the partial instance (cbnb_b200_gemm_4bit_partial, a row-sharded layer's K slice): the output and its
+// copies are fp32, and the epilogue stores the accumulators -- the split order's sums under split-K -- with no bias
+// and no rounding, straight from the fragments.
 #include "common.cuh"
 #include "decode4.cuh"
 #include "hopper_ptx.cuh"
@@ -183,7 +187,7 @@ __device__ __forceinline__ uint32_t gather_nibbles(uint4 v, uint32_t sel, uint32
     return r;
 }
 
-template <typename T, int QT, int MT, bool DQ>
+template <typename T, int QT, int MT, bool DQ, bool PART>
 __global__ void __launch_bounds__(kThreads, 1)
     gemm4_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
                     const Gemm4Params p) {
@@ -422,6 +426,25 @@ __global__ void __launch_bounds__(kThreads, 1)
         // ================================================================== epilogue
         // acc[4j + e]: feature row row0 + 8 * (e >= 2), token column 8j + 2t + (e & 1)
         T* outp = reinterpret_cast<T*>(p.out);
+        if constexpr (PART) {
+            // a warp instruction stores four 32-byte row pieces: whole sectors, without the staging buffer, which at
+            // fp32 would not fit next to the 256-token tile's ring
+            if (splits == 1) {
+#pragma unroll
+                for (int j = 0; j < MT / 8; ++j)
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) {
+                        const int m = m0 + 8 * j + 2 * t + (e & 1);
+                        const int n = e >= 2 ? nb : na;
+                        if (m < p.M && n < p.N) {
+                            const long long o = (long long)m * p.ldc + n;
+                            reinterpret_cast<float*>(p.out)[o] = acc[4 * j + e];
+                            for (int r = 0; r < p.n_peers; ++r) reinterpret_cast<float*>(p.peer_out[r])[o] = acc[4 * j + e];
+                        }
+                    }
+                continue;
+            }
+        }
         if (splits == 1) {
             const T* bias = reinterpret_cast<const T*>(p.bias);
             const float bias_a = (bias != nullptr && a_ok) ? DT<T>::to_f32(bias[na]) : 0.f;
@@ -542,10 +565,16 @@ __global__ void __launch_bounds__(kThreads, 1)
                 float a = 0.f;
                 for (int sp = 0; sp < splits; ++sp) a += __ldcg(ws_tile + ((long long)sp * MT + c) * kTileN + rn);
                 if (nn < p.N) {
-                    const T val = DT<T>::from_f32(a + bias_r);
-                    const long long idx = (long long)m * p.ldc + nn;
-                    outp[idx] = val;
-                    for (int r = 0; r < p.n_peers; ++r) reinterpret_cast<T*>(p.peer_out[r])[idx] = val;
+                    if constexpr (PART) {
+                        const long long idx = (long long)m * p.ldc + nn;
+                        reinterpret_cast<float*>(p.out)[idx] = a;
+                        for (int r = 0; r < p.n_peers; ++r) reinterpret_cast<float*>(p.peer_out[r])[idx] = a;
+                    } else {
+                        const T val = DT<T>::from_f32(a + bias_r);
+                        const long long idx = (long long)m * p.ldc + nn;
+                        outp[idx] = val;
+                        for (int r = 0; r < p.n_peers; ++r) reinterpret_cast<T*>(p.peer_out[r])[idx] = val;
+                    }
                 }
             }
         }
@@ -643,7 +672,7 @@ Workspace* get_workspace(cudaStream_t stream, size_t partial_bytes, size_t n_cou
     return &e->ws;
 }
 
-template <typename T, int QT, int MT, bool DQ>
+template <typename T, int QT, int MT, bool DQ, bool PART>
 bool launch_mt(const T* A, Gemm4Params& p, int force_splits, cudaStream_t stream) {
     constexpr bool kSS = QT == kDecoded;
     using Cfg = StageCfg<T, MT, kSS>;
@@ -653,7 +682,7 @@ bool launch_mt(const T* A, Gemm4Params& p, int force_splits, cudaStream_t stream
     static bool attr_set[64] = {};
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return false;
-    auto kern = gemm4_tc_kernel<T, QT, MT, DQ>;
+    auto kern = gemm4_tc_kernel<T, QT, MT, DQ, PART>;
     if (!attr_set[dev]) {
         if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes) != cudaSuccess) {
             set_last_error("gemm4_tc smem attr", cudaGetLastError());
@@ -753,13 +782,18 @@ bool launch_mt(const T* A, Gemm4Params& p, int force_splits, cudaStream_t stream
 } // namespace
 
 // Returns true if the tensor-core path handled the call.
-// `peers` / `n_peers`: up to 7 additional output bases (same ldc) that receive a copy of every element.
+// `peers` / `n_peers`: up to 7 additional output bases (same ldc) that receive a copy of every element.  (PART: the
+// destinations are `out`'s, and `peers` is not read.)
 // `mt_override`: token tile (16 | 32 | 64 | 128 | 256, 0 = by M); `force_splits`: K split per tile (0 = by the grid).
-template <typename T>
+template <typename T, bool PART>
 bool launch_gemm4_tc(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
-                     const float* absmax_code, const float* absmax_offset, T* out, const T* bias, int M, int N, int K,
-                     int ldc, int blocksize, int quant_type, cudaStream_t stream, void* const* peers, int n_peers,
-                     int mt_override, int force_splits) {
+                     const float* absmax_code, const float* absmax_offset, typename OutArg<T, PART>::type out,
+                     const T* bias, int M, int N, int K, int ldc, int blocksize, int quant_type, cudaStream_t stream,
+                     void* const* peers, int n_peers, int mt_override, int force_splits) {
+    if constexpr (PART) {
+        peers = reinterpret_cast<void* const*>(out.p + 1);
+        n_peers = out.n - 1;
+    }
     if (n_peers < 0 || n_peers > 7) return false;
     if (M <= 0 || N <= 0) return true;
     if (K < 64 || (K % 64) != 0) return false;
@@ -791,7 +825,7 @@ bool launch_gemm4_tc(const T* A, const uint8_t* B, const float* absmax, const ui
     p.absmax_code = absmax_code;
     p.absmax_offset = absmax_offset;
     p.bias = bias;
-    p.out = out;
+    if constexpr (PART) p.out = out.p[0]; else p.out = out;
     p.n_peers = n_peers;
     for (int r = 0; r < n_peers; ++r) p.peer_out[r] = peers[r];
     p.M = M;
@@ -799,19 +833,19 @@ bool launch_gemm4_tc(const T* A, const uint8_t* B, const float* absmax, const ui
     p.K = K;
     p.ldc = ldc;
     p.log2_bs = ilog2_pow2(blocksize);
-    bool vec = (ldc % (16 / (int)sizeof(T))) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0;
+    bool vec = (ldc % (16 / (int)sizeof(T))) == 0 && (reinterpret_cast<uintptr_t>(p.out) & 15) == 0;
     for (int r = 0; r < n_peers; ++r) vec = vec && (reinterpret_cast<uintptr_t>(peers[r]) & 15) == 0;
     p.out_vec = vec ? 1 : 0;
 
 #define BNB200_DISPATCH_MT(QT, DQ)                                                                                     \
     switch (MT) {                                                                                                      \
-    case 16: return launch_mt<T, QT, 16, DQ>(A, p, force_splits, stream);                                              \
-    case 32: return launch_mt<T, QT, 32, DQ>(A, p, force_splits, stream);                                              \
-    case 64: return launch_mt<T, QT, 64, DQ>(A, p, force_splits, stream);                                              \
-    case 128: return launch_mt<T, QT, 128, DQ>(A, p, force_splits, stream);                                            \
+    case 16: return launch_mt<T, QT, 16, DQ, PART>(A, p, force_splits, stream);                                        \
+    case 32: return launch_mt<T, QT, 32, DQ, PART>(A, p, force_splits, stream);                                        \
+    case 64: return launch_mt<T, QT, 64, DQ, PART>(A, p, force_splits, stream);                                        \
+    case 128: return launch_mt<T, QT, 128, DQ, PART>(A, p, force_splits, stream);                                      \
     default:                                                                                                           \
         if constexpr (tf32) return false;                                                                              \
-        else return launch_mt<T, QT, 256, DQ>(A, p, force_splits, stream);                                             \
+        else return launch_mt<T, QT, 256, DQ, PART>(A, p, force_splits, stream);                                       \
     }
     const bool dq = absmax_8bit != nullptr;
     if (quant_type == kNF4) {
@@ -862,13 +896,17 @@ int staged_plan(int M, int N, int K, int sms, int* panel_rows) {
     return (int)best;
 }
 
-// panel_rows 0: the panel of staged_plan (DESIGN.md section 3.1)
-template <typename T>
+// panel_rows 0: the panel of staged_plan (DESIGN.md section 3.1).  PART: as in launch_gemm4_tc.
+template <typename T, bool PART>
 bool launch_gemm4_staged(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
-                         const float* absmax_code, const float* absmax_offset, T* out, const T* bias, int M, int N,
-                         int K, int ldc, int blocksize, int quant_type, cudaStream_t stream, void* const* peers,
-                         int n_peers, int mt_override, int panel_rows) {
+                         const float* absmax_code, const float* absmax_offset, typename OutArg<T, PART>::type out,
+                         const T* bias, int M, int N, int K, int ldc, int blocksize, int quant_type,
+                         cudaStream_t stream, void* const* peers, int n_peers, int mt_override, int panel_rows) {
     static_assert(!std::is_same<T, float>::value, "the staged route has 16-bit instances only");
+    if constexpr (PART) {
+        peers = reinterpret_cast<void* const*>(out.p + 1);
+        n_peers = out.n - 1;
+    }
     if (n_peers < 0 || n_peers > 7) return false;
     if (M <= 0 || N <= 0) return true;
     if (K < 64 || (K % 64) != 0) return false;
@@ -894,7 +932,10 @@ bool launch_gemm4_staged(const T* A, const uint8_t* B, const float* absmax, cons
         return false;
     }
     T* panel = reinterpret_cast<T*>(ws->ptr);
-    bool vec = (ldc % (16 / (int)sizeof(T))) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0;
+    using TO = typename std::conditional<PART, float, T>::type;  // the output element
+    TO* out0;
+    if constexpr (PART) out0 = out.p[0]; else out0 = out;
+    bool vec = (ldc % (16 / (int)sizeof(T))) == 0 && (reinterpret_cast<uintptr_t>(out0) & 15) == 0;
     for (int r = 0; r < n_peers; ++r) vec = vec && (reinterpret_cast<uintptr_t>(peers[r]) & 15) == 0;
     for (int n0 = 0; n0 < N; n0 += panel_rows) {
         const int rows = N - n0 < panel_rows ? N - n0 : panel_rows;
@@ -904,29 +945,31 @@ bool launch_gemm4_staged(const T* A, const uint8_t* B, const float* absmax, cons
         Gemm4Params p{};
         p.B = reinterpret_cast<const uint8_t*>(panel);
         p.bias = bias != nullptr ? bias + n0 : nullptr;
-        p.out = out + n0;
+        p.out = out0 + n0;
         p.n_peers = n_peers;
-        for (int r = 0; r < n_peers; ++r) p.peer_out[r] = reinterpret_cast<T*>(peers[r]) + n0;
+        for (int r = 0; r < n_peers; ++r) p.peer_out[r] = reinterpret_cast<TO*>(peers[r]) + n0;
         p.M = M;
         p.N = rows;
         p.K = K;
         p.ldc = ldc;
         p.log2_bs = ilog2_pow2(blocksize);
         p.out_vec = vec ? 1 : 0;
-        const bool ok = MT == 256 ? launch_mt<T, kDecoded, 256, false>(A, p, 1, stream)
-                                  : launch_mt<T, kDecoded, 128, false>(A, p, 1, stream);
+        const bool ok = MT == 256 ? launch_mt<T, kDecoded, 256, false, PART>(A, p, 1, stream)
+                                  : launch_mt<T, kDecoded, 128, false, PART>(A, p, 1, stream);
         if (!ok) return false;
     }
     return true;
 }
 
-template bool launch_gemm4_staged<__nv_bfloat16>(const __nv_bfloat16*, const uint8_t*, const float*, const uint8_t*,
-                                                 const float*, const float*, __nv_bfloat16*, const __nv_bfloat16*,
-                                                 int, int, int, int, int, int, cudaStream_t, void* const*, int, int,
-                                                 int);
-template bool launch_gemm4_staged<__half>(const __half*, const uint8_t*, const float*, const uint8_t*, const float*,
-                                          const float*, __half*, const __half*, int, int, int, int, int, int,
-                                          cudaStream_t, void* const*, int, int, int);
+#define BNB200_STAGED_INST(T, PART, OUT)                                                                               \
+    template bool launch_gemm4_staged<T, PART>(const T*, const uint8_t*, const float*, const uint8_t*, const float*,   \
+                                               const float*, OUT, const T*, int, int, int, int, int, int,              \
+                                               cudaStream_t, void* const*, int, int, int);
+BNB200_STAGED_INST(__nv_bfloat16, false, __nv_bfloat16*)
+BNB200_STAGED_INST(__half, false, __half*)
+BNB200_STAGED_INST(__nv_bfloat16, true, PartialOuts)
+BNB200_STAGED_INST(__half, true, PartialOuts)
+#undef BNB200_STAGED_INST
 
 // The staged GEMM alone on an already decoded weight W[N, K] (no workspace): for timing the route's phases.
 template <typename T>
@@ -944,23 +987,24 @@ bool launch_gemm_decoded(const T* A, const T* W, T* out, const T* bias, int M, i
     p.K = K;
     p.ldc = ldc;
     p.out_vec = ((ldc % (16 / (int)sizeof(T))) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0) ? 1 : 0;
-    return mt == 256 ? launch_mt<T, kDecoded, 256, false>(A, p, 1, stream)
-                     : launch_mt<T, kDecoded, 128, false>(A, p, 1, stream);
+    return mt == 256 ? launch_mt<T, kDecoded, 256, false, false>(A, p, 1, stream)
+                     : launch_mt<T, kDecoded, 128, false, false>(A, p, 1, stream);
 }
 template bool launch_gemm_decoded<__nv_bfloat16>(const __nv_bfloat16*, const __nv_bfloat16*, __nv_bfloat16*,
                                                  const __nv_bfloat16*, int, int, int, int, int, cudaStream_t);
 template bool launch_gemm_decoded<__half>(const __half*, const __half*, __half*, const __half*, int, int, int, int, int,
                                           cudaStream_t);
 
-template bool launch_gemm4_tc<__nv_bfloat16>(const __nv_bfloat16*, const uint8_t*, const float*, const uint8_t*,
-                                             const float*, const float*, __nv_bfloat16*, const __nv_bfloat16*, int,
-                                             int, int, int, int, int, cudaStream_t, void* const*, int, int, int);
-template bool launch_gemm4_tc<__half>(const __half*, const uint8_t*, const float*, const uint8_t*, const float*,
-                                      const float*, __half*, const __half*, int, int, int, int, int, int,
-                                      cudaStream_t, void* const*, int, int, int);
-// fp32 activations and output, TF32 tensor cores
-template bool launch_gemm4_tc<float>(const float*, const uint8_t*, const float*, const uint8_t*, const float*,
-                                     const float*, float*, const float*, int, int, int, int, int, int, cudaStream_t,
-                                     void* const*, int, int, int);
+#define BNB200_TC_INST(T, PART, OUT)                                                                                   \
+    template bool launch_gemm4_tc<T, PART>(const T*, const uint8_t*, const float*, const uint8_t*, const float*,       \
+                                           const float*, OUT, const T*, int, int, int, int, int, int, cudaStream_t,    \
+                                           void* const*, int, int, int);
+BNB200_TC_INST(__nv_bfloat16, false, __nv_bfloat16*)
+BNB200_TC_INST(__half, false, __half*)
+BNB200_TC_INST(float, false, float*)  // fp32 activations and output, TF32 tensor cores
+BNB200_TC_INST(__nv_bfloat16, true, PartialOuts)
+BNB200_TC_INST(__half, true, PartialOuts)
+BNB200_TC_INST(float, true, PartialOuts)
+#undef BNB200_TC_INST
 
 } // namespace bnb200

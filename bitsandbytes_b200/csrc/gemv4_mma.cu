@@ -89,11 +89,13 @@ __device__ __forceinline__ float lds_f1(uint32_t a) {
 // cp.async (slower, it bypasses L1), 3 or 4 CTAs per SM through a register cap, a byte-indexed shared-memory decode
 // table (profiles/r02_decode_regime.md).
 // NT = groups of 8 tokens (1: M <= 8, 2: M <= 16): the decoded weight fragments feed NT MMAs each.
-template <typename T, int QT, int W, int NT>
+// PART: the partial instance (fp32 sums to every destination of `out`, no bias, no rounding).
+template <typename T, int QT, int W, int NT, bool PART>
 __global__ void __launch_bounds__(W * 32, 32 / W)
     gemv4_mma_kernel(const T* __restrict__ A, const uint8_t* __restrict__ B, const float* absmax,
                      const uint8_t* absmax_8bit, const float* absmax_code, const float* absmax_offset,
-                     T* __restrict__ out, const T* __restrict__ bias, int M, int N, int K, int ldc, int log2_bs) {
+                     typename OutArg<T, PART>::type out, const T* __restrict__ bias, int M, int N, int K, int ldc,
+                     int log2_bs) {
     __shared__ float red[W][kGRows * 8 * NT];
     extern __shared__ __align__(16) uint8_t ring_smem[];
     const int warp = threadIdx.x >> 5;
@@ -248,18 +250,22 @@ __global__ void __launch_bounds__(W * 32, 32 / W)
             float acc = 0.f;
 #pragma unroll
             for (int w = 0; w < W; ++w) acc += red[w][idx];
-            const float b = bias != nullptr ? DT<T>::to_f32(bias[n]) : 0.f;
-            out[(long long)tok * ldc + n] = DT<T>::from_f32(acc + b);
+            if constexpr (PART) {
+                for (int d = 0; d < out.n; ++d) out.p[d][(long long)tok * ldc + n] = acc;
+            } else {
+                const float b = bias != nullptr ? DT<T>::to_f32(bias[n]) : 0.f;
+                out[(long long)tok * ldc + n] = DT<T>::from_f32(acc + b);
+            }
         }
     }
 }
 
 // the ring needs the dynamic shared-memory opt-in (per device and instantiation)
-template <typename T, int QT, int W, int NT>
+template <typename T, int QT, int W, int NT, bool PART>
 bool launch_mma_variant(dim3 grid, cudaStream_t stream, const T* A, const uint8_t* B, const float* absmax,
-                        const uint8_t* absmax_8bit, const float* absmax_code, const float* absmax_offset, T* out,
-                        const T* bias, int M, int N, int K, int ldc, int l2) {
-    auto kern = gemv4_mma_kernel<T, QT, W, NT>;
+                        const uint8_t* absmax_8bit, const float* absmax_code, const float* absmax_offset,
+                        typename OutArg<T, PART>::type out, const T* bias, int M, int N, int K, int ldc, int l2) {
+    auto kern = gemv4_mma_kernel<T, QT, W, NT, PART>;
     constexpr int kSmem = W * kRing * kRingStageBytes;
     static bool attr_set[64] = {};
     int dev = 0;
@@ -280,10 +286,10 @@ bool launch_mma_variant(dim3 grid, cudaStream_t stream, const T* A, const uint8_
 } // namespace
 
 // M <= 16, 16-bit activations, K % 64 == 0, power-of-two blocksize >= 32, 16-byte aligned A and B.
-template <typename T>
+template <typename T, bool PART>
 bool launch_gemv4_mma(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
-                      const float* absmax_code, const float* absmax_offset, T* out, const T* bias, int M, int N, int K,
-                      int ldc, int blocksize, int quant_type, cudaStream_t stream) {
+                      const float* absmax_code, const float* absmax_offset, typename OutArg<T, PART>::type out,
+                      const T* bias, int M, int N, int K, int ldc, int blocksize, int quant_type, cudaStream_t stream) {
     if (M <= 0 || N <= 0) return true;
     if (M > 16 || K < 64 || (K % 64) != 0) return false;
     if (blocksize < 32 || (blocksize & (blocksize - 1)) != 0) return false;
@@ -306,10 +312,10 @@ bool launch_gemv4_mma(const T* A, const uint8_t* B, const float* absmax, const u
 #define BNB200_GEMV_MMA(QT, WV)                                                                                        \
     do {                                                                                                               \
         if (M <= 8)                                                                                                    \
-            ok = launch_mma_variant<T, QT, WV, 1>(grid, stream, A, B, absmax, absmax_8bit, absmax_code,               \
+            ok = launch_mma_variant<T, QT, WV, 1, PART>(grid, stream, A, B, absmax, absmax_8bit, absmax_code,               \
                                                   absmax_offset, out, bias, M, N, K, ldc, l2);                        \
         else                                                                                                           \
-            ok = launch_mma_variant<T, QT, WV, 2>(grid, stream, A, B, absmax, absmax_8bit, absmax_code,               \
+            ok = launch_mma_variant<T, QT, WV, 2, PART>(grid, stream, A, B, absmax, absmax_8bit, absmax_code,               \
                                                   absmax_offset, out, bias, M, N, K, ldc, l2);                        \
     } while (0)
     bool ok = false;
@@ -328,11 +334,17 @@ bool launch_gemv4_mma(const T* A, const uint8_t* B, const float* absmax, const u
     return true;
 }
 
-template bool launch_gemv4_mma<__nv_bfloat16>(const __nv_bfloat16*, const uint8_t*, const float*, const uint8_t*,
-                                              const float*, const float*, __nv_bfloat16*, const __nv_bfloat16*, int,
-                                              int, int, int, int, int, cudaStream_t);
-template bool launch_gemv4_mma<__half>(const __half*, const uint8_t*, const float*, const uint8_t*, const float*,
-                                       const float*, __half*, const __half*, int, int, int, int, int, int,
-                                       cudaStream_t);
+template bool launch_gemv4_mma<__nv_bfloat16, false>(const __nv_bfloat16*, const uint8_t*, const float*,
+                                                     const uint8_t*, const float*, const float*, __nv_bfloat16*,
+                                                     const __nv_bfloat16*, int, int, int, int, int, int, cudaStream_t);
+template bool launch_gemv4_mma<__half, false>(const __half*, const uint8_t*, const float*, const uint8_t*, const float*,
+                                              const float*, __half*, const __half*, int, int, int, int, int, int,
+                                              cudaStream_t);
+template bool launch_gemv4_mma<__nv_bfloat16, true>(const __nv_bfloat16*, const uint8_t*, const float*, const uint8_t*,
+                                                    const float*, const float*, PartialOuts, const __nv_bfloat16*, int,
+                                                    int, int, int, int, int, cudaStream_t);
+template bool launch_gemv4_mma<__half, true>(const __half*, const uint8_t*, const float*, const uint8_t*, const float*,
+                                             const float*, PartialOuts, const __half*, int, int, int, int, int, int,
+                                             cudaStream_t);
 
 } // namespace bnb200

@@ -80,10 +80,11 @@ struct Scale {
 
 // `lut` = 16 fp32 code values (NF4 / FP4 table, or the caller's `datatype` array for the
 // legacy gemv entry point).  vec_ok: K % 8 == 0 and 16-byte aligned A rows / 4-byte aligned B rows.
-template <typename T>
+// PART (here and in gemv4_fast_kernel): the partial instance, fp32 sums to every destination of `out`, no bias.
+template <typename T, bool PART>
 __device__ __forceinline__ void
     gemv4_simt_body(const T* __restrict__ A, const uint8_t* __restrict__ B, Scale sc,
-                      const float* __restrict__ lut16_gmem, int quant_type, T* __restrict__ out,
+                      const float* __restrict__ lut16_gmem, int quant_type, typename OutArg<T, PART>::type out,
                       const T* __restrict__ bias, int M, int N, int K, int ldc, int blocksize, int vec_ok) {
     // power-of-two block sizes (all the API allows) index by shift; anything else divides
     const int log2_bs = ((blocksize & (blocksize - 1)) == 0) ? (31 - __clz(blocksize)) : -1;
@@ -171,10 +172,17 @@ __device__ __forceinline__ void
         for (int o = 16; o > 0; o >>= 1) acc[i] += __shfl_xor_sync(0xffffffffu, acc[i], o);
     }
     if (lane == 0) {
-        const float b = bias != nullptr ? DT<T>::to_f32(bias[n]) : 0.f;
+        if constexpr (PART) {
 #pragma unroll
-        for (int i = 0; i < kMB; ++i)
-            if (i < mcount) out[(long long)(m_base + i) * ldc + n] = DT<T>::from_f32(acc[i] + b);
+            for (int i = 0; i < kMB; ++i)
+                if (i < mcount)
+                    for (int d = 0; d < out.n; ++d) out.p[d][(long long)(m_base + i) * ldc + n] = acc[i];
+        } else {
+            const float b = bias != nullptr ? DT<T>::to_f32(bias[n]) : 0.f;
+#pragma unroll
+            for (int i = 0; i < kMB; ++i)
+                if (i < mcount) out[(long long)(m_base + i) * ldc + n] = DT<T>::from_f32(acc[i] + b);
+        }
     }
 }
 
@@ -201,11 +209,12 @@ template <> __device__ __forceinline__ void widen2<__half>(uint32_t pair, float&
     hi = f.y;
 }
 
-template <typename T, int QT, int MB>
+template <typename T, int QT, int MB, bool PART>
 __global__ void __launch_bounds__(kWarpsPerCta * 32)
     gemv4_fast_kernel(const T* __restrict__ A, const uint8_t* __restrict__ B, const float* absmax,
                       const uint8_t* absmax_8bit, const float* absmax_code, const float* absmax_offset,
-                      T* __restrict__ out, const T* __restrict__ bias, int M, int N, int K, int ldc, int log2_bs) {
+                      typename OutArg<T, PART>::type out, const T* __restrict__ bias, int M, int N, int K, int ldc,
+                      int log2_bs) {
     const int lane = threadIdx.x & 31;
     const int n = blockIdx.x * kWarpsPerCta + (threadIdx.x >> 5);
     if (n >= N) return;
@@ -273,30 +282,39 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32)
         for (int o = 16; o > 0; o >>= 1) acc[i] += __shfl_xor_sync(0xffffffffu, acc[i], o);
     }
     if (lane == 0) {
-        const float b = bias != nullptr ? DT<T>::to_f32(bias[n]) : 0.f;
+        if constexpr (PART) {
 #pragma unroll
-        for (int i = 0; i < MB; ++i)
-            if (i < M) out[(long long)i * ldc + n] = DT<T>::from_f32(acc[i] + b);
+            for (int i = 0; i < MB; ++i)
+                if (i < M)
+                    for (int d = 0; d < out.n; ++d) out.p[d][(long long)i * ldc + n] = acc[i];
+        } else {
+            const float b = bias != nullptr ? DT<T>::to_f32(bias[n]) : 0.f;
+#pragma unroll
+            for (int i = 0; i < MB; ++i)
+                if (i < M) out[(long long)i * ldc + n] = DT<T>::from_f32(acc[i] + b);
+        }
     }
 }
 
-template <typename T>
+template <typename T, bool PART>
 __global__ void __launch_bounds__(kWarpsPerCta * 32)
     gemv4_simt_kernel(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
-                      const float* absmax_code, const float* absmax_offset, const float* lut16, int quant_type, T* out,
-                      const T* bias, int M, int N, int K, int ldc, int blocksize, int vec_ok) {
+                      const float* absmax_code, const float* absmax_offset, const float* lut16, int quant_type,
+                      typename OutArg<T, PART>::type out, const T* bias, int M, int N, int K, int ldc, int blocksize,
+                      int vec_ok) {
     // the offset is fetched on the device: no host sync on the launch path
     Scale sc{absmax, absmax_8bit, absmax_code,
              (absmax_8bit != nullptr && absmax_offset != nullptr) ? __ldg(absmax_offset) : 0.f};
-    gemv4_simt_body<T>(A, B, sc, lut16, quant_type, out, bias, M, N, K, ldc, blocksize, vec_ok);
+    gemv4_simt_body<T, PART>(A, B, sc, lut16, quant_type, out, bias, M, N, K, ldc, blocksize, vec_ok);
 }
 
 } // namespace
 
-template <typename T>
+template <typename T, bool PART>
 void launch_gemv4_simt(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
                        const float* absmax_code, const float* absmax_offset, const float* lut16, int quant_type,
-                       T* out, const T* bias, int M, int N, int K, int ldc, int blocksize, cudaStream_t stream) {
+                       typename OutArg<T, PART>::type out, const T* bias, int M, int N, int K, int ldc, int blocksize,
+                       cudaStream_t stream) {
     if (M <= 0 || N <= 0) return;
     if constexpr (!std::is_same<T, float>::value) {
         const bool pow2 = blocksize >= 32 && (blocksize & (blocksize - 1)) == 0;
@@ -307,8 +325,8 @@ void launch_gemv4_simt(const T* A, const uint8_t* B, const float* absmax, const 
             const dim3 g((N + kWarpsPerCta - 1) / kWarpsPerCta);
             const int l2 = ilog2_pow2(blocksize);
 #define BNB200_FAST(QT, MBV)                                                                                           \
-    gemv4_fast_kernel<T, QT, MBV><<<g, kWarpsPerCta * 32, 0, stream>>>(A, B, absmax, absmax_8bit, absmax_code,         \
-                                                                       absmax_offset, out, bias, M, N, K, ldc, l2)
+    gemv4_fast_kernel<T, QT, MBV, PART><<<g, kWarpsPerCta * 32, 0, stream>>>(A, B, absmax, absmax_8bit, absmax_code,   \
+                                                                             absmax_offset, out, bias, M, N, K, ldc, l2)
             if (quant_type == kNF4) {
                 if (M == 1) BNB200_FAST(kNF4, 1);
                 else if (M == 2) BNB200_FAST(kNF4, 2);
@@ -328,16 +346,19 @@ void launch_gemv4_simt(const T* A, const uint8_t* B, const float* absmax, const 
     const bool vec_ok = (K % 8 == 0) && ((reinterpret_cast<uintptr_t>(A) & 15) == 0) &&
                         ((reinterpret_cast<uintptr_t>(B) & 3) == 0) && (blocksize % 8 == 0);
     dim3 grid((N + kWarpsPerCta - 1) / kWarpsPerCta, (M + kMB - 1) / kMB);
-    gemv4_simt_kernel<T><<<grid, kWarpsPerCta * 32, 0, stream>>>(A, B, absmax, absmax_8bit, absmax_code,
+    gemv4_simt_kernel<T, PART><<<grid, kWarpsPerCta * 32, 0, stream>>>(A, B, absmax, absmax_8bit, absmax_code,
                                                                  absmax_offset, lut16, quant_type, out, bias, M, N, K,
                                                                  ldc, blocksize, vec_ok ? 1 : 0);
     BNB200_CHECK_LAUNCH("gemv4_simt");
 }
 
 #define INST(T)                                                                                                        \
-    template void launch_gemv4_simt<T>(const T*, const uint8_t*, const float*, const uint8_t*, const float*,           \
-                                       const float*, const float*, int, T*, const T*, int, int, int, int, int,         \
-                                       cudaStream_t);
+    template void launch_gemv4_simt<T, false>(const T*, const uint8_t*, const float*, const uint8_t*, const float*,    \
+                                              const float*, const float*, int, T*, const T*, int, int, int, int, int,  \
+                                              cudaStream_t);                                                           \
+    template void launch_gemv4_simt<T, true>(const T*, const uint8_t*, const float*, const uint8_t*, const float*,     \
+                                             const float*, const float*, int, PartialOuts, const T*, int, int, int,    \
+                                             int, int, cudaStream_t);
 INST(float)
 INST(__half)
 INST(__nv_bfloat16)

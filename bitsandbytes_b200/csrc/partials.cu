@@ -1,0 +1,120 @@
+// partials.cu -- the rank-order reduction of a row-sharded 4-bit layer (bitsandbytes_b200/parallel.py).
+//
+// Every rank r of a row-parallel layer computes P_r[M, N], the fp32 partial product of its K slice
+// (cbnb_b200_gemm_4bit_partial), and every rank then holds all of them.  This kernel produces
+//
+//     out[m, n] = T( (((P_0 + P_1) + P_2) + ... + P_{w-1})[m, n] + bias[n] )
+//
+// fp32 additions in rank order, the bias added in fp32, one rounding to T: every rank computes the same bits, and
+// with one rank the result is the plain GEMM's, T(acc + bias) (bias 0 when absent, as in the GEMM epilogues).
+// The kernel reads 4 * w * M * N bytes and writes M * N elements: HBM-bound, so each thread moves 16-byte vectors.
+#include "common.cuh"
+
+namespace bnb200 {
+
+namespace {
+
+constexpr int kReduceThreads = 256;
+
+template <typename T> __device__ __forceinline__ void store_vec(T* dst, const float (&v)[16 / sizeof(T)]);
+template <> __device__ __forceinline__ void store_vec<float>(float* dst, const float (&v)[4]) {
+    *reinterpret_cast<float4*>(dst) = make_float4(v[0], v[1], v[2], v[3]);
+}
+template <> __device__ __forceinline__ void store_vec<__half>(__half* dst, const float (&v)[8]) {
+    *reinterpret_cast<uint4*>(dst) = make_uint4(pack2<__half>(v[0], v[1]), pack2<__half>(v[2], v[3]),
+                                                pack2<__half>(v[4], v[5]), pack2<__half>(v[6], v[7]));
+}
+template <> __device__ __forceinline__ void store_vec<__nv_bfloat16>(__nv_bfloat16* dst, const float (&v)[8]) {
+    *reinterpret_cast<uint4*>(dst) =
+        make_uint4(pack2<__nv_bfloat16>(v[0], v[1]), pack2<__nv_bfloat16>(v[2], v[3]),
+                   pack2<__nv_bfloat16>(v[4], v[5]), pack2<__nv_bfloat16>(v[6], v[7]));
+}
+
+// VEC: V = 16 / sizeof(T) consecutive outputs per thread, 16-byte loads of the partials and one 16-byte store
+// (N % V == 0, ldc % V == 0, part_stride % 4 == 0, 16-byte aligned bases); otherwise one element per thread.
+template <typename T, bool VEC>
+__global__ void __launch_bounds__(kReduceThreads)
+    reduce_partials_kernel(const float* __restrict__ parts, int world, long long part_stride, T* __restrict__ out,
+                           const T* __restrict__ bias, int M, int N, int ldc) {
+    constexpr int V = VEC ? 16 / (int)sizeof(T) : 1;
+    const int per_row = N / V;
+    const long long total = (long long)M * per_row;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+         i += (long long)gridDim.x * blockDim.x) {
+        const int m = (int)(i / per_row);
+        const int n = (int)(i - (long long)m * per_row) * V;
+        const float* src = parts + (long long)m * N + n;
+        float s[V];
+        if constexpr (VEC) {
+#pragma unroll
+            for (int h = 0; h < V / 4; ++h) {
+                const float4 v = __ldcs(reinterpret_cast<const float4*>(src) + h);
+                s[4 * h] = v.x;
+                s[4 * h + 1] = v.y;
+                s[4 * h + 2] = v.z;
+                s[4 * h + 3] = v.w;
+            }
+            for (int r = 1; r < world; ++r) {
+#pragma unroll
+                for (int h = 0; h < V / 4; ++h) {
+                    const float4 v = __ldcs(reinterpret_cast<const float4*>(src + r * part_stride) + h);
+                    s[4 * h] = __fadd_rn(s[4 * h], v.x);
+                    s[4 * h + 1] = __fadd_rn(s[4 * h + 1], v.y);
+                    s[4 * h + 2] = __fadd_rn(s[4 * h + 2], v.z);
+                    s[4 * h + 3] = __fadd_rn(s[4 * h + 3], v.w);
+                }
+            }
+        } else {
+            s[0] = src[0];
+            for (int r = 1; r < world; ++r) s[0] = __fadd_rn(s[0], src[r * part_stride]);
+        }
+#pragma unroll
+        for (int j = 0; j < V; ++j) s[j] = __fadd_rn(s[j], bias != nullptr ? DT<T>::to_f32(bias[n + j]) : 0.f);
+        T* dst = out + (long long)m * ldc + n;
+        if constexpr (VEC) {
+            store_vec<T>(dst, s);
+        } else {
+            dst[0] = DT<T>::from_f32(s[0]);
+        }
+    }
+}
+
+template <typename T>
+void launch_typed(const float* parts, int world, long long part_stride, T* out, const T* bias, int M, int N, int ldc,
+                  cudaStream_t stream) {
+    constexpr int V = 16 / (int)sizeof(T);
+    const bool vec = N % V == 0 && ldc % V == 0 && part_stride % 4 == 0 &&
+                     (reinterpret_cast<uintptr_t>(parts) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0;
+    const long long items = (long long)M * (vec ? N / V : N);
+    // a few waves of resident CTAs, each thread looping over the rest
+    const long long blocks = (items + kReduceThreads - 1) / kReduceThreads;
+    const long long cap = (long long)device_sm_count() * 8;
+    const int grid = (int)(blocks < cap ? blocks : cap);
+    if (vec)
+        reduce_partials_kernel<T, true><<<grid, kReduceThreads, 0, stream>>>(parts, world, part_stride, out, bias, M, N,
+                                                                             ldc);
+    else
+        reduce_partials_kernel<T, false><<<grid, kReduceThreads, 0, stream>>>(parts, world, part_stride, out, bias, M,
+                                                                              N, ldc);
+    BNB200_CHECK_LAUNCH("reduce_partials");
+}
+
+} // namespace
+
+bool launch_reduce_partials(const float* parts, int world, long long part_stride, void* out, const void* bias, int M,
+                            int N, int ldc, int dtype, cudaStream_t stream) {
+    if (world < 1 || part_stride < 0 || ldc < N) return false;
+    if (M <= 0 || N <= 0) return true;
+    if (dtype == 0 || dtype == 3)
+        launch_typed<float>(parts, world, part_stride, (float*)out, (const float*)bias, M, N, ldc, stream);
+    else if (dtype == 1)
+        launch_typed<__half>(parts, world, part_stride, (__half*)out, (const __half*)bias, M, N, ldc, stream);
+    else if (dtype == 2)
+        launch_typed<__nv_bfloat16>(parts, world, part_stride, (__nv_bfloat16*)out, (const __nv_bfloat16*)bias, M, N,
+                                    ldc, stream);
+    else
+        return false;
+    return true;
+}
+
+} // namespace bnb200

@@ -149,6 +149,20 @@ void cbnb_b200_quantize_blockwise(const float* code, const void* A, float* absma
  * `outs` is a HOST array.  Returns 0, or 100 if the shape does not take the wgmma path. */
 int cbnb_b200_gemm_4bit_multi_out(const void* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit, const float* absmax_code, const float* absmax_offset, void* const* outs, int n_outs, const void* bias, int M, int N, int K, int ldc, int blocksize, int quant_type, int dtype, bnb_stream_t stream);
 
+/* Partial GEMM of a row-sharded layer (input features split across ranks; no reference counterpart).
+ * outs[0..n_outs)[m, n] (fp32, row stride ldc) = sum_k A[m, k] * W[n, k], accumulated in fp32 with no bias and no
+ * rounding, by the kernel and K split the plain 4-bit GEMM takes for the same shape and dtype (0 = fp32, 1 = fp16,
+ * 2 = bf16, 3 = fp32 with TF32 allowed; see cbnb_b200_gemm_4bit_path).  `outs` is a HOST array of at most 8 device
+ * addresses: the local buffer and, for the fused exchange, the same slot in the peers' buffers.  Returns 0, 1 for a bad
+ * destination list, or 100 for a dtype it does not serve. */
+int cbnb_b200_gemm_4bit_partial(const void* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit, const float* absmax_code, const float* absmax_offset, float* const* outs, int n_outs, int M, int N, int K, int ldc, int blocksize, int quant_type, int dtype, bnb_stream_t stream);
+
+/* out[m, n] (row stride ldc) = T( (((P_0 + P_1) + ...) + P_{world-1})[m, n] + bias[n] ), P_r = parts + r * part_stride,
+ * each [M, N] fp32 with row stride N: the partials summed in rank order in fp32, the bias (T[N] or NULL) added in fp32,
+ * one rounding to T.  dtype 0 or 3 = fp32, 1 = fp16, 2 = bf16.  Returns 0, or 100 for a dtype or argument it does not
+ * serve. */
+int cbnb_b200_reduce_partials(const float* parts, int world, long long part_stride, void* out, const void* bias, int M, int N, int ldc, int dtype, bnb_stream_t stream);
+
 /* Which kernel a (M, N, K, blocksize, dtype) 4-bit GEMM takes: 0 = CUDA-core GEMV,
  * 1 = wgmma GEMM, 2 = generic CUDA-core kernel, 3 = mma.sync decode kernel (M <= 8).
  * dtype for the 4-bit GEMM entries below: 0 = fp32, 1 = fp16, 2 = bf16, 3 = fp32 with TF32 allowed -- the
