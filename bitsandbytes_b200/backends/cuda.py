@@ -721,6 +721,213 @@ def int8_mixed_mm_flags(A, CA, CB, SCA, SCB, col_flags, bias=None) -> torch.Tens
     return out
 
 
+# ------------------------------------------------------------------------------------------ tensor-parallel LLM.int8()
+def _int8_acts(what: str, A: torch.Tensor) -> tuple[torch.Tensor, int, int]:
+    if A.dtype not in (torch.float16, torch.bfloat16) or not A.is_cuda:
+        raise ValueError(f"{what}: A must be a float16 or bfloat16 CUDA tensor, got {A.dtype} on {A.device}")
+    cols = A.shape[-1]
+    rows = A.numel() // cols if cols else 0
+    _check_sizes(what, rows, cols)
+    return A.contiguous(), rows, cols
+
+
+def int8_row_stats(A: torch.Tensor, threshold: float):
+    """(row_stats fp32 [rows], col_flags int32 [cols] or None): the statistics half of
+    :func:`int8_vectorwise_quant_flags` -- the absmax of each row over the entries below ``threshold`` and the columns
+    holding an entry at or above it -- without the codes."""
+    A, rows, cols = _int8_acts("int8_row_stats", A)
+    if threshold < 0.0:
+        raise ValueError("int8_row_stats: threshold must be non-negative")
+    row_stats = torch.empty(rows, device=A.device, dtype=torch.float32)
+    flags = torch.zeros(cols, device=A.device, dtype=torch.int32) if threshold > 0.0 else None
+    if rows == 0:
+        return row_stats, flags
+    with _on_device(A):
+        rc = lib.cbnb_b200_int8_row_stats(A.data_ptr(), row_stats.data_ptr(),
+                                          flags.data_ptr() if flags is not None else None, float(threshold), rows, cols,
+                                          _DTYPE_ID[A.dtype], _stream(A))
+    lib.check("int8_row_stats")
+    if rc != 0:
+        raise RuntimeError(f"int8_row_stats: the library refused the call (code {rc})")
+    return row_stats, flags
+
+
+def int8_quant_with_stats(A: torch.Tensor, row_stats: torch.Tensor, threshold: float) -> torch.Tensor:
+    """The codes half of :func:`int8_vectorwise_quant_flags`: ``int8(rint(A * (127 / row_stats)))`` with the kernel's
+    rounding, entries at or above ``threshold`` -> 0, for given statistics (fp32 [rows] on A's device)."""
+    A, rows, cols = _int8_acts("int8_quant_with_stats", A)
+    if row_stats.dtype != torch.float32 or row_stats.shape != (rows,) or row_stats.device != A.device:
+        raise ValueError(f"int8_quant_with_stats: row_stats must be float32 [{rows}] on {A.device}")
+    q = torch.empty(A.shape, device=A.device, dtype=torch.int8)
+    if rows == 0:
+        return q
+    row_stats = row_stats.contiguous()
+    with _on_device(A):
+        rc = lib.cbnb_b200_int8_quant_with_stats(A.data_ptr(), q.data_ptr(), row_stats.data_ptr(), float(threshold),
+                                                 rows, cols, _DTYPE_ID[A.dtype], _stream(A))
+    lib.check("int8_quant_with_stats")
+    if rc != 0:
+        raise RuntimeError(f"int8_quant_with_stats: the library refused the call (code {rc})")
+    return q
+
+
+def _dest_ptrs(what: str, outs, dtype: torch.dtype, device, need: int) -> list[int]:
+    """Device addresses of 1..8 destinations: tensors (checked: dtype, device, room for ``need`` elements) or raw
+    addresses of peers' symmetric-memory buffers, which the caller vouches for."""
+    if not 1 <= len(outs) <= 8:
+        raise ValueError(f"{what}: between 1 and 8 destinations, got {len(outs)}")
+    ptrs = []
+    for o in outs:
+        if isinstance(o, torch.Tensor):
+            if o.dtype != dtype or o.device != device:
+                raise ValueError(f"{what}: destinations must be {dtype} on {device}, got {o.dtype} on {o.device}")
+            if o.untyped_storage().nbytes() // o.element_size() - o.storage_offset() < need:
+                raise ValueError(f"{what}: a destination needs {need} elements from its start")
+            ptrs.append(o.data_ptr())
+        else:
+            ptrs.append(int(o))
+    return ptrs
+
+
+def _outlier_operands(what: str, subA, subBT, M: int, N: int, dtype) -> int:
+    """jpad of the padded outlier operands subA [M, jpad] / subBT [N, jpad] (0 when both are None)."""
+    if subA is None and subBT is None:
+        return 0
+    if subA is None or subBT is None:
+        raise ValueError(f"{what}: subA and subBT go together")
+    jpad = subA.shape[-1] if subA.dim() == 2 else -1
+    if (subA.dtype != dtype or subBT.dtype != dtype or subA.shape != (M, jpad) or subBT.shape != (N, jpad)
+            or not subA.is_contiguous() or not subBT.is_contiguous()):
+        raise ValueError(f"{what}: subA / subBT must be contiguous {dtype} [{M}, jpad] / [{N}, jpad]")
+    if not 8 <= jpad <= 64 or jpad % 8 != 0:
+        raise ValueError(f"{what}: jpad must be a multiple of 8 in [8, 64], got {jpad}")
+    if subA.data_ptr() % 16 or subBT.data_ptr() % 16:
+        raise ValueError(f"{what}: subA / subBT must be 16-byte aligned")
+    return jpad
+
+
+def int8_gemm_multi_out(CA, CB, SCA, SCB, outs, ldc: int, dtype: Optional[torch.dtype], bias=None, subA=None,
+                        subBT=None) -> bool:
+    """The int8 GEMM storing every output element to each destination in ``outs`` (row stride ``ldc``): dtype None
+    gives the int32 accumulators (``int8_linear_matmul``), float16 / bfloat16 the fused epilogue of ``int8_scaled_mm``,
+    plus with ``subA`` [M, jpad] / ``subBT`` [N, jpad] (from :func:`int8_outlier_operands`, zero-padded) the outlier term
+    of ``int8_mixed_scaled_mm``.  Each destination holds the single-destination bits.  Returns False when the kernel
+    does not take the shape (K % 16, alignment): the caller takes another route."""
+    if CA.dtype != torch.int8 or CB.dtype != torch.int8 or CB.dim() != 2:
+        raise ValueError("int8_gemm_multi_out: CA and CB must be int8, CB of shape [N, K]")
+    N, K = CB.shape
+    if CA.shape[-1] != K:
+        raise ValueError(f"int8_gemm_multi_out: CA {tuple(CA.shape)} does not match CB {tuple(CB.shape)}")
+    M = CA.numel() // K if K else 0
+    _check_sizes("int8_gemm_multi_out", M, N, K, ldc)
+    if ldc < N:
+        raise ValueError(f"int8_gemm_multi_out: ldc ({ldc}) < N ({N})")
+    if dtype is None:
+        if bias is not None or subA is not None or subBT is not None:
+            raise ValueError("int8_gemm_multi_out: the int32 form takes no bias and no outlier operands")
+        epi, out_dtype = 0, torch.int32
+    elif dtype in (torch.float16, torch.bfloat16):
+        epi, out_dtype = _DTYPE_ID[dtype], dtype
+        if SCA.dtype != torch.float32 or SCB.dtype != torch.float32 or SCA.shape != (M,) or SCB.shape != (N,):
+            raise ValueError(f"int8_gemm_multi_out: SCA / SCB must be float32 [{M}] / [{N}]")
+        if bias is not None and (bias.dtype != dtype or bias.shape != (N,)):
+            raise ValueError(f"int8_gemm_multi_out: bias must be {dtype} [{N}]")
+    else:
+        raise ValueError(f"int8_gemm_multi_out: dtype must be None, float16 or bfloat16, got {dtype}")
+    jpad = _outlier_operands("int8_gemm_multi_out", subA, subBT, M, N, dtype)
+    ptrs = _dest_ptrs("int8_gemm_multi_out", outs, out_dtype, CA.device, (M - 1) * ldc + N if M > 0 else 0)
+    if M == 0 or N == 0:
+        return True
+    CA, CB = CA.contiguous(), CB.contiguous()
+    SCA = SCA.contiguous() if SCA is not None else None
+    SCB = SCB.contiguous() if SCB is not None else None
+    bias = bias.contiguous() if bias is not None else None
+    arr = (ct.c_void_p * len(ptrs))(*ptrs)
+    with _on_device(CA):
+        rc = lib.cbnb_b200_int8_gemm_multi_out(
+            CA.data_ptr(), CB.data_ptr(), SCA.data_ptr() if SCA is not None else None,
+            SCB.data_ptr() if SCB is not None else None, bias.data_ptr() if bias is not None else None,
+            subA.data_ptr() if subA is not None else None, subBT.data_ptr() if subBT is not None else None, jpad,
+            ct.cast(arr, ct.c_void_p), len(ptrs), M, N, K, ldc, epi, _stream(CA))
+    lib.check("int8_gemm_multi_out")
+    return rc == 0
+
+
+def int8_outlier_operands(A, CB, SCB, cols: torch.Tensor, jpad: Optional[int] = None):
+    """(subA [M, jpad], subBT [N, jpad]) of A's dtype: ``subA[m, j] = A[m, cols[j]]`` and ``subBT[n, j] = T((CB[n,
+    cols[j]] * SCB[n]) * (1/127))``, as the fused LLM.int8() route builds them, zero past ``len(cols)``.  ``jpad``
+    defaults to ``len(cols)`` rounded up to a multiple of 8."""
+    dtype = A.dtype
+    if dtype not in (torch.float16, torch.bfloat16):
+        raise ValueError(f"int8_outlier_operands: A must be float16 or bfloat16, got {dtype}")
+    if CB.dtype != torch.int8 or CB.dim() != 2 or SCB.dtype != torch.float32 or SCB.shape != (CB.shape[0],):
+        raise ValueError("int8_outlier_operands: CB must be int8 [N, K] and SCB float32 [N]")
+    N, K = CB.shape
+    if A.shape[-1] != K:
+        raise ValueError(f"int8_outlier_operands: A {tuple(A.shape)} does not match CB {tuple(CB.shape)}")
+    J = int(cols.numel())
+    jpad = -(-J // 8) * 8 if jpad is None else jpad
+    if jpad < J or jpad % 8 != 0:
+        raise ValueError(f"int8_outlier_operands: jpad ({jpad}) must be a multiple of 8 >= {J}")
+    M = A.numel() // K if K else 0
+    _check_sizes("int8_outlier_operands", M, N, K, jpad)
+    subA = torch.zeros((M, jpad), device=A.device, dtype=dtype)
+    subBT = torch.zeros((N, jpad), device=A.device, dtype=dtype)
+    if jpad == 0 or M + N == 0:
+        return subA, subBT
+    A2 = A.reshape(M, K).contiguous()
+    cols = cols.to(device=A.device, dtype=torch.int64).contiguous()
+    with _on_device(A):
+        lib.cbnb_b200_int8_outlier_prep(A2.data_ptr(), CB.contiguous().data_ptr(), SCB.contiguous().data_ptr(),
+                                        cols.data_ptr(), J, jpad, M, N, K, _DTYPE_ID[dtype], subA.data_ptr(),
+                                        subBT.data_ptr(), _stream(A))
+    lib.check("int8_outlier_operands")
+    return subA, subBT
+
+
+def int8_reduce_partials(parts: torch.Tensor, SCA, SCB, dtype: torch.dtype, bias=None, subA=None, subBT=None,
+                         out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """``out = epilogue(parts[0] + ... + parts[w-1])``: the exact int32 partials ``[w, M, N]`` of a K-sharded LLM.int8()
+    layer summed, then dequantised exactly as the int8 GEMM's epilogue does (``SCA`` [M], ``SCB`` [N], the bias rules of
+    fp16 / bf16 output), with the outlier term of ``subA`` [M, jpad] / ``subBT`` [N, jpad] when given.  ``out`` may be
+    an ``[M, N]`` view with unit column stride and any row stride."""
+    if parts.dtype != torch.int32 or parts.dim() != 3 or not parts.is_cuda:
+        raise ValueError(f"int8_reduce_partials: parts must be a [world, M, N] int32 CUDA tensor, got {parts.dtype} "
+                         f"{tuple(parts.shape)} on {parts.device}")
+    if dtype not in (torch.float16, torch.bfloat16):
+        raise ValueError(f"int8_reduce_partials: dtype must be float16 or bfloat16, got {dtype}")
+    world, M, N = parts.shape
+    if world < 1:
+        raise ValueError("int8_reduce_partials: no partials")
+    if (SCA.dtype != torch.float32 or SCB.dtype != torch.float32 or SCA.shape != (M,) or SCB.shape != (N,)
+            or SCA.device != parts.device or SCB.device != parts.device):
+        raise ValueError(f"int8_reduce_partials: SCA / SCB must be float32 [{M}] / [{N}] on {parts.device}")
+    if bias is not None and (bias.dtype != dtype or bias.shape != (N,) or bias.device != parts.device):
+        raise ValueError(f"int8_reduce_partials: bias must be {dtype} [{N}] on {parts.device}")
+    jpad = _outlier_operands("int8_reduce_partials", subA, subBT, M, N, dtype)
+    if out is None:
+        out = torch.empty((M, N), dtype=dtype, device=parts.device)
+    elif (out.dtype != dtype or out.shape != (M, N) or out.device != parts.device
+          or (M > 1 and out.stride(1) != 1) or out.stride(0) < N):
+        raise ValueError(f"int8_reduce_partials: out must be {dtype} [{M}, {N}] with unit column stride on "
+                         f"{parts.device}")
+    _check_sizes("int8_reduce_partials", M, N, out.stride(0), world)
+    if M == 0 or N == 0:
+        return out
+    parts = parts.contiguous()
+    SCA, SCB = SCA.contiguous(), SCB.contiguous()
+    bias = bias.contiguous() if bias is not None else None
+    with _on_device(parts):
+        rc = lib.cbnb_b200_int8_reduce_partials(
+            parts.data_ptr(), world, M * N, SCA.data_ptr(), SCB.data_ptr(), bias.data_ptr() if bias is not None else None,
+            subA.data_ptr() if subA is not None else None, subBT.data_ptr() if subBT is not None else None, jpad,
+            out.data_ptr(), M, N, out.stride(0), _DTYPE_ID[dtype], _stream(parts))
+    lib.check("int8_reduce_partials")
+    if rc != 0:
+        raise RuntimeError(f"int8_reduce_partials: the library refused the call (code {rc})")
+    return out
+
+
 # ------------------------------------------------------------------------------------------ optimizers (section 8 f-4)
 # optimizer name -> (native id, bf16 served by the reference-named 32-bit symbol)  (reference
 # backends/cuda/ops.py:985-1066: lamb is adam with max_unorm, lars is momentum with max_unorm)

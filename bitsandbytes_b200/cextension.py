@@ -96,6 +96,15 @@ def _signatures():
     sig["cbnb_b200_int8_mixed_mm_dev"] = ([_VOIDP] * 11 + [_I32] * 4 + [_VOIDP], _I32)
     # (A, out, rowStats, col_flags, threshold, rows, cols, dtype, stream)
     sig["cbnb_b200_int8_vector_quant_flags"] = ([_VOIDP] * 4 + [ct.c_float] + [_I32] * 3 + [_VOIDP], None)
+    # (A, rowStats, col_flags, threshold, rows, cols, dtype, stream) -> int
+    sig["cbnb_b200_int8_row_stats"] = ([_VOIDP] * 3 + [ct.c_float] + [_I32] * 3 + [_VOIDP], _I32)
+    # (A, out, rowStats, threshold, rows, cols, dtype, stream) -> int
+    sig["cbnb_b200_int8_quant_with_stats"] = ([_VOIDP] * 3 + [ct.c_float] + [_I32] * 3 + [_VOIDP], _I32)
+    # (CA, CB, SCA, SCB, bias, subA, subBT, jpad, outs, n_outs, M, N, K, ldc, epi, stream) -> int
+    sig["cbnb_b200_int8_gemm_multi_out"] = ([_VOIDP] * 7 + [_I32, _VOIDP] + [_I32] * 6 + [_VOIDP], _I32)
+    # (parts, world, part_stride, SCA, SCB, bias, subA, subBT, jpad, out, M, N, ldc, dtype, stream) -> int
+    sig["cbnb_b200_int8_reduce_partials"] = ([_VOIDP, _I32, ct.c_longlong] + [_VOIDP] * 5 + [_I32, _VOIDP] + [_I32] * 4
+                                             + [_VOIDP], _I32)
     # (A, B, value, n)
     sig["cfill_fp32"] = ([_VOIDP, _VOIDP, ct.c_float, ct.c_long], None)
     sig["cfill_uint8"] = ([_VOIDP, _VOIDP, ct.c_ubyte, ct.c_long], None)

@@ -86,7 +86,15 @@ void launch_dequant_mm_int32_fp16(const int* A, const float* rowStats, const flo
 int launch_int8_gemm(const int8_t* acts, const int8_t* weights, void* out, const float* SCA, const float* SCB,
                      const void* bias, int M, int N, int K, int ldc, int epi, cudaStream_t stream,
                      const void* subA = nullptr, const void* subBT = nullptr, int jpad = 0,
-                     const int* jcount = nullptr, const int* cols = nullptr, const void* A = nullptr);
+                     const int* jcount = nullptr, const int* cols = nullptr, const void* A = nullptr,
+                     void* const* outs = nullptr, int n_outs = 0);
+void launch_int8_row_stats(const void* A, float* rowStats, int* col_flags, float threshold, int rows, int cols,
+                           int dtype, cudaStream_t stream);
+void launch_int8_quant_with_stats(const void* A, int8_t* out, const float* rowStats, float threshold, int rows,
+                                  int cols, int dtype, cudaStream_t stream);
+bool launch_reduce_int8_partials(const int* parts, int world, long long part_stride, const float* SCA, const float* SCB,
+                                 const void* bias, const void* subA, const void* subBT, int jpad, void* out, int M,
+                                 int N, int ldc, int dtype, cudaStream_t stream);
 void launch_int8_outlier_prep(const void* A, const int8_t* CB, const float* SCB, const long long* cols, int J, int jpad,
                               int M, int N, int K, int dtype, void* subA, void* subBT, cudaStream_t stream);
 void launch_int8_outlier_prep_dev(const void* A, int8_t* CA, const int8_t* CB, const float* SCB, const int* cols,
@@ -695,6 +703,63 @@ void cbnb_b200_int8_vector_quant_flags(const void* A, int8_t* out, float* rowSta
         return;
     }
     launch_int8_vector_quant(A, out, rowStats, col_flags, threshold, rows, cols, dtype, stream);
+}
+
+// ---------------------------------------------------------------- tensor-parallel LLM.int8() (parallel.py)
+// The two halves of cbnb_b200_int8_vector_quant_flags, for a row-parallel layer whose ranks combine their row
+// statistics (a max) before quantising: rowStats[rows] and col_flags[cols] (int32, zeroed by the caller; NULL when
+// threshold == 0) without codes, then the codes of A from given statistics, with the same rounding.  dtype 1 = fp16,
+// 2 = bf16.  Return 0, or 100 with the error message set.
+int cbnb_b200_int8_row_stats(const void* A, float* rowStats, int* col_flags, float threshold, int rows, int cols,
+                             int dtype, cudaStream_t stream) {
+    if (dtype != 1 && dtype != 2) {
+        set_last_error_msg("int8_row_stats: dtype must be 1 (fp16) or 2 (bf16)");
+        return 100;
+    }
+    launch_int8_row_stats(A, rowStats, col_flags, threshold, rows, cols, dtype, stream);
+    return 0;
+}
+
+int cbnb_b200_int8_quant_with_stats(const void* A, int8_t* out, const float* rowStats, float threshold, int rows,
+                                    int cols, int dtype, cudaStream_t stream) {
+    if (dtype != 1 && dtype != 2) {
+        set_last_error_msg("int8_quant_with_stats: dtype must be 1 (fp16) or 2 (bf16)");
+        return 100;
+    }
+    launch_int8_quant_with_stats(A, out, rowStats, threshold, rows, cols, dtype, stream);
+    return 0;
+}
+
+// The int8 GEMM of cbnb_b200_int8_scaled_mm (epi 1 / 2, with the outlier term of cbnb_b200_int8_mixed_mm when
+// jpad > 0) or of cigemmlt_32 (epi 0: int32 accumulators, jpad 0), storing every output element to each of
+// outs[0 .. n_outs) (1 <= n_outs <= 8, device addresses: local buffers or peers' mapped buffers) at row stride ldc.
+// Every destination holds the bits of the single-destination call.  Returns 0; 100 with the error message set for bad
+// arguments; 100 without a message when the shape is not served (K % 16, alignment: the caller takes another route).
+int cbnb_b200_int8_gemm_multi_out(const int8_t* CA, const int8_t* CB, const float* SCA, const float* SCB,
+                                  const void* bias, const void* subA, const void* subBT, int jpad, void* const* outs,
+                                  int n_outs, int M, int N, int K, int ldc, int epi, cudaStream_t stream) {
+    if (outs == nullptr || n_outs < 1 || n_outs > 8 || epi < 0 || epi > 2 || ldc < N || (epi == 0 && jpad != 0)) {
+        set_last_error_msg("int8_gemm_multi_out: needs 1 <= n_outs <= 8, epi 0 / 1 / 2, ldc >= N, no outliers at epi 0");
+        return 100;
+    }
+    return launch_int8_gemm(CA, CB, nullptr, SCA, SCB, bias, M, N, K, ldc, epi, stream, subA, subBT, jpad, nullptr,
+                            nullptr, nullptr, outs, n_outs);
+}
+
+// out[m, n] (row stride ldc) = the int8 GEMM epilogue of cbnb_b200_int8_scaled_mm / cbnb_b200_int8_mixed_mm applied
+// to sum_r parts[r][m, n]: the int32 partials of a K-sharded layer ([M, N] each, row stride N, one every part_stride
+// elements), summed exactly, then dequantised with SCA[M] / SCB[N], the bias, and for jpad > 0 the outlier term of
+// subA[M, jpad] . subBT[N, jpad]^T.  dtype 1 = fp16, 2 = bf16.  Returns 0, or 100 with the error message set.
+int cbnb_b200_int8_reduce_partials(const int* parts, int world, long long part_stride, const float* SCA,
+                                   const float* SCB, const void* bias, const void* subA, const void* subBT, int jpad,
+                                   void* out, int M, int N, int ldc, int dtype, cudaStream_t stream) {
+    if (!launch_reduce_int8_partials(parts, world, part_stride, SCA, SCB, bias, subA, subBT, jpad, out, M, N, ldc, dtype,
+                                     stream)) {
+        set_last_error_msg("int8_reduce_partials: needs world >= 1, ldc >= N, dtype 1 / 2, jpad a multiple of 8 "
+                           "<= 64 with 16-byte aligned outlier operands");
+        return 100;
+    }
+    return 0;
 }
 
 // =====================================================================================

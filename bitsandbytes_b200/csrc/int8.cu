@@ -59,7 +59,10 @@ __device__ __forceinline__ int8_t quant_one(float v, float scale) {
 
 // One CTA per row.  thr_stat = threshold as the reference's first pass sees it (rounded to T),
 // thr = raw fp32 threshold used by the second pass (reference kernels.cu:1358 vs :1378).
-template <typename T, bool kVec>
+// MODE 0: statistics, flags and codes.  MODE 1: the row statistics and the outlier flags only (no codes).  MODE 2: the
+// codes only, from the statistics given in rowStats -- the two halves of MODE 0, for a row-parallel layer whose ranks
+// combine their statistics (a max over the ranks) before quantising.
+template <typename T, bool kVec, int MODE = 0>
 __global__ void __launch_bounds__(kVqThreads)
     int8_vector_quant_kernel(const T* __restrict__ A, int8_t* __restrict__ out, float* __restrict__ rowStats,
                              int* __restrict__ col_flags, float thr, float thr_stat, int rows, int cols) {
@@ -82,22 +85,28 @@ __global__ void __launch_bounds__(kVqThreads)
             cache[j] = make_uint4(0, 0, 0, 0);
             if (vi < nvec) cache[j] = ldg_stream_v4(a + 8 * vi);
         }
+        float row_absmax;
+        if constexpr (MODE != 2) {
 #pragma unroll
-        for (int j = 0; j < kVqVecs; ++j) {
-            const int vi = threadIdx.x + j * kVqThreads;
-            if (vi < nvec) {
-                float v[8];
-                unpack8<T>(cache[j], v);
+            for (int j = 0; j < kVqVecs; ++j) {
+                const int vi = threadIdx.x + j * kVqThreads;
+                if (vi < nvec) {
+                    float v[8];
+                    unpack8<T>(cache[j], v);
 #pragma unroll
-                for (int t = 0; t < 8; ++t) {
-                    const float av = fabsf(v[t]);
-                    if (!sparse || av < thr_stat) m = fmaxf(m, av);
-                    if (sparse && col_flags != nullptr && av >= thr) col_flags[8 * vi + t] = 1;
+                    for (int t = 0; t < 8; ++t) {
+                        const float av = fabsf(v[t]);
+                        if (!sparse || av < thr_stat) m = fmaxf(m, av);
+                        if (sparse && col_flags != nullptr && av >= thr) col_flags[8 * vi + t] = 1;
+                    }
                 }
             }
+            row_absmax = block_max(m, sred);
+            if (threadIdx.x == 0) rowStats[row] = row_absmax;
+            if constexpr (MODE == 1) return;
+        } else {
+            row_absmax = rowStats[row];
         }
-        const float row_absmax = block_max(m, sred);
-        if (threadIdx.x == 0) rowStats[row] = row_absmax;
         const float scale = div_approx_ftz(127.0f, row_absmax);  // __fdividef
 #pragma unroll
         for (int j = 0; j < kVqVecs; ++j) {
@@ -115,13 +124,19 @@ __global__ void __launch_bounds__(kVqThreads)
             }
         }
     } else {
-        for (int c = threadIdx.x; c < cols; c += kVqThreads) {
-            const float av = fabsf(DT<T>::to_f32(a[c]));
-            if (!sparse || av < thr_stat) m = fmaxf(m, av);
-            if (sparse && col_flags != nullptr && av >= thr) col_flags[c] = 1;
+        float row_absmax;
+        if constexpr (MODE != 2) {
+            for (int c = threadIdx.x; c < cols; c += kVqThreads) {
+                const float av = fabsf(DT<T>::to_f32(a[c]));
+                if (!sparse || av < thr_stat) m = fmaxf(m, av);
+                if (sparse && col_flags != nullptr && av >= thr) col_flags[c] = 1;
+            }
+            row_absmax = block_max(m, sred);
+            if (threadIdx.x == 0) rowStats[row] = row_absmax;
+            if constexpr (MODE == 1) return;
+        } else {
+            row_absmax = rowStats[row];
         }
-        const float row_absmax = block_max(m, sred);
-        if (threadIdx.x == 0) rowStats[row] = row_absmax;
         const float scale = div_approx_ftz(127.0f, row_absmax);
         for (int c = threadIdx.x; c < cols; c += kVqThreads) {
             const float v = DT<T>::to_f32(a[c]);
@@ -410,6 +425,50 @@ void launch_int8_zero_columns(int8_t* CA, const long long* cols, int J, int rows
     const int grid = (int)(want < 132 * 16 ? want : 132 * 16);
     int8_zero_columns_kernel<<<grid, 256, 0, stream>>>(CA, cols, J, rows, K);
     BNB200_CHECK_LAUNCH("int8_zero_columns");
+}
+
+namespace {
+
+template <int MODE>
+void vector_quant_mode(const void* A, int8_t* out, float* rowStats, int* col_flags, float threshold, int rows, int cols,
+                       int dtype, cudaStream_t stream) {
+    const bool vec = (cols % 8 == 0) && (cols <= kVqThreads * kVqVecs * 8) &&
+                     ((reinterpret_cast<uintptr_t>(A) & 15) == 0) && ((reinterpret_cast<uintptr_t>(out) & 7) == 0);
+    float thr_stat = threshold;
+    if (dtype == 1) thr_stat = __half2float(__float2half_rn(threshold));
+    if (dtype == 2) thr_stat = __bfloat162float(__float2bfloat16_rn(threshold));
+#define BNB200_VQ(T)                                                                                                   \
+    if (vec)                                                                                                           \
+        int8_vector_quant_kernel<T, true, MODE><<<rows, kVqThreads, 0, stream>>>((const T*)A, out, rowStats, col_flags, \
+                                                                                 threshold, thr_stat, rows, cols);     \
+    else                                                                                                               \
+        int8_vector_quant_kernel<T, false, MODE><<<rows, kVqThreads, 0, stream>>>((const T*)A, out, rowStats,          \
+                                                                                  col_flags, threshold, thr_stat, rows, \
+                                                                                  cols)
+    if (dtype == 1) {
+        BNB200_VQ(__half);
+    } else {
+        BNB200_VQ(__nv_bfloat16);
+    }
+#undef BNB200_VQ
+}
+
+} // namespace
+
+// The two halves of launch_int8_vector_quant (same kernel, same rounding): the row statistics and outlier flags of
+// A[rows, cols] without codes, and the codes from given statistics (outliers -> 0 when threshold > 0).
+void launch_int8_row_stats(const void* A, float* rowStats, int* col_flags, float threshold, int rows, int cols,
+                           int dtype, cudaStream_t stream) {
+    if (rows <= 0 || cols <= 0) return;
+    vector_quant_mode<1>(A, nullptr, rowStats, col_flags, threshold, rows, cols, dtype, stream);
+    BNB200_CHECK_LAUNCH("int8_row_stats");
+}
+
+void launch_int8_quant_with_stats(const void* A, int8_t* out, const float* rowStats, float threshold, int rows,
+                                  int cols, int dtype, cudaStream_t stream) {
+    if (rows <= 0 || cols <= 0) return;
+    vector_quant_mode<2>(A, out, const_cast<float*>(rowStats), nullptr, threshold, rows, cols, dtype, stream);
+    BNB200_CHECK_LAUNCH("int8_quant_with_stats");
 }
 
 void launch_int8_vector_quant(const void* A, int8_t* out, float* rowStats, int* col_flags, float threshold, int rows,

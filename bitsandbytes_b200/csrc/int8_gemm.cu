@@ -9,8 +9,11 @@
 // mixed decomposition (reference backends/default/ops.py:64-100: `output.addmm(subA, subB)` after the int8
 // matmul), adds the OUTLIER term  sum_j subA[m, j] * subB[j, n]  (fp16/bf16 products, fp32 accumulation)
 // in the same epilogue, so the second pass over out[M, N] and the cuBLAS call of the reference chain are gone.
+#include <type_traits>
+
 #include "common.cuh"
 #include "hopper_ptx.cuh"
+#include "int8_epilogue.cuh"
 
 namespace bnb200 {
 
@@ -37,6 +40,8 @@ template <int JMAX> struct I8Cfg {
     static constexpr int kStages = JMAX > 0 ? 5 : 6;
 };
 
+constexpr int kI8MaxOuts = 8;
+
 // EPI: 0 = int32 out, 1 = fp16 out, 2 = bf16 out (fused dequant)
 struct I8Params {
     void* out;
@@ -57,31 +62,25 @@ struct I8Params {
     const int8_t* CB;   // [N, K] weight codes
 };
 
-// 8 consecutive T -> fp32
-template <int EPI> __device__ __forceinline__ void i8_unpack8(const uint4& r, float (&v)[8]) {
-    const uint32_t w[4] = {r.x, r.y, r.z, r.w};
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        if (EPI == 1) {
-            const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&w[i]));
-            v[2 * i] = f.x;
-            v[2 * i + 1] = f.y;
-        } else {
-            v[2 * i] = __uint_as_float(w[i] << 16);
-            v[2 * i + 1] = __uint_as_float(w[i] & 0xffff0000u);
-        }
-    }
-}
+// the parameters of a kMulti instance: every output element is stored to outs[0 .. n_outs) (row stride ldc) instead
+// of `out` (a type of its own, so that the single-destination instances keep their parameter block)
+struct I8MultiParams : I8Params {
+    void* outs[kI8MaxOuts];
+    int n_outs;
+};
+template <bool kMulti> using I8ParamsOf = typename std::conditional<kMulti, I8MultiParams, I8Params>::type;
 
 // JMAX: capacity of the fused outlier term (0 = none): subA of the CTA's 128 tokens and subBT of its 128 features
 // are staged in shared memory after the main loop.
 // kDevJ (JMAX = 64): the outlier count is read from device memory, so one launch serves any J.  The first JMAX columns
 // come from subA / subBT; the rest are gathered from A and CB, JMAX at a time, into the same shared-memory buffers and
 // continue the same fp32 sum in column order.
-template <int EPI, int JMAX, bool kDevJ = false>
+// kMulti: every output element goes to each of p.outs[0 .. p.n_outs) (a local buffer and the peers' mapped buffers of a
+// tensor-parallel layer) instead of p.out; the values are those of the single-destination instance.
+template <int EPI, int JMAX, bool kDevJ = false, bool kMulti = false>
 __global__ void __launch_bounds__(kI8Threads, 1)
     int8_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                        const I8Params p) {
+                        const I8ParamsOf<kMulti> p) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     constexpr int kStages = I8Cfg<JMAX>::kStages;
@@ -257,12 +256,25 @@ __global__ void __launch_bounds__(kI8Threads, 1)
             const int n = n0 + 8 * j + 2 * t;  // this thread's two consecutive columns n, n + 1
             const int v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
             if (EPI == 0) {
+                // (the single-destination store is spelled out apart, so that it compiles as before)
+                if constexpr (kMulti) {
+                    for (int d = 0; d < p.n_outs; ++d) {
+                        int* dst = reinterpret_cast<int*>(p.outs[d]) + (long long)m * p.ldc + n;
+                        if (n + 1 < p.N && (reinterpret_cast<uintptr_t>(dst) & 7) == 0) {
+                            *reinterpret_cast<int2*>(dst) = make_int2(v0, v1);
+                        } else {
+                            if (n < p.N) dst[0] = v0;
+                            if (n + 1 < p.N) dst[1] = v1;
+                        }
+                    }
+                } else {
                 int* dst = reinterpret_cast<int*>(p.out) + (long long)m * p.ldc + n;
                 if (n + 1 < p.N && (reinterpret_cast<uintptr_t>(dst) & 7) == 0) {
                     *reinterpret_cast<int2*>(dst) = make_int2(v0, v1);
                 } else {
                     if (n < p.N) dst[0] = v0;
                     if (n + 1 < p.N) dst[1] = v1;
+                }
                 }
             } else {
             // outlier term of this token and columns n, n + 1: sum_j subA[m, j] * subBT[n, j] in j order (fp32 fma)
@@ -299,21 +311,20 @@ __global__ void __launch_bounds__(kI8Threads, 1)
                     if (EPI == 1) b = __half2float(reinterpret_cast<const __half*>(p.bias)[nn]);
                     else b = __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p.bias)[nn]);
                 }
-                if (EPI == 1) {
-                    f[u] = dequant_value(v, sca, scb, b);
-                    // reference: the int8 result is an fp16 tensor, then addmm adds the fp32-accumulated
-                    // outlier product and rounds once more
-                    if (add_ol) f[u] = __half2float(__float2half_rn(f[u])) + ol[u];
-                } else {
-                    // bf16 output, bit-identical to the reference chain (backends/cuda/ops.py:186-210): the kernel
-                    // result is fp16, a non-fp16 bias is added by `out.add_(bias)` on the fp16 tensor (fp32 add,
-                    // one rounding to fp16), then `.to(bfloat16)`.
-                    f[u] = __half2float(__float2half_rn(dequant_value(v, sca, scb, 0.f)));
-                    if (p.bias != nullptr) f[u] = __half2float(__float2half_rn(f[u] + b));
-                    if (add_ol) f[u] = __bfloat162float(__float2bfloat16_rn(f[u])) + ol[u];
-                }
+                f[u] = int8_epilogue_value<EPI>(v, sca, scb, b, p.bias != nullptr, add_ol, ol[u]);
             }
             const uint32_t w = EPI == 1 ? pack2<__half>(f[0], f[1]) : pack2<__nv_bfloat16>(f[0], f[1]);
+            if constexpr (kMulti) {
+                for (int d = 0; d < p.n_outs; ++d) {
+                    uint16_t* dst = reinterpret_cast<uint16_t*>(p.outs[d]) + (long long)m * p.ldc + n;
+                    if (n + 1 < p.N && (reinterpret_cast<uintptr_t>(dst) & 3) == 0) {
+                        *reinterpret_cast<uint32_t*>(dst) = w;
+                    } else {
+                        if (n < p.N) dst[0] = (uint16_t)w;
+                        if (n + 1 < p.N) dst[1] = (uint16_t)(w >> 16);
+                    }
+                }
+            } else {
             uint16_t* dst = reinterpret_cast<uint16_t*>(p.out) + (long long)m * p.ldc + n;
             if (n + 1 < p.N && (reinterpret_cast<uintptr_t>(dst) & 3) == 0) {
                 *reinterpret_cast<uint32_t*>(dst) = w;
@@ -322,18 +333,19 @@ __global__ void __launch_bounds__(kI8Threads, 1)
                 if (n + 1 < p.N) dst[1] = (uint16_t)(w >> 16);
             }
             }
+            }
         }
     }
 }
 
-template <int EPI, int JMAX = 0, bool kDevJ = false>
-int launch_i8(const CUtensorMap& ta, const CUtensorMap& tb, I8Params& p, cudaStream_t stream) {
+template <int EPI, int JMAX = 0, bool kDevJ = false, bool kMulti = false>
+int launch_i8(const CUtensorMap& ta, const CUtensorMap& tb, I8ParamsOf<kMulti>& p, cudaStream_t stream) {
     constexpr size_t smem_bytes =
         1024 + size_t(I8Cfg<JMAX>::kStages) * kI8StageBytes + 256 + size_t(kI8TileM + kI8TileN) * JMAX * 2;
     static bool attr_set[64] = {};  // the shared-memory opt-in is per device
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 1;
-    auto kern = int8_gemm_tc_kernel<EPI, JMAX, kDevJ>;
+    auto kern = int8_gemm_tc_kernel<EPI, JMAX, kDevJ, kMulti>;
     p.kblocks = (p.K + kI8BK - 1) / kI8BK;
     if (!attr_set[dev]) {
         if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes) != cudaSuccess) {
@@ -365,10 +377,13 @@ int launch_i8(const CUtensorMap& ta, const CUtensorMap& tb, I8Params& p, cudaStr
 // subA / subBT / jpad: the fused outlier term (epi 1 / 2 only; jpad a multiple of 8, <= 64), or NULL / 0.
 // jcount / cols / A: the outlier count on the device, the ascending outlier columns and the T[M, K] activations they
 // index (epi 1 / 2 only; jpad = 64 is then the row pitch of subA / subBT), or NULL.
+// outs / n_outs: 1 <= n_outs <= 8 destinations (device addresses, row stride ldc) that each receive every output element
+// in place of `out` (not with jcount), or NULL / 0.
 int launch_int8_gemm(const int8_t* acts, const int8_t* weights, void* out, const float* SCA,
                                 const float* SCB, const void* bias, int M, int N, int K, int ldc, int epi,
                                 cudaStream_t stream, const void* subA, const void* subBT, int jpad,
-                                const int* jcount, const int* cols, const void* A) {
+                                const int* jcount, const int* cols, const void* A, void* const* outs, int n_outs) {
+    if (n_outs < 0 || n_outs > kI8MaxOuts || (n_outs > 0 && (outs == nullptr || jcount != nullptr))) return 100;
     if (M <= 0 || N <= 0) return 0;
     if (K <= 0 || (K % 16) != 0) return 100;
     if (jpad != 0 && (epi == 0 || jpad < 0 || jpad > 64 || (jpad % 8) != 0 || subA == nullptr || subBT == nullptr ||
@@ -395,6 +410,24 @@ int launch_int8_gemm(const int8_t* acts, const int8_t* weights, void* out, const
     p.cols = cols;
     p.A = A;
     p.CB = weights;
+    if (n_outs > 0) {
+        I8MultiParams pm{};
+        static_cast<I8Params&>(pm) = p;
+        for (int d = 0; d < n_outs; ++d) pm.outs[d] = outs[d];
+        pm.n_outs = n_outs;
+        if (epi == 0) return launch_i8<0, 0, false, true>(ta, tb, pm, stream);
+#define BNB200_I8_MULTI(E)                                                                                             \
+        if (jpad == 0) return launch_i8<E, 0, false, true>(ta, tb, pm, stream);                                         \
+        if (jpad <= 8) return launch_i8<E, 8, false, true>(ta, tb, pm, stream);                                         \
+        if (jpad <= 16) return launch_i8<E, 16, false, true>(ta, tb, pm, stream);                                       \
+        if (jpad <= 32) return launch_i8<E, 32, false, true>(ta, tb, pm, stream);                                       \
+        return launch_i8<E, 64, false, true>(ta, tb, pm, stream);
+        if (epi == 1) {
+            BNB200_I8_MULTI(1)
+        }
+        BNB200_I8_MULTI(2)
+#undef BNB200_I8_MULTI
+    }
     if (jcount != nullptr)
         return epi == 1 ? launch_i8<1, 64, true>(ta, tb, p, stream) : launch_i8<2, 64, true>(ta, tb, p, stream);
     if (jpad > 0) {

@@ -8,7 +8,15 @@
 // fp32 additions in rank order, the bias added in fp32, one rounding to T: every rank computes the same bits, and
 // with one rank the result is the plain GEMM's, T(acc + bias) (bias 0 when absent, as in the GEMM epilogues).
 // The kernel reads 4 * w * M * N bytes and writes M * N elements: HBM-bound, so each thread moves 16-byte vectors.
+//
+// The LLM.int8() layer (reduce_int8_partials_kernel) has exact int32 partials P_r = CA_r . CB_r^T instead: their sum is
+// the unsharded GEMM's accumulator whatever the order, and the kernel then applies the GEMM's own per-element epilogue
+// (int8_epilogue_value: dequantisation, fp16 rounding, the bf16 bias rule, the outlier term of the fused route), so that
+// every rank holds the unsharded layer's output bit for bit.
+#include <type_traits>
+
 #include "common.cuh"
+#include "int8_epilogue.cuh"
 
 namespace bnb200 {
 
@@ -99,7 +107,113 @@ void launch_typed(const float* parts, int world, long long part_stride, T* out, 
     BNB200_CHECK_LAUNCH("reduce_partials");
 }
 
+// EPI 1: fp16 out, 2: bf16 out.  VEC: 8 consecutive outputs per thread, two 16-byte loads of each rank's int32 partial
+// and one 16-byte store (N % 8 == 0, ldc % 8 == 0, part_stride % 4 == 0, 16-byte aligned bases); otherwise one output
+// per thread.  jpad > 0: add the outlier term sum_j subA[m, j] * subBT[n, j] over the jpad (zero-padded) columns, in
+// column order, as the GEMM's JMAX instances do.
+template <int EPI, bool VEC>
+__global__ void __launch_bounds__(kReduceThreads)
+    reduce_int8_partials_kernel(const int* __restrict__ parts, int world, long long part_stride,
+                                const float* __restrict__ SCA, const float* __restrict__ SCB, const void* __restrict__ bias,
+                                const uint4* __restrict__ subA, const uint4* __restrict__ subBT, int jpad,
+                                void* __restrict__ out, int M, int N, int ldc) {
+    using T = typename std::conditional<EPI == 1, __half, __nv_bfloat16>::type;
+    constexpr int V = VEC ? 8 : 1;
+    const int per_row = N / V;
+    const long long total = (long long)M * per_row;
+    const T* b_t = reinterpret_cast<const T*>(bias);
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+         i += (long long)gridDim.x * blockDim.x) {
+        const int m = (int)(i / per_row);
+        const int n = (int)(i - (long long)m * per_row) * V;
+        const int* src = parts + (long long)m * N + n;
+        int acc[V];
+        if constexpr (VEC) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int4 v = __ldcs(reinterpret_cast<const int4*>(src) + h);
+                acc[4 * h] = v.x;
+                acc[4 * h + 1] = v.y;
+                acc[4 * h + 2] = v.z;
+                acc[4 * h + 3] = v.w;
+            }
+            for (int r = 1; r < world; ++r) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int4 v = __ldcs(reinterpret_cast<const int4*>(src + r * part_stride) + h);
+                    acc[4 * h] += v.x;
+                    acc[4 * h + 1] += v.y;
+                    acc[4 * h + 2] += v.z;
+                    acc[4 * h + 3] += v.w;
+                }
+            }
+        } else {
+            acc[0] = src[0];
+            for (int r = 1; r < world; ++r) acc[0] += src[r * part_stride];
+        }
+        float ol[V];
+#pragma unroll
+        for (int u = 0; u < V; ++u) ol[u] = 0.f;
+        for (int q = 0; q < jpad / 8; ++q) {
+            float a8[8];
+            i8_unpack8<EPI>(__ldg(subA + (long long)m * (jpad / 8) + q), a8);
+#pragma unroll
+            for (int u = 0; u < V; ++u) {
+                float b8[8];
+                i8_unpack8<EPI>(__ldg(subBT + (long long)(n + u) * (jpad / 8) + q), b8);
+#pragma unroll
+                for (int x = 0; x < 8; ++x) ol[u] = fmaf(a8[x], b8[x], ol[u]);
+            }
+        }
+        const float sca = __ldg(SCA + m);
+        float f[V];
+#pragma unroll
+        for (int u = 0; u < V; ++u) {
+            const float b = b_t != nullptr ? DT<T>::to_f32(b_t[n + u]) : 0.f;
+            f[u] = int8_epilogue_value<EPI>(acc[u], sca, __ldg(SCB + n + u), b, b_t != nullptr, jpad > 0, ol[u]);
+        }
+        T* dst = reinterpret_cast<T*>(out) + (long long)m * ldc + n;
+        if constexpr (VEC) {
+            store_vec<T>(dst, f);
+        } else {
+            dst[0] = DT<T>::from_f32(f[0]);
+        }
+    }
+}
+
 } // namespace
+
+bool launch_reduce_int8_partials(const int* parts, int world, long long part_stride, const float* SCA, const float* SCB,
+                                 const void* bias, const void* subA, const void* subBT, int jpad, void* out, int M,
+                                 int N, int ldc, int dtype, cudaStream_t stream) {
+    if (world < 1 || part_stride < 0 || ldc < N || (dtype != 1 && dtype != 2)) return false;
+    if (jpad < 0 || jpad > 64 || jpad % 8 != 0) return false;
+    if (jpad > 0 && (subA == nullptr || subBT == nullptr || (reinterpret_cast<uintptr_t>(subA) & 15) != 0 ||
+                     (reinterpret_cast<uintptr_t>(subBT) & 15) != 0))
+        return false;
+    if (M <= 0 || N <= 0) return true;
+    const bool vec = N % 8 == 0 && ldc % 8 == 0 && part_stride % 4 == 0 &&
+                     (reinterpret_cast<uintptr_t>(parts) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0;
+    const long long items = (long long)M * (vec ? N / 8 : N);
+    const long long blocks = (items + kReduceThreads - 1) / kReduceThreads;
+    const long long cap = (long long)device_sm_count() * 8;
+    const int grid = (int)(blocks < cap ? blocks : cap);
+    const uint4* a = reinterpret_cast<const uint4*>(subA);
+    const uint4* bt = reinterpret_cast<const uint4*>(subBT);
+#define BNB200_RI8(E, VEC)                                                                                             \
+    reduce_int8_partials_kernel<E, VEC><<<grid, kReduceThreads, 0, stream>>>(parts, world, part_stride, SCA, SCB, bias, \
+                                                                             a, bt, jpad, out, M, N, ldc)
+    if (dtype == 1) {
+        if (vec) BNB200_RI8(1, true);
+        else BNB200_RI8(1, false);
+    } else {
+        if (vec) BNB200_RI8(2, true);
+        else BNB200_RI8(2, false);
+    }
+#undef BNB200_RI8
+    BNB200_CHECK_LAUNCH("reduce_int8_partials");
+    return true;
+}
 
 bool launch_reduce_partials(const float* parts, int world, long long part_stride, void* out, const void* bias, int M,
                             int N, int ldc, int dtype, cudaStream_t stream) {

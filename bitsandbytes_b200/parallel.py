@@ -56,7 +56,9 @@ import torch
 import torch.distributed as dist
 
 from . import functional as F
-from .backends.cuda import gemm_4bit_into, gemm_4bit_multi_out, gemm_4bit_partial, reduce_partials
+from .backends.cuda import (gemm_4bit_into, gemm_4bit_multi_out, gemm_4bit_partial, int8_gemm_multi_out,
+                            int8_outlier_operands, int8_quant_with_stats, int8_reduce_partials, int8_row_stats,
+                            int8_zero_columns, reduce_partials)
 
 
 @dataclass
@@ -295,16 +297,18 @@ class RowParallelLinear4bit(torch.nn.Module):
 
 
 class PeerPartials:
-    """Two symmetric-memory ``[world, M, N]`` fp32 partial slots shared by the ranks of ``group``."""
+    """Two symmetric-memory ``[world, M, N]`` partial slots shared by the ranks of ``group`` (fp32 for the 4-bit layer,
+    int32 for the int8 one)."""
 
-    def __init__(self, M: int, N: int, device, group: Optional[dist.ProcessGroup] = None):
+    def __init__(self, M: int, N: int, device, group: Optional[dist.ProcessGroup] = None,
+                 dtype: torch.dtype = torch.float32):
         import torch.distributed._symmetric_memory as symm_mem
 
         group = group if group is not None else dist.group.WORLD
-        self.M, self.N = M, N
+        self.M, self.N, self.dtype = M, N, dtype
         self.bufs, self.handles = [], []
         for _ in range(2):
-            t = symm_mem.empty((dist.get_world_size(group), M, N), dtype=torch.float32, device=device)
+            t = symm_mem.empty((dist.get_world_size(group), M, N), dtype=dtype, device=device)
             self.handles.append(symm_mem.rendezvous(t, group))
             self.bufs.append(t)
         self.world = self.handles[0].world_size
@@ -324,8 +328,8 @@ def fused_forward_row(layer: RowParallelLinear4bit, x: torch.Tensor, peers: Peer
     s = layer.shard
     x_r = layer.local_input(x)
     M = x_r.numel() // s.K
-    if M != peers.M or s.rows != peers.N:
-        raise ValueError("PeerPartials was built for a different output shape")
+    if M != peers.M or s.rows != peers.N or peers.dtype != torch.float32:
+        raise ValueError("PeerPartials was built for a different output shape or dtype")
     local, bases, handle = peers.slot()
     off = peers.rank * M * s.rows * 4  # this rank's slot, in bytes
     # own buffer first, then the peers
@@ -339,3 +343,399 @@ def fused_forward_row(layer: RowParallelLinear4bit, x: torch.Tensor, peers: Peer
 def reassemble_shards(shards: list[Shard4bit]) -> tuple[torch.Tensor, torch.Tensor]:
     """Inverse of slice_quantized_weight for the plain (non-nested) case: (packed, absmax)."""
     return torch.cat([s.packed for s in shards]), torch.cat([s.absmax for s in shards])
+
+
+# ====================================================================================== tensor-parallel LLM.int8()
+# Column and row sharding of the inference Linear8bitLt (``has_fp16_weights=False``).  The weight is quantised once,
+# globally (CB [N, K] int8, SCB [N] fp32 row absmax) and every shard is a slice of it.  Both layers return, on every
+# rank, the unsharded layer's output bit for bit:
+#   * column (rank r owns output rows [r*N/w, (r+1)*N/w)): every rank quantises the replicated x exactly as the
+#     unsharded layer does and runs the same GEMM on its rows; each output element's epilogue depends only on its own
+#     row and column, so the slices are the unsharded output's columns.
+#   * row (rank r owns input features [k0, k1)): the statistics of x are combined before quantising (the row absmax is
+#     a max over the ranks' slices), the int32 partials CA_r . CB_r^T add up exactly to the unsharded accumulator, and
+#     the reduction applies the GEMM's own per-element epilogue once.  The outlier columns of the ranks, concatenated
+#     in rank order, are the unsharded ascending list, and their operands are the unsharded ones.
+# Beyond 64 outlier columns the unsharded layer adds the outlier product with `addmm`; both layers then run that same
+# `addmm` on the same full-size operands.  Inference only: no backward, ``state.idx`` is not kept.
+
+_INT8_FUSED_J = 64  # outlier columns the GEMM epilogue takes; beyond, the unsharded layer runs the addmm chain
+
+
+@dataclass
+class Shard8bit:
+    """The slice of a globally quantised int8 weight owned by one rank."""
+
+    CB: torch.Tensor   # int8 [rows, K] (row shard) | [N, K / world] (K shard)
+    SCB: torch.Tensor  # fp32 [rows] (row shard) | [N], replicated (K shard)
+    rows: int
+    row0: int
+    K: int
+    k0: int = 0
+
+
+def _check_rank(world: int, rank: int) -> None:
+    if world < 1 or not 0 <= rank < world:
+        raise ValueError(f"rank {rank} outside a world of {world}")
+
+
+def slice_int8_weight(CB: torch.Tensor, SCB: torch.Tensor, world: int, rank: int) -> Shard8bit:
+    """Rank's output rows ``CB[n0:n1]`` and ``SCB[n0:n1]`` of a weight quantised once, globally."""
+    _check_rank(world, rank)
+    N, K = CB.shape
+    row0, rows = shard_rows(N, world, rank)
+    return Shard8bit(CB=CB[row0:row0 + rows].contiguous(), SCB=SCB[row0:row0 + rows].contiguous(), rows=rows,
+                     row0=row0, K=K)
+
+
+def slice_int8_weight_k(CB: torch.Tensor, SCB: torch.Tensor, world: int, rank: int) -> Shard8bit:
+    """Rank's input features ``CB[:, k0:k1]`` (repacked once) of a weight quantised once, globally.  ``SCB`` is the
+    full-row absmax and stays replicated.  Requires ``K % (16 * world) == 0``, so that every shard stays on the int8
+    GEMM."""
+    _check_rank(world, rank)
+    N, K = CB.shape
+    if K % (16 * world) != 0:
+        raise ValueError(f"in_features ({K}) must be a multiple of 16 * world ({16 * world}) to shard by input features")
+    kr = K // world
+    k0 = rank * kr
+    return Shard8bit(CB=CB[:, k0:k0 + kr].contiguous(), SCB=SCB.contiguous(), rows=N, row0=0, K=kr, k0=k0)
+
+
+def _group_world_rank(group) -> tuple[int, int]:
+    if dist.is_initialized():
+        return dist.get_world_size(group), dist.get_rank(group)
+    return 1, 0
+
+
+def _state_of(module) -> tuple[torch.Tensor, torch.Tensor, float]:
+    """(CB, SCB, threshold) of an inference Linear8bitLt on the GPU."""
+    if module.state.has_fp16_weights:
+        raise ValueError("the tensor-parallel int8 layers shard an inference Linear8bitLt (has_fp16_weights=False)")
+    CB = module.state.CB if module.state.CB is not None else module.weight.CB
+    SCB = module.state.SCB if module.state.SCB is not None else module.weight.SCB
+    if CB is None or SCB is None:
+        raise ValueError("the Linear8bitLt is not quantised yet: move it to the GPU first")
+    return CB, SCB, float(module.state.threshold)
+
+
+def _no_capture(threshold: float, what: str) -> None:
+    if threshold > 0.0 and torch.cuda.is_current_stream_capturing():
+        raise RuntimeError(f"{what}: threshold > 0 needs the outlier count on the host and cannot run under CUDA-graph "
+                           "capture; capture with threshold 0")
+
+
+@dataclass
+class Int8Input:
+    """The activations of a column-parallel layer quantised as the unsharded layer quantises them."""
+
+    A: torch.Tensor       # [M, K] of the input dtype
+    CA: torch.Tensor      # int8 [M, K], outlier columns zeroed
+    SCA: torch.Tensor     # fp32 [M]
+    cols: Optional[torch.Tensor]  # int64 ascending outlier columns, or None
+
+    @property
+    def J(self) -> int:
+        return 0 if self.cols is None else int(self.cols.numel())
+
+
+class ColumnParallelLinear8bitLt(torch.nn.Module):
+    """LLM.int8() ``y = x @ W^T + b`` with W's output features split across the process group.  Every rank's output
+    equals the unsharded inference ``Linear8bitLt`` output (its columns, with ``gather_output=False``) bit for bit."""
+
+    def __init__(self, shard: Shard8bit, out_features: int, bias: Optional[torch.Tensor] = None,
+                 group: Optional[dist.ProcessGroup] = None, gather_output: bool = True, threshold: float = 0.0):
+        super().__init__()
+        self.shard = shard
+        self.out_features = out_features
+        self.group = group
+        self.gather_output = gather_output
+        self.threshold = float(threshold)
+        self.bias_shard = None if bias is None else bias[shard.row0:shard.row0 + shard.rows].contiguous()
+        self._stage = None
+
+    @classmethod
+    def from_quantized(cls, CB, SCB, bias=None, group=None, threshold: float = 0.0, gather_output: bool = True):
+        world, rank = _group_world_rank(group)
+        return cls(slice_int8_weight(CB, SCB, world, rank), CB.shape[0], bias, group, gather_output, threshold)
+
+    @classmethod
+    def from_linear8bitlt(cls, module, group=None, gather_output: bool = True):
+        CB, SCB, threshold = _state_of(module)
+        return cls.from_quantized(CB, SCB, module.bias, group, threshold, gather_output)
+
+    def _bias(self, dtype):
+        b = self.bias_shard
+        return None if b is None else b.to(dtype)
+
+    def quantize(self, x: torch.Tensor) -> Int8Input:
+        """x [..., K] -> the codes, statistics and outlier columns of the unsharded layer (the same on every rank)."""
+        _no_capture(self.threshold, "ColumnParallelLinear8bitLt")
+        A = x.reshape(-1, self.shard.K)
+        CA, SCA, cols = F.int8_vectorwise_quant(A.to(torch.float16), threshold=self.threshold)
+        return Int8Input(A, CA, SCA, cols if self.threshold > 0.0 else None)
+
+    def local_forward(self, q: Int8Input, out: Optional[torch.Tensor] = None, ldc: Optional[int] = None):
+        """This rank's [M, rows] columns of the unsharded output, without the outlier term past 64 columns (see
+        :meth:`outlier_rows`); written into ``out`` (row stride ``ldc``) when given."""
+        s = self.shard
+        dtype = q.A.dtype
+        M = q.A.shape[0]
+        if out is None:
+            out = torch.empty((M, s.rows), device=q.A.device, dtype=dtype)
+            ldc = s.rows
+        if not self._gemm(q, [out], ldc):
+            # shapes the int8 GEMM does not take (K % 16): the library's own route, copied into place
+            if 0 < q.J <= _INT8_FUSED_J:
+                y, _ = torch.ops.bitsandbytes.int8_mixed_scaled_mm(q.A, q.CA, s.CB, q.SCA, s.SCB, q.cols,
+                                                                   self._bias(dtype))
+            else:
+                y = torch.ops.bitsandbytes.int8_scaled_mm.default(q.CA, s.CB, q.SCA, s.SCB, bias=self._bias(dtype),
+                                                                  dtype=dtype)
+            out.copy_(y.view(M, s.rows))
+        return out
+
+    def _gemm(self, q: Int8Input, outs, ldc: int) -> bool:
+        s = self.shard
+        subA = subBT = None
+        if 0 < q.J <= _INT8_FUSED_J:
+            subA, subBT = int8_outlier_operands(q.A, s.CB, s.SCB, q.cols)
+        return int8_gemm_multi_out(q.CA, s.CB, q.SCA, s.SCB, outs, ldc, q.A.dtype, self._bias(q.A.dtype), subA, subBT)
+
+    def outlier_rows(self, q: Int8Input) -> torch.Tensor:
+        """This rank's rows [rows, J] of the dequantised outlier weight columns (J > 64: the addmm operand)."""
+        s = self.shard
+        return F.int8_vectorwise_dequant(s.CB[:, q.cols].contiguous(), s.SCB).to(q.A.dtype)
+
+    @staticmethod
+    def finish(full: torch.Tensor, q: Int8Input, subBT: torch.Tensor) -> torch.Tensor:
+        """The unsharded layer's outlier step past 64 columns on the gathered [M, N] output and [N, J] weight columns:
+        the same ``addmm`` on the same operands."""
+        subA = q.A[:, q.cols].contiguous()
+        return full.addmm(subA, subBT.t())
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        s = self.shard
+        lead = x.shape[:-1]
+        q = self.quantize(x)
+        M = q.A.shape[0]
+        world, rank = _group_world_rank(self.group)
+        chain = q.J > _INT8_FUSED_J
+        if world == 1:
+            y = self.local_forward(q)
+            if chain:
+                y = self.finish(y, q, self.outlier_rows(q))
+            return y.view(*lead, s.rows)
+        if not self.gather_output and not chain:
+            return self.local_forward(q).view(*lead, s.rows)
+        full = self._gather(q, M, world, rank)
+        if chain:
+            rows = self.outlier_rows(q)
+            subBT = torch.empty((world * s.rows, q.J), device=x.device, dtype=x.dtype)
+            dist.all_gather_into_tensor(subBT, rows, group=self.group)
+            full = self.finish(full, q, subBT)
+        if not self.gather_output:
+            full = full[:, s.row0:s.row0 + s.rows].contiguous()
+        return full.reshape(*lead, full.shape[-1])
+
+    def _gather(self, q: Int8Input, M: int, world: int, rank: int) -> torch.Tensor:
+        s = self.shard
+        dtype = q.A.dtype
+        if self._stage is None or self._stage.shape[1] != M or self._stage.dtype != dtype:
+            self._stage = torch.empty((world, M, s.rows), device=q.A.device, dtype=dtype)
+        self.local_forward(q, self._stage[rank], s.rows)
+        dist.all_gather_into_tensor(self._stage.view(-1), self._stage[rank].reshape(-1), group=self.group)
+        return self._stage.permute(1, 0, 2).reshape(M, world * s.rows)
+
+
+def fused_forward_col8(layer: ColumnParallelLinear8bitLt, x: torch.Tensor, peers: PeerGather) -> torch.Tensor:
+    """``layer(x)`` with the all-gather fused into the int8 GEMM epilogue: each output element is stored into this
+    rank's columns of every rank's symmetric ``[M, N]`` buffer.  Past 64 outlier columns, or for a shape the GEMM does
+    not take, the local GEMM + NCCL route fills the same slot.  Returns this rank's [M, N] slot."""
+    s = layer.shard
+    q = layer.quantize(x)
+    M = q.A.shape[0]
+    if M != peers.M or layer.out_features != peers.N or x.dtype != peers.dtype:
+        raise ValueError("PeerGather was built for a different output shape / dtype")
+    local, bases, handle = peers.slot()
+    col_bytes = s.row0 * local.element_size()
+    order = [peers.rank] + [r for r in range(peers.world) if r != peers.rank]
+    ok = q.J <= _INT8_FUSED_J and layer._gemm(q, [bases[r] + col_bytes for r in order], peers.N)
+    if not ok:
+        full = layer._gather(q, M, peers.world, peers.rank)
+        if q.J > _INT8_FUSED_J:
+            subBT = torch.empty((layer.out_features, q.J), device=x.device, dtype=x.dtype)
+            dist.all_gather_into_tensor(subBT, layer.outlier_rows(q), group=layer.group)
+            full = layer.finish(full, q, subBT)
+        local.copy_(full)
+    handle.barrier(channel=0)  # every rank's stores have landed everywhere
+    return local
+
+
+@dataclass
+class Int8Stats:
+    """One rank's share of the row statistics of a row-parallel layer's input."""
+
+    x16: torch.Tensor               # fp16 [M, K / world]: the slice as the unsharded layer quantises it
+    row_stats: torch.Tensor         # fp32 [M]: absmax of the slice's entries below the threshold
+    flags: Optional[torch.Tensor]   # int32 [K / world]: the slice's outlier columns (threshold > 0)
+
+
+class RowParallelLinear8bitLt(torch.nn.Module):
+    """LLM.int8() ``y = x @ W^T + b`` with W's input features split across the process group: every rank returns the
+    whole ``[..., N]`` output, equal to the unsharded inference ``Linear8bitLt`` output bit for bit.
+
+    The forward pass runs in steps a single process can also drive rank by rank: :meth:`local_stats` -> a max over the
+    ranks -> :meth:`local_codes` -> :meth:`partial_forward` (+ :meth:`outlier_operands`) -> an exchange ->
+    :meth:`reduce`."""
+
+    def __init__(self, shard: Shard8bit, in_features: int, bias: Optional[torch.Tensor] = None,
+                 group: Optional[dist.ProcessGroup] = None, input_is_parallel: bool = True, threshold: float = 0.0):
+        super().__init__()
+        self.shard = shard
+        self.in_features = in_features
+        self.out_features = shard.rows
+        self.group = group
+        self.input_is_parallel = input_is_parallel
+        self.threshold = float(threshold)
+        self.bias = None if bias is None else bias.contiguous()
+        self._stage = None
+
+    @classmethod
+    def from_quantized(cls, CB, SCB, bias=None, group=None, threshold: float = 0.0, input_is_parallel: bool = True):
+        world, rank = _group_world_rank(group)
+        return cls(slice_int8_weight_k(CB, SCB, world, rank), CB.shape[1], bias, group, input_is_parallel, threshold)
+
+    @classmethod
+    def from_linear8bitlt(cls, module, group=None, input_is_parallel: bool = True):
+        CB, SCB, threshold = _state_of(module)
+        return cls.from_quantized(CB, SCB, module.bias, group, threshold, input_is_parallel)
+
+    def local_input(self, x: torch.Tensor) -> torch.Tensor:
+        """This rank's ``x_r[M, K/world]``: ``x`` itself, or its slice when the layer takes the full input."""
+        s = self.shard
+        if self.input_is_parallel:
+            if x.shape[-1] != s.K:
+                raise ValueError(f"expected this rank's {s.K} input features, got {x.shape[-1]}")
+            return x.reshape(-1, s.K)
+        if x.shape[-1] != self.in_features:
+            raise ValueError(f"expected {self.in_features} input features, got {x.shape[-1]}")
+        return x.reshape(-1, self.in_features)[:, s.k0:s.k0 + s.K]
+
+    def local_stats(self, x_r: torch.Tensor) -> Int8Stats:
+        """Step 1: the slice's row absmax and outlier flags, with the unsharded quantiser's rounding."""
+        _no_capture(self.threshold, "RowParallelLinear8bitLt")
+        x16 = x_r.to(torch.float16).contiguous()
+        row_stats, flags = int8_row_stats(x16, self.threshold)
+        return Int8Stats(x16, row_stats, flags)
+
+    def local_codes(self, st: Int8Stats, SCA: torch.Tensor) -> tuple[torch.Tensor, Optional[torch.Tensor]]:
+        """Step 3: (CA_r, local outlier columns or None) from the global statistics ``SCA`` (the max over the ranks).
+        The outlier columns are zeroed in CA_r for more than one row, as the unsharded quantiser does."""
+        CA = int8_quant_with_stats(st.x16, SCA, self.threshold)
+        if st.flags is None:
+            return CA, None
+        cols = torch.nonzero(st.flags).view(-1)  # data-dependent: a host synchronisation, as in the unsharded layer
+        if cols.numel() and CA.shape[0] > 1:
+            int8_zero_columns(CA, cols)
+        return CA, cols
+
+    def partial_forward(self, CA: torch.Tensor, outs, ldc: Optional[int] = None) -> bool:
+        """Step 4: the exact int32 partial ``CA_r . CB_r^T`` to every destination in ``outs``."""
+        s = self.shard
+        return int8_gemm_multi_out(CA, s.CB, None, None, outs, s.rows if ldc is None else ldc, None)
+
+    def outlier_operands(self, x_r: torch.Tensor, cols: torch.Tensor, jpad: int):
+        """(subA_r [M, jpad], subBT_r [N, jpad]): the rank's outlier columns of x and of the weight, zero-padded."""
+        s = self.shard
+        return int8_outlier_operands(x_r, s.CB, s.SCB, cols, jpad)
+
+    def reduce(self, parts: torch.Tensor, SCA: torch.Tensor, dtype: torch.dtype, subA=None, subBT=None,
+               out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Step 6: the [M, N] output from the [world, M, N] int32 partials and the global outlier operands (subA
+        [M, J], subBT [N, J] in rank order, or None): the GEMM epilogue with the outlier term up to 64 columns, the
+        unsharded layer's addmm beyond."""
+        bias = None if self.bias is None else self.bias.to(dtype)
+        J = 0 if subA is None else subA.shape[1]
+        if J == 0 or J > _INT8_FUSED_J:
+            y = int8_reduce_partials(parts, SCA, self.shard.SCB, dtype, bias, out=out)
+            return y if J == 0 else y.addmm(subA, subBT.t())
+        jpad = -(-J // 8) * 8
+        pa = torch.zeros((subA.shape[0], jpad), device=subA.device, dtype=dtype)
+        pb = torch.zeros((subBT.shape[0], jpad), device=subBT.device, dtype=dtype)
+        pa[:, :J] = subA
+        pb[:, :J] = subBT
+        return int8_reduce_partials(parts, SCA, self.shard.SCB, dtype, bias, pa, pb, out=out)
+
+    @staticmethod
+    def combine_outliers(operands, counts):
+        """The global (subA [M, J], subBT [N, J]) from every rank's padded operands and outlier count, in rank order
+        (None when there is no outlier column)."""
+        if sum(counts) == 0:
+            return None, None
+        subA = torch.cat([a[:, :j] for (a, _), j in zip(operands, counts)], dim=1).contiguous()
+        subBT = torch.cat([b[:, :j] for (_, b), j in zip(operands, counts)], dim=1).contiguous()
+        return subA, subBT
+
+    def _exchange_outliers(self, x_r, cols, world: int):
+        """Every rank's outlier count and operands, gathered in rank order through NCCL (None, None without any)."""
+        if cols is None:
+            return None, None
+        dev = x_r.device
+        counts = [int(cols.numel())]
+        if world > 1:
+            counts_t = torch.empty(world, device=dev, dtype=torch.int64)
+            dist.all_gather_into_tensor(counts_t, torch.tensor(counts, device=dev, dtype=torch.int64), group=self.group)
+            counts = counts_t.tolist()
+        if sum(counts) == 0:
+            return None, None
+        P = max(8, -(-max(counts) // 8) * 8)
+        a, b = self.outlier_operands(x_r, cols, P)
+        if world == 1:
+            return self.combine_outliers([(a, b)], counts)
+        M = x_r.shape[0]
+        every = torch.empty((world, M + self.shard.rows, P), device=dev, dtype=x_r.dtype)
+        dist.all_gather_into_tensor(every.view(-1), torch.cat((a, b)).reshape(-1), group=self.group)
+        return self.combine_outliers([(every[r, :M], every[r, M:]) for r in range(world)], counts)
+
+    def _prologue(self, x: torch.Tensor):
+        x_r = self.local_input(x)
+        world, rank = _group_world_rank(self.group)
+        st = self.local_stats(x_r)
+        SCA = st.row_stats
+        if world > 1:
+            dist.all_reduce(SCA, op=dist.ReduceOp.MAX, group=self.group)
+        CA, cols = self.local_codes(st, SCA)
+        return x_r, world, rank, SCA, CA, cols
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        s = self.shard
+        lead = x.shape[:-1]
+        x_r, world, rank, SCA, CA, cols = self._prologue(x)
+        M = x_r.shape[0]
+        if self._stage is None or self._stage.shape[:2] != (world, M) or self._stage.device != x.device:
+            self._stage = torch.empty((world, M, s.rows), device=x.device, dtype=torch.int32)
+        if not self.partial_forward(CA, [self._stage[rank]]):
+            raise RuntimeError("the int8 GEMM does not take this shard shape")
+        if world > 1:
+            dist.all_gather_into_tensor(self._stage.view(-1), self._stage[rank].reshape(-1), group=self.group)
+        subA, subBT = self._exchange_outliers(x_r, cols, world)
+        return self.reduce(self._stage, SCA, x.dtype, subA, subBT).view(*lead, s.rows)
+
+
+def fused_forward_row8(layer: RowParallelLinear8bitLt, x: torch.Tensor, peers: PeerPartials) -> torch.Tensor:
+    """``layer(x)`` with the exchange of the int32 partials fused into the GEMM epilogue: ``P_r`` is stored into slot r
+    of every rank's symmetric buffer, one barrier publishes them, and each rank reduces its own buffer.  The row
+    statistics (a max) and the outlier operands still travel through NCCL."""
+    s = layer.shard
+    x_r, world, rank, SCA, CA, cols = layer._prologue(x)
+    M = x_r.shape[0]
+    if M != peers.M or s.rows != peers.N or peers.dtype != torch.int32:
+        raise ValueError("PeerPartials was built for a different output shape or dtype (int32 partials)")
+    local, bases, handle = peers.slot()
+    off = peers.rank * M * s.rows * 4
+    order = [peers.rank] + [r for r in range(peers.world) if r != peers.rank]
+    if not layer.partial_forward(CA, [bases[r] + off for r in order]):
+        raise RuntimeError("the int8 GEMM does not take this shard shape")
+    subA, subBT = layer._exchange_outliers(x_r, cols, peers.world)
+    handle.barrier(channel=0)  # every rank's partial has landed everywhere
+    return layer.reduce(local, SCA, x.dtype, subA, subBT).view(*x.shape[:-1], s.rows)

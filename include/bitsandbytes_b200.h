@@ -243,6 +243,19 @@ int cbnb_b200_int8_mixed_mm_dev(const int8_t* CA, const int8_t* CB, const float*
  * that type; the reference kernel is fp16-only). */
 void cbnb_b200_int8_vector_quant_flags(const void* A, int8_t* out, float* rowStats, int* col_flags, float threshold, int rows, int cols, int dtype, bnb_stream_t stream);
 
+/* Tensor-parallel LLM.int8() (bitsandbytes_b200/parallel.py).  All return 0, or 100 with the error message set.
+ * The two halves of cbnb_b200_int8_vector_quant_flags, same kernel and rounding: the row statistics and the outlier
+ * flags (int32, zeroed by the caller, NULL at threshold 0) without codes; the codes from given row statistics. */
+int cbnb_b200_int8_row_stats(const void* A, float* rowStats, int* col_flags, float threshold, int rows, int cols, int dtype, bnb_stream_t stream);
+int cbnb_b200_int8_quant_with_stats(const void* A, int8_t* out, const float* rowStats, float threshold, int rows, int cols, int dtype, bnb_stream_t stream);
+/* The int8 GEMM (epi 0 int32, 1 fp16, 2 bf16; jpad > 0: the outlier term of cbnb_b200_int8_mixed_mm) storing every
+ * output element to each of outs[0..n_outs), n_outs <= 8, row stride ldc.  A shape the kernel does not take (K % 16,
+ * alignment, jpad > 64) returns 100 without an error message. */
+int cbnb_b200_int8_gemm_multi_out(const int8_t* CA, const int8_t* CB, const float* SCA, const float* SCB, const void* bias, const void* subA, const void* subBT, int jpad, void* const* outs, int n_outs, int M, int N, int K, int ldc, int epi, bnb_stream_t stream);
+/* out = the int8 GEMM epilogue (dtype 1 fp16, 2 bf16) of sum_r parts[r], the exact int32 partials of a K-sharded
+ * layer, with SCA, SCB, bias and, for jpad > 0, the outlier term subA[M, jpad] . subBT[N, jpad]^T. */
+int cbnb_b200_int8_reduce_partials(const int* parts, int world, long long part_stride, const float* SCA, const float* SCB, const void* bias, const void* subA, const void* subBT, int jpad, void* out, int M, int N, int ldc, int dtype, bnb_stream_t stream);
+
 /* =====================================================================
  * 3. Present for loader compatibility, outside the hot path
  * ===================================================================== */

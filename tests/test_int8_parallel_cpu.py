@@ -1,0 +1,142 @@
+"""CPU tests of the tensor-parallel LLM.int8() layers: the row and input-feature slices of a globally quantised weight,
+the sharding errors, and the argument checks of the native wrappers (against a fake library)."""
+import pytest
+import torch
+
+import bitsandbytes_b200.backends.cuda as cb
+from bitsandbytes_b200.parallel import (ColumnParallelLinear8bitLt, RowParallelLinear8bitLt, slice_int8_weight,
+                                        slice_int8_weight_k)
+
+
+def _weight(N=64, K=256, seed=3):
+    g = torch.Generator().manual_seed(seed)
+    CB = torch.randint(-127, 128, (N, K), generator=g, dtype=torch.int8)
+    SCB = torch.rand(N, generator=g) * 3
+    return CB, SCB
+
+
+@pytest.mark.parametrize("world", [1, 2, 4, 8])
+def test_row_slices_reassemble(world):
+    CB, SCB = _weight()
+    bias = torch.randn(64)
+    shards = [slice_int8_weight(CB, SCB, world, r) for r in range(world)]
+    assert torch.equal(torch.cat([s.CB for s in shards]), CB)
+    assert torch.equal(torch.cat([s.SCB for s in shards]), SCB)
+    layers = [ColumnParallelLinear8bitLt(s, 64, bias) for s in shards]
+    assert torch.equal(torch.cat([L.bias_shard for L in layers]), bias)
+    assert all(s.CB.is_contiguous() and s.rows == 64 // world and s.row0 == r * (64 // world)
+               for r, s in enumerate(shards))
+
+
+@pytest.mark.parametrize("world", [1, 2, 4, 8])
+def test_k_slices_reassemble(world):
+    CB, SCB = _weight()
+    bias = torch.randn(64)
+    shards = [slice_int8_weight_k(CB, SCB, world, r) for r in range(world)]
+    assert torch.equal(torch.cat([s.CB for s in shards], dim=1), CB)
+    assert all(torch.equal(s.SCB, SCB) for s in shards)  # the full-row absmax, replicated
+    assert [s.k0 for s in shards] == [r * 256 // world for r in range(world)]
+    assert all(s.CB.is_contiguous() and s.K == 256 // world and s.rows == 64 for s in shards)
+    layers = [RowParallelLinear8bitLt(s, 256, bias, input_is_parallel=False) for s in shards]
+    assert all(torch.equal(L.bias, bias) for L in layers)
+    x = torch.randn(3, 5, 256)
+    assert torch.equal(torch.cat([L.local_input(x) for L in layers], dim=1), x.reshape(15, 256))
+
+
+def test_sharding_errors():
+    CB, SCB = _weight(N=60, K=256)
+    with pytest.raises(ValueError, match="divisible"):
+        slice_int8_weight(CB, SCB, 8, 0)               # N % world
+    with pytest.raises(ValueError, match="16"):
+        slice_int8_weight_k(CB, SCB, 32, 0)            # 256 % (16 * 32)
+    with pytest.raises(ValueError, match="16"):
+        slice_int8_weight_k(*_weight(K=200), 2, 0)     # 200 % 32
+    for bad in (-1, 4):
+        with pytest.raises(ValueError, match="rank"):
+            slice_int8_weight(*_weight(), 4, bad)
+        with pytest.raises(ValueError, match="rank"):
+            slice_int8_weight_k(*_weight(), 4, bad)
+    layer = RowParallelLinear8bitLt(slice_int8_weight_k(*_weight(), 4, 1), 256)
+    with pytest.raises(ValueError):
+        layer.local_input(torch.randn(2, 256))         # the full input to a layer that takes its slice
+
+
+class _FakeLib:
+    def __init__(self):
+        self.calls = []
+
+    def __getattr__(self, name):
+        if not name.startswith("cbnb_b200_"):
+            raise AttributeError(name)
+
+        def call(*args):
+            self.calls.append(name)
+            return 0
+        return call
+
+    def check(self, what=""):
+        pass
+
+
+@pytest.fixture
+def fake(monkeypatch):
+    lib = _FakeLib()
+    monkeypatch.setattr(cb, "lib", lib)
+    monkeypatch.setattr(cb, "_stream", lambda t: 0)
+    return lib
+
+
+def _gemm_args(M=8, N=32, K=64):
+    CA = torch.zeros(M, K, dtype=torch.int8)
+    CB = torch.zeros(N, K, dtype=torch.int8)
+    return CA, CB, torch.ones(M), torch.ones(N)
+
+
+def test_gemm_multi_out_checks(fake):
+    CA, CB, SCA, SCB = _gemm_args()
+    i32 = lambda *s: torch.zeros(*s, dtype=torch.int32)  # noqa: E731
+    assert cb.int8_gemm_multi_out(CA, CB, None, None, [i32(8, 32)] * 8, 32, None)
+    assert fake.calls == ["cbnb_b200_int8_gemm_multi_out"]
+    with pytest.raises(ValueError, match="between 1 and 8"):
+        cb.int8_gemm_multi_out(CA, CB, None, None, [i32(8, 32)] * 9, 32, None)
+    with pytest.raises(ValueError, match="between 1 and 8"):
+        cb.int8_gemm_multi_out(CA, CB, None, None, [], 32, None)
+    with pytest.raises(ValueError, match="elements"):
+        cb.int8_gemm_multi_out(CA, CB, None, None, [i32(7 * 40 + 32 - 1)], 40, None)  # room for a ragged ldc
+    with pytest.raises(ValueError, match="ldc"):
+        cb.int8_gemm_multi_out(CA, CB, None, None, [i32(8, 32)], 31, None)
+    with pytest.raises(ValueError, match="int32"):
+        cb.int8_gemm_multi_out(CA, CB, None, None, [torch.zeros(8, 32)], 32, None)
+    with pytest.raises(ValueError, match="int8"):
+        cb.int8_gemm_multi_out(CA.float(), CB, None, None, [i32(8, 32)], 32, None)
+    with pytest.raises(ValueError, match="bias"):
+        cb.int8_gemm_multi_out(CA, CB, None, None, [i32(8, 32)], 32, None, bias=torch.zeros(32))
+    h = torch.zeros(8, 32, dtype=torch.float16)
+    with pytest.raises(ValueError, match="SCA"):
+        cb.int8_gemm_multi_out(CA, CB, SCA[:7], SCB, [h], 32, torch.float16)
+    with pytest.raises(ValueError, match="bias"):
+        cb.int8_gemm_multi_out(CA, CB, SCA, SCB, [h], 32, torch.float16, bias=torch.zeros(32, dtype=torch.bfloat16))
+    with pytest.raises(ValueError, match="jpad"):
+        cb.int8_gemm_multi_out(CA, CB, SCA, SCB, [h], 32, torch.float16, subA=torch.zeros(8, 12, dtype=torch.float16),
+                               subBT=torch.zeros(32, 12, dtype=torch.float16))
+    with pytest.raises(ValueError, match="together"):
+        cb.int8_gemm_multi_out(CA, CB, SCA, SCB, [h], 32, torch.float16, subA=torch.zeros(8, 8, dtype=torch.float16))
+    with pytest.raises(ValueError, match="dtype"):
+        cb.int8_gemm_multi_out(CA, CB, SCA, SCB, [torch.zeros(8, 32)], 32, torch.float32)
+    assert fake.calls == ["cbnb_b200_int8_gemm_multi_out"]
+
+
+def test_reduce_and_quant_checks(fake):
+    _, _, SCA, SCB = _gemm_args()
+    with pytest.raises(ValueError, match="int32 CUDA"):
+        cb.int8_reduce_partials(torch.zeros(2, 8, 32, dtype=torch.int32), SCA, SCB, torch.float16)  # on the CPU
+    with pytest.raises(ValueError, match="int32"):
+        cb.int8_reduce_partials(torch.zeros(2, 8, 32), SCA, SCB, torch.float16)
+    with pytest.raises(ValueError, match="float16 or bfloat16"):
+        cb.int8_row_stats(torch.zeros(4, 16), 0.0)
+    with pytest.raises(ValueError, match="float16 or bfloat16"):
+        cb.int8_quant_with_stats(torch.zeros(4, 16, dtype=torch.int8), torch.ones(4), 0.0)
+    with pytest.raises(ValueError, match="jpad"):
+        cb.int8_outlier_operands(torch.zeros(4, 64, dtype=torch.float16), torch.zeros(32, 64, dtype=torch.int8),
+                                 torch.ones(32), torch.arange(5), jpad=4)
+    assert fake.calls == []
