@@ -195,36 +195,39 @@ def gemm_4bit_dtype_id(dtype: torch.dtype) -> int:
     return _DTYPE_ID[dtype]
 
 
-def gemm_4bit_into(A, B, shapeB, absmax, blocksize, quant_type, bias, absmax_8bit, absmax_code, absmax_offset,
-                   out: torch.Tensor, ldc: int) -> None:
-    """out[:, :N] (row stride ldc) = A . dequant(B)^T + bias.  Shared by the op and the sharded linear.  fp32 ``A``
-    runs on TF32 tensor cores when PyTorch's fp32 matmul precision allows TF32 (:func:`gemm_4bit_dtype_id`)."""
-    K = A.shape[-1]
+def _gemm_4bit_operands(what: str, A, B, shapeB, absmax, blocksize, quant_type, bias, absmax_8bit, absmax_code,
+                        absmax_offset, ldc: int):
+    """The checked operands of a 4-bit GEMM: (contiguous A, contiguous B, the fp32 offset or None, M, N, K)."""
+    N, K = shapeB[0], shapeB[1]
+    if A.shape[-1] != K:
+        raise RuntimeError(f"A inner dim ({A.shape[-1]}) does not match weight ({K})")
     M = A.numel() // K if K else 0
-    N = shapeB[0]
-    if K != shapeB[1]:
-        raise RuntimeError(f"A inner dim ({K}) does not match weight ({shapeB[1]})")
-    _check_sizes("gemm_4bit", M, N, K, ldc)
+    _check_sizes(what, M, N, K, ldc)
+    if A.dtype not in _DTYPE_ID:
+        raise RuntimeError(f"unsupported dtype {A.dtype}")
     if absmax.dtype != torch.float32:
         raise RuntimeError(f"absmax must be float32, got {absmax.dtype}")
     if quant_type not in _QT_ID:
         raise RuntimeError(f"quant_type must be nf4 or fp4, got {quant_type}")
+    if blocksize not in _4BIT_BLOCKSIZES:
+        raise RuntimeError(f"invalid blocksize {blocksize}")
+    if (absmax_8bit is None) != (absmax_code is None) or (absmax_8bit is None) != (absmax_offset is None):
+        raise RuntimeError("absmax_8bit, absmax_code and absmax_offset must be given together")
     if bias is not None:
         if bias.ndim != 1:
             raise RuntimeError(f"bias must be 1D, got {bias.ndim}D")
         if bias.dtype != A.dtype:
             raise RuntimeError(f"bias dtype ({bias.dtype}) must match A dtype ({A.dtype})")
-    if A.dtype not in _DTYPE_ID:
-        raise RuntimeError(f"unsupported dtype {A.dtype}")
-    if (absmax_8bit is None) != (absmax_code is None) or (absmax_8bit is None) != (absmax_offset is None):
-        raise RuntimeError("absmax_8bit, absmax_code and absmax_offset must be given together")
-    if blocksize not in _4BIT_BLOCKSIZES:
-        raise RuntimeError(f"invalid blocksize {blocksize}")
-    A = A.contiguous()
-    B = B.contiguous()
-    off = None
-    if absmax_offset is not None:
-        off = absmax_offset.to(dtype=torch.float32).contiguous()
+    off = absmax_offset.to(dtype=torch.float32).contiguous() if absmax_offset is not None else None
+    return A.contiguous(), B.contiguous(), off, M, N, K
+
+
+def gemm_4bit_into(A, B, shapeB, absmax, blocksize, quant_type, bias, absmax_8bit, absmax_code, absmax_offset,
+                   out: torch.Tensor, ldc: int) -> None:
+    """out[:, :N] (row stride ldc) = A . dequant(B)^T + bias.  Shared by the op and the sharded linear.  fp32 ``A``
+    runs on TF32 tensor cores when PyTorch's fp32 matmul precision allows TF32 (:func:`gemm_4bit_dtype_id`)."""
+    A, B, off, M, N, K = _gemm_4bit_operands("gemm_4bit", A, B, shapeB, absmax, blocksize, quant_type, bias,
+                                             absmax_8bit, absmax_code, absmax_offset, ldc)
     with _on_device(A):
         lib.cbnb_b200_gemm_4bit_strided(
             A.data_ptr(), B.data_ptr(), absmax.data_ptr(),
@@ -238,27 +241,23 @@ def gemm_4bit_into(A, B, shapeB, absmax, blocksize, quant_type, bias, absmax_8bi
 
 def gemm_4bit_multi_out(A, B, shapeB, absmax, blocksize: int, quant_type: str, bias, absmax_8bit, absmax_code,
                         absmax_offset, out_ptrs, ldc: int) -> bool:
-    """Fused GEMM + all-gather: every output element is stored to each raw device address in
-    ``out_ptrs`` (local buffer first, then the peers' -- symmetric memory / CUDA IPC mappings), row
-    stride ``ldc`` elements.  Returns False when the shape does not take the wgmma kernel (the caller
-    falls back to a local output + a collective)."""
-    N, K = shapeB
-    M = A.numel() // K
+    """Fused GEMM + all-gather: every output element is stored to each destination in ``out_ptrs`` (local buffer
+    first, then the peers' -- symmetric memory / CUDA IPC mappings), row stride ``ldc`` elements.  A destination is a
+    tensor of A's dtype, checked here, or a raw device address, which the caller vouches for.  Returns False when the
+    shape does not take the wgmma kernel (the caller falls back to a local output + a collective)."""
+    A, B, off, M, N, K = _gemm_4bit_operands("gemm_4bit_multi_out", A, B, shapeB, absmax, blocksize, quant_type, bias,
+                                             absmax_8bit, absmax_code, absmax_offset, ldc)
+    ptrs = _dest_ptrs("gemm_4bit_multi_out", out_ptrs, A.dtype, A.device, M, N, ldc, RuntimeError)
     if A.dtype not in (torch.float16, torch.bfloat16):
         return False
-    if not 1 <= len(out_ptrs) <= 8:
-        raise RuntimeError("gemm_4bit_multi_out: between 1 and 8 destinations")
-    A = A.contiguous()
-    B = B.contiguous()
-    off = absmax_offset.to(dtype=torch.float32).contiguous() if absmax_offset is not None else None
-    arr = (ct.c_void_p * len(out_ptrs))(*[int(p) for p in out_ptrs])
+    arr = (ct.c_void_p * len(ptrs))(*ptrs)
     with _on_device(A):
         rc = lib.cbnb_b200_gemm_4bit_multi_out(
             A.data_ptr(), B.data_ptr(), absmax.data_ptr(),
             absmax_8bit.data_ptr() if absmax_8bit is not None else None,
             absmax_code.data_ptr() if absmax_code is not None else None,
             off.data_ptr() if off is not None else None,
-            ct.cast(arr, ct.c_void_p), len(out_ptrs), bias.data_ptr() if bias is not None else None,
+            ct.cast(arr, ct.c_void_p), len(ptrs), bias.data_ptr() if bias is not None else None,
             M, N, K, ldc, blocksize, _QT_ID[quant_type], _DTYPE_ID[A.dtype], _stream(A))
     lib.check("gemm_4bit_multi_out")
     return rc == 0
@@ -272,42 +271,11 @@ def gemm_4bit_partial(A, B, shapeB, absmax, blocksize: int, quant_type: str, abs
     for.  The kernel and its K split are the ones the plain GEMM takes for this shape (fp32 ``A`` follows
     :func:`gemm_4bit_dtype_id`), so with one shard the result is the plain GEMM's accumulator.  Returns False when
     the library does not serve the call (the caller takes another route)."""
-    N, K = shapeB
-    if A.shape[-1] != K:
-        raise RuntimeError(f"A inner dim ({A.shape[-1]}) does not match weight ({K})")
-    M = A.numel() // K if K else 0
-    _check_sizes("gemm_4bit_partial", M, N, K, ldc)
-    if A.dtype not in _DTYPE_ID:
-        raise RuntimeError(f"unsupported dtype {A.dtype}")
-    if absmax.dtype != torch.float32:
-        raise RuntimeError(f"absmax must be float32, got {absmax.dtype}")
-    if quant_type not in _QT_ID:
-        raise RuntimeError(f"quant_type must be nf4 or fp4, got {quant_type}")
-    if blocksize not in _4BIT_BLOCKSIZES:
-        raise RuntimeError(f"invalid blocksize {blocksize}")
-    if (absmax_8bit is None) != (absmax_code is None) or (absmax_8bit is None) != (absmax_offset is None):
-        raise RuntimeError("absmax_8bit, absmax_code and absmax_offset must be given together")
-    if not 1 <= len(outs) <= 8:
-        raise RuntimeError("gemm_4bit_partial: between 1 and 8 destinations")
-    if ldc < N:
-        raise RuntimeError(f"gemm_4bit_partial: ldc ({ldc}) < N ({N})")
-    need = (M - 1) * ldc + N if M > 0 else 0
-    ptrs = []
-    for o in outs:
-        if isinstance(o, torch.Tensor):
-            if o.dtype != torch.float32 or o.device != A.device:
-                raise RuntimeError(f"gemm_4bit_partial: destinations must be float32 on {A.device}, got {o.dtype} on "
-                                   f"{o.device}")
-            if o.untyped_storage().nbytes() // 4 - o.storage_offset() < need:
-                raise RuntimeError(f"gemm_4bit_partial: a destination needs {need} elements from its start")
-            ptrs.append(o.data_ptr())
-        else:
-            ptrs.append(int(o))
+    A, B, off, M, N, K = _gemm_4bit_operands("gemm_4bit_partial", A, B, shapeB, absmax, blocksize, quant_type, None,
+                                             absmax_8bit, absmax_code, absmax_offset, ldc)
+    ptrs = _dest_ptrs("gemm_4bit_partial", outs, torch.float32, A.device, M, N, ldc, RuntimeError)
     if M == 0 or N == 0:
         return True
-    A = A.contiguous()
-    B = B.contiguous()
-    off = absmax_offset.to(dtype=torch.float32).contiguous() if absmax_offset is not None else None
     arr = (ct.c_void_p * len(ptrs))(*ptrs)
     with _on_device(A):
         rc = lib.cbnb_b200_gemm_4bit_partial(
@@ -771,18 +739,22 @@ def int8_quant_with_stats(A: torch.Tensor, row_stats: torch.Tensor, threshold: f
     return q
 
 
-def _dest_ptrs(what: str, outs, dtype: torch.dtype, device, need: int) -> list[int]:
-    """Device addresses of 1..8 destinations: tensors (checked: dtype, device, room for ``need`` elements) or raw
-    addresses of peers' symmetric-memory buffers, which the caller vouches for."""
+def _dest_ptrs(what: str, outs, dtype: torch.dtype, device, M: int, N: int, ldc: int, exc=ValueError) -> list[int]:
+    """Device addresses of 1..8 destinations of an [M, N] output at row stride ``ldc``: tensors (checked: dtype,
+    device, room for the output) or raw addresses of peers' symmetric-memory buffers, which the caller vouches for.
+    Raises ``exc`` (each public wrapper keeps its own exception type)."""
     if not 1 <= len(outs) <= 8:
-        raise ValueError(f"{what}: between 1 and 8 destinations, got {len(outs)}")
+        raise exc(f"{what}: between 1 and 8 destinations, got {len(outs)}")
+    if ldc < N:
+        raise exc(f"{what}: ldc ({ldc}) < N ({N})")
+    need = (M - 1) * ldc + N if M > 0 else 0
     ptrs = []
     for o in outs:
         if isinstance(o, torch.Tensor):
             if o.dtype != dtype or o.device != device:
-                raise ValueError(f"{what}: destinations must be {dtype} on {device}, got {o.dtype} on {o.device}")
+                raise exc(f"{what}: destinations must be {dtype} on {device}, got {o.dtype} on {o.device}")
             if o.untyped_storage().nbytes() // o.element_size() - o.storage_offset() < need:
-                raise ValueError(f"{what}: a destination needs {need} elements from its start")
+                raise exc(f"{what}: a destination needs {need} elements from its start")
             ptrs.append(o.data_ptr())
         else:
             ptrs.append(int(o))
@@ -820,8 +792,6 @@ def int8_gemm_multi_out(CA, CB, SCA, SCB, outs, ldc: int, dtype: Optional[torch.
         raise ValueError(f"int8_gemm_multi_out: CA {tuple(CA.shape)} does not match CB {tuple(CB.shape)}")
     M = CA.numel() // K if K else 0
     _check_sizes("int8_gemm_multi_out", M, N, K, ldc)
-    if ldc < N:
-        raise ValueError(f"int8_gemm_multi_out: ldc ({ldc}) < N ({N})")
     if dtype is None:
         if bias is not None or subA is not None or subBT is not None:
             raise ValueError("int8_gemm_multi_out: the int32 form takes no bias and no outlier operands")
@@ -835,7 +805,7 @@ def int8_gemm_multi_out(CA, CB, SCA, SCB, outs, ldc: int, dtype: Optional[torch.
     else:
         raise ValueError(f"int8_gemm_multi_out: dtype must be None, float16 or bfloat16, got {dtype}")
     jpad = _outlier_operands("int8_gemm_multi_out", subA, subBT, M, N, dtype)
-    ptrs = _dest_ptrs("int8_gemm_multi_out", outs, out_dtype, CA.device, (M - 1) * ldc + N if M > 0 else 0)
+    ptrs = _dest_ptrs("int8_gemm_multi_out", outs, out_dtype, CA.device, M, N, ldc)
     if M == 0 or N == 0:
         return True
     CA, CB = CA.contiguous(), CB.contiguous()

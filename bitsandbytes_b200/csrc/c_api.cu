@@ -47,7 +47,8 @@ bool launch_optimizer8bit_blockwise_list_dev(int opt, int dtype, const OptimTens
                                              const float* lr_dev, const float* q1, const float* q2, float gnorm_scale,
                                              bool skip_zeros, cudaStream_t st);
 
-// PART = true: the partial instances (fp32 accumulators to every destination of a PartialOuts, no bias, no rounding)
+// PART = true: the partial instances (fp32 accumulators to every destination of an OutList<float>, no bias, no
+// rounding)
 template <typename T, bool PART = false>
 void launch_gemv4_simt(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
                        const float* absmax_code, const float* absmax_offset, const float* lut16, int quant_type,
@@ -59,14 +60,14 @@ bool launch_gemv4_mma(const T* A, const uint8_t* B, const float* absmax, const u
                       const T* bias, int M, int N, int K, int ldc, int blocksize, int quant_type, cudaStream_t stream);
 template <typename T, bool PART = false>
 bool launch_gemm4_tc(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
-                     const float* absmax_code, const float* absmax_offset, typename OutArg<T, PART>::type out,
+                     const float* absmax_code, const float* absmax_offset, const OutList<OutElem<T, PART>>& outs,
                      const T* bias, int M, int N, int K, int ldc, int blocksize, int quant_type, cudaStream_t stream,
-                     void* const* peers = nullptr, int n_peers = 0, int mt_override = 0, int force_splits = 0);
+                     int mt_override = 0, int force_splits = 0);
 template <typename T, bool PART = false>
 bool launch_gemm4_staged(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
-                         const float* absmax_code, const float* absmax_offset, typename OutArg<T, PART>::type out,
+                         const float* absmax_code, const float* absmax_offset, const OutList<OutElem<T, PART>>& outs,
                          const T* bias, int M, int N, int K, int ldc, int blocksize, int quant_type,
-                         cudaStream_t stream, void* const* peers, int n_peers, int mt_override, int panel_rows);
+                         cudaStream_t stream, int mt_override = 0, int panel_rows = 0);
 // partials.cu
 bool launch_reduce_partials(const float* parts, int world, long long part_stride, void* out, const void* bias, int M,
                             int N, int ldc, int dtype, cudaStream_t stream);
@@ -264,43 +265,84 @@ static bool staged_route(int M, int N, int K, int blocksize, int dtype) {
     return staged_waves > 0 && tiles >= sms && staged_waves <= (tiles + sms - 1) / sms;
 }
 
-// PART: the partial form (cbnb_b200_gemm_4bit_partial), the same kernel choice with the partial instances
-template <typename T, bool PART = false>
-static void gemm_4bit_dispatch(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
-                               const float* absmax_code, const float* absmax_offset,
-                               typename OutArg<T, PART>::type out, const T* bias, int M, int N, int K, int ldc,
-                               int blocksize, int quant_type, int dtype, cudaStream_t stream) {
-    if (M <= 0 || N <= 0) return;
+template <typename TO> static OutList<TO> as_list(TO* out) { return OutList<TO>{{out}, 1}; }
+template <typename TO> static const OutList<TO>& as_list(const OutList<TO>& outs) { return outs; }
+
+// outs[0..n) of a C entry, which has checked 1 <= n <= kMaxOuts
+template <typename TO, typename P> static OutList<TO> out_list(P const* outs, int n) {
+    OutList<TO> l{};
+    for (int i = 0; i < n; ++i) l.p[i] = (TO*)outs[i];
+    l.n = n;
+    return l;
+}
+
+// The 4-bit GEMM of the plain, multi-destination and partial entries.  out: T* (one destination of T), OutList<T> (a
+// list of destinations of T) or, for the partial instances (PART), OutList<float>.  Returns false, with nothing
+// computed, for a bad quant_type (the error message set) or for a list of T that no kernel serves.
+template <typename T, bool PART = false, typename Out = typename OutArg<T, PART>::type>
+static bool gemm_4bit_dispatch(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
+                               const float* absmax_code, const float* absmax_offset, Out out, const T* bias, int M,
+                               int N, int K, int ldc, int blocksize, int quant_type, int dtype, cudaStream_t stream) {
+    if (M <= 0 || N <= 0) return true;
     if (quant_type != kFP4 && quant_type != kNF4) {
         set_last_error_msg("gemm_4bit: quant_type must be 1 (FP4) or 2 (NF4)");
-        return;
+        return false;
     }
-    const int path = choose_path(M, N, K, blocksize, dtype);
+    // The GEMV, the mma.sync decode kernel and the CUDA-core kernel store to one destination of T.  A list of T, even
+    // of one destination, therefore takes path 1 (staged or fused, by staged_route) wherever the wgmma GEMM serves the
+    // shape, and is refused elsewhere.  At M <= 8 the plain call takes path 0 or 3 instead, so there a list's
+    // destinations do not hold the plain call's bits.
+    constexpr bool kList = !PART && std::is_same<Out, OutList<T>>::value;
+    int path = 1;
+    if constexpr (kList) {
+        if (!tc_shape_ok(M, N, K, blocksize, dtype)) return false;
+    } else {
+        path = choose_path(M, N, K, blocksize, dtype);
+    }
+    const OutList<OutElem<T, PART>>& outs = as_list(out);
     if (path == 1 && staged_route(M, N, K, blocksize, dtype)) {
         if constexpr (!std::is_same<T, float>::value) {
-            if (launch_gemm4_staged<T, PART>(A, B, absmax, absmax_8bit, absmax_code, absmax_offset, out, bias, M, N, K,
-                                             ldc, blocksize, quant_type, stream, nullptr, 0, 0, 0))
-                return;
+            if (launch_gemm4_staged<T, PART>(A, B, absmax, absmax_8bit, absmax_code, absmax_offset, outs, bias, M, N,
+                                             K, ldc, blocksize, quant_type, stream))
+                return true;
         }
     }
-    if (path == 3) {
-        if constexpr (!std::is_same<T, float>::value) {
+    if constexpr (!kList && !std::is_same<T, float>::value) {
+        if (path == 3) {
             if (launch_gemv4_mma<T, PART>(A, B, absmax, absmax_8bit, absmax_code, absmax_offset, out, bias, M, N, K,
                                           ldc, blocksize, quant_type, stream))
-                return;
-            if (launch_gemm4_tc<T, PART>(A, B, absmax, absmax_8bit, absmax_code, absmax_offset, out, bias, M, N, K,
+                return true;
+            if (launch_gemm4_tc<T, PART>(A, B, absmax, absmax_8bit, absmax_code, absmax_offset, outs, bias, M, N, K,
                                          ldc, blocksize, quant_type, stream))
-                return;
+                return true;
         }
     }
-    if (path == 1) {
-        // (fp32 takes path 1 only as dtype 3: the TF32 instance)
-        if (launch_gemm4_tc<T, PART>(A, B, absmax, absmax_8bit, absmax_code, absmax_offset, out, bias, M, N, K, ldc,
-                                     blocksize, quant_type, stream))
-            return;
+    // (fp32 takes path 1 only as dtype 3: the TF32 instance)
+    if (path == 1 && launch_gemm4_tc<T, PART>(A, B, absmax, absmax_8bit, absmax_code, absmax_offset, outs, bias, M, N,
+                                              K, ldc, blocksize, quant_type, stream))
+        return true;
+    if constexpr (kList) {
+        return false;
+    } else {
+        launch_gemv4_simt<T, PART>(A, B, absmax, absmax_8bit, absmax_code, absmax_offset, nullptr, quant_type, out,
+                                   bias, M, N, K, ldc, blocksize, stream);
+        return true;
     }
-    launch_gemv4_simt<T, PART>(A, B, absmax, absmax_8bit, absmax_code, absmax_offset, nullptr, quant_type, out, bias,
-                               M, N, K, ldc, blocksize, stream);
+}
+
+// The element type of the ABI's dtype id (0 and 3 fp32, 1 fp16, 2 bf16): calls f(T()) and returns true for an id in
+// the entry's kIds (bits 1 << id), false for any other.
+constexpr unsigned kIdF16 = 1u << 1, kIdBF16 = 1u << 2, kIdTF32 = 1u << 3, kIdAny = 0xfu;
+template <unsigned kIds, typename F> static bool with_dtype(int dtype, F&& f) {
+    if (dtype < 0 || dtype > 3 || (kIds & (1u << dtype)) == 0) return false;
+    if (dtype == 1) {
+        f(__half());
+    } else if (dtype == 2) {
+        f(__nv_bfloat16());
+    } else if constexpr ((kIds & (1u | kIdTF32)) != 0) {
+        f(float());
+    }
+    return true;
 }
 
 } // namespace bnb200
@@ -398,18 +440,12 @@ void cbnb_b200_gemm_4bit_strided(const void* A, const uint8_t* B, const float* a
                                  const float* absmax_code, const float* absmax_offset, void* out, const void* bias,
                                  int M, int N, int K, int ldc, int blocksize, int quant_type, int dtype,
                                  cudaStream_t stream) {
-    if (dtype == 0 || dtype == 3)
-        gemm_4bit_dispatch<float>((const float*)A, B, absmax, absmax_8bit, absmax_code, absmax_offset, (float*)out,
-                                  (const float*)bias, M, N, K, ldc, blocksize, quant_type, dtype, stream);
-    else if (dtype == 1)
-        gemm_4bit_dispatch<__half>((const __half*)A, B, absmax, absmax_8bit, absmax_code, absmax_offset, (__half*)out,
-                                   (const __half*)bias, M, N, K, ldc, blocksize, quant_type, 1, stream);
-    else if (dtype == 2)
-        gemm_4bit_dispatch<__nv_bfloat16>((const __nv_bfloat16*)A, B, absmax, absmax_8bit, absmax_code, absmax_offset,
-                                          (__nv_bfloat16*)out, (const __nv_bfloat16*)bias, M, N, K, ldc, blocksize,
-                                          quant_type, 2, stream);
-    else
-        set_last_error_msg("gemm_4bit_strided: bad dtype");
+    const bool known = with_dtype<kIdAny>(dtype, [&](auto t) {
+        using T = decltype(t);
+        gemm_4bit_dispatch<T>((const T*)A, B, absmax, absmax_8bit, absmax_code, absmax_offset, (T*)out, (const T*)bias,
+                              M, N, K, ldc, blocksize, quant_type, dtype, stream);
+    });
+    if (!known) set_last_error_msg("gemm_4bit_strided: bad dtype");
 }
 
 // Fused all-gather: the tensor-core kernel's epilogue stores every output element to outs[0..n_outs)
@@ -420,33 +456,18 @@ int cbnb_b200_gemm_4bit_multi_out(const void* A, const uint8_t* B, const float* 
                                   const float* absmax_code, const float* absmax_offset, void* const* outs, int n_outs,
                                   const void* bias, int M, int N, int K, int ldc, int blocksize, int quant_type,
                                   int dtype, cudaStream_t stream) {
-    if (n_outs < 1 || n_outs > 8 || outs == nullptr) {
+    if (n_outs < 1 || n_outs > kMaxOuts || outs == nullptr) {
         set_last_error_msg("gemm_4bit_multi_out: 1 <= n_outs <= 8");
         return 1;
     }
     if (M <= 0 || N <= 0) return 0;
-    if (!tc_shape_ok(M, N, K, blocksize, dtype)) return 100;
-    // the route the plain call takes for this shape, so that every destination holds the same bits
-    if (staged_route(M, N, K, blocksize, dtype)) {
-        if (dtype == 1 && launch_gemm4_staged<__half>((const __half*)A, B, absmax, absmax_8bit, absmax_code,
-                                                      absmax_offset, (__half*)outs[0], (const __half*)bias, M, N, K,
-                                                      ldc, blocksize, quant_type, stream, outs + 1, n_outs - 1, 0, 0))
-            return 0;
-        if (dtype == 2 && launch_gemm4_staged<__nv_bfloat16>((const __nv_bfloat16*)A, B, absmax, absmax_8bit,
-                                                             absmax_code, absmax_offset, (__nv_bfloat16*)outs[0],
-                                                             (const __nv_bfloat16*)bias, M, N, K, ldc, blocksize,
-                                                             quant_type, stream, outs + 1, n_outs - 1, 0, 0))
-            return 0;
-    }
     bool ok = false;
-    if (dtype == 1)
-        ok = launch_gemm4_tc<__half>((const __half*)A, B, absmax, absmax_8bit, absmax_code, absmax_offset,
-                                     (__half*)outs[0], (const __half*)bias, M, N, K, ldc, blocksize, quant_type, stream,
-                                     outs + 1, n_outs - 1);
-    else if (dtype == 2)
-        ok = launch_gemm4_tc<__nv_bfloat16>((const __nv_bfloat16*)A, B, absmax, absmax_8bit, absmax_code,
-                                            absmax_offset, (__nv_bfloat16*)outs[0], (const __nv_bfloat16*)bias, M, N, K,
-                                            ldc, blocksize, quant_type, stream, outs + 1, n_outs - 1);
+    with_dtype<kIdF16 | kIdBF16>(dtype, [&](auto t) {
+        using T = decltype(t);
+        ok = gemm_4bit_dispatch<T, false, OutList<T>>((const T*)A, B, absmax, absmax_8bit, absmax_code, absmax_offset,
+                                                      out_list<T>(outs, n_outs), (const T*)bias, M, N, K, ldc,
+                                                      blocksize, quant_type, dtype, stream);
+    });
     return ok ? 0 : 100;
 }
 
@@ -458,25 +479,17 @@ int cbnb_b200_gemm_4bit_partial(const void* A, const uint8_t* B, const float* ab
                                 const float* absmax_code, const float* absmax_offset, float* const* outs, int n_outs,
                                 int M, int N, int K, int ldc, int blocksize, int quant_type, int dtype,
                                 cudaStream_t stream) {
-    if (n_outs < 1 || n_outs > kMaxPartialOuts || outs == nullptr) {
+    if (n_outs < 1 || n_outs > kMaxOuts || outs == nullptr) {
         set_last_error_msg("gemm_4bit_partial: 1 <= n_outs <= 8");
         return 1;
     }
-    if (dtype < 0 || dtype > 3) return 100;
-    PartialOuts po{};
-    for (int i = 0; i < n_outs; ++i) po.p[i] = outs[i];
-    po.n = n_outs;
-    if (dtype == 0 || dtype == 3)
-        gemm_4bit_dispatch<float, true>((const float*)A, B, absmax, absmax_8bit, absmax_code, absmax_offset, po,
-                                        nullptr, M, N, K, ldc, blocksize, quant_type, dtype, stream);
-    else if (dtype == 1)
-        gemm_4bit_dispatch<__half, true>((const __half*)A, B, absmax, absmax_8bit, absmax_code, absmax_offset, po,
-                                         nullptr, M, N, K, ldc, blocksize, quant_type, 1, stream);
-    else
-        gemm_4bit_dispatch<__nv_bfloat16, true>((const __nv_bfloat16*)A, B, absmax, absmax_8bit, absmax_code,
-                                                absmax_offset, po, nullptr, M, N, K, ldc, blocksize, quant_type, 2,
-                                                stream);
-    return 0;
+    const bool known = with_dtype<kIdAny>(dtype, [&](auto t) {
+        using T = decltype(t);
+        gemm_4bit_dispatch<T, true>((const T*)A, B, absmax, absmax_8bit, absmax_code, absmax_offset,
+                                    out_list<float>(outs, n_outs), nullptr, M, N, K, ldc, blocksize, quant_type, dtype,
+                                    stream);
+    });
+    return known ? 0 : 100;
 }
 
 // out[m, n] (row stride ldc) = T(((parts[0] + parts[1]) + ... + parts[world - 1])[m, n] + bias[n]): the partials
@@ -498,18 +511,11 @@ int cbnb_b200_gemm_4bit_pair(const void* A, const uint8_t* B, const float* absma
     if (M <= 0 || N <= 0) return 0;
     if (trace != nullptr || force_splits < 0) return 100;
     bool ok = false;
-    if (dtype == 1)
-        ok = launch_gemm4_tc<__half>((const __half*)A, B, absmax, absmax_8bit, absmax_code, absmax_offset,
-                                     (__half*)out, (const __half*)bias, M, N, K, ldc, blocksize, quant_type, stream,
-                                     nullptr, 0, mt, force_splits);
-    else if (dtype == 2)
-        ok = launch_gemm4_tc<__nv_bfloat16>((const __nv_bfloat16*)A, B, absmax, absmax_8bit, absmax_code,
-                                            absmax_offset, (__nv_bfloat16*)out, (const __nv_bfloat16*)bias, M, N, K,
-                                            ldc, blocksize, quant_type, stream, nullptr, 0, mt, force_splits);
-    else if (dtype == 3)
-        ok = launch_gemm4_tc<float>((const float*)A, B, absmax, absmax_8bit, absmax_code, absmax_offset, (float*)out,
-                                    (const float*)bias, M, N, K, ldc, blocksize, quant_type, stream, nullptr, 0, mt,
-                                    force_splits);
+    with_dtype<kIdF16 | kIdBF16 | kIdTF32>(dtype, [&](auto t) {
+        using T = decltype(t);
+        ok = launch_gemm4_tc<T>((const T*)A, B, absmax, absmax_8bit, absmax_code, absmax_offset, as_list((T*)out),
+                                (const T*)bias, M, N, K, ldc, blocksize, quant_type, stream, mt, force_splits);
+    });
     return ok ? 0 : 100;
 }
 
@@ -521,18 +527,15 @@ int cbnb_b200_gemm_4bit_staged(const void* A, const uint8_t* B, const float* abs
                                const float* absmax_code, const float* absmax_offset, void* const* outs, int n_outs,
                                const void* bias, int M, int N, int K, int ldc, int blocksize, int quant_type, int dtype,
                                int mt, int panel_rows, cudaStream_t stream) {
-    if (n_outs < 1 || n_outs > 8 || outs == nullptr) return 100;
+    if (n_outs < 1 || n_outs > kMaxOuts || outs == nullptr) return 100;
     if (M <= 0 || N <= 0) return 0;
     bool ok = false;
-    if (dtype == 1)
-        ok = launch_gemm4_staged<__half>((const __half*)A, B, absmax, absmax_8bit, absmax_code, absmax_offset,
-                                         (__half*)outs[0], (const __half*)bias, M, N, K, ldc, blocksize, quant_type,
-                                         stream, outs + 1, n_outs - 1, mt, panel_rows);
-    else if (dtype == 2)
-        ok = launch_gemm4_staged<__nv_bfloat16>((const __nv_bfloat16*)A, B, absmax, absmax_8bit, absmax_code,
-                                                absmax_offset, (__nv_bfloat16*)outs[0], (const __nv_bfloat16*)bias, M,
-                                                N, K, ldc, blocksize, quant_type, stream, outs + 1, n_outs - 1, mt,
-                                                panel_rows);
+    with_dtype<kIdF16 | kIdBF16>(dtype, [&](auto t) {
+        using T = decltype(t);
+        ok = launch_gemm4_staged<T>((const T*)A, B, absmax, absmax_8bit, absmax_code, absmax_offset,
+                                    out_list<T>(outs, n_outs), (const T*)bias, M, N, K, ldc, blocksize, quant_type,
+                                    stream, mt, panel_rows);
+    });
     return ok ? 0 : 100;
 }
 
@@ -546,26 +549,21 @@ int cbnb_b200_dequantize_4bit_panel(const uint8_t* B, const float* absmax, const
     if (K < 64 || (K % 64) != 0 || n0 < 0 || (n0 % 128) != 0 || blocksize < 32 || (blocksize & (blocksize - 1)) != 0 ||
         (quant_type != kNF4 && quant_type != kFP4) || (reinterpret_cast<uintptr_t>(B) & 15) != 0)
         return 100;
-    if (dtype == 1)
-        launch_dequantize4_panel<__half>(B, absmax, absmax_8bit, absmax_code, absmax_offset, (__half*)out, blocksize,
-                                         quant_type, n0, rows, K, stream);
-    else if (dtype == 2)
-        launch_dequantize4_panel<__nv_bfloat16>(B, absmax, absmax_8bit, absmax_code, absmax_offset,
-                                                (__nv_bfloat16*)out, blocksize, quant_type, n0, rows, K, stream);
-    else
-        return 100;
-    return 0;
+    const bool known = with_dtype<kIdF16 | kIdBF16>(dtype, [&](auto t) {
+        using T = decltype(t);
+        launch_dequantize4_panel<T>(B, absmax, absmax_8bit, absmax_code, absmax_offset, (T*)out, blocksize, quant_type,
+                                    n0, rows, K, stream);
+    });
+    return known ? 0 : 100;
 }
 
 int cbnb_b200_gemm_decoded(const void* A, const void* W, void* out, const void* bias, int M, int N, int K, int ldc,
                            int dtype, int mt, cudaStream_t stream) {
     bool ok = false;
-    if (dtype == 1)
-        ok = launch_gemm_decoded<__half>((const __half*)A, (const __half*)W, (__half*)out, (const __half*)bias, M, N, K,
-                                         ldc, mt, stream);
-    else if (dtype == 2)
-        ok = launch_gemm_decoded<__nv_bfloat16>((const __nv_bfloat16*)A, (const __nv_bfloat16*)W, (__nv_bfloat16*)out,
-                                                (const __nv_bfloat16*)bias, M, N, K, ldc, mt, stream);
+    with_dtype<kIdF16 | kIdBF16>(dtype, [&](auto t) {
+        using T = decltype(t);
+        ok = launch_gemm_decoded<T>((const T*)A, (const T*)W, (T*)out, (const T*)bias, M, N, K, ldc, mt, stream);
+    });
     return ok ? 0 : 100;
 }
 

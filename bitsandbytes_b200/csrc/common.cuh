@@ -14,6 +14,8 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 namespace bnb200 {
 
 // csrc/common.h:3-7 of the reference: DataType_t { General8bit = 0, FP4 = 1, NF4 = 2 }
@@ -214,21 +216,24 @@ void set_last_error_msg(const char* msg);
 
 int device_sm_count();
 
-// ---------------------------------------------------------------- partial outputs (cbnb_b200_gemm_4bit_partial)
-// The destinations of a partial 4-bit GEMM: the fp32 accumulators, with no bias and no rounding, stored to each of
-// p[0..n) at the same row stride (a row-sharded layer's slot in every rank's buffer).
-constexpr int kMaxPartialOuts = 8;
-struct PartialOuts {
-    float* p[kMaxPartialOuts];
+// ---------------------------------------------------------------- 4-bit GEMM destinations
+// The destinations of a 4-bit GEMM: every output element is stored to each of p[0..n) at the same row stride (a
+// sharded layer's slot in every rank's buffer).  OutList<float> carries the partial instances' fp32 accumulators
+// (cbnb_b200_gemm_4bit_partial), with no bias and no rounding.
+constexpr int kMaxOuts = 8;
+template <typename TO> struct OutList {
+    TO* p[kMaxOuts];
     int n;
 };
-// The output argument of a 4-bit GEMM kernel or launcher: T* (bias added, rounded once to T), or, for the partial
-// instances (PART), the fp32 destinations.
+// The element a 4-bit GEMM stores: T, or fp32 for the partial instances (PART)
+template <typename T, bool PART> using OutElem = typename std::conditional<PART, float, T>::type;
+// The output argument of a small-M 4-bit GEMM kernel or launcher: T* (bias added, rounded once to T), or, for the
+// partial instances (PART), the fp32 destinations.
 template <typename T, bool PART> struct OutArg {
     using type = T* __restrict__;
 };
 template <typename T> struct OutArg<T, true> {
-    using type = PartialOuts;
+    using type = OutList<float>;
 };
 
 // ---------------------------------------------------------------- optimizer tensor lists (optim.cu, c_api.cu)

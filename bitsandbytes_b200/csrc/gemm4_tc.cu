@@ -781,20 +781,15 @@ bool launch_mt(const T* A, Gemm4Params& p, int force_splits, cudaStream_t stream
 
 } // namespace
 
-// Returns true if the tensor-core path handled the call.
-// `peers` / `n_peers`: up to 7 additional output bases (same ldc) that receive a copy of every element.  (PART: the
-// destinations are `out`'s, and `peers` is not read.)
+// Returns true if the tensor-core path handled the call.  Every output element is stored to each of outs.p[0..n)
+// (same ldc).
 // `mt_override`: token tile (16 | 32 | 64 | 128 | 256, 0 = by M); `force_splits`: K split per tile (0 = by the grid).
 template <typename T, bool PART>
 bool launch_gemm4_tc(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
-                     const float* absmax_code, const float* absmax_offset, typename OutArg<T, PART>::type out,
+                     const float* absmax_code, const float* absmax_offset, const OutList<OutElem<T, PART>>& outs,
                      const T* bias, int M, int N, int K, int ldc, int blocksize, int quant_type, cudaStream_t stream,
-                     void* const* peers, int n_peers, int mt_override, int force_splits) {
-    if constexpr (PART) {
-        peers = reinterpret_cast<void* const*>(out.p + 1);
-        n_peers = out.n - 1;
-    }
-    if (n_peers < 0 || n_peers > 7) return false;
+                     int mt_override, int force_splits) {
+    if (outs.n < 1 || outs.n > kMaxOuts) return false;
     if (M <= 0 || N <= 0) return true;
     if (K < 64 || (K % 64) != 0) return false;
     if (blocksize < 32 || (blocksize & (blocksize - 1)) != 0) return false;
@@ -825,16 +820,16 @@ bool launch_gemm4_tc(const T* A, const uint8_t* B, const float* absmax, const ui
     p.absmax_code = absmax_code;
     p.absmax_offset = absmax_offset;
     p.bias = bias;
-    if constexpr (PART) p.out = out.p[0]; else p.out = out;
-    p.n_peers = n_peers;
-    for (int r = 0; r < n_peers; ++r) p.peer_out[r] = peers[r];
+    p.out = outs.p[0];
+    p.n_peers = outs.n - 1;
+    for (int r = 1; r < outs.n; ++r) p.peer_out[r - 1] = outs.p[r];
     p.M = M;
     p.N = N;
     p.K = K;
     p.ldc = ldc;
     p.log2_bs = ilog2_pow2(blocksize);
-    bool vec = (ldc % (16 / (int)sizeof(T))) == 0 && (reinterpret_cast<uintptr_t>(p.out) & 15) == 0;
-    for (int r = 0; r < n_peers; ++r) vec = vec && (reinterpret_cast<uintptr_t>(peers[r]) & 15) == 0;
+    bool vec = (ldc % (16 / (int)sizeof(T))) == 0;
+    for (int r = 0; r < outs.n; ++r) vec = vec && (reinterpret_cast<uintptr_t>(outs.p[r]) & 15) == 0;
     p.out_vec = vec ? 1 : 0;
 
 #define BNB200_DISPATCH_MT(QT, DQ)                                                                                     \
@@ -896,18 +891,14 @@ int staged_plan(int M, int N, int K, int sms, int* panel_rows) {
     return (int)best;
 }
 
-// panel_rows 0: the panel of staged_plan (DESIGN.md section 3.1).  PART: as in launch_gemm4_tc.
+// panel_rows 0: the panel of staged_plan (DESIGN.md section 3.1).  outs: as in launch_gemm4_tc.
 template <typename T, bool PART>
 bool launch_gemm4_staged(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
-                         const float* absmax_code, const float* absmax_offset, typename OutArg<T, PART>::type out,
+                         const float* absmax_code, const float* absmax_offset, const OutList<OutElem<T, PART>>& outs,
                          const T* bias, int M, int N, int K, int ldc, int blocksize, int quant_type,
-                         cudaStream_t stream, void* const* peers, int n_peers, int mt_override, int panel_rows) {
+                         cudaStream_t stream, int mt_override, int panel_rows) {
     static_assert(!std::is_same<T, float>::value, "the staged route has 16-bit instances only");
-    if constexpr (PART) {
-        peers = reinterpret_cast<void* const*>(out.p + 1);
-        n_peers = out.n - 1;
-    }
-    if (n_peers < 0 || n_peers > 7) return false;
+    if (outs.n < 1 || outs.n > kMaxOuts) return false;
     if (M <= 0 || N <= 0) return true;
     if (K < 64 || (K % 64) != 0) return false;
     if (blocksize < 32 || (blocksize & (blocksize - 1)) != 0) return false;
@@ -932,11 +923,8 @@ bool launch_gemm4_staged(const T* A, const uint8_t* B, const float* absmax, cons
         return false;
     }
     T* panel = reinterpret_cast<T*>(ws->ptr);
-    using TO = typename std::conditional<PART, float, T>::type;  // the output element
-    TO* out0;
-    if constexpr (PART) out0 = out.p[0]; else out0 = out;
-    bool vec = (ldc % (16 / (int)sizeof(T))) == 0 && (reinterpret_cast<uintptr_t>(out0) & 15) == 0;
-    for (int r = 0; r < n_peers; ++r) vec = vec && (reinterpret_cast<uintptr_t>(peers[r]) & 15) == 0;
+    bool vec = (ldc % (16 / (int)sizeof(T))) == 0;
+    for (int r = 0; r < outs.n; ++r) vec = vec && (reinterpret_cast<uintptr_t>(outs.p[r]) & 15) == 0;
     for (int n0 = 0; n0 < N; n0 += panel_rows) {
         const int rows = N - n0 < panel_rows ? N - n0 : panel_rows;
         launch_dequantize4_panel<T>(B, absmax, absmax_8bit, absmax_code, absmax_offset, panel, blocksize, quant_type,
@@ -945,9 +933,9 @@ bool launch_gemm4_staged(const T* A, const uint8_t* B, const float* absmax, cons
         Gemm4Params p{};
         p.B = reinterpret_cast<const uint8_t*>(panel);
         p.bias = bias != nullptr ? bias + n0 : nullptr;
-        p.out = out0 + n0;
-        p.n_peers = n_peers;
-        for (int r = 0; r < n_peers; ++r) p.peer_out[r] = reinterpret_cast<TO*>(peers[r]) + n0;
+        p.out = outs.p[0] + n0;
+        p.n_peers = outs.n - 1;
+        for (int r = 1; r < outs.n; ++r) p.peer_out[r - 1] = outs.p[r] + n0;
         p.M = M;
         p.N = rows;
         p.K = K;
@@ -961,14 +949,14 @@ bool launch_gemm4_staged(const T* A, const uint8_t* B, const float* absmax, cons
     return true;
 }
 
-#define BNB200_STAGED_INST(T, PART, OUT)                                                                               \
+#define BNB200_STAGED_INST(T, PART)                                                                                    \
     template bool launch_gemm4_staged<T, PART>(const T*, const uint8_t*, const float*, const uint8_t*, const float*,   \
-                                               const float*, OUT, const T*, int, int, int, int, int, int,              \
-                                               cudaStream_t, void* const*, int, int, int);
-BNB200_STAGED_INST(__nv_bfloat16, false, __nv_bfloat16*)
-BNB200_STAGED_INST(__half, false, __half*)
-BNB200_STAGED_INST(__nv_bfloat16, true, PartialOuts)
-BNB200_STAGED_INST(__half, true, PartialOuts)
+                                               const float*, const OutList<OutElem<T, PART>>&, const T*, int, int,     \
+                                               int, int, int, int, cudaStream_t, int, int);
+BNB200_STAGED_INST(__nv_bfloat16, false)
+BNB200_STAGED_INST(__half, false)
+BNB200_STAGED_INST(__nv_bfloat16, true)
+BNB200_STAGED_INST(__half, true)
 #undef BNB200_STAGED_INST
 
 // The staged GEMM alone on an already decoded weight W[N, K] (no workspace): for timing the route's phases.
@@ -995,16 +983,16 @@ template bool launch_gemm_decoded<__nv_bfloat16>(const __nv_bfloat16*, const __n
 template bool launch_gemm_decoded<__half>(const __half*, const __half*, __half*, const __half*, int, int, int, int, int,
                                           cudaStream_t);
 
-#define BNB200_TC_INST(T, PART, OUT)                                                                                   \
+#define BNB200_TC_INST(T, PART)                                                                                        \
     template bool launch_gemm4_tc<T, PART>(const T*, const uint8_t*, const float*, const uint8_t*, const float*,       \
-                                           const float*, OUT, const T*, int, int, int, int, int, int, cudaStream_t,    \
-                                           void* const*, int, int, int);
-BNB200_TC_INST(__nv_bfloat16, false, __nv_bfloat16*)
-BNB200_TC_INST(__half, false, __half*)
-BNB200_TC_INST(float, false, float*)  // fp32 activations and output, TF32 tensor cores
-BNB200_TC_INST(__nv_bfloat16, true, PartialOuts)
-BNB200_TC_INST(__half, true, PartialOuts)
-BNB200_TC_INST(float, true, PartialOuts)
+                                           const float*, const OutList<OutElem<T, PART>>&, const T*, int, int, int,    \
+                                           int, int, int, cudaStream_t, int, int);
+BNB200_TC_INST(__nv_bfloat16, false)
+BNB200_TC_INST(__half, false)
+BNB200_TC_INST(float, false)  // fp32 activations and output, TF32 tensor cores
+BNB200_TC_INST(__nv_bfloat16, true)
+BNB200_TC_INST(__half, true)
+BNB200_TC_INST(float, true)
 #undef BNB200_TC_INST
 
 } // namespace bnb200

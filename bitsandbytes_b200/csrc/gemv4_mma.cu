@@ -341,10 +341,10 @@ template bool launch_gemv4_mma<__half, false>(const __half*, const uint8_t*, con
                                               const float*, __half*, const __half*, int, int, int, int, int, int,
                                               cudaStream_t);
 template bool launch_gemv4_mma<__nv_bfloat16, true>(const __nv_bfloat16*, const uint8_t*, const float*, const uint8_t*,
-                                                    const float*, const float*, PartialOuts, const __nv_bfloat16*, int,
+                                                    const float*, const float*, OutList<float>, const __nv_bfloat16*, int,
                                                     int, int, int, int, int, cudaStream_t);
 template bool launch_gemv4_mma<__half, true>(const __half*, const uint8_t*, const float*, const uint8_t*, const float*,
-                                             const float*, PartialOuts, const __half*, int, int, int, int, int, int,
+                                             const float*, OutList<float>, const __half*, int, int, int, int, int, int,
                                              cudaStream_t);
 
 } // namespace bnb200

@@ -357,7 +357,7 @@ void launch_gemv4_simt(const T* A, const uint8_t* B, const float* absmax, const 
                                               const float*, const float*, int, T*, const T*, int, int, int, int, int,  \
                                               cudaStream_t);                                                           \
     template void launch_gemv4_simt<T, true>(const T*, const uint8_t*, const float*, const uint8_t*, const float*,     \
-                                             const float*, const float*, int, PartialOuts, const T*, int, int, int,    \
+                                             const float*, const float*, int, OutList<float>, const T*, int, int, int, \
                                              int, int, cudaStream_t);
 INST(float)
 INST(__half)

@@ -123,8 +123,7 @@ class ColumnParallelLinear4bit(torch.nn.Module):
 
     @classmethod
     def from_quantized(cls, packed, qs: F.QuantState, bias=None, group=None, gather_output=True):
-        world = dist.get_world_size(group) if dist.is_initialized() else 1
-        rank = dist.get_rank(group) if dist.is_initialized() else 0
+        world, rank = _group_world_rank(group)
         return cls(slice_quantized_weight(packed, qs, world, rank), qs.shape[0], bias, group, gather_output)
 
     def local_forward(self, x: torch.Tensor, out: Optional[torch.Tensor] = None, ldc: Optional[int] = None):
@@ -142,29 +141,59 @@ class ColumnParallelLinear4bit(torch.nn.Module):
         s = self.shard
         lead = x.shape[:-1]
         M = x.numel() // s.K
-        world = dist.get_world_size(self.group) if dist.is_initialized() else 1
+        world, _ = _group_world_rank(self.group)
         if world == 1 or not self.gather_output:
             return self.local_forward(x).view(*lead, s.rows)
-        if self._stage is None or self._stage.shape[1] != M or self._stage.dtype != x.dtype:
-            self._stage = torch.empty((world, M, s.rows), device=x.device, dtype=x.dtype)
-        rank = dist.get_rank(self.group)
-        self.local_forward(x, self._stage[rank], s.rows)
-        dist.all_gather_into_tensor(self._stage.view(-1), self._stage[rank].reshape(-1), group=self.group)
-        # [world, M, rows] -> [M, world*rows]
-        return self._stage.permute(1, 0, 2).reshape(*lead, world * s.rows)
+        return _gather_columns(self, x, M, x.dtype, x.device).reshape(*lead, world * s.rows)
 
 
-class PeerGather:
-    """Two symmetric-memory ``[M, N]`` output slots shared by the ranks of ``group``."""
+def _group_world_rank(group) -> tuple[int, int]:
+    if dist.is_initialized():
+        return dist.get_world_size(group), dist.get_rank(group)
+    return 1, 0
 
-    def __init__(self, M: int, N: int, dtype: torch.dtype, device, group: Optional[dist.ProcessGroup] = None):
+
+def _gather_columns(layer, inp, M: int, dtype: torch.dtype, device) -> torch.Tensor:
+    """The ``[M, world * rows]`` output of a column-parallel layer: ``layer.local_forward`` writes this rank's
+    ``[M, rows]`` block into its slot of a ``[world, M, rows]`` stage (kept on the layer for the next call), and the
+    stage is all-gathered.  The blocks sit side by side along the inner dimension of a row-major matrix, which
+    ``all_gather_into_tensor`` cannot write in place, hence the stage and the permute."""
+    world, rank = _group_world_rank(layer.group)
+    rows = layer.shard.rows
+    stage = layer._stage
+    if stage is None or stage.shape != (world, M, rows) or stage.dtype != dtype or stage.device != device:
+        stage = layer._stage = torch.empty((world, M, rows), device=device, dtype=dtype)
+    layer.local_forward(inp, stage[rank], rows)
+    dist.all_gather_into_tensor(stage.view(-1), stage[rank].reshape(-1), group=layer.group)
+    return stage.permute(1, 0, 2).reshape(M, world * rows)
+
+
+def _gather_partials(layer, inp, M: int, dtype: torch.dtype, device, what: str) -> torch.Tensor:
+    """The ``[world, M, N]`` partials of a row-parallel layer: ``layer.partial_forward`` writes this rank's into its
+    slot of a stage (kept on the layer for the next call), and the stage is all-gathered."""
+    world, rank = _group_world_rank(layer.group)
+    stage = layer._stage
+    if stage is None or stage.shape[:2] != (world, M) or stage.device != device:
+        stage = layer._stage = torch.empty((world, M, layer.shard.rows), device=device, dtype=dtype)
+    if not layer.partial_forward(inp, [stage[rank]]):
+        raise RuntimeError(f"{what} does not serve this shard shape")
+    if world > 1:
+        dist.all_gather_into_tensor(stage.view(-1), stage[rank].reshape(-1), group=layer.group)
+    return stage
+
+
+class _PeerSlots:
+    """Two symmetric-memory buffers of ``shape`` shared by the ranks of ``group``, used in turn, so that a rank may
+    start step i + 1 while a peer still reads step i."""
+
+    def __init__(self, shape, dtype: torch.dtype, device, group: Optional[dist.ProcessGroup]):
         import torch.distributed._symmetric_memory as symm_mem
 
         group = group if group is not None else dist.group.WORLD
-        self.M, self.N, self.dtype = M, N, dtype
+        self.dtype = dtype
         self.bufs, self.handles = [], []
         for _ in range(2):
-            t = symm_mem.empty((M, N), dtype=dtype, device=device)
+            t = symm_mem.empty(shape, dtype=dtype, device=device)
             self.handles.append(symm_mem.rendezvous(t, group))
             self.bufs.append(t)
         self.world = self.handles[0].world_size
@@ -177,6 +206,19 @@ class PeerGather:
         self.step += 1
         return self.bufs[i], [int(p) for p in self.handles[i].buffer_ptrs], self.handles[i]
 
+    def dest_ptrs(self, bases, offset: int) -> list[int]:
+        """The address ``offset`` bytes into every rank's buffer of a slot (``bases`` from :meth:`slot`): this rank's
+        own buffer first, as the multi-destination GEMMs take their local output, then the peers in rank order."""
+        return [bases[r] + offset for r in [self.rank] + [r for r in range(self.world) if r != self.rank]]
+
+
+class PeerGather(_PeerSlots):
+    """Two symmetric-memory ``[M, N]`` output slots shared by the ranks of ``group``."""
+
+    def __init__(self, M: int, N: int, dtype: torch.dtype, device, group: Optional[dist.ProcessGroup] = None):
+        super().__init__((M, N), dtype, device, group)
+        self.M, self.N = M, N
+
 
 def fused_forward(layer: "ColumnParallelLinear4bit", x: torch.Tensor, peers: PeerGather) -> torch.Tensor:
     """``layer(x)`` with the all-gather fused into the GEMM epilogue; returns this rank's [M, N] slot."""
@@ -185,17 +227,11 @@ def fused_forward(layer: "ColumnParallelLinear4bit", x: torch.Tensor, peers: Pee
     if M != peers.M or layer.out_features != peers.N or x.dtype != peers.dtype:
         raise ValueError("PeerGather was built for a different output shape / dtype")
     local, bases, handle = peers.slot()
-    col_bytes = s.row0 * local.element_size()
-    # own buffer first, then the peers
-    order = [peers.rank] + [r for r in range(peers.world) if r != peers.rank]
-    ptrs = [bases[r] + col_bytes for r in order]
+    ptrs = peers.dest_ptrs(bases, s.row0 * local.element_size())
     ok = gemm_4bit_multi_out(x, s.packed, (s.rows, s.K), s.absmax, s.blocksize, s.quant_type, layer.bias_shard,
                              s.absmax_8bit, s.absmax_code, s.absmax_offset, ptrs, peers.N)
     if not ok:  # shape outside the tensor-core kernel: local slice + NCCL all-gather into the same slot
-        stage = torch.empty((peers.world, M, s.rows), device=x.device, dtype=x.dtype)
-        layer.local_forward(x, stage[peers.rank], s.rows)
-        dist.all_gather_into_tensor(stage.view(-1), stage[peers.rank].reshape(-1), group=layer.group)
-        local.copy_(stage.permute(1, 0, 2).reshape(M, peers.N))
+        local.copy_(_gather_columns(layer, x, M, x.dtype, x.device))
     handle.barrier(channel=0)  # every rank's stores have landed everywhere
     return local
 
@@ -225,8 +261,7 @@ def slice_quantized_weight_k(packed: torch.Tensor, qs: F.QuantState, world: int,
     (:func:`nested_scales`): the shard decodes to the same weights bit for bit."""
     N, K = qs.shape
     bs = qs.blocksize
-    if world < 1 or not 0 <= rank < world:
-        raise ValueError(f"rank {rank} outside a world of {world}")
+    _check_rank(world, rank)
     if K % (world * bs) != 0:
         raise ValueError(f"in_features ({K}) must be a multiple of world * blocksize ({world} * {bs}) to shard by "
                          "input features")
@@ -259,8 +294,7 @@ class RowParallelLinear4bit(torch.nn.Module):
 
     @classmethod
     def from_quantized(cls, packed, qs: F.QuantState, bias=None, group=None, input_is_parallel=True):
-        world = dist.get_world_size(group) if dist.is_initialized() else 1
-        rank = dist.get_rank(group) if dist.is_initialized() else 0
+        world, rank = _group_world_rank(group)
         return cls(slice_quantized_weight_k(packed, qs, world, rank), qs.shape[1], bias, group, input_is_parallel)
 
     def local_input(self, x: torch.Tensor) -> torch.Tensor:
@@ -283,43 +317,20 @@ class RowParallelLinear4bit(torch.nn.Module):
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         s = self.shard
         x_r = self.local_input(x)
-        lead = x_r.shape[:-1]
         M = x_r.numel() // s.K
-        world = dist.get_world_size(self.group) if dist.is_initialized() else 1
-        rank = dist.get_rank(self.group) if dist.is_initialized() else 0
-        if self._stage is None or self._stage.shape[:2] != (world, M) or self._stage.device != x.device:
-            self._stage = torch.empty((world, M, s.rows), device=x.device, dtype=torch.float32)
-        if not self.partial_forward(x_r, [self._stage[rank]]):
-            raise RuntimeError("gemm_4bit_partial does not serve this shape or dtype")
-        if world > 1:
-            dist.all_gather_into_tensor(self._stage.view(-1), self._stage[rank].reshape(-1), group=self.group)
-        return reduce_partials(self._stage, x.dtype, self.bias).view(*lead, s.rows)
+        parts = _gather_partials(self, x_r, M, torch.float32, x.device, "gemm_4bit_partial")
+        return reduce_partials(parts, x.dtype, self.bias).view(*x_r.shape[:-1], s.rows)
 
 
-class PeerPartials:
+class PeerPartials(_PeerSlots):
     """Two symmetric-memory ``[world, M, N]`` partial slots shared by the ranks of ``group`` (fp32 for the 4-bit layer,
     int32 for the int8 one)."""
 
     def __init__(self, M: int, N: int, device, group: Optional[dist.ProcessGroup] = None,
                  dtype: torch.dtype = torch.float32):
-        import torch.distributed._symmetric_memory as symm_mem
-
-        group = group if group is not None else dist.group.WORLD
-        self.M, self.N, self.dtype = M, N, dtype
-        self.bufs, self.handles = [], []
-        for _ in range(2):
-            t = symm_mem.empty((dist.get_world_size(group), M, N), dtype=dtype, device=device)
-            self.handles.append(symm_mem.rendezvous(t, group))
-            self.bufs.append(t)
-        self.world = self.handles[0].world_size
-        self.rank = self.handles[0].rank
-        self.step = 0
-
-    def slot(self):
-        """(local [world, M, N] tensor, [base address of that slot on rank r for every r], handle) of the next step."""
-        i = self.step & 1
-        self.step += 1
-        return self.bufs[i], [int(p) for p in self.handles[i].buffer_ptrs], self.handles[i]
+        world, _ = _group_world_rank(group)
+        super().__init__((world, M, N), dtype, device, group)
+        self.M, self.N = M, N
 
 
 def fused_forward_row(layer: RowParallelLinear4bit, x: torch.Tensor, peers: PeerPartials) -> torch.Tensor:
@@ -331,11 +342,8 @@ def fused_forward_row(layer: RowParallelLinear4bit, x: torch.Tensor, peers: Peer
     if M != peers.M or s.rows != peers.N or peers.dtype != torch.float32:
         raise ValueError("PeerPartials was built for a different output shape or dtype")
     local, bases, handle = peers.slot()
-    off = peers.rank * M * s.rows * 4  # this rank's slot, in bytes
-    # own buffer first, then the peers
-    order = [peers.rank] + [r for r in range(peers.world) if r != peers.rank]
-    if not layer.partial_forward(x_r, [bases[r] + off for r in order]):
-        raise RuntimeError("gemm_4bit_partial does not serve this shape or dtype")
+    if not layer.partial_forward(x_r, peers.dest_ptrs(bases, peers.rank * M * s.rows * 4)):
+        raise RuntimeError("gemm_4bit_partial does not serve this shard shape")
     handle.barrier(channel=0)  # every rank's partial has landed everywhere
     return reduce_partials(local, x.dtype, layer.bias).view(*x_r.shape[:-1], s.rows)
 
@@ -399,12 +407,6 @@ def slice_int8_weight_k(CB: torch.Tensor, SCB: torch.Tensor, world: int, rank: i
     kr = K // world
     k0 = rank * kr
     return Shard8bit(CB=CB[:, k0:k0 + kr].contiguous(), SCB=SCB.contiguous(), rows=N, row0=0, K=kr, k0=k0)
-
-
-def _group_world_rank(group) -> tuple[int, int]:
-    if dist.is_initialized():
-        return dist.get_world_size(group), dist.get_rank(group)
-    return 1, 0
 
 
 def _state_of(module) -> tuple[torch.Tensor, torch.Tensor, float]:
@@ -518,7 +520,7 @@ class ColumnParallelLinear8bitLt(torch.nn.Module):
         lead = x.shape[:-1]
         q = self.quantize(x)
         M = q.A.shape[0]
-        world, rank = _group_world_rank(self.group)
+        world, _ = _group_world_rank(self.group)
         chain = q.J > _INT8_FUSED_J
         if world == 1:
             y = self.local_forward(q)
@@ -527,7 +529,7 @@ class ColumnParallelLinear8bitLt(torch.nn.Module):
             return y.view(*lead, s.rows)
         if not self.gather_output and not chain:
             return self.local_forward(q).view(*lead, s.rows)
-        full = self._gather(q, M, world, rank)
+        full = _gather_columns(self, q, M, q.A.dtype, q.A.device)
         if chain:
             rows = self.outlier_rows(q)
             subBT = torch.empty((world * s.rows, q.J), device=x.device, dtype=x.dtype)
@@ -536,15 +538,6 @@ class ColumnParallelLinear8bitLt(torch.nn.Module):
         if not self.gather_output:
             full = full[:, s.row0:s.row0 + s.rows].contiguous()
         return full.reshape(*lead, full.shape[-1])
-
-    def _gather(self, q: Int8Input, M: int, world: int, rank: int) -> torch.Tensor:
-        s = self.shard
-        dtype = q.A.dtype
-        if self._stage is None or self._stage.shape[1] != M or self._stage.dtype != dtype:
-            self._stage = torch.empty((world, M, s.rows), device=q.A.device, dtype=dtype)
-        self.local_forward(q, self._stage[rank], s.rows)
-        dist.all_gather_into_tensor(self._stage.view(-1), self._stage[rank].reshape(-1), group=self.group)
-        return self._stage.permute(1, 0, 2).reshape(M, world * s.rows)
 
 
 def fused_forward_col8(layer: ColumnParallelLinear8bitLt, x: torch.Tensor, peers: PeerGather) -> torch.Tensor:
@@ -557,11 +550,9 @@ def fused_forward_col8(layer: ColumnParallelLinear8bitLt, x: torch.Tensor, peers
     if M != peers.M or layer.out_features != peers.N or x.dtype != peers.dtype:
         raise ValueError("PeerGather was built for a different output shape / dtype")
     local, bases, handle = peers.slot()
-    col_bytes = s.row0 * local.element_size()
-    order = [peers.rank] + [r for r in range(peers.world) if r != peers.rank]
-    ok = q.J <= _INT8_FUSED_J and layer._gemm(q, [bases[r] + col_bytes for r in order], peers.N)
+    ok = q.J <= _INT8_FUSED_J and layer._gemm(q, peers.dest_ptrs(bases, s.row0 * local.element_size()), peers.N)
     if not ok:
-        full = layer._gather(q, M, peers.world, peers.rank)
+        full = _gather_columns(layer, q, M, q.A.dtype, q.A.device)
         if q.J > _INT8_FUSED_J:
             subBT = torch.empty((layer.out_features, q.J), device=x.device, dtype=x.dtype)
             dist.all_gather_into_tensor(subBT, layer.outlier_rows(q), group=layer.group)
@@ -699,27 +690,21 @@ class RowParallelLinear8bitLt(torch.nn.Module):
 
     def _prologue(self, x: torch.Tensor):
         x_r = self.local_input(x)
-        world, rank = _group_world_rank(self.group)
+        world, _ = _group_world_rank(self.group)
         st = self.local_stats(x_r)
         SCA = st.row_stats
         if world > 1:
             dist.all_reduce(SCA, op=dist.ReduceOp.MAX, group=self.group)
         CA, cols = self.local_codes(st, SCA)
-        return x_r, world, rank, SCA, CA, cols
+        return x_r, world, SCA, CA, cols
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         s = self.shard
         lead = x.shape[:-1]
-        x_r, world, rank, SCA, CA, cols = self._prologue(x)
-        M = x_r.shape[0]
-        if self._stage is None or self._stage.shape[:2] != (world, M) or self._stage.device != x.device:
-            self._stage = torch.empty((world, M, s.rows), device=x.device, dtype=torch.int32)
-        if not self.partial_forward(CA, [self._stage[rank]]):
-            raise RuntimeError("the int8 GEMM does not take this shard shape")
-        if world > 1:
-            dist.all_gather_into_tensor(self._stage.view(-1), self._stage[rank].reshape(-1), group=self.group)
+        x_r, world, SCA, CA, cols = self._prologue(x)
+        parts = _gather_partials(self, CA, x_r.shape[0], torch.int32, x.device, "the int8 GEMM")
         subA, subBT = self._exchange_outliers(x_r, cols, world)
-        return self.reduce(self._stage, SCA, x.dtype, subA, subBT).view(*lead, s.rows)
+        return self.reduce(parts, SCA, x.dtype, subA, subBT).view(*lead, s.rows)
 
 
 def fused_forward_row8(layer: RowParallelLinear8bitLt, x: torch.Tensor, peers: PeerPartials) -> torch.Tensor:
@@ -727,15 +712,13 @@ def fused_forward_row8(layer: RowParallelLinear8bitLt, x: torch.Tensor, peers: P
     of every rank's symmetric buffer, one barrier publishes them, and each rank reduces its own buffer.  The row
     statistics (a max) and the outlier operands still travel through NCCL."""
     s = layer.shard
-    x_r, world, rank, SCA, CA, cols = layer._prologue(x)
+    x_r, _, SCA, CA, cols = layer._prologue(x)
     M = x_r.shape[0]
     if M != peers.M or s.rows != peers.N or peers.dtype != torch.int32:
         raise ValueError("PeerPartials was built for a different output shape or dtype (int32 partials)")
     local, bases, handle = peers.slot()
-    off = peers.rank * M * s.rows * 4
-    order = [peers.rank] + [r for r in range(peers.world) if r != peers.rank]
-    if not layer.partial_forward(CA, [bases[r] + off for r in order]):
-        raise RuntimeError("the int8 GEMM does not take this shard shape")
+    if not layer.partial_forward(CA, peers.dest_ptrs(bases, peers.rank * M * s.rows * 4)):
+        raise RuntimeError("the int8 GEMM does not serve this shard shape")
     subA, subBT = layer._exchange_outliers(x_r, cols, peers.world)
     handle.barrier(channel=0)  # every rank's partial has landed everywhere
     return layer.reduce(local, SCA, x.dtype, subA, subBT).view(*x.shape[:-1], s.rows)

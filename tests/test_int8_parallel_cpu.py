@@ -1,5 +1,6 @@
 """CPU tests of the tensor-parallel LLM.int8() layers: the row and input-feature slices of a globally quantised weight,
-the sharding errors, and the argument checks of the native wrappers (against a fake library)."""
+the sharding errors, and the argument checks of the native wrappers (against a fake library), including the 4-bit
+multi-destination and partial GEMMs, and the destination order of the symmetric-memory slots."""
 import pytest
 import torch
 
@@ -140,3 +141,80 @@ def test_reduce_and_quant_checks(fake):
         cb.int8_outlier_operands(torch.zeros(4, 64, dtype=torch.float16), torch.zeros(32, 64, dtype=torch.int8),
                                  torch.ones(32), torch.arange(5), jpad=4)
     assert fake.calls == []
+
+
+def _gemm4_args(M=8, N=32, K=64, dtype=torch.bfloat16):
+    """(A, B, shapeB, absmax, blocksize, quant_type) of an NF4 weight [N, K], blocksize 64."""
+    return (torch.zeros(M, K, dtype=dtype), torch.zeros(N * K // 2, dtype=torch.uint8), (N, K),
+            torch.ones(N * K // 64), 64, "nf4")
+
+
+def test_gemm_4bit_multi_out_checks(fake):
+    """The fused all-gather wrapper checks its operands and destinations as the plain GEMM does, before any native
+    call; a raw address is the caller's to vouch for."""
+    A, B, shapeB, absmax, bs, qt = _gemm4_args()
+
+    def call(*, A=A, shapeB=shapeB, bs=bs, qt=qt, bias=None, outs=(0x1000, 0x2000), ldc=32):
+        return cb.gemm_4bit_multi_out(A, B, shapeB, absmax, bs, qt, bias, None, None, None, list(outs), ldc)
+
+    assert call() and call(outs=[torch.zeros(8, 32, dtype=torch.bfloat16)])
+    assert fake.calls == ["cbnb_b200_gemm_4bit_multi_out"] * 2
+    for kwargs, match in [({"bs": 48}, "blocksize"), ({"qt": "int4"}, "quant_type"), ({"shapeB": (32, 128)}, "inner"),
+                          ({"outs": []}, "between 1 and 8"), ({"outs": [0x1000] * 9}, "between 1 and 8"),
+                          ({"ldc": 31}, "ldc"), ({"bias": torch.zeros(32)}, "bias"),
+                          ({"outs": [torch.zeros(8, 32)]}, "bfloat16"),
+                          ({"outs": [torch.zeros(7 * 32 + 31, dtype=torch.bfloat16)]}, "elements")]:
+        with pytest.raises(RuntimeError, match=match):
+            call(**kwargs)
+    assert not call(A=A.float())  # fp32 activations do not take the wgmma kernel: the caller falls back
+    assert fake.calls == ["cbnb_b200_gemm_4bit_multi_out"] * 2
+
+
+def test_destination_checks_keep_each_wrappers_exception(fake):
+    """The 4-bit partial GEMM raises RuntimeError and the int8 multi-destination GEMM ValueError for the same bad
+    destination lists."""
+    A, B, shapeB, absmax, bs, qt = _gemm4_args()
+    CA, CB, _, _ = _gemm_args()
+    f32, i32 = torch.zeros(8, 32), torch.zeros(8, 32, dtype=torch.int32)
+    assert cb.gemm_4bit_partial(A, B, shapeB, absmax, bs, qt, None, None, None, [f32] * 8, 32)
+    assert cb.int8_gemm_multi_out(CA, CB, None, None, [i32] * 8, 32, None)
+    short = 7 * 32 + 31  # one element less than an [8, 32] output needs
+    for outs, ldc in [([f32] * 9, 32), ([], 32), ([f32], 31), ([torch.zeros(short)], 32), ([i32], 32)]:
+        with pytest.raises(RuntimeError):
+            cb.gemm_4bit_partial(A, B, shapeB, absmax, bs, qt, None, None, None, outs, ldc)
+    for outs, ldc in [([i32] * 9, 32), ([], 32), ([i32], 31), ([torch.zeros(short, dtype=torch.int32)], 32), ([f32], 32)]:
+        with pytest.raises(ValueError):
+            cb.int8_gemm_multi_out(CA, CB, None, None, outs, ldc, None)
+    assert fake.calls == ["cbnb_b200_gemm_4bit_partial", "cbnb_b200_int8_gemm_multi_out"]
+
+
+@pytest.mark.parametrize("world", [1, 2, 3, 8])
+def test_peer_slots_list_the_own_buffer_first(monkeypatch, world):
+    """For every rank of a simulated world, the destination list of a symmetric-memory slot is this rank's own buffer
+    at the offset, then the peers' in rank order, and successive steps alternate between the two slots."""
+    import torch.distributed._symmetric_memory as symm_mem
+
+    import bitsandbytes_b200.parallel as par
+
+    class Handle:
+        def __init__(self, slot, rank):
+            self.world_size, self.rank = world, rank
+            self.buffer_ptrs = [(slot + 1) * 1_000_000 + r * 10_000 for r in range(world)]
+
+    for rank in range(world):
+        made = []
+        monkeypatch.setattr(par, "_group_world_rank", lambda group: (world, rank))
+        monkeypatch.setattr(symm_mem, "empty", lambda shape, dtype, device: torch.empty(shape, dtype=dtype))
+        monkeypatch.setattr(symm_mem, "rendezvous", lambda t, group: made.append(t) or Handle(len(made) - 1, rank))
+        gather = par.PeerGather(4, 16, torch.bfloat16, "cpu")
+        parts = par.PeerPartials(4, 16, "cpu", dtype=torch.int32)
+        assert (gather.M, gather.N, gather.dtype, gather.world, gather.rank) == (4, 16, torch.bfloat16, world, rank)
+        assert (parts.M, parts.N, parts.dtype, parts.world, parts.rank) == (4, 16, torch.int32, world, rank)
+        assert parts.bufs[0].shape == (world, 4, 16) and gather.bufs[0].shape == (4, 16)
+        order = [rank] + [r for r in range(world) if r != rank]
+        for peers, slot0 in ((gather, 0), (parts, 2)):
+            for step in range(3):
+                local, bases, _ = peers.slot()
+                assert local is peers.bufs[step & 1]
+                assert bases == [(slot0 + (step & 1) + 1) * 1_000_000 + r * 10_000 for r in range(world)]
+                assert peers.dest_ptrs(bases, 96) == [bases[r] + 96 for r in order]
