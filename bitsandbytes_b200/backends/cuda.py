@@ -289,6 +289,33 @@ def gemm_4bit_partial(A, B, shapeB, absmax, blocksize: int, quant_type: str, abs
     return rc == 0
 
 
+def gemm_4bit_partial_scatter(A, B, shapeB, absmax, blocksize: int, quant_type: str, absmax_8bit, absmax_code,
+                              absmax_offset, outs, ldc: int) -> bool:
+    """:func:`gemm_4bit_partial` with the rows scattered over ``outs`` in rank order instead of copied to each: with
+    ``w = len(outs)`` and ``M`` rows, row ``m`` is stored to ``outs[m // (M/w)]`` at row ``m % (M/w)`` (row stride
+    ``ldc``), the partial of a sequence-parallel layer whose rank s owns tokens ``[s*M/w, (s+1)*M/w)``.  Same kernel,
+    K split and fp32 sums as :func:`gemm_4bit_partial`.  ``M % w == 0`` is required."""
+    A, B, off, M, N, K = _gemm_4bit_operands("gemm_4bit_partial_scatter", A, B, shapeB, absmax, blocksize, quant_type,
+                                             None, absmax_8bit, absmax_code, absmax_offset, ldc)
+    n = len(outs)
+    if n < 1 or M < n or M % n != 0:
+        raise RuntimeError(f"gemm_4bit_partial_scatter: {M} rows do not split evenly over {n} destinations")
+    ptrs = _dest_ptrs("gemm_4bit_partial_scatter", outs, torch.float32, A.device, M // n, N, ldc, RuntimeError)
+    if N == 0:
+        return True
+    arr = (ct.c_void_p * n)(*ptrs)
+    with _on_device(A):
+        rc = lib.cbnb_b200_gemm_4bit_partial_scatter(
+            A.data_ptr(), B.data_ptr(), absmax.data_ptr(),
+            absmax_8bit.data_ptr() if absmax_8bit is not None else None,
+            absmax_code.data_ptr() if absmax_code is not None else None,
+            off.data_ptr() if off is not None else None,
+            ct.cast(arr, ct.c_void_p), n, M // n, M, N, K, ldc, blocksize, _QT_ID[quant_type],
+            gemm_4bit_dtype_id(A.dtype), _stream(A))
+    lib.check("gemm_4bit_partial_scatter")
+    return rc == 0
+
+
 def reduce_partials(parts: torch.Tensor, dtype: torch.dtype, bias: Optional[torch.Tensor] = None,
                     out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """``out = dtype((((parts[0] + parts[1]) + ...) + parts[w-1]) + bias)``: the ``[w, M, N]`` fp32 partials of a

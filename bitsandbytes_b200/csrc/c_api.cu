@@ -492,6 +492,31 @@ int cbnb_b200_gemm_4bit_partial(const void* A, const uint8_t* B, const float* ab
     return known ? 0 : 100;
 }
 
+// The partial GEMM of a sequence-parallel row-sharded layer: cbnb_b200_gemm_4bit_partial with the rows scattered
+// instead of copied.  Row m is stored to outs[m / rows_per_out] at row m % rows_per_out (row stride ldc, fp32), so
+// outs is in rank order: outs[s] receives the tokens of rank s.  Same kernel and K split as the partial entry.
+// Returns 0, 1 unless 1 <= n_outs <= 8, rows_per_out >= 1 and n_outs * rows_per_out == M, or 100 for a bad dtype.
+int cbnb_b200_gemm_4bit_partial_scatter(const void* A, const uint8_t* B, const float* absmax,
+                                        const uint8_t* absmax_8bit, const float* absmax_code,
+                                        const float* absmax_offset, float* const* outs, int n_outs, int rows_per_out,
+                                        int M, int N, int K, int ldc, int blocksize, int quant_type, int dtype,
+                                        cudaStream_t stream) {
+    if (n_outs < 1 || n_outs > kMaxOuts || outs == nullptr || rows_per_out < 1 ||
+        (long long)n_outs * rows_per_out != M) {
+        set_last_error_msg("gemm_4bit_partial_scatter: needs 1 <= n_outs <= 8, rows_per_out >= 1 and "
+                           "n_outs * rows_per_out == M");
+        return 1;
+    }
+    OutList<float> list = out_list<float>(outs, n_outs);
+    list.rows_per_out = rows_per_out;
+    const bool known = with_dtype<kIdAny>(dtype, [&](auto t) {
+        using T = decltype(t);
+        gemm_4bit_dispatch<T, true>((const T*)A, B, absmax, absmax_8bit, absmax_code, absmax_offset, list, nullptr, M,
+                                    N, K, ldc, blocksize, quant_type, dtype, stream);
+    });
+    return known ? 0 : 100;
+}
+
 // out[m, n] (row stride ldc) = T(((parts[0] + parts[1]) + ... + parts[world - 1])[m, n] + bias[n]): the partials
 // [M, N] (row stride N, one every part_stride elements) summed in rank order in fp32, the bias added in fp32, one
 // rounding.  dtype 0 or 3 = fp32, 1 = fp16, 2 = bf16.  Returns 0, or 100 for a dtype or world it does not serve.

@@ -219,12 +219,26 @@ int device_sm_count();
 // ---------------------------------------------------------------- 4-bit GEMM destinations
 // The destinations of a 4-bit GEMM: every output element is stored to each of p[0..n) at the same row stride (a
 // sharded layer's slot in every rank's buffer).  OutList<float> carries the partial instances' fp32 accumulators
-// (cbnb_b200_gemm_4bit_partial), with no bias and no rounding.
+// (cbnb_b200_gemm_4bit_partial), with no bias and no rounding.  rows_per_out > 0 (the partial instances only,
+// cbnb_b200_gemm_4bit_partial_scatter) scatters the rows instead: row m goes to p[m / rows_per_out] only, at row
+// m % rows_per_out, so that each rank of a sequence-parallel layer receives its own tokens.
 constexpr int kMaxOuts = 8;
 template <typename TO> struct OutList {
     TO* p[kMaxOuts];
     int n;
+    int rows_per_out;  // 0: every row to every destination
 };
+
+// The partial instances' store of element (m, n) of the fp32 output: to every destination of `outs`, or, with
+// rows_per_out > 0, to destination m / rows_per_out at row m % rows_per_out.
+__device__ __forceinline__ void store_partial(const OutList<float>& outs, int m, int n, long long ldc, float v) {
+    if (outs.rows_per_out > 0) {
+        const int d = m / outs.rows_per_out;
+        outs.p[d][(m - d * outs.rows_per_out) * ldc + n] = v;
+    } else {
+        for (int d = 0; d < outs.n; ++d) outs.p[d][m * ldc + n] = v;
+    }
+}
 // The element a 4-bit GEMM stores: T, or fp32 for the partial instances (PART)
 template <typename T, bool PART> using OutElem = typename std::conditional<PART, float, T>::type;
 // The output argument of a small-M 4-bit GEMM kernel or launcher: T* (bias added, rounded once to T), or, for the

@@ -46,7 +46,8 @@
 //
 // PART is the partial instance (cbnb_b200_gemm_4bit_partial, a row-sharded layer's K slice): the output and its
 // copies are fp32, and the epilogue stores the accumulators -- the split order's sums under split-K -- with no bias
-// and no rounding, straight from the fragments.
+// and no rounding, straight from the fragments.  With rows_per_out > 0 (cbnb_b200_gemm_4bit_partial_scatter, a
+// sequence-parallel layer) each output row goes to one copy only, the one of the rank that owns the token.
 #include "common.cuh"
 #include "decode4.cuh"
 #include "hopper_ptx.cuh"
@@ -96,7 +97,22 @@ struct Gemm4Params {
     int n_tiles;                 // N tiles of 128 (tile = m_tile * n_tiles + n_tile)
     int tiles_total;
     int splits;                  // K splits per tile (1 = none)
+    int rows_per_out;            // PART only: 0 = every row to out and the peers; > 0 = row m to copy m / rows_per_out
+                                 //   (0 = out, d = peer_out[d - 1]) at row m % rows_per_out (OutList::rows_per_out)
 };
+
+// The partial instances' store of element (m, n) of the fp32 output (m < M, n < N), routed as p.rows_per_out says.
+__device__ __forceinline__ void store_partial(const Gemm4Params& p, int m, int n, float v) {
+    if (p.rows_per_out > 0) {
+        const int d = m / p.rows_per_out;
+        float* dst = reinterpret_cast<float*>(d == 0 ? p.out : p.peer_out[d - 1]);
+        dst[(long long)(m - d * p.rows_per_out) * p.ldc + n] = v;
+    } else {
+        const long long o = (long long)m * p.ldc + n;
+        reinterpret_cast<float*>(p.out)[o] = v;
+        for (int r = 0; r < p.n_peers; ++r) reinterpret_cast<float*>(p.peer_out[r])[o] = v;
+    }
+}
 
 // the staged instance: D[64 x MT] += A[64 x 16] * X[MT x 16]^T with both operands from descriptors
 template <typename T, int MT>
@@ -430,6 +446,19 @@ __global__ void __launch_bounds__(kThreads, 1)
             // a warp instruction stores four 32-byte row pieces: whole sectors, without the staging buffer, which at
             // fp32 would not fit next to the 256-token tile's ring
             if (splits == 1) {
+                // When every row of the tile goes to one destination (one destination; or, scattered, a tile inside
+                // one rank's tokens) its base is found once per tile, not per element as store_partial does.
+                float* dst = nullptr;
+                long long dst_off = 0;
+                if (p.rows_per_out == 0) {
+                    if (p.n_peers == 0) dst = reinterpret_cast<float*>(p.out);
+                } else {
+                    const int d = m0 / p.rows_per_out;
+                    if ((min(m0 + MT, p.M) - 1) / p.rows_per_out == d) {
+                        dst = reinterpret_cast<float*>(d == 0 ? p.out : p.peer_out[d - 1]);
+                        dst_off = (long long)d * p.rows_per_out * p.ldc;
+                    }
+                }
 #pragma unroll
                 for (int j = 0; j < MT / 8; ++j)
 #pragma unroll
@@ -437,9 +466,8 @@ __global__ void __launch_bounds__(kThreads, 1)
                         const int m = m0 + 8 * j + 2 * t + (e & 1);
                         const int n = e >= 2 ? nb : na;
                         if (m < p.M && n < p.N) {
-                            const long long o = (long long)m * p.ldc + n;
-                            reinterpret_cast<float*>(p.out)[o] = acc[4 * j + e];
-                            for (int r = 0; r < p.n_peers; ++r) reinterpret_cast<float*>(p.peer_out[r])[o] = acc[4 * j + e];
+                            if (dst != nullptr) dst[(long long)m * p.ldc + n - dst_off] = acc[4 * j + e];
+                            else store_partial(p, m, n, acc[4 * j + e]);
                         }
                     }
                 continue;
@@ -566,9 +594,7 @@ __global__ void __launch_bounds__(kThreads, 1)
                 for (int sp = 0; sp < splits; ++sp) a += __ldcg(ws_tile + ((long long)sp * MT + c) * kTileN + rn);
                 if (nn < p.N) {
                     if constexpr (PART) {
-                        const long long idx = (long long)m * p.ldc + nn;
-                        reinterpret_cast<float*>(p.out)[idx] = a;
-                        for (int r = 0; r < p.n_peers; ++r) reinterpret_cast<float*>(p.peer_out[r])[idx] = a;
+                        store_partial(p, m, nn, a);
                     } else {
                         const T val = DT<T>::from_f32(a + bias_r);
                         const long long idx = (long long)m * p.ldc + nn;
@@ -823,6 +849,7 @@ bool launch_gemm4_tc(const T* A, const uint8_t* B, const float* absmax, const ui
     p.out = outs.p[0];
     p.n_peers = outs.n - 1;
     for (int r = 1; r < outs.n; ++r) p.peer_out[r - 1] = outs.p[r];
+    p.rows_per_out = outs.rows_per_out;
     p.M = M;
     p.N = N;
     p.K = K;
@@ -936,6 +963,7 @@ bool launch_gemm4_staged(const T* A, const uint8_t* B, const float* absmax, cons
         p.out = outs.p[0] + n0;
         p.n_peers = outs.n - 1;
         for (int r = 1; r < outs.n; ++r) p.peer_out[r - 1] = outs.p[r] + n0;
+        p.rows_per_out = outs.rows_per_out;
         p.M = M;
         p.N = rows;
         p.K = K;

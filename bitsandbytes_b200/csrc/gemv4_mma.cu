@@ -89,7 +89,7 @@ __device__ __forceinline__ float lds_f1(uint32_t a) {
 // cp.async (slower, it bypasses L1), 3 or 4 CTAs per SM through a register cap, a byte-indexed shared-memory decode
 // table (profiles/r02_decode_regime.md).
 // NT = groups of 8 tokens (1: M <= 8, 2: M <= 16): the decoded weight fragments feed NT MMAs each.
-// PART: the partial instance (fp32 sums to every destination of `out`, no bias, no rounding).
+// PART: the partial instance (fp32 sums to the destinations of `out` by store_partial, no bias, no rounding).
 template <typename T, int QT, int W, int NT, bool PART>
 __global__ void __launch_bounds__(W * 32, 32 / W)
     gemv4_mma_kernel(const T* __restrict__ A, const uint8_t* __restrict__ B, const float* absmax,
@@ -251,7 +251,7 @@ __global__ void __launch_bounds__(W * 32, 32 / W)
 #pragma unroll
             for (int w = 0; w < W; ++w) acc += red[w][idx];
             if constexpr (PART) {
-                for (int d = 0; d < out.n; ++d) out.p[d][(long long)tok * ldc + n] = acc;
+                store_partial(out, tok, n, ldc, acc);
             } else {
                 const float b = bias != nullptr ? DT<T>::to_f32(bias[n]) : 0.f;
                 out[(long long)tok * ldc + n] = DT<T>::from_f32(acc + b);

@@ -80,7 +80,8 @@ struct Scale {
 
 // `lut` = 16 fp32 code values (NF4 / FP4 table, or the caller's `datatype` array for the
 // legacy gemv entry point).  vec_ok: K % 8 == 0 and 16-byte aligned A rows / 4-byte aligned B rows.
-// PART (here and in gemv4_fast_kernel): the partial instance, fp32 sums to every destination of `out`, no bias.
+// PART (here and in gemv4_fast_kernel): the partial instance, fp32 sums to the destinations of `out` (store_partial:
+// every one, or each row to its own), no bias.
 template <typename T, bool PART>
 __device__ __forceinline__ void
     gemv4_simt_body(const T* __restrict__ A, const uint8_t* __restrict__ B, Scale sc,
@@ -175,8 +176,7 @@ __device__ __forceinline__ void
         if constexpr (PART) {
 #pragma unroll
             for (int i = 0; i < kMB; ++i)
-                if (i < mcount)
-                    for (int d = 0; d < out.n; ++d) out.p[d][(long long)(m_base + i) * ldc + n] = acc[i];
+                if (i < mcount) store_partial(out, m_base + i, n, ldc, acc[i]);
         } else {
             const float b = bias != nullptr ? DT<T>::to_f32(bias[n]) : 0.f;
 #pragma unroll
@@ -285,8 +285,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32)
         if constexpr (PART) {
 #pragma unroll
             for (int i = 0; i < MB; ++i)
-                if (i < M)
-                    for (int d = 0; d < out.n; ++d) out.p[d][(long long)i * ldc + n] = acc[i];
+                if (i < M) store_partial(out, i, n, ldc, acc[i]);
         } else {
             const float b = bias != nullptr ? DT<T>::to_f32(bias[n]) : 0.f;
 #pragma unroll

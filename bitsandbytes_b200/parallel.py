@@ -46,6 +46,21 @@ fp32 sum, as split-K does; with one rank it is the unsharded result exactly.  Th
 through ``all_gather_into_tensor``; fused (``PeerPartials`` + ``fused_forward_row``), the GEMM epilogue
 stores ``P_r`` into slot r of every rank's symmetric ``[world, M, N]`` buffer, one barrier publishes
 them and each rank reduces locally.
+
+Sequence parallelism (``sequence_parallel=True`` on both layers, Megatron's ``[s, b, h]`` layout).  The activations
+between the column -> row pair (norms, residuals) are sharded by token: the first dimension of the activation is split
+over the ranks, so the flattened rows ``[r*M/w, (r+1)*M/w)`` belong to rank r, and ``x.shape[0] % world == 0`` is
+required (``ValueError`` otherwise).  The column layer takes its rank's ``[M/w, ..., K]`` tokens, all-gathers them
+along dim 0 (NCCL ``all_gather_into_tensor``, or ``fused_forward_col_sp``: a copy into this rank's rows of every
+rank's symmetric ``[M, K]`` buffer and one barrier) and returns its ``[M, ..., N/w]`` features, bit for bit the
+non-SP layer on the gathered input (it needs ``gather_output=False``).  The row layer runs the same partial GEMM as
+without SP (same M: same kernel, tile and K split) and hands back only its tokens, ``[x.shape[0]/w, ..., N]``, bit for
+bit rows ``[r*M/w, (r+1)*M/w)`` of the non-SP output, since ``reduce_partials`` works element by element in rank order.
+Unfused, the ``[M, N]`` partial is exchanged by ``all_to_all_single`` into a ``[w, M/w, N]`` buffer (not NCCL's
+reduce-scatter, whose summation order is not rank order); fused (``fused_forward_row_sp``, ``PeerPartials(M/w, N)``),
+the GEMM epilogue stores the rows of rank s into slot r of rank s's buffer (``gemm_4bit_partial_scatter``).  Either way
+a rank sends ``4*M*N*(w-1)/w`` bytes, w times less than the all-gather of the partials, and reduces ``4*M*N`` bytes
+instead of ``4*w*M*N``.
 """
 from __future__ import annotations
 
@@ -56,9 +71,9 @@ import torch
 import torch.distributed as dist
 
 from . import functional as F
-from .backends.cuda import (gemm_4bit_into, gemm_4bit_multi_out, gemm_4bit_partial, int8_gemm_multi_out,
-                            int8_outlier_operands, int8_quant_with_stats, int8_reduce_partials, int8_row_stats,
-                            int8_zero_columns, reduce_partials)
+from .backends.cuda import (gemm_4bit_into, gemm_4bit_multi_out, gemm_4bit_partial, gemm_4bit_partial_scatter,
+                            int8_gemm_multi_out, int8_outlier_operands, int8_quant_with_stats, int8_reduce_partials,
+                            int8_row_stats, int8_zero_columns, reduce_partials)
 
 
 @dataclass
@@ -112,19 +127,26 @@ class ColumnParallelLinear4bit(torch.nn.Module):
     """``y = x @ dequant(W)^T + b`` with W's output features split across the process group."""
 
     def __init__(self, shard: Shard4bit, out_features: int, bias: Optional[torch.Tensor] = None,
-                 group: Optional[dist.ProcessGroup] = None, gather_output: bool = True):
+                 group: Optional[dist.ProcessGroup] = None, gather_output: bool = True,
+                 sequence_parallel: bool = False):
         super().__init__()
+        if sequence_parallel and gather_output:
+            raise ValueError("sequence_parallel=True hands each rank all tokens of its feature slice: it needs "
+                             "gather_output=False")
         self.shard = shard
         self.out_features = out_features
         self.group = group
         self.gather_output = gather_output
+        self.sequence_parallel = sequence_parallel
         self.bias_shard = None if bias is None else bias[shard.row0:shard.row0 + shard.rows].contiguous()
         self._stage = None
 
     @classmethod
-    def from_quantized(cls, packed, qs: F.QuantState, bias=None, group=None, gather_output=True):
+    def from_quantized(cls, packed, qs: F.QuantState, bias=None, group=None, gather_output=True,
+                       sequence_parallel=False):
         world, rank = _group_world_rank(group)
-        return cls(slice_quantized_weight(packed, qs, world, rank), qs.shape[0], bias, group, gather_output)
+        return cls(slice_quantized_weight(packed, qs, world, rank), qs.shape[0], bias, group, gather_output,
+                   sequence_parallel)
 
     def local_forward(self, x: torch.Tensor, out: Optional[torch.Tensor] = None, ldc: Optional[int] = None):
         """This rank's [M, rows] slice; written into ``out`` (row stride ``ldc`` elements) if given."""
@@ -139,12 +161,25 @@ class ColumnParallelLinear4bit(torch.nn.Module):
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         s = self.shard
+        world, _ = _group_world_rank(self.group)
+        if self.sequence_parallel and world > 1:
+            full = torch.empty((world * x.shape[0], *x.shape[1:]), device=x.device, dtype=x.dtype)
+            dist.all_gather_into_tensor(full, x.contiguous(), group=self.group)
+            x = full
         lead = x.shape[:-1]
         M = x.numel() // s.K
-        world, _ = _group_world_rank(self.group)
         if world == 1 or not self.gather_output:
             return self.local_forward(x).view(*lead, s.rows)
         return _gather_columns(self, x, M, x.dtype, x.device).reshape(*lead, world * s.rows)
+
+
+def sp_rows(x: torch.Tensor, world: int) -> int:
+    """Tokens per rank of a sequence-parallel activation ``x[s, ..., features]``: the flattened rows
+    ``[r*M/world, (r+1)*M/world)`` belong to rank r, which needs ``x.shape[0] % world == 0``."""
+    if x.dim() < 2 or x.shape[0] % world != 0:
+        raise ValueError(f"sequence parallelism splits the first dimension of the activation over the ranks: "
+                         f"{tuple(x.shape)} does not split over a world of {world}")
+    return x.numel() // x.shape[-1] // world
 
 
 def _group_world_rank(group) -> tuple[int, int]:
@@ -210,6 +245,11 @@ class _PeerSlots:
         """The address ``offset`` bytes into every rank's buffer of a slot (``bases`` from :meth:`slot`): this rank's
         own buffer first, as the multi-destination GEMMs take their local output, then the peers in rank order."""
         return [bases[r] + offset for r in [self.rank] + [r for r in range(self.world) if r != self.rank]]
+
+    def scatter_ptrs(self, bases, offset: int) -> list[int]:
+        """The address ``offset`` bytes into every rank's buffer of a slot, in rank order, as the scatter GEMM takes its
+        destinations (rank s's rows to rank s)."""
+        return [bases[r] + offset for r in range(self.world)]
 
 
 class PeerGather(_PeerSlots):
@@ -282,20 +322,25 @@ class RowParallelLinear4bit(torch.nn.Module):
     whole ``[..., N]`` output, the same bits on every rank."""
 
     def __init__(self, shard: Shard4bit, in_features: int, bias: Optional[torch.Tensor] = None,
-                 group: Optional[dist.ProcessGroup] = None, input_is_parallel: bool = True):
+                 group: Optional[dist.ProcessGroup] = None, input_is_parallel: bool = True,
+                 sequence_parallel: bool = False):
         super().__init__()
         self.shard = shard
         self.in_features = in_features
         self.out_features = shard.rows
         self.group = group
         self.input_is_parallel = input_is_parallel
+        self.sequence_parallel = sequence_parallel
         self.bias = None if bias is None else bias.contiguous()
         self._stage = None
+        self._sp_bufs = None
 
     @classmethod
-    def from_quantized(cls, packed, qs: F.QuantState, bias=None, group=None, input_is_parallel=True):
+    def from_quantized(cls, packed, qs: F.QuantState, bias=None, group=None, input_is_parallel=True,
+                       sequence_parallel=False):
         world, rank = _group_world_rank(group)
-        return cls(slice_quantized_weight_k(packed, qs, world, rank), qs.shape[1], bias, group, input_is_parallel)
+        return cls(slice_quantized_weight_k(packed, qs, world, rank), qs.shape[1], bias, group, input_is_parallel,
+                   sequence_parallel)
 
     def local_input(self, x: torch.Tensor) -> torch.Tensor:
         """This rank's ``x_r[..., K/world]``: ``x`` itself, or its slice when the layer takes the full input."""
@@ -314,12 +359,43 @@ class RowParallelLinear4bit(torch.nn.Module):
         return gemm_4bit_partial(x_r, s.packed, (s.rows, s.K), s.absmax, s.blocksize, s.quant_type, None, None, None,
                                  outs, s.rows if ldc is None else ldc)
 
+    def partial_scatter(self, x_r: torch.Tensor, outs, ldc: Optional[int] = None) -> bool:
+        """:meth:`partial_forward` with the rows of ``P_r`` split over ``outs`` in rank order: rank s's tokens go to
+        ``outs[s]`` (sequence parallelism)."""
+        s = self.shard
+        return gemm_4bit_partial_scatter(x_r, s.packed, (s.rows, s.K), s.absmax, s.blocksize, s.quant_type, None, None,
+                                         None, outs, s.rows if ldc is None else ldc)
+
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         s = self.shard
         x_r = self.local_input(x)
         M = x_r.numel() // s.K
+        if self.sequence_parallel:
+            return self._sp_forward(x_r, x.dtype)
         parts = _gather_partials(self, x_r, M, torch.float32, x.device, "gemm_4bit_partial")
         return reduce_partials(parts, x.dtype, self.bias).view(*x_r.shape[:-1], s.rows)
+
+    def _sp_exchange(self, x_r: torch.Tensor) -> torch.Tensor:
+        """This rank's ``[world, M/world, N]`` partials of its own tokens, chunk r from rank r: the full ``[M, N]``
+        partial into a send buffer, then an all-to-all (NCCL's reduce-scatter would sum in another order)."""
+        world, _ = _group_world_rank(self.group)
+        Ms = sp_rows(x_r, world)
+        shape = (world, Ms, self.shard.rows)
+        bufs = self._sp_bufs
+        if bufs is None or bufs[0].shape != shape or bufs[0].device != x_r.device:
+            bufs = self._sp_bufs = (torch.empty(shape, device=x_r.device), torch.empty(shape, device=x_r.device))
+        send, recv = bufs
+        if not self.partial_forward(x_r, [send]):
+            raise RuntimeError("gemm_4bit_partial does not serve this shard shape")
+        if world == 1:
+            return send
+        dist.all_to_all_single(recv, send, group=self.group)
+        return recv
+
+    def _sp_forward(self, x_r: torch.Tensor, dtype: torch.dtype) -> torch.Tensor:
+        world, _ = _group_world_rank(self.group)
+        parts = self._sp_exchange(x_r)
+        return reduce_partials(parts, dtype, self.bias).view(x_r.shape[0] // world, *x_r.shape[1:-1], self.shard.rows)
 
 
 class PeerPartials(_PeerSlots):
@@ -346,6 +422,39 @@ def fused_forward_row(layer: RowParallelLinear4bit, x: torch.Tensor, peers: Peer
         raise RuntimeError("gemm_4bit_partial does not serve this shard shape")
     handle.barrier(channel=0)  # every rank's partial has landed everywhere
     return reduce_partials(local, x.dtype, layer.bias).view(*x_r.shape[:-1], s.rows)
+
+
+def fused_forward_row_sp(layer: RowParallelLinear4bit, x: torch.Tensor, peers: PeerPartials) -> torch.Tensor:
+    """The sequence-parallel ``layer(x)`` (this rank's tokens only) with the reduce-scatter fused into the GEMM
+    epilogue: the rows of ``P_r`` that belong to rank s are stored into slot r of rank s's ``[world, M/world, N]``
+    buffer (``peers = PeerPartials(M // world, N)``), one barrier publishes them, and each rank reduces its own."""
+    s = layer.shard
+    x_r = layer.local_input(x)
+    Ms = sp_rows(x_r, peers.world)
+    if Ms != peers.M or s.rows != peers.N or peers.dtype != torch.float32:
+        raise ValueError("PeerPartials was built for a different output shape or dtype")
+    local, bases, handle = peers.slot()
+    if not layer.partial_scatter(x_r, peers.scatter_ptrs(bases, peers.rank * Ms * s.rows * 4)):
+        local.copy_(layer._sp_exchange(x_r))  # the scatter GEMM refused the call: the NCCL route fills the slot
+    handle.barrier(channel=0)  # every rank's rows have landed at their owner
+    return reduce_partials(local, x.dtype, layer.bias).view(x_r.shape[0] // peers.world, *x_r.shape[1:-1], s.rows)
+
+
+def fused_forward_col_sp(layer: ColumnParallelLinear4bit, x: torch.Tensor, peers: PeerGather) -> torch.Tensor:
+    """The sequence-parallel ``layer(x)`` with the token all-gather through symmetric memory: this rank copies its
+    ``[M/world, ..., K]`` tokens into its rows of every rank's ``[M, K]`` buffer (``peers = PeerGather(M, K, dtype)``),
+    one barrier publishes them, and the local GEMM reads the gathered tokens.  Returns ``[M, ..., N/world]``."""
+    s = layer.shard
+    world, rank = peers.world, peers.rank
+    Ms = x.numel() // s.K
+    if world * Ms != peers.M or s.K != peers.N or x.dtype != peers.dtype:
+        raise ValueError("PeerGather was built for a different token count / input width / dtype")
+    local, _, handle = peers.slot()
+    xs = x.reshape(Ms, s.K)
+    for r in range(world):
+        handle.get_buffer(r, (Ms, s.K), x.dtype, rank * Ms * s.K).copy_(xs)
+    handle.barrier(channel=0)  # every rank's tokens have landed everywhere
+    return layer.local_forward(local).view(world * x.shape[0], *x.shape[1:-1], s.rows)
 
 
 def reassemble_shards(shards: list[Shard4bit]) -> tuple[torch.Tensor, torch.Tensor]:

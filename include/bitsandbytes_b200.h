@@ -157,6 +157,13 @@ int cbnb_b200_gemm_4bit_multi_out(const void* A, const uint8_t* B, const float* 
  * destination list, or 100 for a dtype it does not serve. */
 int cbnb_b200_gemm_4bit_partial(const void* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit, const float* absmax_code, const float* absmax_offset, float* const* outs, int n_outs, int M, int N, int K, int ldc, int blocksize, int quant_type, int dtype, bnb_stream_t stream);
 
+/* The partial GEMM of a sequence-parallel row-sharded layer: cbnb_b200_gemm_4bit_partial (same kernel, K split and
+ * fp32 sums) with the rows scattered instead of copied.  Row m is stored to outs[m / rows_per_out] at row
+ * m % rows_per_out (row stride ldc), so `outs` is in RANK order: outs[s] receives the tokens of rank s.  Returns 0, 1
+ * unless 1 <= n_outs <= 8, rows_per_out >= 1 and n_outs * rows_per_out == M (error message set), or 100 for a dtype it
+ * does not serve. */
+int cbnb_b200_gemm_4bit_partial_scatter(const void* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit, const float* absmax_code, const float* absmax_offset, float* const* outs, int n_outs, int rows_per_out, int M, int N, int K, int ldc, int blocksize, int quant_type, int dtype, bnb_stream_t stream);
+
 /* out[m, n] (row stride ldc) = T( (((P_0 + P_1) + ...) + P_{world-1})[m, n] + bias[n] ), P_r = parts + r * part_stride,
  * each [M, N] fp32 with row stride N: the partials summed in rank order in fp32, the bias (T[N] or NULL) added in fp32,
  * one rounding to T.  dtype 0 or 3 = fp32, 1 = fp16, 2 = bf16.  Returns 0, or 100 for a dtype or argument it does not
