@@ -850,6 +850,35 @@ def int8_gemm_multi_out(CA, CB, SCA, SCB, outs, ldc: int, dtype: Optional[torch.
     return rc == 0
 
 
+def int8_gemm_partial_scatter(CA, CB, outs, ldc: int) -> bool:
+    """The exact int32 partial ``CA . CB^T`` with its rows scattered over ``outs`` in rank order: with ``w = len(outs)``
+    and ``M`` rows, row ``m`` is stored to ``outs[m // (M/w)]`` at row ``m % (M/w)`` (row stride ``ldc``), the partial of
+    a sequence-parallel K-sharded layer whose rank s owns tokens ``[s*M/w, (s+1)*M/w)``.  Same kernel and bits as
+    :func:`int8_gemm_multi_out` with dtype None.  ``M % w == 0`` is required.  A destination is an int32 CUDA tensor,
+    checked here, or a raw device address, which the caller vouches for.  Returns False when the kernel does not take
+    the shape (K % 16, alignment)."""
+    if CA.dtype != torch.int8 or CB.dtype != torch.int8 or CB.dim() != 2:
+        raise RuntimeError("int8_gemm_partial_scatter: CA and CB must be int8, CB of shape [N, K]")
+    N, K = CB.shape
+    if CA.shape[-1] != K:
+        raise RuntimeError(f"int8_gemm_partial_scatter: CA {tuple(CA.shape)} does not match CB {tuple(CB.shape)}")
+    M = CA.numel() // K if K else 0
+    _check_sizes("int8_gemm_partial_scatter", M, N, K, ldc)
+    n = len(outs)
+    if n < 1 or M < n or M % n != 0:
+        raise RuntimeError(f"int8_gemm_partial_scatter: {M} rows do not split evenly over {n} destinations")
+    ptrs = _dest_ptrs("int8_gemm_partial_scatter", outs, torch.int32, CA.device, M // n, N, ldc, RuntimeError)
+    if N == 0:
+        return True
+    CA, CB = CA.contiguous(), CB.contiguous()
+    arr = (ct.c_void_p * n)(*ptrs)
+    with _on_device(CA):
+        rc = lib.cbnb_b200_int8_gemm_partial_scatter(CA.data_ptr(), CB.data_ptr(), ct.cast(arr, ct.c_void_p), n, M // n,
+                                                     M, N, K, ldc, _stream(CA))
+    lib.check("int8_gemm_partial_scatter")
+    return rc == 0
+
+
 def int8_outlier_operands(A, CB, SCB, cols: torch.Tensor, jpad: Optional[int] = None):
     """(subA [M, jpad], subBT [N, jpad]) of A's dtype: ``subA[m, j] = A[m, cols[j]]`` and ``subBT[n, j] = T((CB[n,
     cols[j]] * SCB[n]) * (1/127))``, as the fused LLM.int8() route builds them, zero past ``len(cols)``.  ``jpad``

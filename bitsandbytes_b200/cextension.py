@@ -105,6 +105,8 @@ def _signatures():
     sig["cbnb_b200_int8_quant_with_stats"] = ([_VOIDP] * 3 + [ct.c_float] + [_I32] * 3 + [_VOIDP], _I32)
     # (CA, CB, SCA, SCB, bias, subA, subBT, jpad, outs, n_outs, M, N, K, ldc, epi, stream) -> int
     sig["cbnb_b200_int8_gemm_multi_out"] = ([_VOIDP] * 7 + [_I32, _VOIDP] + [_I32] * 6 + [_VOIDP], _I32)
+    # (CA, CB, outs, n_outs, rows_per_out, M, N, K, ldc, stream) -> int
+    sig["cbnb_b200_int8_gemm_partial_scatter"] = ([_VOIDP] * 3 + [_I32] * 6 + [_VOIDP], _I32)
     # (parts, world, part_stride, SCA, SCB, bias, subA, subBT, jpad, out, M, N, ldc, dtype, stream) -> int
     sig["cbnb_b200_int8_reduce_partials"] = ([_VOIDP, _I32, ct.c_longlong] + [_VOIDP] * 5 + [_I32, _VOIDP] + [_I32] * 4
                                              + [_VOIDP], _I32)

@@ -88,7 +88,7 @@ int launch_int8_gemm(const int8_t* acts, const int8_t* weights, void* out, const
                      const void* bias, int M, int N, int K, int ldc, int epi, cudaStream_t stream,
                      const void* subA = nullptr, const void* subBT = nullptr, int jpad = 0,
                      const int* jcount = nullptr, const int* cols = nullptr, const void* A = nullptr,
-                     void* const* outs = nullptr, int n_outs = 0);
+                     void* const* outs = nullptr, int n_outs = 0, int rows_per_out = 0);
 void launch_int8_row_stats(const void* A, float* rowStats, int* col_flags, float threshold, int rows, int cols,
                            int dtype, cudaStream_t stream);
 void launch_int8_quant_with_stats(const void* A, int8_t* out, const float* rowStats, float threshold, int rows,
@@ -767,6 +767,23 @@ int cbnb_b200_int8_gemm_multi_out(const int8_t* CA, const int8_t* CB, const floa
     }
     return launch_int8_gemm(CA, CB, nullptr, SCA, SCB, bias, M, N, K, ldc, epi, stream, subA, subBT, jpad, nullptr,
                             nullptr, nullptr, outs, n_outs);
+}
+
+// The int32 partial GEMM of a sequence-parallel K-sharded int8 layer: cbnb_b200_int8_gemm_multi_out at epi 0 with the
+// rows scattered instead of copied.  Row m is stored to outs[m / rows_per_out] at row m % rows_per_out (row stride
+// ldc), so outs is in rank order: outs[s] receives the tokens of rank s.  Returns 0; 1 with the error message set
+// unless 1 <= n_outs <= 8, rows_per_out >= 1, n_outs * rows_per_out == M and ldc >= N; 100 when the shape is not
+// served (K % 16, alignment: the caller takes another route).
+int cbnb_b200_int8_gemm_partial_scatter(const int8_t* CA, const int8_t* CB, int32_t* const* outs, int n_outs,
+                                        int rows_per_out, int M, int N, int K, int ldc, cudaStream_t stream) {
+    if (outs == nullptr || n_outs < 1 || n_outs > 8 || rows_per_out < 1 || (long long)n_outs * rows_per_out != M ||
+        ldc < N) {
+        set_last_error_msg("int8_gemm_partial_scatter: needs 1 <= n_outs <= 8, rows_per_out >= 1, "
+                           "n_outs * rows_per_out == M and ldc >= N");
+        return 1;
+    }
+    return launch_int8_gemm(CA, CB, nullptr, nullptr, nullptr, nullptr, M, N, K, ldc, 0, stream, nullptr, nullptr, 0,
+                            nullptr, nullptr, nullptr, reinterpret_cast<void* const*>(outs), n_outs, rows_per_out);
 }
 
 // out[m, n] (row stride ldc) = the int8 GEMM epilogue of cbnb_b200_int8_scaled_mm / cbnb_b200_int8_mixed_mm applied

@@ -229,12 +229,23 @@ template <typename TO> struct OutList {
     int rows_per_out;  // 0: every row to every destination
 };
 
+// Where a scattering GEMM (rows_per_out > 0) stores output row m: destination m / rows_per_out, at its row
+// m % rows_per_out.  The one statement of that rule for the 4-bit partial stores and the int8 partial scatter.
+struct ScatterRow {
+    int out;
+    int row;
+};
+__device__ __forceinline__ ScatterRow scatter_row(int m, int rows_per_out) {
+    const int d = m / rows_per_out;
+    return {d, m - d * rows_per_out};
+}
+
 // The partial instances' store of element (m, n) of the fp32 output: to every destination of `outs`, or, with
 // rows_per_out > 0, to destination m / rows_per_out at row m % rows_per_out.
 __device__ __forceinline__ void store_partial(const OutList<float>& outs, int m, int n, long long ldc, float v) {
     if (outs.rows_per_out > 0) {
-        const int d = m / outs.rows_per_out;
-        outs.p[d][(m - d * outs.rows_per_out) * ldc + n] = v;
+        const ScatterRow r = scatter_row(m, outs.rows_per_out);
+        outs.p[r.out][r.row * ldc + n] = v;
     } else {
         for (int d = 0; d < outs.n; ++d) outs.p[d][m * ldc + n] = v;
     }

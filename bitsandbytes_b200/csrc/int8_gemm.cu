@@ -67,6 +67,9 @@ struct I8Params {
 struct I8MultiParams : I8Params {
     void* outs[kI8MaxOuts];
     int n_outs;
+    // EPI 0 only: 0 = every row to every destination; > 0 = row m to outs[m / rows_per_out] only, at row
+    // m % rows_per_out (scatter_row: each rank of a sequence-parallel layer receives its own tokens' partials)
+    int rows_per_out;
 };
 template <bool kMulti> using I8ParamsOf = typename std::conditional<kMulti, I8MultiParams, I8Params>::type;
 
@@ -251,6 +254,14 @@ __global__ void __launch_bounds__(kI8Threads, 1)
         if (m >= p.M) continue;
         float sca = 0.f;
         if (EPI != 0) sca = __ldg(p.SCA + m);
+        // scattered rows: row m's one destination, found once for the column loop (a 128-token tile may span ranks)
+        int* srow = nullptr;
+        if constexpr (EPI == 0 && kMulti) {
+            if (p.rows_per_out > 0) {
+                const ScatterRow sr = scatter_row(m, p.rows_per_out);
+                srow = reinterpret_cast<int*>(p.outs[sr.out]) + (long long)sr.row * p.ldc;
+            }
+        }
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
             const int n = n0 + 8 * j + 2 * t;  // this thread's two consecutive columns n, n + 1
@@ -258,8 +269,10 @@ __global__ void __launch_bounds__(kI8Threads, 1)
             if (EPI == 0) {
                 // (the single-destination store is spelled out apart, so that it compiles as before)
                 if constexpr (kMulti) {
-                    for (int d = 0; d < p.n_outs; ++d) {
-                        int* dst = reinterpret_cast<int*>(p.outs[d]) + (long long)m * p.ldc + n;
+                    const int n_dst = srow != nullptr ? 1 : p.n_outs;
+                    for (int d = 0; d < n_dst; ++d) {
+                        int* dst =
+                            (srow != nullptr ? srow : reinterpret_cast<int*>(p.outs[d]) + (long long)m * p.ldc) + n;
                         if (n + 1 < p.N && (reinterpret_cast<uintptr_t>(dst) & 7) == 0) {
                             *reinterpret_cast<int2*>(dst) = make_int2(v0, v1);
                         } else {
@@ -379,11 +392,15 @@ int launch_i8(const CUtensorMap& ta, const CUtensorMap& tb, I8ParamsOf<kMulti>& 
 // index (epi 1 / 2 only; jpad = 64 is then the row pitch of subA / subBT), or NULL.
 // outs / n_outs: 1 <= n_outs <= 8 destinations (device addresses, row stride ldc) that each receive every output element
 // in place of `out` (not with jcount), or NULL / 0.
+// rows_per_out > 0 (epi 0 with outs only): row m goes to outs[m / rows_per_out] only, at row m % rows_per_out.
 int launch_int8_gemm(const int8_t* acts, const int8_t* weights, void* out, const float* SCA,
                                 const float* SCB, const void* bias, int M, int N, int K, int ldc, int epi,
                                 cudaStream_t stream, const void* subA, const void* subBT, int jpad,
-                                const int* jcount, const int* cols, const void* A, void* const* outs, int n_outs) {
+                                const int* jcount, const int* cols, const void* A, void* const* outs, int n_outs,
+                                int rows_per_out) {
     if (n_outs < 0 || n_outs > kI8MaxOuts || (n_outs > 0 && (outs == nullptr || jcount != nullptr))) return 100;
+    if (rows_per_out < 0 || (rows_per_out > 0 && (epi != 0 || n_outs == 0 || (long long)n_outs * rows_per_out != M)))
+        return 100;
     if (M <= 0 || N <= 0) return 0;
     if (K <= 0 || (K % 16) != 0) return 100;
     if (jpad != 0 && (epi == 0 || jpad < 0 || jpad > 64 || (jpad % 8) != 0 || subA == nullptr || subBT == nullptr ||
@@ -415,6 +432,7 @@ int launch_int8_gemm(const int8_t* acts, const int8_t* weights, void* out, const
         static_cast<I8Params&>(pm) = p;
         for (int d = 0; d < n_outs; ++d) pm.outs[d] = outs[d];
         pm.n_outs = n_outs;
+        pm.rows_per_out = rows_per_out;
         if (epi == 0) return launch_i8<0, 0, false, true>(ta, tb, pm, stream);
 #define BNB200_I8_MULTI(E)                                                                                             \
         if (jpad == 0) return launch_i8<E, 0, false, true>(ta, tb, pm, stream);                                         \

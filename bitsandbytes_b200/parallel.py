@@ -72,8 +72,9 @@ import torch.distributed as dist
 
 from . import functional as F
 from .backends.cuda import (gemm_4bit_into, gemm_4bit_multi_out, gemm_4bit_partial, gemm_4bit_partial_scatter,
-                            int8_gemm_multi_out, int8_outlier_operands, int8_quant_with_stats, int8_reduce_partials,
-                            int8_row_stats, int8_zero_columns, reduce_partials)
+                            int8_gemm_multi_out, int8_gemm_partial_scatter, int8_outlier_operands, int8_quant_with_stats,
+                            int8_reduce_partials, int8_row_stats, int8_vectorwise_quant_flags, int8_zero_columns,
+                            reduce_partials)
 
 
 @dataclass
@@ -475,6 +476,20 @@ def reassemble_shards(shards: list[Shard4bit]) -> tuple[torch.Tensor, torch.Tens
 #     in rank order, are the unsharded ascending list, and their operands are the unsharded ones.
 # Beyond 64 outlier columns the unsharded layer adds the outlier product with `addmm`; both layers then run that same
 # `addmm` on the same full-size operands.  Inference only: no backward, ``state.idx`` is not kept.
+#
+# Sequence parallelism (``sequence_parallel=True``, as for the 4-bit layers: rank r owns the flattened tokens
+# ``[r*M/w, (r+1)*M/w)`` of an activation whose first dimension splits over the ranks).  The outputs stay the unsharded
+# bits: the column layer returns ``[M, ..., N/w]``, the row layer its tokens' rows ``[M/w, ..., N]``.
+#   * column: LLM.int8() quantises each token on its own except for the zeroing of the outlier columns, so a rank
+#     quantises only its tokens, the ranks agree on the outlier columns (an all-reduce MAX of the flags) and zero them,
+#     and the int8 codes, the row statistics and the outlier columns of x are all-gathered instead of the activations:
+#     half the bytes of fp16 / bf16, and 1/w of the quantisation work.  Needs ``gather_output=False`` and K % 16 == 0.
+#   * row: the prologue is unchanged; the outlier counts are gathered before the GEMM, so every rank knows which route
+#     runs before any partial is stored.  Up to 64 outlier columns, the int32 partial's rows go to the ranks that own
+#     them (``all_to_all_single``, or the scatter GEMM into symmetric memory) and each rank reduces its ``[w, M/w, N]``
+#     with its rows of SCA and subA: the reduction works element by element, so these are the unsharded rows.  Past 64,
+#     an `addmm` on M/w rows need not give the bits of the one on M rows, so both routes run the non-SP computation and
+#     keep their rows: the slow path, with the non-SP exchange and reduction.
 
 _INT8_FUSED_J = 64  # outlier columns the GEMM epilogue takes; beyond, the unsharded layer runs the addmm chain
 
@@ -539,10 +554,15 @@ def _no_capture(threshold: float, what: str) -> None:
 class Int8Input:
     """The activations of a column-parallel layer quantised as the unsharded layer quantises them."""
 
-    A: torch.Tensor       # [M, K] of the input dtype
+    A: Optional[torch.Tensor]  # [M, K] of the input dtype; None with sequence parallelism (only subA is gathered)
     CA: torch.Tensor      # int8 [M, K], outlier columns zeroed
     SCA: torch.Tensor     # fp32 [M]
     cols: Optional[torch.Tensor]  # int64 ascending outlier columns, or None
+    dtype: torch.dtype    # the input dtype
+    # sequence parallelism, gathered over the ranks: x[:, cols] zero-padded to [M, jpad] with this rank's subBT
+    # [rows, jpad] (J <= 64: the GEMM's outlier operands), or [M, J] (J > 64: the addmm operand)
+    subA: Optional[torch.Tensor] = None
+    subBT: Optional[torch.Tensor] = None
 
     @property
     def J(self) -> int:
@@ -551,28 +571,39 @@ class Int8Input:
 
 class ColumnParallelLinear8bitLt(torch.nn.Module):
     """LLM.int8() ``y = x @ W^T + b`` with W's output features split across the process group.  Every rank's output
-    equals the unsharded inference ``Linear8bitLt`` output (its columns, with ``gather_output=False``) bit for bit."""
+    equals the unsharded inference ``Linear8bitLt`` output (its columns, with ``gather_output=False``) bit for bit.
+    With ``sequence_parallel=True`` the input is this rank's tokens ``[M/w, ..., K]`` and the output ``[M, ..., N/w]``."""
 
     def __init__(self, shard: Shard8bit, out_features: int, bias: Optional[torch.Tensor] = None,
-                 group: Optional[dist.ProcessGroup] = None, gather_output: bool = True, threshold: float = 0.0):
+                 group: Optional[dist.ProcessGroup] = None, gather_output: bool = True, threshold: float = 0.0,
+                 sequence_parallel: bool = False):
         super().__init__()
+        if sequence_parallel and gather_output:
+            raise ValueError("sequence_parallel=True hands each rank all tokens of its feature slice: it needs "
+                             "gather_output=False")
+        if sequence_parallel and shard.K % 16 != 0:
+            raise ValueError(f"sequence_parallel=True gathers int8 codes for the int8 GEMM: in_features ({shard.K}) "
+                             "must be a multiple of 16")
         self.shard = shard
         self.out_features = out_features
         self.group = group
         self.gather_output = gather_output
         self.threshold = float(threshold)
+        self.sequence_parallel = sequence_parallel
         self.bias_shard = None if bias is None else bias[shard.row0:shard.row0 + shard.rows].contiguous()
         self._stage = None
 
     @classmethod
-    def from_quantized(cls, CB, SCB, bias=None, group=None, threshold: float = 0.0, gather_output: bool = True):
+    def from_quantized(cls, CB, SCB, bias=None, group=None, threshold: float = 0.0, gather_output: bool = True,
+                       sequence_parallel: bool = False):
         world, rank = _group_world_rank(group)
-        return cls(slice_int8_weight(CB, SCB, world, rank), CB.shape[0], bias, group, gather_output, threshold)
+        return cls(slice_int8_weight(CB, SCB, world, rank), CB.shape[0], bias, group, gather_output, threshold,
+                   sequence_parallel)
 
     @classmethod
-    def from_linear8bitlt(cls, module, group=None, gather_output: bool = True):
+    def from_linear8bitlt(cls, module, group=None, gather_output: bool = True, sequence_parallel: bool = False):
         CB, SCB, threshold = _state_of(module)
-        return cls.from_quantized(CB, SCB, module.bias, group, threshold, gather_output)
+        return cls.from_quantized(CB, SCB, module.bias, group, threshold, gather_output, sequence_parallel)
 
     def _bias(self, dtype):
         b = self.bias_shard
@@ -583,18 +614,78 @@ class ColumnParallelLinear8bitLt(torch.nn.Module):
         _no_capture(self.threshold, "ColumnParallelLinear8bitLt")
         A = x.reshape(-1, self.shard.K)
         CA, SCA, cols = F.int8_vectorwise_quant(A.to(torch.float16), threshold=self.threshold)
-        return Int8Input(A, CA, SCA, cols if self.threshold > 0.0 else None)
+        return Int8Input(A, CA, SCA, cols if self.threshold > 0.0 else None, A.dtype)
+
+    def local_quantize(self, x: torch.Tensor):
+        """Sequence parallelism, step 1: (x_s [M/w, K], codes, row statistics, outlier flags or None) of this rank's
+        tokens in one pass of the unsharded quantiser, the outlier columns not yet zeroed."""
+        _no_capture(self.threshold, "ColumnParallelLinear8bitLt")
+        xs = x.reshape(-1, self.shard.K)
+        CA, SCA, flags = int8_vectorwise_quant_flags(xs.to(torch.float16), self.threshold)
+        return xs, CA, SCA, flags
+
+    def local_outliers(self, xs: torch.Tensor, CA: torch.Tensor, cols: Optional[torch.Tensor], M: int):
+        """Sequence parallelism, step 3, given the outlier columns of all M tokens (the union of the ranks' flags): zeroes
+        them in this rank's codes (for M > 1, as the unsharded quantiser does) and returns this rank's share of the
+        outlier operands, (subA_s [M/w, jpad], subBT [rows, jpad]) up to 64 columns, (x_s[:, cols] [M/w, J], None)
+        beyond, (None, None) without any."""
+        J = 0 if cols is None else int(cols.numel())
+        if J == 0:
+            return None, None
+        if M > 1:
+            int8_zero_columns(CA, cols)
+        if J <= _INT8_FUSED_J:
+            return int8_outlier_operands(xs, self.shard.CB, self.shard.SCB, cols)
+        return xs[:, cols].contiguous(), None
+
+    def sp_quantize(self, x: torch.Tensor, peers: Optional["PeerInt8Input"] = None) -> Int8Input:
+        """The quantised input of all M tokens from this rank's ``[M/w, ..., K]``: local quantisation, the outlier
+        columns agreed by an all-reduce MAX of the flags (a host synchronisation, as in the unsharded layer), then the
+        codes and row statistics all-gathered through NCCL or, with ``peers``, copied into this rank's rows of every
+        rank's symmetric slot and published by one barrier.  The outlier columns of x travel through NCCL."""
+        world, rank = _group_world_rank(self.group)
+        K = self.shard.K
+        Ms = x.numel() // K
+        M = world * Ms
+        if peers is not None and (peers.M != M or peers.K != K):
+            raise ValueError("PeerInt8Input was built for a different token count / input width")
+        xs, CA_s, SCA_s, flags = self.local_quantize(x)
+        cols = None
+        if flags is not None:
+            if world > 1:
+                dist.all_reduce(flags, op=dist.ReduceOp.MAX, group=self.group)
+            cols = torch.nonzero(flags).view(-1)
+        subA_s, subBT = self.local_outliers(xs, CA_s, cols, M)
+        if peers is None:
+            CA = torch.empty((M, K), device=x.device, dtype=torch.int8)
+            SCA = torch.empty(M, device=x.device, dtype=torch.float32)
+            dist.all_gather_into_tensor(CA, CA_s, group=self.group)
+            dist.all_gather_into_tensor(SCA, SCA_s, group=self.group)
+        else:
+            local, _, handle = peers.slot()
+            for r in range(world):
+                handle.get_buffer(r, (Ms, K), torch.int8, rank * Ms * K).copy_(CA_s)
+                handle.get_buffer(r, (Ms,), torch.float32, M * K // 4 + rank * Ms).copy_(SCA_s)
+            handle.barrier(channel=0)  # every rank's codes and statistics have landed everywhere
+            CA, SCA = peers.codes(local), peers.stats(local)
+        subA = None
+        if subA_s is not None:
+            subA = torch.empty((M, subA_s.shape[1]), device=x.device, dtype=x.dtype)
+            dist.all_gather_into_tensor(subA, subA_s, group=self.group)
+        return Int8Input(None, CA, SCA, cols, x.dtype, subA, subBT)
 
     def local_forward(self, q: Int8Input, out: Optional[torch.Tensor] = None, ldc: Optional[int] = None):
         """This rank's [M, rows] columns of the unsharded output, without the outlier term past 64 columns (see
         :meth:`outlier_rows`); written into ``out`` (row stride ``ldc``) when given."""
         s = self.shard
-        dtype = q.A.dtype
-        M = q.A.shape[0]
+        dtype = q.dtype
+        M = q.CA.shape[0]
         if out is None:
-            out = torch.empty((M, s.rows), device=q.A.device, dtype=dtype)
+            out = torch.empty((M, s.rows), device=q.CA.device, dtype=dtype)
             ldc = s.rows
         if not self._gemm(q, [out], ldc):
+            if q.A is None:
+                raise RuntimeError("the int8 GEMM does not serve this shard shape")
             # shapes the int8 GEMM does not take (K % 16): the library's own route, copied into place
             if 0 < q.J <= _INT8_FUSED_J:
                 y, _ = torch.ops.bitsandbytes.int8_mixed_scaled_mm(q.A, q.CA, s.CB, q.SCA, s.SCB, q.cols,
@@ -609,26 +700,31 @@ class ColumnParallelLinear8bitLt(torch.nn.Module):
         s = self.shard
         subA = subBT = None
         if 0 < q.J <= _INT8_FUSED_J:
-            subA, subBT = int8_outlier_operands(q.A, s.CB, s.SCB, q.cols)
-        return int8_gemm_multi_out(q.CA, s.CB, q.SCA, s.SCB, outs, ldc, q.A.dtype, self._bias(q.A.dtype), subA, subBT)
+            subA, subBT = (q.subA, q.subBT) if q.A is None else int8_outlier_operands(q.A, s.CB, s.SCB, q.cols)
+        return int8_gemm_multi_out(q.CA, s.CB, q.SCA, s.SCB, outs, ldc, q.dtype, self._bias(q.dtype), subA, subBT)
 
     def outlier_rows(self, q: Int8Input) -> torch.Tensor:
         """This rank's rows [rows, J] of the dequantised outlier weight columns (J > 64: the addmm operand)."""
         s = self.shard
-        return F.int8_vectorwise_dequant(s.CB[:, q.cols].contiguous(), s.SCB).to(q.A.dtype)
+        return F.int8_vectorwise_dequant(s.CB[:, q.cols].contiguous(), s.SCB).to(q.dtype)
 
     @staticmethod
     def finish(full: torch.Tensor, q: Int8Input, subBT: torch.Tensor) -> torch.Tensor:
         """The unsharded layer's outlier step past 64 columns on the gathered [M, N] output and [N, J] weight columns:
         the same ``addmm`` on the same operands."""
-        subA = q.A[:, q.cols].contiguous()
+        subA = q.A[:, q.cols].contiguous() if q.A is not None else q.subA
         return full.addmm(subA, subBT.t())
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
+        world, _ = _group_world_rank(self.group)
+        if self.sequence_parallel and world > 1:
+            return self._output(self.sp_quantize(x), (world * x.shape[0], *x.shape[1:-1]))
+        return self._output(self.quantize(x), x.shape[:-1])
+
+    def _output(self, q: Int8Input, lead) -> torch.Tensor:
+        """The layer's output from the quantised input of all M tokens (``lead``: its leading dimensions)."""
         s = self.shard
-        lead = x.shape[:-1]
-        q = self.quantize(x)
-        M = q.A.shape[0]
+        M = q.CA.shape[0]
         world, _ = _group_world_rank(self.group)
         chain = q.J > _INT8_FUSED_J
         if world == 1:
@@ -638,10 +734,10 @@ class ColumnParallelLinear8bitLt(torch.nn.Module):
             return y.view(*lead, s.rows)
         if not self.gather_output and not chain:
             return self.local_forward(q).view(*lead, s.rows)
-        full = _gather_columns(self, q, M, q.A.dtype, q.A.device)
+        full = _gather_columns(self, q, M, q.dtype, q.CA.device)
         if chain:
             rows = self.outlier_rows(q)
-            subBT = torch.empty((world * s.rows, q.J), device=x.device, dtype=x.dtype)
+            subBT = torch.empty((world * s.rows, q.J), device=q.CA.device, dtype=q.dtype)
             dist.all_gather_into_tensor(subBT, rows, group=self.group)
             full = self.finish(full, q, subBT)
         if not self.gather_output:
@@ -671,6 +767,35 @@ def fused_forward_col8(layer: ColumnParallelLinear8bitLt, x: torch.Tensor, peers
     return local
 
 
+class PeerInt8Input(_PeerSlots):
+    """Two symmetric-memory slots for the gathered input of a sequence-parallel int8 column layer: ``[M*K int8 codes |
+    M fp32 row statistics]`` in one buffer, so that one barrier publishes both (``K % 16 == 0`` keeps the statistics
+    aligned)."""
+
+    def __init__(self, M: int, K: int, device, group: Optional[dist.ProcessGroup] = None):
+        if K % 16 != 0:
+            raise ValueError(f"in_features ({K}) must be a multiple of 16")
+        super().__init__((M * K + 4 * M,), torch.uint8, device, group)
+        self.M, self.K = M, K
+
+    def codes(self, local: torch.Tensor) -> torch.Tensor:
+        """The int8 [M, K] codes of a slot."""
+        return local[:self.M * self.K].view(torch.int8).view(self.M, self.K)
+
+    def stats(self, local: torch.Tensor) -> torch.Tensor:
+        """The fp32 [M] row statistics of a slot."""
+        return local[self.M * self.K:].view(torch.float32)
+
+
+def fused_forward_col8_sp(layer: ColumnParallelLinear8bitLt, x: torch.Tensor, peers: PeerInt8Input) -> torch.Tensor:
+    """The sequence-parallel ``layer(x)`` with the gather of the quantised tokens through symmetric memory: this rank
+    quantises its ``[M/w, ..., K]`` tokens and copies the codes and row statistics into its rows of every rank's slot
+    (``peers = PeerInt8Input(M, K)``), one barrier publishes them, and the local GEMM reads the gathered codes.  Returns
+    ``[M, ..., N/w]``."""
+    world, _ = _group_world_rank(layer.group)
+    return layer._output(layer.sp_quantize(x, peers), (world * x.shape[0], *x.shape[1:-1]))
+
+
 @dataclass
 class Int8Stats:
     """One rank's share of the row statistics of a row-parallel layer's input."""
@@ -686,10 +811,11 @@ class RowParallelLinear8bitLt(torch.nn.Module):
 
     The forward pass runs in steps a single process can also drive rank by rank: :meth:`local_stats` -> a max over the
     ranks -> :meth:`local_codes` -> :meth:`partial_forward` (+ :meth:`outlier_operands`) -> an exchange ->
-    :meth:`reduce`."""
+    :meth:`reduce`.  With ``sequence_parallel=True`` each rank returns only its tokens' rows, ``[M/w, ..., N]``."""
 
     def __init__(self, shard: Shard8bit, in_features: int, bias: Optional[torch.Tensor] = None,
-                 group: Optional[dist.ProcessGroup] = None, input_is_parallel: bool = True, threshold: float = 0.0):
+                 group: Optional[dist.ProcessGroup] = None, input_is_parallel: bool = True, threshold: float = 0.0,
+                 sequence_parallel: bool = False):
         super().__init__()
         self.shard = shard
         self.in_features = in_features
@@ -697,18 +823,22 @@ class RowParallelLinear8bitLt(torch.nn.Module):
         self.group = group
         self.input_is_parallel = input_is_parallel
         self.threshold = float(threshold)
+        self.sequence_parallel = sequence_parallel
         self.bias = None if bias is None else bias.contiguous()
         self._stage = None
+        self._sp_bufs = None
 
     @classmethod
-    def from_quantized(cls, CB, SCB, bias=None, group=None, threshold: float = 0.0, input_is_parallel: bool = True):
+    def from_quantized(cls, CB, SCB, bias=None, group=None, threshold: float = 0.0, input_is_parallel: bool = True,
+                       sequence_parallel: bool = False):
         world, rank = _group_world_rank(group)
-        return cls(slice_int8_weight_k(CB, SCB, world, rank), CB.shape[1], bias, group, input_is_parallel, threshold)
+        return cls(slice_int8_weight_k(CB, SCB, world, rank), CB.shape[1], bias, group, input_is_parallel, threshold,
+                   sequence_parallel)
 
     @classmethod
-    def from_linear8bitlt(cls, module, group=None, input_is_parallel: bool = True):
+    def from_linear8bitlt(cls, module, group=None, input_is_parallel: bool = True, sequence_parallel: bool = False):
         CB, SCB, threshold = _state_of(module)
-        return cls.from_quantized(CB, SCB, module.bias, group, threshold, input_is_parallel)
+        return cls.from_quantized(CB, SCB, module.bias, group, threshold, input_is_parallel, sequence_parallel)
 
     def local_input(self, x: torch.Tensor) -> torch.Tensor:
         """This rank's ``x_r[M, K/world]``: ``x`` itself, or its slice when the layer takes the full input."""
@@ -744,6 +874,12 @@ class RowParallelLinear8bitLt(torch.nn.Module):
         s = self.shard
         return int8_gemm_multi_out(CA, s.CB, None, None, outs, s.rows if ldc is None else ldc, None)
 
+    def partial_scatter(self, CA: torch.Tensor, outs, ldc: Optional[int] = None) -> bool:
+        """:meth:`partial_forward` with the rows of the partial split over ``outs`` in rank order: rank s's tokens go to
+        ``outs[s]`` (sequence parallelism)."""
+        s = self.shard
+        return int8_gemm_partial_scatter(CA, s.CB, outs, s.rows if ldc is None else ldc)
+
     def outlier_operands(self, x_r: torch.Tensor, cols: torch.Tensor, jpad: int):
         """(subA_r [M, jpad], subBT_r [N, jpad]): the rank's outlier columns of x and of the weight, zero-padded."""
         s = self.shard
@@ -776,16 +912,26 @@ class RowParallelLinear8bitLt(torch.nn.Module):
         subBT = torch.cat([b[:, :j] for (_, b), j in zip(operands, counts)], dim=1).contiguous()
         return subA, subBT
 
-    def _exchange_outliers(self, x_r, cols, world: int):
-        """Every rank's outlier count and operands, gathered in rank order through NCCL (None, None without any)."""
+    def _outlier_counts(self, x_r, cols, world: int) -> Optional[list[int]]:
+        """Every rank's outlier count in rank order, gathered through NCCL (None at threshold 0)."""
         if cols is None:
-            return None, None
+            return None
         dev = x_r.device
         counts = [int(cols.numel())]
         if world > 1:
             counts_t = torch.empty(world, device=dev, dtype=torch.int64)
             dist.all_gather_into_tensor(counts_t, torch.tensor(counts, device=dev, dtype=torch.int64), group=self.group)
             counts = counts_t.tolist()
+        return counts
+
+    def _exchange_outliers(self, x_r, cols, world: int, counts: Optional[list[int]] = None):
+        """Every rank's outlier count (unless given) and operands, gathered in rank order through NCCL (None, None
+        without any)."""
+        if cols is None:
+            return None, None
+        dev = x_r.device
+        if counts is None:
+            counts = self._outlier_counts(x_r, cols, world)
         if sum(counts) == 0:
             return None, None
         P = max(8, -(-max(counts) // 8) * 8)
@@ -808,12 +954,61 @@ class RowParallelLinear8bitLt(torch.nn.Module):
         return x_r, world, SCA, CA, cols
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
+        if self.sequence_parallel:
+            return self._sp_forward(x)
         s = self.shard
         lead = x.shape[:-1]
         x_r, world, SCA, CA, cols = self._prologue(x)
         parts = _gather_partials(self, CA, x_r.shape[0], torch.int32, x.device, "the int8 GEMM")
         subA, subBT = self._exchange_outliers(x_r, cols, world)
         return self.reduce(parts, SCA, x.dtype, subA, subBT).view(*lead, s.rows)
+
+    def _sp_exchange(self, CA: torch.Tensor, Ms: int) -> torch.Tensor:
+        """This rank's ``[world, M/world, N]`` int32 partials of its own tokens, chunk r from rank r: the full ``[M, N]``
+        partial into a send buffer, then an all-to-all (NCCL's reduce-scatter would not keep the exact int32 sum
+        followed by the unsharded epilogue)."""
+        world, _ = _group_world_rank(self.group)
+        shape = (world, Ms, self.shard.rows)
+        bufs = self._sp_bufs
+        if bufs is None or bufs[0].shape != shape or bufs[0].device != CA.device:
+            bufs = self._sp_bufs = tuple(torch.empty(shape, device=CA.device, dtype=torch.int32) for _ in range(2))
+        send, recv = bufs
+        if not self.partial_forward(CA, [send]):
+            raise RuntimeError("the int8 GEMM does not serve this shard shape")
+        if world == 1:
+            return send
+        dist.all_to_all_single(recv, send, group=self.group)
+        return recv
+
+    def _sp_forward(self, x: torch.Tensor, peers: Optional[PeerPartials] = None) -> torch.Tensor:
+        """The sequence-parallel forward: this rank's rows ``[M/w, ..., N]`` of the non-SP output.  The partials of this
+        rank's tokens arrive through :meth:`_sp_exchange` or, with ``peers``, from every rank's scatter GEMM into this
+        rank's symmetric ``[world, M/world, N]`` slot."""
+        s = self.shard
+        world, rank = _group_world_rank(self.group)
+        Ms = sp_rows(x, world)
+        if peers is not None and (Ms != peers.M or s.rows != peers.N or peers.dtype != torch.int32):
+            raise ValueError("PeerPartials was built for a different output shape or dtype (int32 partials)")
+        x_r, world, SCA, CA, cols = self._prologue(x)
+        counts = self._outlier_counts(x_r, cols, world)  # before the GEMM: every rank then takes the same route
+        mine = slice(rank * Ms, (rank + 1) * Ms)
+        lead = (x.shape[0] // world, *x.shape[1:-1], s.rows)
+        if counts is not None and sum(counts) > _INT8_FUSED_J:
+            # The slow path: an addmm on this rank's rows need not give the bits of the one on all M rows, so the
+            # non-SP computation runs (all partials, full reduction, addmm) and this rank keeps its rows.
+            parts = _gather_partials(self, CA, x_r.shape[0], torch.int32, x.device, "the int8 GEMM")
+            subA, subBT = self._exchange_outliers(x_r, cols, world, counts)
+            return self.reduce(parts, SCA, x.dtype, subA, subBT)[mine].view(lead)
+        if peers is None:
+            parts = self._sp_exchange(CA, Ms)
+            subA, subBT = self._exchange_outliers(x_r, cols, world, counts)
+        else:
+            parts, bases, handle = peers.slot()
+            if not self.partial_scatter(CA, peers.scatter_ptrs(bases, peers.rank * Ms * s.rows * 4)):
+                parts.copy_(self._sp_exchange(CA, Ms))  # the scatter GEMM refused the call: the NCCL route fills it
+            subA, subBT = self._exchange_outliers(x_r, cols, world, counts)
+            handle.barrier(channel=0)  # every rank's rows have landed at their owner
+        return self.reduce(parts, SCA[mine], x.dtype, None if subA is None else subA[mine], subBT).view(lead)
 
 
 def fused_forward_row8(layer: RowParallelLinear8bitLt, x: torch.Tensor, peers: PeerPartials) -> torch.Tensor:
@@ -831,3 +1026,12 @@ def fused_forward_row8(layer: RowParallelLinear8bitLt, x: torch.Tensor, peers: P
     subA, subBT = layer._exchange_outliers(x_r, cols, peers.world)
     handle.barrier(channel=0)  # every rank's partial has landed everywhere
     return layer.reduce(local, SCA, x.dtype, subA, subBT).view(*x.shape[:-1], s.rows)
+
+
+def fused_forward_row8_sp(layer: RowParallelLinear8bitLt, x: torch.Tensor, peers: PeerPartials) -> torch.Tensor:
+    """The sequence-parallel ``layer(x)`` (this rank's tokens only) with the exchange of the int32 partials fused into
+    the GEMM epilogue: the rows of ``P_r`` that belong to rank s are stored into slot r of rank s's ``[world, M/world,
+    N]`` buffer (``peers = PeerPartials(M // world, N, dtype=torch.int32)``), one barrier publishes them, and each rank
+    reduces its own with its rows of the statistics and outlier operands.  Past 64 outlier columns the slow path of the
+    NCCL route runs instead (:meth:`RowParallelLinear8bitLt._sp_forward`)."""
+    return layer._sp_forward(x, peers)

@@ -259,6 +259,12 @@ int cbnb_b200_int8_quant_with_stats(const void* A, int8_t* out, const float* row
  * output element to each of outs[0..n_outs), n_outs <= 8, row stride ldc.  A shape the kernel does not take (K % 16,
  * alignment, jpad > 64) returns 100 without an error message. */
 int cbnb_b200_int8_gemm_multi_out(const int8_t* CA, const int8_t* CB, const float* SCA, const float* SCB, const void* bias, const void* subA, const void* subBT, int jpad, void* const* outs, int n_outs, int M, int N, int K, int ldc, int epi, bnb_stream_t stream);
+/* The int32 partial GEMM of a sequence-parallel K-sharded layer: cbnb_b200_int8_gemm_multi_out at epi 0 with the rows
+ * scattered instead of copied.  Row m is stored to outs[m / rows_per_out] at row m % rows_per_out (row stride ldc), so
+ * `outs` is in RANK order: outs[s] receives the tokens of rank s.  Returns 0; 1 with the error message set unless
+ * 1 <= n_outs <= 8, rows_per_out >= 1, n_outs * rows_per_out == M and ldc >= N; 100 for a shape the kernel does not
+ * take (K % 16, alignment). */
+int cbnb_b200_int8_gemm_partial_scatter(const int8_t* CA, const int8_t* CB, int32_t* const* outs, int n_outs, int rows_per_out, int M, int N, int K, int ldc, bnb_stream_t stream);
 /* out = the int8 GEMM epilogue (dtype 1 fp16, 2 bf16) of sum_r parts[r], the exact int32 partials of a K-sharded
  * layer, with SCA, SCB, bias and, for jpad > 0, the outlier term subA[M, jpad] . subBT[N, jpad]^T. */
 int cbnb_b200_int8_reduce_partials(const int* parts, int world, long long part_stride, const float* SCA, const float* SCB, const void* bias, const void* subA, const void* subBT, int jpad, void* out, int M, int N, int ldc, int dtype, bnb_stream_t stream);
