@@ -61,6 +61,19 @@ reduce-scatter, whose summation order is not rank order); fused (``fused_forward
 the GEMM epilogue stores the rows of rank s into slot r of rank s's buffer (``gemm_4bit_partial_scatter``).  Either way
 a rank sends ``4*M*N*(w-1)/w`` bytes, w times less than the all-gather of the partials, and reduces ``4*M*N`` bytes
 instead of ``4*w*M*N``.
+
+Training (QLoRA under tensor and sequence parallelism).  Both layers' forward runs through a ``torch.autograd.Function``
+(the same bits as before) whose backward gives the input gradient ``grad_x = grad_y . dequant(W)`` and nothing else:
+the sharded weights and biases stay frozen.  The column layer's rank r holds ``P_r = G_r . dequant(W_r)`` in fp32, ``G_r``
+its columns of ``grad_y``, and the partials meet as in the row layer's forward: all-gathered and summed in rank order by
+``reduce_partials`` (every rank holds the same bits; with one rank ``grad_x = T(P_0)``), or, with sequence parallelism,
+exchanged by token with ``all_to_all_single`` so that each rank reduces only its tokens' rows, which are the non-SP
+result's rows bit for bit.  The row layer needs no exchange, ``grad_x_r = grad_y . dequant(W_r)`` rounded once, after an
+all-gather of ``grad_y``'s token rows under sequence parallelism; with ``input_is_parallel=False`` (the whole replicated
+input, of which the layer uses its columns) the ranks' ``grad_x_r`` are all-gathered along the features, in rank order,
+into the whole input gradient.  Both products run as dequantise + cuBLAS (:func:`input_grad_dequant_matmul`, chosen in
+``_input_grad`` from the timings against the library's input-gradient kernel, ``gemm_4bit_input_grad``).  The
+``fused_forward*`` routes stay inference only and refuse an input that requires grad.
 """
 from __future__ import annotations
 
@@ -71,8 +84,8 @@ import torch
 import torch.distributed as dist
 
 from . import functional as F
-from .backends.cuda import (gemm_4bit_into, gemm_4bit_multi_out, gemm_4bit_partial, gemm_4bit_partial_scatter,
-                            int8_gemm_multi_out, int8_gemm_partial_scatter, int8_outlier_operands, int8_quant_with_stats,
+from .backends.cuda import (gemm_4bit_into, gemm_4bit_multi_out, gemm_4bit_partial,
+                            gemm_4bit_partial_scatter, int8_gemm_multi_out, int8_gemm_partial_scatter, int8_outlier_operands, int8_quant_with_stats,
                             int8_reduce_partials, int8_row_stats, int8_vectorwise_quant_flags, int8_zero_columns,
                             reduce_partials)
 
@@ -161,6 +174,9 @@ class ColumnParallelLinear4bit(torch.nn.Module):
         return out
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
+        return _ColumnParallel4bitFn.apply(x, self)
+
+    def _forward(self, x: torch.Tensor) -> torch.Tensor:
         s = self.shard
         world, _ = _group_world_rank(self.group)
         if self.sequence_parallel and world > 1:
@@ -172,6 +188,80 @@ class ColumnParallelLinear4bit(torch.nn.Module):
         if world == 1 or not self.gather_output:
             return self.local_forward(x).view(*lead, s.rows)
         return _gather_columns(self, x, M, x.dtype, x.device).reshape(*lead, world * s.rows)
+
+    def input_grad_partial(self, grad_y: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
+        """This rank's fp32 partial ``P_r = G_r . dequant(W_r)`` of the input gradient into ``out`` ``[M, K]``: ``G_r``
+        is ``grad_y`` itself (``[M, rows]``, this rank's output) or, for the ``[M, world * rows]`` gathered output, this
+        rank's columns of it, read in place."""
+        s = self.shard
+        G = grad_y.reshape(-1, grad_y.shape[-1])
+        if G.shape[1] != s.rows:
+            G = G[:, s.row0:s.row0 + s.rows]
+        return _input_grad(G, s, out)
+
+    def _backward(self, grad_y: torch.Tensor, x_shape) -> torch.Tensor:
+        s = self.shard
+        world, rank = _group_world_rank(self.group)
+        M = grad_y.numel() // grad_y.shape[-1]
+        if self.sequence_parallel and world > 1:
+            # the partial over all M tokens, its rows sent to the ranks that own them: chunk r of recv is rank r's
+            send = torch.empty((world, M // world, s.K), device=grad_y.device)
+            self.input_grad_partial(grad_y, send.view(M, s.K))
+            recv = torch.empty_like(send)
+            dist.all_to_all_single(recv, send, group=self.group)
+            return reduce_partials(recv, grad_y.dtype).view(x_shape)
+        stage = torch.empty((world, M, s.K), device=grad_y.device)
+        self.input_grad_partial(grad_y, stage[rank])
+        if world > 1:
+            dist.all_gather_into_tensor(stage.view(-1), stage[rank].reshape(-1), group=self.group)
+        return reduce_partials(stage, grad_y.dtype).view(x_shape)
+
+
+class _ColumnParallel4bitFn(torch.autograd.Function):
+    """``ColumnParallelLinear4bit``'s forward, with the input gradient as its backward (the shard stays frozen)."""
+
+    @staticmethod
+    def forward(ctx, x, layer):
+        ctx.layer, ctx.x_shape = layer, x.shape
+        return layer._forward(x)
+
+    @staticmethod
+    def backward(ctx, grad_y):
+        return ctx.layer._backward(grad_y, ctx.x_shape), None
+
+
+def input_grad_dequant_matmul(G: torch.Tensor, shard: Shard4bit, dtype: torch.dtype) -> torch.Tensor:
+    """``G . dequant(W)`` ``[M, K]`` by dequantise + ``torch.matmul``: the shard decoded to G's dtype as
+    ``dequantize_4bit`` decodes it, multiplied by cuBLAS with an output of ``dtype`` -- G's dtype, or fp32 on the fp32
+    accumulation of the 16-bit operands for a partial."""
+    s = shard
+    scales = s.absmax
+    if s.absmax_8bit is not None:
+        scales = _nested_scales(s.absmax_8bit, s.absmax, s.absmax_code, s.absmax_offset)
+    W = F.dequantize_4bit(s.packed, absmax=scales, out=torch.empty((s.rows, s.K), device=G.device, dtype=G.dtype),
+                          blocksize=s.blocksize, quant_type=s.quant_type)
+    if dtype == G.dtype:
+        return torch.matmul(G, W)
+    if G.dtype != torch.float32:
+        return torch.mm(G, W, out_dtype=torch.float32)  # 16-bit operands, fp32 accumulation and output
+    return torch.matmul(G.float(), W.float())
+
+
+def _input_grad(G: torch.Tensor, shard: Shard4bit, out: torch.Tensor) -> torch.Tensor:
+    """``out[M, K] = G . dequant(W)`` (``G`` ``[M, rows]`` in any layout): fp32 ``out`` receives the unrounded partial,
+    one of G's dtype the sum rounded once.  The route is chosen here, from the timings on an H100 (DESIGN.md section 6,
+    tools/time_gemm4_input_grad.py): dequantise + cuBLAS -- with an fp32 output from the 16-bit operands for a partial
+    -- is as fast as the input-gradient kernel or faster at every shape and token count measured but one (4096 x 4096
+    at 256 tokens, not a range of M), so the layers take it at every M; the kernel (``gemm_4bit_input_grad``) stays in
+    the library."""
+    out.copy_(input_grad_dequant_matmul(G, shard, out.dtype))
+    return out
+
+
+def _no_grad_route(x: torch.Tensor, what: str) -> None:
+    if torch.is_grad_enabled() and x.requires_grad:
+        raise RuntimeError(f"{what} is inference only and would drop the input gradient: call the layer itself to "
+                           "train, or run this under torch.no_grad()")
 
 
 def sp_rows(x: torch.Tensor, world: int) -> int:
@@ -263,6 +353,7 @@ class PeerGather(_PeerSlots):
 
 def fused_forward(layer: "ColumnParallelLinear4bit", x: torch.Tensor, peers: PeerGather) -> torch.Tensor:
     """``layer(x)`` with the all-gather fused into the GEMM epilogue; returns this rank's [M, N] slot."""
+    _no_grad_route(x, "fused_forward")
     s = layer.shard
     M = x.numel() // s.K
     if M != peers.M or layer.out_features != peers.N or x.dtype != peers.dtype:
@@ -286,10 +377,14 @@ def nested_scales(qs: F.QuantState) -> torch.Tensor:
     """The fp32 scale of every quantisation block of a double-quantised state, computed as the kernels fetch it
     (``ScaleSrc::load_as``): ``(code2[absmax_8bit] * absmax2[block // 256])`` rounded, flushed to zero below the
     normal range, then ``+ offset`` rounded."""
-    a2 = qs.state2.absmax.float()
-    idx = torch.arange(qs.absmax.numel(), device=a2.device) // 256
-    prod = _ftz(_ftz(qs.state2.code.float()[qs.absmax.long()]) * _ftz(a2[idx]))
-    return prod + qs.offset.reshape(()).float().to(prod.device)
+    return _nested_scales(qs.absmax, qs.state2.absmax, qs.state2.code, qs.offset)
+
+
+def _nested_scales(absmax_8bit, absmax2, code, offset) -> torch.Tensor:
+    a2 = absmax2.float()
+    idx = torch.arange(absmax_8bit.numel(), device=a2.device) // 256
+    prod = _ftz(_ftz(code.float()[absmax_8bit.long()]) * _ftz(a2[idx]))
+    return prod + offset.reshape(()).float().to(prod.device)
 
 
 def slice_quantized_weight_k(packed: torch.Tensor, qs: F.QuantState, world: int, rank: int) -> Shard4bit:
@@ -368,13 +463,37 @@ class RowParallelLinear4bit(torch.nn.Module):
                                          None, outs, s.rows if ldc is None else ldc)
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
+        return _RowParallel4bitFn.apply(x, self)
+
+    def input_grad(self, grad_y: torch.Tensor) -> torch.Tensor:
+        """``grad_x_r = grad_y . dequant(W_r)`` ``[M, K/world]`` for the ``[..., N]`` output gradient of all M tokens."""
         s = self.shard
-        x_r = self.local_input(x)
+        G = grad_y.reshape(-1, s.rows)
+        return _input_grad(G, s, torch.empty((G.shape[0], s.K), device=G.device, dtype=G.dtype))
+
+    def _backward(self, grad_y: torch.Tensor, x_shape) -> torch.Tensor:
+        world, _ = _group_world_rank(self.group)
+        if self.sequence_parallel and world > 1:
+            # this rank's tokens' rows of grad_y -> all M rows, in rank order (= token order)
+            full = torch.empty((world * grad_y.shape[0], *grad_y.shape[1:]), device=grad_y.device, dtype=grad_y.dtype)
+            dist.all_gather_into_tensor(full, grad_y.contiguous(), group=self.group)
+            grad_y = full
+        g = self.input_grad(grad_y)
+        if not self.input_is_parallel and world > 1:
+            # the layer took the whole (replicated) input and used only its columns: the input gradient is every rank's
+            # columns, all-gathered in rank order (the backward of the scatter)
+            parts = torch.empty((world, *g.shape), device=g.device, dtype=g.dtype)
+            dist.all_gather_into_tensor(parts, g, group=self.group)
+            g = parts.permute(1, 0, 2).reshape(g.shape[0], world * g.shape[1])
+        return g.view(x_shape)
+
+    def _forward(self, x_r: torch.Tensor) -> torch.Tensor:
+        s = self.shard
         M = x_r.numel() // s.K
         if self.sequence_parallel:
-            return self._sp_forward(x_r, x.dtype)
-        parts = _gather_partials(self, x_r, M, torch.float32, x.device, "gemm_4bit_partial")
-        return reduce_partials(parts, x.dtype, self.bias).view(*x_r.shape[:-1], s.rows)
+            return self._sp_forward(x_r, x_r.dtype)
+        parts = _gather_partials(self, x_r, M, torch.float32, x_r.device, "gemm_4bit_partial")
+        return reduce_partials(parts, x_r.dtype, self.bias).view(*x_r.shape[:-1], s.rows)
 
     def _sp_exchange(self, x_r: torch.Tensor) -> torch.Tensor:
         """This rank's ``[world, M/world, N]`` partials of its own tokens, chunk r from rank r: the full ``[M, N]``
@@ -399,6 +518,19 @@ class RowParallelLinear4bit(torch.nn.Module):
         return reduce_partials(parts, dtype, self.bias).view(x_r.shape[0] // world, *x_r.shape[1:-1], self.shard.rows)
 
 
+class _RowParallel4bitFn(torch.autograd.Function):
+    """``RowParallelLinear4bit``'s forward, with the input gradient as its backward (the shard stays frozen)."""
+
+    @staticmethod
+    def forward(ctx, x, layer):
+        ctx.layer, ctx.x_shape = layer, x.shape
+        return layer._forward(layer.local_input(x))
+
+    @staticmethod
+    def backward(ctx, grad_y):
+        return ctx.layer._backward(grad_y, ctx.x_shape), None
+
+
 class PeerPartials(_PeerSlots):
     """Two symmetric-memory ``[world, M, N]`` partial slots shared by the ranks of ``group`` (fp32 for the 4-bit layer,
     int32 for the int8 one)."""
@@ -413,6 +545,7 @@ class PeerPartials(_PeerSlots):
 def fused_forward_row(layer: RowParallelLinear4bit, x: torch.Tensor, peers: PeerPartials) -> torch.Tensor:
     """``layer(x)`` with the exchange of the partials fused into the GEMM epilogue: ``P_r`` is stored into slot r of
     every rank's buffer, one barrier publishes them, and each rank reduces them in rank order."""
+    _no_grad_route(x, "fused_forward_row")
     s = layer.shard
     x_r = layer.local_input(x)
     M = x_r.numel() // s.K
@@ -429,6 +562,7 @@ def fused_forward_row_sp(layer: RowParallelLinear4bit, x: torch.Tensor, peers: P
     """The sequence-parallel ``layer(x)`` (this rank's tokens only) with the reduce-scatter fused into the GEMM
     epilogue: the rows of ``P_r`` that belong to rank s are stored into slot r of rank s's ``[world, M/world, N]``
     buffer (``peers = PeerPartials(M // world, N)``), one barrier publishes them, and each rank reduces its own."""
+    _no_grad_route(x, "fused_forward_row_sp")
     s = layer.shard
     x_r = layer.local_input(x)
     Ms = sp_rows(x_r, peers.world)
@@ -445,6 +579,7 @@ def fused_forward_col_sp(layer: ColumnParallelLinear4bit, x: torch.Tensor, peers
     """The sequence-parallel ``layer(x)`` with the token all-gather through symmetric memory: this rank copies its
     ``[M/world, ..., K]`` tokens into its rows of every rank's ``[M, K]`` buffer (``peers = PeerGather(M, K, dtype)``),
     one barrier publishes them, and the local GEMM reads the gathered tokens.  Returns ``[M, ..., N/world]``."""
+    _no_grad_route(x, "fused_forward_col_sp")
     s = layer.shard
     world, rank = peers.world, peers.rank
     Ms = x.numel() // s.K

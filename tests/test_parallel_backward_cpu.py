@@ -1,0 +1,101 @@
+"""CPU tests of the tensor-parallel Linear4bit backward: the argument checks of the input-gradient wrapper (against a fake
+library), the refusal of grad-requiring input by the symmetric-memory routes, and the collectives the backward runs in a
+simulated world of 4."""
+import pytest
+import torch
+
+import bitsandbytes_b200.backends.cuda as cb
+import bitsandbytes_b200.parallel as par
+from bitsandbytes_b200.parallel import ColumnParallelLinear4bit, RowParallelLinear4bit, Shard4bit
+from tests.test_sequence_parallel_cpu import _FakeLib
+
+
+def _shard(N=64, K=128, row0=0):
+    return Shard4bit(packed=torch.zeros(N * K // 2, dtype=torch.uint8), absmax=torch.ones(N * K // 64),
+                     absmax_8bit=None, absmax_code=None, absmax_offset=None, rows=N, row0=row0, K=K, blocksize=64,
+                     quant_type="nf4")
+
+
+@pytest.fixture
+def fake(monkeypatch):
+    lib = _FakeLib()
+    monkeypatch.setattr(cb, "lib", lib)
+    monkeypatch.setattr(cb, "_stream", lambda t: 0)
+    return lib
+
+
+def test_input_grad_wrapper_checks(fake):
+    """Bad G / out shapes, dtypes or strides raise before any native call; fp32 G is declined (False) without one; a
+    good call passes the row strides and the part flag."""
+    B, absmax = torch.zeros(64 * 128 // 2, dtype=torch.uint8), torch.ones(64 * 128 // 64)
+
+    def call(G, out):
+        return cb.gemm_4bit_input_grad(G, B, (64, 128), absmax, 64, "nf4", None, None, None, out)
+
+    G = torch.zeros(8, 64, dtype=torch.bfloat16)
+    for g, o in [(torch.zeros(8, 32, dtype=torch.bfloat16), torch.zeros(8, 128)),      # N mismatch
+                 (torch.zeros(64, 8, dtype=torch.bfloat16).t(), torch.zeros(8, 128)),   # column stride
+                 (G, torch.zeros(8, 127)),                                              # out shape
+                 (G, torch.zeros(8, 128, dtype=torch.float16))]:                        # out dtype
+        with pytest.raises(RuntimeError, match="gemm_4bit_input_grad"):
+            call(g, o)
+    assert fake.calls == []
+    assert not call(torch.zeros(8, 64), torch.zeros(8, 128)) and fake.calls == []
+    wide = torch.zeros(8, 192, dtype=torch.bfloat16)
+    assert call(wide[:, 64:128], torch.zeros(8, 136)[:, :128])
+    assert call(G, torch.zeros(8, 128, dtype=torch.bfloat16))
+    # (G, ldg, B, absmax, a8, code, offset, out, ldc, M, N, K, blocksize, quant_type, dtype, part, stream)
+    assert [(a[1], a[8], a[9], a[10], a[11], a[15]) for _, a in fake.calls] == [(192, 136, 8, 64, 128, 1),
+                                                                               (64, 128, 8, 64, 128, 0)]
+
+
+def test_fused_routes_refuse_grad_requiring_input():
+    col, row = ColumnParallelLinear4bit(_shard(), 64), RowParallelLinear4bit(_shard(), 128)
+    x = torch.zeros(4, 128, requires_grad=True)
+    for fn, layer in [(par.fused_forward, col), (par.fused_forward_col_sp, col), (par.fused_forward_row, row),
+                      (par.fused_forward_row_sp, row)]:
+        with pytest.raises(RuntimeError, match="inference only"):
+            fn(layer, x, None)
+
+
+@pytest.fixture
+def world4(monkeypatch, fake):
+    """A world of 4 seen from rank 1: the collectives record their shapes, the kernels are the fake library's."""
+    calls = []
+
+    def all_to_all_single(out, inp, group=None):
+        calls.append(("all_to_all_single", tuple(out.shape), tuple(inp.shape)))
+        out.copy_(inp)
+
+    def all_gather_into_tensor(out, inp, group=None):
+        calls.append(("all_gather_into_tensor", tuple(out.shape), tuple(inp.shape)))
+        out.copy_(inp.reshape(1, -1).expand(4, -1).reshape(out.shape))
+
+    monkeypatch.setattr(par, "_group_world_rank", lambda group: (4, 1))
+    monkeypatch.setattr(par.dist, "all_to_all_single", all_to_all_single)
+    monkeypatch.setattr(par.dist, "all_gather_into_tensor", all_gather_into_tensor)
+    monkeypatch.setattr(par, "reduce_partials", lambda parts, dtype, bias=None: parts.sum(0).to(dtype))
+    monkeypatch.setattr(par, "input_grad_dequant_matmul",
+                        lambda G, shard, dtype: torch.zeros(G.shape[0], shard.K, dtype=dtype))
+    return calls
+
+
+def test_backward_collectives_in_a_world_of_4(world4, fake):
+    """Column layer: the partials all-gathered as [4, M, K] (the gradient of the gathered output read in place at this
+    rank's columns), or exchanged by token under sequence parallelism; row layer: no exchange, or the token rows of
+    grad_y all-gathered under sequence parallelism.  Every input gets a gradient of its shape."""
+    M, K, rows = 8, 128, 64
+    col = ColumnParallelLinear4bit(_shard(rows, K, row0=rows), 4 * rows)
+    x = torch.zeros(M, K, dtype=torch.bfloat16, requires_grad=True)
+    col._backward(torch.zeros(M, 4 * rows, dtype=torch.bfloat16), x.shape)
+    sp = ColumnParallelLinear4bit(_shard(rows, K), 4 * rows, gather_output=False, sequence_parallel=True)
+    assert sp._backward(torch.zeros(M, rows, dtype=torch.bfloat16), (M // 4, K)).shape == (M // 4, K)
+    row = RowParallelLinear4bit(_shard(rows, K), 4 * K)
+    assert row._backward(torch.zeros(M, rows, dtype=torch.bfloat16), (M, K)).shape == (M, K)
+    row_sp = RowParallelLinear4bit(_shard(rows, K), 4 * K, sequence_parallel=True)
+    assert row_sp._backward(torch.zeros(M // 4, rows, dtype=torch.bfloat16), (M, K)).shape == (M, K)
+    assert world4 == [("all_gather_into_tensor", (4 * M * K,), (M * K,)),
+                      ("all_to_all_single", (4, M // 4, K), (4, M // 4, K)),
+                      ("all_gather_into_tensor", (M, rows), (M // 4, rows))]
+    # every product is dequantise + cuBLAS (the fake above): no native call
+    assert fake.calls == []
