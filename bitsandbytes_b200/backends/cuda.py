@@ -549,6 +549,40 @@ def int8_zero_columns(q: torch.Tensor, cols: torch.Tensor) -> None:
     lib.check("int8_zero_columns")
 
 
+def int8_dequant_rows(CB: torch.Tensor, SCB: torch.Tensor, dtype: torch.dtype,
+                      out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The weight of LLM.int8()'s input gradient, ``W[n, k] = dtype(CB[n, k] * (SCB[n] * (1/127)))``, in one pass: the
+    bits of ``CB.to(dtype, copy=True).mul_(SCB.unsqueeze(1).mul(1.0 / 127.0))`` for fp16 / bf16.  ``CB`` is int8
+    ``[rows, cols]``, ``SCB`` fp32 ``[rows]``; ``out`` may be a ``[rows, cols]`` view with unit column stride and any row
+    stride."""
+    if CB.dtype != torch.int8 or CB.dim() != 2:
+        raise RuntimeError(f"int8_dequant_rows: CB must be a 2-D int8 tensor, got {CB.dtype} {tuple(CB.shape)}")
+    rows, cols = CB.shape
+    if SCB.dtype != torch.float32 or SCB.shape != (rows,) or SCB.device != CB.device:
+        raise RuntimeError(f"int8_dequant_rows: SCB must be float32 [{rows}] on {CB.device}, got {SCB.dtype} "
+                           f"{tuple(SCB.shape)} on {SCB.device}")
+    if dtype not in (torch.float16, torch.bfloat16):
+        raise RuntimeError(f"int8_dequant_rows: dtype must be float16 or bfloat16, got {dtype}")
+    if out is None:
+        out = torch.empty((rows, cols), device=CB.device, dtype=dtype)
+    elif (out.dtype != dtype or out.shape != (rows, cols) or out.device != CB.device
+          or (rows > 1 and out.stride(0) < cols) or (cols > 1 and out.stride(1) != 1)):
+        raise RuntimeError(f"int8_dequant_rows: out must be {dtype} [{rows}, {cols}] with unit column stride and row "
+                           f"stride >= {cols} on {CB.device}")
+    ldo = out.stride(0) if rows > 1 else cols
+    _check_sizes("int8_dequant_rows", rows, cols, ldo)
+    if rows == 0 or cols == 0:
+        return out
+    CB, SCB = CB.contiguous(), SCB.contiguous()
+    with _on_device(CB):
+        rc = lib.cbnb_b200_int8_dequant_rows(CB.data_ptr(), SCB.data_ptr(), out.data_ptr(), ldo, rows, cols,
+                                             _DTYPE_ID[dtype], _stream(CB))
+    lib.check("int8_dequant_rows")
+    if rc != 0:
+        raise RuntimeError(f"int8_dequant_rows: the library refused the call (code {rc})")
+    return out
+
+
 @kernel("int8_vectorwise_quant")
 def _int8_vectorwise_quant(A: torch.Tensor, threshold=0.0):
     if A.dtype != torch.float16:

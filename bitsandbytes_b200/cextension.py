@@ -93,6 +93,8 @@ def _signatures():
     sig["cbnb_b200_int8_outlier_prep"] = ([_VOIDP] * 4 + [_I32] * 6 + [_VOIDP] * 3, None)
     # (A, out, col_stats, threshold, rows, cols, dtype, stream) -> int
     sig["cbnb_b200_int8_col_quant"] = ([_VOIDP] * 3 + [ct.c_float] + [_I32] * 3 + [_VOIDP], _I32)
+    # (CB, SCB, out, ldo, rows, cols, dtype, stream) -> int
+    sig["cbnb_b200_int8_dequant_rows"] = ([_VOIDP] * 3 + [_I32] * 4 + [_VOIDP], _I32)
     # (CA, cols, J, rows, K, stream)
     sig["cbnb_b200_int8_zero_columns"] = ([_VOIDP] * 2 + [_I32] * 3 + [_VOIDP], None)
     # (col_flags, K, cols, count, stream)

@@ -109,6 +109,8 @@ void launch_int8_outlier_compact(const int* col_flags, int K, int* cols, int* co
 void launch_int8_zero_columns(int8_t* CA, const long long* cols, int J, int rows, int K, cudaStream_t stream);
 bool launch_int8_col_quant(const void* A, int8_t* out, float* col_stats, float threshold, int rows, int cols, int dtype,
                            cudaStream_t stream);
+bool launch_int8_dequant_rows(const int8_t* CB, const float* SCB, void* out, int ldo, int rows, int cols, int dtype,
+                              cudaStream_t stream);
 
 template <typename T, int FUNC> void launch_elementwise(T* A, const T* B, T value, long n);
 
@@ -763,6 +765,20 @@ int cbnb_b200_int8_mixed_mm_dev(const int8_t* CA, const int8_t* CB, const float*
 int cbnb_b200_int8_col_quant(const void* A, int8_t* out, float* col_stats, float threshold, int rows, int cols, int dtype,
                              cudaStream_t stream) {
     return launch_int8_col_quant(A, out, col_stats, threshold, rows, cols, dtype, stream) ? 0 : 100;
+}
+
+// The weight of LLM.int8()'s input gradient in one pass: out[n, k] (row stride ldo) = T(float(CB[n, k]) * s[n]), s[n] =
+// SCB[n] * fp32(1/127), the bits of `CB.to(T, copy=True).mul_(SCB.unsqueeze(1).mul(1.0 / 127.0))`.  CB [rows, cols]
+// contiguous.  dtype 1 = fp16, 2 = bf16.  Returns 0; 1 with the error message set for bad arguments; 100, with nothing
+// written, for any other dtype.
+int cbnb_b200_int8_dequant_rows(const int8_t* CB, const float* SCB, void* out, int ldo, int rows, int cols, int dtype,
+                                cudaStream_t stream) {
+    const bool empty = rows == 0 || cols == 0;
+    if (rows < 0 || cols < 0 || ldo < cols || (!empty && (CB == nullptr || SCB == nullptr || out == nullptr))) {
+        set_last_error_msg("int8_dequant_rows: needs CB, SCB and out, rows >= 0, cols >= 0 and ldo >= cols");
+        return 1;
+    }
+    return launch_int8_dequant_rows(CB, SCB, out, ldo, rows, cols, dtype, stream) ? 0 : 100;
 }
 
 void cdequant_mm_int32_fp16(int* A, float* rowStats, float* colStats, __half* out, __half* bias, int numRows,

@@ -9,6 +9,8 @@
 //                       route that a CUDA graph can capture (no torch.nonzero, no host sync).
 //   int8 GEMM           lives in int8_gemm.cu.
 //   dequant_mm_int32    replaces reference kdequant_mm_int32_fp16 (csrc/kernels.cu:1396-1448).
+//   int8_dequant_rows   the weight of the input gradient, W = T(CB * SCB / 127), in one pass (the reference's
+//                       MatMul8bitLt.backward builds it with two torch kernels and a temporary).
 #include "common.cuh"
 #include "hopper_ptx.cuh"
 
@@ -342,6 +344,59 @@ __global__ void __launch_bounds__(256) int8_col_quant_kernel(const T* __restrict
     }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// The dequantised int8 weight for the input gradient of LLM.int8(): out[n, k] (row stride ldo) = T(float(CB[n, k]) * s)
+// with s = SCB[n] * fp32(1/127), the arithmetic of `CB.to(T).mul_(SCB.unsqueeze(1).mul(1.0 / 127.0))` (an fp32 scale,
+// one fp32 product, one rounding to T) in one read of the codes and one write of T.
+// blockIdx.y walks rows, blockIdx.x chunks of 16-code vectors within a row.  kVec: the codes and the output are
+// 16-byte aligned at the same column of every row (aligned bases, (ldo - cols) % 8 == 0), so a row is a scalar head up
+// to the first 16-byte aligned code, 16-code vectors (one 16-byte load, two 16-byte stores) and a scalar tail; the head
+// and tail are the first CTA's.  Otherwise every element is scalar.
+constexpr int kDqThreads = 256;
+
+template <typename T>
+__device__ __forceinline__ void dequant_rows_one(const int8_t* cb, T* o, int k, float s) {
+    o[k] = DT<T>::from_f32(__fmul_rn((float)cb[k], s));
+}
+
+template <typename T, bool kVec>
+__global__ void __launch_bounds__(kDqThreads)
+    int8_dequant_rows_kernel(const int8_t* __restrict__ CB, const float* __restrict__ SCB, T* __restrict__ out,
+                             long long ldo, int rows, int cols) {
+    for (int n = blockIdx.y; n < rows; n += gridDim.y) {
+        const int8_t* cb = CB + (long long)n * cols;
+        T* o = out + (long long)n * ldo;
+        const float s = __fmul_rn(__ldg(SCB + n), 7.874015718698502e-3f);
+        if constexpr (kVec) {
+            const int head = min((int)((16 - (((long long)n * cols) & 15)) & 15), cols);
+            const int nvec = (cols - head) >> 4;
+            const int tail0 = head + 16 * nvec;
+            const int v = blockIdx.x * kDqThreads + threadIdx.x;
+            if (v < nvec) {
+                const int k0 = head + 16 * v;
+                const uint4 q = ldg_stream_v4(cb + k0);
+                const uint32_t w[4] = {q.x, q.y, q.z, q.w};
+                uint32_t p[8];
+#pragma unroll
+                for (int i = 0; i < 8; ++i) {
+                    const uint32_t b = w[i >> 1] >> (16 * (i & 1));
+                    p[i] = pack2<T>(__fmul_rn((float)(int8_t)(b & 0xffu), s), __fmul_rn((float)(int8_t)(b >> 8), s));
+                }
+                *reinterpret_cast<uint4*>(o + k0) = make_uint4(p[0], p[1], p[2], p[3]);
+                *reinterpret_cast<uint4*>(o + k0 + 8) = make_uint4(p[4], p[5], p[6], p[7]);
+            }
+            const int t = threadIdx.x;
+            if (blockIdx.x == 0) {
+                if (t < head) dequant_rows_one(cb, o, t, s);
+                if (t >= 32 && t - 32 < cols - tail0) dequant_rows_one(cb, o, tail0 + t - 32, s);
+            }
+        } else {
+            for (int k = blockIdx.x * kDqThreads + threadIdx.x; k < cols; k += gridDim.x * kDqThreads)
+                dequant_rows_one(cb, o, k, s);
+        }
+    }
+}
+
 } // namespace
 
 // ---------------------------------------------------------------- launch wrappers
@@ -415,6 +470,32 @@ bool launch_int8_col_quant(const void* A, int8_t* out, float* col_stats, float t
     }
 #undef BNB200_COLQ
     BNB200_CHECK_LAUNCH("int8_col_quant");
+    return true;
+}
+
+// out[rows, cols] (row stride ldo) = T(CB[n, k] * (SCB[n] * fp32(1/127))); dtype: 1 fp16, 2 bf16 (false: dtype not
+// served, nothing launched)
+bool launch_int8_dequant_rows(const int8_t* CB, const float* SCB, void* out, int ldo, int rows, int cols, int dtype,
+                              cudaStream_t stream) {
+    if (dtype != 1 && dtype != 2) return false;
+    if (rows <= 0 || cols <= 0) return true;
+    const bool vec = ((reinterpret_cast<uintptr_t>(CB) & 15) == 0) && ((reinterpret_cast<uintptr_t>(out) & 15) == 0) &&
+                     ((ldo - cols) % 8 == 0);
+    const int per_row = vec ? cols / 16 : cols;  // threads' work items per row
+    const int chunks = (per_row + kDqThreads - 1) / kDqThreads;
+    const dim3 grid(chunks > 0 ? chunks : 1, rows < 65535 ? rows : 65535);
+#define BNB200_DQR(T)                                                                                                  \
+    if (vec)                                                                                                           \
+        int8_dequant_rows_kernel<T, true><<<grid, kDqThreads, 0, stream>>>(CB, SCB, (T*)out, ldo, rows, cols);        \
+    else                                                                                                               \
+        int8_dequant_rows_kernel<T, false><<<grid, kDqThreads, 0, stream>>>(CB, SCB, (T*)out, ldo, rows, cols)
+    if (dtype == 1) {
+        BNB200_DQR(__half);
+    } else {
+        BNB200_DQR(__nv_bfloat16);
+    }
+#undef BNB200_DQR
+    BNB200_CHECK_LAUNCH("int8_dequant_rows");
     return true;
 }
 

@@ -73,7 +73,9 @@ all-gather of ``grad_y``'s token rows under sequence parallelism; with ``input_i
 input, of which the layer uses its columns) the ranks' ``grad_x_r`` are all-gathered along the features, in rank order,
 into the whole input gradient.  Both products run as dequantise + cuBLAS (:func:`input_grad_dequant_matmul`, chosen in
 ``_input_grad`` from the timings against the library's input-gradient kernel, ``gemm_4bit_input_grad``).  The
-``fused_forward*`` routes stay inference only and refuse an input that requires grad.
+tensor-parallel LLM.int8() layers below share this backward (``_ColumnInputGrad``, ``_RowInputGrad``); only the
+dequantised weight differs (``Shard4bit.dequantize``, ``Shard8bit.dequantize``).  The ``fused_forward*`` routes stay
+inference only and refuse an input that requires grad.
 """
 from __future__ import annotations
 
@@ -85,7 +87,8 @@ import torch.distributed as dist
 
 from . import functional as F
 from .backends.cuda import (gemm_4bit_into, gemm_4bit_multi_out, gemm_4bit_partial,
-                            gemm_4bit_partial_scatter, int8_gemm_multi_out, int8_gemm_partial_scatter, int8_outlier_operands, int8_quant_with_stats,
+                            gemm_4bit_partial_scatter, int8_dequant_rows, int8_gemm_multi_out, int8_gemm_partial_scatter,
+                            int8_outlier_operands, int8_quant_with_stats,
                             int8_reduce_partials, int8_row_stats, int8_vectorwise_quant_flags, int8_zero_columns,
                             reduce_partials)
 
@@ -105,6 +108,15 @@ class Shard4bit:
     blocksize: int
     quant_type: str
     k0: int = 0                     # first input feature of a K shard (slice_quantized_weight_k)
+
+    def dequantize(self, dtype: torch.dtype) -> torch.Tensor:
+        """The shard's weight ``[rows, K]`` decoded to ``dtype`` as ``dequantize_4bit`` decodes it."""
+        scales = self.absmax
+        if self.absmax_8bit is not None:
+            scales = _nested_scales(self.absmax_8bit, self.absmax, self.absmax_code, self.absmax_offset)
+        out = torch.empty((self.rows, self.K), device=self.packed.device, dtype=dtype)
+        return F.dequantize_4bit(self.packed, absmax=scales, out=out, blocksize=self.blocksize,
+                                 quant_type=self.quant_type)
 
 
 def shard_rows(N: int, world: int, rank: int) -> tuple[int, int]:
@@ -137,7 +149,80 @@ def slice_quantized_weight(packed: torch.Tensor, qs: F.QuantState, world: int, r
                      quant_type=qs.quant_type)
 
 
-class ColumnParallelLinear4bit(torch.nn.Module):
+class _ColumnInputGrad:
+    """The backward of a column-parallel layer, shared by the 4-bit and the int8 layers: the layer provides ``shard``
+    (``rows``, ``row0``, ``K`` and ``dequantize(dtype)``), ``group`` and ``sequence_parallel``."""
+
+    def input_grad_partial(self, grad_y: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
+        """This rank's fp32 partial ``P_r = G_r . W_r`` of the input gradient into ``out`` ``[M, K]``: ``G_r`` is
+        ``grad_y`` itself (``[M, rows]``, this rank's output) or, for the ``[M, world * rows]`` gathered output, this
+        rank's columns of it, read in place."""
+        s = self.shard
+        G = grad_y.reshape(-1, grad_y.shape[-1])
+        if G.shape[1] != s.rows:
+            G = G[:, s.row0:s.row0 + s.rows]
+        return _input_grad(G, s, out)
+
+    def _backward(self, grad_y: torch.Tensor, x_shape) -> torch.Tensor:
+        s = self.shard
+        world, rank = _group_world_rank(self.group)
+        M = grad_y.numel() // grad_y.shape[-1]
+        if self.sequence_parallel and world > 1:
+            # the partial over all M tokens, its rows sent to the ranks that own them: chunk r of recv is rank r's
+            send = torch.empty((world, M // world, s.K), device=grad_y.device)
+            self.input_grad_partial(grad_y, send.view(M, s.K))
+            recv = torch.empty_like(send)
+            dist.all_to_all_single(recv, send, group=self.group)
+            return reduce_partials(recv, grad_y.dtype).view(x_shape)
+        stage = torch.empty((world, M, s.K), device=grad_y.device)
+        self.input_grad_partial(grad_y, stage[rank])
+        if world > 1:
+            dist.all_gather_into_tensor(stage.view(-1), stage[rank].reshape(-1), group=self.group)
+        return reduce_partials(stage, grad_y.dtype).view(x_shape)
+
+
+class _RowInputGrad:
+    """The backward of a row-parallel layer, shared by the 4-bit and the int8 layers: the layer provides ``shard``
+    (``rows``, ``K`` and ``dequantize(dtype)``), ``group``, ``input_is_parallel`` and ``sequence_parallel``."""
+
+    def input_grad(self, grad_y: torch.Tensor) -> torch.Tensor:
+        """``grad_x_r = grad_y . W_r`` ``[M, K/world]`` for the ``[..., N]`` output gradient of all M tokens."""
+        s = self.shard
+        G = grad_y.reshape(-1, s.rows)
+        return _input_grad(G, s, torch.empty((G.shape[0], s.K), device=G.device, dtype=G.dtype))
+
+    def _backward(self, grad_y: torch.Tensor, x_shape) -> torch.Tensor:
+        world, _ = _group_world_rank(self.group)
+        if self.sequence_parallel and world > 1:
+            # this rank's tokens' rows of grad_y -> all M rows, in rank order (= token order)
+            full = torch.empty((world * grad_y.shape[0], *grad_y.shape[1:]), device=grad_y.device, dtype=grad_y.dtype)
+            dist.all_gather_into_tensor(full, grad_y.contiguous(), group=self.group)
+            grad_y = full
+        g = self.input_grad(grad_y)
+        if not self.input_is_parallel and world > 1:
+            # the layer took the whole (replicated) input and used only its columns: the input gradient is every rank's
+            # columns, all-gathered in rank order (the backward of the scatter)
+            parts = torch.empty((world, *g.shape), device=g.device, dtype=g.dtype)
+            dist.all_gather_into_tensor(parts, g, group=self.group)
+            g = parts.permute(1, 0, 2).reshape(g.shape[0], world * g.shape[1])
+        return g.view(x_shape)
+
+
+class _ParallelFn(torch.autograd.Function):
+    """A tensor-parallel layer's forward (``layer._forward``), with the input gradient as its backward
+    (``layer._backward``): the shard and the bias stay frozen."""
+
+    @staticmethod
+    def forward(ctx, x, layer):
+        ctx.layer, ctx.x_shape = layer, x.shape
+        return layer._forward(x)
+
+    @staticmethod
+    def backward(ctx, grad_y):
+        return ctx.layer._backward(grad_y, ctx.x_shape), None
+
+
+class ColumnParallelLinear4bit(_ColumnInputGrad, torch.nn.Module):
     """``y = x @ dequant(W)^T + b`` with W's output features split across the process group."""
 
     def __init__(self, shard: Shard4bit, out_features: int, bias: Optional[torch.Tensor] = None,
@@ -174,7 +259,7 @@ class ColumnParallelLinear4bit(torch.nn.Module):
         return out
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
-        return _ColumnParallel4bitFn.apply(x, self)
+        return _ParallelFn.apply(x, self)
 
     def _forward(self, x: torch.Tensor) -> torch.Tensor:
         s = self.shard
@@ -189,57 +274,13 @@ class ColumnParallelLinear4bit(torch.nn.Module):
             return self.local_forward(x).view(*lead, s.rows)
         return _gather_columns(self, x, M, x.dtype, x.device).reshape(*lead, world * s.rows)
 
-    def input_grad_partial(self, grad_y: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
-        """This rank's fp32 partial ``P_r = G_r . dequant(W_r)`` of the input gradient into ``out`` ``[M, K]``: ``G_r``
-        is ``grad_y`` itself (``[M, rows]``, this rank's output) or, for the ``[M, world * rows]`` gathered output, this
-        rank's columns of it, read in place."""
-        s = self.shard
-        G = grad_y.reshape(-1, grad_y.shape[-1])
-        if G.shape[1] != s.rows:
-            G = G[:, s.row0:s.row0 + s.rows]
-        return _input_grad(G, s, out)
 
-    def _backward(self, grad_y: torch.Tensor, x_shape) -> torch.Tensor:
-        s = self.shard
-        world, rank = _group_world_rank(self.group)
-        M = grad_y.numel() // grad_y.shape[-1]
-        if self.sequence_parallel and world > 1:
-            # the partial over all M tokens, its rows sent to the ranks that own them: chunk r of recv is rank r's
-            send = torch.empty((world, M // world, s.K), device=grad_y.device)
-            self.input_grad_partial(grad_y, send.view(M, s.K))
-            recv = torch.empty_like(send)
-            dist.all_to_all_single(recv, send, group=self.group)
-            return reduce_partials(recv, grad_y.dtype).view(x_shape)
-        stage = torch.empty((world, M, s.K), device=grad_y.device)
-        self.input_grad_partial(grad_y, stage[rank])
-        if world > 1:
-            dist.all_gather_into_tensor(stage.view(-1), stage[rank].reshape(-1), group=self.group)
-        return reduce_partials(stage, grad_y.dtype).view(x_shape)
-
-
-class _ColumnParallel4bitFn(torch.autograd.Function):
-    """``ColumnParallelLinear4bit``'s forward, with the input gradient as its backward (the shard stays frozen)."""
-
-    @staticmethod
-    def forward(ctx, x, layer):
-        ctx.layer, ctx.x_shape = layer, x.shape
-        return layer._forward(x)
-
-    @staticmethod
-    def backward(ctx, grad_y):
-        return ctx.layer._backward(grad_y, ctx.x_shape), None
-
-
-def input_grad_dequant_matmul(G: torch.Tensor, shard: Shard4bit, dtype: torch.dtype) -> torch.Tensor:
-    """``G . dequant(W)`` ``[M, K]`` by dequantise + ``torch.matmul``: the shard decoded to G's dtype as
-    ``dequantize_4bit`` decodes it, multiplied by cuBLAS with an output of ``dtype`` -- G's dtype, or fp32 on the fp32
-    accumulation of the 16-bit operands for a partial."""
-    s = shard
-    scales = s.absmax
-    if s.absmax_8bit is not None:
-        scales = _nested_scales(s.absmax_8bit, s.absmax, s.absmax_code, s.absmax_offset)
-    W = F.dequantize_4bit(s.packed, absmax=scales, out=torch.empty((s.rows, s.K), device=G.device, dtype=G.dtype),
-                          blocksize=s.blocksize, quant_type=s.quant_type)
+def input_grad_dequant_matmul(G: torch.Tensor, shard, dtype: torch.dtype) -> torch.Tensor:
+    """``G . W`` ``[M, K]`` by dequantise + ``torch.matmul``: the shard's weight (a :class:`Shard4bit` decoded as
+    ``dequantize_4bit`` decodes it, a :class:`Shard8bit` as ``MatMul8bitLt.backward`` dequantises it) in G's dtype,
+    multiplied by cuBLAS with an output of ``dtype`` -- G's dtype, or fp32 on the fp32 accumulation of the 16-bit
+    operands for a partial."""
+    W = shard.dequantize(G.dtype)
     if dtype == G.dtype:
         return torch.matmul(G, W)
     if G.dtype != torch.float32:
@@ -247,13 +288,13 @@ def input_grad_dequant_matmul(G: torch.Tensor, shard: Shard4bit, dtype: torch.dt
     return torch.matmul(G.float(), W.float())
 
 
-def _input_grad(G: torch.Tensor, shard: Shard4bit, out: torch.Tensor) -> torch.Tensor:
-    """``out[M, K] = G . dequant(W)`` (``G`` ``[M, rows]`` in any layout): fp32 ``out`` receives the unrounded partial,
-    one of G's dtype the sum rounded once.  The route is chosen here, from the timings on an H100 (DESIGN.md section 6,
-    tools/time_gemm4_input_grad.py): dequantise + cuBLAS -- with an fp32 output from the 16-bit operands for a partial
-    -- is as fast as the input-gradient kernel or faster at every shape and token count measured but one (4096 x 4096
-    at 256 tokens, not a range of M), so the layers take it at every M; the kernel (``gemm_4bit_input_grad``) stays in
-    the library."""
+def _input_grad(G: torch.Tensor, shard, out: torch.Tensor) -> torch.Tensor:
+    """``out[M, K] = G . W`` (``G`` ``[M, rows]`` in any layout, ``shard`` a Shard4bit or Shard8bit): fp32 ``out``
+    receives the unrounded partial, one of G's dtype the sum rounded once.  The route is chosen here, from the timings
+    on an H100 (DESIGN.md section 6, tools/time_gemm4_input_grad.py): dequantise + cuBLAS -- with an fp32 output from
+    the 16-bit operands for a partial -- is as fast as the 4-bit input-gradient kernel or faster at every shape and
+    token count measured but one (4096 x 4096 at 256 tokens, not a range of M), so the layers take it at every M; the
+    kernel (``gemm_4bit_input_grad``) stays in the library.  The int8 layers have no other route."""
     out.copy_(input_grad_dequant_matmul(G, shard, out.dtype))
     return out
 
@@ -413,7 +454,7 @@ def slice_quantized_weight_k(packed: torch.Tensor, qs: F.QuantState, world: int,
                      row0=0, K=kr, blocksize=bs, quant_type=qs.quant_type, k0=k0)
 
 
-class RowParallelLinear4bit(torch.nn.Module):
+class RowParallelLinear4bit(_RowInputGrad, torch.nn.Module):
     """``y = x @ dequant(W)^T + b`` with W's input features split across the process group: every rank returns the
     whole ``[..., N]`` output, the same bits on every rank."""
 
@@ -463,32 +504,11 @@ class RowParallelLinear4bit(torch.nn.Module):
                                          None, outs, s.rows if ldc is None else ldc)
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
-        return _RowParallel4bitFn.apply(x, self)
+        return _ParallelFn.apply(x, self)
 
-    def input_grad(self, grad_y: torch.Tensor) -> torch.Tensor:
-        """``grad_x_r = grad_y . dequant(W_r)`` ``[M, K/world]`` for the ``[..., N]`` output gradient of all M tokens."""
+    def _forward(self, x: torch.Tensor) -> torch.Tensor:
         s = self.shard
-        G = grad_y.reshape(-1, s.rows)
-        return _input_grad(G, s, torch.empty((G.shape[0], s.K), device=G.device, dtype=G.dtype))
-
-    def _backward(self, grad_y: torch.Tensor, x_shape) -> torch.Tensor:
-        world, _ = _group_world_rank(self.group)
-        if self.sequence_parallel and world > 1:
-            # this rank's tokens' rows of grad_y -> all M rows, in rank order (= token order)
-            full = torch.empty((world * grad_y.shape[0], *grad_y.shape[1:]), device=grad_y.device, dtype=grad_y.dtype)
-            dist.all_gather_into_tensor(full, grad_y.contiguous(), group=self.group)
-            grad_y = full
-        g = self.input_grad(grad_y)
-        if not self.input_is_parallel and world > 1:
-            # the layer took the whole (replicated) input and used only its columns: the input gradient is every rank's
-            # columns, all-gathered in rank order (the backward of the scatter)
-            parts = torch.empty((world, *g.shape), device=g.device, dtype=g.dtype)
-            dist.all_gather_into_tensor(parts, g, group=self.group)
-            g = parts.permute(1, 0, 2).reshape(g.shape[0], world * g.shape[1])
-        return g.view(x_shape)
-
-    def _forward(self, x_r: torch.Tensor) -> torch.Tensor:
-        s = self.shard
+        x_r = self.local_input(x)
         M = x_r.numel() // s.K
         if self.sequence_parallel:
             return self._sp_forward(x_r, x_r.dtype)
@@ -516,19 +536,6 @@ class RowParallelLinear4bit(torch.nn.Module):
         world, _ = _group_world_rank(self.group)
         parts = self._sp_exchange(x_r)
         return reduce_partials(parts, dtype, self.bias).view(x_r.shape[0] // world, *x_r.shape[1:-1], self.shard.rows)
-
-
-class _RowParallel4bitFn(torch.autograd.Function):
-    """``RowParallelLinear4bit``'s forward, with the input gradient as its backward (the shard stays frozen)."""
-
-    @staticmethod
-    def forward(ctx, x, layer):
-        ctx.layer, ctx.x_shape = layer, x.shape
-        return layer._forward(layer.local_input(x))
-
-    @staticmethod
-    def backward(ctx, grad_y):
-        return ctx.layer._backward(grad_y, ctx.x_shape), None
 
 
 class PeerPartials(_PeerSlots):
@@ -610,7 +617,13 @@ def reassemble_shards(shards: list[Shard4bit]) -> tuple[torch.Tensor, torch.Tens
 #     the reduction applies the GEMM's own per-element epilogue once.  The outlier columns of the ranks, concatenated
 #     in rank order, are the unsharded ascending list, and their operands are the unsharded ones.
 # Beyond 64 outlier columns the unsharded layer adds the outlier product with `addmm`; both layers then run that same
-# `addmm` on the same full-size operands.  Inference only: no backward, ``state.idx`` is not kept.
+# `addmm` on the same full-size operands.  ``state.idx`` is not kept.
+#
+# Training (LoRA on an 8-bit base).  Both layers run their forward through ``_ParallelFn`` (the same bits) and share the
+# 4-bit layers' backward (``_ColumnInputGrad`` / ``_RowInputGrad``): the input gradient ``grad_y . W`` and nothing else,
+# W = T(CB * SCB / 127) dequantised in one pass (``Shard8bit.dequantize``) as ``MatMul8bitLt.backward`` dequantises it.
+# As there, the outlier decomposition of the forward leaves the gradient alone: the whole CB enters it, so the backward
+# needs no outlier list and no host synchronisation.
 #
 # Sequence parallelism (``sequence_parallel=True``, as for the 4-bit layers: rank r owns the flattened tokens
 # ``[r*M/w, (r+1)*M/w)`` of an activation whose first dimension splits over the ranks).  The outputs stay the unsharded
@@ -639,6 +652,11 @@ class Shard8bit:
     row0: int
     K: int
     k0: int = 0
+
+    def dequantize(self, dtype: torch.dtype) -> torch.Tensor:
+        """The shard's weight ``[rows, K]`` in ``dtype`` (fp16 / bf16) as ``MatMul8bitLt.backward`` dequantises it,
+        ``dtype(CB * (SCB / 127))`` row by row, in one pass (``int8_dequant_rows``)."""
+        return int8_dequant_rows(self.CB, self.SCB, dtype)
 
 
 def _check_rank(world: int, rank: int) -> None:
@@ -704,7 +722,7 @@ class Int8Input:
         return 0 if self.cols is None else int(self.cols.numel())
 
 
-class ColumnParallelLinear8bitLt(torch.nn.Module):
+class ColumnParallelLinear8bitLt(_ColumnInputGrad, torch.nn.Module):
     """LLM.int8() ``y = x @ W^T + b`` with W's output features split across the process group.  Every rank's output
     equals the unsharded inference ``Linear8bitLt`` output (its columns, with ``gather_output=False``) bit for bit.
     With ``sequence_parallel=True`` the input is this rank's tokens ``[M/w, ..., K]`` and the output ``[M, ..., N/w]``."""
@@ -851,6 +869,9 @@ class ColumnParallelLinear8bitLt(torch.nn.Module):
         return full.addmm(subA, subBT.t())
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
+        return _ParallelFn.apply(x, self)
+
+    def _forward(self, x: torch.Tensor) -> torch.Tensor:
         world, _ = _group_world_rank(self.group)
         if self.sequence_parallel and world > 1:
             return self._output(self.sp_quantize(x), (world * x.shape[0], *x.shape[1:-1]))
@@ -884,6 +905,7 @@ def fused_forward_col8(layer: ColumnParallelLinear8bitLt, x: torch.Tensor, peers
     """``layer(x)`` with the all-gather fused into the int8 GEMM epilogue: each output element is stored into this
     rank's columns of every rank's symmetric ``[M, N]`` buffer.  Past 64 outlier columns, or for a shape the GEMM does
     not take, the local GEMM + NCCL route fills the same slot.  Returns this rank's [M, N] slot."""
+    _no_grad_route(x, "fused_forward_col8")
     s = layer.shard
     q = layer.quantize(x)
     M = q.A.shape[0]
@@ -927,6 +949,7 @@ def fused_forward_col8_sp(layer: ColumnParallelLinear8bitLt, x: torch.Tensor, pe
     quantises its ``[M/w, ..., K]`` tokens and copies the codes and row statistics into its rows of every rank's slot
     (``peers = PeerInt8Input(M, K)``), one barrier publishes them, and the local GEMM reads the gathered codes.  Returns
     ``[M, ..., N/w]``."""
+    _no_grad_route(x, "fused_forward_col8_sp")
     world, _ = _group_world_rank(layer.group)
     return layer._output(layer.sp_quantize(x, peers), (world * x.shape[0], *x.shape[1:-1]))
 
@@ -940,7 +963,7 @@ class Int8Stats:
     flags: Optional[torch.Tensor]   # int32 [K / world]: the slice's outlier columns (threshold > 0)
 
 
-class RowParallelLinear8bitLt(torch.nn.Module):
+class RowParallelLinear8bitLt(_RowInputGrad, torch.nn.Module):
     """LLM.int8() ``y = x @ W^T + b`` with W's input features split across the process group: every rank returns the
     whole ``[..., N]`` output, equal to the unsharded inference ``Linear8bitLt`` output bit for bit.
 
@@ -1089,6 +1112,9 @@ class RowParallelLinear8bitLt(torch.nn.Module):
         return x_r, world, SCA, CA, cols
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
+        return _ParallelFn.apply(x, self)
+
+    def _forward(self, x: torch.Tensor) -> torch.Tensor:
         if self.sequence_parallel:
             return self._sp_forward(x)
         s = self.shard
@@ -1150,6 +1176,7 @@ def fused_forward_row8(layer: RowParallelLinear8bitLt, x: torch.Tensor, peers: P
     """``layer(x)`` with the exchange of the int32 partials fused into the GEMM epilogue: ``P_r`` is stored into slot r
     of every rank's symmetric buffer, one barrier publishes them, and each rank reduces its own buffer.  The row
     statistics (a max) and the outlier operands still travel through NCCL."""
+    _no_grad_route(x, "fused_forward_row8")
     s = layer.shard
     x_r, _, SCA, CA, cols = layer._prologue(x)
     M = x_r.shape[0]
@@ -1169,4 +1196,5 @@ def fused_forward_row8_sp(layer: RowParallelLinear8bitLt, x: torch.Tensor, peers
     N]`` buffer (``peers = PeerPartials(M // world, N, dtype=torch.int32)``), one barrier publishes them, and each rank
     reduces its own with its rows of the statistics and outlier operands.  Past 64 outlier columns the slow path of the
     NCCL route runs instead (:meth:`RowParallelLinear8bitLt._sp_forward`)."""
+    _no_grad_route(x, "fused_forward_row8_sp")
     return layer._sp_forward(x, peers)

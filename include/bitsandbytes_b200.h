@@ -237,6 +237,12 @@ void cbnb_b200_int8_outlier_prep(const void* A, const int8_t* CB, const float* S
  * out[r,c] = int8(rint(float(T(A[r,c] * 127)) / col_stats[c])), outliers -> 0.  dtype 1 = fp16, 2 = bf16.  Returns 0 / 100. */
 int cbnb_b200_int8_col_quant(const void* A, int8_t* out, float* col_stats, float threshold, int rows, int cols, int dtype, bnb_stream_t stream);
 
+/* The weight of LLM.int8()'s input gradient in one pass: out[n, k] (row stride ldo >= cols) =
+ * T(float(CB[n, k]) * s[n]), s[n] = SCB[n] * fp32(1/127), the bits of `CB.to(T).mul_(SCB.unsqueeze(1).mul(1.0 / 127.0))`.
+ * CB [rows, cols] int8 contiguous, SCB [rows] fp32.  dtype 1 = fp16, 2 = bf16.  Returns 0; 1 with the error message set
+ * for bad arguments; 100, with nothing written, for any other dtype. */
+int cbnb_b200_int8_dequant_rows(const int8_t* CB, const float* SCB, void* out, int ldo, int rows, int cols, int dtype, bnb_stream_t stream);
+
 /* CA[:, cols[j]] = 0 for the J outlier columns (reference backends/cuda/ops.py:233-236). */
 void cbnb_b200_int8_zero_columns(int8_t* CA, const long long* cols, int J, int rows, int K, bnb_stream_t stream);
 
