@@ -396,6 +396,51 @@ def reduce_partials(parts: torch.Tensor, dtype: torch.dtype, bias: Optional[torc
     return out
 
 
+def reduce_partials_ptrs(ptrs, M: int, N: int, dtype: torch.dtype, row0: int = 0, rows: Optional[int] = None,
+                         bias: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """:func:`reduce_partials` over 1..8 ``[M, N]`` fp32 partials in separate buffers, listed in rank order, and only
+    over the rows ``[row0, row0 + rows)``: ``out[m] = dtype(((ptrs[0] + ptrs[1]) + ...)[row0 + m] + bias)``, the same
+    bits as :func:`reduce_partials` on the stacked partials.  A partial is a contiguous fp32 ``[M, N]`` CUDA tensor,
+    checked here, or a raw device address (a peer's symmetric-memory slot), which the caller vouches for.  ``out`` may
+    be a ``[rows, N]`` view with unit column stride and any row stride."""
+    if dtype not in _DTYPE_ID:
+        raise RuntimeError(f"reduce_partials_ptrs: unsupported dtype {dtype}")
+    rows = M - row0 if rows is None else rows
+    if M < 0 or N < 0 or row0 < 0 or rows < 0 or row0 + rows > M:
+        raise RuntimeError(f"reduce_partials_ptrs: the row window [{row0}, {row0 + rows}) is outside the {M} rows")
+    tensors = [p for p in ptrs if isinstance(p, torch.Tensor)]
+    device = out.device if out is not None else tensors[0].device if tensors else torch.device(
+        "cuda", torch.cuda.current_device())
+    if device.type != "cuda":
+        raise RuntimeError(f"reduce_partials_ptrs: the partials must be on a CUDA device, got {device}")
+    if any(p.shape != (M, N) or not p.is_contiguous() for p in tensors):
+        raise RuntimeError(f"reduce_partials_ptrs: partials must be contiguous [{M}, {N}] tensors (the kernel reads them "
+                           "at row stride N)")
+    addrs = _dest_ptrs("reduce_partials_ptrs", ptrs, torch.float32, device, M, N, N, RuntimeError)
+    if bias is not None and (bias.dtype != dtype or bias.shape != (N,) or bias.device != device):
+        raise RuntimeError(f"reduce_partials_ptrs: bias must be {dtype} [{N}] on {device}")
+    if bias is not None:
+        bias = bias.contiguous()
+    if out is None:
+        out = torch.empty((rows, N), dtype=dtype, device=device)
+    elif (out.dtype != dtype or out.shape != (rows, N) or (N > 1 and out.stride(1) != 1)
+          or (rows > 1 and out.stride(0) < N)):
+        raise RuntimeError(f"reduce_partials_ptrs: out must be {dtype} [{rows}, {N}] with unit column stride on "
+                           f"{device}")
+    _check_sizes("reduce_partials_ptrs", M, N, out.stride(0))
+    if rows == 0 or N == 0:
+        return out
+    arr = (ct.c_void_p * len(addrs))(*addrs)
+    with _on_device(out):
+        rc = lib.cbnb_b200_reduce_partials_ptrs(ct.cast(arr, ct.c_void_p), len(addrs), row0, rows, out.data_ptr(),
+                                                bias.data_ptr() if bias is not None else None, M, N, out.stride(0),
+                                                _DTYPE_ID[dtype], _stream(out))
+    lib.check("reduce_partials_ptrs")
+    if rc != 0:
+        raise RuntimeError(f"reduce_partials_ptrs: the library refused the call (code {rc})")
+    return out
+
+
 @kernel("gemm_4bit")
 def _gemm_4bit(A, B, shapeB, absmax, blocksize: int, quant_type: str, bias=None, absmax_8bit=None, absmax_code=None,
                absmax_offset=None):

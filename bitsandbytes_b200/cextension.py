@@ -78,6 +78,8 @@ def _signatures():
     sig["cbnb_b200_gemm_4bit_input_grad_panel"] = ([_VOIDP, _I32] + [_VOIDP] * 6 + [_I32] * 9 + [_VOIDP], _I32)
     # (parts, world, part_stride, out, bias, M, N, ldc, dtype, stream) -> int
     sig["cbnb_b200_reduce_partials"] = ([_VOIDP, _I32, ct.c_longlong, _VOIDP, _VOIDP] + [_I32] * 4 + [_VOIDP], _I32)
+    # (parts, n_parts, row0, rows, out, bias, M, N, ldc, dtype, stream) -> int
+    sig["cbnb_b200_reduce_partials_ptrs"] = ([_VOIDP] + [_I32] * 3 + [_VOIDP] * 2 + [_I32] * 4 + [_VOIDP], _I32)
     # (A, B, absmax, absmax_8bit, absmax_code, absmax_offset, outs, n_outs, bias, M, N, K, ldc, blocksize, quant_type,
     #  dtype, mt, panel_rows, stream) -> int
     sig["cbnb_b200_gemm_4bit_staged"] = ([_VOIDP] * 7 + [_I32] + [_VOIDP] + [_I32] * 9 + [_VOIDP], _I32)

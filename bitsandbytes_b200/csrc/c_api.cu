@@ -75,6 +75,9 @@ int launch_gemm4_input_grad(const T* G, int ldg, const uint8_t* B, const float* 
 // partials.cu
 bool launch_reduce_partials(const float* parts, int world, long long part_stride, void* out, const void* bias, int M,
                             int N, int ldc, int dtype, cudaStream_t stream);
+int max_reduce_parts();
+bool launch_reduce_partials_ptrs(const float* const* parts, int n_parts, int row0, int rows, void* out,
+                                 const void* bias, int N, int ldc, int dtype, cudaStream_t stream);
 template <typename T>
 bool launch_gemm_decoded(const T* A, const T* W, T* out, const T* bias, int M, int N, int K, int ldc, int mt,
                          cudaStream_t stream);
@@ -556,6 +559,31 @@ int cbnb_b200_gemm_4bit_partial_scatter(const void* A, const uint8_t* B, const f
 int cbnb_b200_reduce_partials(const float* parts, int world, long long part_stride, void* out, const void* bias, int M,
                               int N, int ldc, int dtype, cudaStream_t stream) {
     return launch_reduce_partials(parts, world, part_stride, out, bias, M, N, ldc, dtype, stream) ? 0 : 100;
+}
+
+// cbnb_b200_reduce_partials over partials in separate buffers: out[m, n] (row stride ldc, m < rows) =
+// T(((parts[0] + parts[1]) + ... + parts[n_parts - 1])[row0 + m, n] + bias[n]), each parts[r] an [M, N] fp32 partial at
+// row stride N -- a rank's own buffer or a peer's symmetric-memory mapping -- listed in rank order.  The same
+// element-wise arithmetic as cbnb_b200_reduce_partials, so the same bits.  dtype 0 or 3 = fp32, 1 = fp16, 2 = bf16.
+// Returns 0; 1 with the error message set unless 1 <= n_parts <= 8, every partial is non-null and 4-byte aligned, out
+// (and bias, when given) are aligned to their element, 0 <= row0, 0 <= rows, row0 + rows <= M and ldc >= N; or 100
+// for a dtype it does not serve.
+int cbnb_b200_reduce_partials_ptrs(const float* const* parts, int n_parts, int row0, int rows, void* out,
+                                   const void* bias, int M, int N, int ldc, int dtype, cudaStream_t stream) {
+    if (dtype < 0 || dtype > 3) return 100;
+    const uintptr_t esz = dtype == 1 || dtype == 2 ? 2 : 4;
+    bool ok = parts != nullptr && n_parts >= 1 && n_parts <= max_reduce_parts() && row0 >= 0 && rows >= 0 && M >= 0 &&
+              N >= 0 && (long long)row0 + rows <= M && ldc >= N && out != nullptr &&
+              (reinterpret_cast<uintptr_t>(out) & (esz - 1)) == 0 &&
+              (reinterpret_cast<uintptr_t>(bias) & (esz - 1)) == 0;
+    for (int r = 0; ok && r < n_parts; ++r)
+        ok = parts[r] != nullptr && (reinterpret_cast<uintptr_t>(parts[r]) & 3) == 0;
+    if (!ok) {
+        set_last_error_msg("reduce_partials_ptrs: needs 1 <= n_parts <= 8 non-null, 4-byte aligned partials, out and "
+                           "bias aligned to their element, 0 <= row0, 0 <= rows, row0 + rows <= M and ldc >= N");
+        return 1;
+    }
+    return launch_reduce_partials_ptrs(parts, n_parts, row0, rows, out, bias, N, ldc, dtype, stream) ? 0 : 100;
 }
 
 // The input gradient of a 4-bit linear layer: out[m, k] (row stride ldc) = sum over n of G[m, n] * dequant(W)[n, k],

@@ -23,6 +23,7 @@ namespace bnb200 {
 namespace {
 
 constexpr int kReduceThreads = 256;
+constexpr int kMaxParts = 8;  // partial buffers the pointer-list reduction takes: one per rank of a node
 
 template <typename T> __device__ __forceinline__ void store_vec(T* dst, const float (&v)[16 / sizeof(T)]);
 template <> __device__ __forceinline__ void store_vec<float>(float* dst, const float (&v)[4]) {
@@ -36,6 +37,34 @@ template <> __device__ __forceinline__ void store_vec<__nv_bfloat16>(__nv_bfloat
     *reinterpret_cast<uint4*>(dst) =
         make_uint4(pack2<__nv_bfloat16>(v[0], v[1]), pack2<__nv_bfloat16>(v[2], v[3]),
                    pack2<__nv_bfloat16>(v[4], v[5]), pack2<__nv_bfloat16>(v[6], v[7]));
+}
+
+// The element-wise arithmetic both fp32 reductions share, so that they give the same bits: the first partial taken
+// as it is, each further one added in fp32 (round to nearest) in rank order, then the bias added in fp32 and one
+// rounding to T.
+__device__ __forceinline__ void first4(float* s, const float4 v) {
+    s[0] = v.x;
+    s[1] = v.y;
+    s[2] = v.z;
+    s[3] = v.w;
+}
+__device__ __forceinline__ void add4(float* s, const float4 v) {
+    s[0] = __fadd_rn(s[0], v.x);
+    s[1] = __fadd_rn(s[1], v.y);
+    s[2] = __fadd_rn(s[2], v.z);
+    s[3] = __fadd_rn(s[3], v.w);
+}
+template <typename T, bool VEC, int V>
+__device__ __forceinline__ void bias_round_store(float (&s)[V], const T* __restrict__ bias, T* __restrict__ out, int m,
+                                                 int n, int ldc) {
+#pragma unroll
+    for (int j = 0; j < V; ++j) s[j] = __fadd_rn(s[j], bias != nullptr ? DT<T>::to_f32(bias[n + j]) : 0.f);
+    T* dst = out + (long long)m * ldc + n;
+    if constexpr (VEC) {
+        store_vec<T>(dst, s);
+    } else {
+        dst[0] = DT<T>::from_f32(s[0]);
+    }
 }
 
 // VEC: V = 16 / sizeof(T) consecutive outputs per thread, 16-byte loads of the partials and one 16-byte store
@@ -55,35 +84,70 @@ __global__ void __launch_bounds__(kReduceThreads)
         float s[V];
         if constexpr (VEC) {
 #pragma unroll
-            for (int h = 0; h < V / 4; ++h) {
-                const float4 v = __ldcs(reinterpret_cast<const float4*>(src) + h);
-                s[4 * h] = v.x;
-                s[4 * h + 1] = v.y;
-                s[4 * h + 2] = v.z;
-                s[4 * h + 3] = v.w;
-            }
+            for (int h = 0; h < V / 4; ++h) first4(s + 4 * h, __ldcs(reinterpret_cast<const float4*>(src) + h));
             for (int r = 1; r < world; ++r) {
 #pragma unroll
-                for (int h = 0; h < V / 4; ++h) {
-                    const float4 v = __ldcs(reinterpret_cast<const float4*>(src + r * part_stride) + h);
-                    s[4 * h] = __fadd_rn(s[4 * h], v.x);
-                    s[4 * h + 1] = __fadd_rn(s[4 * h + 1], v.y);
-                    s[4 * h + 2] = __fadd_rn(s[4 * h + 2], v.z);
-                    s[4 * h + 3] = __fadd_rn(s[4 * h + 3], v.w);
-                }
+                for (int h = 0; h < V / 4; ++h)
+                    add4(s + 4 * h, __ldcs(reinterpret_cast<const float4*>(src + r * part_stride) + h));
             }
         } else {
             s[0] = src[0];
             for (int r = 1; r < world; ++r) s[0] = __fadd_rn(s[0], src[r * part_stride]);
         }
-#pragma unroll
-        for (int j = 0; j < V; ++j) s[j] = __fadd_rn(s[j], bias != nullptr ? DT<T>::to_f32(bias[n + j]) : 0.f);
-        T* dst = out + (long long)m * ldc + n;
+        bias_round_store<T, VEC>(s, bias, out, m, n, ldc);
+    }
+}
+
+// The same reduction over partials that live in separate buffers, parts.p[0 .. n_parts) in rank order (on the GPU:
+// the peers' symmetric-memory slots, read over NVLink), restricted to the rows [row0, row0 + rows) of the [M, N]
+// partials; out row m is partial row row0 + m.  Every load of an element group, one per rank, is issued before the
+// first add, so that the remote reads overlap; the adds then run in rank order as above.
+struct PartPtrs {
+    const float* p[kMaxParts];
+};
+
+template <typename T, bool VEC>
+__global__ void __launch_bounds__(kReduceThreads)
+    reduce_partials_ptrs_kernel(const PartPtrs parts, int n_parts, int row0, T* __restrict__ out,
+                                const T* __restrict__ bias, int rows, int N, int ldc) {
+    constexpr int V = VEC ? 16 / (int)sizeof(T) : 1;
+    const int per_row = N / V;
+    const long long total = (long long)rows * per_row;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+         i += (long long)gridDim.x * blockDim.x) {
+        const int m = (int)(i / per_row);
+        const int n = (int)(i - (long long)m * per_row) * V;
+        const long long off = (long long)(row0 + m) * N + n;
+        float s[V];
         if constexpr (VEC) {
-            store_vec<T>(dst, s);
+            float4 v[kMaxParts][V / 4];
+#pragma unroll
+            for (int r = 0; r < kMaxParts; ++r) {
+                if (r < n_parts) {
+#pragma unroll
+                    for (int h = 0; h < V / 4; ++h) v[r][h] = __ldcs(reinterpret_cast<const float4*>(parts.p[r] + off) + h);
+                }
+            }
+#pragma unroll
+            for (int h = 0; h < V / 4; ++h) first4(s + 4 * h, v[0][h]);
+#pragma unroll
+            for (int r = 1; r < kMaxParts; ++r) {
+                if (r < n_parts) {
+#pragma unroll
+                    for (int h = 0; h < V / 4; ++h) add4(s + 4 * h, v[r][h]);
+                }
+            }
         } else {
-            dst[0] = DT<T>::from_f32(s[0]);
+            float v[kMaxParts];
+#pragma unroll
+            for (int r = 0; r < kMaxParts; ++r)
+                if (r < n_parts) v[r] = __ldcs(parts.p[r] + off);
+            s[0] = v[0];
+#pragma unroll
+            for (int r = 1; r < kMaxParts; ++r)
+                if (r < n_parts) s[0] = __fadd_rn(s[0], v[r]);
         }
+        bias_round_store<T, VEC>(s, bias, out, m, n, ldc);
     }
 }
 
@@ -105,6 +169,25 @@ void launch_typed(const float* parts, int world, long long part_stride, T* out, 
         reduce_partials_kernel<T, false><<<grid, kReduceThreads, 0, stream>>>(parts, world, part_stride, out, bias, M,
                                                                               N, ldc);
     BNB200_CHECK_LAUNCH("reduce_partials");
+}
+
+template <typename T>
+void launch_ptrs_typed(const PartPtrs& parts, int n_parts, int row0, T* out, const T* bias, int rows, int N, int ldc,
+                       cudaStream_t stream) {
+    constexpr int V = 16 / (int)sizeof(T);
+    bool vec = N % V == 0 && ldc % V == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0;
+    for (int r = 0; r < n_parts; ++r) vec = vec && (reinterpret_cast<uintptr_t>(parts.p[r]) & 15) == 0;
+    const long long items = (long long)rows * (vec ? N / V : N);
+    const long long blocks = (items + kReduceThreads - 1) / kReduceThreads;
+    const long long cap = (long long)device_sm_count() * 8;
+    const int grid = (int)(blocks < cap ? blocks : cap);
+    if (vec)
+        reduce_partials_ptrs_kernel<T, true><<<grid, kReduceThreads, 0, stream>>>(parts, n_parts, row0, out, bias, rows,
+                                                                                  N, ldc);
+    else
+        reduce_partials_ptrs_kernel<T, false><<<grid, kReduceThreads, 0, stream>>>(parts, n_parts, row0, out, bias,
+                                                                                   rows, N, ldc);
+    BNB200_CHECK_LAUNCH("reduce_partials_ptrs");
 }
 
 // EPI 1: fp16 out, 2: bf16 out.  VEC: 8 consecutive outputs per thread, two 16-byte loads of each rank's int32 partial
@@ -228,6 +311,25 @@ bool launch_reduce_partials(const float* parts, int world, long long part_stride
                                     ldc, stream);
     else
         return false;
+    return true;
+}
+
+int max_reduce_parts() { return kMaxParts; }
+
+// The caller (c_api.cu) has checked the arguments: 1 <= n_parts <= kMaxParts, the window inside M, aligned pointers.
+bool launch_reduce_partials_ptrs(const float* const* parts, int n_parts, int row0, int rows, void* out,
+                                 const void* bias, int N, int ldc, int dtype, cudaStream_t stream) {
+    if (dtype < 0 || dtype > 3) return false;
+    if (rows <= 0 || N <= 0) return true;
+    PartPtrs p{};
+    for (int r = 0; r < n_parts; ++r) p.p[r] = parts[r];
+    if (dtype == 0 || dtype == 3)
+        launch_ptrs_typed<float>(p, n_parts, row0, (float*)out, (const float*)bias, rows, N, ldc, stream);
+    else if (dtype == 1)
+        launch_ptrs_typed<__half>(p, n_parts, row0, (__half*)out, (const __half*)bias, rows, N, ldc, stream);
+    else
+        launch_ptrs_typed<__nv_bfloat16>(p, n_parts, row0, (__nv_bfloat16*)out, (const __nv_bfloat16*)bias, rows, N,
+                                         ldc, stream);
     return true;
 }
 

@@ -74,8 +74,16 @@ input, of which the layer uses its columns) the ranks' ``grad_x_r`` are all-gath
 into the whole input gradient.  Both products run as dequantise + cuBLAS (:func:`input_grad_dequant_matmul`, chosen in
 ``_input_grad`` from the timings against the library's input-gradient kernel, ``gemm_4bit_input_grad``).  The
 tensor-parallel LLM.int8() layers below share this backward (``_ColumnInputGrad``, ``_RowInputGrad``); only the
-dequantised weight differs (``Shard4bit.dequantize``, ``Shard8bit.dequantize``).  The ``fused_forward*`` routes stay
-inference only and refuse an input that requires grad.
+dequantised weight differs (``Shard4bit.dequantize``, ``Shard8bit.dequantize``).
+
+The ``fused_forward*`` routes train when given ``grad_peers`` (:class:`PeerInputGrad`, two symmetric-memory slots): the
+forward is the route's own, through the same ``torch.autograd.Function``, and the backward is the layer's, with the
+exchange through symmetric memory instead of NCCL.  The column layer's rank r stores its fp32 partial into its own slot,
+one barrier, and each rank reduces the peers' slots in rank order (``reduce_partials_ptrs``, the arithmetic of
+``reduce_partials``): all M rows, or only its tokens' rows under sequence parallelism.  The row layer copies its
+tokens' rows of ``grad_y`` (sequence parallelism) or its columns of the input gradient (``input_is_parallel=False``)
+into every rank's slot, one barrier.  The gradients are the NCCL route's bit for bit.  Without ``grad_peers`` the fused
+routes refuse an input that requires grad, as before.
 """
 from __future__ import annotations
 
@@ -90,7 +98,7 @@ from .backends.cuda import (gemm_4bit_into, gemm_4bit_multi_out, gemm_4bit_parti
                             gemm_4bit_partial_scatter, int8_dequant_rows, int8_gemm_multi_out, int8_gemm_partial_scatter,
                             int8_outlier_operands, int8_quant_with_stats,
                             int8_reduce_partials, int8_row_stats, int8_vectorwise_quant_flags, int8_zero_columns,
-                            reduce_partials)
+                            reduce_partials, reduce_partials_ptrs)
 
 
 @dataclass
@@ -163,10 +171,18 @@ class _ColumnInputGrad:
             G = G[:, s.row0:s.row0 + s.rows]
         return _input_grad(G, s, out)
 
-    def _backward(self, grad_y: torch.Tensor, x_shape) -> torch.Tensor:
+    def _backward(self, grad_y: torch.Tensor, x_shape, peers: Optional["PeerInputGrad"] = None) -> torch.Tensor:
         s = self.shard
         world, rank = _group_world_rank(self.group)
         M = grad_y.numel() // grad_y.shape[-1]
+        if peers is not None:
+            # the partial into this rank's own slot; once every rank's is complete, each rank reduces, in rank order,
+            # the rows it owns (its tokens under sequence parallelism, all M otherwise) straight from the peers' slots
+            local, bases, handle = peers.slot()
+            self.input_grad_partial(grad_y, local)
+            handle.barrier(channel=0)  # every rank's partial is complete
+            row0, rows = (rank * (M // world), M // world) if self.sequence_parallel else (0, M)
+            return reduce_partials_ptrs(peers.scatter_ptrs(bases, 0), M, s.K, grad_y.dtype, row0, rows).view(x_shape)
         if self.sequence_parallel and world > 1:
             # the partial over all M tokens, its rows sent to the ranks that own them: chunk r of recv is rank r's
             send = torch.empty((world, M // world, s.K), device=grad_y.device)
@@ -191,35 +207,53 @@ class _RowInputGrad:
         G = grad_y.reshape(-1, s.rows)
         return _input_grad(G, s, torch.empty((G.shape[0], s.K), device=G.device, dtype=G.dtype))
 
-    def _backward(self, grad_y: torch.Tensor, x_shape) -> torch.Tensor:
-        world, _ = _group_world_rank(self.group)
+    def _backward(self, grad_y: torch.Tensor, x_shape, peers: Optional["PeerInputGrad"] = None) -> torch.Tensor:
+        world, rank = _group_world_rank(self.group)
         if self.sequence_parallel and world > 1:
             # this rank's tokens' rows of grad_y -> all M rows, in rank order (= token order)
-            full = torch.empty((world * grad_y.shape[0], *grad_y.shape[1:]), device=grad_y.device, dtype=grad_y.dtype)
-            dist.all_gather_into_tensor(full, grad_y.contiguous(), group=self.group)
+            if peers is None:
+                full = torch.empty((world * grad_y.shape[0], *grad_y.shape[1:]), device=grad_y.device,
+                                   dtype=grad_y.dtype)
+                dist.all_gather_into_tensor(full, grad_y.contiguous(), group=self.group)
+            else:  # copied into this rank's rows of every rank's slot
+                Ms, N = grad_y.numel() // grad_y.shape[-1], grad_y.shape[-1]
+                full, _, handle = peers.slot()
+                for r in range(world):
+                    handle.get_buffer(r, (Ms, N), grad_y.dtype, rank * Ms * N).copy_(grad_y.reshape(Ms, N))
+                handle.barrier(channel=0)  # every rank's rows have landed everywhere
             grad_y = full
         g = self.input_grad(grad_y)
         if not self.input_is_parallel and world > 1:
             # the layer took the whole (replicated) input and used only its columns: the input gradient is every rank's
             # columns, all-gathered in rank order (the backward of the scatter)
-            parts = torch.empty((world, *g.shape), device=g.device, dtype=g.dtype)
-            dist.all_gather_into_tensor(parts, g, group=self.group)
-            g = parts.permute(1, 0, 2).reshape(g.shape[0], world * g.shape[1])
+            if peers is None:
+                parts = torch.empty((world, *g.shape), device=g.device, dtype=g.dtype)
+                dist.all_gather_into_tensor(parts, g, group=self.group)
+                g = parts.permute(1, 0, 2).reshape(g.shape[0], world * g.shape[1])
+            else:  # copied into this rank's columns of every rank's slot
+                M, k0 = g.shape[0], self.shard.k0
+                full, _, handle = peers.slot()
+                for r in range(world):
+                    handle.get_buffer(r, (M, self.in_features), g.dtype, 0)[:, k0:k0 + g.shape[1]].copy_(g)
+                handle.barrier(channel=0)  # every rank's columns have landed everywhere
+                # a copy: the slot is rewritten two exchanges later, and autograd may keep the gradient (x.grad)
+                g = full.clone()
         return g.view(x_shape)
 
 
 class _ParallelFn(torch.autograd.Function):
-    """A tensor-parallel layer's forward (``layer._forward``), with the input gradient as its backward
-    (``layer._backward``): the shard and the bias stay frozen."""
+    """A tensor-parallel layer's forward (``layer._forward``, or the body of a fused route), with the input gradient as
+    its backward (``layer._backward``, exchanging through NCCL, or through ``peers`` for a fused route): the shard and
+    the bias stay frozen."""
 
     @staticmethod
-    def forward(ctx, x, layer):
-        ctx.layer, ctx.x_shape = layer, x.shape
-        return layer._forward(x)
+    def forward(ctx, x, layer, body=None, peers=None):
+        ctx.layer, ctx.x_shape, ctx.peers = layer, x.shape, peers
+        return layer._forward(x) if body is None else body(x)
 
     @staticmethod
     def backward(ctx, grad_y):
-        return ctx.layer._backward(grad_y, ctx.x_shape), None
+        return ctx.layer._backward(grad_y, ctx.x_shape, ctx.peers), None, None, None
 
 
 class ColumnParallelLinear4bit(_ColumnInputGrad, torch.nn.Module):
@@ -299,10 +333,39 @@ def _input_grad(G: torch.Tensor, shard, out: torch.Tensor) -> torch.Tensor:
     return out
 
 
-def _no_grad_route(x: torch.Tensor, what: str) -> None:
-    if torch.is_grad_enabled() and x.requires_grad:
-        raise RuntimeError(f"{what} is inference only and would drop the input gradient: call the layer itself to "
-                           "train, or run this under torch.no_grad()")
+def _fused_route(what: str, layer, x: torch.Tensor, body, grad_peers: Optional["PeerInputGrad"], slot,
+                 copy_out: bool = False) -> torch.Tensor:
+    """``body(x)``, a fused route's forward, as it is or, for an input that requires grad, through :class:`_ParallelFn`
+    with the layer's backward exchanging through ``grad_peers``, checked once here against ``slot()``: the (shape,
+    dtype) of the slot that backward exchanges through, (None, None) for none.  Without ``grad_peers`` such an input is
+    refused: the route would drop its gradient.
+
+    ``copy_out``: the body returns its symmetric-memory output slot, which the peers' GEMM epilogues rewrite two calls
+    later.  Inference uses the output at once; autograd may keep it until the backward (SiLU, a norm or a product save
+    their input), so a training call returns a copy."""
+    if not (torch.is_grad_enabled() and x.requires_grad):
+        return body(x)
+    if grad_peers is None:
+        raise RuntimeError(f"{what} is inference only without grad_peers and would drop the input gradient: pass "
+                           "grad_peers=PeerInputGrad(...) to train through it, call the layer itself, or run this under "
+                           "torch.no_grad()")
+    _check_peer_grad(grad_peers, layer.group, *slot())
+    return _ParallelFn.apply(x, layer, (lambda x: body(x).clone()) if copy_out else body, grad_peers)
+
+
+def _col_route(what: str, layer, x: torch.Tensor, body, grad_peers, sp: bool, copy_out: bool = False) -> torch.Tensor:
+    """A column layer's fused route: its backward reduces from fp32 ``[M, K]`` slots, M all tokens (``world`` times
+    this rank's under sequence parallelism)."""
+    def slot():
+        world = _group_world_rank(layer.group)[0] if sp else 1
+        return (world * (x.numel() // layer.shard.K), layer.shard.K), torch.float32
+    return _fused_route(what, layer, x, body, grad_peers, slot, copy_out)
+
+
+def _row_route(what: str, layer, x: torch.Tensor, body, grad_peers) -> torch.Tensor:
+    """A row layer's fused route: its backward's slot follows from the layer (:func:`_row_grad_slot`)."""
+    return _fused_route(what, layer, x, body, grad_peers, lambda: _row_grad_slot(layer, x.numel() // x.shape[-1],
+                                                                                  x.dtype))
 
 
 def sp_rows(x: torch.Tensor, world: int) -> int:
@@ -392,9 +455,70 @@ class PeerGather(_PeerSlots):
         self.M, self.N = M, N
 
 
-def fused_forward(layer: "ColumnParallelLinear4bit", x: torch.Tensor, peers: PeerGather) -> torch.Tensor:
-    """``layer(x)`` with the all-gather fused into the GEMM epilogue; returns this rank's [M, N] slot."""
-    _no_grad_route(x, "fused_forward")
+class PeerInputGrad(_PeerSlots):
+    """Two symmetric-memory ``[M, F]`` slots of ``dtype`` through which the backward of a fused route exchanges (pass it
+    as ``grad_peers``); allocate it once, outside a timed or captured step, as :class:`PeerGather`.
+
+    * column layer (``fused_forward``, ``fused_forward_col8`` and their ``_sp`` forms): fp32 ``[M, K]``, M all tokens.
+      Rank r stores its partial ``P_r = G_r . W_r`` into its own slot, one barrier, and each rank reduces the peers'
+      slots in rank order (``reduce_partials_ptrs``): all M rows, or only its own tokens' rows under sequence
+      parallelism -- a reduce-scatter by pull, with the bits of the ``all_to_all_single`` route.
+    * row layer, sequence parallel: ``[M, N]`` of the activation dtype; rank r copies its tokens' rows of ``grad_y``
+      into its rows of every rank's slot, one barrier, then ``G . W_r``.
+    * row layer, ``input_is_parallel=False``: ``[M, in_features]`` of the activation dtype; rank r copies its
+      ``grad_x_r`` into its columns ``[k0, k0 + K/w)`` of every rank's slot, one barrier.  The gradient is a copy of the
+      slot, which the peers rewrite two exchanges later.
+    * row layer, ``input_is_parallel=True`` without sequence parallelism: no exchange; only the group is checked.
+
+    Reuse: a rank writes slot i (its own, or its rows / columns of the peers') again only two exchanges later, after the
+    barrier of the exchange in between, which no peer reaches before its reads of slot i -- enqueued earlier on its
+    stream -- have completed."""
+
+    def __init__(self, M: int, F: int, dtype: torch.dtype, device, group: Optional[dist.ProcessGroup] = None):
+        super().__init__((M, F), dtype, device, group)
+        self.M, self.F = M, F
+        self.group = group
+
+
+def _check_peer_grad(peers, group, shape=None, dtype: Optional[torch.dtype] = None) -> None:
+    """``peers`` is a :class:`PeerInputGrad` of ``group`` and, when ``shape`` is given, of that slot shape and dtype."""
+    if not isinstance(peers, PeerInputGrad):
+        raise ValueError(f"grad_peers must be a PeerInputGrad, got {type(peers).__name__}")
+    world = dist.group.WORLD if dist.is_initialized() else None
+    if (peers.group if peers.group is not None else world) is not (group if group is not None else world):
+        raise ValueError("grad_peers was built for another process group than the layer's")
+    if shape is not None and ((peers.M, peers.F) != tuple(shape) or peers.dtype != dtype):
+        raise ValueError(f"PeerInputGrad was built for [{peers.M}, {peers.F}] {peers.dtype}; this backward exchanges "
+                         f"{list(shape)} {dtype}")
+
+
+def _row_grad_slot(layer, M: int, dtype: torch.dtype):
+    """(shape, dtype) of the slot the fused backward of a row layer exchanges through for M tokens, or (None, None)
+    when it exchanges nothing.  Sequence parallelism with ``input_is_parallel=False`` exchanges twice, ``[M, N]`` then
+    ``[M, in_features]``, which one PeerInputGrad serves only when the two agree."""
+    world, _ = _group_world_rank(layer.group)
+    shapes = set()
+    if layer.sequence_parallel and world > 1:
+        shapes.add((M, layer.out_features))
+    if not layer.input_is_parallel and world > 1:
+        shapes.add((M, layer.in_features))
+    if len(shapes) > 1:
+        raise ValueError("a sequence-parallel row layer with input_is_parallel=False exchanges [M, out_features] and "
+                         "[M, in_features] gradients: one PeerInputGrad serves both only when they are equal")
+    return (shapes.pop(), dtype) if shapes else (None, None)
+
+
+def fused_forward(layer: "ColumnParallelLinear4bit", x: torch.Tensor, peers: PeerGather,
+                  grad_peers: Optional[PeerInputGrad] = None) -> torch.Tensor:
+    """``layer(x)`` with the all-gather fused into the GEMM epilogue; returns this rank's [M, N] slot, valid until the
+    slot comes round again two calls later.  With ``grad_peers = PeerInputGrad(M, K, torch.float32)`` an input that
+    requires grad gets its gradient, exchanged through symmetric memory, and the call returns a copy of the slot, which
+    autograd may keep until the backward."""
+    return _col_route("fused_forward", layer, x, lambda x: _fused_forward(layer, x, peers), grad_peers, sp=False,
+                      copy_out=True)
+
+
+def _fused_forward(layer: "ColumnParallelLinear4bit", x: torch.Tensor, peers: PeerGather) -> torch.Tensor:
     s = layer.shard
     M = x.numel() // s.K
     if M != peers.M or layer.out_features != peers.N or x.dtype != peers.dtype:
@@ -549,10 +673,15 @@ class PeerPartials(_PeerSlots):
         self.M, self.N = M, N
 
 
-def fused_forward_row(layer: RowParallelLinear4bit, x: torch.Tensor, peers: PeerPartials) -> torch.Tensor:
+def fused_forward_row(layer: RowParallelLinear4bit, x: torch.Tensor, peers: PeerPartials,
+                      grad_peers: Optional[PeerInputGrad] = None) -> torch.Tensor:
     """``layer(x)`` with the exchange of the partials fused into the GEMM epilogue: ``P_r`` is stored into slot r of
-    every rank's buffer, one barrier publishes them, and each rank reduces them in rank order."""
-    _no_grad_route(x, "fused_forward_row")
+    every rank's buffer, one barrier publishes them, and each rank reduces them in rank order.  With ``grad_peers``
+    an input that requires grad gets its gradient, exchanged through symmetric memory."""
+    return _row_route("fused_forward_row", layer, x, lambda x: _fused_forward_row(layer, x, peers), grad_peers)
+
+
+def _fused_forward_row(layer: RowParallelLinear4bit, x: torch.Tensor, peers: PeerPartials) -> torch.Tensor:
     s = layer.shard
     x_r = layer.local_input(x)
     M = x_r.numel() // s.K
@@ -565,11 +694,17 @@ def fused_forward_row(layer: RowParallelLinear4bit, x: torch.Tensor, peers: Peer
     return reduce_partials(local, x.dtype, layer.bias).view(*x_r.shape[:-1], s.rows)
 
 
-def fused_forward_row_sp(layer: RowParallelLinear4bit, x: torch.Tensor, peers: PeerPartials) -> torch.Tensor:
+def fused_forward_row_sp(layer: RowParallelLinear4bit, x: torch.Tensor, peers: PeerPartials,
+                         grad_peers: Optional[PeerInputGrad] = None) -> torch.Tensor:
     """The sequence-parallel ``layer(x)`` (this rank's tokens only) with the reduce-scatter fused into the GEMM
     epilogue: the rows of ``P_r`` that belong to rank s are stored into slot r of rank s's ``[world, M/world, N]``
-    buffer (``peers = PeerPartials(M // world, N)``), one barrier publishes them, and each rank reduces its own."""
-    _no_grad_route(x, "fused_forward_row_sp")
+    buffer (``peers = PeerPartials(M // world, N)``), one barrier publishes them, and each rank reduces its own.  With
+    ``grad_peers = PeerInputGrad(M, N, x.dtype)`` an input that requires grad gets its gradient: the token rows of
+    ``grad_y`` gathered through symmetric memory."""
+    return _row_route("fused_forward_row_sp", layer, x, lambda x: _fused_forward_row_sp(layer, x, peers), grad_peers)
+
+
+def _fused_forward_row_sp(layer: RowParallelLinear4bit, x: torch.Tensor, peers: PeerPartials) -> torch.Tensor:
     s = layer.shard
     x_r = layer.local_input(x)
     Ms = sp_rows(x_r, peers.world)
@@ -582,11 +717,18 @@ def fused_forward_row_sp(layer: RowParallelLinear4bit, x: torch.Tensor, peers: P
     return reduce_partials(local, x.dtype, layer.bias).view(x_r.shape[0] // peers.world, *x_r.shape[1:-1], s.rows)
 
 
-def fused_forward_col_sp(layer: ColumnParallelLinear4bit, x: torch.Tensor, peers: PeerGather) -> torch.Tensor:
+def fused_forward_col_sp(layer: ColumnParallelLinear4bit, x: torch.Tensor, peers: PeerGather,
+                         grad_peers: Optional[PeerInputGrad] = None) -> torch.Tensor:
     """The sequence-parallel ``layer(x)`` with the token all-gather through symmetric memory: this rank copies its
     ``[M/world, ..., K]`` tokens into its rows of every rank's ``[M, K]`` buffer (``peers = PeerGather(M, K, dtype)``),
-    one barrier publishes them, and the local GEMM reads the gathered tokens.  Returns ``[M, ..., N/world]``."""
-    _no_grad_route(x, "fused_forward_col_sp")
+    one barrier publishes them, and the local GEMM reads the gathered tokens.  Returns ``[M, ..., N/world]``.  With
+    ``grad_peers = PeerInputGrad(M, K, torch.float32)`` an input that requires grad gets the gradient of its tokens,
+    reduced from the peers' partials."""
+    return _col_route("fused_forward_col_sp", layer, x, lambda x: _fused_forward_col_sp(layer, x, peers), grad_peers,
+                      sp=True)
+
+
+def _fused_forward_col_sp(layer: ColumnParallelLinear4bit, x: torch.Tensor, peers: PeerGather) -> torch.Tensor:
     s = layer.shard
     world, rank = peers.world, peers.rank
     Ms = x.numel() // s.K
@@ -901,11 +1043,18 @@ class ColumnParallelLinear8bitLt(_ColumnInputGrad, torch.nn.Module):
         return full.reshape(*lead, full.shape[-1])
 
 
-def fused_forward_col8(layer: ColumnParallelLinear8bitLt, x: torch.Tensor, peers: PeerGather) -> torch.Tensor:
+def fused_forward_col8(layer: ColumnParallelLinear8bitLt, x: torch.Tensor, peers: PeerGather,
+                      grad_peers: Optional[PeerInputGrad] = None) -> torch.Tensor:
     """``layer(x)`` with the all-gather fused into the int8 GEMM epilogue: each output element is stored into this
     rank's columns of every rank's symmetric ``[M, N]`` buffer.  Past 64 outlier columns, or for a shape the GEMM does
-    not take, the local GEMM + NCCL route fills the same slot.  Returns this rank's [M, N] slot."""
-    _no_grad_route(x, "fused_forward_col8")
+    not take, the local GEMM + NCCL route fills the same slot.  Returns this rank's [M, N] slot.  With ``grad_peers =
+    PeerInputGrad(M, K, torch.float32)`` an input that requires grad gets its gradient (the outlier decomposition
+    leaves it alone, as in the layer's own backward), and the call returns a copy of the slot, as ``fused_forward``."""
+    return _col_route("fused_forward_col8", layer, x, lambda x: _fused_forward_col8(layer, x, peers), grad_peers,
+                      sp=False, copy_out=True)
+
+
+def _fused_forward_col8(layer: ColumnParallelLinear8bitLt, x: torch.Tensor, peers: PeerGather) -> torch.Tensor:
     s = layer.shard
     q = layer.quantize(x)
     M = q.A.shape[0]
@@ -944,14 +1093,17 @@ class PeerInt8Input(_PeerSlots):
         return local[self.M * self.K:].view(torch.float32)
 
 
-def fused_forward_col8_sp(layer: ColumnParallelLinear8bitLt, x: torch.Tensor, peers: PeerInt8Input) -> torch.Tensor:
+def fused_forward_col8_sp(layer: ColumnParallelLinear8bitLt, x: torch.Tensor, peers: PeerInt8Input,
+                          grad_peers: Optional[PeerInputGrad] = None) -> torch.Tensor:
     """The sequence-parallel ``layer(x)`` with the gather of the quantised tokens through symmetric memory: this rank
     quantises its ``[M/w, ..., K]`` tokens and copies the codes and row statistics into its rows of every rank's slot
     (``peers = PeerInt8Input(M, K)``), one barrier publishes them, and the local GEMM reads the gathered codes.  Returns
-    ``[M, ..., N/w]``."""
-    _no_grad_route(x, "fused_forward_col8_sp")
+    ``[M, ..., N/w]``.  With ``grad_peers = PeerInputGrad(M, K, torch.float32)`` an input that requires grad gets the
+    gradient of its tokens, reduced from the peers' partials."""
     world, _ = _group_world_rank(layer.group)
-    return layer._output(layer.sp_quantize(x, peers), (world * x.shape[0], *x.shape[1:-1]))
+    return _col_route("fused_forward_col8_sp", layer, x,
+                      lambda x: layer._output(layer.sp_quantize(x, peers), (world * x.shape[0], *x.shape[1:-1])),
+                      grad_peers, sp=True)
 
 
 @dataclass
@@ -1172,11 +1324,16 @@ class RowParallelLinear8bitLt(_RowInputGrad, torch.nn.Module):
         return self.reduce(parts, SCA[mine], x.dtype, None if subA is None else subA[mine], subBT).view(lead)
 
 
-def fused_forward_row8(layer: RowParallelLinear8bitLt, x: torch.Tensor, peers: PeerPartials) -> torch.Tensor:
+def fused_forward_row8(layer: RowParallelLinear8bitLt, x: torch.Tensor, peers: PeerPartials,
+                      grad_peers: Optional[PeerInputGrad] = None) -> torch.Tensor:
     """``layer(x)`` with the exchange of the int32 partials fused into the GEMM epilogue: ``P_r`` is stored into slot r
     of every rank's symmetric buffer, one barrier publishes them, and each rank reduces its own buffer.  The row
-    statistics (a max) and the outlier operands still travel through NCCL."""
-    _no_grad_route(x, "fused_forward_row8")
+    statistics (a max) and the outlier operands still travel through NCCL.  With ``grad_peers`` an input that requires
+    grad gets its gradient, exchanged through symmetric memory."""
+    return _row_route("fused_forward_row8", layer, x, lambda x: _fused_forward_row8(layer, x, peers), grad_peers)
+
+
+def _fused_forward_row8(layer: RowParallelLinear8bitLt, x: torch.Tensor, peers: PeerPartials) -> torch.Tensor:
     s = layer.shard
     x_r, _, SCA, CA, cols = layer._prologue(x)
     M = x_r.shape[0]
@@ -1190,11 +1347,13 @@ def fused_forward_row8(layer: RowParallelLinear8bitLt, x: torch.Tensor, peers: P
     return layer.reduce(local, SCA, x.dtype, subA, subBT).view(*x.shape[:-1], s.rows)
 
 
-def fused_forward_row8_sp(layer: RowParallelLinear8bitLt, x: torch.Tensor, peers: PeerPartials) -> torch.Tensor:
+def fused_forward_row8_sp(layer: RowParallelLinear8bitLt, x: torch.Tensor, peers: PeerPartials,
+                         grad_peers: Optional[PeerInputGrad] = None) -> torch.Tensor:
     """The sequence-parallel ``layer(x)`` (this rank's tokens only) with the exchange of the int32 partials fused into
     the GEMM epilogue: the rows of ``P_r`` that belong to rank s are stored into slot r of rank s's ``[world, M/world,
     N]`` buffer (``peers = PeerPartials(M // world, N, dtype=torch.int32)``), one barrier publishes them, and each rank
     reduces its own with its rows of the statistics and outlier operands.  Past 64 outlier columns the slow path of the
-    NCCL route runs instead (:meth:`RowParallelLinear8bitLt._sp_forward`)."""
-    _no_grad_route(x, "fused_forward_row8_sp")
-    return layer._sp_forward(x, peers)
+    NCCL route runs instead (:meth:`RowParallelLinear8bitLt._sp_forward`).  With ``grad_peers = PeerInputGrad(M, N,
+    x.dtype)`` an input that requires grad gets its gradient: the token rows of ``grad_y`` gathered through symmetric
+    memory."""
+    return _row_route("fused_forward_row8_sp", layer, x, lambda x: layer._sp_forward(x, peers), grad_peers)

@@ -182,6 +182,13 @@ int cbnb_b200_gemm_4bit_input_grad_panel(const void* G, int ldg, const uint8_t* 
  * serve. */
 int cbnb_b200_reduce_partials(const float* parts, int world, long long part_stride, void* out, const void* bias, int M, int N, int ldc, int dtype, bnb_stream_t stream);
 
+/* cbnb_b200_reduce_partials over n_parts (1..8) separate [M, N] fp32 partials, parts[r] in rank order (a rank's own
+ * buffer or a peer's symmetric-memory mapping), restricted to the rows [row0, row0 + rows): out[m, n] (row stride ldc,
+ * m < rows) = T( (((P_0 + P_1) + ...) + P_{n_parts-1})[row0 + m, n] + bias[n] ), the same bits as
+ * cbnb_b200_reduce_partials.  Returns 0, 1 with the error message set for bad arguments (n_parts outside 1..8, a null
+ * or misaligned pointer, a window past M, ldc < N), or 100 for a dtype it does not serve. */
+int cbnb_b200_reduce_partials_ptrs(const float* const* parts, int n_parts, int row0, int rows, void* out, const void* bias, int M, int N, int ldc, int dtype, bnb_stream_t stream);
+
 /* Which kernel a (M, N, K, blocksize, dtype) 4-bit GEMM takes: 0 = CUDA-core GEMV,
  * 1 = wgmma GEMM, 2 = generic CUDA-core kernel, 3 = mma.sync decode kernel (M <= 8).
  * dtype for the 4-bit GEMM entries below: 0 = fp32, 1 = fp16, 2 = bf16, 3 = fp32 with TF32 allowed -- the
