@@ -1283,3 +1283,93 @@ def optimizer_update_8bit_blockwise_multi(optimizer_name, g, p, state1, state2, 
         _launch_list(what, fn, optimizer_name, g0, descs,
                      (float(beta1), float(beta2), float(beta3), float(alpha), float(eps), float(weight_decay), *scalars,
                       qmap1.data_ptr(), qmap2.data_ptr() if two else None, float(gnorm_scale), bool(skip_zeros)))
+
+
+# ---- data-parallel steps: one rank's pieces of flat gradient / parameter buffers, gradients summed over the ranks
+_OPTIMIZER_PEERS = tuple(name for name in _OPTIMIZER_ID if name != "ademamix")
+_peers_capacity = None
+
+
+def optimizer_peers_capacity() -> int:
+    """Pieces per data-parallel launch: the descriptor list shares the kernel parameters with the peer addresses."""
+    global _peers_capacity
+    if _peers_capacity is None:
+        _peers_capacity = int(lib.cbnb_b200_optimizer_peers_capacity())
+    return _peers_capacity
+
+
+def _peer_args(what, g, p, step, grad_srcs, param_dsts, grad_local, param_local):
+    """Check the peer arguments: 1..8 sources and destinations (addresses), the local flat buffers holding every piece
+    (g[i] inside grad_local, p[i] inside param_local) and host steps.  Returns the two address arrays."""
+    srcs, dsts = [int(a) for a in grad_srcs], [int(a) for a in param_dsts]
+    if not 1 <= len(srcs) <= 8 or not 1 <= len(dsts) <= 8:
+        raise ValueError(f"{what}: {len(srcs)} gradient sources and {len(dsts)} parameter destinations (1..8 each)")
+    if any(a == 0 for a in srcs + dsts):
+        raise ValueError(f"{what}: a null gradient source or parameter destination")
+    for name, flat in (("grad_local", grad_local), ("param_local", param_local)):
+        if (not isinstance(flat, torch.Tensor) or not flat.is_contiguous() or flat.dtype != grad_local.dtype
+                or flat.numel() != grad_local.numel() or flat.device != grad_local.device):
+            raise ValueError(f"{what}: {name} must be a contiguous flat buffer like grad_local")
+    es = grad_local.element_size()
+    for i, (gi, pi) in enumerate(zip(g, p)):
+        for t, flat in ((gi, grad_local), (pi, param_local)):
+            off = t.data_ptr() - flat.data_ptr()
+            if t.dtype != flat.dtype or off < 0 or off % es or off // es + t.numel() > flat.numel():
+                raise ValueError(f"{what}: piece {i} is not a {flat.dtype} view inside the local flat buffers")
+    if any(isinstance(s, torch.Tensor) for s in step):
+        raise ValueError(f"{what}: the data-parallel step takes host steps (no capturable form)")
+    return (ct.c_void_p * len(srcs))(*srcs), (ct.c_void_p * len(dsts))(*dsts)
+
+
+def _launch_peers(what, fn, optimizer_name, g0, descs, srcs, dsts, grad_local, param_local, grad_scale, scalars):
+    """fn(optimizer, dtype, tensors, count, srcs, world, dsts, ndst, grad_local, param_local, numel, grad_scale,
+    *scalars, stream) once per capacity chunk of descs."""
+    cap, k, size = optimizer_peers_capacity(), len(descs), ct.sizeof(cext.OptimTensor)
+    for lo in range(0, k, cap):
+        rc = fn(_OPTIMIZER_ID[optimizer_name], _DTYPE_ID[g0.dtype], ct.addressof(descs) + lo * size, min(cap, k - lo),
+                ct.cast(srcs, ct.c_void_p), len(srcs), ct.cast(dsts, ct.c_void_p), len(dsts), grad_local.data_ptr(),
+                param_local.data_ptr(), grad_local.numel(), float(grad_scale), *scalars, _stream(g0))
+        lib.check(what)
+        if rc != 0:
+            raise RuntimeError(f"{what}: native call returned {rc}")
+
+
+def optimizer_update_32bit_multi_peers(optimizer_name, g, p, state1, state2, beta1, beta2, beta3, alpha, eps,
+                                       weight_decay, step, lr, grad_srcs, param_dsts, grad_local, param_local,
+                                       grad_scale, skip_zeros=False):
+    """optimizer_update_32bit_multi for one data-parallel rank: g and p list pieces of the local flat buffers grad_local
+    and param_local; the gradient of each element is the fp32 sum, in rank order, of the buffers at the addresses
+    grad_srcs (each laid out as grad_local) times grad_scale, rounded once to the dtype; the new parameters go to each
+    address of param_dsts (laid out as param_local), not to p unless param_local is among them."""
+    what = "optimizer_update_32bit_multi_peers"
+    g0, descs, _ = _optimizer_list(what, optimizer_name, _OPTIMIZER_PEERS, g, p, state1, state2, None, None, step, False)
+    if descs is None:
+        return
+    srcs, dsts = _peer_args(what, g, p, step, grad_srcs, param_dsts, grad_local, param_local)
+    with _on_device(g0):
+        _launch_peers(what, lib.cbnb_b200_optimizer_update_32bit_multi_peers, optimizer_name, g0, descs, srcs, dsts,
+                      grad_local, param_local, grad_scale,
+                      (float(beta1), float(beta2), float(beta3), float(alpha), float(eps), float(weight_decay),
+                       float(lr), bool(skip_zeros)))
+
+
+def optimizer_update_8bit_blockwise_multi_peers(optimizer_name, g, p, state1, state2, beta1, beta2, beta3, alpha, eps,
+                                                step, lr, qmap1, qmap2, absmax1, absmax2, weight_decay, grad_srcs,
+                                                param_dsts, grad_local, param_local, grad_scale, skip_zeros=False):
+    """optimizer_update_8bit_blockwise_multi for one data-parallel rank; the gradient and parameter exchange as
+    optimizer_update_32bit_multi_peers.  Every piece starts on a 256-element block of its tensor."""
+    what = "optimizer_update_8bit_blockwise_multi_peers"
+    g0, descs, _ = _optimizer_list(what, optimizer_name, [n for n in _OPTIMIZER_8BIT if n in _OPTIMIZER_PEERS], g, p,
+                                   state1, state2, absmax1, absmax2, step, True)
+    if descs is None:
+        return
+    srcs, dsts = _peer_args(what, g, p, step, grad_srcs, param_dsts, grad_local, param_local)
+    two = optimizer_name == "adam"
+    for q in (qmap1, qmap2) if two else (qmap1,):
+        if q is None or q.device != g0.device or not q.is_contiguous() or q.dtype != torch.float32 or q.numel() < 256:
+            raise ValueError(f"{what}: the code books must be contiguous fp32 [256] tensors on {g0.device}")
+    with _on_device(g0):
+        _launch_peers(what, lib.cbnb_b200_optimizer_update_8bit_blockwise_multi_peers, optimizer_name, g0, descs, srcs,
+                      dsts, grad_local, param_local, grad_scale,
+                      (float(beta1), float(beta2), float(beta3), float(alpha), float(eps), float(weight_decay),
+                       float(lr), qmap1.data_ptr(), qmap2.data_ptr() if two else None, bool(skip_zeros)))

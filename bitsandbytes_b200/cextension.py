@@ -161,6 +161,12 @@ def _signatures():
                                                           _VOIDP], _I32)
     sig["cbnb_b200_optimizer_update_8bit_blockwise_multi_dev"] = ([_I32, _I32, _VOIDP, _I32] + [_F] * 7 + [_VOIDP] * 3
                                                                    + [_F, ct.c_bool, _VOIDP], _I32)
+    # the data-parallel forms: (optimizer, dtype, tensors, count, grad_srcs, world, param_dsts, ndst, grad_local,
+    #  param_local, numel, grad_scale, beta1 .. lr, [q1, q2,] skip_zeros, stream) -> int
+    sig["cbnb_b200_optimizer_peers_capacity"] = ([], _I32)
+    peers = [_I32, _I32, _VOIDP, _I32, _VOIDP, _I32, _VOIDP, _I32, _VOIDP, _VOIDP, ct.c_longlong] + [_F] * 8
+    sig["cbnb_b200_optimizer_update_32bit_multi_peers"] = (peers + [ct.c_bool, _VOIDP], _I32)
+    sig["cbnb_b200_optimizer_update_8bit_blockwise_multi_peers"] = (peers + [_VOIDP, _VOIDP, ct.c_bool, _VOIDP], _I32)
     return sig
 
 

@@ -46,6 +46,19 @@ bool launch_optimizer8bit_blockwise_list_dev(int opt, int dtype, const OptimTens
                                              float beta2, float beta3, float alpha, float eps, float wd, float lr,
                                              const float* lr_dev, const float* q1, const float* q2, float gnorm_scale,
                                              bool skip_zeros, cudaStream_t st);
+int optimizer_peers_capacity();
+int optimizer_max_peers();
+bool launch_optimizer32bit_list_peers(int opt, int dtype, const OptimTensor* ts, int count,
+                                      const void* const* grad_srcs, int world, void* const* param_dsts, int ndst,
+                                      const void* grad_local, const void* param_local, float grad_scale, float beta1,
+                                      float beta2, float beta3, float alpha, float eps, float wd, float lr,
+                                      bool skip_zeros, cudaStream_t st);
+bool launch_optimizer8bit_blockwise_list_peers(int opt, int dtype, const OptimTensor* ts, int count,
+                                               const void* const* grad_srcs, int world, void* const* param_dsts,
+                                               int ndst, const void* grad_local, const void* param_local,
+                                               float grad_scale, float beta1, float beta2, float beta3, float alpha,
+                                               float eps, float wd, float lr, const float* q1, const float* q2,
+                                               bool skip_zeros, cudaStream_t st);
 
 // PART = true: the partial instances (fp32 accumulators to every destination of an OutList<float>, no bias, no
 // rounding)
@@ -1046,6 +1059,100 @@ int cbnb_b200_optimizer_update_8bit_blockwise_multi_dev(int optimizer, int dtype
     launch_optimizer8bit_blockwise_list_dev(optimizer, dtype, tensors, count, beta1, beta2, beta3, alpha, eps,
                                             weight_decay, lr, lr_dev, quantiles1, quantiles2, gnorm_scale, skip_zeros,
                                             stream);
+    return 0;
+}
+
+// Data-parallel steps of one rank's pieces of flat buffers (optim/sharded.py): the _multi entries with the gradient
+// summed over `world` source buffers in rank order and the new parameters written to `ndst` destination buffers.  Every
+// descriptor's g and p must lie inside the local flat buffers [grad_local, + numel) and [param_local, + numel).
+int cbnb_b200_optimizer_peers_capacity(void) { return optimizer_peers_capacity(); }
+
+static bool optimizer_peers_ok(const char* what, int optimizer, const OptimTensor* tensors, int count, int dtype,
+                               const void* const* grad_srcs, int world, void* const* param_dsts, int ndst,
+                               const void* grad_local, const void* param_local, long long numel) {
+    char msg[200];
+    msg[0] = 0;
+    const uintptr_t es = dtype == 0 ? 4 : 2;
+    auto misaligned = [es](const void* v) { return v == nullptr || (reinterpret_cast<uintptr_t>(v) % es) != 0; };
+    if (optimizer == 5)
+        snprintf(msg, sizeof(msg), "%s: AdEMAMix has no data-parallel step", what);
+    else if (world < 1 || world > optimizer_max_peers() || ndst < 1 || ndst > optimizer_max_peers() ||
+             grad_srcs == nullptr || param_dsts == nullptr)
+        snprintf(msg, sizeof(msg), "%s: %d gradient sources and %d parameter destinations (1..%d each)", what, world,
+                 ndst, optimizer_max_peers());
+    else if (misaligned(grad_local) || misaligned(param_local) || numel < 0)
+        snprintf(msg, sizeof(msg), "%s: the local flat buffers must be non-null and aligned to their element", what);
+    for (int r = 0; !msg[0] && r < world; ++r)
+        if (misaligned(grad_srcs[r]))
+            snprintf(msg, sizeof(msg), "%s: gradient source %d is null or not aligned to its element", what, r);
+    for (int r = 0; !msg[0] && r < ndst; ++r)
+        if (misaligned(param_dsts[r]))
+            snprintf(msg, sizeof(msg), "%s: parameter destination %d is null or not aligned to its element", what, r);
+    for (int i = 0; !msg[0] && i < count; ++i) {
+        const long long go = static_cast<const char*>(tensors[i].g) - static_cast<const char*>(grad_local);
+        const long long po = static_cast<const char*>(tensors[i].p) - static_cast<const char*>(param_local);
+        const long long bytes = tensors[i].n * (long long)es, end = numel * (long long)es;
+        if (tensors[i].n < 0 || go < 0 || po < 0 || go % (long long)es || po % (long long)es || go + bytes > end ||
+            po + bytes > end)
+            snprintf(msg, sizeof(msg), "%s: tensor %d lies outside the local flat buffers of %lld elements", what, i,
+                     numel);
+    }
+    if (!msg[0]) return true;
+    set_last_error_msg(msg);
+    return false;
+}
+
+int cbnb_b200_optimizer_update_32bit_multi_peers(int optimizer, int dtype, const OptimTensor* tensors, int count,
+                                                 const void* const* grad_srcs, int world, void* const* param_dsts,
+                                                 int ndst, const void* grad_local, const void* param_local,
+                                                 long long numel, float grad_scale, float beta1, float beta2,
+                                                 float beta3, float alpha, float eps, float weight_decay, float lr,
+                                                 bool skip_zeros, cudaStream_t stream) {
+    const char* what = "optimizer_update_32bit_multi_peers";
+    if (count < 0 || count > optimizer_peers_capacity() || (count > 0 && tensors == nullptr) || optimizer < 0 ||
+        optimizer > 5 || dtype < 0 || dtype > 2) {
+        char msg[160];
+        snprintf(msg, sizeof(msg), "%s: %d tensors (at most %d per call), optimizer id %d, dtype id %d", what, count,
+                 optimizer_peers_capacity(), optimizer, dtype);
+        set_last_error_msg(msg);
+        return 100;
+    }
+    if (!optimizer_peers_ok(what, optimizer, tensors, count, dtype, grad_srcs, world, param_dsts, ndst, grad_local,
+                            param_local, numel))
+        return 1;
+    launch_optimizer32bit_list_peers(optimizer, dtype, tensors, count, grad_srcs, world, param_dsts, ndst, grad_local,
+                                     param_local, grad_scale, beta1, beta2, beta3, alpha, eps, weight_decay, lr,
+                                     skip_zeros, stream);
+    return 0;
+}
+
+int cbnb_b200_optimizer_update_8bit_blockwise_multi_peers(int optimizer, int dtype, const OptimTensor* tensors,
+                                                          int count, const void* const* grad_srcs, int world,
+                                                          void* const* param_dsts, int ndst, const void* grad_local,
+                                                          const void* param_local, long long numel, float grad_scale,
+                                                          float beta1, float beta2, float beta3, float alpha, float eps,
+                                                          float weight_decay, float lr, const float* quantiles1,
+                                                          const float* quantiles2, bool skip_zeros,
+                                                          cudaStream_t stream) {
+    const char* what = "optimizer_update_8bit_blockwise_multi_peers";
+    if (count < 0 || count > optimizer_peers_capacity() || (count > 0 && tensors == nullptr) || optimizer < 0 ||
+        optimizer > 5 || dtype < 0 || dtype > 2) {
+        char msg[160];
+        snprintf(msg, sizeof(msg), "%s: %d tensors (at most %d per call), optimizer id %d, dtype id %d", what, count,
+                 optimizer_peers_capacity(), optimizer, dtype);
+        set_last_error_msg(msg);
+        return 100;
+    }
+    if (!optimizer_peers_ok(what, optimizer, tensors, count, dtype, grad_srcs, world, param_dsts, ndst, grad_local,
+                            param_local, numel))
+        return 1;
+    if (quantiles1 == nullptr || (optimizer == 0 && quantiles2 == nullptr)) {
+        set_last_error_msg("optimizer_update_8bit_blockwise_multi_peers: missing code book");
+        return 1;
+    }
+    launch_optimizer8bit_blockwise_list_peers(optimizer, dtype, tensors, count, grad_srcs, world, param_dsts, ndst,
+                                              grad_local, param_local, grad_scale, beta1, beta2, beta3, alpha, eps,
+                                              weight_decay, lr, quantiles1, quantiles2, skip_zeros, stream);
     return 0;
 }
 

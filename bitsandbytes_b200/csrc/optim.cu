@@ -28,6 +28,7 @@
 #include "q8_search.cuh"
 
 #include <cfloat>
+#include <type_traits>
 
 namespace bnb200 {
 
@@ -69,6 +70,37 @@ struct OptimList {
 };
 static_assert(sizeof(OptimList) + kScalarParamBytes <= kKernelParamBytes, "kernel parameters exceed 32764 bytes");
 
+// Peer instances (PEERS = NP > 0, the _peers entries): the step of one data-parallel rank whose tensors are pieces of a
+// flat buffer that every rank holds a copy of (ZeRO stage 1, optim/sharded.py).  Each descriptor keeps the rank's own
+// pieces: p and g in the local flat parameter and gradient buffers, the piece's state.  The gradient of an element is
+// T(fp32(((g_0 + g_1) + ...) + g_{w-1}) * grad_scale), read at the same byte offset from the local gradient base in each
+// of the w source buffers, summed in rank order and rounded once; the new parameter goes to the same offset from the
+// local parameter base in each of the ndst destinations (the local buffer among them).  The rest of the update is the
+// PEERS = 0 arithmetic on that gradient.  The descriptor list is shorter by the peer arguments.  NP, the compiled
+// bound on the number of sources (1, 2, 4 or 8; the launch takes the least that holds w), sizes the registers that hold
+// the w loads in flight, so a launch over few ranks keeps the occupancy of the PEERS = 0 instances.
+constexpr int kMaxPeers = 8;
+struct PeerArgs {
+    const void* g[kMaxPeers];  // gradient source bases, rank order (w of them)
+    void* p[kMaxPeers];        // parameter destination bases (ndst of them)
+    const char* g_local;       // the local flat gradient: a descriptor's g lies at g_local + offset
+    const char* p_local;       // the local flat parameters
+    float grad_scale;
+    int w, ndst;
+};
+constexpr int kPeerListCap =
+    (kKernelParamBytes - kScalarParamBytes - 16 - (int)sizeof(PeerArgs)) / (sizeof(OptimTensor) + sizeof(long long));
+
+struct PeerOptimList {
+    long long start[kPeerListCap + 1];
+    OptimTensor t[kPeerListCap];
+    int count;
+    PeerArgs peers;
+};
+static_assert(sizeof(PeerOptimList) + kScalarParamBytes <= kKernelParamBytes, "kernel parameters exceed 32764 bytes");
+
+template <int PEERS> using ListOf = std::conditional_t<(PEERS > 0), PeerOptimList, OptimList>;
+
 // the per-launch scalars
 struct OptimScalars {
     float beta1, beta2, beta3, alpha, eps, weight_decay, lr, gnorm_scale;
@@ -91,7 +123,8 @@ __global__ void __launch_bounds__(256) optim_step_increment_kernel(const __grid_
 }
 
 // the tensor of work item `item`: the last i >= lo with start[i] <= item (tensors without items are skipped)
-__device__ __forceinline__ int find_tensor(const OptimList& L, long long item, int lo) {
+template <typename L_>
+__device__ __forceinline__ int find_tensor(const L_& L, long long item, int lo) {
     int hi = L.count - 1;
     while (lo < hi) {
         const int mid = (lo + hi + 1) >> 1;
@@ -101,6 +134,94 @@ __device__ __forceinline__ int find_tensor(const OptimList& L, long long item, i
             hi = mid - 1;
     }
     return lo;
+}
+
+// fp32 add and multiply in IEEE round-to-nearest with subnormals kept and no contraction into an fma: this file is
+// compiled with --use_fast_math (flush to zero), and the peers' gradient sum must be the one a plain fp32 sum gives
+__device__ __forceinline__ float add_rn(float a, float b) {
+    float r;
+    asm("add.rn.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+    return r;
+}
+__device__ __forceinline__ float mul_rn(float a, float b) {
+    float r;
+    asm("mul.rn.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+    return r;
+}
+
+// K consecutive elements i .. i + K - 1 of src: one or two 16-byte accesses, or one 8-byte access, when `vec` (all K in
+// range, src + i aligned); otherwise element by element, 0 past n
+template <typename T, int K>
+__device__ __forceinline__ void load_k(const T* src, long i, long n, bool vec, T (&v)[K]) {
+    constexpr int B = K * (int)sizeof(T);
+    if constexpr (B % 16 == 0) {
+        if (vec) {
+#pragma unroll
+            for (int c = 0; c < B / 16; ++c) reinterpret_cast<uint4*>(v)[c] = reinterpret_cast<const uint4*>(src + i)[c];
+            return;
+        }
+    } else if constexpr (B == 8) {
+        if (vec) {
+            *reinterpret_cast<uint2*>(v) = *reinterpret_cast<const uint2*>(src + i);
+            return;
+        }
+    }
+#pragma unroll
+    for (int j = 0; j < K; ++j) v[j] = (i + j < n) ? src[i + j] : round_to<T>(0.0f);
+}
+template <typename T, int K>
+__device__ __forceinline__ void store_k(T* dst, long i, long n, bool vec, const T (&v)[K]) {
+    constexpr int B = K * (int)sizeof(T);
+    if constexpr (B % 16 == 0) {
+        if (vec) {
+#pragma unroll
+            for (int c = 0; c < B / 16; ++c) reinterpret_cast<uint4*>(dst + i)[c] = reinterpret_cast<const uint4*>(v)[c];
+            return;
+        }
+    } else if constexpr (B == 8) {
+        if (vec) {
+            *reinterpret_cast<uint2*>(dst + i) = *reinterpret_cast<const uint2*>(v);
+            return;
+        }
+    }
+#pragma unroll
+    for (int j = 0; j < K; ++j)
+        if (i + j < n) dst[i + j] = v[j];
+}
+
+// Elements i .. i + K - 1 of a piece's gradient, the piece `goff` bytes from the local gradient base: the w <= NP
+// sources' values are all loaded before the rank-order fp32 sum, scaled by grad_scale and rounded once to T
+template <typename T, int K, int NP>
+__device__ __forceinline__ void peer_grad(const PeerArgs& P, long goff, long i, long n, bool vec, T (&v)[K]) {
+    alignas(K * sizeof(T) < 16 ? K * sizeof(T) : 16) T x[NP][K];
+#pragma unroll
+    for (int r = 0; r < NP; ++r)
+        if (r < P.w) load_k<T, K>(reinterpret_cast<const T*>(static_cast<const char*>(P.g[r]) + goff), i, n, vec, x[r]);
+#pragma unroll
+    for (int j = 0; j < K; ++j) {
+        float acc = widen<T>(x[0][j]);
+#pragma unroll
+        for (int r = 1; r < NP; ++r)
+            if (r < P.w) acc = add_rn(acc, widen<T>(x[r][j]));
+        v[j] = round_to<T>(mul_rn(acc, P.grad_scale));
+    }
+}
+
+// the new parameter values of elements i .. i + K - 1 of a piece `poff` bytes from the local parameter base, to every
+// destination
+template <typename T, int K>
+__device__ __forceinline__ void peer_store(const PeerArgs& P, long poff, long i, long n, bool vec, const T (&v)[K]) {
+#pragma unroll
+    for (int r = 0; r < kMaxPeers; ++r)
+        if (r < P.ndst) store_k<T, K>(reinterpret_cast<T*>(static_cast<char*>(P.p[r]) + poff), i, n, vec, v);
+}
+
+// every base 16-byte aligned: then a piece's vector accesses are aligned in every buffer when they are in the local one
+__device__ __forceinline__ bool peers_aligned(const PeerArgs& P) {
+    uintptr_t bits = reinterpret_cast<uintptr_t>(P.g_local) | reinterpret_cast<uintptr_t>(P.p_local);
+    for (int r = 0; r < P.w; ++r) bits |= reinterpret_cast<uintptr_t>(P.g[r]);
+    for (int r = 0; r < P.ndst; ++r) bits |= reinterpret_cast<uintptr_t>(P.p[r]);
+    return (bits & 15) == 0;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -234,8 +355,8 @@ constexpr int kOpt32Chunk = 4096;  // elements per work item of the 32-bit kerne
 // fma, and the vector path is bit-identical to the scalar one (and to the reference); fp32 already moves 128 bytes
 // per warp access.  Otherwise one element per access.  The choice is made per tensor, so a misaligned view in the list
 // does not demote the others.  max_unorm > 0 (LAMB / LARS) takes a list of one: unorm and param_norm belong to it.
-template <typename T, int OPT, bool DEV>
-__global__ void __launch_bounds__(512) optim32_kernel(const __grid_constant__ OptimList list, const OptimScalars s,
+template <typename T, int OPT, bool DEV, int PEERS = 0>
+__global__ void __launch_bounds__(512, PEERS > 0 ? 1 : 0) optim32_kernel(const __grid_constant__ ListOf<PEERS> list, const OptimScalars s,
                                                       const float* unorm, float max_unorm, float param_norm,
                                                       const float* lr_dev) {
     constexpr bool two = OPT == kAdam || OPT == kAdemamix;
@@ -250,6 +371,8 @@ __global__ void __launch_bounds__(512) optim32_kernel(const __grid_constant__ Op
         q.update_scale = us > cap ? cap / us : 1.0f;
     }
     const long long total = list.start[list.count];
+    bool peers_vec = true;
+    if constexpr (PEERS) peers_vec = peers_aligned(list.peers);
     int ti = 0;
     for (long long item = blockIdx.x; item < total; item += gridDim.x) {
         ti = find_tensor(list, item, ti);
@@ -265,18 +388,31 @@ __global__ void __launch_bounds__(512) optim32_kernel(const __grid_constant__ Op
         q.step_size = -q.lr * q.correction2 / q.correction1;
         const long c0 = (item - list.start[ti]) * kOpt32Chunk;
         const long c1 = c0 + kOpt32Chunk < n ? c0 + kOpt32Chunk : n;
+        long goff = 0, poff = 0;  // (PEERS) the piece's byte offsets in the flat buffers
+        if constexpr (PEERS) {
+            goff = reinterpret_cast<const char*>(g) - list.peers.g_local;
+            poff = reinterpret_cast<const char*>(p) - list.peers.p_local;
+        }
         auto one = [&](long i) {
             T pt = p[i];
             float a = s1[i], b = two ? s2[i] : 0.f, c = OPT == kAdemamix ? s1[n + i] : 0.f;
-            opt32_element<T, OPT>(q, g[i], pt, a, b, c);
-            p[i] = pt;
+            if constexpr (PEERS) {
+                T gt[1], pn[1];
+                peer_grad<T, 1, PEERS>(list.peers, goff, i, n, false, gt);
+                opt32_element<T, OPT>(q, gt[0], pt, a, b, c);
+                pn[0] = pt;
+                peer_store<T, 1>(list.peers, poff, i, n, false, pn);
+            } else {
+                opt32_element<T, OPT>(q, g[i], pt, a, b, c);
+                p[i] = pt;
+            }
             s1[i] = a;
             if (two) s2[i] = b;
             if (OPT == kAdemamix) s1[n + i] = c;
         };
         auto al = [](const void* v, uintptr_t m) { return (reinterpret_cast<uintptr_t>(v) & m) == 0; };
         const bool vec = sizeof(T) == 2 && al(g, sizeof(T) * 4 - 1) && al(p, sizeof(T) * 4 - 1) && al(s1, 15) &&
-                         al(s2, 15) && (OPT != kAdemamix || (n & 3) == 0);
+                         al(s2, 15) && (OPT != kAdemamix || (n & 3) == 0) && peers_vec;
         if (vec) {
             using V = typename Vec4<T>::type;
             for (long i = c0 + 4 * threadIdx.x; i < c1; i += 4 * blockDim.x) {
@@ -284,7 +420,11 @@ __global__ void __launch_bounds__(512) optim32_kernel(const __grid_constant__ Op
                     for (long j = i; j < n; ++j) one(j);
                     break;
                 }
-                V gv4 = *reinterpret_cast<const V*>(g + i);
+                V gv4;
+                if constexpr (PEERS)
+                    peer_grad<T, 4, PEERS>(list.peers, goff, i, n, true, *reinterpret_cast<T(*)[4]>(&gv4));
+                else
+                    gv4 = *reinterpret_cast<const V*>(g + i);
                 V pv4 = *reinterpret_cast<const V*>(p + i);
                 float4 a4 = *reinterpret_cast<const float4*>(s1 + i);
                 float4 b4 = two ? *reinterpret_cast<const float4*>(s2 + i) : make_float4(0.f, 0.f, 0.f, 0.f);
@@ -296,7 +436,10 @@ __global__ void __launch_bounds__(512) optim32_kernel(const __grid_constant__ Op
                 float* c = reinterpret_cast<float*>(&c4);
 #pragma unroll
                 for (int k = 0; k < 4; ++k) opt32_element<T, OPT>(q, gt[k], pt[k], a[k], b[k], c[k]);
-                *reinterpret_cast<V*>(p + i) = pv4;
+                if constexpr (PEERS)
+                    peer_store<T, 4>(list.peers, poff, i, n, true, *reinterpret_cast<const T(*)[4]>(&pv4));
+                else
+                    *reinterpret_cast<V*>(p + i) = pv4;
                 *reinterpret_cast<float4*>(s1 + i) = a4;
                 if (two) *reinterpret_cast<float4*>(s2 + i) = b4;
                 if (OPT == kAdemamix) *reinterpret_cast<float4*>(s1 + n + i) = c4;
@@ -404,7 +547,7 @@ template <typename T> struct Tensor8 {
     int step;
     bool aligned;     // 16-byte p / g and 8-byte state accesses allowed
 
-    template <bool DEV> __device__ __forceinline__ void load(const OptimList& L, int i) {
+    template <bool DEV, typename L_> __device__ __forceinline__ void load(const L_& L, int i) {
         const OptimTensor& d = L.t[i];
         p = static_cast<T*>(d.p);
         g = static_cast<const T*>(d.g);
@@ -421,8 +564,8 @@ template <typename T> struct Tensor8 {
 };
 
 // reference csrc/kernels.cu:914-1150
-template <typename T, int OPT, bool ONE, bool DEV>
-__global__ void __launch_bounds__(256) optim8_2state_kernel(const __grid_constant__ OptimList list, const OptimScalars s,
+template <typename T, int OPT, bool ONE, bool DEV, int PEERS = 0>
+__global__ void __launch_bounds__(256, PEERS > 0 ? 1 : 0) optim8_2state_kernel(const __grid_constant__ ListOf<PEERS> list, const OptimScalars s,
                                                             const float* qmap1, const float* qmap2,
                                                             const float* lr_dev) {
     const float beta1 = s.beta1, beta2 = s.beta2, beta3 = s.beta3, alpha = s.alpha, eps = s.eps;
@@ -445,6 +588,8 @@ __global__ void __launch_bounds__(256) optim8_2state_kernel(const __grid_constan
     const int lane = threadIdx.x & 31;
     const long long total = list.start[list.count];
     const long long warps = (long long)gridDim.x * (blockDim.x >> 5);
+    bool peers_vec = true;
+    if constexpr (PEERS) peers_vec = peers_aligned(list.peers);
     int ti = 0;
     for (long long item = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); item < total; item += warps) {
         ti = ONE ? 0 : find_tensor(list, item, ti);
@@ -465,11 +610,14 @@ __global__ void __launch_bounds__(256) optim8_2state_kernel(const __grid_constan
         const float am1 = absmax1[blk], am2 = absmax2[blk];
         const float am3 = OPT == kAdemamix ? absmax1[(n + base) / kOptBlock] : 0.f;
         const long i0 = base + lane * 8;
-        const bool vec = aligned && base + kOptBlock <= n;
+        const bool vec = aligned && base + kOptBlock <= n && peers_vec;
         alignas(16) T gts[8];
         alignas(16) T pts[8];
         alignas(8) unsigned char c1s[8], c2s[8], c3s[8];
-        load8<T>(g, i0, n, vec, round_to<T>(0.0f), gts);
+        if constexpr (PEERS)
+            peer_grad<T, 8, PEERS>(list.peers, reinterpret_cast<const char*>(g) - list.peers.g_local, i0, n, vec, gts);
+        else
+            load8<T>(g, i0, n, vec, round_to<T>(0.0f), gts);
         load8c(state1, i0, n, vec, 128, c1s);
         load8c(state2, i0, n, vec, 0, c2s);
         if (OPT == kAdemamix) load8c(state1 + n, i0, n, vec && (n & 7) == 0, 128, c3s);
@@ -523,7 +671,10 @@ __global__ void __launch_bounds__(256) optim8_2state_kernel(const __grid_constan
             c2s[j] = (unsigned char)cb2.search(__fdividef(s2[j], m2));
             if (OPT == kAdemamix) c3s[j] = quant_signed(cb1, s3[j], m3);
         }
-        store8<T>(p, i0, n, vec, pts);
+        if constexpr (PEERS)
+            peer_store<T, 8>(list.peers, reinterpret_cast<const char*>(p) - list.peers.p_local, i0, n, vec, pts);
+        else
+            store8<T>(p, i0, n, vec, pts);
         store8c(state1, i0, n, vec, c1s);
         store8c(state2, i0, n, vec, c2s);
         if (OPT == kAdemamix) store8c(state1 + n, i0, n, vec && (n & 7) == 0, c3s);
@@ -531,8 +682,8 @@ __global__ void __launch_bounds__(256) optim8_2state_kernel(const __grid_constan
 }
 
 // reference csrc/kernels.cu:1152-1325
-template <typename T, int OPT, bool ONE, bool DEV>
-__global__ void __launch_bounds__(256) optim8_1state_kernel(const __grid_constant__ OptimList list, const OptimScalars s,
+template <typename T, int OPT, bool ONE, bool DEV, int PEERS = 0>
+__global__ void __launch_bounds__(256, PEERS > 0 ? 1 : 0) optim8_1state_kernel(const __grid_constant__ ListOf<PEERS> list, const OptimScalars s,
                                                             const float* qmap1, const float* lr_dev) {
     const float beta1 = s.beta1, beta2 = s.beta2, eps = s.eps, weight_decay = s.weight_decay;
     const float lr = launch_lr<DEV>(s, lr_dev);
@@ -550,6 +701,8 @@ __global__ void __launch_bounds__(256) optim8_1state_kernel(const __grid_constan
     const int lane = threadIdx.x & 31;
     const long long total = list.start[list.count];
     const long long warps = (long long)gridDim.x * (blockDim.x >> 5);
+    bool peers_vec = true;
+    if constexpr (PEERS) peers_vec = peers_aligned(list.peers);
     int ti = 0;
     for (long long item = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); item < total; item += warps) {
         ti = ONE ? 0 : find_tensor(list, item, ti);
@@ -565,11 +718,14 @@ __global__ void __launch_bounds__(256) optim8_1state_kernel(const __grid_constan
         const long base = blk * kOptBlock;
         const float am1 = absmax1[blk];
         const long i0 = base + lane * 8;
-        const bool vec = aligned && base + kOptBlock <= n;
+        const bool vec = aligned && base + kOptBlock <= n && peers_vec;
         alignas(16) T gts[8];
         alignas(16) T pts[8];
         alignas(8) unsigned char c1s[8];
-        load8<T>(g, i0, n, vec, round_to<T>(0.0f), gts);
+        if constexpr (PEERS)
+            peer_grad<T, 8, PEERS>(list.peers, reinterpret_cast<const char*>(g) - list.peers.g_local, i0, n, vec, gts);
+        else
+            load8<T>(g, i0, n, vec, round_to<T>(0.0f), gts);
         load8<T>(p, i0, n, vec, round_to<T>(0.0f), pts);
         load8c(state1, i0, n, vec, 128, c1s);
         float s1[8];
@@ -628,7 +784,10 @@ __global__ void __launch_bounds__(256) optim8_1state_kernel(const __grid_constan
             }
             c1s[j] = quant_signed(cb1, s1[j], m1);
         }
-        store8<T>(p, i0, n, vec, pts);
+        if constexpr (PEERS)
+            peer_store<T, 8>(list.peers, reinterpret_cast<const char*>(p) - list.peers.p_local, i0, n, vec, pts);
+        else
+            store8<T>(p, i0, n, vec, pts);
         store8c(state1, i0, n, vec, c1s);
     }
 }
@@ -641,7 +800,7 @@ int grid_for(long work_items, int per_cta) {
 }
 
 // the list of a launch: the tensors and the work-item prefix counts; returns the number of work items
-long long make_list(OptimList& L, const OptimTensor* ts, int count, long long per_item) {
+template <typename L_> long long make_list(L_& L, const OptimTensor* ts, int count, long long per_item) {
     long long total = 0;
     for (int i = 0; i < count; ++i) {
         L.t[i] = ts[i];
@@ -782,6 +941,79 @@ bool list8(int opt, int dtype, const OptimTensor* ts, int count, const OptimScal
     return false;
 }
 
+// One peer launch (count <= kPeerListCap): 32-bit (eight = false) or 8-bit state, NP >= w sources.  AdEMAMix has no
+// peer instances (its third state sits at state1 + n, relative to the whole tensor).
+template <typename T, int OPT, int NP>
+void run_peers_np(bool eight, const PeerOptimList& L, long long items, const OptimScalars& s, const float* q1,
+                  const float* q2, cudaStream_t stream) {
+    if (!eight)
+        optim32_kernel<T, OPT, false, NP><<<grid_for(items, 1), 512, 0, stream>>>(L, s, nullptr, 0.0f, 0.0f, nullptr);
+    else if constexpr (OPT == kAdam)
+        optim8_2state_kernel<T, OPT, false, false, NP><<<grid_for(items, 8), 256, 0, stream>>>(L, s, q1, q2, nullptr);
+    else
+        optim8_1state_kernel<T, OPT, false, false, NP><<<grid_for(items, 8), 256, 0, stream>>>(L, s, q1, nullptr);
+}
+
+template <typename T, int OPT>
+bool run_peers(bool eight, const OptimTensor* ts, int count, const OptimScalars& s, const float* q1, const float* q2,
+               const PeerArgs& P, cudaStream_t stream) {
+    if constexpr (OPT == kAdemamix) {
+        return false;
+    } else {
+        PeerOptimList L;
+        L.peers = P;
+        const long long items = make_list(L, ts, count, eight ? kOptBlock : kOpt32Chunk);
+        if (items > 0) {
+            if (P.w <= 1)
+                run_peers_np<T, OPT, 1>(eight, L, items, s, q1, q2, stream);
+            else if (P.w <= 2)
+                run_peers_np<T, OPT, 2>(eight, L, items, s, q1, q2, stream);
+            else if (P.w <= 4)
+                run_peers_np<T, OPT, 4>(eight, L, items, s, q1, q2, stream);
+            else
+                run_peers_np<T, OPT, kMaxPeers>(eight, L, items, s, q1, q2, stream);
+        }
+        BNB200_CHECK_LAUNCH(eight ? "optimizer8bit_blockwise_peers" : "optimizer32bit_peers");
+        return true;
+    }
+}
+
+template <typename T>
+bool dispatch_peers(int opt, bool eight, const OptimTensor* ts, int count, const OptimScalars& s, const float* q1,
+                    const float* q2, const PeerArgs& P, cudaStream_t st) {
+    switch (opt) {
+    case kAdam: return run_peers<T, kAdam>(eight, ts, count, s, q1, q2, P, st);
+    case kMomentum: return run_peers<T, kMomentum>(eight, ts, count, s, q1, q2, P, st);
+    case kRmsprop: return run_peers<T, kRmsprop>(eight, ts, count, s, q1, q2, P, st);
+    case kAdagrad: return run_peers<T, kAdagrad>(eight, ts, count, s, q1, q2, P, st);
+    case kLion: return run_peers<T, kLion>(eight, ts, count, s, q1, q2, P, st);
+    }
+    return false;
+}
+
+bool list_peers(int opt, int dtype, bool eight, const OptimTensor* ts, int count, const OptimScalars& s,
+                const float* q1, const float* q2, const PeerArgs& P, cudaStream_t st) {
+    switch (dtype) {
+    case 0: return dispatch_peers<float>(opt, eight, ts, count, s, q1, q2, P, st);
+    case 1: return dispatch_peers<__half>(opt, eight, ts, count, s, q1, q2, P, st);
+    case 2: return dispatch_peers<__nv_bfloat16>(opt, eight, ts, count, s, q1, q2, P, st);
+    }
+    return false;
+}
+
+PeerArgs peer_args(const void* const* grad_srcs, int world, void* const* param_dsts, int ndst, const void* grad_local,
+                   const void* param_local, float grad_scale) {
+    PeerArgs P{};
+    for (int r = 0; r < world; ++r) P.g[r] = grad_srcs[r];
+    for (int r = 0; r < ndst; ++r) P.p[r] = param_dsts[r];
+    P.g_local = static_cast<const char*>(grad_local);
+    P.p_local = static_cast<const char*>(param_local);
+    P.grad_scale = grad_scale;
+    P.w = world;
+    P.ndst = ndst;
+    return P;
+}
+
 OptimTensor one_tensor(void* p, const void* g, void* s1, void* s2, float* a1, float* a2, long n, int step) {
     return OptimTensor{p, g, s1, s2, a1, a2, (long long)n, step, 0};
 }
@@ -838,6 +1070,31 @@ bool launch_optimizer8bit_blockwise_list_dev(int opt, int dtype, const OptimTens
                                              bool skip_zeros, cudaStream_t st) {
     const OptimScalars s{beta1, beta2, beta3, alpha, eps, wd, lr, gnorm_scale, skip_zeros};
     return list8(opt, dtype, ts, count, s, q1, q2, true, lr_dev, st);
+}
+
+int optimizer_peers_capacity() { return kPeerListCap; }
+int optimizer_max_peers() { return kMaxPeers; }
+
+// count <= optimizer_peers_capacity(), 1 <= world, ndst <= kMaxPeers: one launch; false for an unknown id or AdEMAMix
+bool launch_optimizer32bit_list_peers(int opt, int dtype, const OptimTensor* ts, int count,
+                                      const void* const* grad_srcs, int world, void* const* param_dsts, int ndst,
+                                      const void* grad_local, const void* param_local, float grad_scale, float beta1,
+                                      float beta2, float beta3, float alpha, float eps, float wd, float lr,
+                                      bool skip_zeros, cudaStream_t st) {
+    const OptimScalars s{beta1, beta2, beta3, alpha, eps, wd, lr, 1.0f, skip_zeros};
+    const PeerArgs P = peer_args(grad_srcs, world, param_dsts, ndst, grad_local, param_local, grad_scale);
+    return list_peers(opt, dtype, false, ts, count, s, nullptr, nullptr, P, st);
+}
+
+bool launch_optimizer8bit_blockwise_list_peers(int opt, int dtype, const OptimTensor* ts, int count,
+                                               const void* const* grad_srcs, int world, void* const* param_dsts,
+                                               int ndst, const void* grad_local, const void* param_local,
+                                               float grad_scale, float beta1, float beta2, float beta3, float alpha,
+                                               float eps, float wd, float lr, const float* q1, const float* q2,
+                                               bool skip_zeros, cudaStream_t st) {
+    const OptimScalars s{beta1, beta2, beta3, alpha, eps, wd, lr, 1.0f, skip_zeros};
+    const PeerArgs P = peer_args(grad_srcs, world, param_dsts, ndst, grad_local, param_local, grad_scale);
+    return list_peers(opt, dtype, true, ts, count, s, q1, q2, P, st);
 }
 
 } // namespace bnb200

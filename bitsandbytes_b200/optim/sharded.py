@@ -1,0 +1,375 @@
+"""Optimizer state sharded over data-parallel ranks (ZeRO stage 1), with the single-GPU optimizer's results.
+
+``ShardedOptimizer(AdamW8bit(model.parameters()))`` moves the parameters that require grad into one flat buffer per
+dtype, and their gradients into a flat buffer of the same layout: tensor t starts at 256 x (the blocks of the tensors
+before it), so every 256-element block of the 8-bit state is a block of one tensor, and its tail up to the block end is
+padding.  The buffer holds ``w * S`` elements, ``S = ceil(B / w) * 256`` for B blocks, and rank r owns ``[r*S,
+(r+1)*S)``: the pieces of the tensors inside that range, each a run of whole blocks of its tensor (plus the tensor's
+last, partial block when the range holds it).  A rank keeps optimizer state for its pieces only, about 1/w of the
+unsharded optimizer's bytes; whether a tensor's state is 8-bit is decided on the whole tensor (``min_8bit_size``).
+
+``step()`` exchanges the gradients with ``all_to_all_single`` into a ``[w, S]`` buffer (rank s's slice of rank r's
+gradient lands in row r on rank s), then runs one kernel per group of pieces that share their launch arguments
+(``_Update.group_key``): it sums the w ranks' gradients element by element in rank order in fp32, scales the sum by
+``grad_scale`` (default 1/w, the mean), rounds it once to the parameter dtype and updates the rank's pieces with the
+unsharded kernels' arithmetic; an ``all_gather_into_tensor`` hands every rank the new parameters.  With one rank there
+is nothing to exchange.
+
+After k steps every rank's parameters, and ``consolidated_state_dict()``, equal bit for bit those of one unsharded
+optimizer fed at each step the gradient ``T(rank-order fp32 sum * fp32(grad_scale))``, with one exception: fp32
+parameters whose state is 32-bit Lion.  There the unsharded kernel contracts the decoupled weight decay and the step
+into one fma in some unrolled copies of its element loop and not in others, so its own result depends on where an
+element falls in the loop; the sharded parameters and state are then within a few ulp of it, and a parameter whose
+``sign(beta1 * m + (1 - beta1) * g)`` argument is within rounding of zero may take the other sign.
+
+A parameter without a gradient at ``step()`` is updated with a zero gradient, as DDP's ``find_unused_parameters``
+reduces zeros; the unsharded optimizer would skip it instead.
+"""
+from __future__ import annotations
+
+from typing import Optional
+
+import torch
+import torch.distributed as dist
+
+from ..backends.cuda import optimizer_update_32bit_multi_peers, optimizer_update_8bit_blockwise_multi_peers
+from ..parallel import _group_world_rank
+from .optimizer import _STATE_BLOCK, Optimizer2State, Optimizer8bit, _Update, group_updates
+
+_QUANT_KEY = Optimizer8bit._FSDP_WRAPPED_QUANT_STATE_KEY
+_STATE_KEYS = ("state1", "state2", "absmax1", "absmax2")
+
+
+def _blocks(n: int) -> int:
+    return -(-n // _STATE_BLOCK)
+
+
+def partition(numels, world: int):
+    """The layout of one flat buffer: (starts, S, pieces), pieces[r] = [(tensor index, offset in the tensor, numel)] of
+    rank r, in tensor order."""
+    starts, B = [], 0
+    for n in numels:
+        starts.append(B * _STATE_BLOCK)
+        B += _blocks(n)
+    S = -(-B // world) * _STATE_BLOCK
+    pieces = []
+    for r in range(world):
+        lo, hi, mine = r * S, (r + 1) * S, []
+        for t, (s, n) in enumerate(zip(starts, numels)):
+            a, b = max(lo, s), min(hi, s + n)
+            if a < b:
+                mine.append((t, a - s, b - a))
+        pieces.append(mine)
+    return starts, S, pieces
+
+
+class _PieceUpdate(_Update):
+    """A piece's launch arguments: p, its view of the local flat parameters; g, of the flat gradient."""
+
+    __slots__ = ("flat", "g")
+
+
+class _Flat:
+    """The parameters of one dtype: flat parameter and gradient buffers, the layout, this rank's pieces."""
+
+    def __init__(self, params, dtype, device, world: int, rank: int):
+        self.params, self.dtype = params, dtype
+        self.numels = [p.numel() for p in params]
+        self.starts, self.S, pieces = partition(self.numels, world)
+        self.pieces = pieces[rank]
+        n = world * self.S
+        self.param = torch.zeros(n, dtype=dtype, device=device)
+        self.grad = torch.zeros(n, dtype=dtype, device=device)
+        self.recv = None  # the [w, S] gradient exchange buffer, made at the first step
+
+
+class ShardedOptimizer(torch.optim.Optimizer):
+    """Shard a bnb optimizer's state over the data-parallel ranks of ``group`` (see the module documentation).
+
+    ``optimizer``: an 8-bit / 32-bit / mixed Adam, AdamW, SGD (momentum), RMSprop, Adagrad or Lion of ``bnb.optim``
+    that has taken no step.  Its ``param_groups`` are this object's, so learning-rate schedulers work on either.
+    ``grad_scale``: the factor of the summed gradient, 1/w (the mean) by default.  The model is not wrapped: run
+    ``loss.backward(); opt.step(); opt.zero_grad()`` on every rank."""
+
+    def __init__(self, optimizer, group=None, grad_scale: Optional[float] = None):
+        if not isinstance(optimizer, Optimizer8bit):
+            raise ValueError(f"ShardedOptimizer wraps a bitsandbytes_b200 optimizer, got {type(optimizer).__name__}")
+        if optimizer.is_paged:
+            raise ValueError("ShardedOptimizer does not support paged optimizer state")
+        if optimizer.capturable:
+            raise ValueError("ShardedOptimizer does not support capturable=True")
+        if optimizer.optimizer_name == "ademamix":
+            raise ValueError("ShardedOptimizer does not support AdEMAMix: its kernels address the third state "
+                             "relative to the whole tensor")
+        if any(len(s) for s in optimizer.state.values()):
+            raise ValueError("ShardedOptimizer wraps an optimizer that has taken no step: this one already has state")
+        # (torch's constructor for the hooks and the type learning-rate schedulers check; the groups are then shared)
+        super().__init__([dict(g) for g in optimizer.param_groups], optimizer.defaults)
+        self.optimizer, self.group = optimizer, group
+        self.param_groups, self.defaults = optimizer.param_groups, optimizer.defaults
+        optimizer.check_overrides()
+        self.world, self.rank = _group_world_rank(group)
+        self.grad_scale = 1.0 / self.world if grad_scale is None else float(grad_scale)
+        # (gindex, pindex, p, config) of every parameter that requires grad, in the optimizer's order
+        self.entries = []
+        for gi, g in enumerate(optimizer.param_groups):
+            for pi, p in enumerate(g["params"]):
+                if p.requires_grad:
+                    config = optimizer.get_config(gi, pi, g)
+                    if config["max_unorm"] > 0.0:
+                        raise ValueError("ShardedOptimizer does not support max_unorm > 0 (LAMB, LARS): the trust "
+                                         "ratio needs the whole tensor's norm")
+                    self.entries.append((gi, pi, p, config))
+        devices = {p.device for _, _, p, _ in self.entries}
+        if len(devices) > 1:
+            raise ValueError(f"ShardedOptimizer needs every parameter on one device, got {sorted(map(str, devices))}")
+        self.device = devices.pop() if devices else torch.device("cuda", torch.cuda.current_device())
+        by_dtype = {}
+        for i, (_, _, p, _) in enumerate(self.entries):
+            by_dtype.setdefault(p.dtype, []).append(i)
+        self.flats, self.steps = [], [0] * len(self.entries)
+        for dtype, idx in by_dtype.items():
+            flat = _Flat([self.entries[i][2] for i in idx], dtype, self.device, self.world, self.rank)
+            flat.index = idx
+            self._bind(flat)
+            self.flats.append(flat)
+        self._make_state()
+
+    # ---- construction
+    def _bind(self, flat: _Flat) -> None:
+        """Parameters into the flat buffer (rank 0's values on every rank), gradients as views of the flat gradient."""
+        with torch.no_grad():
+            for p, s, n in zip(flat.params, flat.starts, flat.numels):
+                flat.param[s:s + n].copy_(p.data.reshape(-1))
+            if self.world > 1:
+                src = dist.get_global_rank(self.group, 0) if self.group is not None else 0
+                dist.broadcast(flat.param, src=src, group=self.group)
+        flat.views = []
+        for p, s, n in zip(flat.params, flat.starts, flat.numels):
+            if p.grad is not None:
+                flat.grad[s:s + n].copy_(p.grad.reshape(-1))
+            p.data = flat.param[s:s + n].view_as(p)
+            p.grad = flat.grad[s:s + n].view_as(p)
+            flat.views.append(p.grad)
+
+    def _make_state(self) -> None:
+        """State of this rank's pieces: 8-bit or 32-bit as the whole tensor's would be."""
+        opt = self.optimizer
+        two = isinstance(opt, Optimizer2State)
+        self.pieces = []  # (flat, entry index, first flat element, numel, state)
+        for flat in self.flats:
+            for t, off, n in flat.pieces:
+                e = flat.index[t]
+                _, _, p, config = self.entries[e]
+                dtype = opt._state_dtype(config, p)
+                st = {"state1": torch.zeros(n, dtype=dtype, device=self.device)}
+                if two:
+                    st["state2"] = torch.zeros(n, dtype=dtype, device=self.device)
+                if dtype == torch.uint8:
+                    st["qmap1"] = opt._qmap("dynamic", self.device)
+                    st["absmax1"] = torch.zeros(_blocks(n), dtype=torch.float32, device=self.device)
+                    if two:
+                        st["qmap2"] = opt._qmap("udynamic", self.device)
+                        st["absmax2"] = torch.zeros(_blocks(n), dtype=torch.float32, device=self.device)
+                self.pieces.append((flat, e, flat.starts[t] + off, n, st))
+
+    # ---- the training loop
+    def zero_grad(self, set_to_none: bool = True) -> None:
+        """Zero the flat gradients; every ``p.grad`` stays (or becomes again) its view of the flat gradient."""
+        for flat in self.flats:
+            flat.grad.zero_()
+            for p, v in zip(flat.params, flat.views):
+                p.grad = v
+
+    def _gather_grads(self) -> None:
+        """A ``p.grad`` that is not its view (None, or rebound by the user) goes into its slot: zeros for None."""
+        with torch.no_grad():
+            for flat in self.flats:
+                for p, v, s, n in zip(flat.params, flat.views, flat.starts, flat.numels):
+                    if p.grad is v:
+                        continue
+                    if p.grad is None:
+                        flat.grad[s:s + n].zero_()
+                    else:
+                        flat.grad[s:s + n].copy_(p.grad.reshape(-1))
+                    p.grad = v
+
+    def _updates(self):
+        """The launch arguments of this rank's pieces, grouped as the unsharded optimizer groups its tensors."""
+        opt, two = self.optimizer, isinstance(self.optimizer, Optimizer2State)
+        updates = []
+        for flat, e, s, n, st in self.pieces:
+            gi, pi, _, _ = self.entries[e]
+            config = opt.get_config(gi, pi, self.param_groups[gi])  # (read at every step: lr schedules)
+            st["step"] = self.steps[e]
+            betas = config["betas"]
+            beta3 = betas[2] if two and len(betas) >= 3 else 0.0
+            u = _PieceUpdate(opt.optimizer_name, flat.param[s:s + n], st, config, betas[0], betas[1], beta3,
+                        config.get("alpha", 0.0) if two else 0.0)
+            u.flat, u.g = flat, flat.grad[s:s + n]
+            updates.append(u)
+        return group_updates(updates)
+
+    def _launch(self, batch, srcs, dsts) -> None:
+        u, st = batch[0], batch[0].state
+        flat = u.flat
+        g, p = [b.g for b in batch], [b.p for b in batch]
+        s1 = [b.state["state1"] for b in batch]
+        s2 = [b.state["state2"] for b in batch] if "state2" in st else None
+        steps = [b.state["step"] for b in batch]
+        if st["state1"].dtype == torch.float32:
+            optimizer_update_32bit_multi_peers(u.name, g, p, s1, s2, u.beta1, u.beta2, u.beta3, u.alpha, u.eps,
+                                               u.weight_decay, steps, u.lr, srcs, dsts, flat.grad, flat.param,
+                                               self.grad_scale, skip_zeros=u.skip_zeros)
+        else:
+            a1 = [b.state["absmax1"] for b in batch]
+            a2 = [b.state["absmax2"] for b in batch] if s2 is not None else None
+            optimizer_update_8bit_blockwise_multi_peers(u.name, g, p, s1, s2, u.beta1, u.beta2, u.beta3, u.alpha,
+                                                        u.eps, steps, u.lr, st["qmap1"], st.get("qmap2"), a1, a2,
+                                                        u.weight_decay, srcs, dsts, flat.grad, flat.param,
+                                                        self.grad_scale, skip_zeros=u.skip_zeros)
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        self._gather_grads()
+        self.steps = [k + 1 for k in self.steps]
+        batches = self._updates()
+        self._exchange(batches)
+        return loss
+
+    def _exchange(self, batches) -> None:
+        """Gradients in by all-to-all, one launch per batch of pieces, parameters out by all-gather."""
+        if self.world == 1:  # nothing to exchange: the local gradient is the only source
+            for batch in batches:
+                f = batch[0].flat
+                self._launch(batch, [f.grad.data_ptr()], [f.param.data_ptr()])
+            return
+        srcs = {}
+        for f in self.flats:
+            if f.recv is None:
+                f.recv = torch.empty_like(f.grad)
+            dist.all_to_all_single(f.recv, f.grad, group=self.group)
+            es, s0 = f.grad.element_size(), self.rank * f.S
+            srcs[id(f)] = [f.recv.data_ptr() + (r * f.S - s0) * es for r in range(self.world)]
+        for batch in batches:
+            f = batch[0].flat
+            self._launch(batch, srcs[id(f)], [f.param.data_ptr()])
+        for f in self.flats:
+            s0 = self.rank * f.S
+            dist.all_gather_into_tensor(f.param, f.param[s0:s0 + f.S], group=self.group)
+
+    # ---- checkpoints
+    def _param_ids(self):
+        """id(p) -> index in the optimizer's state dict (torch numbers the parameters across the groups)."""
+        ids, k = {}, 0
+        for g in self.param_groups:
+            for p in g["params"]:
+                ids[id(p)] = k
+                k += 1
+        return ids
+
+    def state_dict(self):
+        """This rank's shard: every piece's state with its tensor, offset and size, and the partition it came from."""
+        ids = self._param_ids()
+        pieces = []
+        for flat, e, s, n, st in self.pieces:
+            pieces.append({"param": ids[id(self.entries[e][2])], "offset": s - flat.starts[flat.index.index(e)], "numel": n,
+                           "state": {k: v for k, v in st.items() if k in _STATE_KEYS}})
+        sd = self.optimizer.state_dict()
+        return {"sharded": {"world": self.world, "rank": self.rank,
+                            "numels": [[f.numels[t] for t in range(len(f.numels))] for f in self.flats]},
+                "pieces": pieces, "steps": {ids[id(p)]: self.steps[i] for i, (_, _, p, _) in enumerate(self.entries)},
+                "param_groups": sd["param_groups"]}
+
+    def consolidated_state_dict(self, to: int = 0):
+        """The unsharded optimizer's ``state_dict()``, with its tensors on the CPU, on group rank ``to``; None on the
+        other ranks.  Only rank ``to`` receives the other shards, so no GPU holds the whole state."""
+        mine = self.state_dict()
+        local = [{"param": q["param"], "offset": q["offset"], "numel": q["numel"],
+                  "state": {k: v.cpu() for k, v in q["state"].items()}} for q in mine["pieces"]]
+        if self.world > 1:
+            every = [None] * self.world if self.rank == to else None
+            dst = dist.get_global_rank(self.group, to) if self.group is not None else to
+            dist.gather_object(local, every, dst=dst, group=self.group)
+            if self.rank != to:
+                return None
+        else:
+            every = [local]
+        by_param = {}
+        for shard in every:
+            for q in shard:
+                by_param.setdefault(q["param"], []).append(q)
+        ids = self._param_ids()
+        opt = self.optimizer
+        state = {}
+        for i, (_, _, p, config) in enumerate(self.entries):
+            k = ids[id(p)]
+            parts = sorted(by_param.get(k, []), key=lambda q: q["offset"])
+            wrapped = {}
+            for key in _STATE_KEYS:
+                if parts and key in parts[0]["state"]:
+                    full = torch.cat([q["state"][key] for q in parts])
+                    wrapped[key] = full.view(p.shape) if key.startswith("state") else full
+            if not parts:  # an empty tensor: the unsharded optimizer's zero-size state
+                dtype = opt._state_dtype(config, p)
+                wrapped["state1"] = torch.zeros(p.shape, dtype=dtype)
+                if isinstance(opt, Optimizer2State):
+                    wrapped["state2"] = torch.zeros(p.shape, dtype=dtype)
+                if dtype == torch.uint8:
+                    wrapped["absmax1"] = torch.zeros(0)
+                    if isinstance(opt, Optimizer2State):
+                        wrapped["absmax2"] = torch.zeros(0)
+            if wrapped["state1"].dtype == torch.uint8:
+                wrapped["qmap1"] = opt._qmap("dynamic", self.device).cpu()
+                if "state2" in wrapped:
+                    wrapped["qmap2"] = opt._qmap("udynamic", self.device).cpu()
+            state[k] = {"step": self.steps[i], _QUANT_KEY: wrapped}
+        return {"state": state, "param_groups": mine["param_groups"]}
+
+    def load_state_dict(self, state_dict) -> None:
+        """Load this optimizer's own shard (same world, rank and parameters), or an unsharded optimizer's state dict
+        (``consolidated_state_dict()`` or a plain optimizer's), of which every rank takes its blocks: a checkpoint taken
+        at one world size loads at another through the consolidated form."""
+        groups = state_dict["param_groups"]
+        if len(groups) != len(self.param_groups) or any(len(g["params"]) != len(s["params"])
+                                                        for g, s in zip(self.param_groups, groups)):
+            raise ValueError("loaded state dict does not match the optimizer's parameter groups")
+        ids = self._param_ids()
+        if "sharded" in state_dict:
+            mine = self.state_dict()
+            if state_dict["sharded"] != mine["sharded"] or [(q["param"], q["offset"], q["numel"])
+                                                            for q in state_dict["pieces"]] != \
+                    [(q["param"], q["offset"], q["numel"]) for q in mine["pieces"]]:
+                raise ValueError("this shard was saved with another partition (world, rank or parameters): load the "
+                                 "consolidated_state_dict() instead")
+            for (_, _, _, _, st), q in zip(self.pieces, state_dict["pieces"]):
+                for key, v in q["state"].items():
+                    st[key] = v.to(self.device, copy=True)
+            steps = state_dict["steps"]
+        else:
+            full = state_dict["state"]
+            for flat, e, s, n, st in self.pieces:
+                k = ids[id(self.entries[e][2])]
+                off = s - flat.starts[flat.index.index(e)]
+                if k not in full:
+                    raise ValueError(f"loaded state dict has no state for parameter {k}")
+                src = dict(full[k])
+                src.update(src.pop(_QUANT_KEY, {}))
+                for key in _STATE_KEYS:
+                    if key not in src:
+                        continue
+                    v = src[key].reshape(-1)
+                    part = v[off:off + n] if key.startswith("state") else v[off // _STATE_BLOCK:
+                                                                              off // _STATE_BLOCK + _blocks(n)]
+                    if key in st and part.dtype != st[key].dtype:
+                        raise ValueError(f"loaded state of parameter {k} is {part.dtype}, this optimizer keeps "
+                                         f"{st[key].dtype}")
+                    st[key] = part.to(self.device, copy=True)
+            steps = {k: int(v["step"]) for k, v in full.items()}
+        self.steps = [int(steps.get(ids[id(p)], 0)) for _, _, p, _ in self.entries]
+        for g, s in zip(self.param_groups, groups):
+            g.update({k: v for k, v in s.items() if k != "params"})

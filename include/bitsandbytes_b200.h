@@ -353,6 +353,18 @@ int cbnb_b200_optimizer_update_8bit_blockwise_multi(int optimizer, int dtype, co
  * learning rate, bit for bit.  Return 0, or 100 with the message set (also for a NULL step_ptr). */
 int cbnb_b200_optimizer_update_32bit_multi_dev(int optimizer, int dtype, const bnb_b200_optim_tensor_t* tensors, int count, float beta1, float beta2, float beta3, float alpha, float eps, float weight_decay, float lr, const float* lr_dev, float gnorm_scale, bool skip_zeros, bnb_stream_t stream);
 int cbnb_b200_optimizer_update_8bit_blockwise_multi_dev(int optimizer, int dtype, const bnb_b200_optim_tensor_t* tensors, int count, float beta1, float beta2, float beta3, float alpha, float eps, float weight_decay, float lr, const float* lr_dev, const float* quantiles1, const float* quantiles2, float gnorm_scale, bool skip_zeros, bnb_stream_t stream);
+/* Data-parallel multi-tensor steps (sharded optimizer state, ZeRO stage 1): each descriptor is a piece of a rank's
+ * local flat gradient and parameter buffers of `numel` elements, g = grad_local + o_g and p = param_local + o_p (byte
+ * offsets).  The gradient of element i is T(fp32(((G_0[i] + G_1[i]) + ...) + G_{world-1}[i]) * grad_scale), G_r the
+ * dtype array at grad_srcs[r] + o_g: an fp32 sum in rank order, rounded once; the parameter is read from p, and the new
+ * value is written to param_dsts[d] + o_p for each of the ndst destinations (not to p unless param_local is one of
+ * them).  Everything else is the _multi entries' arithmetic with gnorm_scale = 1, bit for bit.  1 <= world, ndst <= 8;
+ * AdEMAMix (id 5) is refused.  count <= cbnb_b200_optimizer_peers_capacity().  Return 0; 100 for a bad count or id;
+ * 1 for a bad source, destination, base, code book or a piece outside the local buffers -- with
+ * cbnb_b200_last_error_message() set and nothing launched. */
+int cbnb_b200_optimizer_peers_capacity(void);
+int cbnb_b200_optimizer_update_32bit_multi_peers(int optimizer, int dtype, const bnb_b200_optim_tensor_t* tensors, int count, const void* const* grad_srcs, int world, void* const* param_dsts, int ndst, const void* grad_local, const void* param_local, long long numel, float grad_scale, float beta1, float beta2, float beta3, float alpha, float eps, float weight_decay, float lr, bool skip_zeros, bnb_stream_t stream);
+int cbnb_b200_optimizer_update_8bit_blockwise_multi_peers(int optimizer, int dtype, const bnb_b200_optim_tensor_t* tensors, int count, const void* const* grad_srcs, int world, void* const* param_dsts, int ndst, const void* grad_local, const void* param_local, long long numel, float grad_scale, float beta1, float beta2, float beta3, float alpha, float eps, float weight_decay, float lr, const float* quantiles1, const float* quantiles2, bool skip_zeros, bnb_stream_t stream);
 
 #ifdef __cplusplus
 }
