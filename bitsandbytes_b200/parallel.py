@@ -21,7 +21,7 @@ all-gather.  The gather is along the inner dimension of a row-major matrix, whic
 N/world]`` staging buffer; ``gather_output=False`` hands back the local slice instead (what
 a following row-parallel layer wants).
 
-Fused exchange (``PeerGather`` + ``forward_fused``): the output lives in symmetric memory
+Fused exchange (``PeerGather`` + ``fused_forward``): the output lives in symmetric memory
 (``torch.distributed._symmetric_memory``: one ``[M, N]`` buffer per rank, every rank holds the
 peers' mappings) and the GEMM epilogue stores each output element into ITS columns of EVERY rank's
 buffer -- the all-gather rides on the kernel's own stores over NVLink / NVSwitch, tile by tile,
@@ -77,8 +77,8 @@ tensor-parallel LLM.int8() layers below share this backward (``_ColumnInputGrad`
 dequantised weight differs (``Shard4bit.dequantize``, ``Shard8bit.dequantize``).
 
 The ``fused_forward*`` routes train when given ``grad_peers`` (:class:`PeerInputGrad`, two symmetric-memory slots): the
-forward is the route's own, through the same ``torch.autograd.Function``, and the backward is the layer's, with the
-exchange through symmetric memory instead of NCCL.  The column layer's rank r stores its fp32 partial into its own slot,
+forward and the backward are the layer's, through the same ``torch.autograd.Function``, each with its exchange through
+symmetric memory instead of NCCL.  The column layer's rank r stores its fp32 partial into its own slot,
 one barrier, and each rank reduces the peers' slots in rank order (``reduce_partials_ptrs``, the arithmetic of
 ``reduce_partials``): all M rows, or only its tokens' rows under sequence parallelism.  The row layer copies its
 tokens' rows of ``grad_y`` (sequence parallelism) or its columns of the input gradient (``input_is_parallel=False``)
@@ -171,6 +171,12 @@ class _ColumnInputGrad:
             G = G[:, s.row0:s.row0 + s.rows]
         return _input_grad(G, s, out)
 
+    def _grad_slot(self, x: torch.Tensor, sp: bool):
+        """(shape, dtype) of the slot the fused backward exchanges through for the input ``x`` of a route in mode ``sp``:
+        fp32 ``[M, K]``, M all tokens (``world`` times this rank's under sequence parallelism)."""
+        world = _group_world_rank(self.group)[0] if sp else 1
+        return (world * (x.numel() // self.shard.K), self.shard.K), torch.float32
+
     def _backward(self, grad_y: torch.Tensor, x_shape, peers: Optional["PeerInputGrad"] = None) -> torch.Tensor:
         s = self.shard
         world, rank = _group_world_rank(self.group)
@@ -207,6 +213,23 @@ class _RowInputGrad:
         G = grad_y.reshape(-1, s.rows)
         return _input_grad(G, s, torch.empty((G.shape[0], s.K), device=G.device, dtype=G.dtype))
 
+    def _grad_slot(self, x: torch.Tensor, sp: bool):
+        """(shape, dtype) of the slot the fused backward exchanges through for the input ``x``, or (None, None) when it
+        exchanges nothing; it follows the layer's own flags, whatever the route's mode ``sp``.  Sequence parallelism with
+        ``input_is_parallel=False`` exchanges twice, ``[M, N]`` then ``[M, in_features]``, which one PeerInputGrad serves
+        only when the two agree."""
+        world, _ = _group_world_rank(self.group)
+        M = x.numel() // x.shape[-1]
+        shapes = set()
+        if self.sequence_parallel and world > 1:
+            shapes.add((M, self.out_features))
+        if not self.input_is_parallel and world > 1:
+            shapes.add((M, self.in_features))
+        if len(shapes) > 1:
+            raise ValueError("a sequence-parallel row layer with input_is_parallel=False exchanges [M, out_features] and "
+                             "[M, in_features] gradients: one PeerInputGrad serves both only when they are equal")
+        return (shapes.pop(), x.dtype) if shapes else (None, None)
+
     def _backward(self, grad_y: torch.Tensor, x_shape, peers: Optional["PeerInputGrad"] = None) -> torch.Tensor:
         world, rank = _group_world_rank(self.group)
         if self.sequence_parallel and world > 1:
@@ -242,18 +265,20 @@ class _RowInputGrad:
 
 
 class _ParallelFn(torch.autograd.Function):
-    """A tensor-parallel layer's forward (``layer._forward``, or the body of a fused route), with the input gradient as
-    its backward (``layer._backward``, exchanging through NCCL, or through ``peers`` for a fused route): the shard and
-    the bias stay frozen."""
+    """A tensor-parallel layer's forward (``layer._forward``, exchanging through NCCL, or through ``peers`` in the mode
+    ``sp`` of a fused route), with the input gradient as its backward (``layer._backward``, exchanging through NCCL, or
+    through ``grad_peers`` for a fused route): the shard and the bias stay frozen.  ``copy_out``: the forward returns a
+    copy of its output (see :func:`_fused_route`)."""
 
     @staticmethod
-    def forward(ctx, x, layer, body=None, peers=None):
-        ctx.layer, ctx.x_shape, ctx.peers = layer, x.shape, peers
-        return layer._forward(x) if body is None else body(x)
+    def forward(ctx, x, layer, peers=None, sp=None, grad_peers=None, copy_out=False):
+        ctx.layer, ctx.x_shape, ctx.peers = layer, x.shape, grad_peers
+        y = layer._forward(x, peers, sp)
+        return y.clone() if copy_out else y
 
     @staticmethod
     def backward(ctx, grad_y):
-        return ctx.layer._backward(grad_y, ctx.x_shape, ctx.peers), None, None, None
+        return ctx.layer._backward(grad_y, ctx.x_shape, ctx.peers), None, None, None, None, None
 
 
 class ColumnParallelLinear4bit(_ColumnInputGrad, torch.nn.Module):
@@ -295,15 +320,41 @@ class ColumnParallelLinear4bit(_ColumnInputGrad, torch.nn.Module):
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         return _ParallelFn.apply(x, self)
 
-    def _forward(self, x: torch.Tensor) -> torch.Tensor:
+    def _forward(self, x: torch.Tensor, peers: Optional["PeerGather"] = None,
+                 sp: Optional[bool] = None) -> torch.Tensor:
+        """The layer's output.  ``sp`` (default: ``sequence_parallel``) chooses the mode.  With ``peers`` the exchange
+        goes through its symmetric-memory slot, followed by one barrier: under sequence parallelism this rank's tokens
+        are copied into its rows of every rank's ``[M, K]`` slot and the local output returned; otherwise the GEMM
+        epilogue stores the output into this rank's columns of every rank's ``[M, N]`` slot (the NCCL gather filling
+        the slot when the GEMM refuses the call), and the slot itself is returned, whatever ``gather_output`` says."""
         s = self.shard
         world, _ = _group_world_rank(self.group)
-        if self.sequence_parallel and world > 1:
-            full = torch.empty((world * x.shape[0], *x.shape[1:]), device=x.device, dtype=x.dtype)
-            dist.all_gather_into_tensor(full, x.contiguous(), group=self.group)
-            x = full
+        if self.sequence_parallel if sp is None else sp:
+            if peers is not None:
+                Ms = x.numel() // s.K
+                _check_peers(peers, peers.world * Ms, s.K, x.dtype, "token count / input width / dtype")
+                local, _, handle = peers.slot()
+                xs = x.reshape(Ms, s.K)
+                for r in range(peers.world):
+                    handle.get_buffer(r, (Ms, s.K), x.dtype, peers.rank * Ms * s.K).copy_(xs)
+                handle.barrier(channel=0)  # every rank's tokens have landed everywhere
+                return self.local_forward(local).view(peers.world * x.shape[0], *x.shape[1:-1], s.rows)
+            if world > 1:
+                full = torch.empty((world * x.shape[0], *x.shape[1:]), device=x.device, dtype=x.dtype)
+                dist.all_gather_into_tensor(full, x.contiguous(), group=self.group)
+                x = full
         lead = x.shape[:-1]
         M = x.numel() // s.K
+        if peers is not None:
+            _check_peers(peers, M, self.out_features, x.dtype, "output shape / dtype")
+            local, bases, handle = peers.slot()
+            ptrs = peers.dest_ptrs(bases, s.row0 * local.element_size())
+            ok = gemm_4bit_multi_out(x, s.packed, (s.rows, s.K), s.absmax, s.blocksize, s.quant_type, self.bias_shard,
+                                     s.absmax_8bit, s.absmax_code, s.absmax_offset, ptrs, peers.N)
+            if not ok:  # shape outside the tensor-core kernel: local slice + NCCL all-gather into the same slot
+                local.copy_(_gather_columns(self, x, M, x.dtype, x.device))
+            handle.barrier(channel=0)  # every rank's stores have landed everywhere
+            return local
         if world == 1 or not self.gather_output:
             return self.local_forward(x).view(*lead, s.rows)
         return _gather_columns(self, x, M, x.dtype, x.device).reshape(*lead, world * s.rows)
@@ -333,39 +384,24 @@ def _input_grad(G: torch.Tensor, shard, out: torch.Tensor) -> torch.Tensor:
     return out
 
 
-def _fused_route(what: str, layer, x: torch.Tensor, body, grad_peers: Optional["PeerInputGrad"], slot,
+def _fused_route(what: str, layer, x: torch.Tensor, peers, sp: bool, grad_peers: Optional["PeerInputGrad"],
                  copy_out: bool = False) -> torch.Tensor:
-    """``body(x)``, a fused route's forward, as it is or, for an input that requires grad, through :class:`_ParallelFn`
-    with the layer's backward exchanging through ``grad_peers``, checked once here against ``slot()``: the (shape,
-    dtype) of the slot that backward exchanges through, (None, None) for none.  Without ``grad_peers`` such an input is
-    refused: the route would drop its gradient.
+    """``layer._forward(x, peers, sp)``, a fused route's forward, as it is or, for an input that requires grad, through
+    :class:`_ParallelFn` with the layer's backward exchanging through ``grad_peers``, checked once here against the slot
+    that backward exchanges through (``layer._grad_slot``).  Without ``grad_peers`` such an input is refused: the route
+    would drop its gradient.
 
-    ``copy_out``: the body returns its symmetric-memory output slot, which the peers' GEMM epilogues rewrite two calls
-    later.  Inference uses the output at once; autograd may keep it until the backward (SiLU, a norm or a product save
-    their input), so a training call returns a copy."""
+    ``copy_out``: the forward returns its symmetric-memory output slot, which the peers' GEMM epilogues rewrite two
+    calls later.  Inference uses the output at once; autograd may keep it until the backward (SiLU, a norm or a product
+    save their input), so a training call returns a copy."""
     if not (torch.is_grad_enabled() and x.requires_grad):
-        return body(x)
+        return layer._forward(x, peers, sp)
     if grad_peers is None:
         raise RuntimeError(f"{what} is inference only without grad_peers and would drop the input gradient: pass "
                            "grad_peers=PeerInputGrad(...) to train through it, call the layer itself, or run this under "
                            "torch.no_grad()")
-    _check_peer_grad(grad_peers, layer.group, *slot())
-    return _ParallelFn.apply(x, layer, (lambda x: body(x).clone()) if copy_out else body, grad_peers)
-
-
-def _col_route(what: str, layer, x: torch.Tensor, body, grad_peers, sp: bool, copy_out: bool = False) -> torch.Tensor:
-    """A column layer's fused route: its backward reduces from fp32 ``[M, K]`` slots, M all tokens (``world`` times
-    this rank's under sequence parallelism)."""
-    def slot():
-        world = _group_world_rank(layer.group)[0] if sp else 1
-        return (world * (x.numel() // layer.shard.K), layer.shard.K), torch.float32
-    return _fused_route(what, layer, x, body, grad_peers, slot, copy_out)
-
-
-def _row_route(what: str, layer, x: torch.Tensor, body, grad_peers) -> torch.Tensor:
-    """A row layer's fused route: its backward's slot follows from the layer (:func:`_row_grad_slot`)."""
-    return _fused_route(what, layer, x, body, grad_peers, lambda: _row_grad_slot(layer, x.numel() // x.shape[-1],
-                                                                                  x.dtype))
+    _check_peer_grad(grad_peers, layer.group, *layer._grad_slot(x, sp))
+    return _ParallelFn.apply(x, layer, peers, sp, grad_peers, copy_out)
 
 
 def sp_rows(x: torch.Tensor, world: int) -> int:
@@ -398,6 +434,13 @@ def _gather_columns(layer, inp, M: int, dtype: torch.dtype, device) -> torch.Ten
     return stage.permute(1, 0, 2).reshape(M, world * rows)
 
 
+def _check_peers(peers, M: int, N: int, dtype: torch.dtype, what: str) -> None:
+    """``peers`` (a :class:`PeerGather` or :class:`PeerPartials`) was built for ``[M, N]`` of ``dtype``: checked on the
+    host before any launch."""
+    if M != peers.M or N != peers.N or dtype != peers.dtype:
+        raise ValueError(f"{type(peers).__name__} was built for a different {what}")
+
+
 def _gather_partials(layer, inp, M: int, dtype: torch.dtype, device, what: str) -> torch.Tensor:
     """The ``[world, M, N]`` partials of a row-parallel layer: ``layer.partial_forward`` writes this rank's into its
     slot of a stage (kept on the layer for the next call), and the stage is all-gathered."""
@@ -410,6 +453,24 @@ def _gather_partials(layer, inp, M: int, dtype: torch.dtype, device, what: str) 
     if world > 1:
         dist.all_gather_into_tensor(stage.view(-1), stage[rank].reshape(-1), group=layer.group)
     return stage
+
+
+def _sp_exchange(layer, inp, Ms: int, dtype: torch.dtype, what: str) -> torch.Tensor:
+    """A sequence-parallel row layer's ``[world, M/world, N]`` partials of this rank's tokens, chunk r from rank r:
+    ``layer.partial_forward`` writes the full ``[M, N]`` partial of ``dtype`` into a send buffer (kept on the layer with
+    its receive buffer for the next call), then an all-to-all (NCCL's reduce-scatter would sum in another order)."""
+    world, _ = _group_world_rank(layer.group)
+    shape = (world, Ms, layer.shard.rows)
+    bufs = layer._sp_bufs
+    if bufs is None or bufs[0].shape != shape or bufs[0].device != inp.device:
+        bufs = layer._sp_bufs = tuple(torch.empty(shape, device=inp.device, dtype=dtype) for _ in range(2))
+    send, recv = bufs
+    if not layer.partial_forward(inp, [send]):
+        raise RuntimeError(f"{what} does not serve this shard shape")
+    if world == 1:
+        return send
+    dist.all_to_all_single(recv, send, group=layer.group)
+    return recv
 
 
 class _PeerSlots:
@@ -492,45 +553,13 @@ def _check_peer_grad(peers, group, shape=None, dtype: Optional[torch.dtype] = No
                          f"{list(shape)} {dtype}")
 
 
-def _row_grad_slot(layer, M: int, dtype: torch.dtype):
-    """(shape, dtype) of the slot the fused backward of a row layer exchanges through for M tokens, or (None, None)
-    when it exchanges nothing.  Sequence parallelism with ``input_is_parallel=False`` exchanges twice, ``[M, N]`` then
-    ``[M, in_features]``, which one PeerInputGrad serves only when the two agree."""
-    world, _ = _group_world_rank(layer.group)
-    shapes = set()
-    if layer.sequence_parallel and world > 1:
-        shapes.add((M, layer.out_features))
-    if not layer.input_is_parallel and world > 1:
-        shapes.add((M, layer.in_features))
-    if len(shapes) > 1:
-        raise ValueError("a sequence-parallel row layer with input_is_parallel=False exchanges [M, out_features] and "
-                         "[M, in_features] gradients: one PeerInputGrad serves both only when they are equal")
-    return (shapes.pop(), dtype) if shapes else (None, None)
-
-
 def fused_forward(layer: "ColumnParallelLinear4bit", x: torch.Tensor, peers: PeerGather,
                   grad_peers: Optional[PeerInputGrad] = None) -> torch.Tensor:
     """``layer(x)`` with the all-gather fused into the GEMM epilogue; returns this rank's [M, N] slot, valid until the
     slot comes round again two calls later.  With ``grad_peers = PeerInputGrad(M, K, torch.float32)`` an input that
     requires grad gets its gradient, exchanged through symmetric memory, and the call returns a copy of the slot, which
     autograd may keep until the backward."""
-    return _col_route("fused_forward", layer, x, lambda x: _fused_forward(layer, x, peers), grad_peers, sp=False,
-                      copy_out=True)
-
-
-def _fused_forward(layer: "ColumnParallelLinear4bit", x: torch.Tensor, peers: PeerGather) -> torch.Tensor:
-    s = layer.shard
-    M = x.numel() // s.K
-    if M != peers.M or layer.out_features != peers.N or x.dtype != peers.dtype:
-        raise ValueError("PeerGather was built for a different output shape / dtype")
-    local, bases, handle = peers.slot()
-    ptrs = peers.dest_ptrs(bases, s.row0 * local.element_size())
-    ok = gemm_4bit_multi_out(x, s.packed, (s.rows, s.K), s.absmax, s.blocksize, s.quant_type, layer.bias_shard,
-                             s.absmax_8bit, s.absmax_code, s.absmax_offset, ptrs, peers.N)
-    if not ok:  # shape outside the tensor-core kernel: local slice + NCCL all-gather into the same slot
-        local.copy_(_gather_columns(layer, x, M, x.dtype, x.device))
-    handle.barrier(channel=0)  # every rank's stores have landed everywhere
-    return local
+    return _fused_route("fused_forward", layer, x, peers, False, grad_peers, copy_out=True)
 
 
 def _ftz(t: torch.Tensor) -> torch.Tensor:
@@ -630,36 +659,39 @@ class RowParallelLinear4bit(_RowInputGrad, torch.nn.Module):
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         return _ParallelFn.apply(x, self)
 
-    def _forward(self, x: torch.Tensor) -> torch.Tensor:
+    def _forward(self, x: torch.Tensor, peers: Optional["PeerPartials"] = None,
+                 sp: Optional[bool] = None) -> torch.Tensor:
+        """The layer's output.  ``sp`` (default: ``sequence_parallel``) chooses the mode.  With ``peers`` the partials
+        are exchanged through its symmetric-memory slot, followed by one barrier: the GEMM epilogue stores ``P_r`` into
+        slot r of every rank's buffer or, under sequence parallelism, the rows of rank s's tokens into slot r of rank
+        s's buffer (the NCCL exchange filling the slot when the scatter GEMM refuses the call)."""
         s = self.shard
+        world, _ = _group_world_rank(self.group)
         x_r = self.local_input(x)
-        M = x_r.numel() // s.K
-        if self.sequence_parallel:
-            return self._sp_forward(x_r, x_r.dtype)
-        parts = _gather_partials(self, x_r, M, torch.float32, x_r.device, "gemm_4bit_partial")
-        return reduce_partials(parts, x_r.dtype, self.bias).view(*x_r.shape[:-1], s.rows)
-
-    def _sp_exchange(self, x_r: torch.Tensor) -> torch.Tensor:
-        """This rank's ``[world, M/world, N]`` partials of its own tokens, chunk r from rank r: the full ``[M, N]``
-        partial into a send buffer, then an all-to-all (NCCL's reduce-scatter would sum in another order)."""
-        world, _ = _group_world_rank(self.group)
-        Ms = sp_rows(x_r, world)
-        shape = (world, Ms, self.shard.rows)
-        bufs = self._sp_bufs
-        if bufs is None or bufs[0].shape != shape or bufs[0].device != x_r.device:
-            bufs = self._sp_bufs = (torch.empty(shape, device=x_r.device), torch.empty(shape, device=x_r.device))
-        send, recv = bufs
-        if not self.partial_forward(x_r, [send]):
-            raise RuntimeError("gemm_4bit_partial does not serve this shard shape")
-        if world == 1:
-            return send
-        dist.all_to_all_single(recv, send, group=self.group)
-        return recv
-
-    def _sp_forward(self, x_r: torch.Tensor, dtype: torch.dtype) -> torch.Tensor:
-        world, _ = _group_world_rank(self.group)
-        parts = self._sp_exchange(x_r)
-        return reduce_partials(parts, dtype, self.bias).view(x_r.shape[0] // world, *x_r.shape[1:-1], self.shard.rows)
+        if self.sequence_parallel if sp is None else sp:
+            Ms = sp_rows(x_r, world)
+            lead = (x_r.shape[0] // world, *x_r.shape[1:-1])
+            if peers is None:
+                parts = _sp_exchange(self, x_r, Ms, torch.float32, "gemm_4bit_partial")
+            else:
+                _check_peers(peers, Ms, s.rows, torch.float32, "output shape or dtype")
+                parts, bases, handle = peers.slot()
+                if not self.partial_scatter(x_r, peers.scatter_ptrs(bases, peers.rank * Ms * s.rows * 4)):
+                    # the scatter GEMM refused the call: the NCCL route fills the slot
+                    parts.copy_(_sp_exchange(self, x_r, Ms, torch.float32, "gemm_4bit_partial"))
+                handle.barrier(channel=0)  # every rank's rows have landed at their owner
+        else:
+            M = x_r.numel() // s.K
+            lead = x_r.shape[:-1]
+            if peers is None:
+                parts = _gather_partials(self, x_r, M, torch.float32, x_r.device, "gemm_4bit_partial")
+            else:
+                _check_peers(peers, M, s.rows, torch.float32, "output shape or dtype")
+                parts, bases, handle = peers.slot()
+                if not self.partial_forward(x_r, peers.dest_ptrs(bases, peers.rank * M * s.rows * 4)):
+                    raise RuntimeError("gemm_4bit_partial does not serve this shard shape")
+                handle.barrier(channel=0)  # every rank's partial has landed everywhere
+        return reduce_partials(parts, x_r.dtype, self.bias).view(*lead, s.rows)
 
 
 class PeerPartials(_PeerSlots):
@@ -678,20 +710,7 @@ def fused_forward_row(layer: RowParallelLinear4bit, x: torch.Tensor, peers: Peer
     """``layer(x)`` with the exchange of the partials fused into the GEMM epilogue: ``P_r`` is stored into slot r of
     every rank's buffer, one barrier publishes them, and each rank reduces them in rank order.  With ``grad_peers``
     an input that requires grad gets its gradient, exchanged through symmetric memory."""
-    return _row_route("fused_forward_row", layer, x, lambda x: _fused_forward_row(layer, x, peers), grad_peers)
-
-
-def _fused_forward_row(layer: RowParallelLinear4bit, x: torch.Tensor, peers: PeerPartials) -> torch.Tensor:
-    s = layer.shard
-    x_r = layer.local_input(x)
-    M = x_r.numel() // s.K
-    if M != peers.M or s.rows != peers.N or peers.dtype != torch.float32:
-        raise ValueError("PeerPartials was built for a different output shape or dtype")
-    local, bases, handle = peers.slot()
-    if not layer.partial_forward(x_r, peers.dest_ptrs(bases, peers.rank * M * s.rows * 4)):
-        raise RuntimeError("gemm_4bit_partial does not serve this shard shape")
-    handle.barrier(channel=0)  # every rank's partial has landed everywhere
-    return reduce_partials(local, x.dtype, layer.bias).view(*x_r.shape[:-1], s.rows)
+    return _fused_route("fused_forward_row", layer, x, peers, False, grad_peers)
 
 
 def fused_forward_row_sp(layer: RowParallelLinear4bit, x: torch.Tensor, peers: PeerPartials,
@@ -701,20 +720,7 @@ def fused_forward_row_sp(layer: RowParallelLinear4bit, x: torch.Tensor, peers: P
     buffer (``peers = PeerPartials(M // world, N)``), one barrier publishes them, and each rank reduces its own.  With
     ``grad_peers = PeerInputGrad(M, N, x.dtype)`` an input that requires grad gets its gradient: the token rows of
     ``grad_y`` gathered through symmetric memory."""
-    return _row_route("fused_forward_row_sp", layer, x, lambda x: _fused_forward_row_sp(layer, x, peers), grad_peers)
-
-
-def _fused_forward_row_sp(layer: RowParallelLinear4bit, x: torch.Tensor, peers: PeerPartials) -> torch.Tensor:
-    s = layer.shard
-    x_r = layer.local_input(x)
-    Ms = sp_rows(x_r, peers.world)
-    if Ms != peers.M or s.rows != peers.N or peers.dtype != torch.float32:
-        raise ValueError("PeerPartials was built for a different output shape or dtype")
-    local, bases, handle = peers.slot()
-    if not layer.partial_scatter(x_r, peers.scatter_ptrs(bases, peers.rank * Ms * s.rows * 4)):
-        local.copy_(layer._sp_exchange(x_r))  # the scatter GEMM refused the call: the NCCL route fills the slot
-    handle.barrier(channel=0)  # every rank's rows have landed at their owner
-    return reduce_partials(local, x.dtype, layer.bias).view(x_r.shape[0] // peers.world, *x_r.shape[1:-1], s.rows)
+    return _fused_route("fused_forward_row_sp", layer, x, peers, True, grad_peers)
 
 
 def fused_forward_col_sp(layer: ColumnParallelLinear4bit, x: torch.Tensor, peers: PeerGather,
@@ -724,22 +730,7 @@ def fused_forward_col_sp(layer: ColumnParallelLinear4bit, x: torch.Tensor, peers
     one barrier publishes them, and the local GEMM reads the gathered tokens.  Returns ``[M, ..., N/world]``.  With
     ``grad_peers = PeerInputGrad(M, K, torch.float32)`` an input that requires grad gets the gradient of its tokens,
     reduced from the peers' partials."""
-    return _col_route("fused_forward_col_sp", layer, x, lambda x: _fused_forward_col_sp(layer, x, peers), grad_peers,
-                      sp=True)
-
-
-def _fused_forward_col_sp(layer: ColumnParallelLinear4bit, x: torch.Tensor, peers: PeerGather) -> torch.Tensor:
-    s = layer.shard
-    world, rank = peers.world, peers.rank
-    Ms = x.numel() // s.K
-    if world * Ms != peers.M or s.K != peers.N or x.dtype != peers.dtype:
-        raise ValueError("PeerGather was built for a different token count / input width / dtype")
-    local, _, handle = peers.slot()
-    xs = x.reshape(Ms, s.K)
-    for r in range(world):
-        handle.get_buffer(r, (Ms, s.K), x.dtype, rank * Ms * s.K).copy_(xs)
-    handle.barrier(channel=0)  # every rank's tokens have landed everywhere
-    return layer.local_forward(local).view(world * x.shape[0], *x.shape[1:-1], s.rows)
+    return _fused_route("fused_forward_col_sp", layer, x, peers, True, grad_peers)
 
 
 def reassemble_shards(shards: list[Shard4bit]) -> tuple[torch.Tensor, torch.Tensor]:
@@ -1013,18 +1004,31 @@ class ColumnParallelLinear8bitLt(_ColumnInputGrad, torch.nn.Module):
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         return _ParallelFn.apply(x, self)
 
-    def _forward(self, x: torch.Tensor) -> torch.Tensor:
+    def _forward(self, x: torch.Tensor, peers=None, sp: Optional[bool] = None) -> torch.Tensor:
+        """The layer's output.  ``sp`` (default: ``sequence_parallel``) chooses the mode; ``peers`` is a
+        :class:`PeerInt8Input` under sequence parallelism (:meth:`sp_quantize`), a :class:`PeerGather` otherwise
+        (:meth:`_output`)."""
         world, _ = _group_world_rank(self.group)
-        if self.sequence_parallel and world > 1:
-            return self._output(self.sp_quantize(x), (world * x.shape[0], *x.shape[1:-1]))
-        return self._output(self.quantize(x), x.shape[:-1])
+        if (self.sequence_parallel if sp is None else sp) and (world > 1 or peers is not None):
+            return self._output(self.sp_quantize(x, peers), (world * x.shape[0], *x.shape[1:-1]))
+        return self._output(self.quantize(x), x.shape[:-1], peers)
 
-    def _output(self, q: Int8Input, lead) -> torch.Tensor:
-        """The layer's output from the quantised input of all M tokens (``lead``: its leading dimensions)."""
+    def _output(self, q: Int8Input, lead, peers: Optional["PeerGather"] = None) -> torch.Tensor:
+        """The layer's output from the quantised input of all M tokens (``lead``: its leading dimensions).  With
+        ``peers`` the int8 GEMM epilogue stores each output element into this rank's columns of every rank's ``[M, N]``
+        slot, or, past 64 outlier columns or for a shape the GEMM does not take, the NCCL route fills the slot; one
+        barrier, and the slot itself is returned, whatever ``gather_output`` says."""
         s = self.shard
         M = q.CA.shape[0]
         world, _ = _group_world_rank(self.group)
         chain = q.J > _INT8_FUSED_J
+        if peers is not None:
+            _check_peers(peers, M, self.out_features, q.dtype, "output shape / dtype")
+            local, bases, handle = peers.slot()
+            if chain or not self._gemm(q, peers.dest_ptrs(bases, s.row0 * local.element_size()), peers.N):
+                local.copy_(self._gathered(q, M, world, chain))
+            handle.barrier(channel=0)  # every rank's stores have landed everywhere
+            return local
         if world == 1:
             y = self.local_forward(q)
             if chain:
@@ -1032,15 +1036,20 @@ class ColumnParallelLinear8bitLt(_ColumnInputGrad, torch.nn.Module):
             return y.view(*lead, s.rows)
         if not self.gather_output and not chain:
             return self.local_forward(q).view(*lead, s.rows)
-        full = _gather_columns(self, q, M, q.dtype, q.CA.device)
-        if chain:
-            rows = self.outlier_rows(q)
-            subBT = torch.empty((world * s.rows, q.J), device=q.CA.device, dtype=q.dtype)
-            dist.all_gather_into_tensor(subBT, rows, group=self.group)
-            full = self.finish(full, q, subBT)
+        full = self._gathered(q, M, world, chain)
         if not self.gather_output:
             full = full[:, s.row0:s.row0 + s.rows].contiguous()
         return full.reshape(*lead, full.shape[-1])
+
+    def _gathered(self, q: Int8Input, M: int, world: int, chain: bool) -> torch.Tensor:
+        """The ``[M, N]`` output of all ranks through NCCL: the columns all-gathered and, past 64 outlier columns, the
+        unsharded layer's addmm on the all-gathered outlier weight rows."""
+        full = _gather_columns(self, q, M, q.dtype, q.CA.device)
+        if chain:
+            subBT = torch.empty((world * self.shard.rows, q.J), device=q.CA.device, dtype=q.dtype)
+            dist.all_gather_into_tensor(subBT, self.outlier_rows(q), group=self.group)
+            full = self.finish(full, q, subBT)
+        return full
 
 
 def fused_forward_col8(layer: ColumnParallelLinear8bitLt, x: torch.Tensor, peers: PeerGather,
@@ -1050,27 +1059,7 @@ def fused_forward_col8(layer: ColumnParallelLinear8bitLt, x: torch.Tensor, peers
     not take, the local GEMM + NCCL route fills the same slot.  Returns this rank's [M, N] slot.  With ``grad_peers =
     PeerInputGrad(M, K, torch.float32)`` an input that requires grad gets its gradient (the outlier decomposition
     leaves it alone, as in the layer's own backward), and the call returns a copy of the slot, as ``fused_forward``."""
-    return _col_route("fused_forward_col8", layer, x, lambda x: _fused_forward_col8(layer, x, peers), grad_peers,
-                      sp=False, copy_out=True)
-
-
-def _fused_forward_col8(layer: ColumnParallelLinear8bitLt, x: torch.Tensor, peers: PeerGather) -> torch.Tensor:
-    s = layer.shard
-    q = layer.quantize(x)
-    M = q.A.shape[0]
-    if M != peers.M or layer.out_features != peers.N or x.dtype != peers.dtype:
-        raise ValueError("PeerGather was built for a different output shape / dtype")
-    local, bases, handle = peers.slot()
-    ok = q.J <= _INT8_FUSED_J and layer._gemm(q, peers.dest_ptrs(bases, s.row0 * local.element_size()), peers.N)
-    if not ok:
-        full = _gather_columns(layer, q, M, q.A.dtype, q.A.device)
-        if q.J > _INT8_FUSED_J:
-            subBT = torch.empty((layer.out_features, q.J), device=x.device, dtype=x.dtype)
-            dist.all_gather_into_tensor(subBT, layer.outlier_rows(q), group=layer.group)
-            full = layer.finish(full, q, subBT)
-        local.copy_(full)
-    handle.barrier(channel=0)  # every rank's stores have landed everywhere
-    return local
+    return _fused_route("fused_forward_col8", layer, x, peers, False, grad_peers, copy_out=True)
 
 
 class PeerInt8Input(_PeerSlots):
@@ -1100,10 +1089,7 @@ def fused_forward_col8_sp(layer: ColumnParallelLinear8bitLt, x: torch.Tensor, pe
     (``peers = PeerInt8Input(M, K)``), one barrier publishes them, and the local GEMM reads the gathered codes.  Returns
     ``[M, ..., N/w]``.  With ``grad_peers = PeerInputGrad(M, K, torch.float32)`` an input that requires grad gets the
     gradient of its tokens, reduced from the peers' partials."""
-    world, _ = _group_world_rank(layer.group)
-    return _col_route("fused_forward_col8_sp", layer, x,
-                      lambda x: layer._output(layer.sp_quantize(x, peers), (world * x.shape[0], *x.shape[1:-1])),
-                      grad_peers, sp=True)
+    return _fused_route("fused_forward_col8_sp", layer, x, peers, True, grad_peers)
 
 
 @dataclass
@@ -1266,42 +1252,38 @@ class RowParallelLinear8bitLt(_RowInputGrad, torch.nn.Module):
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         return _ParallelFn.apply(x, self)
 
-    def _forward(self, x: torch.Tensor) -> torch.Tensor:
-        if self.sequence_parallel:
-            return self._sp_forward(x)
+    def _forward(self, x: torch.Tensor, peers: Optional[PeerPartials] = None,
+                 sp: Optional[bool] = None) -> torch.Tensor:
+        """The layer's output.  ``sp`` (default: ``sequence_parallel``) chooses the mode (:meth:`_sp_forward`).  With
+        ``peers`` the GEMM epilogue stores the int32 partial ``P_r`` into slot r of every rank's buffer, and one barrier,
+        after the outlier operands have travelled through NCCL, publishes them."""
+        if self.sequence_parallel if sp is None else sp:
+            return self._sp_forward(x, peers)
         s = self.shard
         lead = x.shape[:-1]
         x_r, world, SCA, CA, cols = self._prologue(x)
-        parts = _gather_partials(self, CA, x_r.shape[0], torch.int32, x.device, "the int8 GEMM")
-        subA, subBT = self._exchange_outliers(x_r, cols, world)
+        M = x_r.shape[0]
+        if peers is None:
+            parts = _gather_partials(self, CA, M, torch.int32, x.device, "the int8 GEMM")
+            subA, subBT = self._exchange_outliers(x_r, cols, world)
+        else:
+            _check_peers(peers, M, s.rows, torch.int32, "output shape or dtype (int32 partials)")
+            parts, bases, handle = peers.slot()
+            if not self.partial_forward(CA, peers.dest_ptrs(bases, peers.rank * M * s.rows * 4)):
+                raise RuntimeError("the int8 GEMM does not serve this shard shape")
+            subA, subBT = self._exchange_outliers(x_r, cols, world)
+            handle.barrier(channel=0)  # every rank's partial has landed everywhere
         return self.reduce(parts, SCA, x.dtype, subA, subBT).view(*lead, s.rows)
-
-    def _sp_exchange(self, CA: torch.Tensor, Ms: int) -> torch.Tensor:
-        """This rank's ``[world, M/world, N]`` int32 partials of its own tokens, chunk r from rank r: the full ``[M, N]``
-        partial into a send buffer, then an all-to-all (NCCL's reduce-scatter would not keep the exact int32 sum
-        followed by the unsharded epilogue)."""
-        world, _ = _group_world_rank(self.group)
-        shape = (world, Ms, self.shard.rows)
-        bufs = self._sp_bufs
-        if bufs is None or bufs[0].shape != shape or bufs[0].device != CA.device:
-            bufs = self._sp_bufs = tuple(torch.empty(shape, device=CA.device, dtype=torch.int32) for _ in range(2))
-        send, recv = bufs
-        if not self.partial_forward(CA, [send]):
-            raise RuntimeError("the int8 GEMM does not serve this shard shape")
-        if world == 1:
-            return send
-        dist.all_to_all_single(recv, send, group=self.group)
-        return recv
 
     def _sp_forward(self, x: torch.Tensor, peers: Optional[PeerPartials] = None) -> torch.Tensor:
         """The sequence-parallel forward: this rank's rows ``[M/w, ..., N]`` of the non-SP output.  The partials of this
-        rank's tokens arrive through :meth:`_sp_exchange` or, with ``peers``, from every rank's scatter GEMM into this
+        rank's tokens arrive through :func:`_sp_exchange` or, with ``peers``, from every rank's scatter GEMM into this
         rank's symmetric ``[world, M/world, N]`` slot."""
         s = self.shard
         world, rank = _group_world_rank(self.group)
         Ms = sp_rows(x, world)
-        if peers is not None and (Ms != peers.M or s.rows != peers.N or peers.dtype != torch.int32):
-            raise ValueError("PeerPartials was built for a different output shape or dtype (int32 partials)")
+        if peers is not None:
+            _check_peers(peers, Ms, s.rows, torch.int32, "output shape or dtype (int32 partials)")
         x_r, world, SCA, CA, cols = self._prologue(x)
         counts = self._outlier_counts(x_r, cols, world)  # before the GEMM: every rank then takes the same route
         mine = slice(rank * Ms, (rank + 1) * Ms)
@@ -1313,12 +1295,12 @@ class RowParallelLinear8bitLt(_RowInputGrad, torch.nn.Module):
             subA, subBT = self._exchange_outliers(x_r, cols, world, counts)
             return self.reduce(parts, SCA, x.dtype, subA, subBT)[mine].view(lead)
         if peers is None:
-            parts = self._sp_exchange(CA, Ms)
+            parts = _sp_exchange(self, CA, Ms, torch.int32, "the int8 GEMM")
             subA, subBT = self._exchange_outliers(x_r, cols, world, counts)
         else:
             parts, bases, handle = peers.slot()
             if not self.partial_scatter(CA, peers.scatter_ptrs(bases, peers.rank * Ms * s.rows * 4)):
-                parts.copy_(self._sp_exchange(CA, Ms))  # the scatter GEMM refused the call: the NCCL route fills it
+                parts.copy_(_sp_exchange(self, CA, Ms, torch.int32, "the int8 GEMM"))  # the scatter GEMM refused
             subA, subBT = self._exchange_outliers(x_r, cols, world, counts)
             handle.barrier(channel=0)  # every rank's rows have landed at their owner
         return self.reduce(parts, SCA[mine], x.dtype, None if subA is None else subA[mine], subBT).view(lead)
@@ -1330,21 +1312,7 @@ def fused_forward_row8(layer: RowParallelLinear8bitLt, x: torch.Tensor, peers: P
     of every rank's symmetric buffer, one barrier publishes them, and each rank reduces its own buffer.  The row
     statistics (a max) and the outlier operands still travel through NCCL.  With ``grad_peers`` an input that requires
     grad gets its gradient, exchanged through symmetric memory."""
-    return _row_route("fused_forward_row8", layer, x, lambda x: _fused_forward_row8(layer, x, peers), grad_peers)
-
-
-def _fused_forward_row8(layer: RowParallelLinear8bitLt, x: torch.Tensor, peers: PeerPartials) -> torch.Tensor:
-    s = layer.shard
-    x_r, _, SCA, CA, cols = layer._prologue(x)
-    M = x_r.shape[0]
-    if M != peers.M or s.rows != peers.N or peers.dtype != torch.int32:
-        raise ValueError("PeerPartials was built for a different output shape or dtype (int32 partials)")
-    local, bases, handle = peers.slot()
-    if not layer.partial_forward(CA, peers.dest_ptrs(bases, peers.rank * M * s.rows * 4)):
-        raise RuntimeError("the int8 GEMM does not serve this shard shape")
-    subA, subBT = layer._exchange_outliers(x_r, cols, peers.world)
-    handle.barrier(channel=0)  # every rank's partial has landed everywhere
-    return layer.reduce(local, SCA, x.dtype, subA, subBT).view(*x.shape[:-1], s.rows)
+    return _fused_route("fused_forward_row8", layer, x, peers, False, grad_peers)
 
 
 def fused_forward_row8_sp(layer: RowParallelLinear8bitLt, x: torch.Tensor, peers: PeerPartials,
@@ -1356,4 +1324,4 @@ def fused_forward_row8_sp(layer: RowParallelLinear8bitLt, x: torch.Tensor, peers
     NCCL route runs instead (:meth:`RowParallelLinear8bitLt._sp_forward`).  With ``grad_peers = PeerInputGrad(M, N,
     x.dtype)`` an input that requires grad gets its gradient: the token rows of ``grad_y`` gathered through symmetric
     memory."""
-    return _row_route("fused_forward_row8_sp", layer, x, lambda x: layer._sp_forward(x, peers), grad_peers)
+    return _fused_route("fused_forward_row8_sp", layer, x, peers, True, grad_peers)

@@ -7,15 +7,7 @@ import torch
 import bitsandbytes_b200.backends.cuda as cb
 import bitsandbytes_b200.parallel as par
 from bitsandbytes_b200.parallel import ColumnParallelLinear8bitLt, RowParallelLinear8bitLt, Shard8bit
-from tests.test_sequence_parallel_cpu import _FakeLib
-
-
-@pytest.fixture
-def fake(monkeypatch):
-    lib = _FakeLib()
-    monkeypatch.setattr(cb, "lib", lib)
-    monkeypatch.setattr(cb, "_stream", lambda t: 0)
-    return lib
+from tests._parallel_sim import fake, simulate  # noqa: F401  (fake: a fixture)
 
 
 def test_dequant_rows_wrapper_checks(fake):
@@ -71,21 +63,11 @@ def world4(monkeypatch, fake):
     MatMul8bitLt.backward and the products run on the CPU."""
     calls = []
 
-    def all_to_all_single(out, inp, group=None):
-        calls.append(("all_to_all_single", tuple(out.shape), tuple(inp.shape)))
-        out.copy_(inp)
-
-    def all_gather_into_tensor(out, inp, group=None):
-        calls.append(("all_gather_into_tensor", tuple(out.shape), tuple(inp.shape)))
-        out.copy_(inp.reshape(1, -1).expand(4, -1).reshape(out.shape))
-
     def dequant_rows(CB, SCB, dtype):
         calls.append(("int8_dequant_rows", tuple(CB.shape), dtype))
         return CB.to(dtype, copy=True).mul_(SCB.unsqueeze(1).mul(1.0 / 127.0))
 
-    monkeypatch.setattr(par, "_group_world_rank", lambda group: (4, 1))
-    monkeypatch.setattr(par.dist, "all_to_all_single", all_to_all_single)
-    monkeypatch.setattr(par.dist, "all_gather_into_tensor", all_gather_into_tensor)
+    simulate(monkeypatch, 4, 1, calls)
     monkeypatch.setattr(par, "reduce_partials", lambda parts, dtype, bias=None: parts.sum(0).to(dtype))
     monkeypatch.setattr(par, "int8_dequant_rows", dequant_rows)
     monkeypatch.setattr(par, "input_grad_dequant_matmul",

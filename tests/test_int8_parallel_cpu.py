@@ -7,6 +7,7 @@ import torch
 import bitsandbytes_b200.backends.cuda as cb
 from bitsandbytes_b200.parallel import (ColumnParallelLinear8bitLt, RowParallelLinear8bitLt, slice_int8_weight,
                                         slice_int8_weight_k)
+from tests._parallel_sim import fake, simulate  # noqa: F401  (fake: a fixture)
 
 
 def _weight(N=64, K=256, seed=3):
@@ -62,31 +63,6 @@ def test_sharding_errors():
         layer.local_input(torch.randn(2, 256))         # the full input to a layer that takes its slice
 
 
-class _FakeLib:
-    def __init__(self):
-        self.calls = []
-
-    def __getattr__(self, name):
-        if not name.startswith("cbnb_b200_"):
-            raise AttributeError(name)
-
-        def call(*args):
-            self.calls.append(name)
-            return 0
-        return call
-
-    def check(self, what=""):
-        pass
-
-
-@pytest.fixture
-def fake(monkeypatch):
-    lib = _FakeLib()
-    monkeypatch.setattr(cb, "lib", lib)
-    monkeypatch.setattr(cb, "_stream", lambda t: 0)
-    return lib
-
-
 def _gemm_args(M=8, N=32, K=64):
     CA = torch.zeros(M, K, dtype=torch.int8)
     CB = torch.zeros(N, K, dtype=torch.int8)
@@ -97,7 +73,7 @@ def test_gemm_multi_out_checks(fake):
     CA, CB, SCA, SCB = _gemm_args()
     i32 = lambda *s: torch.zeros(*s, dtype=torch.int32)  # noqa: E731
     assert cb.int8_gemm_multi_out(CA, CB, None, None, [i32(8, 32)] * 8, 32, None)
-    assert fake.calls == ["cbnb_b200_int8_gemm_multi_out"]
+    assert fake.names() == ["cbnb_b200_int8_gemm_multi_out"]
     with pytest.raises(ValueError, match="between 1 and 8"):
         cb.int8_gemm_multi_out(CA, CB, None, None, [i32(8, 32)] * 9, 32, None)
     with pytest.raises(ValueError, match="between 1 and 8"):
@@ -124,7 +100,7 @@ def test_gemm_multi_out_checks(fake):
         cb.int8_gemm_multi_out(CA, CB, SCA, SCB, [h], 32, torch.float16, subA=torch.zeros(8, 8, dtype=torch.float16))
     with pytest.raises(ValueError, match="dtype"):
         cb.int8_gemm_multi_out(CA, CB, SCA, SCB, [torch.zeros(8, 32)], 32, torch.float32)
-    assert fake.calls == ["cbnb_b200_int8_gemm_multi_out"]
+    assert fake.names() == ["cbnb_b200_int8_gemm_multi_out"]
 
 
 def test_reduce_and_quant_checks(fake):
@@ -140,7 +116,7 @@ def test_reduce_and_quant_checks(fake):
     with pytest.raises(ValueError, match="jpad"):
         cb.int8_outlier_operands(torch.zeros(4, 64, dtype=torch.float16), torch.zeros(32, 64, dtype=torch.int8),
                                  torch.ones(32), torch.arange(5), jpad=4)
-    assert fake.calls == []
+    assert fake.names() == []
 
 
 def _gemm4_args(M=8, N=32, K=64, dtype=torch.bfloat16):
@@ -158,7 +134,7 @@ def test_gemm_4bit_multi_out_checks(fake):
         return cb.gemm_4bit_multi_out(A, B, shapeB, absmax, bs, qt, bias, None, None, None, list(outs), ldc)
 
     assert call() and call(outs=[torch.zeros(8, 32, dtype=torch.bfloat16)])
-    assert fake.calls == ["cbnb_b200_gemm_4bit_multi_out"] * 2
+    assert fake.names() == ["cbnb_b200_gemm_4bit_multi_out"] * 2
     for kwargs, match in [({"bs": 48}, "blocksize"), ({"qt": "int4"}, "quant_type"), ({"shapeB": (32, 128)}, "inner"),
                           ({"outs": []}, "between 1 and 8"), ({"outs": [0x1000] * 9}, "between 1 and 8"),
                           ({"ldc": 31}, "ldc"), ({"bias": torch.zeros(32)}, "bias"),
@@ -167,7 +143,7 @@ def test_gemm_4bit_multi_out_checks(fake):
         with pytest.raises(RuntimeError, match=match):
             call(**kwargs)
     assert not call(A=A.float())  # fp32 activations do not take the wgmma kernel: the caller falls back
-    assert fake.calls == ["cbnb_b200_gemm_4bit_multi_out"] * 2
+    assert fake.names() == ["cbnb_b200_gemm_4bit_multi_out"] * 2
 
 
 def test_destination_checks_keep_each_wrappers_exception(fake):
@@ -185,27 +161,17 @@ def test_destination_checks_keep_each_wrappers_exception(fake):
     for outs, ldc in [([i32] * 9, 32), ([], 32), ([i32], 31), ([torch.zeros(short, dtype=torch.int32)], 32), ([f32], 32)]:
         with pytest.raises(ValueError):
             cb.int8_gemm_multi_out(CA, CB, None, None, outs, ldc, None)
-    assert fake.calls == ["cbnb_b200_gemm_4bit_partial", "cbnb_b200_int8_gemm_multi_out"]
+    assert fake.names() == ["cbnb_b200_gemm_4bit_partial", "cbnb_b200_int8_gemm_multi_out"]
 
 
 @pytest.mark.parametrize("world", [1, 2, 3, 8])
 def test_peer_slots_list_the_own_buffer_first(monkeypatch, world):
     """For every rank of a simulated world, the destination list of a symmetric-memory slot is this rank's own buffer
     at the offset, then the peers' in rank order, and successive steps alternate between the two slots."""
-    import torch.distributed._symmetric_memory as symm_mem
-
     import bitsandbytes_b200.parallel as par
 
-    class Handle:
-        def __init__(self, slot, rank):
-            self.world_size, self.rank = world, rank
-            self.buffer_ptrs = [(slot + 1) * 1_000_000 + r * 10_000 for r in range(world)]
-
     for rank in range(world):
-        made = []
-        monkeypatch.setattr(par, "_group_world_rank", lambda group: (world, rank))
-        monkeypatch.setattr(symm_mem, "empty", lambda shape, dtype, device: torch.empty(shape, dtype=dtype))
-        monkeypatch.setattr(symm_mem, "rendezvous", lambda t, group: made.append(t) or Handle(len(made) - 1, rank))
+        simulate(monkeypatch, world, rank, [])
         gather = par.PeerGather(4, 16, torch.bfloat16, "cpu")
         parts = par.PeerPartials(4, 16, "cpu", dtype=torch.int32)
         assert (gather.M, gather.N, gather.dtype, gather.world, gather.rank) == (4, 16, torch.bfloat16, world, rank)

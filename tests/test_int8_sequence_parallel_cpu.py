@@ -1,44 +1,12 @@
 """CPU tests of the sequence-parallel LLM.int8() layers: the argument checks of the int32 scatter GEMM (against a fake
 library), the rank-order destination list the fused row route hands it, and the layers' shape rules."""
-import ctypes as ct
-
 import pytest
 import torch
 
 import bitsandbytes_b200.backends.cuda as cb
 import bitsandbytes_b200.parallel as par
 from bitsandbytes_b200.parallel import ColumnParallelLinear8bitLt, RowParallelLinear8bitLt, Shard8bit
-
-
-class _FakeLib:
-    """Records every native call; the destination array of a scatter call is read while the call is made."""
-
-    def __init__(self):
-        self.calls = []
-        self.scatter_dests = []
-
-    def __getattr__(self, name):
-        if not name.startswith("cbnb_b200_"):
-            raise AttributeError(name)
-
-        def call(*args):
-            self.calls.append((name, args))
-            if name == "cbnb_b200_int8_gemm_partial_scatter":
-                arr = ct.cast(args[2], ct.POINTER(ct.c_void_p))
-                self.scatter_dests.append([arr[i] for i in range(args[3])])
-            return 0
-        return call
-
-    def check(self, what=""):
-        pass
-
-
-@pytest.fixture
-def fake(monkeypatch):
-    lib = _FakeLib()
-    monkeypatch.setattr(cb, "lib", lib)
-    monkeypatch.setattr(cb, "_stream", lambda t: 0)
-    return lib
+from tests._parallel_sim import fake, simulate  # noqa: F401  (fake: a fixture)
 
 
 def test_scatter_wrapper_checks(fake):
@@ -71,43 +39,17 @@ def test_scatter_wrapper_checks(fake):
     # (CA, CB, outs, n_outs, rows_per_out, M, N, K, ldc, stream)
     assert [args[3:9] for _, args in fake.calls] == [(4, 2, 8, 32, 64, 32), (2, 4, 8, 32, 64, 40),
                                                      (1, 8, 8, 32, 64, 32)]
-    assert fake.scatter_dests[1] == [0x1000, 0x2000]
-
-
-class _Handle:
-    def __init__(self, world, rank, slot):
-        self.world_size, self.rank = world, rank
-        self.buffer_ptrs = [(slot + 1) * 1_000_000 + r * 10_000 for r in range(world)]
-        self.barriers = 0
-
-    def barrier(self, channel=0):
-        self.barriers += 1
+    assert fake.dests[1] == [0x1000, 0x2000]
 
 
 def _simulated_world(monkeypatch, world, rank):
-    """One rank of a simulated world: the collectives check their shapes and copy, the statistics and codes of the row
-    prologue and the reduction are CPU stand-ins, symmetric memory hands out fake addresses."""
-    import torch.distributed._symmetric_memory as symm_mem
-
-    def all_gather_into_tensor(out, inp, group=None):
-        assert out.numel() == world * inp.numel()
-        out.copy_(inp.reshape(1, -1).expand(world, -1).reshape(out.shape))
-
-    def all_to_all_single(out, inp, group=None):
-        assert out.shape == inp.shape
-        out.copy_(inp)
-
-    monkeypatch.setattr(par, "_group_world_rank", lambda group: (world, rank))
-    monkeypatch.setattr(par.dist, "all_gather_into_tensor", all_gather_into_tensor)
-    monkeypatch.setattr(par.dist, "all_to_all_single", all_to_all_single)
-    monkeypatch.setattr(par.dist, "all_reduce", lambda t, op=None, group=None: None)
+    """One rank of a simulated world: the statistics and codes of the row prologue and the reduction are CPU
+    stand-ins."""
+    simulate(monkeypatch, world, rank, [])
     monkeypatch.setattr(par, "int8_row_stats", lambda x, thr: (torch.ones(x.shape[0]), None))
     monkeypatch.setattr(par, "int8_quant_with_stats", lambda x, SCA, thr: torch.zeros(x.shape, dtype=torch.int8))
     monkeypatch.setattr(par, "int8_reduce_partials",
                         lambda parts, SCA, SCB, dtype, bias=None, *a, out=None: parts.sum(0).to(dtype))
-    made = []
-    monkeypatch.setattr(symm_mem, "empty", lambda shape, dtype, device: torch.empty(shape, dtype=dtype))
-    monkeypatch.setattr(symm_mem, "rendezvous", lambda t, group: made.append(t) or _Handle(world, rank, len(made) - 1))
 
 
 def _k_shard(N=32, K=64, world=1, rank=0):
@@ -122,7 +64,7 @@ def test_fused_row_route_scatters_in_rank_order(monkeypatch, fake, world):
     Ms, N, K = 2, 32, 48 * world
     for rank in range(world):
         _simulated_world(monkeypatch, world, rank)
-        fake.scatter_dests.clear()
+        fake.dests.clear()
         layer = RowParallelLinear8bitLt(_k_shard(N, K, world, rank), K, sequence_parallel=True)
         peers = par.PeerPartials(Ms, N, "cpu", dtype=torch.int32)
         assert peers.bufs[0].shape == (world, Ms, N) and peers.bufs[0].dtype == torch.int32
@@ -130,7 +72,7 @@ def test_fused_row_route_scatters_in_rank_order(monkeypatch, fake, world):
             y = par.fused_forward_row8_sp(layer, torch.zeros(world * Ms, K // world, dtype=torch.float16), peers)
             assert y.shape == (Ms, N)
             off = rank * Ms * N * 4
-            assert fake.scatter_dests[step] == [(1 + (step & 1)) * 1_000_000 + s * 10_000 + off for s in range(world)]
+            assert fake.dests[step] == [(1 + (step & 1)) * 1_000_000 + s * 10_000 + off for s in range(world)]
         assert all(h.barriers == (2 if i == 0 else 1) for i, h in enumerate(peers.handles))
 
 

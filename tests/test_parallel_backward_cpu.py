@@ -7,21 +7,13 @@ import torch
 import bitsandbytes_b200.backends.cuda as cb
 import bitsandbytes_b200.parallel as par
 from bitsandbytes_b200.parallel import ColumnParallelLinear4bit, RowParallelLinear4bit, Shard4bit
-from tests.test_sequence_parallel_cpu import _FakeLib
+from tests._parallel_sim import fake, simulate  # noqa: F401  (fake: a fixture)
 
 
 def _shard(N=64, K=128, row0=0):
     return Shard4bit(packed=torch.zeros(N * K // 2, dtype=torch.uint8), absmax=torch.ones(N * K // 64),
                      absmax_8bit=None, absmax_code=None, absmax_offset=None, rows=N, row0=row0, K=K, blocksize=64,
                      quant_type="nf4")
-
-
-@pytest.fixture
-def fake(monkeypatch):
-    lib = _FakeLib()
-    monkeypatch.setattr(cb, "lib", lib)
-    monkeypatch.setattr(cb, "_stream", lambda t: 0)
-    return lib
 
 
 def test_input_grad_wrapper_checks(fake):
@@ -63,17 +55,7 @@ def world4(monkeypatch, fake):
     """A world of 4 seen from rank 1: the collectives record their shapes, the kernels are the fake library's."""
     calls = []
 
-    def all_to_all_single(out, inp, group=None):
-        calls.append(("all_to_all_single", tuple(out.shape), tuple(inp.shape)))
-        out.copy_(inp)
-
-    def all_gather_into_tensor(out, inp, group=None):
-        calls.append(("all_gather_into_tensor", tuple(out.shape), tuple(inp.shape)))
-        out.copy_(inp.reshape(1, -1).expand(4, -1).reshape(out.shape))
-
-    monkeypatch.setattr(par, "_group_world_rank", lambda group: (4, 1))
-    monkeypatch.setattr(par.dist, "all_to_all_single", all_to_all_single)
-    monkeypatch.setattr(par.dist, "all_gather_into_tensor", all_gather_into_tensor)
+    simulate(monkeypatch, 4, 1, calls)
     monkeypatch.setattr(par, "reduce_partials", lambda parts, dtype, bias=None: parts.sum(0).to(dtype))
     monkeypatch.setattr(par, "input_grad_dequant_matmul",
                         lambda G, shard, dtype: torch.zeros(G.shape[0], shard.K, dtype=dtype))

@@ -6,31 +6,7 @@ import torch
 import bitsandbytes_b200.backends.cuda as cb
 import bitsandbytes_b200.parallel as par
 from bitsandbytes_b200.parallel import ColumnParallelLinear4bit, RowParallelLinear4bit, Shard4bit
-
-
-class _FakeLib:
-    def __init__(self):
-        self.calls = []
-
-    def __getattr__(self, name):
-        if not name.startswith("cbnb_b200_"):
-            raise AttributeError(name)
-
-        def call(*args):
-            self.calls.append((name, args))
-            return 0
-        return call
-
-    def check(self, what=""):
-        pass
-
-
-@pytest.fixture
-def fake(monkeypatch):
-    lib = _FakeLib()
-    monkeypatch.setattr(cb, "lib", lib)
-    monkeypatch.setattr(cb, "_stream", lambda t: 0)
-    return lib
+from tests._parallel_sim import fake, simulate  # noqa: F401  (fake: a fixture)
 
 
 def _gemm4_args(M=8, N=32, K=64, dtype=torch.bfloat16):
@@ -73,19 +49,9 @@ def test_scatter_wrapper_checks(fake):
 def test_scatter_destinations_are_in_rank_order(monkeypatch, world):
     """For every rank of a simulated world, the scatter list of a [world, M/world, N] slot is slot r (this rank's) of
     every rank's buffer, in rank order, and successive steps alternate between the two slots."""
-    import torch.distributed._symmetric_memory as symm_mem
-
-    class Handle:
-        def __init__(self, slot, rank):
-            self.world_size, self.rank = world, rank
-            self.buffer_ptrs = [(slot + 1) * 1_000_000 + r * 10_000 for r in range(world)]
-
     Ms, N = 4, 16
     for rank in range(world):
-        made = []
-        monkeypatch.setattr(par, "_group_world_rank", lambda group: (world, rank))
-        monkeypatch.setattr(symm_mem, "empty", lambda shape, dtype, device: torch.empty(shape, dtype=dtype))
-        monkeypatch.setattr(symm_mem, "rendezvous", lambda t, group: made.append(t) or Handle(len(made) - 1, rank))
+        simulate(monkeypatch, world, rank, [])
         peers = par.PeerPartials(Ms, N, "cpu")
         assert peers.bufs[0].shape == (world, Ms, N)
         for step in range(3):
@@ -111,17 +77,7 @@ def test_column_layer_rejects_sp_with_gathered_output():
 @pytest.fixture
 def world4(monkeypatch, fake):
     """A simulated world of 4 on the CPU: the collectives only check their shapes, the reduction sums on the CPU."""
-    def all_to_all_single(out, inp, group=None):
-        assert out.shape == inp.shape
-        out.copy_(inp)
-
-    def all_gather_into_tensor(out, inp, group=None):
-        assert out.numel() == 4 * inp.numel()
-        out.copy_(inp.reshape(1, -1).expand(4, -1).reshape(out.shape))
-
-    monkeypatch.setattr(par, "_group_world_rank", lambda group: (4, 1))
-    monkeypatch.setattr(par.dist, "all_to_all_single", all_to_all_single)
-    monkeypatch.setattr(par.dist, "all_gather_into_tensor", all_gather_into_tensor)
+    simulate(monkeypatch, 4, 1, [])
     monkeypatch.setattr(par, "reduce_partials", lambda parts, dtype, bias=None: parts.sum(0).to(dtype))
     return fake
 
