@@ -8,7 +8,8 @@
 //
 // One warp per output feature n; the 32 lanes split K in 8-element chunks (4 packed bytes,
 // one coalesced 128-byte read per warp per step), kUnroll steps in flight.  Up to MB = 4
-// tokens are accumulated per pass (blockIdx.y walks M in chunks of MB).
+// tokens are accumulated per pass (blockIdx.y walks M in chunks of MB; beyond 65535 chunks, the
+// gridDim.y limit, the launcher covers M in several launches).
 //
 // Numerics are those of the tensor-core path and of dequantize + matmul, not of the
 // reference SIMT kernel (which additionally rounds every product to T,
@@ -79,14 +80,15 @@ struct Scale {
 };
 
 // `lut` = 16 fp32 code values (NF4 / FP4 table, or the caller's `datatype` array for the
-// legacy gemv entry point).  vec_ok: K % 8 == 0 and 16-byte aligned A rows / 4-byte aligned B rows.
+// legacy gemv entry point).  VEC, the vector body: K % 8 == 0, blocksize % 8 == 0, 16-byte aligned A rows and
+// 4-byte aligned B rows; otherwise the scalar body.  A CTA serves up to MB tokens from m_first + blockIdx.y * MB.
 // PART (here and in gemv4_fast_kernel): the partial instance, fp32 sums to the destinations of `out` (store_partial:
 // every one, or each row to its own), no bias.
-template <typename T, bool PART>
+template <typename T, bool PART, bool VEC>
 __device__ __forceinline__ void
     gemv4_simt_body(const T* __restrict__ A, const uint8_t* __restrict__ B, Scale sc,
                       const float* __restrict__ lut16_gmem, int quant_type, typename OutArg<T, PART>::type out,
-                      const T* __restrict__ bias, int M, int N, int K, int ldc, int blocksize, int vec_ok) {
+                      const T* __restrict__ bias, int M, int N, int K, int ldc, int blocksize, int m_first) {
     // power-of-two block sizes (all the API allows) index by shift; anything else divides
     const int log2_bs = ((blocksize & (blocksize - 1)) == 0) ? (31 - __clz(blocksize)) : -1;
     __shared__ float2 lut2[256];
@@ -105,7 +107,7 @@ __device__ __forceinline__ void
 
     const int lane = threadIdx.x & 31;
     const int n = blockIdx.x * kWarpsPerCta + (threadIdx.x >> 5);
-    const int m_base = blockIdx.y * kMB;
+    const int m_base = m_first + blockIdx.y * kMB;
     if (n >= N) return;
     const int mcount = (M - m_base < kMB) ? (M - m_base) : kMB;
 
@@ -115,7 +117,7 @@ __device__ __forceinline__ void
 
     const long long e_row = (long long)n * K;  // flat element index of W[n, 0]
 
-    if (vec_ok) {
+    if constexpr (VEC) {
         const uint8_t* brow = B + (e_row >> 1);
         const int chunks = K >> 3;  // 8-element chunks
         for (int c0 = lane; c0 < chunks; c0 += 32 * kUnroll) {
@@ -295,16 +297,16 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32)
     }
 }
 
-template <typename T, bool PART>
+template <typename T, bool PART, bool VEC>
 __global__ void __launch_bounds__(kWarpsPerCta * 32)
     gemv4_simt_kernel(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
                       const float* absmax_code, const float* absmax_offset, const float* lut16, int quant_type,
                       typename OutArg<T, PART>::type out, const T* bias, int M, int N, int K, int ldc, int blocksize,
-                      int vec_ok) {
+                      int m_first) {
     // the offset is fetched on the device: no host sync on the launch path
     Scale sc{absmax, absmax_8bit, absmax_code,
              (absmax_8bit != nullptr && absmax_offset != nullptr) ? __ldg(absmax_offset) : 0.f};
-    gemv4_simt_body<T, PART>(A, B, sc, lut16, quant_type, out, bias, M, N, K, ldc, blocksize, vec_ok);
+    gemv4_simt_body<T, PART, VEC>(A, B, sc, lut16, quant_type, out, bias, M, N, K, ldc, blocksize, m_first);
 }
 
 } // namespace
@@ -344,11 +346,23 @@ void launch_gemv4_simt(const T* A, const uint8_t* B, const float* absmax, const 
     }
     const bool vec_ok = (K % 8 == 0) && ((reinterpret_cast<uintptr_t>(A) & 15) == 0) &&
                         ((reinterpret_cast<uintptr_t>(B) & 3) == 0) && (blocksize % 8 == 0);
-    dim3 grid((N + kWarpsPerCta - 1) / kWarpsPerCta, (M + kMB - 1) / kMB);
-    gemv4_simt_kernel<T, PART><<<grid, kWarpsPerCta * 32, 0, stream>>>(A, B, absmax, absmax_8bit, absmax_code,
-                                                                 absmax_offset, lut16, quant_type, out, bias, M, N, K,
-                                                                 ldc, blocksize, vec_ok ? 1 : 0);
-    BNB200_CHECK_LAUNCH("gemv4_simt");
+    // gridDim.y is at most 65535: from 262 141 tokens on, M is covered in launches of 65535 groups of kMB tokens,
+    // each told its first token.  (A loop over the groups inside the kernel instead takes the fp32 vector body from
+    // 64 to 170 registers, ptxas -v.)
+    constexpr int kMaxGroups = 65535;
+    const int m_groups = (M - 1) / kMB + 1;
+    for (int g0 = 0; g0 < m_groups; g0 += kMaxGroups) {
+        const dim3 grid((N + kWarpsPerCta - 1) / kWarpsPerCta, m_groups - g0 < kMaxGroups ? m_groups - g0 : kMaxGroups);
+        if (vec_ok)
+            gemv4_simt_kernel<T, PART, true><<<grid, kWarpsPerCta * 32, 0, stream>>>(
+                A, B, absmax, absmax_8bit, absmax_code, absmax_offset, lut16, quant_type, out, bias, M, N, K, ldc,
+                blocksize, g0 * kMB);
+        else
+            gemv4_simt_kernel<T, PART, false><<<grid, kWarpsPerCta * 32, 0, stream>>>(
+                A, B, absmax, absmax_8bit, absmax_code, absmax_offset, lut16, quant_type, out, bias, M, N, K, ldc,
+                blocksize, g0 * kMB);
+        BNB200_CHECK_LAUNCH("gemv4_simt");
+    }
 }
 
 #define INST(T)                                                                                                        \
