@@ -400,6 +400,16 @@ void launch_quantize_blockwise_impl(const float* code, const T* A, float* absmax
 template <typename T, int QT>
 void launch_quantize_blockwise(const float* code, const T* A, float* absmax, uint8_t* out, int blocksize, long long n,
                                cudaStream_t stream) {
+    if (blocksize < 1) {
+        set_last_error_msg("quantize_blockwise: blocksize must be >= 1");
+        return;
+    }
+    // two codes per byte, packed from each block's first element: an odd blocksize would start every other block
+    // in the middle of a byte that the previous block also writes
+    if (QT != kGeneral8bit && (blocksize & 1) != 0) {
+        set_last_error_msg("quantize_blockwise: the 4-bit quantizer needs an even blocksize");
+        return;
+    }
     if (QT == kGeneral8bit) {
         // default: the bracket-table search (bit-identical, CPU-proven and GPU-tested); BNB_B200_Q8_WALK=1 keeps the
         // reference's 7-step walk for A/B measurements
@@ -676,6 +686,10 @@ __global__ void __launch_bounds__(256)
 template <typename T, int QT>
 void launch_dequantize_blockwise(const float* code, const uint8_t* A, const float* absmax, T* out, int blocksize,
                                  long long n, cudaStream_t stream) {
+    if (blocksize < 1) {
+        set_last_error_msg("dequantize_blockwise: blocksize must be >= 1");
+        return;
+    }
     if (n <= 0) return;
     constexpr int OE = 16 / DT<T>::kBytes;
     const bool pow2 = blocksize > 0 && (blocksize & (blocksize - 1)) == 0;

@@ -81,7 +81,7 @@ def quantize(L, A: torch.Tensor, blocksize: int, qt, code=None, dtype="fp32"):
 
 
 def dequantize(L, codes: torch.Tensor, absmax: torch.Tensor, blocksize: int, n: int, qt, code=None, dtype="fp32"):
-    out = torch.zeros(n, device="cuda", dtype=DTYPE[dtype])
+    out = torch.full((n,), float("nan"), device="cuda", dtype=DTYPE[dtype])  # an element never written fails
     suffix = "" if qt is None else f"_{qt}"
     fn = getattr(L, f"cdequantize_blockwise_{dtype}{suffix}")
     fn(ptr(code), ptr(codes), ptr(absmax), ptr(out), blocksize, n, stream())
