@@ -1334,30 +1334,46 @@ def _launch_peers(what, fn, optimizer_name, g0, descs, srcs, dsts, grad_local, p
             raise RuntimeError(f"{what}: native call returned {rc}")
 
 
+def _gnorm_scale_dev(what, gnorm_scale_dev, device):
+    """The address of a device-side gradient factor: a one-element fp32 tensor on the gradients' device."""
+    t = gnorm_scale_dev
+    if (not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or t.numel() != 1 or t.device != device):
+        raise ValueError(f"{what}: gnorm_scale_dev must be a one-element float32 tensor on {device}")
+    return t.data_ptr()
+
+
 def optimizer_update_32bit_multi_peers(optimizer_name, g, p, state1, state2, beta1, beta2, beta3, alpha, eps,
                                        weight_decay, step, lr, grad_srcs, param_dsts, grad_local, param_local,
-                                       grad_scale, skip_zeros=False):
+                                       grad_scale, skip_zeros=False, gnorm_scale_dev=None):
     """optimizer_update_32bit_multi for one data-parallel rank: g and p list pieces of the local flat buffers grad_local
     and param_local; the gradient of each element is the fp32 sum, in rank order, of the buffers at the addresses
     grad_srcs (each laid out as grad_local) times grad_scale, rounded once to the dtype; the new parameters go to each
-    address of param_dsts (laid out as param_local), not to p unless param_local is among them."""
+    address of param_dsts (laid out as param_local), not to p unless param_local is among them.
+
+    gnorm_scale_dev: a one-element fp32 CUDA tensor (a clip coefficient) that the kernel reads and applies as the
+    multi-tensor step applies gnorm_scale; None: 1, no read."""
     what = "optimizer_update_32bit_multi_peers"
     g0, descs, _ = _optimizer_list(what, optimizer_name, _OPTIMIZER_PEERS, g, p, state1, state2, None, None, step, False)
     if descs is None:
         return
     srcs, dsts = _peer_args(what, g, p, step, grad_srcs, param_dsts, grad_local, param_local)
+    scalars = (float(beta1), float(beta2), float(beta3), float(alpha), float(eps), float(weight_decay), float(lr),
+               bool(skip_zeros))
+    fn = lib.cbnb_b200_optimizer_update_32bit_multi_peers
+    if gnorm_scale_dev is not None:
+        what += "_scaled"
+        fn, scalars = (lib.cbnb_b200_optimizer_update_32bit_multi_peers_scaled,
+                       scalars + (_gnorm_scale_dev(what, gnorm_scale_dev, g0.device),))
     with _on_device(g0):
-        _launch_peers(what, lib.cbnb_b200_optimizer_update_32bit_multi_peers, optimizer_name, g0, descs, srcs, dsts,
-                      grad_local, param_local, grad_scale,
-                      (float(beta1), float(beta2), float(beta3), float(alpha), float(eps), float(weight_decay),
-                       float(lr), bool(skip_zeros)))
+        _launch_peers(what, fn, optimizer_name, g0, descs, srcs, dsts, grad_local, param_local, grad_scale, scalars)
 
 
 def optimizer_update_8bit_blockwise_multi_peers(optimizer_name, g, p, state1, state2, beta1, beta2, beta3, alpha, eps,
                                                 step, lr, qmap1, qmap2, absmax1, absmax2, weight_decay, grad_srcs,
-                                                param_dsts, grad_local, param_local, grad_scale, skip_zeros=False):
-    """optimizer_update_8bit_blockwise_multi for one data-parallel rank; the gradient and parameter exchange as
-    optimizer_update_32bit_multi_peers.  Every piece starts on a 256-element block of its tensor."""
+                                                param_dsts, grad_local, param_local, grad_scale, skip_zeros=False,
+                                                gnorm_scale_dev=None):
+    """optimizer_update_8bit_blockwise_multi for one data-parallel rank; the gradient and parameter exchange, and
+    gnorm_scale_dev, as optimizer_update_32bit_multi_peers.  Every piece starts on a 256-element block of its tensor."""
     what = "optimizer_update_8bit_blockwise_multi_peers"
     g0, descs, _ = _optimizer_list(what, optimizer_name, [n for n in _OPTIMIZER_8BIT if n in _OPTIMIZER_PEERS], g, p,
                                    state1, state2, absmax1, absmax2, step, True)
@@ -1368,8 +1384,68 @@ def optimizer_update_8bit_blockwise_multi_peers(optimizer_name, g, p, state1, st
     for q in (qmap1, qmap2) if two else (qmap1,):
         if q is None or q.device != g0.device or not q.is_contiguous() or q.dtype != torch.float32 or q.numel() < 256:
             raise ValueError(f"{what}: the code books must be contiguous fp32 [256] tensors on {g0.device}")
+    scalars = (float(beta1), float(beta2), float(beta3), float(alpha), float(eps), float(weight_decay), float(lr),
+               qmap1.data_ptr(), qmap2.data_ptr() if two else None, bool(skip_zeros))
+    fn = lib.cbnb_b200_optimizer_update_8bit_blockwise_multi_peers
+    if gnorm_scale_dev is not None:
+        what += "_scaled"
+        fn, scalars = (lib.cbnb_b200_optimizer_update_8bit_blockwise_multi_peers_scaled,
+                       scalars + (_gnorm_scale_dev(what, gnorm_scale_dev, g0.device),))
     with _on_device(g0):
-        _launch_peers(what, lib.cbnb_b200_optimizer_update_8bit_blockwise_multi_peers, optimizer_name, g0, descs, srcs,
-                      dsts, grad_local, param_local, grad_scale,
-                      (float(beta1), float(beta2), float(beta3), float(alpha), float(eps), float(weight_decay),
-                       float(lr), qmap1.data_ptr(), qmap2.data_ptr() if two else None, bool(skip_zeros)))
+        _launch_peers(what, fn, optimizer_name, g0, descs, srcs, dsts, grad_local, param_local, grad_scale, scalars)
+
+
+def optimizer_grad_norm_peers(g, grad_srcs, grad_local, grad_scale, norm_type, acc):
+    """Add the norm value of one data-parallel rank's pieces of the reduced gradient into acc (a one-element float64
+    CUDA tensor), on the device: the sum of squares (norm_type 2) or the max |g| (norm_type inf) of every element's
+    gradient T(fp32 rank-order sum over grad_srcs * grad_scale), formed as the peer steps form it.  g lists pieces of
+    the flat buffer grad_local; grad_srcs, as for optimizer_update_32bit_multi_peers.  One launch per capacity chunk,
+    each folding into acc in stream order; nothing is read on the host."""
+    what = "optimizer_grad_norm_peers"
+    inf = _norm_kind(what, norm_type)
+    if not isinstance(acc, torch.Tensor) or acc.dtype != torch.float64 or acc.numel() != 1 or not acc.is_cuda:
+        raise ValueError(f"{what}: acc must be a one-element float64 CUDA tensor")
+    if not g:
+        return
+    if grad_local.dtype not in _DTYPE_ID or not grad_local.is_cuda or acc.device != grad_local.device:
+        raise ValueError(f"{what}: grad_local must be an fp32 / fp16 / bf16 CUDA tensor on acc's device")
+    srcs, _ = _peer_args(what, g, g, [], grad_srcs, [grad_local.data_ptr()], grad_local, grad_local)
+    descs = (cext.OptimTensor * len(g))(*[cext.OptimTensor(0, t.data_ptr(), 0, 0, 0, 0, t.numel(), 0, 0) for t in g])
+    cap, size = optimizer_peers_capacity(), ct.sizeof(cext.OptimTensor)
+    with _on_device(grad_local):
+        for lo in range(0, len(g), cap):
+            rc = lib.cbnb_b200_optimizer_grad_norm_peers(
+                _DTYPE_ID[grad_local.dtype], ct.addressof(descs) + lo * size, min(cap, len(g) - lo),
+                ct.cast(srcs, ct.c_void_p), len(srcs), grad_local.data_ptr(), grad_local.numel(), float(grad_scale),
+                inf, acc.data_ptr(), _stream(grad_local))
+            lib.check(what)
+            if rc != 0:
+                raise RuntimeError(f"{what}: native call returned {rc}")
+
+
+def optimizer_clip_coef(rank_values, norm_type, max_norm, out):
+    """The global gradient norm and clip coefficient from the ranks' values of optimizer_grad_norm_peers (a float64
+    CUDA tensor, rank order), on the device: out (two float32 elements) receives the total norm and the coefficient,
+    the bits of torch's ``(max_norm / (total_norm + 1e-6)).clamp(max=1.0)`` on that fp32 norm."""
+    what = "optimizer_clip_coef"
+    inf = _norm_kind(what, norm_type)
+    if (not isinstance(rank_values, torch.Tensor) or rank_values.dtype != torch.float64 or not rank_values.is_cuda
+            or not rank_values.is_contiguous() or rank_values.numel() < 1):
+        raise ValueError(f"{what}: rank_values must be a contiguous float64 CUDA tensor")
+    if (not isinstance(out, torch.Tensor) or out.dtype != torch.float32 or out.numel() != 2 or not out.is_contiguous()
+            or out.device != rank_values.device):
+        raise ValueError(f"{what}: out must be a contiguous two-element float32 tensor on {rank_values.device}")
+    with _on_device(out):
+        rc = lib.cbnb_b200_optimizer_clip_coef(rank_values.data_ptr(), rank_values.numel(), inf, float(max_norm),
+                                               out.data_ptr(), _stream(out))
+    lib.check(what)
+    if rc != 0:
+        raise RuntimeError(f"{what}: native call returned {rc}")
+
+
+def _norm_kind(what, norm_type) -> bool:
+    """True for the inf norm, False for L2; any other order is refused."""
+    t = float(norm_type)
+    if t not in (2.0, float("inf")):
+        raise ValueError(f"{what}: norm_type must be 2 or inf, got {norm_type}")
+    return t == float("inf")

@@ -167,6 +167,15 @@ def _signatures():
     peers = [_I32, _I32, _VOIDP, _I32, _VOIDP, _I32, _VOIDP, _I32, _VOIDP, _VOIDP, ct.c_longlong] + [_F] * 8
     sig["cbnb_b200_optimizer_update_32bit_multi_peers"] = (peers + [ct.c_bool, _VOIDP], _I32)
     sig["cbnb_b200_optimizer_update_8bit_blockwise_multi_peers"] = (peers + [_VOIDP, _VOIDP, ct.c_bool, _VOIDP], _I32)
+    # the clipped forms: (... skip_zeros, gnorm_scale_dev, stream) -> int
+    sig["cbnb_b200_optimizer_update_32bit_multi_peers_scaled"] = (peers + [ct.c_bool, _VOIDP, _VOIDP], _I32)
+    sig["cbnb_b200_optimizer_update_8bit_blockwise_multi_peers_scaled"] = (peers + [_VOIDP, _VOIDP, ct.c_bool, _VOIDP,
+                                                                                    _VOIDP], _I32)
+    # (dtype, tensors, count, grad_srcs, world, grad_local, numel, grad_scale, inf_norm, acc, stream) -> int
+    sig["cbnb_b200_optimizer_grad_norm_peers"] = ([_I32, _VOIDP, _I32, _VOIDP, _I32, _VOIDP, ct.c_longlong, _F,
+                                                   ct.c_bool, _VOIDP, _VOIDP], _I32)
+    # (rank_values, world, inf_norm, max_norm, out, stream) -> int
+    sig["cbnb_b200_optimizer_clip_coef"] = ([_VOIDP, _I32, ct.c_bool, _F, _VOIDP, _VOIDP], _I32)
     return sig
 
 

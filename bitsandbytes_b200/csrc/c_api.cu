@@ -52,13 +52,18 @@ bool launch_optimizer32bit_list_peers(int opt, int dtype, const OptimTensor* ts,
                                       const void* const* grad_srcs, int world, void* const* param_dsts, int ndst,
                                       const void* grad_local, const void* param_local, float grad_scale, float beta1,
                                       float beta2, float beta3, float alpha, float eps, float wd, float lr,
-                                      bool skip_zeros, cudaStream_t st);
+                                      bool skip_zeros, const float* gnorm_scale_dev, cudaStream_t st);
 bool launch_optimizer8bit_blockwise_list_peers(int opt, int dtype, const OptimTensor* ts, int count,
                                                const void* const* grad_srcs, int world, void* const* param_dsts,
                                                int ndst, const void* grad_local, const void* param_local,
                                                float grad_scale, float beta1, float beta2, float beta3, float alpha,
                                                float eps, float wd, float lr, const float* q1, const float* q2,
-                                               bool skip_zeros, cudaStream_t st);
+                                               bool skip_zeros, const float* gnorm_scale_dev, cudaStream_t st);
+bool launch_optimizer_grad_norm_peers(int dtype, const OptimTensor* ts, int count, const void* const* grad_srcs,
+                                      int world, const void* grad_local, float grad_scale, bool inf, double* acc,
+                                      cudaStream_t st);
+void launch_optimizer_clip_coef(const double* values, int world, bool inf, float max_norm, float* out,
+                                cudaStream_t st);
 
 // PART = true: the partial instances (fp32 accumulators to every destination of an OutList<float>, no bias, no
 // rounding)
@@ -1102,28 +1107,66 @@ static bool optimizer_peers_ok(const char* what, int optimizer, const OptimTenso
     return false;
 }
 
-int cbnb_b200_optimizer_update_32bit_multi_peers(int optimizer, int dtype, const OptimTensor* tensors, int count,
-                                                 const void* const* grad_srcs, int world, void* const* param_dsts,
-                                                 int ndst, const void* grad_local, const void* param_local,
-                                                 long long numel, float grad_scale, float beta1, float beta2,
-                                                 float beta3, float alpha, float eps, float weight_decay, float lr,
-                                                 bool skip_zeros, cudaStream_t stream) {
-    const char* what = "optimizer_update_32bit_multi_peers";
+// count and ids: 100; everything else optimizer_peers_ok checks: 1 (the message set either way)
+static bool optimizer_peers_ids_ok(const char* what, int optimizer, int dtype, const OptimTensor* tensors, int count) {
     if (count < 0 || count > optimizer_peers_capacity() || (count > 0 && tensors == nullptr) || optimizer < 0 ||
         optimizer > 5 || dtype < 0 || dtype > 2) {
         char msg[160];
         snprintf(msg, sizeof(msg), "%s: %d tensors (at most %d per call), optimizer id %d, dtype id %d", what, count,
                  optimizer_peers_capacity(), optimizer, dtype);
         set_last_error_msg(msg);
-        return 100;
+        return false;
     }
+    return true;
+}
+
+static int optimizer_32bit_peers(const char* what, int optimizer, int dtype, const OptimTensor* tensors, int count,
+                                 const void* const* grad_srcs, int world, void* const* param_dsts, int ndst,
+                                 const void* grad_local, const void* param_local, long long numel, float grad_scale,
+                                 float beta1, float beta2, float beta3, float alpha, float eps, float weight_decay,
+                                 float lr, bool skip_zeros, const float* gnorm_scale_dev, cudaStream_t stream) {
+    if (!optimizer_peers_ids_ok(what, optimizer, dtype, tensors, count)) return 100;
     if (!optimizer_peers_ok(what, optimizer, tensors, count, dtype, grad_srcs, world, param_dsts, ndst, grad_local,
                             param_local, numel))
         return 1;
     launch_optimizer32bit_list_peers(optimizer, dtype, tensors, count, grad_srcs, world, param_dsts, ndst, grad_local,
                                      param_local, grad_scale, beta1, beta2, beta3, alpha, eps, weight_decay, lr,
-                                     skip_zeros, stream);
+                                     skip_zeros, gnorm_scale_dev, stream);
     return 0;
+}
+
+static int optimizer_8bit_peers(const char* what, int optimizer, int dtype, const OptimTensor* tensors, int count,
+                                const void* const* grad_srcs, int world, void* const* param_dsts, int ndst,
+                                const void* grad_local, const void* param_local, long long numel, float grad_scale,
+                                float beta1, float beta2, float beta3, float alpha, float eps, float weight_decay,
+                                float lr, const float* quantiles1, const float* quantiles2, bool skip_zeros,
+                                const float* gnorm_scale_dev, cudaStream_t stream) {
+    if (!optimizer_peers_ids_ok(what, optimizer, dtype, tensors, count)) return 100;
+    if (!optimizer_peers_ok(what, optimizer, tensors, count, dtype, grad_srcs, world, param_dsts, ndst, grad_local,
+                            param_local, numel))
+        return 1;
+    if (quantiles1 == nullptr || (optimizer == 0 && quantiles2 == nullptr)) {
+        char msg[160];
+        snprintf(msg, sizeof(msg), "%s: missing code book", what);
+        set_last_error_msg(msg);
+        return 1;
+    }
+    launch_optimizer8bit_blockwise_list_peers(optimizer, dtype, tensors, count, grad_srcs, world, param_dsts, ndst,
+                                              grad_local, param_local, grad_scale, beta1, beta2, beta3, alpha, eps,
+                                              weight_decay, lr, quantiles1, quantiles2, skip_zeros, gnorm_scale_dev,
+                                              stream);
+    return 0;
+}
+
+int cbnb_b200_optimizer_update_32bit_multi_peers(int optimizer, int dtype, const OptimTensor* tensors, int count,
+                                                 const void* const* grad_srcs, int world, void* const* param_dsts,
+                                                 int ndst, const void* grad_local, const void* param_local,
+                                                 long long numel, float grad_scale, float beta1, float beta2,
+                                                 float beta3, float alpha, float eps, float weight_decay, float lr,
+                                                 bool skip_zeros, cudaStream_t stream) {
+    return optimizer_32bit_peers("optimizer_update_32bit_multi_peers", optimizer, dtype, tensors, count, grad_srcs,
+                                 world, param_dsts, ndst, grad_local, param_local, numel, grad_scale, beta1, beta2,
+                                 beta3, alpha, eps, weight_decay, lr, skip_zeros, nullptr, stream);
 }
 
 int cbnb_b200_optimizer_update_8bit_blockwise_multi_peers(int optimizer, int dtype, const OptimTensor* tensors,
@@ -1134,25 +1177,93 @@ int cbnb_b200_optimizer_update_8bit_blockwise_multi_peers(int optimizer, int dty
                                                           float weight_decay, float lr, const float* quantiles1,
                                                           const float* quantiles2, bool skip_zeros,
                                                           cudaStream_t stream) {
-    const char* what = "optimizer_update_8bit_blockwise_multi_peers";
-    if (count < 0 || count > optimizer_peers_capacity() || (count > 0 && tensors == nullptr) || optimizer < 0 ||
-        optimizer > 5 || dtype < 0 || dtype > 2) {
-        char msg[160];
-        snprintf(msg, sizeof(msg), "%s: %d tensors (at most %d per call), optimizer id %d, dtype id %d", what, count,
-                 optimizer_peers_capacity(), optimizer, dtype);
+    return optimizer_8bit_peers("optimizer_update_8bit_blockwise_multi_peers", optimizer, dtype, tensors, count,
+                                grad_srcs, world, param_dsts, ndst, grad_local, param_local, numel, grad_scale, beta1,
+                                beta2, beta3, alpha, eps, weight_decay, lr, quantiles1, quantiles2, skip_zeros,
+                                nullptr, stream);
+}
+
+// The clipped data-parallel steps: as the _peers entries, with the gradient factor (gnorm_scale of the _multi
+// entries) read by each CTA from gnorm_scale_dev in device memory; NULL means 1, the _peers entries' bits.
+int cbnb_b200_optimizer_update_32bit_multi_peers_scaled(int optimizer, int dtype, const OptimTensor* tensors, int count,
+                                                        const void* const* grad_srcs, int world,
+                                                        void* const* param_dsts, int ndst, const void* grad_local,
+                                                        const void* param_local, long long numel, float grad_scale,
+                                                        float beta1, float beta2, float beta3, float alpha, float eps,
+                                                        float weight_decay, float lr, bool skip_zeros,
+                                                        const float* gnorm_scale_dev, cudaStream_t stream) {
+    return optimizer_32bit_peers("optimizer_update_32bit_multi_peers_scaled", optimizer, dtype, tensors, count,
+                                 grad_srcs, world, param_dsts, ndst, grad_local, param_local, numel, grad_scale, beta1,
+                                 beta2, beta3, alpha, eps, weight_decay, lr, skip_zeros, gnorm_scale_dev, stream);
+}
+
+int cbnb_b200_optimizer_update_8bit_blockwise_multi_peers_scaled(
+    int optimizer, int dtype, const OptimTensor* tensors, int count, const void* const* grad_srcs, int world,
+    void* const* param_dsts, int ndst, const void* grad_local, const void* param_local, long long numel,
+    float grad_scale, float beta1, float beta2, float beta3, float alpha, float eps, float weight_decay, float lr,
+    const float* quantiles1, const float* quantiles2, bool skip_zeros, const float* gnorm_scale_dev,
+    cudaStream_t stream) {
+    return optimizer_8bit_peers("optimizer_update_8bit_blockwise_multi_peers_scaled", optimizer, dtype, tensors, count,
+                                grad_srcs, world, param_dsts, ndst, grad_local, param_local, numel, grad_scale, beta1,
+                                beta2, beta3, alpha, eps, weight_decay, lr, quantiles1, quantiles2, skip_zeros,
+                                gnorm_scale_dev, stream);
+}
+
+// The norm of the reduced gradient over one rank's pieces (gradient clipping, optim/sharded.py): each element's
+// gradient is formed as the _peers entries form it; the launch's sum of squares (or max |g|, inf_norm) is added
+// (max-ed) into *acc in fp64, in stream order.  Only each descriptor's g and n are read.
+int cbnb_b200_optimizer_grad_norm_peers(int dtype, const OptimTensor* tensors, int count, const void* const* grad_srcs,
+                                        int world, const void* grad_local, long long numel, float grad_scale,
+                                        bool inf_norm, double* acc, cudaStream_t stream) {
+    const char* what = "optimizer_grad_norm_peers";
+    char msg[200];
+    msg[0] = 0;
+    if (count < 0 || count > optimizer_peers_capacity() || (count > 0 && tensors == nullptr) || dtype < 0 ||
+        dtype > 2) {
+        snprintf(msg, sizeof(msg), "%s: %d tensors (at most %d per call), dtype id %d", what, count,
+                 optimizer_peers_capacity(), dtype);
         set_last_error_msg(msg);
         return 100;
     }
-    if (!optimizer_peers_ok(what, optimizer, tensors, count, dtype, grad_srcs, world, param_dsts, ndst, grad_local,
-                            param_local, numel))
-        return 1;
-    if (quantiles1 == nullptr || (optimizer == 0 && quantiles2 == nullptr)) {
-        set_last_error_msg("optimizer_update_8bit_blockwise_multi_peers: missing code book");
+    const uintptr_t es = dtype == 0 ? 4 : 2;
+    auto misaligned = [](const void* v, uintptr_t a) { return v == nullptr || (reinterpret_cast<uintptr_t>(v) % a); };
+    if (world < 1 || world > optimizer_max_peers() || grad_srcs == nullptr)
+        snprintf(msg, sizeof(msg), "%s: %d gradient sources (1..%d)", what, world, optimizer_max_peers());
+    else if (misaligned(grad_local, es) || numel < 0)
+        snprintf(msg, sizeof(msg), "%s: the local flat gradient must be non-null and aligned to its element", what);
+    else if (misaligned(acc, sizeof(double)))
+        snprintf(msg, sizeof(msg), "%s: the accumulator must be a non-null, aligned double", what);
+    for (int r = 0; !msg[0] && r < world; ++r)
+        if (misaligned(grad_srcs[r], es))
+            snprintf(msg, sizeof(msg), "%s: gradient source %d is null or not aligned to its element", what, r);
+    for (int i = 0; !msg[0] && i < count; ++i) {
+        const long long go = static_cast<const char*>(tensors[i].g) - static_cast<const char*>(grad_local);
+        if (tensors[i].n < 0 || go < 0 || go % (long long)es || go + tensors[i].n * (long long)es > numel * (long long)es)
+            snprintf(msg, sizeof(msg), "%s: tensor %d lies outside the local flat gradient of %lld elements", what, i,
+                     numel);
+    }
+    if (msg[0]) {
+        set_last_error_msg(msg);
         return 1;
     }
-    launch_optimizer8bit_blockwise_list_peers(optimizer, dtype, tensors, count, grad_srcs, world, param_dsts, ndst,
-                                              grad_local, param_local, grad_scale, beta1, beta2, beta3, alpha, eps,
-                                              weight_decay, lr, quantiles1, quantiles2, skip_zeros, stream);
+    return launch_optimizer_grad_norm_peers(dtype, tensors, count, grad_srcs, world, grad_local, grad_scale, inf_norm,
+                                            acc, stream)
+               ? 0
+               : 100;
+}
+
+// The global norm and the clip coefficient from the ranks' values of cbnb_b200_optimizer_grad_norm_peers
+int cbnb_b200_optimizer_clip_coef(const double* rank_values, int world, bool inf_norm, float max_norm, float* out,
+                                  cudaStream_t stream) {
+    if (world < 1 || rank_values == nullptr || reinterpret_cast<uintptr_t>(rank_values) % sizeof(double) ||
+        out == nullptr || reinterpret_cast<uintptr_t>(out) % sizeof(float)) {
+        char msg[160];
+        snprintf(msg, sizeof(msg), "optimizer_clip_coef: %d rank values (at least 1), and non-null aligned buffers",
+                 world);
+        set_last_error_msg(msg);
+        return 1;
+    }
+    launch_optimizer_clip_coef(rank_values, world, inf_norm, max_norm, out, stream);
     return 0;
 }
 

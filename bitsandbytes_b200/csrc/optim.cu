@@ -85,6 +85,7 @@ struct PeerArgs {
     void* p[kMaxPeers];        // parameter destination bases (ndst of them)
     const char* g_local;       // the local flat gradient: a descriptor's g lies at g_local + offset
     const char* p_local;       // the local flat parameters
+    const float* gnorm_scale_dev;  // the clip coefficient in device memory (the _scaled entries); NULL: gnorm_scale
     float grad_scale;
     int w, ndst;
 };
@@ -111,6 +112,15 @@ static_assert(sizeof(OptimScalars) + 5 * sizeof(void*) + 2 * sizeof(float) <= kS
 // the per-launch learning rate: from device memory in the capturable instances when given
 template <bool DEV> __device__ __forceinline__ float launch_lr(const OptimScalars& s, const float* lr_dev) {
     return DEV && lr_dev != nullptr ? *lr_dev : s.lr;
+}
+// the per-launch gradient factor: the peer instances read a clip coefficient from device memory when given, once per
+// CTA, so that a clip computed on the device needs no host round trip
+template <int PEERS, typename L_>
+__device__ __forceinline__ float launch_gnorm_scale(const L_& L, const OptimScalars& s) {
+    if constexpr (PEERS > 0) {
+        if (L.peers.gnorm_scale_dev != nullptr) return *L.peers.gnorm_scale_dev;
+    }
+    return s.gnorm_scale;
 }
 // a descriptor's step: the value (DEV = false) or the device counter it points to
 template <bool DEV> __device__ __forceinline__ int tensor_step(const OptimTensor& d) {
@@ -222,6 +232,109 @@ __device__ __forceinline__ bool peers_aligned(const PeerArgs& P) {
     for (int r = 0; r < P.w; ++r) bits |= reinterpret_cast<uintptr_t>(P.g[r]);
     for (int r = 0; r < P.ndst; ++r) bits |= reinterpret_cast<uintptr_t>(P.p[r]);
     return (bits & 15) == 0;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// The norm of the reduced gradient (gradient clipping over data-parallel ranks)
+// ---------------------------------------------------------------------------------------------------------------
+// peer_norm_kernel forms every element's gradient with peer_grad, the values the peer update will use, and
+// accumulates widen(g)^2 (L2; exact in fp64 for fp32, fp16 and bf16 values) or max |g| (INF; NaN wins) in fp64.  A CTA
+// takes kOpt32Chunk-element chunks of the list, each thread in a fixed order; the block's sum is a fixed shuffle tree,
+// written to partials[blockIdx.x].  peer_norm_add_kernel then adds the partials in index order into *acc, in stream
+// order after earlier launches: the result does not depend on timing, and one value can collect several dtype flats
+// and capacity chunks.  No floating-point atomics.
+constexpr int kNormThreads = 512;
+constexpr int kNormChunk = 4096;  // elements per work item
+
+// fp32 <-> fp64 without flushing subnormals (this file is compiled with --use_fast_math, i.e. -ftz)
+__device__ __forceinline__ double widen64(float v) {
+    double r;
+    asm("cvt.f64.f32 %0, %1;" : "=d"(r) : "f"(v));
+    return r;
+}
+__device__ __forceinline__ float narrow_rn(double v) {
+    float r;
+    asm("cvt.rn.f32.f64 %0, %1;" : "=f"(r) : "d"(v));
+    return r;
+}
+// max with NaN propagation (fmax would drop a NaN)
+__device__ __forceinline__ double nan_max(double a, double b) { return (a != a || a > b) ? a : b; }
+template <bool INF> __device__ __forceinline__ double norm_fold(double acc, double x) {
+    return INF ? nan_max(acc, fabs(x)) : fma(x, x, acc);  // (x * x is exact: the fma rounds only the sum)
+}
+
+template <typename T, int NP, bool INF>
+__global__ void __launch_bounds__(kNormThreads) peer_norm_kernel(const __grid_constant__ PeerOptimList list,
+                                                                 double* partials) {
+    constexpr int K = 16 / (int)sizeof(T);  // elements per 16-byte access
+    __shared__ double wsum[kNormThreads / 32];
+    const PeerArgs& P = list.peers;
+    const bool peers_vec = peers_aligned(P);
+    const long long total = list.start[list.count];
+    double acc = 0.0;
+    int ti = 0;
+    for (long long item = blockIdx.x; item < total; item += gridDim.x) {
+        ti = find_tensor(list, item, ti);
+        const OptimTensor& d = list.t[ti];
+        const long n = d.n;
+        const long goff = static_cast<const char*>(d.g) - P.g_local;
+        const long c0 = (item - list.start[ti]) * kNormChunk;
+        const long c1 = c0 + kNormChunk < n ? c0 + kNormChunk : n;
+        if (peers_vec && (reinterpret_cast<uintptr_t>(d.g) & 15) == 0) {
+            for (long i = c0 + K * threadIdx.x; i < c1; i += K * blockDim.x) {
+                alignas(16) T v[K];
+                peer_grad<T, K, NP>(P, goff, i, n, i + K <= n, v);  // (past n: zeros)
+#pragma unroll
+                for (int j = 0; j < K; ++j) acc = norm_fold<INF>(acc, widen64(widen<T>(v[j])));
+            }
+        } else {
+            for (long i = c0 + threadIdx.x; i < c1; i += blockDim.x) {
+                T v[1];
+                peer_grad<T, 1, NP>(P, goff, i, n, false, v);
+                acc = norm_fold<INF>(acc, widen64(widen<T>(v[0])));
+            }
+        }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const double other = __shfl_xor_sync(0xffffffffu, acc, o);
+        acc = INF ? nan_max(acc, other) : acc + other;
+    }
+    if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = acc;
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        double v = threadIdx.x < (blockDim.x >> 5) ? wsum[threadIdx.x] : 0.0;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const double other = __shfl_xor_sync(0xffffffffu, v, o);
+            v = INF ? nan_max(v, other) : v + other;
+        }
+        if (threadIdx.x == 0) partials[blockIdx.x] = v;
+    }
+}
+
+template <bool INF>
+__global__ void __launch_bounds__(32) peer_norm_add_kernel(const double* partials, int n, double* acc) {
+    if (threadIdx.x != 0) return;
+    double s = *acc;
+    for (int i = 0; i < n; ++i) s = INF ? nan_max(s, partials[i]) : s + partials[i];
+    *acc = s;
+}
+
+// The global norm and the clip coefficient from the w ranks' values (rank order): for L2 the fp64 sum, its fp64
+// square root rounded once to fp32; for INF the max.  The coefficient is, in fp32 and with torch's operations,
+// min((1 / (total_norm + 1e-6)) * max_norm, 1) (`max_norm / t` on a tensor is a reciprocal and a multiply), NaN kept.
+template <bool INF>
+__global__ void __launch_bounds__(32) clip_coef_kernel(const double* values, int w, float max_norm, float* out) {
+    if (threadIdx.x != 0) return;
+    double t = values[0];
+    for (int r = 1; r < w; ++r) t = INF ? nan_max(t, values[r]) : t + values[r];
+    const float norm = narrow_rn(INF ? t : __dsqrt_rn(t));
+    float rcp;
+    asm("rcp.rn.f32 %0, %1;" : "=f"(rcp) : "f"(add_rn(norm, (float)1e-6)));
+    const float coef = mul_rn(rcp, max_norm);
+    out[0] = norm;
+    out[1] = coef > 1.0f ? 1.0f : coef;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -362,7 +475,7 @@ __global__ void __launch_bounds__(512, PEERS > 0 ? 1 : 0) optim32_kernel(const _
     constexpr bool two = OPT == kAdam || OPT == kAdemamix;
     Opt32Args q;
     q.beta1 = s.beta1, q.beta2 = s.beta2, q.beta3 = s.beta3, q.alpha = s.alpha, q.eps = s.eps;
-    q.weight_decay = s.weight_decay, q.lr = launch_lr<DEV>(s, lr_dev), q.gnorm_scale = s.gnorm_scale;
+    q.weight_decay = s.weight_decay, q.lr = launch_lr<DEV>(s, lr_dev), q.gnorm_scale = launch_gnorm_scale<PEERS>(list, s);
     q.skip_zeros = s.skip_zeros;
     q.update_scale = 1.0f;
     if (max_unorm > 0.0f) {
@@ -570,7 +683,7 @@ __global__ void __launch_bounds__(256, PEERS > 0 ? 1 : 0) optim8_2state_kernel(c
                                                             const float* lr_dev) {
     const float beta1 = s.beta1, beta2 = s.beta2, beta3 = s.beta3, alpha = s.alpha, eps = s.eps;
     const float lr = launch_lr<DEV>(s, lr_dev);
-    const float weight_decay = s.weight_decay, gnorm_scale = s.gnorm_scale;
+    const float weight_decay = s.weight_decay, gnorm_scale = launch_gnorm_scale<PEERS>(list, s);
     __shared__ float code1[256];
     __shared__ float code2[256];
     __shared__ float2 fin1[257], fin2[257];
@@ -687,7 +800,7 @@ __global__ void __launch_bounds__(256, PEERS > 0 ? 1 : 0) optim8_1state_kernel(c
                                                             const float* qmap1, const float* lr_dev) {
     const float beta1 = s.beta1, beta2 = s.beta2, eps = s.eps, weight_decay = s.weight_decay;
     const float lr = launch_lr<DEV>(s, lr_dev);
-    const float gnorm_scale = s.gnorm_scale;
+    const float gnorm_scale = launch_gnorm_scale<PEERS>(list, s);
     const bool skip_zeros = s.skip_zeros;
     __shared__ float code1[256];
     __shared__ float2 fin1[257];
@@ -1002,16 +1115,37 @@ bool list_peers(int opt, int dtype, bool eight, const OptimTensor* ts, int count
 }
 
 PeerArgs peer_args(const void* const* grad_srcs, int world, void* const* param_dsts, int ndst, const void* grad_local,
-                   const void* param_local, float grad_scale) {
+                   const void* param_local, float grad_scale, const float* gnorm_scale_dev) {
     PeerArgs P{};
     for (int r = 0; r < world; ++r) P.g[r] = grad_srcs[r];
     for (int r = 0; r < ndst; ++r) P.p[r] = param_dsts[r];
     P.g_local = static_cast<const char*>(grad_local);
     P.p_local = static_cast<const char*>(param_local);
+    P.gnorm_scale_dev = gnorm_scale_dev;
     P.grad_scale = grad_scale;
     P.w = world;
     P.ndst = ndst;
     return P;
+}
+
+template <typename T, bool INF>
+void run_norm(const PeerOptimList& L, int grid, double* partials, cudaStream_t st) {
+    if (L.peers.w <= 1)
+        peer_norm_kernel<T, 1, INF><<<grid, kNormThreads, 0, st>>>(L, partials);
+    else if (L.peers.w <= 2)
+        peer_norm_kernel<T, 2, INF><<<grid, kNormThreads, 0, st>>>(L, partials);
+    else if (L.peers.w <= 4)
+        peer_norm_kernel<T, 4, INF><<<grid, kNormThreads, 0, st>>>(L, partials);
+    else
+        peer_norm_kernel<T, kMaxPeers, INF><<<grid, kNormThreads, 0, st>>>(L, partials);
+}
+
+template <typename T>
+void run_norm(bool inf, const PeerOptimList& L, int grid, double* partials, cudaStream_t st) {
+    if (inf)
+        run_norm<T, true>(L, grid, partials, st);
+    else
+        run_norm<T, false>(L, grid, partials, st);
 }
 
 OptimTensor one_tensor(void* p, const void* g, void* s1, void* s2, float* a1, float* a2, long n, int step) {
@@ -1080,9 +1214,10 @@ bool launch_optimizer32bit_list_peers(int opt, int dtype, const OptimTensor* ts,
                                       const void* const* grad_srcs, int world, void* const* param_dsts, int ndst,
                                       const void* grad_local, const void* param_local, float grad_scale, float beta1,
                                       float beta2, float beta3, float alpha, float eps, float wd, float lr,
-                                      bool skip_zeros, cudaStream_t st) {
+                                      bool skip_zeros, const float* gnorm_scale_dev, cudaStream_t st) {
     const OptimScalars s{beta1, beta2, beta3, alpha, eps, wd, lr, 1.0f, skip_zeros};
-    const PeerArgs P = peer_args(grad_srcs, world, param_dsts, ndst, grad_local, param_local, grad_scale);
+    const PeerArgs P =
+        peer_args(grad_srcs, world, param_dsts, ndst, grad_local, param_local, grad_scale, gnorm_scale_dev);
     return list_peers(opt, dtype, false, ts, count, s, nullptr, nullptr, P, st);
 }
 
@@ -1091,10 +1226,51 @@ bool launch_optimizer8bit_blockwise_list_peers(int opt, int dtype, const OptimTe
                                                int ndst, const void* grad_local, const void* param_local,
                                                float grad_scale, float beta1, float beta2, float beta3, float alpha,
                                                float eps, float wd, float lr, const float* q1, const float* q2,
-                                               bool skip_zeros, cudaStream_t st) {
+                                               bool skip_zeros, const float* gnorm_scale_dev, cudaStream_t st) {
     const OptimScalars s{beta1, beta2, beta3, alpha, eps, wd, lr, 1.0f, skip_zeros};
-    const PeerArgs P = peer_args(grad_srcs, world, param_dsts, ndst, grad_local, param_local, grad_scale);
+    const PeerArgs P =
+        peer_args(grad_srcs, world, param_dsts, ndst, grad_local, param_local, grad_scale, gnorm_scale_dev);
     return list_peers(opt, dtype, true, ts, count, s, q1, q2, P, st);
+}
+
+// count <= optimizer_peers_capacity(), 1 <= world <= kMaxPeers, dtype 0..2: adds the launch's norm value into *acc.
+// false, with the error message set, when the partials' scratch cannot be allocated.
+bool launch_optimizer_grad_norm_peers(int dtype, const OptimTensor* ts, int count, const void* const* grad_srcs,
+                                      int world, const void* grad_local, float grad_scale, bool inf, double* acc,
+                                      cudaStream_t st) {
+    PeerOptimList L;
+    L.peers = peer_args(grad_srcs, world, nullptr, 0, grad_local, grad_local, grad_scale, nullptr);
+    const long long items = make_list(L, ts, count, kNormChunk);
+    if (items == 0) return true;
+    const int grid = grid_for(items, 1);
+    // stream-ordered scratch: no host synchronisation, and launches on other streams never share it
+    double* partials = nullptr;
+    if (cudaMallocAsync(reinterpret_cast<void**>(&partials), grid * sizeof(double), st) != cudaSuccess) {
+        (void)cudaGetLastError();
+        set_last_error_msg("optimizer_grad_norm_peers: could not allocate the partials' scratch");
+        return false;
+    }
+    switch (dtype) {
+    case 0: run_norm<float>(inf, L, grid, partials, st); break;
+    case 1: run_norm<__half>(inf, L, grid, partials, st); break;
+    default: run_norm<__nv_bfloat16>(inf, L, grid, partials, st); break;
+    }
+    if (inf)
+        peer_norm_add_kernel<true><<<1, 32, 0, st>>>(partials, grid, acc);
+    else
+        peer_norm_add_kernel<false><<<1, 32, 0, st>>>(partials, grid, acc);
+    cudaFreeAsync(partials, st);
+    BNB200_CHECK_LAUNCH("optimizer_grad_norm_peers");
+    return true;
+}
+
+void launch_optimizer_clip_coef(const double* values, int world, bool inf, float max_norm, float* out,
+                                cudaStream_t st) {
+    if (inf)
+        clip_coef_kernel<true><<<1, 32, 0, st>>>(values, world, max_norm, out);
+    else
+        clip_coef_kernel<false><<<1, 32, 0, st>>>(values, world, max_norm, out);
+    BNB200_CHECK_LAUNCH("optimizer_clip_coef");
 }
 
 } // namespace bnb200

@@ -24,6 +24,14 @@ element falls in the loop; the sharded parameters and state are then within a fe
 
 A parameter without a gradient at ``step()`` is updated with a zero gradient, as DDP's ``find_unused_parameters``
 reduces zeros; the unsharded optimizer would skip it instead.
+
+``clip_grad_norm_(max_norm, norm_type=2.0)`` clips the global norm of the reduced gradient, which no rank holds (each
+``p.grad`` is the rank's local gradient, so ``torch.nn.utils.clip_grad_norm_`` would clip by a local norm).  It does
+the step's exchange early, runs a norm kernel over the rank's pieces that forms each element's gradient exactly as the
+update will and accumulates in fp64, all-gathers one value per rank, and computes the norm and torch's coefficient
+on the device.  ``step()`` then skips the exchange and hands the coefficient's address to the update kernels, which
+apply it as the unsharded kernels apply ``gnorm_scale``: the step equals the unsharded optimizer's fed the reduced
+gradient with ``gnorm_scale`` = the coefficient.
 """
 from __future__ import annotations
 
@@ -32,7 +40,8 @@ from typing import Optional
 import torch
 import torch.distributed as dist
 
-from ..backends.cuda import optimizer_update_32bit_multi_peers, optimizer_update_8bit_blockwise_multi_peers
+from ..backends.cuda import (optimizer_clip_coef, optimizer_grad_norm_peers, optimizer_update_32bit_multi_peers,
+                             optimizer_update_8bit_blockwise_multi_peers)
 from ..parallel import _group_world_rank
 from .optimizer import _STATE_BLOCK, Optimizer2State, Optimizer8bit, _Update, group_updates
 
@@ -128,6 +137,7 @@ class ShardedOptimizer(torch.optim.Optimizer):
         for i, (_, _, p, _) in enumerate(self.entries):
             by_dtype.setdefault(p.dtype, []).append(i)
         self.flats, self.steps = [], [0] * len(self.entries)
+        self._clip = None  # (gradient sources, coefficient) from clip_grad_norm_ until the step that uses them
         for dtype, idx in by_dtype.items():
             flat = _Flat([self.entries[i][2] for i in idx], dtype, self.device, self.world, self.rank)
             flat.index = idx
@@ -210,54 +220,113 @@ class ShardedOptimizer(torch.optim.Optimizer):
             updates.append(u)
         return group_updates(updates)
 
-    def _launch(self, batch, srcs, dsts) -> None:
+    def _launch(self, batch, srcs, dsts, coef=None) -> None:
         u, st = batch[0], batch[0].state
         flat = u.flat
         g, p = [b.g for b in batch], [b.p for b in batch]
         s1 = [b.state["state1"] for b in batch]
         s2 = [b.state["state2"] for b in batch] if "state2" in st else None
         steps = [b.state["step"] for b in batch]
+        scaled = {} if coef is None else {"gnorm_scale_dev": coef}  # (no clip: the unscaled entries, as before)
         if st["state1"].dtype == torch.float32:
             optimizer_update_32bit_multi_peers(u.name, g, p, s1, s2, u.beta1, u.beta2, u.beta3, u.alpha, u.eps,
                                                u.weight_decay, steps, u.lr, srcs, dsts, flat.grad, flat.param,
-                                               self.grad_scale, skip_zeros=u.skip_zeros)
+                                               self.grad_scale, skip_zeros=u.skip_zeros, **scaled)
         else:
             a1 = [b.state["absmax1"] for b in batch]
             a2 = [b.state["absmax2"] for b in batch] if s2 is not None else None
             optimizer_update_8bit_blockwise_multi_peers(u.name, g, p, s1, s2, u.beta1, u.beta2, u.beta3, u.alpha,
                                                         u.eps, steps, u.lr, st["qmap1"], st.get("qmap2"), a1, a2,
                                                         u.weight_decay, srcs, dsts, flat.grad, flat.param,
-                                                        self.grad_scale, skip_zeros=u.skip_zeros)
+                                                        self.grad_scale, skip_zeros=u.skip_zeros, **scaled)
+
+    @torch.no_grad()
+    def clip_grad_norm_(self, max_norm: float, norm_type: float = 2.0, error_if_nonfinite: bool = False):
+        """Clip the global norm of the reduced gradient to ``max_norm``, as FSDP's method of the same name; call it
+        between ``backward()`` and ``step()``.  Returns the total norm, a 0-dim fp32 CUDA tensor with the same bits on
+        every rank.
+
+        The gradients are exchanged now (the ``all_to_all_single`` of the step, which ``step()`` then skips).  One
+        kernel per flat buffer forms this rank's elements of the reduced gradient exactly as the update will, and
+        accumulates their squares (norm_type 2) or max |g| (inf) in fp64; an ``all_gather_into_tensor`` of one value per
+        rank and a one-thread kernel give the norm, ``sqrt`` of the rank-order sum rounded once to fp32, and the
+        coefficient ``(max_norm / (total_norm + 1e-6)).clamp(max=1.0)``, torch's bits on that norm.  The coefficient
+        stays in device memory; ``step()`` hands its address to the update kernels, which apply it as the unsharded
+        kernels apply ``gnorm_scale``.  Nothing is read on the host, unless ``error_if_nonfinite``: then a non-finite
+        norm raises ``RuntimeError`` (one synchronisation), and ``step()`` would exchange the gradients afresh.
+
+        Unlike ``torch.nn.utils.clip_grad_norm_``: ``p.grad`` is not modified (the local gradients are not the reduced
+        ones; the coefficient is applied inside the update); the norm is computed in fp64 from the reduced gradient and
+        returned in fp32, where torch computes per-tensor norms in the gradient's dtype.  Calling torch's function on a
+        sharded model's parameters clips each rank's local gradients by a local norm, which is not this step.
+
+        ``step()`` uses the gradients as they were here.  A NaN or Inf gradient gives a NaN or Inf norm and torch's
+        coefficient for it (NaN or 0), which the update then applies."""
+        if not isinstance(norm_type, (int, float)) or float(norm_type) not in (2.0, float("inf")):
+            raise ValueError(f"clip_grad_norm_: norm_type must be 2 or inf, got {norm_type!r}")
+        if self._clip is not None:
+            raise RuntimeError("clip_grad_norm_ was already called for this step: call step() first")
+        self._gather_grads()
+        srcs = self._exchange_grads()
+        acc = torch.zeros(1, dtype=torch.float64, device=self.device)
+        for f in self.flats:
+            g = [f.grad[s:s + n] for flat, _, s, n, _ in self.pieces if flat is f]
+            optimizer_grad_norm_peers(g, srcs[id(f)], f.grad, self.grad_scale, norm_type, acc)
+        if self.world > 1:
+            every = torch.empty(self.world, dtype=torch.float64, device=self.device)
+            dist.all_gather_into_tensor(every, acc, group=self.group)
+        else:
+            every = acc
+        out = torch.empty(2, dtype=torch.float32, device=self.device)
+        optimizer_clip_coef(every, norm_type, max_norm, out)
+        total = out[0]
+        if error_if_nonfinite and not torch.isfinite(total).item():
+            raise RuntimeError(f"The total norm of order {float(norm_type)} for gradients from `parameters` is "
+                               "non-finite, so it cannot be clipped. To disable this error and scale the gradients "
+                               "by the non-finite norm anyway, set `error_if_nonfinite=False`")
+        self._clip = (srcs, out[1:])
+        return total
 
     @torch.no_grad()
     def step(self, closure=None):
+        if closure is not None and self._clip is not None:
+            raise RuntimeError("step(closure) after clip_grad_norm_: the closure would recompute gradients that were "
+                               "already exchanged and clipped")
         loss = None
         if closure is not None:
             with torch.enable_grad():
                 loss = closure()
-        self._gather_grads()
+        clip, self._clip = self._clip, None
+        if clip is None:
+            self._gather_grads()
         self.steps = [k + 1 for k in self.steps]
         batches = self._updates()
-        self._exchange(batches)
+        self._exchange(batches, clip)
         return loss
 
-    def _exchange(self, batches) -> None:
-        """Gradients in by all-to-all, one launch per batch of pieces, parameters out by all-gather."""
-        if self.world == 1:  # nothing to exchange: the local gradient is the only source
-            for batch in batches:
-                f = batch[0].flat
-                self._launch(batch, [f.grad.data_ptr()], [f.param.data_ptr()])
-            return
+    def _exchange_grads(self):
+        """Gradients in by all-to-all: id(flat) -> the w gradient source addresses of this rank's pieces."""
         srcs = {}
         for f in self.flats:
+            if self.world == 1:  # nothing to exchange: the local gradient is the only source
+                srcs[id(f)] = [f.grad.data_ptr()]
+                continue
             if f.recv is None:
                 f.recv = torch.empty_like(f.grad)
             dist.all_to_all_single(f.recv, f.grad, group=self.group)
             es, s0 = f.grad.element_size(), self.rank * f.S
             srcs[id(f)] = [f.recv.data_ptr() + (r * f.S - s0) * es for r in range(self.world)]
+        return srcs
+
+    def _exchange(self, batches, clip=None) -> None:
+        """Gradients in (unless clip_grad_norm_ exchanged them: clip = (sources, coefficient)), one launch per batch of
+        pieces, parameters out by all-gather."""
+        srcs, coef = clip if clip is not None else (self._exchange_grads(), None)
         for batch in batches:
             f = batch[0].flat
-            self._launch(batch, srcs[id(f)], [f.param.data_ptr()])
+            self._launch(batch, srcs[id(f)], [f.param.data_ptr()], coef)
+        if self.world == 1:
+            return
         for f in self.flats:
             s0 = self.rank * f.S
             dist.all_gather_into_tensor(f.param, f.param[s0:s0 + f.S], group=self.group)

@@ -365,6 +365,28 @@ int cbnb_b200_optimizer_update_8bit_blockwise_multi_dev(int optimizer, int dtype
 int cbnb_b200_optimizer_peers_capacity(void);
 int cbnb_b200_optimizer_update_32bit_multi_peers(int optimizer, int dtype, const bnb_b200_optim_tensor_t* tensors, int count, const void* const* grad_srcs, int world, void* const* param_dsts, int ndst, const void* grad_local, const void* param_local, long long numel, float grad_scale, float beta1, float beta2, float beta3, float alpha, float eps, float weight_decay, float lr, bool skip_zeros, bnb_stream_t stream);
 int cbnb_b200_optimizer_update_8bit_blockwise_multi_peers(int optimizer, int dtype, const bnb_b200_optim_tensor_t* tensors, int count, const void* const* grad_srcs, int world, void* const* param_dsts, int ndst, const void* grad_local, const void* param_local, long long numel, float grad_scale, float beta1, float beta2, float beta3, float alpha, float eps, float weight_decay, float lr, const float* quantiles1, const float* quantiles2, bool skip_zeros, bnb_stream_t stream);
+/* Clipped data-parallel steps: the _peers entries plus gnorm_scale_dev, an fp32 factor in device memory (the clip
+ * coefficient of cbnb_b200_optimizer_clip_coef) that every CTA reads once and applies where the _multi entries apply
+ * gnorm_scale: the results are those of the _multi entries on the reduced gradient with gnorm_scale = *gnorm_scale_dev,
+ * bit for bit (fp32 32-bit Lion: as the _peers entries).  NULL means 1: the _peers entries' bits.  Return codes and
+ * checks as the _peers entries. */
+int cbnb_b200_optimizer_update_32bit_multi_peers_scaled(int optimizer, int dtype, const bnb_b200_optim_tensor_t* tensors, int count, const void* const* grad_srcs, int world, void* const* param_dsts, int ndst, const void* grad_local, const void* param_local, long long numel, float grad_scale, float beta1, float beta2, float beta3, float alpha, float eps, float weight_decay, float lr, bool skip_zeros, const float* gnorm_scale_dev, bnb_stream_t stream);
+int cbnb_b200_optimizer_update_8bit_blockwise_multi_peers_scaled(int optimizer, int dtype, const bnb_b200_optim_tensor_t* tensors, int count, const void* const* grad_srcs, int world, void* const* param_dsts, int ndst, const void* grad_local, const void* param_local, long long numel, float grad_scale, float beta1, float beta2, float beta3, float alpha, float eps, float weight_decay, float lr, const float* quantiles1, const float* quantiles2, bool skip_zeros, const float* gnorm_scale_dev, bnb_stream_t stream);
+/* The norm of the reduced gradient over one rank's pieces, for global gradient clipping: each element's gradient is
+ * T(fp32 rank-order sum of the world sources * grad_scale), formed as the _peers entries form it, and the call adds
+ * the sum of its squares (inf_norm: takes the max of |g|, NaN kept) in fp64 into *acc, in stream order after earlier
+ * work: a rank's flats and capacity chunks fold into one value.  Deterministic (fixed per-CTA partials, summed in
+ * index order; no floating-point atomics), no host synchronisation.  Only each descriptor's g and n are read; the
+ * pieces must lie inside [grad_local, + numel).  Return 0; 100 for a bad count or dtype id, or when the partials'
+ * scratch cannot be allocated; 1 for a bad source, base, accumulator or piece -- with the message set and nothing
+ * launched. */
+int cbnb_b200_optimizer_grad_norm_peers(int dtype, const bnb_b200_optim_tensor_t* tensors, int count, const void* const* grad_srcs, int world, const void* grad_local, long long numel, float grad_scale, bool inf_norm, double* acc, bnb_stream_t stream);
+/* The global norm and clip coefficient from the world ranks' accumulated values (device memory, rank order): out[0] =
+ * the fp32 total norm (L2: fp64 rank-order sum, fp64 sqrt, rounded once; inf_norm: the max); out[1] = the
+ * coefficient, the bits of torch's (max_norm / (out[0] + 1e-6)).clamp(max=1.0) on an fp32 tensor (NaN kept).  One
+ * tiny kernel, no host synchronisation.  Return 0, or 1 with the message set for world < 1 or a null / misaligned
+ * buffer. */
+int cbnb_b200_optimizer_clip_coef(const double* rank_values, int world, bool inf_norm, float max_norm, float* out, bnb_stream_t stream);
 
 #ifdef __cplusplus
 }
