@@ -1299,8 +1299,9 @@ def optimizer_peers_capacity() -> int:
 
 
 def _peer_args(what, g, p, step, grad_srcs, param_dsts, grad_local, param_local):
-    """Check the peer arguments: 1..8 sources and destinations (addresses), the local flat buffers holding every piece
-    (g[i] inside grad_local, p[i] inside param_local) and host steps.  Returns the two address arrays."""
+    """Check the peer arguments: 1..8 sources and destinations (addresses) and the local flat buffers holding every
+    piece (g[i] inside grad_local, p[i] inside param_local).  Returns the two address arrays.  (step, host steps or
+    device counters, is checked by _optimizer_list.)"""
     srcs, dsts = [int(a) for a in grad_srcs], [int(a) for a in param_dsts]
     if not 1 <= len(srcs) <= 8 or not 1 <= len(dsts) <= 8:
         raise ValueError(f"{what}: {len(srcs)} gradient sources and {len(dsts)} parameter destinations (1..8 each)")
@@ -1316,8 +1317,6 @@ def _peer_args(what, g, p, step, grad_srcs, param_dsts, grad_local, param_local)
             off = t.data_ptr() - flat.data_ptr()
             if t.dtype != flat.dtype or off < 0 or off % es or off // es + t.numel() > flat.numel():
                 raise ValueError(f"{what}: piece {i} is not a {flat.dtype} view inside the local flat buffers")
-    if any(isinstance(s, torch.Tensor) for s in step):
-        raise ValueError(f"{what}: the data-parallel step takes host steps (no capturable form)")
     return (ct.c_void_p * len(srcs))(*srcs), (ct.c_void_p * len(dsts))(*dsts)
 
 
@@ -1342,6 +1341,20 @@ def _gnorm_scale_dev(what, gnorm_scale_dev, device):
     return t.data_ptr()
 
 
+def _peers_entry(what, dev, lr, gnorm_scale_dev, device):
+    """(name, lr, trailing pointer arguments) of the entry a data-parallel step calls: ``what``_dev for device steps
+    (dev: lr may be a tensor, lr_dev; the coefficient may be NULL), ``what``_scaled with a coefficient, else ``what``."""
+    if dev:
+        what += "_dev"
+        lr, lr_dev = _device_lr(what, lr, device)
+        coef = None if gnorm_scale_dev is None else _gnorm_scale_dev(what, gnorm_scale_dev, device)
+        return what, lr, (coef, lr_dev)
+    if gnorm_scale_dev is None:
+        return what, float(lr), ()
+    what += "_scaled"
+    return what, float(lr), (_gnorm_scale_dev(what, gnorm_scale_dev, device),)
+
+
 def optimizer_update_32bit_multi_peers(optimizer_name, g, p, state1, state2, beta1, beta2, beta3, alpha, eps,
                                        weight_decay, step, lr, grad_srcs, param_dsts, grad_local, param_local,
                                        grad_scale, skip_zeros=False, gnorm_scale_dev=None):
@@ -1351,21 +1364,23 @@ def optimizer_update_32bit_multi_peers(optimizer_name, g, p, state1, state2, bet
     address of param_dsts (laid out as param_local), not to p unless param_local is among them.
 
     gnorm_scale_dev: a one-element fp32 CUDA tensor (a clip coefficient) that the kernel reads and applies as the
-    multi-tensor step applies gnorm_scale; None: 1, no read."""
+    multi-tensor step applies gnorm_scale; None: 1, no read.
+
+    Capturable route: when the steps are one-element int32 CUDA tensors (each its own), the kernels read them on the
+    device and lr may be a one-element fp32 CUDA tensor, as in optimizer_update_32bit_multi; but this call does not
+    advance the steps: the caller advances them, on every rank, before the call.  Nothing is read on the host."""
     what = "optimizer_update_32bit_multi_peers"
-    g0, descs, _ = _optimizer_list(what, optimizer_name, _OPTIMIZER_PEERS, g, p, state1, state2, None, None, step, False)
+    g0, descs, dev = _optimizer_list(what, optimizer_name, _OPTIMIZER_PEERS, g, p, state1, state2, None, None, step,
+                                     False)
     if descs is None:
         return
     srcs, dsts = _peer_args(what, g, p, step, grad_srcs, param_dsts, grad_local, param_local)
-    scalars = (float(beta1), float(beta2), float(beta3), float(alpha), float(eps), float(weight_decay), float(lr),
-               bool(skip_zeros))
-    fn = lib.cbnb_b200_optimizer_update_32bit_multi_peers
-    if gnorm_scale_dev is not None:
-        what += "_scaled"
-        fn, scalars = (lib.cbnb_b200_optimizer_update_32bit_multi_peers_scaled,
-                       scalars + (_gnorm_scale_dev(what, gnorm_scale_dev, g0.device),))
+    what, lr, tail = _peers_entry(what, dev, lr, gnorm_scale_dev, g0.device)
+    scalars = (float(beta1), float(beta2), float(beta3), float(alpha), float(eps), float(weight_decay), lr,
+               bool(skip_zeros)) + tail
     with _on_device(g0):
-        _launch_peers(what, fn, optimizer_name, g0, descs, srcs, dsts, grad_local, param_local, grad_scale, scalars)
+        _launch_peers(what, getattr(lib, "cbnb_b200_" + what), optimizer_name, g0, descs, srcs, dsts, grad_local,
+                      param_local, grad_scale, scalars)
 
 
 def optimizer_update_8bit_blockwise_multi_peers(optimizer_name, g, p, state1, state2, beta1, beta2, beta3, alpha, eps,
@@ -1373,9 +1388,10 @@ def optimizer_update_8bit_blockwise_multi_peers(optimizer_name, g, p, state1, st
                                                 param_dsts, grad_local, param_local, grad_scale, skip_zeros=False,
                                                 gnorm_scale_dev=None):
     """optimizer_update_8bit_blockwise_multi for one data-parallel rank; the gradient and parameter exchange, and
-    gnorm_scale_dev, as optimizer_update_32bit_multi_peers.  Every piece starts on a 256-element block of its tensor."""
+    gnorm_scale_dev and device steps (and lr), as optimizer_update_32bit_multi_peers.  Every piece starts on a
+    256-element block of its tensor."""
     what = "optimizer_update_8bit_blockwise_multi_peers"
-    g0, descs, _ = _optimizer_list(what, optimizer_name, [n for n in _OPTIMIZER_8BIT if n in _OPTIMIZER_PEERS], g, p,
+    g0, descs, dev = _optimizer_list(what, optimizer_name, [n for n in _OPTIMIZER_8BIT if n in _OPTIMIZER_PEERS], g, p,
                                    state1, state2, absmax1, absmax2, step, True)
     if descs is None:
         return
@@ -1384,15 +1400,12 @@ def optimizer_update_8bit_blockwise_multi_peers(optimizer_name, g, p, state1, st
     for q in (qmap1, qmap2) if two else (qmap1,):
         if q is None or q.device != g0.device or not q.is_contiguous() or q.dtype != torch.float32 or q.numel() < 256:
             raise ValueError(f"{what}: the code books must be contiguous fp32 [256] tensors on {g0.device}")
-    scalars = (float(beta1), float(beta2), float(beta3), float(alpha), float(eps), float(weight_decay), float(lr),
-               qmap1.data_ptr(), qmap2.data_ptr() if two else None, bool(skip_zeros))
-    fn = lib.cbnb_b200_optimizer_update_8bit_blockwise_multi_peers
-    if gnorm_scale_dev is not None:
-        what += "_scaled"
-        fn, scalars = (lib.cbnb_b200_optimizer_update_8bit_blockwise_multi_peers_scaled,
-                       scalars + (_gnorm_scale_dev(what, gnorm_scale_dev, g0.device),))
+    what, lr, tail = _peers_entry(what, dev, lr, gnorm_scale_dev, g0.device)
+    scalars = (float(beta1), float(beta2), float(beta3), float(alpha), float(eps), float(weight_decay), lr,
+               qmap1.data_ptr(), qmap2.data_ptr() if two else None, bool(skip_zeros)) + tail
     with _on_device(g0):
-        _launch_peers(what, fn, optimizer_name, g0, descs, srcs, dsts, grad_local, param_local, grad_scale, scalars)
+        _launch_peers(what, getattr(lib, "cbnb_b200_" + what), optimizer_name, g0, descs, srcs, dsts, grad_local,
+                      param_local, grad_scale, scalars)
 
 
 def optimizer_grad_norm_peers(g, grad_srcs, grad_local, grad_scale, norm_type, acc):

@@ -171,6 +171,10 @@ def _signatures():
     sig["cbnb_b200_optimizer_update_32bit_multi_peers_scaled"] = (peers + [ct.c_bool, _VOIDP, _VOIDP], _I32)
     sig["cbnb_b200_optimizer_update_8bit_blockwise_multi_peers_scaled"] = (peers + [_VOIDP, _VOIDP, ct.c_bool, _VOIDP,
                                                                                     _VOIDP], _I32)
+    # the capturable forms (descriptors with step_ptr): (... skip_zeros, gnorm_scale_dev, lr_dev, stream) -> int
+    sig["cbnb_b200_optimizer_update_32bit_multi_peers_dev"] = (peers + [ct.c_bool] + [_VOIDP] * 3, _I32)
+    sig["cbnb_b200_optimizer_update_8bit_blockwise_multi_peers_dev"] = (peers + [_VOIDP, _VOIDP, ct.c_bool]
+                                                                        + [_VOIDP] * 3, _I32)
     # (dtype, tensors, count, grad_srcs, world, grad_local, numel, grad_scale, inf_norm, acc, stream) -> int
     sig["cbnb_b200_optimizer_grad_norm_peers"] = ([_I32, _VOIDP, _I32, _VOIDP, _I32, _VOIDP, ct.c_longlong, _F,
                                                    ct.c_bool, _VOIDP, _VOIDP], _I32)

@@ -52,13 +52,15 @@ bool launch_optimizer32bit_list_peers(int opt, int dtype, const OptimTensor* ts,
                                       const void* const* grad_srcs, int world, void* const* param_dsts, int ndst,
                                       const void* grad_local, const void* param_local, float grad_scale, float beta1,
                                       float beta2, float beta3, float alpha, float eps, float wd, float lr,
-                                      bool skip_zeros, const float* gnorm_scale_dev, cudaStream_t st);
+                                      bool skip_zeros, const float* gnorm_scale_dev, bool dev, const float* lr_dev,
+                                      cudaStream_t st);
 bool launch_optimizer8bit_blockwise_list_peers(int opt, int dtype, const OptimTensor* ts, int count,
                                                const void* const* grad_srcs, int world, void* const* param_dsts,
                                                int ndst, const void* grad_local, const void* param_local,
                                                float grad_scale, float beta1, float beta2, float beta3, float alpha,
                                                float eps, float wd, float lr, const float* q1, const float* q2,
-                                               bool skip_zeros, const float* gnorm_scale_dev, cudaStream_t st);
+                                               bool skip_zeros, const float* gnorm_scale_dev, bool dev,
+                                               const float* lr_dev, cudaStream_t st);
 bool launch_optimizer_grad_norm_peers(int dtype, const OptimTensor* ts, int count, const void* const* grad_srcs,
                                       int world, const void* grad_local, float grad_scale, bool inf, double* acc,
                                       cudaStream_t st);
@@ -1120,18 +1122,21 @@ static bool optimizer_peers_ids_ok(const char* what, int optimizer, int dtype, c
     return true;
 }
 
+// dev (the _peers_dev entries): the descriptors carry step pointers (NULL: 100) and lr_dev, if not NULL, replaces lr
 static int optimizer_32bit_peers(const char* what, int optimizer, int dtype, const OptimTensor* tensors, int count,
                                  const void* const* grad_srcs, int world, void* const* param_dsts, int ndst,
                                  const void* grad_local, const void* param_local, long long numel, float grad_scale,
                                  float beta1, float beta2, float beta3, float alpha, float eps, float weight_decay,
-                                 float lr, bool skip_zeros, const float* gnorm_scale_dev, cudaStream_t stream) {
+                                 float lr, bool skip_zeros, const float* gnorm_scale_dev, bool dev,
+                                 const float* lr_dev, cudaStream_t stream) {
     if (!optimizer_peers_ids_ok(what, optimizer, dtype, tensors, count)) return 100;
+    if (dev && !optimizer_steps_ok(what, tensors, count)) return 100;
     if (!optimizer_peers_ok(what, optimizer, tensors, count, dtype, grad_srcs, world, param_dsts, ndst, grad_local,
                             param_local, numel))
         return 1;
     launch_optimizer32bit_list_peers(optimizer, dtype, tensors, count, grad_srcs, world, param_dsts, ndst, grad_local,
                                      param_local, grad_scale, beta1, beta2, beta3, alpha, eps, weight_decay, lr,
-                                     skip_zeros, gnorm_scale_dev, stream);
+                                     skip_zeros, gnorm_scale_dev, dev, lr_dev, stream);
     return 0;
 }
 
@@ -1140,8 +1145,9 @@ static int optimizer_8bit_peers(const char* what, int optimizer, int dtype, cons
                                 const void* grad_local, const void* param_local, long long numel, float grad_scale,
                                 float beta1, float beta2, float beta3, float alpha, float eps, float weight_decay,
                                 float lr, const float* quantiles1, const float* quantiles2, bool skip_zeros,
-                                const float* gnorm_scale_dev, cudaStream_t stream) {
+                                const float* gnorm_scale_dev, bool dev, const float* lr_dev, cudaStream_t stream) {
     if (!optimizer_peers_ids_ok(what, optimizer, dtype, tensors, count)) return 100;
+    if (dev && !optimizer_steps_ok(what, tensors, count)) return 100;
     if (!optimizer_peers_ok(what, optimizer, tensors, count, dtype, grad_srcs, world, param_dsts, ndst, grad_local,
                             param_local, numel))
         return 1;
@@ -1154,7 +1160,7 @@ static int optimizer_8bit_peers(const char* what, int optimizer, int dtype, cons
     launch_optimizer8bit_blockwise_list_peers(optimizer, dtype, tensors, count, grad_srcs, world, param_dsts, ndst,
                                               grad_local, param_local, grad_scale, beta1, beta2, beta3, alpha, eps,
                                               weight_decay, lr, quantiles1, quantiles2, skip_zeros, gnorm_scale_dev,
-                                              stream);
+                                              dev, lr_dev, stream);
     return 0;
 }
 
@@ -1166,7 +1172,7 @@ int cbnb_b200_optimizer_update_32bit_multi_peers(int optimizer, int dtype, const
                                                  bool skip_zeros, cudaStream_t stream) {
     return optimizer_32bit_peers("optimizer_update_32bit_multi_peers", optimizer, dtype, tensors, count, grad_srcs,
                                  world, param_dsts, ndst, grad_local, param_local, numel, grad_scale, beta1, beta2,
-                                 beta3, alpha, eps, weight_decay, lr, skip_zeros, nullptr, stream);
+                                 beta3, alpha, eps, weight_decay, lr, skip_zeros, nullptr, false, nullptr, stream);
 }
 
 int cbnb_b200_optimizer_update_8bit_blockwise_multi_peers(int optimizer, int dtype, const OptimTensor* tensors,
@@ -1180,7 +1186,7 @@ int cbnb_b200_optimizer_update_8bit_blockwise_multi_peers(int optimizer, int dty
     return optimizer_8bit_peers("optimizer_update_8bit_blockwise_multi_peers", optimizer, dtype, tensors, count,
                                 grad_srcs, world, param_dsts, ndst, grad_local, param_local, numel, grad_scale, beta1,
                                 beta2, beta3, alpha, eps, weight_decay, lr, quantiles1, quantiles2, skip_zeros,
-                                nullptr, stream);
+                                nullptr, false, nullptr, stream);
 }
 
 // The clipped data-parallel steps: as the _peers entries, with the gradient factor (gnorm_scale of the _multi
@@ -1194,7 +1200,8 @@ int cbnb_b200_optimizer_update_32bit_multi_peers_scaled(int optimizer, int dtype
                                                         const float* gnorm_scale_dev, cudaStream_t stream) {
     return optimizer_32bit_peers("optimizer_update_32bit_multi_peers_scaled", optimizer, dtype, tensors, count,
                                  grad_srcs, world, param_dsts, ndst, grad_local, param_local, numel, grad_scale, beta1,
-                                 beta2, beta3, alpha, eps, weight_decay, lr, skip_zeros, gnorm_scale_dev, stream);
+                                 beta2, beta3, alpha, eps, weight_decay, lr, skip_zeros, gnorm_scale_dev, false, nullptr,
+                                 stream);
 }
 
 int cbnb_b200_optimizer_update_8bit_blockwise_multi_peers_scaled(
@@ -1206,7 +1213,36 @@ int cbnb_b200_optimizer_update_8bit_blockwise_multi_peers_scaled(
     return optimizer_8bit_peers("optimizer_update_8bit_blockwise_multi_peers_scaled", optimizer, dtype, tensors, count,
                                 grad_srcs, world, param_dsts, ndst, grad_local, param_local, numel, grad_scale, beta1,
                                 beta2, beta3, alpha, eps, weight_decay, lr, quantiles1, quantiles2, skip_zeros,
-                                gnorm_scale_dev, stream);
+                                gnorm_scale_dev, false, nullptr, stream);
+}
+
+// Capturable data-parallel steps: the _peers_scaled entries with each descriptor's step_ptr pointing to the tensor's
+// int32 step counter in device memory, and lr_dev, if not NULL, read in place of lr.  Unlike the _multi_dev entries
+// they read the counters and do not advance them: a parameter's step advances on every rank, also on ranks that hold
+// no piece of it, so the caller advances its counters once per step before the call.
+int cbnb_b200_optimizer_update_32bit_multi_peers_dev(int optimizer, int dtype, const OptimTensor* tensors, int count,
+                                                     const void* const* grad_srcs, int world, void* const* param_dsts,
+                                                     int ndst, const void* grad_local, const void* param_local,
+                                                     long long numel, float grad_scale, float beta1, float beta2,
+                                                     float beta3, float alpha, float eps, float weight_decay, float lr,
+                                                     bool skip_zeros, const float* gnorm_scale_dev,
+                                                     const float* lr_dev, cudaStream_t stream) {
+    return optimizer_32bit_peers("optimizer_update_32bit_multi_peers_dev", optimizer, dtype, tensors, count,
+                                 grad_srcs, world, param_dsts, ndst, grad_local, param_local, numel, grad_scale, beta1,
+                                 beta2, beta3, alpha, eps, weight_decay, lr, skip_zeros, gnorm_scale_dev, true, lr_dev,
+                                 stream);
+}
+
+int cbnb_b200_optimizer_update_8bit_blockwise_multi_peers_dev(
+    int optimizer, int dtype, const OptimTensor* tensors, int count, const void* const* grad_srcs, int world,
+    void* const* param_dsts, int ndst, const void* grad_local, const void* param_local, long long numel,
+    float grad_scale, float beta1, float beta2, float beta3, float alpha, float eps, float weight_decay, float lr,
+    const float* quantiles1, const float* quantiles2, bool skip_zeros, const float* gnorm_scale_dev,
+    const float* lr_dev, cudaStream_t stream) {
+    return optimizer_8bit_peers("optimizer_update_8bit_blockwise_multi_peers_dev", optimizer, dtype, tensors, count,
+                                grad_srcs, world, param_dsts, ndst, grad_local, param_local, numel, grad_scale, beta1,
+                                beta2, beta3, alpha, eps, weight_decay, lr, quantiles1, quantiles2, skip_zeros,
+                                gnorm_scale_dev, true, lr_dev, stream);
 }
 
 // The norm of the reduced gradient over one rank's pieces (gradient clipping, optim/sharded.py): each element's

@@ -276,7 +276,7 @@ struct OptimTensor {
             int step;     // this tensor's own step (1 on its first update)
             int reserved;
         };
-        int* step_ptr;    // the capturable (_dev) entries: the step counter in device memory, advanced by the call
+        int* step_ptr;    // the capturable (_dev) entries: the step counter in device memory (_multi_dev advances it)
     };
 };
 static_assert(sizeof(OptimTensor) == 64, "bnb_b200_optim_tensor_t is 64 bytes");

@@ -1055,21 +1055,37 @@ bool list8(int opt, int dtype, const OptimTensor* ts, int count, const OptimScal
 }
 
 // One peer launch (count <= kPeerListCap): 32-bit (eight = false) or 8-bit state, NP >= w sources.  AdEMAMix has no
-// peer instances (its third state sits at state1 + n, relative to the whole tensor).
-template <typename T, int OPT, int NP>
+// peer instances (its third state sits at state1 + n, relative to the whole tensor).  DEV = true (the _peers_dev
+// entries): the descriptors carry step pointers and lr_dev (if not NULL) replaces s.lr, as in the _dev entries, but
+// the launch does not advance the counters: a parameter's step advances on every rank, also where this rank holds no
+// piece of it, so the caller advances them (optim/sharded.py, once per step for all parameters).
+template <typename T, int OPT, int NP, bool DEV>
 void run_peers_np(bool eight, const PeerOptimList& L, long long items, const OptimScalars& s, const float* q1,
-                  const float* q2, cudaStream_t stream) {
+                  const float* q2, const float* lr_dev, cudaStream_t stream) {
     if (!eight)
-        optim32_kernel<T, OPT, false, NP><<<grid_for(items, 1), 512, 0, stream>>>(L, s, nullptr, 0.0f, 0.0f, nullptr);
+        optim32_kernel<T, OPT, DEV, NP><<<grid_for(items, 1), 512, 0, stream>>>(L, s, nullptr, 0.0f, 0.0f, lr_dev);
     else if constexpr (OPT == kAdam)
-        optim8_2state_kernel<T, OPT, false, false, NP><<<grid_for(items, 8), 256, 0, stream>>>(L, s, q1, q2, nullptr);
+        optim8_2state_kernel<T, OPT, false, DEV, NP><<<grid_for(items, 8), 256, 0, stream>>>(L, s, q1, q2, lr_dev);
     else
-        optim8_1state_kernel<T, OPT, false, false, NP><<<grid_for(items, 8), 256, 0, stream>>>(L, s, q1, nullptr);
+        optim8_1state_kernel<T, OPT, false, DEV, NP><<<grid_for(items, 8), 256, 0, stream>>>(L, s, q1, lr_dev);
+}
+
+template <typename T, int OPT, bool DEV>
+void run_peers_w(bool eight, const PeerOptimList& L, long long items, const OptimScalars& s, const float* q1,
+                 const float* q2, const float* lr_dev, cudaStream_t stream) {
+    if (L.peers.w <= 1)
+        run_peers_np<T, OPT, 1, DEV>(eight, L, items, s, q1, q2, lr_dev, stream);
+    else if (L.peers.w <= 2)
+        run_peers_np<T, OPT, 2, DEV>(eight, L, items, s, q1, q2, lr_dev, stream);
+    else if (L.peers.w <= 4)
+        run_peers_np<T, OPT, 4, DEV>(eight, L, items, s, q1, q2, lr_dev, stream);
+    else
+        run_peers_np<T, OPT, kMaxPeers, DEV>(eight, L, items, s, q1, q2, lr_dev, stream);
 }
 
 template <typename T, int OPT>
 bool run_peers(bool eight, const OptimTensor* ts, int count, const OptimScalars& s, const float* q1, const float* q2,
-               const PeerArgs& P, cudaStream_t stream) {
+               const PeerArgs& P, bool dev, const float* lr_dev, cudaStream_t stream) {
     if constexpr (OPT == kAdemamix) {
         return false;
     } else {
@@ -1077,14 +1093,10 @@ bool run_peers(bool eight, const OptimTensor* ts, int count, const OptimScalars&
         L.peers = P;
         const long long items = make_list(L, ts, count, eight ? kOptBlock : kOpt32Chunk);
         if (items > 0) {
-            if (P.w <= 1)
-                run_peers_np<T, OPT, 1>(eight, L, items, s, q1, q2, stream);
-            else if (P.w <= 2)
-                run_peers_np<T, OPT, 2>(eight, L, items, s, q1, q2, stream);
-            else if (P.w <= 4)
-                run_peers_np<T, OPT, 4>(eight, L, items, s, q1, q2, stream);
+            if (dev)
+                run_peers_w<T, OPT, true>(eight, L, items, s, q1, q2, lr_dev, stream);
             else
-                run_peers_np<T, OPT, kMaxPeers>(eight, L, items, s, q1, q2, stream);
+                run_peers_w<T, OPT, false>(eight, L, items, s, q1, q2, nullptr, stream);
         }
         BNB200_CHECK_LAUNCH(eight ? "optimizer8bit_blockwise_peers" : "optimizer32bit_peers");
         return true;
@@ -1093,23 +1105,23 @@ bool run_peers(bool eight, const OptimTensor* ts, int count, const OptimScalars&
 
 template <typename T>
 bool dispatch_peers(int opt, bool eight, const OptimTensor* ts, int count, const OptimScalars& s, const float* q1,
-                    const float* q2, const PeerArgs& P, cudaStream_t st) {
+                    const float* q2, const PeerArgs& P, bool dev, const float* lr_dev, cudaStream_t st) {
     switch (opt) {
-    case kAdam: return run_peers<T, kAdam>(eight, ts, count, s, q1, q2, P, st);
-    case kMomentum: return run_peers<T, kMomentum>(eight, ts, count, s, q1, q2, P, st);
-    case kRmsprop: return run_peers<T, kRmsprop>(eight, ts, count, s, q1, q2, P, st);
-    case kAdagrad: return run_peers<T, kAdagrad>(eight, ts, count, s, q1, q2, P, st);
-    case kLion: return run_peers<T, kLion>(eight, ts, count, s, q1, q2, P, st);
+    case kAdam: return run_peers<T, kAdam>(eight, ts, count, s, q1, q2, P, dev, lr_dev, st);
+    case kMomentum: return run_peers<T, kMomentum>(eight, ts, count, s, q1, q2, P, dev, lr_dev, st);
+    case kRmsprop: return run_peers<T, kRmsprop>(eight, ts, count, s, q1, q2, P, dev, lr_dev, st);
+    case kAdagrad: return run_peers<T, kAdagrad>(eight, ts, count, s, q1, q2, P, dev, lr_dev, st);
+    case kLion: return run_peers<T, kLion>(eight, ts, count, s, q1, q2, P, dev, lr_dev, st);
     }
     return false;
 }
 
 bool list_peers(int opt, int dtype, bool eight, const OptimTensor* ts, int count, const OptimScalars& s,
-                const float* q1, const float* q2, const PeerArgs& P, cudaStream_t st) {
+                const float* q1, const float* q2, const PeerArgs& P, bool dev, const float* lr_dev, cudaStream_t st) {
     switch (dtype) {
-    case 0: return dispatch_peers<float>(opt, eight, ts, count, s, q1, q2, P, st);
-    case 1: return dispatch_peers<__half>(opt, eight, ts, count, s, q1, q2, P, st);
-    case 2: return dispatch_peers<__nv_bfloat16>(opt, eight, ts, count, s, q1, q2, P, st);
+    case 0: return dispatch_peers<float>(opt, eight, ts, count, s, q1, q2, P, dev, lr_dev, st);
+    case 1: return dispatch_peers<__half>(opt, eight, ts, count, s, q1, q2, P, dev, lr_dev, st);
+    case 2: return dispatch_peers<__nv_bfloat16>(opt, eight, ts, count, s, q1, q2, P, dev, lr_dev, st);
     }
     return false;
 }
@@ -1209,16 +1221,18 @@ bool launch_optimizer8bit_blockwise_list_dev(int opt, int dtype, const OptimTens
 int optimizer_peers_capacity() { return kPeerListCap; }
 int optimizer_max_peers() { return kMaxPeers; }
 
-// count <= optimizer_peers_capacity(), 1 <= world, ndst <= kMaxPeers: one launch; false for an unknown id or AdEMAMix
+// count <= optimizer_peers_capacity(), 1 <= world, ndst <= kMaxPeers: one launch; false for an unknown id or AdEMAMix.
+// dev: the descriptors carry step pointers, read and not advanced, and lr_dev (if not NULL) replaces lr.
 bool launch_optimizer32bit_list_peers(int opt, int dtype, const OptimTensor* ts, int count,
                                       const void* const* grad_srcs, int world, void* const* param_dsts, int ndst,
                                       const void* grad_local, const void* param_local, float grad_scale, float beta1,
                                       float beta2, float beta3, float alpha, float eps, float wd, float lr,
-                                      bool skip_zeros, const float* gnorm_scale_dev, cudaStream_t st) {
+                                      bool skip_zeros, const float* gnorm_scale_dev, bool dev, const float* lr_dev,
+                                      cudaStream_t st) {
     const OptimScalars s{beta1, beta2, beta3, alpha, eps, wd, lr, 1.0f, skip_zeros};
     const PeerArgs P =
         peer_args(grad_srcs, world, param_dsts, ndst, grad_local, param_local, grad_scale, gnorm_scale_dev);
-    return list_peers(opt, dtype, false, ts, count, s, nullptr, nullptr, P, st);
+    return list_peers(opt, dtype, false, ts, count, s, nullptr, nullptr, P, dev, lr_dev, st);
 }
 
 bool launch_optimizer8bit_blockwise_list_peers(int opt, int dtype, const OptimTensor* ts, int count,
@@ -1226,11 +1240,12 @@ bool launch_optimizer8bit_blockwise_list_peers(int opt, int dtype, const OptimTe
                                                int ndst, const void* grad_local, const void* param_local,
                                                float grad_scale, float beta1, float beta2, float beta3, float alpha,
                                                float eps, float wd, float lr, const float* q1, const float* q2,
-                                               bool skip_zeros, const float* gnorm_scale_dev, cudaStream_t st) {
+                                               bool skip_zeros, const float* gnorm_scale_dev, bool dev,
+                                               const float* lr_dev, cudaStream_t st) {
     const OptimScalars s{beta1, beta2, beta3, alpha, eps, wd, lr, 1.0f, skip_zeros};
     const PeerArgs P =
         peer_args(grad_srcs, world, param_dsts, ndst, grad_local, param_local, grad_scale, gnorm_scale_dev);
-    return list_peers(opt, dtype, true, ts, count, s, q1, q2, P, st);
+    return list_peers(opt, dtype, true, ts, count, s, q1, q2, P, dev, lr_dev, st);
 }
 
 // count <= optimizer_peers_capacity(), 1 <= world <= kMaxPeers, dtype 0..2: adds the launch's norm value into *acc.

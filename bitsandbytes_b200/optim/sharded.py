@@ -32,6 +32,15 @@ update will and accumulates in fp64, all-gathers one value per rank, and compute
 on the device.  ``step()`` then skips the exchange and hands the coefficient's address to the update kernels, which
 apply it as the unsharded kernels apply ``gnorm_scale``: the step equals the unsharded optimizer's fed the reduced
 gradient with ``gnorm_scale`` = the coefficient.
+
+Wrapping an optimizer made with ``capturable=True`` makes ``step()`` (and ``clip_grad_norm_``) safe to capture in a CUDA
+graph, with the NCCL collectives inside it: the step counters are one int32 tensor on the device, ``steps``, that
+``step()`` advances for every parameter with one in-place add (on every rank, also for parameters of which the rank
+holds no piece) before the update kernels read it; ``group["lr"]`` may be a one-element fp32 CUDA tensor, read by the
+kernels at every launch; and ``step()`` reads nothing on the host.  The parameters must be on a CUDA device.  The exchange buffers, the clip's buffers and the
+state are made by one eager ``step()`` (after an eager ``clip_grad_norm_`` if the captured region clips), which also
+warms NCCL's communicator; a step that would make one of them while capturing raises.  The results are those of
+``capturable=False``, bit for bit.
 """
 from __future__ import annotations
 
@@ -43,10 +52,15 @@ import torch.distributed as dist
 from ..backends.cuda import (optimizer_clip_coef, optimizer_grad_norm_peers, optimizer_update_32bit_multi_peers,
                              optimizer_update_8bit_blockwise_multi_peers)
 from ..parallel import _group_world_rank
-from .optimizer import _STATE_BLOCK, Optimizer2State, Optimizer8bit, _Update, group_updates
+from .optimizer import _STATE_BLOCK, Optimizer2State, Optimizer8bit, _capturing, _Update, group_updates
 
 _QUANT_KEY = Optimizer8bit._FSDP_WRAPPED_QUANT_STATE_KEY
 _STATE_KEYS = ("state1", "state2", "absmax1", "absmax2")
+
+
+def _graph_device(device: torch.device) -> bool:
+    """Whether work on ``device`` can be captured in a CUDA graph (a CUDA device)."""
+    return device.type == "cuda"
 
 
 def _blocks(n: int) -> int:
@@ -98,15 +112,14 @@ class ShardedOptimizer(torch.optim.Optimizer):
     ``optimizer``: an 8-bit / 32-bit / mixed Adam, AdamW, SGD (momentum), RMSprop, Adagrad or Lion of ``bnb.optim``
     that has taken no step.  Its ``param_groups`` are this object's, so learning-rate schedulers work on either.
     ``grad_scale``: the factor of the summed gradient, 1/w (the mean) by default.  The model is not wrapped: run
-    ``loss.backward(); opt.step(); opt.zero_grad()`` on every rank."""
+    ``loss.backward(); opt.step(); opt.zero_grad()`` on every rank.  An optimizer made with ``capturable=True`` gives a
+    step that can be captured in a CUDA graph (see the module documentation)."""
 
     def __init__(self, optimizer, group=None, grad_scale: Optional[float] = None):
         if not isinstance(optimizer, Optimizer8bit):
             raise ValueError(f"ShardedOptimizer wraps a bitsandbytes_b200 optimizer, got {type(optimizer).__name__}")
         if optimizer.is_paged:
             raise ValueError("ShardedOptimizer does not support paged optimizer state")
-        if optimizer.capturable:
-            raise ValueError("ShardedOptimizer does not support capturable=True")
         if optimizer.optimizer_name == "ademamix":
             raise ValueError("ShardedOptimizer does not support AdEMAMix: its kernels address the third state "
                              "relative to the whole tensor")
@@ -133,11 +146,21 @@ class ShardedOptimizer(torch.optim.Optimizer):
         if len(devices) > 1:
             raise ValueError(f"ShardedOptimizer needs every parameter on one device, got {sorted(map(str, devices))}")
         self.device = devices.pop() if devices else torch.device("cuda", torch.cuda.current_device())
+        if optimizer.capturable and not _graph_device(self.device):
+            raise ValueError(f"ShardedOptimizer with capturable=True needs its parameters on a CUDA device, got "
+                             f"{self.device}: the step counters live there and the step is captured in a CUDA graph")
         by_dtype = {}
         for i, (_, _, p, _) in enumerate(self.entries):
             by_dtype.setdefault(p.dtype, []).append(i)
-        self.flats, self.steps = [], [0] * len(self.entries)
+        self.capturable = optimizer.capturable
+        self.flats = []
+        if self.capturable:  # one device counter per parameter; _counters[e] is entry e's one-element view
+            self.steps = torch.zeros(len(self.entries), dtype=torch.int32, device=self.device)
+            self._counters = list(self.steps.split(1))
+        else:
+            self.steps = [0] * len(self.entries)
         self._clip = None  # (gradient sources, coefficient) from clip_grad_norm_ until the step that uses them
+        self._norm_bufs = None  # capturable: the clip's accumulator, per-rank values and (norm, coefficient)
         for dtype, idx in by_dtype.items():
             flat = _Flat([self.entries[i][2] for i in idx], dtype, self.device, self.world, self.rank)
             flat.index = idx
@@ -211,7 +234,7 @@ class ShardedOptimizer(torch.optim.Optimizer):
         for flat, e, s, n, st in self.pieces:
             gi, pi, _, _ = self.entries[e]
             config = opt.get_config(gi, pi, self.param_groups[gi])  # (read at every step: lr schedules)
-            st["step"] = self.steps[e]
+            st["step"] = self._counters[e] if self.capturable else self.steps[e]
             betas = config["betas"]
             beta3 = betas[2] if two and len(betas) >= 3 else 0.0
             u = _PieceUpdate(opt.optimizer_name, flat.param[s:s + n], st, config, betas[0], betas[1], beta3,
@@ -255,6 +278,10 @@ class ShardedOptimizer(torch.optim.Optimizer):
         kernels apply ``gnorm_scale``.  Nothing is read on the host, unless ``error_if_nonfinite``: then a non-finite
         norm raises ``RuntimeError`` (one synchronisation), and ``step()`` would exchange the gradients afresh.
 
+        Capturable: the call can be captured in a CUDA graph, except with ``error_if_nonfinite`` (a host read), which
+        raises while capturing.  Its buffers are made by the first, eager call and reused, so the returned norm is
+        overwritten by the next call (or replay).
+
         Unlike ``torch.nn.utils.clip_grad_norm_``: ``p.grad`` is not modified (the local gradients are not the reduced
         ones; the coefficient is applied inside the update); the norm is computed in fp64 from the reduced gradient and
         returned in fp32, where torch computes per-tensor norms in the gradient's dtype.  Calling torch's function on a
@@ -266,18 +293,25 @@ class ShardedOptimizer(torch.optim.Optimizer):
             raise ValueError(f"clip_grad_norm_: norm_type must be 2 or inf, got {norm_type!r}")
         if self._clip is not None:
             raise RuntimeError("clip_grad_norm_ was already called for this step: call step() first")
+        capturing = _capturing()
+        if capturing and error_if_nonfinite:
+            raise RuntimeError("clip_grad_norm_(error_if_nonfinite=True) is being captured in a CUDA graph: the check "
+                               "reads the norm on the host.  Capture it with error_if_nonfinite=False.")
+        if self.capturable and self._norm_bufs is None:
+            if capturing:
+                raise RuntimeError(f"{type(self).__name__}.clip_grad_norm_() would create its buffers while a CUDA "
+                                   "graph is being captured: run one eager clip_grad_norm_() and step() before "
+                                   "capturing")
+            self._norm_bufs = self._new_norm_bufs()
         self._gather_grads()
         srcs = self._exchange_grads()
-        acc = torch.zeros(1, dtype=torch.float64, device=self.device)
+        acc, every, out = self._norm_bufs if self.capturable else self._new_norm_bufs()
+        acc.zero_()
         for f in self.flats:
             g = [f.grad[s:s + n] for flat, _, s, n, _ in self.pieces if flat is f]
             optimizer_grad_norm_peers(g, srcs[id(f)], f.grad, self.grad_scale, norm_type, acc)
         if self.world > 1:
-            every = torch.empty(self.world, dtype=torch.float64, device=self.device)
             dist.all_gather_into_tensor(every, acc, group=self.group)
-        else:
-            every = acc
-        out = torch.empty(2, dtype=torch.float32, device=self.device)
         optimizer_clip_coef(every, norm_type, max_norm, out)
         total = out[0]
         if error_if_nonfinite and not torch.isfinite(total).item():
@@ -287,8 +321,19 @@ class ShardedOptimizer(torch.optim.Optimizer):
         self._clip = (srcs, out[1:])
         return total
 
+    def _new_norm_bufs(self):
+        """(fp64 accumulator, the ranks' fp64 values: the accumulator itself at one rank, fp32 (norm, coefficient)).
+        The accumulator is zeroed by each clip_grad_norm_."""
+        acc = torch.empty(1, dtype=torch.float64, device=self.device)
+        every = torch.empty(self.world, dtype=torch.float64, device=self.device) if self.world > 1 else acc
+        return acc, every, torch.empty(2, dtype=torch.float32, device=self.device)
+
     @torch.no_grad()
     def step(self, closure=None):
+        if _capturing() and not self.capturable:
+            raise RuntimeError(f"{type(self).__name__}.step() is being captured in a CUDA graph, but the optimizer was "
+                               "constructed with capturable=False: every replay would repeat this step's step number "
+                               "and learning rate.  Construct it with capturable=True.")
         if closure is not None and self._clip is not None:
             raise RuntimeError("step(closure) after clip_grad_norm_: the closure would recompute gradients that were "
                                "already exchanged and clipped")
@@ -297,11 +342,14 @@ class ShardedOptimizer(torch.optim.Optimizer):
             with torch.enable_grad():
                 loss = closure()
         clip, self._clip = self._clip, None
-        if clip is None:
+        if clip is None:  # (unless clip_grad_norm_ exchanged them: clip = (sources, coefficient))
             self._gather_grads()
-        self.steps = [k + 1 for k in self.steps]
-        batches = self._updates()
-        self._exchange(batches, clip)
+            clip = (self._exchange_grads(), None)
+        if self.capturable:
+            self.steps.add_(1)
+        else:
+            self.steps = [k + 1 for k in self.steps]
+        self._exchange(self._updates(), *clip)
         return loss
 
     def _exchange_grads(self):
@@ -312,16 +360,18 @@ class ShardedOptimizer(torch.optim.Optimizer):
                 srcs[id(f)] = [f.grad.data_ptr()]
                 continue
             if f.recv is None:
+                if _capturing():
+                    raise RuntimeError(f"{type(self).__name__} would create its gradient exchange buffer while a CUDA "
+                                       "graph is being captured: run one eager step() before capturing")
                 f.recv = torch.empty_like(f.grad)
             dist.all_to_all_single(f.recv, f.grad, group=self.group)
             es, s0 = f.grad.element_size(), self.rank * f.S
             srcs[id(f)] = [f.recv.data_ptr() + (r * f.S - s0) * es for r in range(self.world)]
         return srcs
 
-    def _exchange(self, batches, clip=None) -> None:
-        """Gradients in (unless clip_grad_norm_ exchanged them: clip = (sources, coefficient)), one launch per batch of
-        pieces, parameters out by all-gather."""
-        srcs, coef = clip if clip is not None else (self._exchange_grads(), None)
+    def _exchange(self, batches, srcs, coef) -> None:
+        """One launch per batch of pieces on the exchanged gradients (srcs, as from _exchange_grads; coef: the clip
+        coefficient or None), parameters out by all-gather."""
         for batch in batches:
             f = batch[0].flat
             self._launch(batch, srcs[id(f)], [f.param.data_ptr()], coef)
@@ -341,8 +391,18 @@ class ShardedOptimizer(torch.optim.Optimizer):
                 k += 1
         return ids
 
+    def _host_steps(self) -> list:
+        """The steps as ints (capturable: read from the device counters, refused while capturing a graph)."""
+        if not self.capturable:
+            return self.steps
+        if _capturing():
+            raise RuntimeError(f"{type(self).__name__}: a state dict is being taken while a CUDA graph is being "
+                               "captured: it reads the step counters on the host")
+        return self.steps.tolist()
+
     def state_dict(self):
         """This rank's shard: every piece's state with its tensor, offset and size, and the partition it came from."""
+        steps = self._host_steps()
         ids = self._param_ids()
         pieces = []
         for flat, e, s, n, st in self.pieces:
@@ -351,13 +411,14 @@ class ShardedOptimizer(torch.optim.Optimizer):
         sd = self.optimizer.state_dict()
         return {"sharded": {"world": self.world, "rank": self.rank,
                             "numels": [[f.numels[t] for t in range(len(f.numels))] for f in self.flats]},
-                "pieces": pieces, "steps": {ids[id(p)]: self.steps[i] for i, (_, _, p, _) in enumerate(self.entries)},
+                "pieces": pieces, "steps": {ids[id(p)]: steps[i] for i, (_, _, p, _) in enumerate(self.entries)},
                 "param_groups": sd["param_groups"]}
 
     def consolidated_state_dict(self, to: int = 0):
         """The unsharded optimizer's ``state_dict()``, with its tensors on the CPU, on group rank ``to``; None on the
         other ranks.  Only rank ``to`` receives the other shards, so no GPU holds the whole state."""
         mine = self.state_dict()
+        steps = mine["steps"]
         local = [{"param": q["param"], "offset": q["offset"], "numel": q["numel"],
                   "state": {k: v.cpu() for k, v in q["state"].items()}} for q in mine["pieces"]]
         if self.world > 1:
@@ -396,7 +457,7 @@ class ShardedOptimizer(torch.optim.Optimizer):
                 wrapped["qmap1"] = opt._qmap("dynamic", self.device).cpu()
                 if "state2" in wrapped:
                     wrapped["qmap2"] = opt._qmap("udynamic", self.device).cpu()
-            state[k] = {"step": self.steps[i], _QUANT_KEY: wrapped}
+            state[k] = {"step": steps[k], _QUANT_KEY: wrapped}
         return {"state": state, "param_groups": mine["param_groups"]}
 
     def load_state_dict(self, state_dict) -> None:
@@ -417,7 +478,7 @@ class ShardedOptimizer(torch.optim.Optimizer):
                                  "consolidated_state_dict() instead")
             for (_, _, _, _, st), q in zip(self.pieces, state_dict["pieces"]):
                 for key, v in q["state"].items():
-                    st[key] = v.to(self.device, copy=True)
+                    self._load(st, key, v)
             steps = state_dict["steps"]
         else:
             full = state_dict["state"]
@@ -437,8 +498,19 @@ class ShardedOptimizer(torch.optim.Optimizer):
                     if key in st and part.dtype != st[key].dtype:
                         raise ValueError(f"loaded state of parameter {k} is {part.dtype}, this optimizer keeps "
                                          f"{st[key].dtype}")
-                    st[key] = part.to(self.device, copy=True)
+                    self._load(st, key, part)
             steps = {k: int(v["step"]) for k, v in full.items()}
-        self.steps = [int(steps.get(ids[id(p)], 0)) for _, _, p, _ in self.entries]
+        steps = [int(steps.get(ids[id(p)], 0)) for _, _, p, _ in self.entries]
+        if self.capturable:  # in place, as the state: a graph captured before the load continues from it
+            self.steps.copy_(torch.tensor(steps, dtype=torch.int32))
+        else:
+            self.steps = steps
         for g, s in zip(self.param_groups, groups):
             g.update({k: v for k, v in s.items() if k != "params"})
+
+    def _load(self, st, key, v) -> None:
+        """One state tensor of a piece: a copy on the device; capturable, written into the tensor a graph captured."""
+        if self.capturable and key in st and st[key].shape == v.shape and st[key].dtype == v.dtype:
+            st[key].copy_(v)
+        else:
+            st[key] = v.to(self.device, copy=True)

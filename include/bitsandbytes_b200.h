@@ -339,7 +339,7 @@ typedef struct bnb_b200_optim_tensor {
             int step;
             int reserved; /* 0 */
         };
-        int* step_ptr; /* the _dev entries only: the tensor's step counter in device memory */
+        int* step_ptr; /* the _dev entries only (_multi_dev, _peers_dev): the tensor's step counter in device memory */
     };
 } bnb_b200_optim_tensor_t;
 int cbnb_b200_optimizer_multi_capacity(void);
@@ -372,6 +372,15 @@ int cbnb_b200_optimizer_update_8bit_blockwise_multi_peers(int optimizer, int dty
  * checks as the _peers entries. */
 int cbnb_b200_optimizer_update_32bit_multi_peers_scaled(int optimizer, int dtype, const bnb_b200_optim_tensor_t* tensors, int count, const void* const* grad_srcs, int world, void* const* param_dsts, int ndst, const void* grad_local, const void* param_local, long long numel, float grad_scale, float beta1, float beta2, float beta3, float alpha, float eps, float weight_decay, float lr, bool skip_zeros, const float* gnorm_scale_dev, bnb_stream_t stream);
 int cbnb_b200_optimizer_update_8bit_blockwise_multi_peers_scaled(int optimizer, int dtype, const bnb_b200_optim_tensor_t* tensors, int count, const void* const* grad_srcs, int world, void* const* param_dsts, int ndst, const void* grad_local, const void* param_local, long long numel, float grad_scale, float beta1, float beta2, float beta3, float alpha, float eps, float weight_decay, float lr, const float* quantiles1, const float* quantiles2, bool skip_zeros, const float* gnorm_scale_dev, bnb_stream_t stream);
+/* Capturable data-parallel steps, for CUDA graphs: the _peers_scaled entries (gnorm_scale_dev NULL: 1) with each
+ * descriptor's step_ptr pointing to the tensor's int32 step counter in device memory, as in the _multi_dev entries, and
+ * lr_dev, an fp32 value in device memory read in place of lr when not NULL.  These entries read the counters and do NOT
+ * advance them, unlike the _multi_dev entries: a parameter's step must advance on every rank, also on ranks that hold
+ * no piece of it and for zero-size tensors, so the caller advances its counters (once per step, before the call).  With
+ * counters holding k and *lr_dev == lr, the bits of the _peers_scaled entries with step k and that lr.  Return codes
+ * and checks as the _peers_scaled entries, plus 100 with the message set for a NULL step_ptr. */
+int cbnb_b200_optimizer_update_32bit_multi_peers_dev(int optimizer, int dtype, const bnb_b200_optim_tensor_t* tensors, int count, const void* const* grad_srcs, int world, void* const* param_dsts, int ndst, const void* grad_local, const void* param_local, long long numel, float grad_scale, float beta1, float beta2, float beta3, float alpha, float eps, float weight_decay, float lr, bool skip_zeros, const float* gnorm_scale_dev, const float* lr_dev, bnb_stream_t stream);
+int cbnb_b200_optimizer_update_8bit_blockwise_multi_peers_dev(int optimizer, int dtype, const bnb_b200_optim_tensor_t* tensors, int count, const void* const* grad_srcs, int world, void* const* param_dsts, int ndst, const void* grad_local, const void* param_local, long long numel, float grad_scale, float beta1, float beta2, float beta3, float alpha, float eps, float weight_decay, float lr, const float* quantiles1, const float* quantiles2, bool skip_zeros, const float* gnorm_scale_dev, const float* lr_dev, bnb_stream_t stream);
 /* The norm of the reduced gradient over one rank's pieces, for global gradient clipping: each element's gradient is
  * T(fp32 rank-order sum of the world sources * grad_scale), formed as the _peers entries form it, and the call adds
  * the sum of its squares (inf_norm: takes the max of |g|, NaN kept) in fp64 into *acc, in stream order after earlier
