@@ -45,6 +45,10 @@ SCHEMAS = {
     "Tensor(a3!)? state2, float beta1, float beta2, float beta3, float alpha, float eps, int step, float lr, "
     "Tensor(a4!) qmap1, Tensor(a5!)? qmap2, Tensor(a6!) absmax1, Tensor(a7!)? absmax2, float weight_decay, "
     "float gnorm_scale, bool skip_zeros=False) -> ()",
+    # no reference counterpart: the 4-bit form of grouped_mm with a 3-D weight (one launch for every expert of a
+    # mixture-of-experts layer), shapeB = [E, N, K]
+    "gemm_4bit_grouped": "(Tensor A, Tensor B, int[] shapeB, Tensor absmax, int blocksize, str quant_type, Tensor offs, "
+    "Tensor? bias=None, Tensor? absmax_8bit=None, Tensor? absmax_code=None, Tensor? absmax_offset=None) -> Tensor",
 }
 
 _defined = False
@@ -172,6 +176,62 @@ def _(A, B, shapeB, absmax, blocksize, quant_type, bias=None, absmax_8bit=None, 
     torch._check(A.dtype in _FLOATS, lambda: f"A must be float16, bfloat16 or float32, got {A.dtype}")
     torch._check(B.dtype in _4BIT_STORAGE, lambda: f"unsupported 4-bit storage dtype {B.dtype}")
     return torch.empty((*A.shape[:-1], shapeB[0]), device=A.device, dtype=A.dtype)
+
+
+MAX_EXPERTS = 1024  # the grouped GEMM's limit (kMaxExperts in csrc/gemm4_tc.cu)
+
+
+def check_grouped(A, B, shapeB, absmax, blocksize, quant_type, offs, bias=None, absmax_8bit=None, absmax_code=None,
+                  absmax_offset=None):
+    """What the host knows of a gemm_4bit_grouped call, checked: shapes, dtypes, devices and the sizes of the packed
+    weight and its statistics (never the values of ``offs``, which stay on the device).  Returns (E, N, K).  Shared by
+    the CUDA kernel and the shape function."""
+    _check_4bit_common(blocksize, quant_type)
+    torch._check(blocksize in (32, 64, 128, 256, 512, 1024, 2048, 4096), lambda: f"invalid blocksize {blocksize}")
+    torch._check(len(shapeB) == 3, lambda: f"gemm_4bit_grouped: the weight must be an [E, N, K] expert tensor, got "
+                 f"shape {list(shapeB)}")
+    E, N, K = shapeB
+    torch._check(A.dtype in (torch.float16, torch.bfloat16), lambda: f"gemm_4bit_grouped: A must be float16 or "
+                 f"bfloat16, got {A.dtype} (fp32 experts keep the parametrize route)")
+    torch._check(A.dim() == 2 and A.shape[1] == K, lambda: f"gemm_4bit_grouped: A must be [M, {K}] for an [E, N, K] = "
+                 f"{list(shapeB)} weight, got {list(A.shape)} (a weight quantised as [E, K, N] is not served)")
+    torch._check(K > 0 and K % 64 == 0, lambda: f"gemm_4bit_grouped: K = {K} must be a multiple of 64")
+    torch._check(1 <= E <= MAX_EXPERTS, lambda: f"gemm_4bit_grouped: 1 <= E <= {MAX_EXPERTS} experts, got {E}")
+    torch._check(N >= 1, lambda: f"gemm_4bit_grouped: N = {N} must be positive")
+    torch._check(offs.dtype == torch.int32 and tuple(offs.shape) == (E,),
+                 lambda: f"gemm_4bit_grouped: offs must be int32 [{E}], got {offs.dtype} {list(offs.shape)}")
+    torch._check(B.dtype in _4BIT_STORAGE, lambda: f"unsupported 4-bit storage dtype {B.dtype}")
+    n = E * N * K
+    torch._check(B.numel() * B.element_size() == n // 2, lambda: f"gemm_4bit_grouped: B holds "
+                 f"{B.numel() * B.element_size()} bytes, an {list(shapeB)} weight packs into {n // 2}")
+    nblocks = -(n // -blocksize)
+    torch._check(absmax.dtype == torch.float32, lambda: f"absmax must be float32, got {absmax.dtype}")
+    if absmax_8bit is None:
+        torch._check(absmax.numel() == nblocks, lambda: f"gemm_4bit_grouped: absmax must hold {nblocks} scales, got "
+                     f"{absmax.numel()}")
+    else:
+        torch._check(absmax_code is not None and absmax_offset is not None,
+                     lambda: "absmax_8bit, absmax_code and absmax_offset must be given together")
+        torch._check(absmax_8bit.dtype == torch.uint8 and absmax_8bit.numel() == nblocks,
+                     lambda: f"gemm_4bit_grouped: absmax_8bit must be uint8 [{nblocks}]")
+        torch._check(absmax.numel() == -(nblocks // -256), lambda: "gemm_4bit_grouped: nested statistics need "
+                     f"{-(nblocks // -256)} level-2 scales (blocksize 256), got {absmax.numel()}")
+        torch._check(absmax_code.dtype == torch.float32 and absmax_code.numel() == 256,
+                     lambda: "gemm_4bit_grouped: absmax_code must be float32 [256]")
+    if bias is not None:
+        torch._check(bias.dtype == A.dtype and tuple(bias.shape) == (E, N),
+                     lambda: f"gemm_4bit_grouped: bias must be {A.dtype} [{E}, {N}], got {bias.dtype} {list(bias.shape)}")
+    for t in (B, absmax, offs, bias, absmax_8bit, absmax_code, absmax_offset):
+        torch._check(t is None or t.device == A.device, lambda: f"gemm_4bit_grouped: every operand must be on {A.device}")
+    return E, N, K
+
+
+@fake("gemm_4bit_grouped")
+def _(A, B, shapeB, absmax, blocksize, quant_type, offs, bias=None, absmax_8bit=None, absmax_code=None,
+      absmax_offset=None):
+    _, N, _ = check_grouped(A, B, shapeB, absmax, blocksize, quant_type, offs, bias, absmax_8bit, absmax_code,
+                            absmax_offset)
+    return torch.empty((A.shape[0], N), device=A.device, dtype=A.dtype)
 
 
 @fake("dequantize_blockwise")

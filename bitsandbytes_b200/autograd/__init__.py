@@ -1,1 +1,2 @@
-from ._functions import MatMul4Bit, MatMul8bitLt, MatmulLtState, matmul, matmul_4bit  # noqa: F401
+from ._functions import (GroupedMatMul4Bit, MatMul4Bit, MatMul8bitLt, MatmulLtState,  # noqa: F401
+                         grouped_matmul_4bit, matmul, matmul_4bit)

@@ -321,3 +321,83 @@ def matmul_4bit(A, B, quant_state: F.QuantState, out=None, bias=None):
         out.copy_(result)
         return out
     return result
+
+
+def _gemm_4bit_grouped(A, B, quant_state, offs, bias):
+    """The grouped op with plain or double-quantised statistics."""
+    if not quant_state.nested:
+        return torch.ops.bitsandbytes.gemm_4bit_grouped.default(A, B, quant_state.shape, quant_state.absmax,
+                                                                quant_state.blocksize, quant_state.quant_type, offs,
+                                                                bias=bias)
+    if quant_state.state2.blocksize != 256:
+        raise NotImplementedError("nested quantization with state2.blocksize != 256 is not supported")
+    return torch.ops.bitsandbytes.gemm_4bit_grouped.default(
+        A, B, quant_state.shape, quant_state.state2.absmax, quant_state.blocksize, quant_state.quant_type, offs,
+        bias=bias, absmax_8bit=quant_state.absmax, absmax_code=quant_state.state2.code,
+        absmax_offset=quant_state.offset)
+
+
+def _clamped_ends(offs, M):
+    """end_e = min(max(offs[e], end_{e-1}), M), end_{-1} = 0: the kernel's clamp of the expert ends, on the device."""
+    return offs.clamp(min=0).cummax(0).values.clamp(max=M)
+
+
+class GroupedMatMul4Bit(torch.autograd.Function):
+    """The grouped 4-bit GEMM with a frozen weight.  The backward (bf16) dequantises the expert tensor once and runs
+    ``grouped_mm`` for grad_A; nothing in either direction reads ``offs`` on the host."""
+
+    @staticmethod
+    def forward(ctx, A, B, offs, bias, quant_state):
+        out = _gemm_4bit_grouped(A, B, quant_state, offs, bias)
+        ctx.state = quant_state
+        ctx.save_for_backward(B, offs)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        need_A, _, _, need_bias, _ = ctx.needs_input_grad
+        B, offs = ctx.saved_tensors
+        E, N, K = ctx.state.shape
+        M = grad_output.shape[0]
+        ends = _clamped_ends(offs, M)
+        grad_A = grad_bias = None
+        if need_A:
+            W = F.dequantize_4bit(B, ctx.state).to(grad_output.dtype)  # [E, N, K]
+            grad_A = torch.nn.functional.grouped_mm(grad_output.contiguous(), W, offs=ends)
+            # rows past the last expert's end belong to no expert: their gradient is zero
+            routed = torch.arange(M, device=grad_A.device).unsqueeze(1) < ends[-1]
+            grad_A = torch.where(routed, grad_A, torch.zeros((), dtype=grad_A.dtype, device=grad_A.device))
+        if need_bias:
+            # segment sums of grad_output's rows in fp32; the rows past the last end go to a discarded segment E
+            eid = torch.searchsorted(ends, torch.arange(M, device=ends.device, dtype=ends.dtype), right=True)
+            sums = torch.zeros((E + 1, N), dtype=torch.float32, device=grad_output.device)
+            grad_bias = sums.index_add_(0, eid, grad_output.float())[:E].to(grad_output.dtype)
+        return grad_A, None, None, grad_bias, None
+
+
+def grouped_matmul_4bit(A, B, quant_state: F.QuantState, offs, bias=None):
+    """Every expert of a mixture-of-experts layer in one launch, on a 4-bit expert tensor: for the rows of expert e,
+    ``offs[e-1] <= m < offs[e]`` of the expert-sorted ``A [M, K]``, ``out[m] = A[m] . W[e]^T + bias[e]``; rows past
+    ``offs[E-1]`` are zero.  ``B``/``quant_state`` are the ``[E, N, K]`` weight quantised as one tensor
+    (``F.quantize_4bit``, ``Params4bit``), ``offs`` the int32 ``[E]`` end rows on the device (malformed ones are
+    clamped on the device), ``bias`` an optional ``[E, N]``.  The weight is frozen; A and the bias train in bf16 only."""
+    if quant_state is None:
+        raise ValueError("quant_state is required")
+    if len(quant_state.shape) != 3:
+        raise ValueError(f"grouped_matmul_4bit: quant_state.shape must be the [E, N, K] of the expert tensor, got "
+                         f"{list(quant_state.shape)}")
+    E, N, K = quant_state.shape
+    if A.dim() != 2 or A.shape[1] != K:
+        hint = " (the weight was quantised as [E, K, N]: quantise it as [E, N, K])" if A.shape[-1] == N else ""
+        raise ValueError(f"grouped_matmul_4bit: A must be [M, {K}] for an [E, N, K] = {list(quant_state.shape)} "
+                         f"weight, got {list(A.shape)}{hint}")
+    B = B.view(-1, 1)
+    needs_grad = torch.is_grad_enabled() and (A.requires_grad or (bias is not None and bias.requires_grad))
+    if not needs_grad:
+        return _gemm_4bit_grouped(A, B, quant_state, offs, bias)
+    if A.dtype != torch.bfloat16:
+        raise ValueError(f"grouped_matmul_4bit: training runs in bfloat16 only (the input gradient is "
+                         f"torch.nn.functional.grouped_mm), got {A.dtype} with requires_grad")
+    if N % 8 != 0:
+        raise ValueError(f"grouped_matmul_4bit: training needs N % 8 == 0 (grouped_mm's row stride), got N = {N}")
+    return GroupedMatMul4Bit.apply(A, B, offs, bias, quant_state)

@@ -27,7 +27,7 @@ from warnings import warn
 
 import torch
 
-from .._ops import kernel
+from .._ops import check_grouped, kernel
 from .. import cextension as cext
 from ..cextension import lib
 
@@ -449,6 +449,36 @@ def _gemm_4bit(A, B, shapeB, absmax, blocksize: int, quant_type: str, bias=None,
     if out.numel() == 0:
         return out
     gemm_4bit_into(A, B, shapeB, absmax, blocksize, quant_type, bias, absmax_8bit, absmax_code, absmax_offset, out, N)
+    return out
+
+
+@kernel("gemm_4bit_grouped")
+def _gemm_4bit_grouped(A, B, shapeB, absmax, blocksize: int, quant_type: str, offs, bias=None, absmax_8bit=None,
+                       absmax_code=None, absmax_offset=None):
+    """Every expert of a mixture-of-experts layer in one launch: ``out[m] = A[m] . W[e]^T + bias[e]`` for the rows of
+    expert e, ``offs[e-1] <= m < offs[e]`` (offs clamped on the device), and 0 for the rows past ``offs[E-1]``.  Nothing
+    is read back to the host, so the call can be captured in a CUDA graph."""
+    E, N, K = check_grouped(A, B, shapeB, absmax, blocksize, quant_type, offs, bias, absmax_8bit, absmax_code,
+                            absmax_offset)
+    M = A.shape[0]
+    _check_sizes("gemm_4bit_grouped", M, E * N, K)
+    out = torch.empty((M, N), dtype=A.dtype, device=A.device)
+    if M == 0:
+        return out
+    off = _weight_operands(absmax, blocksize, quant_type, absmax_8bit, absmax_code, absmax_offset)
+    A, B, offs = A.contiguous(), B.contiguous(), offs.contiguous()
+    bias = bias.contiguous() if bias is not None else None
+    with _on_device(A):
+        rc = lib.cbnb_b200_gemm_4bit_grouped(
+            A.data_ptr(), B.data_ptr(), absmax.data_ptr(),
+            absmax_8bit.data_ptr() if absmax_8bit is not None else None,
+            absmax_code.data_ptr() if absmax_code is not None else None,
+            off.data_ptr() if off is not None else None,
+            offs.data_ptr(), E, out.data_ptr(), bias.data_ptr() if bias is not None else None,
+            M, N, K, N, blocksize, _QT_ID[quant_type], _DTYPE_ID[A.dtype], _stream(A))
+    lib.check("gemm_4bit_grouped")
+    if rc != 0:
+        raise RuntimeError(f"gemm_4bit_grouped: the library does not serve this call (code {rc})")
     return out
 
 

@@ -92,6 +92,11 @@ template <typename T, bool PART>
 int launch_gemm4_input_grad(const T* G, int ldg, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
                             const float* absmax_code, const float* absmax_offset, OutElem<T, PART>* out, int ldc, int M,
                             int N, int K, int blocksize, int quant_type, cudaStream_t stream, int panel_cols);
+template <typename T>
+bool launch_gemm4_grouped(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
+                          const float* absmax_code, const float* absmax_offset, const int* offs, int E, T* out,
+                          const T* bias, int M, int N, int K, int ldc, int blocksize, int quant_type, int mt,
+                          cudaStream_t stream);
 // partials.cu
 bool launch_reduce_partials(const float* parts, int world, long long part_stride, void* out, const void* bias, int M,
                             int N, int ldc, int dtype, cudaStream_t stream);
@@ -401,6 +406,43 @@ static int gemm_4bit_input_grad(const void* G, int ldg, const uint8_t* B, const 
     return rc;
 }
 
+// The grouped GEMM's token tile: the smallest of 16, 32, 64 and 128 tokens that holds twice the mean rows per expert,
+// 2 ceil(M / E), since under top-k routing many experts get more rows than the mean.  Measured on an H100
+// (tools/time_grouped_gemm4.py, DESIGN.md section 7): at a mean of 16 rows the 32-token tile is the fastest (Qwen3-30B-A3B,
+// 256 tokens: 242 us against 334 us at 16 for gate_up), at a mean of 64 the 128-token tile (Mixtral-8x7B, 256 tokens:
+// 664 us against 766 us at 64 for gate_up), and at a mean of 4 the 16-token tile.  The exception measured: at one token
+// the down projections run 7-11 % faster at 64 tokens than at the rule's 16.
+static int grouped_tile(int M, int E) {
+    const long long want = 2LL * ((M + E - 1) / E);
+    return want <= 16 ? 16 : want <= 32 ? 32 : want <= 64 ? 64 : 128;
+}
+
+// The grouped GEMM of the entries below: 0; 1 with the error message set for bad arguments; 100 when not served,
+// with nothing written and no message; or 100 with the error message set when a launch past those checks fails.
+static int gemm_4bit_grouped(const void* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
+                             const float* absmax_code, const float* absmax_offset, const int* offs, int E, void* out,
+                             const void* bias, int M, int N, int K, int ldc, int blocksize, int quant_type, int dtype,
+                             int mt, cudaStream_t stream) {
+    if (A == nullptr || B == nullptr || absmax == nullptr || offs == nullptr || out == nullptr || M < 0 || N <= 0 ||
+        K <= 0 || E < 1 || ldc < N || (quant_type != kFP4 && quant_type != kNF4) ||
+        (absmax_8bit != nullptr && absmax_code == nullptr)) {
+        set_last_error_msg("gemm_4bit_grouped: needs A, B, absmax, offs and out, M >= 0, N, K >= 1, E >= 1, ldc >= N, "
+                           "quant_type 1 (FP4) or 2 (NF4), and absmax_code with absmax_8bit");
+        return 1;
+    }
+    if (M == 0) return 0;
+    if (mt == 0) mt = grouped_tile(M, E);
+    bool ok = false;
+    const bool known = with_dtype<kIdF16 | kIdBF16>(dtype, [&](auto t) {
+        using T = decltype(t);
+        if constexpr (!std::is_same<T, float>::value) {
+            ok = launch_gemm4_grouped<T>((const T*)A, B, absmax, absmax_8bit, absmax_code, absmax_offset, offs, E,
+                                         (T*)out, (const T*)bias, M, N, K, ldc, blocksize, quant_type, mt, stream);
+        }
+    });
+    return known && ok ? 0 : 100;
+}
+
 } // namespace bnb200
 
 using namespace bnb200;
@@ -696,6 +738,29 @@ int cbnb_b200_gemm_decoded(const void* A, const void* W, void* out, const void* 
         ok = launch_gemm_decoded<T>((const T*)A, (const T*)W, (T*)out, (const T*)bias, M, N, K, ldc, mt, stream);
     });
     return ok ? 0 : 100;
+}
+
+// The grouped 4-bit GEMM of a mixture-of-experts layer (no reference counterpart): out[m, :] (row stride ldc) =
+// T(A[m, :] . W_e^T + bias[e * N ..]) for the rows of expert e, end_{e-1} <= m < end_e, and 0 for the rows past
+// end_{E-1}.  B is E experts' [N, K] weights quantised as one [E * N, K] tensor; offs[E] (int32, on the device) holds the
+// end rows, clamped on the device as end_e = min(max(offs[e], end_{e-1}), M).  Returns 0, 1 with the error message set
+// for bad arguments, or 100, with nothing written, for what the kernel does not serve.  A failure past those checks (a
+// tensor map, the shared-memory opt-in or the launch) also returns 100, with the error message set.
+int cbnb_b200_gemm_4bit_grouped(const void* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
+                                const float* absmax_code, const float* absmax_offset, const int* offs, int E, void* out,
+                                const void* bias, int M, int N, int K, int ldc, int blocksize, int quant_type,
+                                int dtype, cudaStream_t stream) {
+    return gemm_4bit_grouped(A, B, absmax, absmax_8bit, absmax_code, absmax_offset, offs, E, out, bias, M, N, K, ldc,
+                             blocksize, quant_type, dtype, 0, stream);
+}
+
+// Developer / test entry: cbnb_b200_gemm_4bit_grouped at token tile mt (16 | 32 | 64 | 128; 0 = the production rule).
+int cbnb_b200_gemm_4bit_grouped_mt(const void* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
+                                   const float* absmax_code, const float* absmax_offset, const int* offs, int E,
+                                   void* out, const void* bias, int M, int N, int K, int ldc, int blocksize,
+                                   int quant_type, int dtype, int mt, cudaStream_t stream) {
+    return gemm_4bit_grouped(A, B, absmax, absmax_8bit, absmax_code, absmax_offset, offs, E, out, bias, M, N, K, ldc,
+                             blocksize, quant_type, dtype, mt, stream);
 }
 
 int cbnb_b200_gemm_4bit_path(int M, int N, int K, int blocksize, int dtype) {

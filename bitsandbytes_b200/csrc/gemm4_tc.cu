@@ -108,7 +108,17 @@ struct Gemm4Params {
     int splits;                  // K splits per tile (1 = none)
     int rows_per_out;            // PART only: 0 = every row to out and the peers; > 0 = row m to copy m / rows_per_out
                                  //   (0 = out, d = peer_out[d - 1]) at row m % rows_per_out (OutList::rows_per_out)
+    // GROUPED only: B is E experts' [N, K] weights stacked ([E * N, K / 2] codes, N per expert), and the activation
+    // rows of expert e are [end_{e-1}, end_e), end_e = min(max(offs[e], end_{e-1}), M) read on the device
+    const int* offs;
+    int E;
 };
+
+// The grouped instances (GROUPED = true) serve 1 <= E <= kMaxExperts experts per launch: their group table (the
+// clamped end row and the exclusive prefix of the m-tile counts of every expert, plus the scan's per-warp totals) sits
+// in shared memory past the barriers.
+constexpr int kMaxExperts = 1024;
+constexpr int kGroupTabBytes = (2 * kMaxExperts + 1 + 2 * kThreads / 32) * 4;
 
 // The partial instances' store of element (m, n) of the fp32 output (m < M, n < N), routed as p.rows_per_out says.
 __device__ __forceinline__ void store_partial(const Gemm4Params& p, int m, int n, float v) {
@@ -213,7 +223,21 @@ __device__ __forceinline__ uint32_t gather_nibbles(uint4 v, uint32_t sel, uint32
     return r;
 }
 
-template <typename T, int QT, int MT, bool DQ, bool PART>
+// GROUPED: the group table, past the barriers' 256 bytes of the shared memory: gend[e] = end_e, then gtp[e] = the m-tiles
+// of experts 0..e-1 (gtp[E] = all of them), then the scan's per-warp totals.  (Taken where it is used: a table pointer
+// held across the kernel changes cicc's register moves in the other instances.)
+template <typename Cfg> __device__ __forceinline__ int* group_table(uint8_t* so) {
+    return reinterpret_cast<int*>(so + Cfg::kOutBytes + 256);
+}
+
+// GROUPED: the number of units, gtp[E] m-tiles times the n-tiles.  Each role reads it from the table after its register
+// hand-off (a volatile read, which stays there): held from the table build on, across the hand-off, it cost the
+// plain-statistics MT = 64 instances a spill.
+template <typename Cfg> __device__ __forceinline__ int grouped_units(uint8_t* so, const Gemm4Params& p) {
+    return *reinterpret_cast<const volatile int*>(group_table<Cfg>(so) + kMaxExperts + p.E) * p.n_tiles;
+}
+
+template <typename T, int QT, int MT, bool DQ, bool PART, bool GROUPED = false>
 __global__ void __launch_bounds__(kThreads, 1)
     gemm4_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
                     const Gemm4Params p) {
@@ -248,11 +272,14 @@ __global__ void __launch_bounds__(kThreads, 1)
 
     // Work units u = (tile, K split), ordered (tile, split); tile = m_tile * n_tiles + n_tile.  A CTA runs units
     // blockIdx.x, blockIdx.x + gridDim.x, ...; a split launch is one wave, one unit per CTA.
-    const int splits = p.splits;
-    const int units = p.tiles_total * splits;
+    // GROUPED: no K split; m_tile counts the m-tiles of all experts in expert order (expert e's j-th m-tile starts at
+    // row end_{e-1} + j * MT), and the number of units is known once the group table is built.
+    const int splits = GROUPED ? 1 : p.splits;
+    int units = p.tiles_total * splits;
     const int per = (p.kblocks_total + splits - 1) / splits;
     struct Unit {
         int tile, split, n0, m0, st_begin, nst;
+        int m_end, wrow;  // GROUPED: the expert's end row, and its first row of the stacked weight (e * N)
     };
     auto unit_at = [&](int u) {
         Unit w;
@@ -260,6 +287,19 @@ __global__ void __launch_bounds__(kThreads, 1)
         w.split = u - w.tile * splits;
         w.n0 = (w.tile % p.n_tiles) * kTileN;
         w.m0 = (w.tile / p.n_tiles) * MT;
+        if constexpr (GROUPED) {
+            // the expert of m-tile g: the last e with gtp[e] <= g, which has m-tiles since g < gtp[E]
+            const int g = w.tile / p.n_tiles;
+            const int* gend = group_table<Cfg>(so);
+            const int* gtp = gend + kMaxExperts;
+            int lo = 0;
+#pragma unroll
+            for (int step = kMaxExperts / 2; step >= 1; step >>= 1)
+                if (lo + step < p.E && gtp[lo + step] <= g) lo += step;
+            w.m0 = (lo > 0 ? gend[lo - 1] : 0) + (g - gtp[lo]) * MT;
+            w.m_end = gend[lo];
+            w.wrow = lo * p.N;
+        }
         w.st_begin = w.split * per;
         const int st_end = w.st_begin + per < p.kblocks_total ? w.st_begin + per : p.kblocks_total;
         w.nst = st_end - w.st_begin;  // >= 1 by construction
@@ -273,6 +313,66 @@ __global__ void __launch_bounds__(kThreads, 1)
         }
         ptx::fence_barrier_init();
     }
+    if constexpr (GROUPED) {
+        // The group table, built by the whole CTA before the role split (every CTA builds the same one): thread t
+        // takes experts [t * kPer, t * kPer + kPer).  end_e = min(M, max(0, offs[0..e])) -- the clamp of the
+        // contract, as a prefix maximum -- then the m-tile counts ceil((end_e - end_{e-1}) / MT) and their
+        // exclusive prefix sum, each scan over the warp by shuffles and across the 12 warps through shared memory.
+        constexpr int kPer = (kMaxExperts + kThreads - 1) / kThreads;
+        constexpr int kWarps = kThreads / 32;
+        int* gend = group_table<Cfg>(so);
+        int* gtp = gend + kMaxExperts;
+        static_assert(kMaxExperts <= (kThreads - 1) * kPer, "the last thread must hold no expert");
+        int* wtot = gtp + kMaxExperts + 1;  // [kWarps] maxima, then [kWarps] tile counts
+        const int e0 = threadIdx.x * kPer;
+        int v[kPer];
+        int run = 0;
+#pragma unroll
+        for (int i = 0; i < kPer; ++i) {
+            v[i] = e0 + i < p.E ? max(__ldg(p.offs + e0 + i), 0) : 0;
+            run = max(run, v[i]);
+        }
+        int inc = run;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const int o = __shfl_up_sync(0xffffffffu, inc, d);
+            if (lane >= d) inc = max(inc, o);
+        }
+        if (lane == 31) wtot[warp] = inc;
+        __syncthreads();
+        int r = __shfl_up_sync(0xffffffffu, inc, 1);
+        if (lane == 0) r = 0;
+        for (int w2 = 0; w2 < warp; ++w2) r = max(r, wtot[w2]);
+        int prev = min(r, p.M);
+        int cnt[kPer], tiles = 0;
+#pragma unroll
+        for (int i = 0; i < kPer; ++i) {
+            r = max(r, v[i]);
+            v[i] = min(r, p.M);  // end_e (experts past E: end_{E-1}, no rows)
+            cnt[i] = (v[i] - prev + MT - 1) / MT;
+            prev = v[i];
+            tiles += cnt[i];
+        }
+        int incs = tiles;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const int o = __shfl_up_sync(0xffffffffu, incs, d);
+            if (lane >= d) incs += o;
+        }
+        if (lane == 31) wtot[kWarps + warp] = incs;
+        __syncthreads();
+        int base = incs - tiles;
+        for (int w2 = 0; w2 < warp; ++w2) base += wtot[kWarps + w2];
+#pragma unroll
+        for (int i = 0; i < kPer; ++i) {
+            if (e0 + i < p.E) {
+                gend[e0 + i] = v[i];
+                gtp[e0 + i] = base;
+            }
+            base += cnt[i];
+        }
+        if (threadIdx.x == kThreads - 1) gtp[p.E] = base;  // the last thread's experts are past E: base is the total
+    }
     __syncthreads();
 
     // The ring runs continuously over the CTA's units: its slot and phase carry from one unit to the next.
@@ -280,6 +380,7 @@ __global__ void __launch_bounds__(kThreads, 1)
     // (the role test is made provably warp-uniform, as setmaxnreg requires of the whole warpgroup)
     if (__shfl_sync(0xffffffffu, threadIdx.x / 128, 0) == 0) {
         ptx::setmaxnreg_dec<kProducerRegs>();
+        if constexpr (GROUPED) units = grouped_units<Cfg>(so, p);
         if (threadIdx.x == 0) {
             ptx::prefetch_tmap(&tmap_x);
             ptx::prefetch_tmap(&tmap_w);
@@ -302,7 +403,10 @@ __global__ void __launch_bounds__(kThreads, 1)
                         for (int h = 0; h < 2; ++h)
                             ptx::tma_load_2d(sw + slot * kWStageBytes + h * kBK * 128, &tmap_w, &full[slot], w.n0 + 64 * h, k0);
                     } else {
-                        ptx::tma_load_2d(sw + slot * kWStageBytes, &tmap_w, &full[slot], kSS ? k0 : k0 / 2, w.n0);
+                        // (GROUPED: rows of the expert's stacked weight; a tile reaching past its N features loads the
+                        // next expert's codes, which the consumers give zero scales and the epilogue never stores)
+                        ptx::tma_load_2d(sw + slot * kWStageBytes, &tmap_w, &full[slot], kSS ? k0 : k0 / 2,
+                                         GROUPED ? w.wrow + w.n0 : w.n0);
                     }
 #pragma unroll
                     for (int h = 0; h < kBK / Cfg::kSubK; ++h)
@@ -321,6 +425,7 @@ __global__ void __launch_bounds__(kThreads, 1)
 
     // ====================================================================== consumers (warpgroups 1, 2)
     ptx::setmaxnreg_inc<kConsumerRegs>();
+    if constexpr (GROUPED) units = grouped_units<Cfg>(so, p);
     const int ct = threadIdx.x - 128;         // consumer thread 0..255
     const int wg = ct >> 7;                   // consumer warpgroup: feature rows [64 wg, 64 wg + 64) of the tile
     const int g = lane >> 2, t = lane & 3;
@@ -339,8 +444,9 @@ __global__ void __launch_bounds__(kThreads, 1)
         const int n0 = w.n0, m0 = w.m0, st_begin = w.st_begin, nst = w.nst;
         const int na = n0 + row0, nb = na + 8;
         const bool a_ok = na < p.N, b_ok = nb < p.N;
-        const long long e_a = (long long)(a_ok ? na : 0) * p.K;
-        const long long e_b = (long long)(b_ok ? nb : 0) * p.K;
+        // scale element base of the row: GROUPED counts from the start of the stacked weight, (e * N + n) * K
+        const long long e_a = (long long)((GROUPED ? w.wrow : 0) + (a_ok ? na : 0)) * p.K;
+        const long long e_b = (long long)((GROUPED ? w.wrow : 0) + (b_ok ? nb : 0)) * p.K;
 
         // Scales of one stage, one per (row, quantisation block): the 32 codes of a chunk lie inside one block (blocks
         // are >= 32 and aligned), and a block can begin only at a chunk q with (q & smask) == 0.  Fetched one stage ahead.
@@ -502,8 +608,11 @@ __global__ void __launch_bounds__(kThreads, 1)
         }
         if (splits == 1) {
             const T* bias = reinterpret_cast<const T*>(p.bias);
-            const float bias_a = (bias != nullptr && a_ok) ? DT<T>::to_f32(bias[na]) : 0.f;
-            const float bias_b = (bias != nullptr && b_ok) ? DT<T>::to_f32(bias[nb]) : 0.f;
+            // (GROUPED: the expert's weight row base and end row are looked up again rather than held through the
+            // main loop, where they would cost the plain-statistics instances a spill at MT = 64 and 128)
+            const Unit we = GROUPED ? unit_at(u) : w;
+            const float bias_a = (bias != nullptr && a_ok) ? DT<T>::to_f32(bias[(GROUPED ? we.wrow : 0) + na]) : 0.f;
+            const float bias_b = (bias != nullptr && b_ok) ? DT<T>::to_f32(bias[(GROUPED ? we.wrow : 0) + nb]) : 0.f;
             // Stage the rounded tile as [token][feature] rows -- once both warpgroups are done reading the previous
             // unit's tile there -- then store it in 16-byte row pieces of kVec elements: each token row of the tile is
             // 128 contiguous elements of the output.  (fp32: the bias is added in fp32 and nothing is rounded.)
@@ -522,7 +631,8 @@ __global__ void __launch_bounds__(kThreads, 1)
                 for (int idx = ct; idx < MT * (kTileN / kVec); idx += kConsumers) {
                     const int c = idx / (kTileN / kVec), n = n0 + kVec * (idx % (kTileN / kVec));
                     const int m = m0 + c;
-                    if (m >= p.M || n >= p.N) continue;
+                    // (GROUPED: rows past the expert's end are the next expert's, computed and discarded)
+                    if (m >= (GROUPED ? we.m_end : p.M) || n >= p.N) continue;
                     const uint8_t* src = so + c * kPitch + (n - n0) * (int)sizeof(T);
                     const long long o = (long long)m * p.ldc + n;
                     if (p.out_vec && n + kVec <= p.N) {
@@ -641,6 +751,16 @@ __global__ void __launch_bounds__(kThreads, 1)
             }
         }
     }
+    if constexpr (GROUPED) {
+        // rows [end_{E-1}, M) belong to no expert: zeros, each CTA's consumers storing a strided share
+        const int m_tail = group_table<Cfg>(so)[p.E - 1];
+        const long long n_tail = (long long)(p.M - m_tail) * p.N;
+        T* outp = reinterpret_cast<T*>(p.out);
+        for (long long i = (long long)blockIdx.x * kConsumers + ct; i < n_tail; i += (long long)gridDim.x * kConsumers) {
+            const long long m = m_tail + i / p.N;
+            outp[m * p.ldc + i % p.N] = DT<T>::from_f32(0.f);
+        }
+    }
 }
 
 // ------------------------------------------------------------------ host side
@@ -726,17 +846,20 @@ Workspace* get_workspace(cudaStream_t stream, size_t partial_bytes, size_t n_cou
 }
 
 // lda: A's row stride in elements (0 = K)
-template <typename T, int QT, int MT, bool DQ, bool PART>
+template <typename T, int QT, int MT, bool DQ, bool PART, bool GROUPED = false>
 bool launch_mt(const T* A, Gemm4Params& p, int force_splits, cudaStream_t stream, int lda = 0) {
     constexpr bool kSS = QT == kDecoded || QT == kDecodedT;
     using Cfg = StageCfg<T, MT, kSS>;
     constexpr int kBK = Cfg::kBK;
-    constexpr size_t smem_bytes = Cfg::kSmemBytes;
+    constexpr size_t smem_bytes = Cfg::kSmemBytes + (GROUPED ? kGroupTabBytes : 0);
+    static_assert(smem_bytes <= 227 * 1024, "shared memory");
+    static_assert(!GROUPED || (!kSS && !PART && !std::is_same<T, float>::value),
+                  "the grouped instances decode 4-bit codes to fp16 / bf16 and store T");
     // the shared-memory opt-in is PER DEVICE (one process may drive several GPUs)
     static bool attr_set[64] = {};
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return false;
-    auto kern = gemm4_tc_kernel<T, QT, MT, DQ, PART>;
+    auto kern = gemm4_tc_kernel<T, QT, MT, DQ, PART, GROUPED>;
     if (!attr_set[dev]) {
         if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes) != cudaSuccess) {
             set_last_error("gemm4_tc smem attr", cudaGetLastError());
@@ -761,9 +884,9 @@ bool launch_mt(const T* A, Gemm4Params& p, int force_splits, cudaStream_t stream
                             (uint32_t)kTileN, (uint32_t)kBK))
             return false;
     } else {
-        // packed codes as a [N, K/2] byte matrix, 128 x BK/2-byte boxes, BK/2-byte swizzle
-        if (!encode_tmap_2d(&tmap_w, p.B, 1, Cfg::kWRowBytes, (uint64_t)p.N, (uint64_t)p.K / 2, (uint64_t)p.K / 2,
-                            (uint32_t)kTileN, (uint32_t)Cfg::kWRowBytes))
+        // packed codes as a [N, K/2] byte matrix (GROUPED: [E * N, K/2]), 128 x BK/2-byte boxes, BK/2-byte swizzle
+        if (!encode_tmap_2d(&tmap_w, p.B, 1, Cfg::kWRowBytes, (uint64_t)p.N * (GROUPED ? p.E : 1), (uint64_t)p.K / 2,
+                            (uint64_t)p.K / 2, (uint32_t)kTileN, (uint32_t)Cfg::kWRowBytes))
             return false;
     }
     p.kblocks_total = (p.K + kBK - 1) / kBK;
@@ -774,14 +897,17 @@ bool launch_mt(const T* A, Gemm4Params& p, int force_splits, cudaStream_t stream
     if (kBK < gran) gran = kBK;
     p.scale_mask = gran / 32 - 1;
     const int n_tiles = (p.N + kTileN - 1) / kTileN;
-    const int m_tiles = (p.M + MT - 1) / MT;
+    // GROUPED: the m-tiles are counted on the device; each expert adds at most one partial tile, so ceil(M / MT) + E
+    // bounds them and sizes the grid
+    const int m_tiles = (p.M + MT - 1) / MT + (GROUPED ? p.E : 0);
     const int sms = device_sm_count();
     const int tiles = n_tiles * m_tiles;
 
     // K-splitting for small problems: a uniform split so that ONE wave covers the machine.  Split CTAs exchange
-    // fp32 partials through an L2-resident workspace and every split reduces its share of the columns.
+    // fp32 partials through an L2-resident workspace and every split reduces its share of the columns.  (The grouped
+    // instances never split K.)
     int splits = 1;
-    if (force_splits > 0 || tiles * 2 <= sms) {
+    if (!GROUPED && (force_splits > 0 || tiles * 2 <= sms)) {
         int v = force_splits > 0 ? force_splits : sms / tiles;
         // >= two stages per split by default, >= one when the split is forced
         const int max_by_k = force_splits > 0 ? p.kblocks_total : (p.kblocks_total / 2 > 0 ? p.kblocks_total / 2 : 1);
@@ -1056,6 +1182,72 @@ BNB200_TC_INST(__nv_bfloat16, true)
 BNB200_TC_INST(__half, true)
 BNB200_TC_INST(float, true)
 #undef BNB200_TC_INST
+
+// ------------------------------------------------------------------ the grouped GEMM
+// Every expert of a mixture-of-experts layer in one launch of the GROUPED instances (DESIGN.md section 3.1.2):
+// out[m, :] = T(A[m, :] . W_e^T + bias[e * N ..]) for end_{e-1} <= m < end_e, and 0 for end_{E-1} <= m < M, with
+// W_e rows [e * N, (e + 1) * N) of the stacked 4-bit weight and end_e the device-side clamp of offs (Gemm4Params).
+// Each expert's rows are bit for bit what launch_gemm4_tc gives on that expert alone at token tile mt and no K split.
+// mt: 16 | 32 | 64 | 128 (the caller's tile rule).  Returns false, with nothing launched, for what the instances do
+// not serve, or when the launch fails (the error message set).
+template <typename T>
+bool launch_gemm4_grouped(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
+                          const float* absmax_code, const float* absmax_offset, const int* offs, int E, T* out,
+                          const T* bias, int M, int N, int K, int ldc, int blocksize, int quant_type, int mt,
+                          cudaStream_t stream) {
+    static_assert(!std::is_same<T, float>::value, "the grouped GEMM has 16-bit instances only");
+    if (M <= 0) return true;
+    if (N <= 0 || E < 1 || E > kMaxExperts || (long long)E * N > 0x7fffffffLL || K < 64 || (K % 64) != 0) return false;
+    if (blocksize < 32 || (blocksize & (blocksize - 1)) != 0) return false;
+    if ((reinterpret_cast<uintptr_t>(A) & 15) != 0 || (reinterpret_cast<uintptr_t>(B) & 15) != 0) return false;
+    if (quant_type != kNF4 && quant_type != kFP4) return false;
+    Gemm4Params p{};
+    p.B = B;
+    p.absmax = absmax;
+    p.absmax_8bit = absmax_8bit;
+    p.absmax_code = absmax_code;
+    p.absmax_offset = absmax_offset;
+    p.bias = bias;
+    p.out = out;
+    p.M = M;
+    p.N = N;
+    p.K = K;
+    p.ldc = ldc;
+    p.log2_bs = ilog2_pow2(blocksize);
+    p.out_vec = ((ldc % (16 / (int)sizeof(T))) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0) ? 1 : 0;
+    p.offs = offs;
+    p.E = E;
+#define BNB200_GROUPED_MT(QT, DQ)                                                                                      \
+    switch (mt) {                                                                                                      \
+    case 16: return launch_mt<T, QT, 16, DQ, false, true>(A, p, 1, stream);                                            \
+    case 32: return launch_mt<T, QT, 32, DQ, false, true>(A, p, 1, stream);                                            \
+    case 64: return launch_mt<T, QT, 64, DQ, false, true>(A, p, 1, stream);                                            \
+    case 128: return launch_mt<T, QT, 128, DQ, false, true>(A, p, 1, stream);                                          \
+    default: return false;                                                                                             \
+    }
+    const bool dq = absmax_8bit != nullptr;
+    if (quant_type == kNF4) {
+        if (dq) {
+            BNB200_GROUPED_MT(kNF4, true)
+        } else {
+            BNB200_GROUPED_MT(kNF4, false)
+        }
+    } else {
+        if (dq) {
+            BNB200_GROUPED_MT(kFP4, true)
+        } else {
+            BNB200_GROUPED_MT(kFP4, false)
+        }
+    }
+#undef BNB200_GROUPED_MT
+}
+template bool launch_gemm4_grouped<__nv_bfloat16>(const __nv_bfloat16*, const uint8_t*, const float*, const uint8_t*,
+                                                  const float*, const float*, const int*, int, __nv_bfloat16*,
+                                                  const __nv_bfloat16*, int, int, int, int, int, int, int,
+                                                  cudaStream_t);
+template bool launch_gemm4_grouped<__half>(const __half*, const uint8_t*, const float*, const uint8_t*, const float*,
+                                           const float*, const int*, int, __half*, const __half*, int, int, int, int,
+                                           int, int, int, cudaStream_t);
 
 
 // ------------------------------------------------------------------ the input-gradient GEMM

@@ -7,6 +7,7 @@ from .embedding import (  # noqa: F401
     StableEmbedding,
 )
 from .modules import (  # noqa: F401
+    GroupedLinear4bit,
     Int8Params,
     Linear4bit,
     Linear8bitLt,

@@ -19,7 +19,7 @@ import torch
 from torch import nn
 
 from .. import functional as F
-from ..autograd._functions import MatmulLtState, matmul, matmul_4bit
+from ..autograd._functions import MatmulLtState, grouped_matmul_4bit, matmul, matmul_4bit
 from ..functional import QuantState
 
 logger = logging.getLogger(__name__)
@@ -207,18 +207,13 @@ class Linear4bit(nn.Linear):
 
     def _save_to_state_dict(self, destination, prefix, keep_vars):
         super()._save_to_state_dict(destination, prefix, keep_vars)
-        qs = getattr(self.weight, "quant_state", None)
-        if qs is not None:
-            for k, v in qs.as_dict(packed=True).items():
-                destination[prefix + "weight." + k] = v if keep_vars else v.detach()
+        _save_quant_state(self, destination, prefix, keep_vars)
 
-    def forward(self, x: torch.Tensor):
-        fix_4bit_weight_quant_state_from_module(self)
-        quant_state = self.weight.quant_state
+    def _compute_inputs(self, x: torch.Tensor):
+        """x and the bias in the compute dtype (set from the first input unless given)."""
         if not self.compute_type_is_set:
             self.set_compute_type(x)
             self.compute_type_is_set = True
-        inp_dtype = x.dtype
         if self.compute_dtype is not None:
             x = x.to(self.compute_dtype)
         bias = self.bias
@@ -226,7 +221,67 @@ class Linear4bit(nn.Linear):
             if bias.dtype != x.dtype:
                 bias.data = bias.data.to(x.dtype)
             bias = bias.to(self.compute_dtype)
+        return x, bias
+
+    def forward(self, x: torch.Tensor):
+        fix_4bit_weight_quant_state_from_module(self)
+        quant_state = self.weight.quant_state
+        inp_dtype = x.dtype
+        x, bias = self._compute_inputs(x)
         return matmul_4bit(x, self.weight, bias=bias, quant_state=quant_state).to(inp_dtype)
+
+
+def _save_quant_state(module: nn.Module, destination, prefix, keep_vars):
+    """The packed QuantState entries of a 4-bit weight next to it in the state dict (``weight.absmax`` ...), from which
+    ``Params4bit.from_prequantized`` rebuilds it."""
+    qs = getattr(module.weight, "quant_state", None)
+    if qs is not None:
+        for k, v in qs.as_dict(packed=True).items():
+            destination[prefix + "weight." + k] = v if keep_vars else v.detach()
+
+
+class GroupedLinear4bit(nn.Module):
+    """The experts of a mixture-of-experts layer on 4-bit weights: ``num_experts`` linear maps ``in_features ->
+    out_features`` stored as one ``[E, N, K]`` expert tensor, quantised as one tensor on the first move to CUDA (as
+    ``Linear4bit`` quantises its weight), with an optional ``[E, N]`` bias.  ``forward(x, offs)`` takes the
+    expert-sorted rows ``x [M, K]`` and the int32 end row of each expert ``offs [E]`` on the device, and returns
+    ``[M, N]``: every expert in one launch of the grouped GEMM (:func:`bitsandbytes_b200.grouped_matmul_4bit`).
+    Routing (top-k, sorting, scattering back with the router weights) stays with the model."""
+
+    def __init__(self, num_experts, in_features, out_features, bias=False, compute_dtype=None,
+                 compress_statistics=True, quant_type="fp4", quant_storage=torch.uint8, device=None):
+        super().__init__()
+        self.num_experts, self.in_features, self.out_features = num_experts, in_features, out_features
+        w = torch.empty((num_experts, out_features, in_features), device=device)
+        nn.init.kaiming_uniform_(w.view(-1, in_features), a=5**0.5)  # each expert initialised as nn.Linear's weight
+        self.weight = Params4bit(w, requires_grad=False, compress_statistics=compress_statistics, quant_type=quant_type,
+                                 quant_storage=quant_storage, module=self)
+        if bias:
+            bound = 1 / in_features**0.5 if in_features > 0 else 0
+            self.bias = nn.Parameter(torch.empty((num_experts, out_features), device=device).uniform_(-bound, bound))
+        else:
+            self.register_parameter("bias", None)
+        self.compute_dtype = compute_dtype
+        self.compute_type_is_set = compute_dtype is not None
+        self.quant_state = None
+        self.quant_storage = quant_storage
+
+    set_compute_type = Linear4bit.set_compute_type
+    _compute_inputs = Linear4bit._compute_inputs
+
+    def _save_to_state_dict(self, destination, prefix, keep_vars):
+        super()._save_to_state_dict(destination, prefix, keep_vars)
+        _save_quant_state(self, destination, prefix, keep_vars)
+
+    def extra_repr(self) -> str:
+        return (f"num_experts={self.num_experts}, in_features={self.in_features}, out_features={self.out_features}, "
+                f"bias={self.bias is not None}")
+
+    def forward(self, x: torch.Tensor, offs: torch.Tensor):
+        fix_4bit_weight_quant_state_from_module(self)
+        inp_dtype = x.dtype
+        x, bias = self._compute_inputs(x)
+        return grouped_matmul_4bit(x, self.weight, self.weight.quant_state, offs, bias=bias).to(inp_dtype)
 
 
 class LinearFP4(Linear4bit):

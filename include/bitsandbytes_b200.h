@@ -209,6 +209,25 @@ void cbnb_b200_gemm_4bit_force_path(int path);
  * the shape or the options are not served (a forced split must fit one co-resident wave of CTAs). */
 int cbnb_b200_gemm_4bit_pair(const void* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit, const float* absmax_code, const float* absmax_offset, void* out, const void* bias, int M, int N, int K, int ldc, int blocksize, int quant_type, int dtype, int mt, int force_splits, long long* trace, bnb_stream_t stream);
 
+/* Grouped 4-bit GEMM of a mixture-of-experts layer (no reference counterpart; the 4-bit form of grouped_mm with a 3-D
+ * weight): out[m, :] (row stride ldc) = T( A[m, :] . W_e^T (fp32 accumulation) + bias[e * N .. (e + 1) * N) ) for the
+ * rows of expert e, end_{e-1} <= m < end_e, and 0 for end_{E-1} <= m < M.  A is [M, K] fp16 / bf16 (dtype 1 / 2) with
+ * rows sorted by expert; B, absmax (and the nested statistics) are E experts' [N, K] weights quantised as ONE [E * N, K]
+ * tensor, expert e being rows [e * N, (e + 1) * N); bias is T[E * N] or NULL; offs is int32[E] on the device, offs[e]
+ * the end row of expert e, clamped on the device as end_e = min(max(offs[e], end_{e-1}), M) (end_{-1} = 0), so that no
+ * routing makes the kernel read or write outside its operands.  Each expert's rows are bit for bit those of
+ * cbnb_b200_gemm_4bit_pair on that expert alone at the same token tile with force_splits = 1.  Nothing is read back to
+ * the host: the call can be captured in a CUDA graph.  Returns 0, 1 with the error message set for bad arguments (NULL
+ * operand, M < 0, N, K or E < 1, ldc < N, bad quant_type, absmax_8bit without absmax_code), or 100 with nothing
+ * written for what it does not serve: fp32 A (dtype 0 / 3), K not a multiple of 64, E > 1024, a blocksize that is not a
+ * power of two >= 32, A or B not 16-byte aligned.  A failure past those checks (a tensor map the driver does not encode,
+ * a failed shared-memory opt-in or launch) also returns 100, with the error message set, as the input-gradient entries
+ * do: 100 with no message means "not served", 100 with a message an error (the Python layer polls the message first
+ * and raises it).  The _mt form is the test entry with token tile mt (16 | 32 | 64 |
+ * 128; 0 = the production rule, the smallest of those that holds 2 ceil(M / E) tokens). */
+int cbnb_b200_gemm_4bit_grouped(const void* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit, const float* absmax_code, const float* absmax_offset, const int* offs, int E, void* out, const void* bias, int M, int N, int K, int ldc, int blocksize, int quant_type, int dtype, bnb_stream_t stream);
+int cbnb_b200_gemm_4bit_grouped_mt(const void* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit, const float* absmax_code, const float* absmax_offset, const int* offs, int E, void* out, const void* bias, int M, int N, int K, int ldc, int blocksize, int quant_type, int dtype, int mt, bnb_stream_t stream);
+
 /* Developer / test entries for the staged route.  _staged: the whole route with token tile mt (128 | 256,
  * 0 = by the shape) and panel_rows output features per panel (a multiple of 128 whose decoded rows fit the 32 MB
  * per-stream workspace, 0 = the largest such), stores to outs[0..n_outs) as _multi_out; returns 0, or 100 when not
