@@ -321,45 +321,6 @@ def gemm_4bit_partial_scatter(A, B, shapeB, absmax, blocksize: int, quant_type: 
     return rc == 0
 
 
-def gemm_4bit_input_grad(G, B, shapeB, absmax, blocksize: int, quant_type: str, absmax_8bit, absmax_code,
-                         absmax_offset, out: torch.Tensor) -> bool:
-    """The input gradient of a 4-bit layer, ``out[m, k] = sum_n G[m, n] * dequant(B)[n, k]`` (the weight not
-    transposed), one fp32 sum per element.  ``G`` is ``[M, N]`` fp16 / bf16 with unit column stride and any row stride
-    (a column slice of a wider gradient is read in place); ``out`` is ``[M, K]`` with unit column stride, of G's dtype
-    (the sum rounded once) or fp32 (the sum as it is: a tensor-parallel layer's partial).  Returns False, with nothing
-    written, for what the kernel does not serve (fp32 ``G``, N or K not a multiple of 64, a row stride of G not a
-    multiple of 8, unaligned operands); the caller then takes another route.  A ``G`` whose rows are not unit-stride
-    runs of N elements (column-major, expanded, overlapping) raises: make it contiguous first."""
-    N, K = shapeB[0], shapeB[1]
-    if G.dim() != 2 or G.shape[1] != N or (G.shape[0] > 1 and (G.stride(1) != 1 or G.stride(0) < N)):
-        raise RuntimeError(f"gemm_4bit_input_grad: G must be [M, {N}] with unit column stride and row stride >= {N}, "
-                           f"got {tuple(G.shape)} strides {G.stride()}")
-    M = G.shape[0]
-    if out.shape != (M, K) or out.device != G.device or out.dtype not in (G.dtype, torch.float32) or (
-            M > 1 and out.stride(1) != 1):
-        raise RuntimeError(f"gemm_4bit_input_grad: out must be [{M}, {K}] of {G.dtype} or float32 with unit column "
-                           f"stride on {G.device}")
-    ldg = G.stride(0) if M > 1 else N
-    ldc = out.stride(0) if M > 1 else K
-    off = _weight_operands(absmax, blocksize, quant_type, absmax_8bit, absmax_code, absmax_offset)
-    B = B.contiguous()
-    _check_sizes("gemm_4bit_input_grad", M, N, K, ldg, ldc)
-    if G.dtype not in (torch.float16, torch.bfloat16):
-        return False
-    if M == 0:
-        return True
-    with _on_device(G):
-        rc = lib.cbnb_b200_gemm_4bit_input_grad(
-            G.data_ptr(), ldg, B.data_ptr(), absmax.data_ptr(),
-            absmax_8bit.data_ptr() if absmax_8bit is not None else None,
-            absmax_code.data_ptr() if absmax_code is not None else None,
-            off.data_ptr() if off is not None else None,
-            out.data_ptr(), ldc, M, N, K, blocksize, _QT_ID[quant_type], _DTYPE_ID[G.dtype],
-            int(out.dtype == torch.float32), _stream(G))
-    lib.check("gemm_4bit_input_grad")
-    return rc == 0
-
-
 def reduce_partials(parts: torch.Tensor, dtype: torch.dtype, bias: Optional[torch.Tensor] = None,
                     out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """``out = dtype((((parts[0] + parts[1]) + ...) + parts[w-1]) + bias)``: the ``[w, M, N]`` fp32 partials of a

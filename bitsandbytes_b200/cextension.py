@@ -72,10 +72,6 @@ def _signatures():
     # (A, B, absmax, absmax_8bit, absmax_code, absmax_offset, outs, n_outs, rows_per_out, M, N, K, ldc, blocksize,
     #  quant_type, dtype, stream) -> int
     sig["cbnb_b200_gemm_4bit_partial_scatter"] = ([_VOIDP] * 7 + [_I32] * 9 + [_VOIDP], _I32)
-    # (G, ldg, B, absmax, absmax_8bit, absmax_code, absmax_offset, out, ldc, M, N, K, blocksize, quant_type, dtype, part,
-    #  stream) -> int; the _panel form takes panel_cols before the stream
-    sig["cbnb_b200_gemm_4bit_input_grad"] = ([_VOIDP, _I32] + [_VOIDP] * 6 + [_I32] * 8 + [_VOIDP], _I32)
-    sig["cbnb_b200_gemm_4bit_input_grad_panel"] = ([_VOIDP, _I32] + [_VOIDP] * 6 + [_I32] * 9 + [_VOIDP], _I32)
     # (parts, world, part_stride, out, bias, M, N, ldc, dtype, stream) -> int
     sig["cbnb_b200_reduce_partials"] = ([_VOIDP, _I32, ct.c_longlong, _VOIDP, _VOIDP] + [_I32] * 4 + [_VOIDP], _I32)
     # (parts, n_parts, row0, rows, out, bias, M, N, ldc, dtype, stream) -> int

@@ -578,18 +578,14 @@ __global__ void __launch_bounds__(kDqThreads)
 // ScaleSrc::load_as<DQ>, the fetch of the fused GEMM (nested statistics included), and `e0` is the element index of
 // A[0] in the whole weight, so that scale indices count from the weight's start -- a panel may begin inside a
 // quantisation block.  e0 is a multiple of 64: a 64-element unit never straddles a block of >= 64 elements.
-// kCols (the input-gradient GEMM's panel, launch_dequantize4_cols): the units are those of columns [e0, e0 + 64 upr)
-// of every row of a weight with rows of row_len elements -- unit u is row u / upr, columns e0 + 64 (u % upr) -- and
-// A is the whole weight's codes; the output stays dense, [rows, 64 upr].
 constexpr int kD4Warps = 8;
 
-template <typename T, int QT, bool DQ, bool kCols>
-__device__ __forceinline__ void dequantize4_units(const uint8_t* __restrict__ A, const float* __restrict__ absmax,
-                                                  const uint8_t* __restrict__ absmax_8bit,
-                                                  const float* __restrict__ absmax_code,
-                                                  const float* __restrict__ absmax_offset, T* __restrict__ out,
-                                                  int log2_bs, long long n_units, long long e0, int upr,
-                                                  long long row_len) {
+template <typename T, int QT, bool DQ>
+__global__ void __launch_bounds__(kD4Warps * 32, 4)
+    dequantize4_prmt_kernel(const uint8_t* __restrict__ A, const float* __restrict__ absmax,
+                            const uint8_t* __restrict__ absmax_8bit, const float* __restrict__ absmax_code,
+                            const float* __restrict__ absmax_offset, T* __restrict__ out, int log2_bs,
+                            long long n_units /* 64-element units */, long long e0) {
     const ScaleSrc sc{absmax, absmax_8bit, absmax_code, (DQ && absmax_offset) ? __ldg(absmax_offset) : 0.f};
     __shared__ __align__(128) uint8_t stage[kD4Warps][4096];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -601,20 +597,11 @@ __device__ __forceinline__ void dequantize4_units(const uint8_t* __restrict__ A,
         uint4 q0 = make_uint4(0, 0, 0, 0), q1 = q0;
         float s0 = 0.f, s1 = 0.f;
         if (u < n_units) {
-            if constexpr (kCols) {
-                const long long row = u / upr;
-                const long long e = row * row_len + e0 + (u - row * upr) * 64;  // in the whole weight
-                q0 = __ldg(reinterpret_cast<const uint4*>(A + e / 2));
-                q1 = __ldg(reinterpret_cast<const uint4*>(A + e / 2 + 16));
-                s0 = sc.load_as<DQ>(e >> log2_bs);
-                if (two) s1 = sc.load_as<DQ>((e + 32) >> log2_bs);
-            } else {
-                // default caching: the two halves of a 32-byte sector are fetched by consecutive instructions
-                q0 = __ldg(reinterpret_cast<const uint4*>(A + u * 32));
-                q1 = __ldg(reinterpret_cast<const uint4*>(A + u * 32 + 16));
-                s0 = sc.load_as<DQ>((e0 + u * 64) >> log2_bs);
-                if (two) s1 = sc.load_as<DQ>((e0 + u * 64 + 32) >> log2_bs);
-            }
+            // default caching: the two halves of a 32-byte sector are fetched by consecutive instructions
+            q0 = __ldg(reinterpret_cast<const uint4*>(A + u * 32));
+            q1 = __ldg(reinterpret_cast<const uint4*>(A + u * 32 + 16));
+            s0 = sc.load_as<DQ>((e0 + u * 64) >> log2_bs);
+            if (two) s1 = sc.load_as<DQ>((e0 + u * 64 + 32) >> log2_bs);
         }
         uint32_t r[32];
         DecodeTable tab;
@@ -641,26 +628,6 @@ __device__ __forceinline__ void dequantize4_units(const uint8_t* __restrict__ A,
         }
         __syncwarp();
     }
-}
-
-template <typename T, int QT, bool DQ>
-__global__ void __launch_bounds__(kD4Warps * 32, 4)
-    dequantize4_prmt_kernel(const uint8_t* __restrict__ A, const float* __restrict__ absmax,
-                            const uint8_t* __restrict__ absmax_8bit, const float* __restrict__ absmax_code,
-                            const float* __restrict__ absmax_offset, T* __restrict__ out, int log2_bs,
-                            long long n_units /* 64-element units */, long long e0) {
-    dequantize4_units<T, QT, DQ, false>(A, absmax, absmax_8bit, absmax_code, absmax_offset, out, log2_bs, n_units, e0,
-                                        0, 0);
-}
-
-template <typename T, int QT, bool DQ>
-__global__ void __launch_bounds__(kD4Warps * 32, 4)
-    dequantize4_cols_kernel(const uint8_t* __restrict__ A, const float* __restrict__ absmax,
-                            const uint8_t* __restrict__ absmax_8bit, const float* __restrict__ absmax_code,
-                            const float* __restrict__ absmax_offset, T* __restrict__ out, int log2_bs,
-                            long long n_units, long long e0, int upr, long long row_len) {
-    dequantize4_units<T, QT, DQ, true>(A, absmax, absmax_8bit, absmax_code, absmax_offset, out, log2_bs, n_units, e0,
-                                       upr, row_len);
 }
 
 // Generic path: one element per thread; tail / unaligned / tiny or non-power-of-two blocks.
@@ -765,39 +732,6 @@ template void launch_dequantize4_panel<__half>(const uint8_t*, const float*, con
 template void launch_dequantize4_panel<__nv_bfloat16>(const uint8_t*, const float*, const uint8_t*, const float*,
                                                       const float*, __nv_bfloat16*, int, int, int, int, int,
                                                       cudaStream_t);
-
-// Columns [k0, k0 + cols) of every row of an [N, K] 4-bit weight (K, k0 and cols multiples of 64, codes 16-byte
-// aligned) decoded to T into out[N, cols], bit-identical to those columns of F.dequantize_4bit: the input-gradient
-// GEMM's panel.  absmax_8bit != NULL: nested statistics.
-template <typename T>
-void launch_dequantize4_cols(const uint8_t* codes, const float* absmax, const uint8_t* absmax_8bit,
-                             const float* absmax_code, const float* absmax_offset, T* out, int blocksize,
-                             int quant_type, int k0, int cols, int N, int K, cudaStream_t stream) {
-    const int upr = cols / 64;
-    const long long n_units = (long long)N * upr;
-    const long long want = (n_units + kD4Warps * 32 - 1) / (kD4Warps * 32);
-    const int sms = device_sm_count();
-    const int grid = (int)(want < (long long)sms * 4 ? want : (long long)sms * 4);
-    const int lbs = ilog2_pow2(blocksize);
-#define BNB200_COLS(QT, DQ)                                                                                            \
-    dequantize4_cols_kernel<T, QT, DQ><<<grid, kD4Warps * 32, 0, stream>>>(codes, absmax, absmax_8bit, absmax_code,    \
-                                                                           absmax_offset, out, lbs, n_units, k0, upr,  \
-                                                                           (long long)K)
-    if (absmax_8bit != nullptr) {
-        if (quant_type == kNF4) BNB200_COLS(kNF4, true);
-        else BNB200_COLS(kFP4, true);
-    } else {
-        if (quant_type == kNF4) BNB200_COLS(kNF4, false);
-        else BNB200_COLS(kFP4, false);
-    }
-#undef BNB200_COLS
-    BNB200_CHECK_LAUNCH("dequantize4_cols");
-}
-template void launch_dequantize4_cols<__half>(const uint8_t*, const float*, const uint8_t*, const float*, const float*,
-                                              __half*, int, int, int, int, int, int, cudaStream_t);
-template void launch_dequantize4_cols<__nv_bfloat16>(const uint8_t*, const float*, const uint8_t*, const float*,
-                                                     const float*, __nv_bfloat16*, int, int, int, int, int, int,
-                                                     cudaStream_t);
 
 #define INSTANTIATE(T)                                                                                                 \
     template void launch_quantize_blockwise<T, kGeneral8bit>(const float*, const T*, float*, uint8_t*, int, long long, \

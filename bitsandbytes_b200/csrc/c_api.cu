@@ -88,10 +88,6 @@ bool launch_gemm4_staged(const T* A, const uint8_t* B, const float* absmax, cons
                          const float* absmax_code, const float* absmax_offset, const OutList<OutElem<T, PART>>& outs,
                          const T* bias, int M, int N, int K, int ldc, int blocksize, int quant_type,
                          cudaStream_t stream, int mt_override = 0, int panel_rows = 0);
-template <typename T, bool PART>
-int launch_gemm4_input_grad(const T* G, int ldg, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
-                            const float* absmax_code, const float* absmax_offset, OutElem<T, PART>* out, int ldc, int M,
-                            int N, int K, int blocksize, int quant_type, cudaStream_t stream, int panel_cols);
 template <typename T>
 bool launch_gemm4_grouped(const T* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
                           const float* absmax_code, const float* absmax_offset, const int* offs, int E, T* out,
@@ -110,7 +106,6 @@ template <typename T>
 void launch_dequantize4_panel(const uint8_t* codes, const float* absmax, const uint8_t* absmax_8bit,
                               const float* absmax_code, const float* absmax_offset, T* out, int blocksize,
                               int quant_type, int n0, int rows, int K, cudaStream_t stream);
-int staged_max_panel_rows(int K, int elem_bytes);
 int staged_plan(int M, int N, int K, int sms, int* panel_rows);
 void launch_int8_vector_quant(const void* A, int8_t* out, float* rowStats, int* col_flags, float threshold, int rows,
                               int cols, int dtype, cudaStream_t stream);
@@ -379,33 +374,6 @@ template <unsigned kIds, typename F> static bool with_dtype(int dtype, F&& f) {
     return true;
 }
 
-// The input-gradient GEMM of the entries below: 0, 1 with the error message set for bad arguments, 100 when not served.
-static int gemm_4bit_input_grad(const void* G, int ldg, const uint8_t* B, const float* absmax,
-                                const uint8_t* absmax_8bit, const float* absmax_code, const float* absmax_offset,
-                                void* out, int ldc, int M, int N, int K, int blocksize, int quant_type, int dtype,
-                                int part, int panel_cols, cudaStream_t stream) {
-    if (G == nullptr || B == nullptr || absmax == nullptr || out == nullptr || M < 0 || N <= 0 || K <= 0 || ldg < N ||
-        ldc < K || (part != 0 && part != 1) || (quant_type != kFP4 && quant_type != kNF4) ||
-        (absmax_8bit != nullptr && absmax_code == nullptr)) {
-        set_last_error_msg("gemm_4bit_input_grad: needs G, B, absmax and out, M >= 0, N, K >= 1, ldg >= N, ldc >= K, "
-                           "part 0 or 1, quant_type 1 (FP4) or 2 (NF4), and absmax_code with absmax_8bit");
-        return 1;
-    }
-    int rc = 100;
-    with_dtype<kIdF16 | kIdBF16>(dtype, [&](auto t) {
-        using T = decltype(t);
-        if constexpr (!std::is_same<T, float>::value) {
-            rc = part ? launch_gemm4_input_grad<T, true>((const T*)G, ldg, B, absmax, absmax_8bit, absmax_code,
-                                                         absmax_offset, (float*)out, ldc, M, N, K, blocksize,
-                                                         quant_type, stream, panel_cols)
-                      : launch_gemm4_input_grad<T, false>((const T*)G, ldg, B, absmax, absmax_8bit, absmax_code,
-                                                          absmax_offset, (T*)out, ldc, M, N, K, blocksize, quant_type,
-                                                          stream, panel_cols);
-        }
-    });
-    return rc;
-}
-
 // The grouped GEMM's token tile: the smallest of 16, 32, 64 and 128 tokens that holds twice the mean rows per expert,
 // 2 ceil(M / E), since under top-k routing many experts get more rows than the mean.  Measured on an H100
 // (tools/time_grouped_gemm4.py, DESIGN.md section 7): at a mean of 16 rows the 32-token tile is the fastest (Qwen3-30B-A3B,
@@ -646,31 +614,6 @@ int cbnb_b200_reduce_partials_ptrs(const float* const* parts, int n_parts, int r
         return 1;
     }
     return launch_reduce_partials_ptrs(parts, n_parts, row0, rows, out, bias, N, ldc, dtype, stream) ? 0 : 100;
-}
-
-// The input gradient of a 4-bit linear layer: out[m, k] (row stride ldc) = sum over n of G[m, n] * dequant(W)[n, k],
-// W the packed [N, K] weight, G [M, N] fp16 / bf16 at row stride ldg.  part = 0: out is of G's dtype, the fp32 sum
-// rounded once; part = 1: out is fp32, the sum as it is (the partial a tensor-parallel layer reduces in rank order).
-// Returns 0, 1 with the error message set for bad arguments, or 100, with nothing written, for a dtype (fp32 among
-// them) or a shape the kernel does not serve: N or K not a multiple of 64, ldg not a multiple of 8, G or B not
-// 16-byte aligned.  A failure past those checks (no workspace, a failed launch) returns 100 with the error message set.
-int cbnb_b200_gemm_4bit_input_grad(const void* G, int ldg, const uint8_t* B, const float* absmax,
-                                   const uint8_t* absmax_8bit, const float* absmax_code, const float* absmax_offset,
-                                   void* out, int ldc, int M, int N, int K, int blocksize, int quant_type, int dtype,
-                                   int part, cudaStream_t stream) {
-    return gemm_4bit_input_grad(G, ldg, B, absmax, absmax_8bit, absmax_code, absmax_offset, out, ldc, M, N, K,
-                                blocksize, quant_type, dtype, part, 0, stream);
-}
-
-// Developer / test entry: cbnb_b200_gemm_4bit_input_grad with a chosen panel of weight columns (panel_cols: a
-// multiple of 128 whose decoded columns fit the 32 MB workspace, 0 = the production choice); 100 for any other.
-int cbnb_b200_gemm_4bit_input_grad_panel(const void* G, int ldg, const uint8_t* B, const float* absmax,
-                                         const uint8_t* absmax_8bit, const float* absmax_code,
-                                         const float* absmax_offset, void* out, int ldc, int M, int N, int K,
-                                         int blocksize, int quant_type, int dtype, int part, int panel_cols,
-                                         cudaStream_t stream) {
-    return gemm_4bit_input_grad(G, ldg, B, absmax, absmax_8bit, absmax_code, absmax_offset, out, ldc, M, N, K,
-                                blocksize, quant_type, dtype, part, panel_cols, stream);
 }
 
 // Developer / test entry: the tensor-core kernel of gemm4_tc.cu with an explicit token tile (mt = 16 | 32 | 64 |

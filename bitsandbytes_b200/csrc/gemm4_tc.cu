@@ -42,8 +42,7 @@
 //
 // QT = kDecoded is the staged instance of the large-M route (launch_gemm4_staged, below): the weights arrive already
 // decoded, as a [N, K] panel that the producer loads like the activations, and both wgmma operands come from shared
-// memory.  QT = kDecodedT is its input-gradient form (launch_gemm4_input_grad, at the end): the panel is [contraction,
-// features] and the A operand is read MN-major.
+// memory.
 //
 // PART is the partial instance (cbnb_b200_gemm_4bit_partial, a row-sharded layer's K slice): the output and its
 // copies are fp32, and the epilogue stores the accumulators -- the split order's sums under split-K -- with no bias
@@ -64,11 +63,6 @@ template <typename T>
 void launch_dequantize4_panel(const uint8_t* codes, const float* absmax, const uint8_t* absmax_8bit,
                               const float* absmax_code, const float* absmax_offset, T* out, int blocksize,
                               int quant_type, int n0, int rows, int K, cudaStream_t stream);
-// blockwise.cu: columns [k0, k0 + cols) of every row of a 4-bit weight decoded to T, out[N, cols]
-template <typename T>
-void launch_dequantize4_cols(const uint8_t* codes, const float* absmax, const uint8_t* absmax_8bit,
-                             const float* absmax_code, const float* absmax_offset, T* out, int blocksize,
-                             int quant_type, int k0, int cols, int N, int K, cudaStream_t stream);
 
 namespace {
 
@@ -82,9 +76,6 @@ static_assert(128 * kProducerRegs + kConsumers * kConsumerRegs <= 65536, "regist
 constexpr int kBarEpi = 1;    // named barrier of the consumers' epilogue
 // QT of the staged instance: the weights arrive already decoded to T, a [N, K] panel (launch_gemm4_staged)
 constexpr int kDecoded = -1;
-// QT of the input-gradient instance (launch_gemm4_input_grad): the decoded panel is [contraction, features], the A
-// operand read MN-major
-constexpr int kDecodedT = -2;
 
 struct Gemm4Params {
     const uint8_t* B;            // packed codes [N, K/2]
@@ -133,16 +124,15 @@ __device__ __forceinline__ void store_partial(const Gemm4Params& p, int m, int n
     }
 }
 
-// the staged instance: D[64 x MT] += A[64 x 16] * X[MT x 16]^T with both operands from descriptors (A MN-major for
-// kTnspA = 1)
-template <typename T, int MT, int kTnspA = 0>
+// the staged instance: D[64 x MT] += A[64 x 16] * X[MT x 16]^T with both operands from descriptors
+template <typename T, int MT>
 __device__ __forceinline__ void wgmma_step_ss(float (&d)[MT / 2], uint64_t a_desc, uint64_t b_desc) {
     constexpr bool bf = std::is_same<T, __nv_bfloat16>::value;
     static_assert(MT == 128 || MT == 256, "staged token tile");
     if constexpr (MT == 128) {
-        if constexpr (bf) ptx::wgmma_m64n128k16_bf16_ss<kTnspA>(d, a_desc, b_desc); else ptx::wgmma_m64n128k16_f16_ss<kTnspA>(d, a_desc, b_desc);
+        if constexpr (bf) ptx::wgmma_m64n128k16_bf16_ss(d, a_desc, b_desc); else ptx::wgmma_m64n128k16_f16_ss(d, a_desc, b_desc);
     } else {
-        if constexpr (bf) ptx::wgmma_m64n256k16_bf16_ss<kTnspA>(d, a_desc, b_desc); else ptx::wgmma_m64n256k16_f16_ss<kTnspA>(d, a_desc, b_desc);
+        if constexpr (bf) ptx::wgmma_m64n256k16_bf16_ss(d, a_desc, b_desc); else ptx::wgmma_m64n256k16_f16_ss(d, a_desc, b_desc);
     }
 }
 
@@ -241,9 +231,7 @@ template <typename T, int QT, int MT, bool DQ, bool PART, bool GROUPED = false>
 __global__ void __launch_bounds__(kThreads, 1)
     gemm4_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
                     const Gemm4Params p) {
-    // the staged instances: weights from a decoded panel, no decode here; kMN: the panel is [contraction, features]
-    constexpr bool kSS = QT == kDecoded || QT == kDecodedT;
-    constexpr bool kMN = QT == kDecodedT;
+    constexpr bool kSS = QT == kDecoded;  // the staged instance: weights from a decoded panel, no decode here
     using Cfg = StageCfg<T, MT, kSS>;
     constexpr bool kTf32 = Cfg::kTf32;
     constexpr int kBK = Cfg::kBK;
@@ -396,18 +384,10 @@ __global__ void __launch_bounds__(kThreads, 1)
                     ptx::mbar_arrive_expect_tx(&full[slot], kWStageBytes + kXStageBytes);
                     // rows past M, rows past N and columns past K are out of bounds for the tensor maps: TMA
                     // zero-fills.  Packed codes of the tile's 128 output features: bytes [k0/2, k0/2 + BK/2).
-                    if constexpr (kMN) {
-                        // the [BK x 64] panel boxes of the two warpgroups' features: contraction rows k0.., 128-byte
-                        // rows of 64 features
-#pragma unroll
-                        for (int h = 0; h < 2; ++h)
-                            ptx::tma_load_2d(sw + slot * kWStageBytes + h * kBK * 128, &tmap_w, &full[slot], w.n0 + 64 * h, k0);
-                    } else {
-                        // (GROUPED: rows of the expert's stacked weight; a tile reaching past its N features loads the
-                        // next expert's codes, which the consumers give zero scales and the epilogue never stores)
-                        ptx::tma_load_2d(sw + slot * kWStageBytes, &tmap_w, &full[slot], kSS ? k0 : k0 / 2,
-                                         GROUPED ? w.wrow + w.n0 : w.n0);
-                    }
+                    // (GROUPED: rows of the expert's stacked weight; a tile reaching past its N features loads the
+                    // next expert's codes, which the consumers give zero scales and the epilogue never stores)
+                    ptx::tma_load_2d(sw + slot * kWStageBytes, &tmap_w, &full[slot], kSS ? k0 : k0 / 2,
+                                     GROUPED ? w.wrow + w.n0 : w.n0);
 #pragma unroll
                     for (int h = 0; h < kBK / Cfg::kSubK; ++h)
                         ptx::tma_load_2d(sx + slot * kXStageBytes + h * kXSubBytes, &tmap_x, &full[slot],
@@ -517,14 +497,7 @@ __global__ void __launch_bounds__(kThreads, 1)
         auto mma_stage = [&](int s, const uint32_t (&a)[kSteps][4]) {
             const uint32_t xs = ptx::smem_u32(sx + s * kXStageBytes);
             ptx::wgmma_fence();
-            if constexpr (kMN) {
-                // this warpgroup's [BK x 64] box: a k16 step is 16 of its 128-byte rows, two 1024-byte swizzle atoms
-                const uint32_t wa = ptx::smem_u32(sw + s * kWStageBytes + wg * kBK * 128);
-                const uint64_t a_desc = ptx::make_sw128_mnmajor_desc(wa, kBK * 128);
-#pragma unroll
-                for (int j = 0; j < kSteps; ++j)
-                    wgmma_step_ss<T, MT, 1>(acc, a_desc + 128 * j, ptx::make_sw128_kmajor_desc(xs) + 2 * j);
-            } else if constexpr (kSS) {
+            if constexpr (kSS) {
                 // this warpgroup's 64 weight rows: 8 KB into the stage's tile, a 1024-byte-aligned swizzle atom group
                 const uint64_t a_desc = ptx::make_sw128_kmajor_desc(ptx::smem_u32(sw + s * kWStageBytes + wg * 64 * 128));
 #pragma unroll
@@ -845,10 +818,9 @@ Workspace* get_workspace(cudaStream_t stream, size_t partial_bytes, size_t n_cou
     return &e->ws;
 }
 
-// lda: A's row stride in elements (0 = K)
 template <typename T, int QT, int MT, bool DQ, bool PART, bool GROUPED = false>
-bool launch_mt(const T* A, Gemm4Params& p, int force_splits, cudaStream_t stream, int lda = 0) {
-    constexpr bool kSS = QT == kDecoded || QT == kDecodedT;
+bool launch_mt(const T* A, Gemm4Params& p, int force_splits, cudaStream_t stream) {
+    constexpr bool kSS = QT == kDecoded;
     using Cfg = StageCfg<T, MT, kSS>;
     constexpr int kBK = Cfg::kBK;
     constexpr size_t smem_bytes = Cfg::kSmemBytes + (GROUPED ? kGroupTabBytes : 0);
@@ -869,16 +841,10 @@ bool launch_mt(const T* A, Gemm4Params& p, int force_splits, cudaStream_t stream
     }
     CUtensorMap tmap, tmap_w;
     // activations [M, K]: MT x kSubK boxes (128-byte rows), 128-byte swizzle (fp32 for the TF32 instance)
-    if (!encode_tmap_2d(&tmap, A, (int)sizeof(T), 128, (uint64_t)p.M, (uint64_t)p.K,
-                        (uint64_t)(lda > 0 ? lda : p.K) * sizeof(T), (uint32_t)MT, (uint32_t)Cfg::kSubK))
+    if (!encode_tmap_2d(&tmap, A, (int)sizeof(T), 128, (uint64_t)p.M, (uint64_t)p.K, (uint64_t)p.K * sizeof(T),
+                        (uint32_t)MT, (uint32_t)Cfg::kSubK))
         return false;
-    if constexpr (QT == kDecodedT) {
-        // the decoded panel [K, N] of T (contraction rows, N = the panel's features), BK x 64 boxes (128-byte rows),
-        // 128-byte swizzle
-        if (!encode_tmap_2d(&tmap_w, p.B, (int)sizeof(T), 128, (uint64_t)p.K, (uint64_t)p.N, (uint64_t)p.N * sizeof(T),
-                            (uint32_t)kBK, 64u))
-            return false;
-    } else if constexpr (kSS) {
+    if constexpr (kSS) {
         // the decoded panel [N, K] of T, 128 x 64 boxes (128-byte rows), 128-byte swizzle
         if (!encode_tmap_2d(&tmap_w, p.B, (int)sizeof(T), 128, (uint64_t)p.N, (uint64_t)p.K, (uint64_t)p.K * sizeof(T),
                             (uint32_t)kTileN, (uint32_t)kBK))
@@ -1248,77 +1214,5 @@ template bool launch_gemm4_grouped<__nv_bfloat16>(const __nv_bfloat16*, const ui
 template bool launch_gemm4_grouped<__half>(const __half*, const uint8_t*, const float*, const uint8_t*, const float*,
                                            const float*, const int*, int, __half*, const __half*, int, int, int, int,
                                            int, int, int, cudaStream_t);
-
-
-// ------------------------------------------------------------------ the input-gradient GEMM
-// out[m, k] = sum_n G[m, n] * W[n, k] for a packed 4-bit W[N, K]: the product with the weight NOT transposed (the input
-// gradient of y = x W^T), contracted over the output features n.  The staged route turned around: it loops over panels
-// of `panel_cols` columns of W (a multiple of 128), decodes all N rows of the panel into the stream's workspace block
-// (launch_dequantize4_cols: the bits of F.dequantize_4bit) and runs the kDecodedT instance of gemm4_tc_kernel, whose A
-// operand is the panel read MN-major (its 128 features of a tile are two 64-column TMA boxes) and whose B operand is G,
-// K-major over n like the forward's activations.  The contraction is never split: every output element is one fp32
-// sum over n in the same k16 order whatever the panel, and PART stores it as it is while T rounds it once.
-// Limits: N % 64 == 0, K % 64 == 0, G and W 16-byte aligned, ldg % 8 == 0, 16-bit G; returns 100 outside them, before
-// anything is written, and 0 otherwise.  A workspace that cannot be had or a launch that fails also returns 100, with
-// the error message set.  panel_cols 0: the panel of staged_plan.
-template <typename T, bool PART>
-int launch_gemm4_input_grad(const T* G, int ldg, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit,
-                            const float* absmax_code, const float* absmax_offset, OutElem<T, PART>* out, int ldc, int M,
-                            int N, int K, int blocksize, int quant_type, cudaStream_t stream, int panel_cols) {
-    static_assert(!std::is_same<T, float>::value, "the input-gradient GEMM has 16-bit instances only");
-    if (M <= 0) return 0;
-    if (N < 64 || (N % 64) != 0 || K < 64 || (K % 64) != 0 || (ldg % 8) != 0) return 100;
-    if (blocksize < 32 || (blocksize & (blocksize - 1)) != 0) return 100;
-    if ((reinterpret_cast<uintptr_t>(G) & 15) != 0 || (reinterpret_cast<uintptr_t>(B) & 15) != 0) return 100;
-    if (quant_type != kNF4 && quant_type != kFP4) return 100;
-    const int max_cols = staged_max_panel_rows(N, (int)sizeof(T));
-    const int sms = device_sm_count();
-    if (panel_cols == 0) staged_plan(M, K, N, sms, &panel_cols);
-    if (panel_cols <= 0 || panel_cols % kTileN != 0 || panel_cols > max_cols) return 100;
-    const int k_pad = (K + kTileN - 1) / kTileN * kTileN;
-    if (panel_cols > k_pad) panel_cols = k_pad;
-    // 256-token tiles where the whole output's tiles fill the SMs, as on the staged route
-    const int MT = (long long)((M + 255) / 256) * (k_pad / kTileN) >= sms ? 256 : 128;
-    Workspace* ws = get_workspace(stream, (size_t)panel_cols * N * sizeof(T), 0);
-    if (ws == nullptr) {
-        set_last_error_msg("gemm4_tc: could not allocate the input-gradient GEMM's workspace");
-        return 100;
-    }
-    T* panel = reinterpret_cast<T*>(ws->ptr);
-    const bool vec = !PART && (ldc % 8) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0;
-    for (int k0 = 0; k0 < K; k0 += panel_cols) {
-        const int cols = K - k0 < panel_cols ? K - k0 : panel_cols;
-        launch_dequantize4_cols<T>(B, absmax, absmax_8bit, absmax_code, absmax_offset, panel, blocksize, quant_type,
-                                   k0, cols, N, K, stream);
-        // the panel's columns of the output: k0 is a multiple of 128, so the base keeps its 16-byte alignment
-        Gemm4Params p{};
-        p.B = reinterpret_cast<const uint8_t*>(panel);
-        p.out = out + k0;
-        p.M = M;
-        p.N = cols;
-        p.K = N;
-        p.ldc = ldc;
-        p.log2_bs = ilog2_pow2(blocksize);
-        p.out_vec = vec ? 1 : 0;
-        const bool ok = MT == 256 ? launch_mt<T, kDecodedT, 256, false, PART>(G, p, 1, stream, ldg)
-                                  : launch_mt<T, kDecodedT, 128, false, PART>(G, p, 1, stream, ldg);
-        if (!ok) {
-            // every check passed before the first panel: a launch that fails here is an error, not a shape the kernel
-            // declines, and earlier panels may already be in out
-            set_last_error_msg("gemm4_tc: an input-gradient GEMM panel failed to launch");
-            return 100;
-        }
-    }
-    return 0;
-}
-#define BNB200_IG_INST(T, PART)                                                                                        \
-    template int launch_gemm4_input_grad<T, PART>(const T*, int, const uint8_t*, const float*, const uint8_t*,         \
-                                                  const float*, const float*, OutElem<T, PART>*, int, int, int, int,   \
-                                                  int, int, cudaStream_t, int);
-BNB200_IG_INST(__nv_bfloat16, false)
-BNB200_IG_INST(__half, false)
-BNB200_IG_INST(__nv_bfloat16, true)
-BNB200_IG_INST(__half, true)
-#undef BNB200_IG_INST
 
 } // namespace bnb200

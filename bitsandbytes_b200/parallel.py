@@ -72,9 +72,9 @@ result's rows bit for bit.  The row layer needs no exchange, ``grad_x_r = grad_y
 all-gather of ``grad_y``'s token rows under sequence parallelism; with ``input_is_parallel=False`` (the whole replicated
 input, of which the layer uses its columns) the ranks' ``grad_x_r`` are all-gathered along the features, in rank order,
 into the whole input gradient.  Both products run as dequantise + cuBLAS (:func:`input_grad_dequant_matmul`, chosen in
-``_input_grad`` from the timings against the library's input-gradient kernel, ``gemm_4bit_input_grad``).  The
-tensor-parallel LLM.int8() layers below share this backward (``_ColumnInputGrad``, ``_RowInputGrad``); only the
-dequantised weight differs (``Shard4bit.dequantize``, ``Shard8bit.dequantize``).
+``_input_grad`` from timings against a fused 4-bit input-gradient kernel, DESIGN.md section 6).  The tensor-parallel
+LLM.int8() layers below share this backward (``_ColumnInputGrad``, ``_RowInputGrad``); only the dequantised weight
+differs (``Shard4bit.dequantize``, ``Shard8bit.dequantize``).
 
 The ``fused_forward*`` routes train when given ``grad_peers`` (:class:`PeerInputGrad`, two symmetric-memory slots): the
 forward and the backward are the layer's, through the same ``torch.autograd.Function``, each with its exchange through
@@ -375,11 +375,10 @@ def input_grad_dequant_matmul(G: torch.Tensor, shard, dtype: torch.dtype) -> tor
 
 def _input_grad(G: torch.Tensor, shard, out: torch.Tensor) -> torch.Tensor:
     """``out[M, K] = G . W`` (``G`` ``[M, rows]`` in any layout, ``shard`` a Shard4bit or Shard8bit): fp32 ``out``
-    receives the unrounded partial, one of G's dtype the sum rounded once.  The route is chosen here, from the timings
-    on an H100 (DESIGN.md section 6, tools/time_gemm4_input_grad.py): dequantise + cuBLAS -- with an fp32 output from
-    the 16-bit operands for a partial -- is as fast as the 4-bit input-gradient kernel or faster at every shape and
-    token count measured but one (4096 x 4096 at 256 tokens, not a range of M), so the layers take it at every M; the
-    kernel (``gemm_4bit_input_grad``) stays in the library.  The int8 layers have no other route."""
+    receives the unrounded partial, one of G's dtype the sum rounded once.  The route is dequantise + cuBLAS -- with an
+    fp32 output from the 16-bit operands for a partial -- at every M: on an H100 it was as fast as a fused 4-bit
+    input-gradient kernel or faster at every shape and token count measured but one (4096 x 4096 at 256 tokens, not a
+    range of M; DESIGN.md section 6), and that kernel was removed.  The int8 layers have no other route."""
     out.copy_(input_grad_dequant_matmul(G, shard, out.dtype))
     return out
 

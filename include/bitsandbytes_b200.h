@@ -164,18 +164,6 @@ int cbnb_b200_gemm_4bit_partial(const void* A, const uint8_t* B, const float* ab
  * does not serve. */
 int cbnb_b200_gemm_4bit_partial_scatter(const void* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit, const float* absmax_code, const float* absmax_offset, float* const* outs, int n_outs, int rows_per_out, int M, int N, int K, int ldc, int blocksize, int quant_type, int dtype, bnb_stream_t stream);
 
-/* Input gradient of a 4-bit linear layer (no reference counterpart; the layers of parallel.py train through it):
- * out[m, k] (row stride ldc) = sum_n G[m, n] * W[n, k], W the packed [N, K] weight decoded as F.dequantize_4bit does,
- * G [M, N] fp16 / bf16 (dtype 1 / 2) at row stride ldg, accumulated in fp32 over n in one fixed order.  part = 0: out is
- * of G's dtype, the sum rounded once; part = 1: out is fp32, the sum unrounded (a tensor-parallel layer's partial).
- * Returns 0, 1 with the error message set for bad arguments (NULL operand, ldg < N, ldc < K, part not 0/1, bad
- * quant_type), or 100 with nothing written for what the kernel does not serve: fp32 G, N or K not a multiple of 64, ldg
- * not a multiple of 8, G or B not 16-byte aligned; a failure past those checks (no workspace, a failed launch) returns
- * 100 with the error message set.  The _panel form is the test entry that fixes the panel of decoded
- * weight columns (a multiple of 128; 0 = the production choice). */
-int cbnb_b200_gemm_4bit_input_grad(const void* G, int ldg, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit, const float* absmax_code, const float* absmax_offset, void* out, int ldc, int M, int N, int K, int blocksize, int quant_type, int dtype, int part, bnb_stream_t stream);
-int cbnb_b200_gemm_4bit_input_grad_panel(const void* G, int ldg, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit, const float* absmax_code, const float* absmax_offset, void* out, int ldc, int M, int N, int K, int blocksize, int quant_type, int dtype, int part, int panel_cols, bnb_stream_t stream);
-
 /* out[m, n] (row stride ldc) = T( (((P_0 + P_1) + ...) + P_{world-1})[m, n] + bias[n] ), P_r = parts + r * part_stride,
  * each [M, N] fp32 with row stride N: the partials summed in rank order in fp32, the bias (T[N] or NULL) added in fp32,
  * one rounding to T.  dtype 0 or 3 = fp32, 1 = fp16, 2 = bf16.  Returns 0, or 100 for a dtype or argument it does not
@@ -221,9 +209,8 @@ int cbnb_b200_gemm_4bit_pair(const void* A, const uint8_t* B, const float* absma
  * operand, M < 0, N, K or E < 1, ldc < N, bad quant_type, absmax_8bit without absmax_code), or 100 with nothing
  * written for what it does not serve: fp32 A (dtype 0 / 3), K not a multiple of 64, E > 1024, a blocksize that is not a
  * power of two >= 32, A or B not 16-byte aligned.  A failure past those checks (a tensor map the driver does not encode,
- * a failed shared-memory opt-in or launch) also returns 100, with the error message set, as the input-gradient entries
- * do: 100 with no message means "not served", 100 with a message an error (the Python layer polls the message first
- * and raises it).  The _mt form is the test entry with token tile mt (16 | 32 | 64 |
+ * a failed shared-memory opt-in or launch) also returns 100, with the error message set: 100 with no message means
+ * "not served", 100 with a message an error (the Python layer polls the message first and raises it).  The _mt form is the test entry with token tile mt (16 | 32 | 64 |
  * 128; 0 = the production rule, the smallest of those that holds 2 ceil(M / E) tokens). */
 int cbnb_b200_gemm_4bit_grouped(const void* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit, const float* absmax_code, const float* absmax_offset, const int* offs, int E, void* out, const void* bias, int M, int N, int K, int ldc, int blocksize, int quant_type, int dtype, bnb_stream_t stream);
 int cbnb_b200_gemm_4bit_grouped_mt(const void* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit, const float* absmax_code, const float* absmax_offset, const int* offs, int E, void* out, const void* bias, int M, int N, int K, int ldc, int blocksize, int quant_type, int dtype, int mt, bnb_stream_t stream);

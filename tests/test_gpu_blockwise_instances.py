@@ -10,7 +10,7 @@ kernel                                     one grid-stride round                
 quantize_blockwise_kernel                  grid x kQThreads x kQEPT = 4096 elements     8 S CTAs
 quantize_blockwise_generic_kernel          grid x 8 warps, one quant block per warp     8 S CTAs
 dequantize_blockwise_kernel                grid x kDqThreads x kDqUnroll 16-byte vectors 8 S CTAs
-dequantize4_prmt_kernel / _cols_kernel     grid x kD4Warps x 32 units of 64 elements    4 S CTAs
+dequantize4_prmt_kernel                    grid x kD4Warps x 32 units of 64 elements    4 S CTAs
 dequantize_blockwise_generic_kernel        grid x 256 elements                          8 S CTAs
 =========================================  =========================================  ===========================
 
@@ -39,7 +39,6 @@ dequantize_blockwise_kernel<float, QT>          test_dequantize_rounds (4-bit fp
 dequantize_blockwise_kernel<T16, QT>            test_dequantize_rounds (codes + 8 bytes, blocksize 16)
 dequantize_blockwise_generic_kernel<T, QT>      test_dequantize_rounds (tails), test_dequantize_generic_routes
 dequantize4_prmt_kernel<T16, QT, true>          test_nested_panel_decode
-dequantize4_cols_kernel<T16, QT, DQ>            test_input_grad_panel_decode
 ==============================================  ================================================================
 
 Every output buffer carries a guard region past its end (quantize: codes and absmax; dequantize: the output, filled
@@ -204,19 +203,19 @@ def build_dequantize(dtype, qt, n, bs, seed, codes_off=0, out_off=0):
     return inputs, lambda: dequantize_guarded(nat.lib, codes, absmax, bs, n, qt, dtype, code, out_off)
 
 
-def _nested_weight(N, K, qt, dtype, bs, nested, seed):
+def _nested_weight(N, K, qt, dtype, bs, seed):
     import bitsandbytes_b200.functional as F
 
     g = torch.Generator(device="cpu").manual_seed(seed)
     W = torch.randn(N, K, generator=g).to(nat.DTYPE[dtype]).cuda()
-    qW, qs = F.quantize_4bit(W, blocksize=bs, quant_type=qt, compress_statistics=nested)
+    qW, qs = F.quantize_4bit(W, blocksize=bs, quant_type=qt, compress_statistics=True)
     del W
     return qW, qs
 
 
 def build_panel(dtype, qt, bs, N, K, n0, rows, seed):
     """Rows [n0, n0 + rows) of an [N, K] weight quantised with nested statistics, through the panel entry."""
-    qW, qs = _nested_weight(N, K, qt, dtype, bs, True, seed)
+    qW, qs = _nested_weight(N, K, qt, dtype, bs, seed)
     off = qs.offset.to(torch.float32).reshape(1).contiguous()
 
     def go():
@@ -232,27 +231,7 @@ def build_panel(dtype, qt, bs, N, K, n0, rows, seed):
     return dict(qW=qW, qs=qs), go
 
 
-def build_cols(dtype, qt, bs, nested, seed, N=4096, K=4096, panel=4096):
-    """The input-gradient GEMM with G = the identity and one panel of `panel` columns: out = the decoded weight."""
-    qW, qs = _nested_weight(N, K, qt, dtype, bs, nested, seed)
-    G = torch.eye(N, device="cuda", dtype=nat.DTYPE[dtype])
-    off = qs.offset.to(torch.float32).reshape(1).contiguous() if nested else None
-
-    def go():
-        out = torch.full((N, K), float("nan"), device="cuda", dtype=nat.DTYPE[dtype])
-        rc = nat.lib.cbnb_b200_gemm_4bit_input_grad_panel(
-            G.data_ptr(), N, qW.data_ptr(), (qs.state2.absmax if nested else qs.absmax).data_ptr(),
-            qs.absmax.data_ptr() if nested else None, qs.state2.code.data_ptr() if nested else None, nat.ptr(off),
-            out.data_ptr(), K, N, N, K, bs, nat.QT_ID[qt], nat.DTYPE_ID[dtype], 0, panel, nat.stream())
-        sync()
-        nat.check()
-        assert rc == 0
-        return out
-
-    return dict(qW=qW, qs=qs, G=G), go
-
-
-BUILDERS = {"quantize": build_quantize, "dequantize": build_dequantize, "panel": build_panel, "cols": build_cols}
+BUILDERS = {"quantize": build_quantize, "dequantize": build_dequantize, "panel": build_panel}
 
 
 def build(case):
@@ -261,7 +240,7 @@ def build(case):
 
 
 # ----------------------------------------------------------------------- the launch record (profiled children)
-_KERNEL = r"\b((?:de)?quantize(?:_blockwise(?:_generic)?|4_prmt|4_cols)_kernel)<([^<>]*)>"
+_KERNEL = r"\b((?:de)?quantize(?:_blockwise(?:_generic)?|4_prmt)_kernel)<([^<>]*)>"
 
 
 def _instance(name: str):
@@ -358,16 +337,14 @@ def walk_launches():
 NO_RECORD = "torch.profiler recorded no CUDA kernels here: which kernel instance ran is not confirmed"
 
 
-def recorded(launches, case, want, only=None):
-    """Asserts the case's launches (those of kernel `only`, if given): `want` is [(instance tuple, grid x)]; the grids
-    are compared when the trace has them.  Returns NO_RECORD without a record (the caller skips at its end, after the
-    reference comparison), else None."""
+def recorded(launches, case, want):
+    """Asserts the case's launches: `want` is [(instance tuple, grid x)]; the grids are compared when the trace has
+    them.  Returns NO_RECORD without a record (the caller skips at its end, after the reference comparison), else
+    None."""
     got = launches[case_key(case)]["kernels"]
     if got is None:
         return NO_RECORD
     assert not isinstance(got, str), f"the profiled replay of this case failed: {got}"
-    if only is not None:
-        got = [k for k in got if k[0] == only]
     assert [tuple(k[:-1]) for k in got] == [w[0] for w in want], got
     grids = [k[-1] for k in got]
     if all(g is not None for g in grids):
@@ -691,44 +668,6 @@ def test_nested_panel_decode(launches, dtype, qt, bs, K, n0, nrounds):
     finish(recorded(launches, case, [(("dequantize4_prmt_kernel", T_NAME[dtype], DQ_QT_ARG[qt], "1"), grid)]))
 
 
-COLS_ROWS = [
-    pytest.param("bf16", "nf4", 64, True, id="bf16-nf4-bs64-nested"),
-    pytest.param("fp16", "fp4", 64, True, id="fp16-fp4-bs64-nested"),
-    pytest.param("bf16", "fp4", 32, True, id="bf16-fp4-bs32-nested"),
-    pytest.param("fp16", "nf4", 128, True, id="fp16-nf4-bs128-nested"),
-    pytest.param("bf16", "nf4", 256, False, id="bf16-nf4-bs256"),
-    pytest.param("fp16", "fp4", 32, False, id="fp16-fp4-bs32"),
-]
-
-
-def cols_case(dtype, qt, bs, nested):
-    return ["cols", dict(dtype=dtype, qt=qt, bs=bs, nested=nested, seed=bs + 7 * nested)]
-
-
-@pytest.mark.parametrize("dtype,qt,bs,nested", COLS_ROWS)
-def test_input_grad_panel_decode(launches, dtype, qt, bs, nested):
-    """dequantize4_cols_kernel<T16, QT, DQ> through cbnb_b200_gemm_4bit_input_grad_panel with G = the identity: a
-    4096 x 4096 weight in one panel of 4096 columns (the whole 32 MB workspace, 2 grid-stride rounds) comes out as
-    F.dequantize_4bit, bit for bit (FP4's -0 as +0: the sum +0 + -0)."""
-    import bitsandbytes_b200.functional as F
-
-    case = cols_case(dtype, qt, bs, nested)
-    inputs, go = build(case)
-    out = go()
-    qW, qs = inputs["qW"], inputs["qs"]
-    N = K = 4096
-    want = F.dequantize_4bit(qW, qs).view(N, K)
-    if nested:
-        pin_nested_dequantize_4bit(qW, qs, dtype, want)
-    want = torch.where(want == 0, torch.zeros_like(want), want)
-    assert torch.equal(out.view(torch.int16), want.view(torch.int16))
-    units = N * K // 64
-    grid = capped(cdiv(units, D4_UNITS), D4_CAP)
-    assert rounds(units, grid, D4_UNITS) == 2
-    finish(recorded(launches, case, [(("dequantize4_cols_kernel", T_NAME[dtype], DQ_QT_ARG[qt], str(int(nested))),
-                                      grid)], only="dequantize4_cols_kernel"))
-
-
 # ------------------------------------------------------------------------ 5. edges where fast-math kernels go wrong
 FLT_MIN = np.float32(2.0**-126)
 EDGE_BS = 64
@@ -928,5 +867,4 @@ def all_cases():
     cases += [deq_case(*r.values) for r in DEQ_ROWS]
     cases += [deq_generic_case(*r.values) for r in DEQ_GENERIC_ROWS]
     cases += [panel_case(*r.values) for r in PANEL_ROWS]
-    cases += [cols_case(*r.values) for r in COLS_ROWS]
     return cases

@@ -1,151 +1,18 @@
-"""GPU tests of the input-gradient 4-bit GEMM (``out = G . dequant(W)``, the weight not transposed) and of the backward
-of the tensor-parallel Linear4bit layers built on it: exact decode, the rounding relation between the T and fp32
-outputs, the float64 bound, independence of the panel width, strided operands and return codes; then the layers'
-gradients at worlds of 1, 2, 4 and 8 (the ranks simulated in turn on one GPU), rank agreement, the sequence-parallel
-rows, and one training step of a LoRA adapter in front of a column -> row pair."""
+"""GPU tests of the backward of the tensor-parallel Linear4bit layers: their gradients at worlds of 1, 2, 4 and 8 (the
+ranks simulated in turn on one GPU), rank agreement, the sequence-parallel rows, the layers' own forward and backward
+through simulated collectives, the gradient layouts autograd produces, and one training step of a LoRA adapter in front
+of a column -> row pair."""
 import pytest
 import torch
 
 from tests import _native as nat
-from tests.test_gpu_gemm4 import assert_close_to_exact, make_problem
-from tests.test_gpu_gemm4_tf32 import accumulation, ulp32
-from tests.test_gpu_row_parallel import _weights
+from tests.test_gpu_gemm4 import assert_close_to_exact
 
 pytestmark = pytest.mark.gpu
-
-_T = {"bf16": torch.bfloat16, "fp16": torch.float16}
-
-
-def _grad(M, N, dtype, seed=0, ld=None):
-    g = torch.Generator().manual_seed(seed * 7907 + M * 13 + N)
-    full = torch.randn(M, ld or N, generator=g).to(_T[dtype]).cuda()
-    return full[:, :N]
-
-
-def _ig(p, G, part, panel=0, out=None, dtype_id=None, ldg=None, N=None, K=None):
-    """(return code, out) of one input-gradient call through the panel test entry."""
-    M = G.shape[0]
-    N = p["N"] if N is None else N
-    K = p["K"] if K is None else K
-    if out is None:
-        out = torch.full((M, K), float("nan"), device="cuda", dtype=torch.float32 if part else G.dtype)
-    rc = nat.lib.cbnb_b200_gemm_4bit_input_grad_panel(
-        G.data_ptr(), G.stride(0) if ldg is None else ldg, nat.ptr(p["packed"]), nat.ptr(p["absmax"]),
-        nat.ptr(p["absmax_8bit"]), nat.ptr(p["absmax_code"]), nat.ptr(p["absmax_offset"]), out.data_ptr(),
-        out.stride(0), M, N, K, p["bs"], nat.QT_ID[p["qt"]], nat.DTYPE_ID[p["dtype"]] if dtype_id is None else dtype_id,
-        int(part), panel, nat.stream())
-    torch.cuda.synchronize()
-    return rc, out
 
 
 def _bits(t):
     return t.view(torch.int32) if t.dtype == torch.float32 else t.view(torch.int16)
-
-
-# ------------------------------------------------------------------------------------------------------ the kernel
-@pytest.mark.parametrize("qt", ["nf4", "fp4"])
-@pytest.mark.parametrize("dtype", ["bf16", "fp16"])
-@pytest.mark.parametrize("nested,bs", [(False, 32), (False, 64), (False, 128), (False, 512), (False, 4096),
-                                       (True, 32), (True, 64), (True, 128)])
-@pytest.mark.parametrize("M,panel", [(512, 0), (300, 128)])
-def test_identity_gives_the_decoded_weights(qt, dtype, nested, bs, M, panel):
-    """G = rows of the identity: both outputs are rows of the decoded weight, bit for bit (FP4's -0 comes out as +0, the
-    sum +0 + -0).  K = 448 ends in half a tile; panel 128 takes four panels."""
-    N, K = 512, 448
-    p = make_problem(1, N, K, qt, dtype, bs=bs, nested=nested, seed=bs)
-    W = _weights(p, dtype).to(_T[dtype])
-    W = torch.where(W == 0, torch.zeros_like(W), W)
-    G = torch.eye(N, device="cuda", dtype=_T[dtype])[:M]
-    for part in (False, True):
-        rc, out = _ig(p, G, part, panel)
-        assert rc == 0
-        assert torch.equal(_bits(out), _bits(W[:M].to(out.dtype))), f"part={part}"
-    if not nested:
-        import bitsandbytes_b200.functional as F
-
-        ref = F.dequantize_4bit(p["packed"], absmax=p["absmax"], out=torch.empty(N, K, device="cuda", dtype=_T[dtype]),
-                                blocksize=bs, quant_type=qt)
-        assert torch.equal(_bits(ref), _bits(_weights(p, dtype).to(_T[dtype])))
-
-
-@pytest.mark.parametrize("M", [1, 64, 2048, 4096])
-@pytest.mark.parametrize("dtype,qt,nested", [("bf16", "nf4", False), ("fp16", "fp4", True)])
-def test_float64_bound_and_rounding_relation(M, dtype, qt, nested):
-    """Arbitrary G: the fp32 output within half an fp32 ulp plus the accumulation bound over N of G64 . W64, the T
-    output within the bound of the forward tests, and T(PART) equal to the T output bit for bit."""
-    N, K = 1024, 1536
-    p = make_problem(1, N, K, qt, dtype, nested=nested, seed=M)
-    W = _weights(p, dtype)
-    G = _grad(M, N, dtype, seed=M)
-    rc, part = _ig(p, G, True)
-    assert rc == 0
-    rc, t = _ig(p, G, False)
-    assert rc == 0
-    assert torch.equal(_bits(part.to(_T[dtype])), _bits(t))
-    y64 = G.double() @ W.double()
-    tol = 0.5 * ulp32(y64) + accumulation(N, y64)
-    bad = (part.double() - y64).abs() > tol
-    assert not bad.any(), f"{int(bad.sum())} / {bad.numel()} off"
-    assert_close_to_exact(t, y64.cpu().numpy(), dtype, N)
-
-
-@pytest.mark.parametrize("M", [64, 2048])
-def test_result_does_not_depend_on_the_panel(M):
-    """Panels of 128, 256 and 384 columns and the production panel: the same bits, call after call."""
-    N, K = 768, 1280
-    p = make_problem(1, N, K, "nf4", "bf16", seed=2)
-    G = _grad(M, N, "bf16", seed=3)
-    want = _ig(p, G, True)[1]
-    for panel in (128, 256, 384, 0, 0):
-        rc, out = _ig(p, G, True, panel)
-        assert rc == 0 and torch.equal(_bits(out), _bits(want)), f"panel {panel}"
-
-
-@pytest.mark.parametrize("part", [False, True])
-def test_strided_g_gives_the_contiguous_result(part):
-    """G a column slice of a wider gradient (row stride 3 N, offset N) gives the result of its contiguous copy; a
-    ragged output row stride leaves the columns past K untouched."""
-    M, N, K = 200, 512, 640
-    p = make_problem(1, N, K, "fp4", "fp16", seed=4)
-    wide = _grad(M, 3 * N, "fp16", seed=5)
-    G = wide[:, N:2 * N]
-    want = _ig(p, G.contiguous(), part)[1]
-    buf = torch.full((M, K + 8), float("nan"), device="cuda", dtype=torch.float32 if part else torch.float16)
-    rc, _ = _ig(p, G, part, out=buf[:, :K])
-    assert rc == 0
-    assert torch.equal(_bits(buf[:, :K]), _bits(want))
-    assert torch.isnan(buf[:, K:].float()).all()
-
-
-def test_return_codes_write_nothing():
-    N, K = 256, 384
-    p = make_problem(1, N, K, "nf4", "bf16", seed=6)
-    G = _grad(64, N, "bf16", seed=7, ld=N + 64)
-    bad = [dict(ldg=N - 8),                   # ldg < N
-           dict(part=2),                      # part not 0 / 1
-           dict(K=K, out_ld=K - 1)]           # ldc < K
-    for kw in bad:
-        out = torch.full((64, K), float("nan"), device="cuda")
-        ldc = kw.pop("out_ld", None)
-        view = out if ldc is None else torch.as_strided(out, (64, K), (ldc, 1))
-        part = kw.pop("part", 1)
-        rc, _ = _ig(p, G, part, out=view, **kw)
-        assert rc == 1, kw
-        assert torch.isnan(out).all()
-        with pytest.raises(RuntimeError):
-            nat.check()
-    unserved = [dict(dtype_id=0),             # fp32
-                dict(N=N - 32),               # N % 64
-                dict(K=K - 32),               # K % 64
-                dict(ldg=N + 4)]              # ldg % 8
-    for kw in unserved:
-        out = torch.full((64, K), float("nan"), device="cuda")
-        rc, _ = _ig(p, G, True, out=out, **kw)
-        assert rc == 100, kw
-        assert torch.isnan(out).all()
-    Gu = torch.zeros(64 * N + 1, device="cuda", dtype=torch.bfloat16)[1:].view(64, N)  # 2 bytes off 16
-    out = torch.full((64, K), float("nan"), device="cuda")
-    assert _ig(p, Gu, True, out=out)[0] == 100 and torch.isnan(out).all()
 
 
 # ------------------------------------------------------------------------------------------------------ the layers

@@ -1,10 +1,8 @@
-"""CPU tests of the tensor-parallel Linear4bit backward: the argument checks of the input-gradient wrapper (against a fake
-library), the refusal of grad-requiring input by the symmetric-memory routes, and the collectives the backward runs in a
-simulated world of 4."""
+"""CPU tests of the tensor-parallel Linear4bit backward: the refusal of grad-requiring input by the symmetric-memory
+routes, and the collectives the backward runs in a simulated world of 4."""
 import pytest
 import torch
 
-import bitsandbytes_b200.backends.cuda as cb
 import bitsandbytes_b200.parallel as par
 from bitsandbytes_b200.parallel import ColumnParallelLinear4bit, RowParallelLinear4bit, Shard4bit
 from tests._parallel_sim import fake, simulate  # noqa: F401  (fake: a fixture)
@@ -14,31 +12,6 @@ def _shard(N=64, K=128, row0=0):
     return Shard4bit(packed=torch.zeros(N * K // 2, dtype=torch.uint8), absmax=torch.ones(N * K // 64),
                      absmax_8bit=None, absmax_code=None, absmax_offset=None, rows=N, row0=row0, K=K, blocksize=64,
                      quant_type="nf4")
-
-
-def test_input_grad_wrapper_checks(fake):
-    """Bad G / out shapes, dtypes or strides raise before any native call; fp32 G is declined (False) without one; a
-    good call passes the row strides and the part flag."""
-    B, absmax = torch.zeros(64 * 128 // 2, dtype=torch.uint8), torch.ones(64 * 128 // 64)
-
-    def call(G, out):
-        return cb.gemm_4bit_input_grad(G, B, (64, 128), absmax, 64, "nf4", None, None, None, out)
-
-    G = torch.zeros(8, 64, dtype=torch.bfloat16)
-    for g, o in [(torch.zeros(8, 32, dtype=torch.bfloat16), torch.zeros(8, 128)),      # N mismatch
-                 (torch.zeros(64, 8, dtype=torch.bfloat16).t(), torch.zeros(8, 128)),   # column stride
-                 (G, torch.zeros(8, 127)),                                              # out shape
-                 (G, torch.zeros(8, 128, dtype=torch.float16))]:                        # out dtype
-        with pytest.raises(RuntimeError, match="gemm_4bit_input_grad"):
-            call(g, o)
-    assert fake.calls == []
-    assert not call(torch.zeros(8, 64), torch.zeros(8, 128)) and fake.calls == []
-    wide = torch.zeros(8, 192, dtype=torch.bfloat16)
-    assert call(wide[:, 64:128], torch.zeros(8, 136)[:, :128])
-    assert call(G, torch.zeros(8, 128, dtype=torch.bfloat16))
-    # (G, ldg, B, absmax, a8, code, offset, out, ldc, M, N, K, blocksize, quant_type, dtype, part, stream)
-    assert [(a[1], a[8], a[9], a[10], a[11], a[15]) for _, a in fake.calls] == [(192, 136, 8, 64, 128, 1),
-                                                                               (64, 128, 8, 64, 128, 0)]
 
 
 def test_fused_routes_refuse_grad_requiring_input():
