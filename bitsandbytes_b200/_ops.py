@@ -178,7 +178,7 @@ def _(A, B, shapeB, absmax, blocksize, quant_type, bias=None, absmax_8bit=None, 
     return torch.empty((*A.shape[:-1], shapeB[0]), device=A.device, dtype=A.dtype)
 
 
-MAX_EXPERTS = 1024  # the grouped GEMM's limit (kMaxExperts in csrc/gemm4_tc.cu)
+MAX_EXPERTS = 1024  # the grouped kernels' limit (kMaxExperts in csrc/common.cuh)
 
 
 def check_grouped(A, B, shapeB, absmax, blocksize, quant_type, offs, bias=None, absmax_8bit=None, absmax_code=None,

@@ -27,7 +27,7 @@ from warnings import warn
 
 import torch
 
-from .._ops import check_grouped, kernel
+from .._ops import MAX_EXPERTS, check_grouped, kernel
 from .. import cextension as cext
 from ..cextension import lib
 
@@ -421,11 +421,39 @@ def _gemm_4bit_grouped(A, B, shapeB, absmax, blocksize: int, quant_type: str, of
     is read back to the host, so the call can be captured in a CUDA graph."""
     E, N, K = check_grouped(A, B, shapeB, absmax, blocksize, quant_type, offs, bias, absmax_8bit, absmax_code,
                             absmax_offset)
+    out = torch.empty((A.shape[0], N), dtype=A.dtype, device=A.device)
+    _grouped_launch(A, B, E, N, K, absmax, blocksize, quant_type, offs, bias, absmax_8bit, absmax_code, absmax_offset,
+                    out, N)
+    return out
+
+
+def _grouped_out(what: str, out: torch.Tensor, dtype: torch.dtype, device, M: int, N: int, ldc: int) -> None:
+    """``out`` is an ``[M, N]`` tensor of ``dtype`` on ``device``, row-major at row stride ``ldc``, with room for it."""
+    if (out.dim() != 2 or tuple(out.shape) != (M, N) or (N > 1 and out.stride(1) != 1)
+            or (M > 1 and out.stride(0) != ldc)):
+        raise RuntimeError(f"{what}: out must be [{M}, {N}] with unit column stride and row stride ldc = {ldc}, got "
+                           f"{list(out.shape)} with strides {list(out.stride())}")
+    _dest_ptrs(what, [out], dtype, device, M, N, ldc, RuntimeError)
+
+
+def gemm_4bit_grouped_into(A, B, shapeB, absmax, blocksize: int, quant_type: str, offs, bias, absmax_8bit, absmax_code,
+                           absmax_offset, out: torch.Tensor, ldc: int) -> None:
+    """The grouped GEMM of ``gemm_4bit_grouped`` into the caller's ``out``, an ``[M, N]`` view at row stride ``ldc``
+    (elements) -- a column slice of a wider buffer, as the column-parallel expert layer gathers."""
+    E, N, K = check_grouped(A, B, shapeB, absmax, blocksize, quant_type, offs, bias, absmax_8bit, absmax_code,
+                            absmax_offset)
+    _grouped_out("gemm_4bit_grouped", out, A.dtype, A.device, A.shape[0], N, ldc)
+    _grouped_launch(A, B, E, N, K, absmax, blocksize, quant_type, offs, bias, absmax_8bit, absmax_code, absmax_offset,
+                    out, ldc)
+
+
+def _grouped_launch(A, B, E, N, K, absmax, blocksize, quant_type, offs, bias, absmax_8bit, absmax_code, absmax_offset,
+                    out, ldc: int) -> None:
+    """The native grouped GEMM on operands ``check_grouped`` has accepted, into ``out`` at row stride ``ldc``."""
     M = A.shape[0]
-    _check_sizes("gemm_4bit_grouped", M, E * N, K)
-    out = torch.empty((M, N), dtype=A.dtype, device=A.device)
+    _check_sizes("gemm_4bit_grouped", M, E * N, K, ldc)
     if M == 0:
-        return out
+        return
     off = _weight_operands(absmax, blocksize, quant_type, absmax_8bit, absmax_code, absmax_offset)
     A, B, offs = A.contiguous(), B.contiguous(), offs.contiguous()
     bias = bias.contiguous() if bias is not None else None
@@ -436,10 +464,78 @@ def _gemm_4bit_grouped(A, B, shapeB, absmax, blocksize: int, quant_type: str, of
             absmax_code.data_ptr() if absmax_code is not None else None,
             off.data_ptr() if off is not None else None,
             offs.data_ptr(), E, out.data_ptr(), bias.data_ptr() if bias is not None else None,
-            M, N, K, N, blocksize, _QT_ID[quant_type], _DTYPE_ID[A.dtype], _stream(A))
+            M, N, K, ldc, blocksize, _QT_ID[quant_type], _DTYPE_ID[A.dtype], _stream(A))
     lib.check("gemm_4bit_grouped")
     if rc != 0:
         raise RuntimeError(f"gemm_4bit_grouped: the library does not serve this call (code {rc})")
+
+
+def gemm_4bit_grouped_partial(A, B, shapeB, absmax, blocksize: int, quant_type: str, offs, out: torch.Tensor,
+                              ldc: int, mt: int = 0) -> None:
+    """The grouped fp32 partial of a row-sharded expert layer: ``out[m, n] = A[m] . dequant(W[e])[n]`` summed in fp32,
+    with no bias and no rounding, for the rows of expert e (``offs`` as in ``gemm_4bit_grouped``, clamped on the
+    device), and 0 for the rows past ``offs[E-1]``; ``out`` is fp32 at row stride ``ldc``.  The statistics are plain
+    fp32 absmax (:func:`~bitsandbytes_b200.parallel.slice_quantized_weight_k` makes them so).  ``mt`` is the token
+    tile (16, 32, 64 or 128), 0 for the grouped GEMM's rule, which depends on M and E only: a shard then runs the
+    unsharded layer's tile.  Nothing is read back to the host."""
+    E, N, K = check_grouped(A, B, shapeB, absmax, blocksize, quant_type, offs)
+    M = A.shape[0]
+    _check_sizes("gemm_4bit_grouped_partial", M, E * N, K, ldc)
+    _grouped_out("gemm_4bit_grouped_partial", out, torch.float32, A.device, M, N, ldc)
+    if mt not in (0, 16, 32, 64, 128):
+        raise RuntimeError(f"gemm_4bit_grouped_partial: mt must be 0, 16, 32, 64 or 128, got {mt}")
+    if M == 0:
+        return
+    A, B, offs = A.contiguous(), B.contiguous(), offs.contiguous()
+    with _on_device(A):
+        rc = lib.cbnb_b200_gemm_4bit_grouped_partial(
+            A.data_ptr(), B.data_ptr(), absmax.data_ptr(), offs.data_ptr(), E, out.data_ptr(), M, N, K, ldc,
+            blocksize, _QT_ID[quant_type], _DTYPE_ID[A.dtype], mt, _stream(A))
+    lib.check("gemm_4bit_grouped_partial")
+    if rc != 0:
+        raise RuntimeError(f"gemm_4bit_grouped_partial: the library does not serve this call (code {rc})")
+
+
+def reduce_partials_grouped(parts: torch.Tensor, offs: torch.Tensor, dtype: torch.dtype,
+                            bias: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """:func:`reduce_partials` for a row-sharded expert layer: ``out[m] = dtype((((parts[0] + parts[1]) + ...) +
+    parts[w-1])[m] + bias[e])`` for the rows of expert e, ``offs`` the int32 ``[E]`` end rows (clamped on the device as
+    the grouped GEMM clamps them, never read on the host), and 0 for the rows past ``offs[E-1]``.  ``bias`` is
+    ``[E, N]``; ``out`` may be an ``[M, N]`` view with unit column stride and any row stride."""
+    if parts.dtype != torch.float32 or parts.dim() != 3:
+        raise RuntimeError(f"reduce_partials_grouped: parts must be a [world, M, N] float32 tensor, got {parts.dtype} "
+                           f"{tuple(parts.shape)}")
+    if dtype not in (torch.float16, torch.bfloat16):
+        raise RuntimeError(f"reduce_partials_grouped: dtype must be float16 or bfloat16, got {dtype}")
+    world, M, N = parts.shape
+    if world < 1:
+        raise RuntimeError("reduce_partials_grouped: no partials")
+    if offs.dtype != torch.int32 or offs.dim() != 1 or not 1 <= offs.numel() <= MAX_EXPERTS or offs.device != parts.device:
+        raise RuntimeError(f"reduce_partials_grouped: offs must be int32 [E], 1 <= E <= {MAX_EXPERTS}, on "
+                           f"{parts.device}, got {offs.dtype} {tuple(offs.shape)} on {offs.device}")
+    E = offs.numel()
+    if bias is not None and (bias.dtype != dtype or tuple(bias.shape) != (E, N) or bias.device != parts.device):
+        raise RuntimeError(f"reduce_partials_grouped: bias must be {dtype} [{E}, {N}] on {parts.device}")
+    if out is not None and (out.dtype != dtype or out.shape != (M, N) or out.device != parts.device
+                            or (N > 1 and out.stride(1) != 1) or (M > 1 and out.stride(0) < N)):
+        raise RuntimeError(f"reduce_partials_grouped: out must be {dtype} [{M}, {N}] with unit column stride on "
+                           f"{parts.device}")
+    if not parts.is_cuda:
+        raise RuntimeError(f"reduce_partials_grouped: the partials must be on a CUDA device, got {parts.device}")
+    parts, offs = parts.contiguous(), offs.contiguous()
+    bias = bias.contiguous() if bias is not None else None
+    if out is None:
+        out = torch.empty((M, N), dtype=dtype, device=parts.device)
+    _check_sizes("reduce_partials_grouped", M, E * N, out.stride(0), world)
+    if M == 0 or N == 0:
+        return out
+    with _on_device(parts):
+        rc = lib.cbnb_b200_reduce_partials_grouped(parts.data_ptr(), world, M * N, offs.data_ptr(), E, out.data_ptr(),
+                                                   bias.data_ptr() if bias is not None else None, M, N, out.stride(0),
+                                                   _DTYPE_ID[dtype], _stream(parts))
+    lib.check("reduce_partials_grouped")
+    if rc != 0:
+        raise RuntimeError(f"reduce_partials_grouped: the library refused the call (code {rc})")
     return out
 
 

@@ -83,6 +83,11 @@ def _signatures():
     #  dtype, stream) -> int; the _mt form takes mt before the stream
     sig["cbnb_b200_gemm_4bit_grouped"] = ([_VOIDP] * 7 + [_I32] + [_VOIDP] * 2 + [_I32] * 7 + [_VOIDP], _I32)
     sig["cbnb_b200_gemm_4bit_grouped_mt"] = ([_VOIDP] * 7 + [_I32] + [_VOIDP] * 2 + [_I32] * 8 + [_VOIDP], _I32)
+    # (A, B, absmax, offs, E, out, M, N, K, ldc, blocksize, quant_type, dtype, mt, stream) -> int
+    sig["cbnb_b200_gemm_4bit_grouped_partial"] = ([_VOIDP] * 4 + [_I32] + [_VOIDP] + [_I32] * 8 + [_VOIDP], _I32)
+    # (parts, world, part_stride, offs, E, out, bias, M, N, ldc, dtype, stream) -> int
+    sig["cbnb_b200_reduce_partials_grouped"] = ([_VOIDP, _I32, ct.c_longlong, _VOIDP, _I32, _VOIDP, _VOIDP] + [_I32] * 4
+                                                + [_VOIDP], _I32)
     # (B, absmax, absmax_8bit, absmax_code, absmax_offset, out, blocksize, quant_type, dtype, n0, rows, K, stream) -> int
     sig["cbnb_b200_dequantize_4bit_panel"] = ([_VOIDP] * 6 + [_I32] * 6 + [_VOIDP], _I32)
     # (A, W, out, bias, M, N, K, ldc, dtype, mt, stream) -> int

@@ -93,9 +93,15 @@ bool launch_gemm4_grouped(const T* A, const uint8_t* B, const float* absmax, con
                           const float* absmax_code, const float* absmax_offset, const int* offs, int E, T* out,
                           const T* bias, int M, int N, int K, int ldc, int blocksize, int quant_type, int mt,
                           cudaStream_t stream);
+template <typename T>
+bool launch_gemm4_grouped_partial(const T* A, const uint8_t* B, const float* absmax, const int* offs, int E, float* out,
+                                  int M, int N, int K, int ldc, int blocksize, int quant_type, int mt,
+                                  cudaStream_t stream);
 // partials.cu
 bool launch_reduce_partials(const float* parts, int world, long long part_stride, void* out, const void* bias, int M,
                             int N, int ldc, int dtype, cudaStream_t stream);
+bool launch_reduce_partials_grouped(const float* parts, int world, long long part_stride, const int* offs, int E,
+                                    void* out, const void* bias, int M, int N, int ldc, int dtype, cudaStream_t stream);
 int max_reduce_parts();
 bool launch_reduce_partials_ptrs(const float* const* parts, int n_parts, int row0, int rows, void* out,
                                  const void* bias, int N, int ldc, int dtype, cudaStream_t stream);
@@ -704,6 +710,48 @@ int cbnb_b200_gemm_4bit_grouped_mt(const void* A, const uint8_t* B, const float*
                                    int quant_type, int dtype, int mt, cudaStream_t stream) {
     return gemm_4bit_grouped(A, B, absmax, absmax_8bit, absmax_code, absmax_offset, offs, E, out, bias, M, N, K, ldc,
                              blocksize, quant_type, dtype, mt, stream);
+}
+
+// The grouped fp32 partial of a row-sharded expert layer: out[m, n] (fp32, row stride ldc) = A[m, :] . W_e[n, :] for
+// the rows of expert e, with no bias and no rounding, and 0 for the rows past end_{E-1}; offs and B as in
+// cbnb_b200_gemm_4bit_grouped, with plain fp32 absmax.  mt: the token tile (16 | 32 | 64 | 128), 0 = the grouped GEMM's
+// rule for (M, E), so that a shard runs the unsharded layer's tile.  Returns 0; 1 with the error message set for bad
+// arguments; 100, with nothing written, for what the kernel does not serve (nested statistics, K % 64 != 0, E > 1024);
+// or 100 with the error message set when a launch past those checks fails.
+int cbnb_b200_gemm_4bit_grouped_partial(const void* A, const uint8_t* B, const float* absmax, const int* offs, int E,
+                                        float* out, int M, int N, int K, int ldc, int blocksize, int quant_type,
+                                        int dtype, int mt, cudaStream_t stream) {
+    if (A == nullptr || B == nullptr || absmax == nullptr || offs == nullptr || out == nullptr || M < 0 || N <= 0 ||
+        K <= 0 || E < 1 || ldc < N || (quant_type != kFP4 && quant_type != kNF4) ||
+        (mt != 0 && mt != 16 && mt != 32 && mt != 64 && mt != 128)) {
+        set_last_error_msg("gemm_4bit_grouped_partial: needs A, B, absmax, offs and out, M >= 0, N, K >= 1, E >= 1, "
+                           "ldc >= N, quant_type 1 (FP4) or 2 (NF4) and mt 0, 16, 32, 64 or 128");
+        return 1;
+    }
+    if (M == 0) return 0;
+    if (mt == 0) mt = grouped_tile(M, E);
+    bool ok = false;
+    const bool known = with_dtype<kIdF16 | kIdBF16>(dtype, [&](auto t) {
+        using T = decltype(t);
+        if constexpr (!std::is_same<T, float>::value) {
+            ok = launch_gemm4_grouped_partial<T>((const T*)A, B, absmax, offs, E, out, M, N, K, ldc, blocksize,
+                                                 quant_type, mt, stream);
+        }
+    });
+    return known && ok ? 0 : 100;
+}
+
+// The reduction of a row-sharded expert layer: out[m, n] (row stride ldc) = T(((parts[0] + parts[1]) + ... +
+// parts[world - 1])[m, n] + bias[e * N + n]) for the rows of expert e (end rows clamped on the device from offs[E], as
+// the grouped GEMM clamps them), and 0 for the rows past end_{E-1}.  The partials are [M, N] at row stride N, one every
+// part_stride elements; bias is [E, N] or NULL.  The arithmetic of cbnb_b200_reduce_partials: without a bias and
+// without tail rows, the same bits.  dtype 1 = fp16, 2 = bf16.  Returns 0, or 100 for a dtype, world or E it does not
+// serve.
+int cbnb_b200_reduce_partials_grouped(const float* parts, int world, long long part_stride, const int* offs, int E,
+                                      void* out, const void* bias, int M, int N, int ldc, int dtype,
+                                      cudaStream_t stream) {
+    return launch_reduce_partials_grouped(parts, world, part_stride, offs, E, out, bias, M, N, ldc, dtype, stream) ? 0
+                                                                                                                   : 100;
 }
 
 int cbnb_b200_gemm_4bit_path(int M, int N, int K, int blocksize, int dtype) {

@@ -216,6 +216,10 @@ void set_last_error_msg(const char* msg);
 
 int device_sm_count();
 
+// Experts a grouped (mixture-of-experts) launch serves: the grouped GEMM's group table (gemm4_tc.cu) and the grouped
+// reduction's table of end rows (partials.cu) are sized by it; _ops.MAX_EXPERTS is the same limit on the Python side.
+constexpr int kMaxExperts = 1024;
+
 // ---------------------------------------------------------------- 4-bit GEMM destinations
 // The destinations of a 4-bit GEMM: every output element is stored to each of p[0..n) at the same row stride (a
 // sharded layer's slot in every rank's buffer).  OutList<float> carries the partial instances' fp32 accumulators

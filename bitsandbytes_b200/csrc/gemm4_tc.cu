@@ -48,6 +48,8 @@
 // copies are fp32, and the epilogue stores the accumulators -- the split order's sums under split-K -- with no bias
 // and no rounding, straight from the fragments.  With rows_per_out > 0 (cbnb_b200_gemm_4bit_partial_scatter, a
 // sequence-parallel layer) each output row goes to one copy only, the one of the rank that owns the token.
+// GROUPED && PART is the grouped partial instance (cbnb_b200_gemm_4bit_grouped_partial, a row-sharded expert layer):
+// each expert's fp32 rows, masked at the expert's end row, and fp32 zeros in the tail rows.
 #include "common.cuh"
 #include "decode4.cuh"
 #include "hopper_ptx.cuh"
@@ -108,7 +110,6 @@ struct Gemm4Params {
 // The grouped instances (GROUPED = true) serve 1 <= E <= kMaxExperts experts per launch: their group table (the
 // clamped end row and the exclusive prefix of the m-tile counts of every expert, plus the scan's per-warp totals) sits
 // in shared memory past the barriers.
-constexpr int kMaxExperts = 1024;
 constexpr int kGroupTabBytes = (2 * kMaxExperts + 1 + 2 * kThreads / 32) * 4;
 
 // The partial instances' store of element (m, n) of the fp32 output (m < M, n < N), routed as p.rows_per_out says.
@@ -548,7 +549,24 @@ __global__ void __launch_bounds__(kThreads, 1)
         // ================================================================== epilogue
         // acc[4j + e]: feature row row0 + 8 * (e >= 2), token column 8j + 2t + (e & 1)
         T* outp = reinterpret_cast<T*>(p.out);
-        if constexpr (PART) {
+        if constexpr (PART && GROUPED) {
+            // One destination, no scatter.  Rows past the expert's end belong to a later expert or to the tail and
+            // were computed with this expert's weights: they are left to the unit (or the tail loop) that owns them.
+            // The unit is looked up again here for the reason given at the rounded epilogue below, and the rows are
+            // addressed from this thread's first one: with the absolute row of every store, ptxas spilled 8 to 12
+            // bytes in the MT = 128 instances.
+            const Unit we = unit_at(u);
+            const int lim = we.m_end - we.m0 - 2 * t;  // tile row 8j + 2t + (e & 1) is stored when 8j + (e & 1) < lim
+            float* dst = reinterpret_cast<float*>(p.out) + (long long)(we.m0 + 2 * t) * p.ldc;
+#pragma unroll
+            for (int j = 0; j < MT / 8; ++j)
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const int n = e >= 2 ? nb : na;
+                    if (8 * j + (e & 1) < lim && n < p.N) dst[(long long)(8 * j + (e & 1)) * p.ldc + n] = acc[4 * j + e];
+                }
+            continue;
+        } else if constexpr (PART) {
             // a warp instruction stores four 32-byte row pieces: whole sectors, without the staging buffer, which at
             // fp32 would not fit next to the 256-token tile's ring
             if (splits == 1) {
@@ -725,13 +743,14 @@ __global__ void __launch_bounds__(kThreads, 1)
         }
     }
     if constexpr (GROUPED) {
-        // rows [end_{E-1}, M) belong to no expert: zeros, each CTA's consumers storing a strided share
+        // rows [end_{E-1}, M) belong to no expert: zeros (fp32 for PART), each CTA's consumers storing a strided share
         const int m_tail = group_table<Cfg>(so)[p.E - 1];
         const long long n_tail = (long long)(p.M - m_tail) * p.N;
         T* outp = reinterpret_cast<T*>(p.out);
         for (long long i = (long long)blockIdx.x * kConsumers + ct; i < n_tail; i += (long long)gridDim.x * kConsumers) {
             const long long m = m_tail + i / p.N;
-            outp[m * p.ldc + i % p.N] = DT<T>::from_f32(0.f);
+            if constexpr (PART) reinterpret_cast<float*>(p.out)[m * p.ldc + i % p.N] = 0.f;
+            else outp[m * p.ldc + i % p.N] = DT<T>::from_f32(0.f);
         }
     }
 }
@@ -825,8 +844,9 @@ bool launch_mt(const T* A, Gemm4Params& p, int force_splits, cudaStream_t stream
     constexpr int kBK = Cfg::kBK;
     constexpr size_t smem_bytes = Cfg::kSmemBytes + (GROUPED ? kGroupTabBytes : 0);
     static_assert(smem_bytes <= 227 * 1024, "shared memory");
-    static_assert(!GROUPED || (!kSS && !PART && !std::is_same<T, float>::value),
-                  "the grouped instances decode 4-bit codes to fp16 / bf16 and store T");
+    static_assert(!GROUPED || (!kSS && !std::is_same<T, float>::value),
+                  "the grouped instances decode 4-bit codes to fp16 / bf16");
+    static_assert(!(GROUPED && PART && DQ), "the grouped partial instances take plain statistics");
     // the shared-memory opt-in is PER DEVICE (one process may drive several GPUs)
     static bool attr_set[64] = {};
     int dev = 0;
@@ -1214,5 +1234,51 @@ template bool launch_gemm4_grouped<__nv_bfloat16>(const __nv_bfloat16*, const ui
 template bool launch_gemm4_grouped<__half>(const __half*, const uint8_t*, const float*, const uint8_t*, const float*,
                                            const float*, const int*, int, __half*, const __half*, int, int, int, int,
                                            int, int, int, cudaStream_t);
+
+// The grouped fp32 partial of a row-sharded expert layer: out[m, n] (row stride ldc) = A[m, :] . W_e[n, :] for
+// end_{e-1} <= m < end_e, summed in fp32 with no bias and no rounding, and 0 for end_{E-1} <= m < M.  Plain fp32
+// statistics only (a K shard never carries nested ones).  With the same tile, T(P + bias_e) is launch_gemm4_grouped's
+// output bit for bit: same decode, same k16 order, the same accumulators, rounded once.  Returns false as
+// launch_gemm4_grouped does.
+template <typename T>
+bool launch_gemm4_grouped_partial(const T* A, const uint8_t* B, const float* absmax, const int* offs, int E, float* out,
+                                  int M, int N, int K, int ldc, int blocksize, int quant_type, int mt,
+                                  cudaStream_t stream) {
+    static_assert(!std::is_same<T, float>::value, "the grouped GEMM has 16-bit instances only");
+    if (M <= 0) return true;
+    if (N <= 0 || E < 1 || E > kMaxExperts || (long long)E * N > 0x7fffffffLL || K < 64 || (K % 64) != 0) return false;
+    if (blocksize < 32 || (blocksize & (blocksize - 1)) != 0) return false;
+    if ((reinterpret_cast<uintptr_t>(A) & 15) != 0 || (reinterpret_cast<uintptr_t>(B) & 15) != 0) return false;
+    if (quant_type != kNF4 && quant_type != kFP4) return false;
+    Gemm4Params p{};
+    p.B = B;
+    p.absmax = absmax;
+    p.out = out;
+    p.M = M;
+    p.N = N;
+    p.K = K;
+    p.ldc = ldc;
+    p.log2_bs = ilog2_pow2(blocksize);
+    p.offs = offs;
+    p.E = E;
+#define BNB200_GROUPED_PART_MT(QT)                                                                                     \
+    switch (mt) {                                                                                                      \
+    case 16: return launch_mt<T, QT, 16, false, true, true>(A, p, 1, stream);                                          \
+    case 32: return launch_mt<T, QT, 32, false, true, true>(A, p, 1, stream);                                          \
+    case 64: return launch_mt<T, QT, 64, false, true, true>(A, p, 1, stream);                                          \
+    case 128: return launch_mt<T, QT, 128, false, true, true>(A, p, 1, stream);                                        \
+    default: return false;                                                                                             \
+    }
+    if (quant_type == kNF4) {
+        BNB200_GROUPED_PART_MT(kNF4)
+    } else {
+        BNB200_GROUPED_PART_MT(kFP4)
+    }
+#undef BNB200_GROUPED_PART_MT
+}
+template bool launch_gemm4_grouped_partial<__nv_bfloat16>(const __nv_bfloat16*, const uint8_t*, const float*, const int*,
+                                                          int, float*, int, int, int, int, int, int, int, cudaStream_t);
+template bool launch_gemm4_grouped_partial<__half>(const __half*, const uint8_t*, const float*, const int*, int, float*,
+                                                   int, int, int, int, int, int, int, cudaStream_t);
 
 } // namespace bnb200

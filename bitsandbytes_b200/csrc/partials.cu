@@ -151,6 +151,110 @@ __global__ void __launch_bounds__(kReduceThreads)
     }
 }
 
+// The reduction of a row-sharded expert layer (the grouped partials of cbnb_b200_gemm_4bit_grouped_partial): the
+// arithmetic of reduce_partials_kernel, with the bias of the expert that owns row m, bias[e(m) * N + n], and zeros in
+// the rows past end_{E-1}.  Each CTA first clamps offs into its own table of end rows, end_e = min(max(offs[0..e], 0),
+// M) -- the prefix maximum the grouped GEMM computes -- so that nothing is read on the host; a row's expert is then
+// the number of end rows <= m, found by binary search.
+constexpr int kEndsPer = kMaxExperts / kReduceThreads;
+static_assert(kEndsPer * kReduceThreads == kMaxExperts, "each thread clamps kEndsPer experts");
+
+template <typename T, bool VEC>
+__global__ void __launch_bounds__(kReduceThreads)
+    reduce_partials_grouped_kernel(const float* __restrict__ parts, int world, long long part_stride,
+                                   const int* __restrict__ offs, int E, T* __restrict__ out, const T* __restrict__ bias,
+                                   int M, int N, int ldc) {
+    __shared__ int gend[kMaxExperts];
+    __shared__ int wmax[kReduceThreads / 32];
+    {
+        // thread t clamps experts [t * kEndsPer, (t + 1) * kEndsPer): a running maximum over its own, a warp scan of
+        // the maxima by shuffles, then the maxima of the warps before it
+        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+        const int e0 = threadIdx.x * kEndsPer;
+        int v[kEndsPer];
+        int run = 0;
+#pragma unroll
+        for (int i = 0; i < kEndsPer; ++i) {
+            v[i] = e0 + i < E ? max(__ldg(offs + e0 + i), 0) : 0;
+            run = max(run, v[i]);
+        }
+        int inc = run;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const int o = __shfl_up_sync(0xffffffffu, inc, d);
+            if (lane >= d) inc = max(inc, o);
+        }
+        if (lane == 31) wmax[warp] = inc;
+        __syncthreads();
+        int r = __shfl_up_sync(0xffffffffu, inc, 1);
+        if (lane == 0) r = 0;
+        for (int w = 0; w < warp; ++w) r = max(r, wmax[w]);
+#pragma unroll
+        for (int i = 0; i < kEndsPer; ++i) {
+            r = max(r, v[i]);
+            if (e0 + i < E) gend[e0 + i] = min(r, M);
+        }
+        __syncthreads();
+    }
+    const int m_tail = gend[E - 1];
+    constexpr int V = VEC ? 16 / (int)sizeof(T) : 1;
+    const int per_row = N / V;
+    const long long total = (long long)M * per_row;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+         i += (long long)gridDim.x * blockDim.x) {
+        const int m = (int)(i / per_row);
+        const int n = (int)(i - (long long)m * per_row) * V;
+        float s[V];
+        const T* b = nullptr;
+        if (m >= m_tail) {
+#pragma unroll
+            for (int j = 0; j < V; ++j) s[j] = 0.f;
+        } else {
+            // the expert of row m: the first e with end_e > m (there is one, since m < end_{E-1})
+            int lo = 0, hi = E - 1;
+            while (lo < hi) {
+                const int mid = (lo + hi) >> 1;
+                if (gend[mid] > m) hi = mid;
+                else lo = mid + 1;
+            }
+            if (bias != nullptr) b = bias + (long long)lo * N;
+            const float* src = parts + (long long)m * N + n;
+            if constexpr (VEC) {
+#pragma unroll
+                for (int h = 0; h < V / 4; ++h) first4(s + 4 * h, __ldcs(reinterpret_cast<const float4*>(src) + h));
+                for (int r = 1; r < world; ++r) {
+#pragma unroll
+                    for (int h = 0; h < V / 4; ++h)
+                        add4(s + 4 * h, __ldcs(reinterpret_cast<const float4*>(src + r * part_stride) + h));
+                }
+            } else {
+                s[0] = src[0];
+                for (int r = 1; r < world; ++r) s[0] = __fadd_rn(s[0], src[r * part_stride]);
+            }
+        }
+        bias_round_store<T, VEC>(s, b, out, m, n, ldc);
+    }
+}
+
+template <typename T>
+void launch_grouped_typed(const float* parts, int world, long long part_stride, const int* offs, int E, T* out,
+                          const T* bias, int M, int N, int ldc, cudaStream_t stream) {
+    constexpr int V = 16 / (int)sizeof(T);
+    const bool vec = N % V == 0 && ldc % V == 0 && part_stride % 4 == 0 &&
+                     (reinterpret_cast<uintptr_t>(parts) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0;
+    const long long items = (long long)M * (vec ? N / V : N);
+    const long long blocks = (items + kReduceThreads - 1) / kReduceThreads;
+    const long long cap = (long long)device_sm_count() * 8;
+    const int grid = (int)(blocks < cap ? blocks : cap);
+    if (vec)
+        reduce_partials_grouped_kernel<T, true><<<grid, kReduceThreads, 0, stream>>>(parts, world, part_stride, offs, E,
+                                                                                     out, bias, M, N, ldc);
+    else
+        reduce_partials_grouped_kernel<T, false><<<grid, kReduceThreads, 0, stream>>>(parts, world, part_stride, offs,
+                                                                                      E, out, bias, M, N, ldc);
+    BNB200_CHECK_LAUNCH("reduce_partials_grouped");
+}
+
 template <typename T>
 void launch_typed(const float* parts, int world, long long part_stride, T* out, const T* bias, int M, int N, int ldc,
                   cudaStream_t stream) {
@@ -309,6 +413,21 @@ bool launch_reduce_partials(const float* parts, int world, long long part_stride
     else if (dtype == 2)
         launch_typed<__nv_bfloat16>(parts, world, part_stride, (__nv_bfloat16*)out, (const __nv_bfloat16*)bias, M, N,
                                     ldc, stream);
+    else
+        return false;
+    return true;
+}
+
+bool launch_reduce_partials_grouped(const float* parts, int world, long long part_stride, const int* offs, int E,
+                                    void* out, const void* bias, int M, int N, int ldc, int dtype, cudaStream_t stream) {
+    if (world < 1 || part_stride < 0 || ldc < N || E < 1 || E > kMaxExperts || offs == nullptr) return false;
+    if (M <= 0 || N <= 0) return true;
+    if (dtype == 1)
+        launch_grouped_typed<__half>(parts, world, part_stride, offs, E, (__half*)out, (const __half*)bias, M, N, ldc,
+                                     stream);
+    else if (dtype == 2)
+        launch_grouped_typed<__nv_bfloat16>(parts, world, part_stride, offs, E, (__nv_bfloat16*)out,
+                                            (const __nv_bfloat16*)bias, M, N, ldc, stream);
     else
         return false;
     return true;

@@ -94,18 +94,19 @@ import torch
 import torch.distributed as dist
 
 from . import functional as F
-from .backends.cuda import (gemm_4bit_into, gemm_4bit_multi_out, gemm_4bit_partial,
-                            gemm_4bit_partial_scatter, int8_dequant_rows, int8_gemm_multi_out, int8_gemm_partial_scatter,
-                            int8_outlier_operands, int8_quant_with_stats,
+from .backends.cuda import (gemm_4bit_grouped_into, gemm_4bit_grouped_partial, gemm_4bit_into, gemm_4bit_multi_out,
+                            gemm_4bit_partial, gemm_4bit_partial_scatter, int8_dequant_rows, int8_gemm_multi_out,
+                            int8_gemm_partial_scatter, int8_outlier_operands, int8_quant_with_stats,
                             int8_reduce_partials, int8_row_stats, int8_vectorwise_quant_flags, int8_zero_columns,
-                            reduce_partials, reduce_partials_ptrs)
+                            reduce_partials, reduce_partials_grouped, reduce_partials_ptrs)
 
 
 @dataclass
 class Shard4bit:
-    """The slice of a quantised [N, K] weight owned by one rank."""
+    """The slice of a quantised [N, K] weight owned by one rank; with ``experts`` = E > 1, the slice of every expert of
+    an [E, N, K] expert tensor, stacked as an [E, rows, K] weight."""
 
-    packed: torch.Tensor            # uint8 [rows*K/2]
+    packed: torch.Tensor            # uint8 [experts*rows*K/2]
     absmax: torch.Tensor            # fp32 [rows*K/bs]  (plain)  |  level-2 absmax slice (nested)
     absmax_8bit: Optional[torch.Tensor]
     absmax_code: Optional[torch.Tensor]
@@ -116,13 +117,14 @@ class Shard4bit:
     blocksize: int
     quant_type: str
     k0: int = 0                     # first input feature of a K shard (slice_quantized_weight_k)
+    experts: int = 1                # experts of a grouped shard (slice_grouped_weight, slice_grouped_weight_k)
 
     def dequantize(self, dtype: torch.dtype) -> torch.Tensor:
-        """The shard's weight ``[rows, K]`` decoded to ``dtype`` as ``dequantize_4bit`` decodes it."""
+        """The shard's weight ``[experts * rows, K]`` decoded to ``dtype`` as ``dequantize_4bit`` decodes it."""
         scales = self.absmax
         if self.absmax_8bit is not None:
             scales = _nested_scales(self.absmax_8bit, self.absmax, self.absmax_code, self.absmax_offset)
-        out = torch.empty((self.rows, self.K), device=self.packed.device, dtype=dtype)
+        out = torch.empty((self.experts * self.rows, self.K), device=self.packed.device, dtype=dtype)
         return F.dequantize_4bit(self.packed, absmax=scales, out=out, blocksize=self.blocksize,
                                  quant_type=self.quant_type)
 
@@ -418,17 +420,17 @@ def _group_world_rank(group) -> tuple[int, int]:
     return 1, 0
 
 
-def _gather_columns(layer, inp, M: int, dtype: torch.dtype, device) -> torch.Tensor:
-    """The ``[M, world * rows]`` output of a column-parallel layer: ``layer.local_forward`` writes this rank's
-    ``[M, rows]`` block into its slot of a ``[world, M, rows]`` stage (kept on the layer for the next call), and the
-    stage is all-gathered.  The blocks sit side by side along the inner dimension of a row-major matrix, which
+def _gather_columns(layer, inp, M: int, dtype: torch.dtype, device, **kw) -> torch.Tensor:
+    """The ``[M, world * rows]`` output of a column-parallel layer: ``layer.local_forward`` (given ``kw``) writes this
+    rank's ``[M, rows]`` block into its slot of a ``[world, M, rows]`` stage (kept on the layer for the next call), and
+    the stage is all-gathered.  The blocks sit side by side along the inner dimension of a row-major matrix, which
     ``all_gather_into_tensor`` cannot write in place, hence the stage and the permute."""
     world, rank = _group_world_rank(layer.group)
     rows = layer.shard.rows
     stage = layer._stage
     if stage is None or stage.shape != (world, M, rows) or stage.dtype != dtype or stage.device != device:
         stage = layer._stage = torch.empty((world, M, rows), device=device, dtype=dtype)
-    layer.local_forward(inp, stage[rank], rows)
+    layer.local_forward(inp, stage[rank], rows, **kw)
     dist.all_gather_into_tensor(stage.view(-1), stage[rank].reshape(-1), group=layer.group)
     return stage.permute(1, 0, 2).reshape(M, world * rows)
 
@@ -440,14 +442,14 @@ def _check_peers(peers, M: int, N: int, dtype: torch.dtype, what: str) -> None:
         raise ValueError(f"{type(peers).__name__} was built for a different {what}")
 
 
-def _gather_partials(layer, inp, M: int, dtype: torch.dtype, device, what: str) -> torch.Tensor:
-    """The ``[world, M, N]`` partials of a row-parallel layer: ``layer.partial_forward`` writes this rank's into its
-    slot of a stage (kept on the layer for the next call), and the stage is all-gathered."""
+def _gather_partials(layer, inp, M: int, dtype: torch.dtype, device, what: str, **kw) -> torch.Tensor:
+    """The ``[world, M, N]`` partials of a row-parallel layer: ``layer.partial_forward`` (given ``kw``) writes this
+    rank's into its slot of a stage (kept on the layer for the next call), and the stage is all-gathered."""
     world, rank = _group_world_rank(layer.group)
     stage = layer._stage
     if stage is None or stage.shape[:2] != (world, M) or stage.device != device:
         stage = layer._stage = torch.empty((world, M, layer.shard.rows), device=device, dtype=dtype)
-    if not layer.partial_forward(inp, [stage[rank]]):
+    if not layer.partial_forward(inp, [stage[rank]], **kw):
         raise RuntimeError(f"{what} does not serve this shard shape")
     if world > 1:
         dist.all_gather_into_tensor(stage.view(-1), stage[rank].reshape(-1), group=layer.group)
@@ -735,6 +737,175 @@ def fused_forward_col_sp(layer: ColumnParallelLinear4bit, x: torch.Tensor, peers
 def reassemble_shards(shards: list[Shard4bit]) -> tuple[torch.Tensor, torch.Tensor]:
     """Inverse of slice_quantized_weight for the plain (non-nested) case: (packed, absmax)."""
     return torch.cat([s.packed for s in shards]), torch.cat([s.absmax for s in shards])
+
+
+# ====================================================================================== tensor-parallel expert layers
+# Mixture-of-experts layers on a 4-bit [E, N, K] expert tensor (GroupedLinear4bit's weight, quantised once, globally),
+# sharded as the dense layers are: the column layer (gate_up) holds output rows [r*N/w, (r+1)*N/w) of EVERY expert, the
+# row layer (down) input features [r*K/w, (r+1)*K/w) of every expert.  Routing stays with the model: each layer takes
+# the expert-sorted rows x [M, K] and the int32 end row of every expert, offs [E], on the device.  ``offs`` and the token
+# rows must be the same on every rank.  Nothing reads offs on the host, so a forward can be captured in a CUDA graph.
+#   * column: one grouped GEMM on the shard (the unsharded kernel and tile on fewer rows per expert), so the gathered
+#     output is GroupedLinear4bit's bit for bit.
+#   * row: the grouped fp32 partial of the shard (the unsharded layer's tile, which depends on M and E only), the
+#     partials gathered as the dense row layer gathers them, and a rank-order reduction that adds each row's expert
+#     bias and rounds once.  With one rank that is GroupedLinear4bit's output bit for bit; with more it differs only by
+#     the order of the fp32 sum.
+# Inference only: an input that requires grad, sequence parallelism and the symmetric-memory routes are refused.
+
+def slice_grouped_weight(packed: torch.Tensor, qs: F.QuantState, world: int, rank: int) -> Shard4bit:
+    """Cut rank's output rows ``[r*N/w, (r+1)*N/w)`` out of every expert of an ``[E, N, K]`` expert tensor quantised
+    once, globally, and stack them as an ``[E, N/w, K]`` shard.  Requires ``K % blocksize == 0`` and ``N % world == 0``.
+    Nested statistics stay nested when every expert's slice starts and ends on a 256-block boundary; otherwise they
+    become plain fp32 scales computed as the kernels fetch them (:func:`nested_scales`), which decode to the same
+    weights bit for bit.
+
+    A fused ``gate_up`` tensor that stacks gate and up along N is cut into contiguous N ranges, so the slice of a rank
+    holds matching gate and up rows only if the tensor interleaves them that way; the layer does not reorder."""
+    if len(qs.shape) != 3:
+        raise ValueError(f"slice_grouped_weight: the state must be of an [E, N, K] expert tensor, got {list(qs.shape)}")
+    E, N, K = qs.shape
+    bs = qs.blocksize
+    _check_rank(world, rank)
+    if K % bs != 0:
+        raise ValueError(f"in_features ({K}) must be a multiple of the blocksize ({bs}) to shard by rows")
+    row0, rows = shard_rows(N, world, rank)
+    flat = packed.reshape(-1).view(torch.uint8) if packed.dtype != torch.uint8 else packed.reshape(-1)
+    codes = flat[:E * N * K // 2].view(E, N * K // 2)[:, row0 * K // 2:(row0 + rows) * K // 2].contiguous().view(-1)
+    nb = N * K // bs  # quantisation blocks per expert
+    a0, a1 = row0 * K // bs, (row0 + rows) * K // bs
+    common = dict(rows=rows, row0=row0, K=K, blocksize=bs, quant_type=qs.quant_type, experts=E)
+    if qs.nested and all((e * nb + a0) % 256 == 0 for e in range(E)) and (a1 - a0) % 256 == 0:
+        a2 = torch.cat([qs.state2.absmax[(e * nb + a0) // 256:(e * nb + a1) // 256] for e in range(E)])
+        return Shard4bit(packed=codes, absmax=a2, absmax_8bit=qs.absmax.reshape(E, nb)[:, a0:a1].contiguous().view(-1),
+                         absmax_code=qs.state2.code, absmax_offset=qs.offset.reshape(1).float(), **common)
+    scales = nested_scales(qs) if qs.nested else qs.absmax
+    return Shard4bit(packed=codes, absmax=scales.reshape(E, nb)[:, a0:a1].contiguous().view(-1), absmax_8bit=None,
+                     absmax_code=None, absmax_offset=None, **common)
+
+
+def slice_grouped_weight_k(packed: torch.Tensor, qs: F.QuantState, world: int, rank: int) -> Shard4bit:
+    """Rank's input features ``[r*K/w, (r+1)*K/w)`` of every expert of an ``[E, N, K]`` expert tensor:
+    :func:`slice_quantized_weight_k` of the flattened ``[E*N, K]`` weight (the same rules; plain fp32 scales), as an
+    ``[E, N, K/w]`` shard."""
+    if len(qs.shape) != 3:
+        raise ValueError(f"slice_grouped_weight_k: the state must be of an [E, N, K] expert tensor, got "
+                         f"{list(qs.shape)}")
+    E, N, K = qs.shape
+    flat = F.QuantState(absmax=qs.absmax, shape=torch.Size([E * N, K]), code=qs.code, blocksize=qs.blocksize,
+                        quant_type=qs.quant_type, dtype=qs.dtype, offset=qs.offset, state2=qs.state2)
+    s = slice_quantized_weight_k(packed, flat, world, rank)
+    s.rows, s.experts = N, E
+    return s
+
+
+def _grouped_inference_only(what: str, x: torch.Tensor) -> None:
+    if torch.is_grad_enabled() and x.requires_grad:
+        raise RuntimeError(f"{what} is inference only: the input requires grad, and training through the tensor-parallel "
+                           "expert layers is not implemented (run it under torch.no_grad() or detach the input)")
+
+
+class _GroupedNoFusedRoute:
+    """The fused symmetric-memory routes (``fused_forward*``) call ``_forward`` / ``_grad_slot``: refused."""
+
+    def _refuse(self, *args, **kwargs):
+        raise RuntimeError(f"{type(self).__name__} has no symmetric-memory route: call the layer itself")
+
+    _forward = _grad_slot = _refuse
+
+
+def _no_sequence_parallel(cls, sequence_parallel: bool) -> None:
+    if sequence_parallel:
+        raise ValueError(f"{cls.__name__} does not support sequence_parallel=True")
+
+
+class ColumnParallelGroupedLinear4bit(_GroupedNoFusedRoute, torch.nn.Module):
+    """The experts of a mixture-of-experts layer with their output features split across the process group (gate_up):
+    ``forward(x, offs)`` gives this rank's ``[M, N/w]`` columns, or with ``gather_output`` the whole ``[M, N]``,
+    GroupedLinear4bit's output bit for bit.  ``bias`` is the full ``[E, N]`` bias, of which the layer keeps its
+    ``[E, N/w]`` slice.  See :func:`slice_grouped_weight` for fused gate_up tensors."""
+
+    def __init__(self, shard: Shard4bit, out_features: int, bias: Optional[torch.Tensor] = None,
+                 group: Optional[dist.ProcessGroup] = None, gather_output: bool = True, sequence_parallel: bool = False):
+        super().__init__()
+        _no_sequence_parallel(type(self), sequence_parallel)
+        self.shard = shard
+        self.out_features = out_features
+        self.group = group
+        self.gather_output = gather_output
+        self.bias_shard = None if bias is None else \
+            bias.reshape(shard.experts, out_features)[:, shard.row0:shard.row0 + shard.rows].contiguous()
+        self._stage = None
+
+    @classmethod
+    def from_quantized(cls, packed, qs: F.QuantState, bias=None, group=None, gather_output=True,
+                       sequence_parallel=False):
+        world, rank = _group_world_rank(group)
+        return cls(slice_grouped_weight(packed, qs, world, rank), qs.shape[1], bias, group, gather_output,
+                   sequence_parallel)
+
+    def local_forward(self, x: torch.Tensor, out: Optional[torch.Tensor] = None, ldc: Optional[int] = None, *,
+                      offs: torch.Tensor) -> torch.Tensor:
+        """This rank's ``[M, N/w]`` columns; written into ``out`` (row stride ``ldc`` elements) if given."""
+        s = self.shard
+        if out is None:
+            out = torch.empty((x.shape[0], s.rows), device=x.device, dtype=x.dtype)
+            ldc = s.rows
+        gemm_4bit_grouped_into(x, s.packed, (s.experts, s.rows, s.K), s.absmax, s.blocksize, s.quant_type, offs,
+                               self.bias_shard, s.absmax_8bit, s.absmax_code, s.absmax_offset, out, ldc)
+        return out
+
+    def forward(self, x: torch.Tensor, offs: torch.Tensor) -> torch.Tensor:
+        _grouped_inference_only(type(self).__name__, x)
+        world, _ = _group_world_rank(self.group)
+        if world == 1 or not self.gather_output:
+            return self.local_forward(x, offs=offs)
+        return _gather_columns(self, x, x.shape[0], x.dtype, x.device, offs=offs)
+
+
+class RowParallelGroupedLinear4bit(_GroupedNoFusedRoute, torch.nn.Module):
+    """The experts of a mixture-of-experts layer with their input features split across the process group (down):
+    ``forward(x, offs)`` returns the whole ``[M, N]`` output, the same bits on every rank.  Each rank computes the fp32
+    partial of its K slice for every expert (no bias, no rounding), the partials are all-gathered, and every rank sums
+    them in rank order, adds the bias of each row's expert (``bias`` ``[E, N]``) and rounds once."""
+
+    def __init__(self, shard: Shard4bit, in_features: int, bias: Optional[torch.Tensor] = None,
+                 group: Optional[dist.ProcessGroup] = None, input_is_parallel: bool = True,
+                 sequence_parallel: bool = False):
+        super().__init__()
+        _no_sequence_parallel(type(self), sequence_parallel)
+        self.shard = shard
+        self.in_features = in_features
+        self.out_features = shard.rows
+        self.group = group
+        self.input_is_parallel = input_is_parallel
+        self.bias = None if bias is None else bias.reshape(shard.experts, shard.rows).contiguous()
+        self._stage = None
+
+    @classmethod
+    def from_quantized(cls, packed, qs: F.QuantState, bias=None, group=None, input_is_parallel=True,
+                       sequence_parallel=False):
+        world, rank = _group_world_rank(group)
+        return cls(slice_grouped_weight_k(packed, qs, world, rank), qs.shape[2], bias, group, input_is_parallel,
+                   sequence_parallel)
+
+    local_input = RowParallelLinear4bit.local_input
+
+    def partial_forward(self, x_r: torch.Tensor, outs, ldc: Optional[int] = None, *, offs: torch.Tensor) -> bool:
+        """``P_r = x_r . dequant(W_r)^T`` of every expert's rows in fp32 (no bias, no rounding) into ``outs[0]``."""
+        s = self.shard
+        if len(outs) != 1:
+            raise ValueError("the grouped partial GEMM writes one destination")
+        gemm_4bit_grouped_partial(x_r, s.packed, (s.experts, s.rows, s.K), s.absmax, s.blocksize, s.quant_type, offs,
+                                  outs[0], s.rows if ldc is None else ldc)
+        return True
+
+    def forward(self, x: torch.Tensor, offs: torch.Tensor) -> torch.Tensor:
+        _grouped_inference_only(type(self).__name__, x)
+        x_r = self.local_input(x)
+        parts = _gather_partials(self, x_r, x_r.shape[0], torch.float32, x_r.device, "gemm_4bit_grouped_partial",
+                                 offs=offs)
+        return reduce_partials_grouped(parts, offs, x_r.dtype, self.bias)
 
 
 # ====================================================================================== tensor-parallel LLM.int8()

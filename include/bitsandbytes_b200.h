@@ -215,6 +215,22 @@ int cbnb_b200_gemm_4bit_pair(const void* A, const uint8_t* B, const float* absma
 int cbnb_b200_gemm_4bit_grouped(const void* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit, const float* absmax_code, const float* absmax_offset, const int* offs, int E, void* out, const void* bias, int M, int N, int K, int ldc, int blocksize, int quant_type, int dtype, bnb_stream_t stream);
 int cbnb_b200_gemm_4bit_grouped_mt(const void* A, const uint8_t* B, const float* absmax, const uint8_t* absmax_8bit, const float* absmax_code, const float* absmax_offset, const int* offs, int E, void* out, const void* bias, int M, int N, int K, int ldc, int blocksize, int quant_type, int dtype, int mt, bnb_stream_t stream);
 
+/* Row-sharded (input-feature-sharded) expert layers.  cbnb_b200_gemm_4bit_grouped_partial: out[m, n] (fp32, row stride
+ * ldc) = A[m, :] . W_e[n, :] summed in fp32, no bias and no rounding, for the rows of expert e, and 0 for the rows past
+ * end_{E-1}; A, B, offs as in cbnb_b200_gemm_4bit_grouped, absmax plain fp32 (a shard never carries nested statistics).
+ * mt: token tile 16 | 32 | 64 | 128, 0 = the grouped GEMM's rule for (M, E).  With the same tile, T(P + bias_e) is
+ * cbnb_b200_gemm_4bit_grouped_mt's output bit for bit.  Returns 0; 1 with the error message set for bad arguments
+ * (NULL operand, M < 0, N, K or E < 1, ldc < N, bad quant_type or mt); 100 with nothing written for what it does not
+ * serve (fp32 A, K not a multiple of 64, E > 1024, a bad blocksize, misaligned A or B), or 100 with the message set
+ * when a launch fails.
+ * cbnb_b200_reduce_partials_grouped: out[m, n] (row stride ldc) = T(((parts[0] + parts[1]) + ... + parts[world-1])[m, n]
+ * + bias[e * N + n]) for the rows of expert e (end rows clamped on the device from offs, as the grouped GEMM does), 0
+ * for the rows past end_{E-1}; the partials [M, N] at row stride N, one every part_stride elements; bias T[E * N] or
+ * NULL.  The element arithmetic of cbnb_b200_reduce_partials.  dtype 1 = fp16, 2 = bf16.  Returns 0, or 100 for a dtype,
+ * world or E (1..1024) it does not serve.  Neither call reads offs on the host. */
+int cbnb_b200_gemm_4bit_grouped_partial(const void* A, const uint8_t* B, const float* absmax, const int* offs, int E, float* out, int M, int N, int K, int ldc, int blocksize, int quant_type, int dtype, int mt, bnb_stream_t stream);
+int cbnb_b200_reduce_partials_grouped(const float* parts, int world, long long part_stride, const int* offs, int E, void* out, const void* bias, int M, int N, int ldc, int dtype, bnb_stream_t stream);
+
 /* Developer / test entries for the staged route.  _staged: the whole route with token tile mt (128 | 256,
  * 0 = by the shape) and panel_rows output features per panel (a multiple of 128 whose decoded rows fit the 32 MB
  * per-stream workspace, 0 = the largest such), stores to outs[0..n_outs) as _multi_out; returns 0, or 100 when not
