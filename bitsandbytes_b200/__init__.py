@@ -7,8 +7,9 @@ Layout (only what the path needs):
     csrc/              CUDA kernels + the extern "C" boundary
     _ops.py            torch.library schemas (namespace ``bitsandbytes::``) + the CUDA kernels' host side
     functional.py      QuantState, quantize/dequantize_{blockwise,4bit}, int8_* ...
-    autograd/          matmul_4bit / grouped_matmul_4bit / matmul (MatMul4Bit, GroupedMatMul4Bit, MatMul8bitLt)
-    nn/                Linear4bit, GroupedLinear4bit, Params4bit, Linear8bitLt, Int8Params
+    autograd/          matmul_4bit / grouped_matmul_4bit / matmul / grouped_matmul_8bit (MatMul4Bit, GroupedMatMul4Bit,
+                       MatMul8bitLt, GroupedMatMul8bitLt)
+    nn/                Linear4bit, GroupedLinear4bit, Params4bit, Linear8bitLt, GroupedLinear8bitLt, Int8Params
     parallel.py        column-sharded Linear4bit over NCCL (one process per GPU)
     optim/             optimizers with 32-bit / blockwise 8-bit state (Adam, AdamW, Lion, SGD, RMSprop, ...)
 """
@@ -24,7 +25,7 @@ def __getattr__(name):
 
     if name in _LAZY:
         return importlib.import_module(f"{__name__}.{name}")
-    if name in ("matmul", "matmul_4bit", "grouped_matmul_4bit", "MatmulLtState"):
+    if name in ("matmul", "matmul_4bit", "grouped_matmul_4bit", "grouped_matmul_8bit", "MatmulLtState"):
         mod = importlib.import_module(f"{__name__}.autograd._functions")
         return getattr(mod, name)
     raise AttributeError(f"module {__name__!r} has no attribute {name!r}")

@@ -49,6 +49,9 @@ SCHEMAS = {
     # mixture-of-experts layer), shapeB = [E, N, K]
     "gemm_4bit_grouped": "(Tensor A, Tensor B, int[] shapeB, Tensor absmax, int blocksize, str quant_type, Tensor offs, "
     "Tensor? bias=None, Tensor? absmax_8bit=None, Tensor? absmax_code=None, Tensor? absmax_offset=None) -> Tensor",
+    # no reference counterpart: LLM.int8() over every expert of a mixture-of-experts layer in one GEMM launch, CB the
+    # [E, N, K] int8 expert tensor and SCB its [E * N] row statistics
+    "int8_grouped_mm": "(Tensor A, Tensor CB, Tensor SCB, Tensor offs, float threshold=0.0, Tensor? bias=None) -> Tensor",
 }
 
 _defined = False
@@ -231,6 +234,38 @@ def _(A, B, shapeB, absmax, blocksize, quant_type, offs, bias=None, absmax_8bit=
       absmax_offset=None):
     _, N, _ = check_grouped(A, B, shapeB, absmax, blocksize, quant_type, offs, bias, absmax_8bit, absmax_code,
                             absmax_offset)
+    return torch.empty((A.shape[0], N), device=A.device, dtype=A.dtype)
+
+
+def check_int8_grouped(A, CB, SCB, offs, threshold=0.0, bias=None):
+    """What the host knows of an int8_grouped_mm call, checked: shapes, dtypes and devices (never the values of
+    ``offs``, which stay on the device).  Returns (E, N, K).  Shared by the CUDA kernel and the shape function."""
+    torch._check(A.dtype in (torch.float16, torch.bfloat16), lambda: f"int8_grouped_mm: A must be float16 or bfloat16, "
+                 f"got {A.dtype}")
+    torch._check(CB.dtype == torch.int8 and CB.dim() == 3, lambda: f"int8_grouped_mm: CB must be the int8 [E, N, K] "
+                 f"expert tensor, got {CB.dtype} {list(CB.shape)}")
+    E, N, K = CB.shape
+    torch._check(1 <= E <= MAX_EXPERTS, lambda: f"int8_grouped_mm: 1 <= E <= {MAX_EXPERTS} experts, got {E}")
+    torch._check(N >= 1, lambda: f"int8_grouped_mm: N = {N} must be positive")
+    torch._check(K > 0 and K % 16 == 0, lambda: f"int8_grouped_mm: K = {K} must be a positive multiple of 16")
+    torch._check(A.dim() == 2 and A.shape[1] == K, lambda: f"int8_grouped_mm: A must be [M, {K}] for an [E, N, K] = "
+                 f"{list(CB.shape)} weight, got {list(A.shape)}")
+    torch._check(SCB.dtype == torch.float32 and tuple(SCB.shape) == (E * N,), lambda: f"int8_grouped_mm: SCB must be "
+                 f"float32 [{E * N}] (the row statistics of the [E * N, K] codes), got {SCB.dtype} {list(SCB.shape)}")
+    torch._check(offs.dtype == torch.int32 and tuple(offs.shape) == (E,),
+                 lambda: f"int8_grouped_mm: offs must be int32 [{E}], got {offs.dtype} {list(offs.shape)}")
+    torch._check(threshold >= 0.0, lambda: f"int8_grouped_mm: threshold must be non-negative, got {threshold}")
+    if bias is not None:
+        torch._check(bias.dtype == A.dtype and tuple(bias.shape) == (E, N),
+                     lambda: f"int8_grouped_mm: bias must be {A.dtype} [{E}, {N}], got {bias.dtype} {list(bias.shape)}")
+    for t in (CB, SCB, offs, bias):
+        torch._check(t is None or t.device == A.device, lambda: f"int8_grouped_mm: every operand must be on {A.device}")
+    return E, N, K
+
+
+@fake("int8_grouped_mm")
+def _(A, CB, SCB, offs, threshold=0.0, bias=None):
+    _, N, _ = check_int8_grouped(A, CB, SCB, offs, threshold, bias)
     return torch.empty((A.shape[0], N), device=A.device, dtype=A.dtype)
 
 

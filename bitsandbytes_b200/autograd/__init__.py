@@ -1,2 +1,2 @@
-from ._functions import (GroupedMatMul4Bit, MatMul4Bit, MatMul8bitLt, MatmulLtState,  # noqa: F401
-                         grouped_matmul_4bit, matmul, matmul_4bit)
+from ._functions import (GroupedMatMul4Bit, GroupedMatMul8bitLt, MatMul4Bit, MatMul8bitLt,  # noqa: F401
+                         MatmulLtState, grouped_matmul_4bit, grouped_matmul_8bit, matmul, matmul_4bit)

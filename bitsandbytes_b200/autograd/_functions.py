@@ -25,7 +25,8 @@ from warnings import warn
 import torch
 
 from .. import functional as F
-from ..backends.cuda import int8_mixed_mm_flags, int8_vectorwise_quant_flags, int8_zero_columns
+from .._ops import check_int8_grouped
+from ..backends.cuda import int8_dequant_rows, int8_mixed_mm_flags, int8_vectorwise_quant_flags, int8_zero_columns
 
 logger = logging.getLogger(__name__)
 
@@ -342,6 +343,27 @@ def _clamped_ends(offs, M):
     return offs.clamp(min=0).cummax(0).values.clamp(max=M)
 
 
+def _grouped_backward(grad_output, offs, E, N, need_A, need_bias, weight):
+    """(grad_A, grad_bias) of a grouped expert GEMM with a frozen weight: ``weight()`` gives the dequantised ``[E, N,
+    K]`` expert tensor in grad_output's dtype, grad_A is ``grouped_mm`` over the clamped ends with the rows past the
+    last end zeroed, and grad_bias the per-expert segment sums of grad_output.  Nothing reads ``offs`` on the host."""
+    M = grad_output.shape[0]
+    ends = _clamped_ends(offs, M)
+    grad_A = grad_bias = None
+    if need_A:
+        W = weight()  # [E, N, K]
+        grad_A = torch.nn.functional.grouped_mm(grad_output.contiguous(), W, offs=ends)
+        # rows past the last expert's end belong to no expert: their gradient is zero
+        routed = torch.arange(M, device=grad_A.device).unsqueeze(1) < ends[-1]
+        grad_A = torch.where(routed, grad_A, torch.zeros((), dtype=grad_A.dtype, device=grad_A.device))
+    if need_bias:
+        # segment sums of grad_output's rows in fp32; the rows past the last end go to a discarded segment E
+        eid = torch.searchsorted(ends, torch.arange(M, device=ends.device, dtype=ends.dtype), right=True)
+        sums = torch.zeros((E + 1, N), dtype=torch.float32, device=grad_output.device)
+        grad_bias = sums.index_add_(0, eid, grad_output.float())[:E].to(grad_output.dtype)
+    return grad_A, grad_bias
+
+
 class GroupedMatMul4Bit(torch.autograd.Function):
     """The grouped 4-bit GEMM with a frozen weight.  The backward (bf16) dequantises the expert tensor once and runs
     ``grouped_mm`` for grad_A; nothing in either direction reads ``offs`` on the host."""
@@ -358,20 +380,8 @@ class GroupedMatMul4Bit(torch.autograd.Function):
         need_A, _, _, need_bias, _ = ctx.needs_input_grad
         B, offs = ctx.saved_tensors
         E, N, K = ctx.state.shape
-        M = grad_output.shape[0]
-        ends = _clamped_ends(offs, M)
-        grad_A = grad_bias = None
-        if need_A:
-            W = F.dequantize_4bit(B, ctx.state).to(grad_output.dtype)  # [E, N, K]
-            grad_A = torch.nn.functional.grouped_mm(grad_output.contiguous(), W, offs=ends)
-            # rows past the last expert's end belong to no expert: their gradient is zero
-            routed = torch.arange(M, device=grad_A.device).unsqueeze(1) < ends[-1]
-            grad_A = torch.where(routed, grad_A, torch.zeros((), dtype=grad_A.dtype, device=grad_A.device))
-        if need_bias:
-            # segment sums of grad_output's rows in fp32; the rows past the last end go to a discarded segment E
-            eid = torch.searchsorted(ends, torch.arange(M, device=ends.device, dtype=ends.dtype), right=True)
-            sums = torch.zeros((E + 1, N), dtype=torch.float32, device=grad_output.device)
-            grad_bias = sums.index_add_(0, eid, grad_output.float())[:E].to(grad_output.dtype)
+        grad_A, grad_bias = _grouped_backward(grad_output, offs, E, N, need_A, need_bias,
+                                              lambda: F.dequantize_4bit(B, ctx.state).to(grad_output.dtype))
         return grad_A, None, None, grad_bias, None
 
 
@@ -401,3 +411,46 @@ def grouped_matmul_4bit(A, B, quant_state: F.QuantState, offs, bias=None):
     if N % 8 != 0:
         raise ValueError(f"grouped_matmul_4bit: training needs N % 8 == 0 (grouped_mm's row stride), got N = {N}")
     return GroupedMatMul4Bit.apply(A, B, offs, bias, quant_state)
+
+
+class GroupedMatMul8bitLt(torch.autograd.Function):
+    """The grouped LLM.int8() GEMM with a frozen weight.  The backward (bf16) takes grad_A through ``grouped_mm`` with
+    the whole expert tensor dequantised as ``MatMul8bitLt.backward`` dequantises a weight, ``CB * (SCB / 127)`` with the
+    outliers ignored; nothing in either direction reads ``offs`` on the host."""
+
+    @staticmethod
+    def forward(ctx, A, CB, SCB, offs, bias, threshold):
+        out = torch.ops.bitsandbytes.int8_grouped_mm.default(A, CB, SCB, offs, threshold=threshold, bias=bias)
+        ctx.save_for_backward(CB, SCB, offs)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        need_A, _, _, _, need_bias, _ = ctx.needs_input_grad
+        CB, SCB, offs = ctx.saved_tensors
+        E, N, K = CB.shape
+        grad_A, grad_bias = _grouped_backward(
+            grad_output, offs, E, N, need_A, need_bias,
+            lambda: int8_dequant_rows(CB.reshape(E * N, K), SCB, grad_output.dtype).view(E, N, K))
+        return grad_A, None, None, None, grad_bias, None
+
+
+def grouped_matmul_8bit(A, CB, SCB, offs, threshold=0.0, bias=None):
+    """Every expert of a mixture-of-experts layer in one int8 GEMM launch: for the rows of expert e,
+    ``offs[e-1] <= m < offs[e]`` of the expert-sorted ``A [M, K]`` (fp16 / bf16), ``out[m]`` is what the inference
+    ``Linear8bitLt`` with this ``threshold`` computes on expert e's rows alone -- its own outlier columns included -- and
+    rows past ``offs[E-1]`` are zero.  ``CB [E, N, K]`` / ``SCB [E * N]`` are the expert tensor quantised row-wise as one
+    tensor (``F.int8_vectorwise_quant``, ``Int8Params``), ``offs`` the int32 ``[E]`` end rows on the device (malformed
+    ones are clamped on the device), ``bias`` an optional ``[E, N]``.  The weight is frozen; A and the bias train in
+    bf16 only."""
+    check_int8_grouped(A, CB, SCB, offs, threshold, bias)
+    needs_grad = torch.is_grad_enabled() and (A.requires_grad or (bias is not None and bias.requires_grad))
+    if not needs_grad:
+        return torch.ops.bitsandbytes.int8_grouped_mm.default(A, CB, SCB, offs, threshold=threshold, bias=bias)
+    if A.dtype != torch.bfloat16:
+        raise ValueError(f"grouped_matmul_8bit: training runs in bfloat16 only (the input gradient is "
+                         f"torch.nn.functional.grouped_mm), got {A.dtype} with requires_grad")
+    N = CB.shape[1]
+    if N % 8 != 0:
+        raise ValueError(f"grouped_matmul_8bit: training needs N % 8 == 0 (grouped_mm's row stride), got N = {N}")
+    return GroupedMatMul8bitLt.apply(A, CB, SCB, offs, bias, float(threshold))

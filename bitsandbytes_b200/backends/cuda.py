@@ -27,7 +27,7 @@ from warnings import warn
 
 import torch
 
-from .._ops import MAX_EXPERTS, check_grouped, kernel
+from .._ops import MAX_EXPERTS, check_grouped, check_int8_grouped, kernel
 from .. import cextension as cext
 from ..cextension import lib
 
@@ -923,6 +923,62 @@ def int8_mixed_mm_flags(A, CA, CB, SCA, SCB, col_flags, bias=None) -> torch.Tens
     if rc != 0:
         raise RuntimeError(f"int8_mixed_mm_flags: the int8 GEMM does not take this shape (code {rc}): "
                            f"A={tuple(A.shape)} CB={tuple(CB.shape)}")
+    return out
+
+
+@kernel("int8_grouped_mm")
+def _int8_grouped_mm(A, CB, SCB, offs, threshold=0.0, bias=None):
+    return int8_grouped_mm(A, CB, SCB, offs, threshold, bias)
+
+
+def int8_grouped_mm(A, CB, SCB, offs, threshold=0.0, bias=None) -> torch.Tensor:
+    """LLM.int8() over every expert of a mixture-of-experts layer in one GEMM launch.  ``A [M, K]`` holds the
+    expert-sorted rows, ``CB [E, N, K]`` / ``SCB [E * N]`` the expert tensor quantised row-wise as one tensor, ``offs``
+    the int32 ``[E]`` end rows (clamped on the device), ``bias`` an optional ``[E, N]``.  The rows of expert e are bit
+    for bit what the inference ``Linear8bitLt`` (same threshold) computes on them alone, with each expert's own outlier
+    columns; rows past ``offs[E-1]`` are +0.  Nothing is read back to the host and no allocation depends on the data,
+    so the call can be captured in a CUDA graph and replayed for any routing and any outlier sets."""
+    E, N, K = check_int8_grouped(A, CB, SCB, offs, threshold, bias)
+    M = A.shape[0]
+    _check_sizes("int8_grouped_mm", M, E * N, K, M * K, E * K, E * N * INT8_OUTLIER_CAPACITY)
+    out = torch.empty((M, N), dtype=A.dtype, device=A.device)
+    if M == 0:
+        return out
+    A, CB, SCB, offs = A.contiguous(), CB.contiguous(), SCB.contiguous(), offs.contiguous()
+    bias = bias.contiguous() if bias is not None else None
+    dtype, stream, dev = _DTYPE_ID[A.dtype], _stream(A), A.device
+    # the row codes and statistics of A as fp16, as MatMul8bitLt quantises it (outlier entries -> 0 codes)
+    A16 = A if A.dtype == torch.float16 else A.to(torch.float16)
+    CA = torch.empty((M, K), device=dev, dtype=torch.int8)
+    SCA = torch.empty(M, device=dev, dtype=torch.float32)
+    outl = [None] * 5  # A, subA, subBT, cols, count
+    with _on_device(A):
+        lib.cbnb_b200_int8_vector_quant_flags(A16.data_ptr(), CA.data_ptr(), SCA.data_ptr(), None, float(threshold), M,
+                                              K, _DTYPE_ID[torch.float16], stream)
+        lib.check("int8_grouped_mm")
+        if threshold > 0.0:
+            ends = torch.empty(E, device=dev, dtype=torch.int32)
+            flags = torch.empty((E, K), device=dev, dtype=torch.int32)
+            cols = torch.empty((E, K), device=dev, dtype=torch.int32)
+            count = torch.empty(E, device=dev, dtype=torch.int32)
+            subA = torch.empty((M, INT8_OUTLIER_CAPACITY), device=dev, dtype=A.dtype)
+            subBT = torch.empty((E * N, INT8_OUTLIER_CAPACITY), device=dev, dtype=A.dtype)
+            rc = lib.cbnb_b200_int8_grouped_outliers(A.data_ptr(), A16.data_ptr(), CA.data_ptr(), CB.data_ptr(),
+                                                     SCB.data_ptr(), offs.data_ptr(), E, float(threshold),
+                                                     ends.data_ptr(), flags.data_ptr(), cols.data_ptr(),
+                                                     count.data_ptr(), subA.data_ptr(), subBT.data_ptr(), M, N, K,
+                                                     dtype, stream)
+            lib.check("int8_grouped_mm")
+            if rc != 0:
+                raise RuntimeError(f"int8_grouped_mm: the library refused the outlier preparation (code {rc})")
+            outl = [t.data_ptr() for t in (A, subA, subBT, cols, count)]
+        rc = lib.cbnb_b200_int8_grouped_mm(CA.data_ptr(), CB.data_ptr(), SCA.data_ptr(), SCB.data_ptr(),
+                                           bias.data_ptr() if bias is not None else None, offs.data_ptr(), E, *outl,
+                                           out.data_ptr(), M, N, K, dtype, stream)
+    lib.check("int8_grouped_mm")
+    if rc != 0:
+        raise RuntimeError(f"int8_grouped_mm: the library does not serve this call (code {rc}): A={tuple(A.shape)} "
+                           f"CB={tuple(CB.shape)}")
     return out
 
 

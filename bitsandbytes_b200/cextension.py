@@ -110,6 +110,11 @@ def _signatures():
     sig["cbnb_b200_int8_outlier_prep_dev"] = ([_VOIDP] * 6 + [_I32] * 4 + [_VOIDP] * 3, None)
     # (CA, CB, SCA, SCB, bias, A, subA, subBT, cols, count, out, M, N, K, dtype, stream) -> int
     sig["cbnb_b200_int8_mixed_mm_dev"] = ([_VOIDP] * 11 + [_I32] * 4 + [_VOIDP], _I32)
+    # (A, A16, CA, CB, SCB, offs, E, threshold, ends, flags, cols, count, subA, subBT, M, N, K, dtype, stream) -> int
+    sig["cbnb_b200_int8_grouped_outliers"] = ([_VOIDP] * 6 + [_I32, ct.c_float] + [_VOIDP] * 6 + [_I32] * 4 + [_VOIDP],
+                                              _I32)
+    # (CA, CB, SCA, SCB, bias, offs, E, A, subA, subBT, cols, count, out, M, N, K, dtype, stream) -> int
+    sig["cbnb_b200_int8_grouped_mm"] = ([_VOIDP] * 6 + [_I32] + [_VOIDP] * 6 + [_I32] * 4 + [_VOIDP], _I32)
     # (A, out, rowStats, col_flags, threshold, rows, cols, dtype, stream)
     sig["cbnb_b200_int8_vector_quant_flags"] = ([_VOIDP] * 4 + [ct.c_float] + [_I32] * 3 + [_VOIDP], None)
     # (A, rowStats, col_flags, threshold, rows, cols, dtype, stream) -> int

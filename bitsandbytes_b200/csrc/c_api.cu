@@ -135,6 +135,13 @@ void launch_int8_outlier_prep_dev(const void* A, int8_t* CA, const int8_t* CB, c
                                   const int* count, int cap, int M, int N, int K, int dtype, void* subA, void* subBT,
                                   cudaStream_t stream);
 void launch_int8_outlier_compact(const int* col_flags, int K, int* cols, int* count, cudaStream_t stream);
+void launch_int8_grouped_outliers(const void* A, const void* A16, int8_t* CA, const int8_t* CB, const float* SCB,
+                                  const int* offs, int E, float threshold, int* ends, int* flags, int* cols, int* count,
+                                  void* subA, void* subBT, int M, int N, int K, int dtype, cudaStream_t stream);
+int launch_int8_gemm_grouped(const int8_t* CA, const int8_t* CB, void* out, const float* SCA, const float* SCB,
+                             const void* bias, const int* offs, int E, int M, int N, int K, int epi, const void* A,
+                             const void* subA, const void* subBT, const int* cols, const int* count,
+                             cudaStream_t stream);
 void launch_int8_zero_columns(int8_t* CA, const long long* cols, int J, int rows, int K, cudaStream_t stream);
 bool launch_int8_col_quant(const void* A, int8_t* out, float* col_stats, float threshold, int rows, int cols, int dtype,
                            cudaStream_t stream);
@@ -862,6 +869,54 @@ int cbnb_b200_int8_mixed_mm_dev(const int8_t* CA, const int8_t* CB, const float*
                                 void* out, int M, int N, int K, int dtype, cudaStream_t stream) {
     if (dtype != 1 && dtype != 2) return 100;
     return launch_int8_gemm(CA, CB, out, SCA, SCB, bias, M, N, K, N, dtype, stream, subA, subBT, 64, count, cols, A);
+}
+
+// ---------------------------------------------------------------- grouped LLM.int8() (mixture-of-experts layers)
+// The per-expert outliers of cbnb_b200_int8_grouped_mm, on the device: ends[E] (the clamped end rows), flags[E, K] (the
+// columns where a row of expert e of A16, the fp16 activations, has |a| >= threshold), cols[E, K] / count[E] (each
+// expert's ascending list), subA [M, 64] (each row's own expert's first 64 outlier columns of A), subBT [E * N, 64]
+// (each routed expert's dequantised weight columns), and CA zeroed in each row's expert's outlier columns when the
+// expert has more than one row.  Nothing depends on the data but the values written.  Returns 0, or 1 with the error
+// message set for bad arguments.
+int cbnb_b200_int8_grouped_outliers(const void* A, const void* A16, int8_t* CA, const int8_t* CB, const float* SCB,
+                                    const int* offs, int E, float threshold, int* ends, int* flags, int* cols,
+                                    int* count, void* subA, void* subBT, int M, int N, int K, int dtype,
+                                    cudaStream_t stream) {
+    if (A == nullptr || A16 == nullptr || CA == nullptr || CB == nullptr || SCB == nullptr || offs == nullptr ||
+        ends == nullptr || flags == nullptr || cols == nullptr || count == nullptr || subA == nullptr ||
+        subBT == nullptr || E < 1 || E > kMaxExperts || M < 0 || N <= 0 || K <= 0 || !(threshold > 0.f) ||
+        (dtype != 1 && dtype != 2)) {
+        set_last_error_msg("int8_grouped_outliers: needs every operand, 1 <= E <= 1024, M >= 0, N, K >= 1, "
+                           "threshold > 0 and dtype 1 (fp16) or 2 (bf16)");
+        return 1;
+    }
+    launch_int8_grouped_outliers(A, A16, CA, CB, SCB, offs, E, threshold, ends, flags, cols, count, subA, subBT, M, N,
+                                 K, dtype, stream);
+    return 0;
+}
+
+// The grouped LLM.int8() GEMM of a mixture-of-experts layer (no reference counterpart): out[m, :] (row stride N) = the
+// epilogue of cbnb_b200_int8_scaled_mm (count NULL) or cbnb_b200_int8_mixed_mm_dev (count from
+// cbnb_b200_int8_grouped_outliers) with expert e's weights CB[e * N ..], SCB[e * N ..], bias[e * N ..] for the rows of
+// expert e, end_{e-1} <= m < end_e, and +0 for the rows past end_{E-1}; offs[E] (int32, on the device) holds the end
+// rows, clamped on the device as end_e = min(max(offs[e], end_{e-1}), M).  Each expert's rows are bit for bit what
+// those entries give on that expert's rows alone.  Returns 0; 1 with the error message set for bad arguments; 100, with
+// nothing written and no message, for what the kernel does not serve (K % 16 != 0, E > 1024, unaligned codes); 100
+// with the error message set when the launch fails.
+int cbnb_b200_int8_grouped_mm(const int8_t* CA, const int8_t* CB, const float* SCA, const float* SCB, const void* bias,
+                              const int* offs, int E, const void* A, const void* subA, const void* subBT,
+                              const int* cols, const int* count, void* out, int M, int N, int K, int dtype,
+                              cudaStream_t stream) {
+    if (CA == nullptr || CB == nullptr || SCA == nullptr || SCB == nullptr || offs == nullptr || out == nullptr ||
+        M < 0 || N <= 0 || K <= 0 || E < 1 || (dtype != 1 && dtype != 2)) {
+        set_last_error_msg("int8_grouped_mm: needs CA, CB, SCA, SCB, offs and out, M >= 0, N, K >= 1, E >= 1 and "
+                           "dtype 1 (fp16) or 2 (bf16)");
+        return 1;
+    }
+    const int rc =
+        launch_int8_gemm_grouped(CA, CB, out, SCA, SCB, bias, offs, E, M, N, K, dtype, A, subA, subBT, cols, count,
+                                 stream);
+    return rc == 0 ? 0 : 100;
 }
 
 // Column-wise absmax + int8 codes of A[rows, cols] (the column half of the reference's int8_double_quant,

@@ -230,8 +230,8 @@ __global__ void __launch_bounds__(256)
 // One CTA walks the flags in tiles of 1024 columns: a ballot per warp counts and ranks the flagged columns of the warp,
 // and the counts of the warps before it place them.
 constexpr int kCompactThreads = 1024;
-__global__ void __launch_bounds__(kCompactThreads)
-    int8_outlier_compact_kernel(const int* __restrict__ flags, int K, int* __restrict__ cols, int* __restrict__ count) {
+__device__ __forceinline__ void outlier_compact(const int* __restrict__ flags, int K, int* __restrict__ cols,
+                                                int* __restrict__ count) {
     __shared__ int s_warp[kCompactThreads / 32];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     int base = 0;
@@ -253,6 +253,122 @@ __global__ void __launch_bounds__(kCompactThreads)
         __syncthreads();  // s_warp is rewritten by the next tile
     }
     if (threadIdx.x == 0) *count = base;
+}
+
+__global__ void __launch_bounds__(kCompactThreads)
+    int8_outlier_compact_kernel(const int* __restrict__ flags, int K, int* __restrict__ cols, int* __restrict__ count) {
+    outlier_compact(flags, K, cols, count);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// The grouped (mixture-of-experts) route: each expert's outlier columns are those where one of ITS rows has
+// |a| >= threshold, as a Linear8bitLt call on that expert's rows alone finds them.  The row codes and statistics do not
+// depend on the expert (int8_vector_quant_kernel gives them); the flags, the column lists and the operands do.
+// end_e = min(max(offs[e], end_{e-1}), M), end_{-1} = 0: the grouped GEMMs' clamp of the expert ends, one thread per expert.
+constexpr int kEndsThreads = 1024;
+static_assert(kMaxExperts <= kEndsThreads, "one thread per expert");
+__global__ void __launch_bounds__(kEndsThreads)
+    int8_group_ends_kernel(const int* __restrict__ offs, int E, int M, int* __restrict__ ends) {
+    __shared__ int s_warp[kEndsThreads / 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int v = threadIdx.x < E ? max(offs[threadIdx.x], 0) : 0;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const int o = __shfl_up_sync(0xffffffffu, v, d);
+        if (lane >= d) v = max(v, o);
+    }
+    if (lane == 31) s_warp[warp] = v;
+    __syncthreads();
+    for (int w = 0; w < warp; ++w) v = max(v, s_warp[w]);
+    if (threadIdx.x < E) ends[threadIdx.x] = min(v, M);
+}
+
+// the expert of row m < ends[E - 1]: the first e with ends[e] > m
+__device__ __forceinline__ int expert_of_row(const int* __restrict__ ends, int E, int m) {
+    int lo = 0, hi = E - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (__ldg(ends + mid) > m) hi = mid;
+        else lo = mid + 1;
+    }
+    return lo;
+}
+
+// flags[e, c] = 1 where a row of expert e has |A16[m, c]| >= thr (A16: the activations as fp16, as LLM.int8() quantises
+// them; the comparison of int8_vector_quant_kernel's flags).  One CTA per row; rows past end_{E-1} flag nothing.
+__global__ void __launch_bounds__(256)
+    int8_grouped_flags_kernel(const __half* __restrict__ A16, const int* __restrict__ ends, int E, int K, float thr,
+                              int* __restrict__ flags) {
+    const int m = blockIdx.x;
+    if (m >= __ldg(ends + E - 1)) return;
+    const __half* a = A16 + (long long)m * K;
+    int* f = flags + (long long)expert_of_row(ends, E, m) * K;
+    for (int c = threadIdx.x; c < K; c += 256)
+        if (fabsf(__half2float(a[c])) >= thr) f[c] = 1;
+}
+
+// each expert's flags -> its ascending column list cols[e, :count[e]], one CTA per expert
+__global__ void __launch_bounds__(kCompactThreads)
+    int8_outlier_compact_grouped_kernel(const int* __restrict__ flags, int K, int* __restrict__ cols,
+                                        int* __restrict__ count) {
+    const long long off = (long long)blockIdx.x * K;
+    outlier_compact(flags + off, K, cols + off, count + blockIdx.x);
+}
+
+// The operands of the grouped GEMM's outlier term, one warp per row of [subA rows M | subBT rows E * N]:
+//   subA[m, j]  = A[m, cols_e[j]] for the first min(count_e, 64) columns of row m's expert e, zero-padded to 64 (rows
+//                 past end_{E-1}: zeros), and CA[m, cols_e[j]] = 0 for all count_e of them when the expert has more than
+//                 one row (int8_vectorwise_quant's rows > 1 rule: a single row's outliers are zero codes already);
+//   subBT[e * N + n, j] = T((float(CB[e * N + n, cols_e[j]]) * SCB[e * N + n]) * (1/127)) for the first
+//                 min(count_e, 64) columns, zero-padded to a multiple of 8 -- the columns the GEMM reads -- and written
+//                 only for experts with rows and outliers.
+// The grid depends on the shapes only.
+constexpr int kOutlierCap = 64;
+template <typename T>
+__global__ void __launch_bounds__(256)
+    int8_grouped_outlier_prep_kernel(const T* __restrict__ A, int8_t* __restrict__ CA, const int8_t* __restrict__ CB,
+                                     const float* __restrict__ SCB, const int* __restrict__ ends,
+                                     const int* __restrict__ cols, const int* __restrict__ count, int E, int M, int N,
+                                     int K, T* __restrict__ subA, T* __restrict__ subBT) {
+    const int lane = threadIdx.x & 31;
+    const long long rows = (long long)M + (long long)E * N;
+    const int m_tail = __ldg(ends + E - 1);
+    for (long long r = ((long long)blockIdx.x * 256 + threadIdx.x) >> 5; r < rows; r += ((long long)gridDim.x * 256) >> 5) {
+        if (r < M) {
+            T* sa = subA + r * kOutlierCap;
+            if (r >= m_tail) {
+                sa[lane] = DT<T>::from_f32(0.f);
+                sa[lane + 32] = DT<T>::from_f32(0.f);
+                continue;
+            }
+            const int e = expert_of_row(ends, E, (int)r);
+            const int all = __ldg(count + e);
+            const int J = min(all, kOutlierCap);
+            const int* ce = cols + (long long)e * K;
+            const T* a = A + r * K;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int j = lane + 32 * h;
+                sa[j] = j < J ? a[__ldg(ce + j)] : DT<T>::from_f32(0.f);
+            }
+            const int rows_e = __ldg(ends + e) - (e > 0 ? __ldg(ends + e - 1) : 0);
+            if (rows_e > 1)
+                for (int j = lane; j < all; j += 32) CA[r * K + __ldg(ce + j)] = 0;
+        } else {
+            const long long w = r - M;
+            const int e = (int)(w / N);
+            if (__ldg(ends + e) == (e > 0 ? __ldg(ends + e - 1) : 0)) continue;  // no rows: never read
+            const int J = min(__ldg(count + e), kOutlierCap);
+            const int jpad = (J + 7) & ~7;
+            const int* ce = cols + (long long)e * K;
+            const float scb = __ldg(SCB + w);
+            for (int j = lane; j < jpad; j += 32) {
+                float v = 0.f;
+                if (j < J) v = __fmul_rn(__fmul_rn((float)CB[w * K + __ldg(ce + j)], scb), 7.874015718698502e-3f);
+                subBT[w * kOutlierCap + j] = DT<T>::from_f32(v);
+            }
+        }
+    }
 }
 
 // CA[:, cols[j]] = 0 for every outlier column (reference backends/cuda/ops.py:233-236, a torch index_put there)
@@ -439,6 +555,30 @@ void launch_int8_outlier_prep_dev(const void* A, int8_t* CA, const int8_t* CB, c
 void launch_int8_outlier_compact(const int* col_flags, int K, int* cols, int* count, cudaStream_t stream) {
     int8_outlier_compact_kernel<<<1, kCompactThreads, 0, stream>>>(col_flags, K, cols, count);
     BNB200_CHECK_LAUNCH("int8_outlier_compact");
+}
+
+// The per-expert outliers of the grouped int8 GEMM (launch_int8_gemm_grouped), in four launches whose grids depend on
+// the shapes only: the clamped ends[E] of offs, flags[E, K] from A16 (the fp16 activations), each expert's column list
+// cols[E, K] and count[E], then subA [M, 64], subBT [E * N, 64] and CA's zeroed outlier columns.  A is T[M, K] (dtype
+// 1 fp16, 2 bf16).
+void launch_int8_grouped_outliers(const void* A, const void* A16, int8_t* CA, const int8_t* CB, const float* SCB,
+                                  const int* offs, int E, float threshold, int* ends, int* flags, int* cols, int* count,
+                                  void* subA, void* subBT, int M, int N, int K, int dtype, cudaStream_t stream) {
+    int8_group_ends_kernel<<<1, kEndsThreads, 0, stream>>>(offs, E, M, ends);
+    cudaMemsetAsync(flags, 0, sizeof(int) * (size_t)E * K, stream);
+    if (M > 0) int8_grouped_flags_kernel<<<M, 256, 0, stream>>>((const __half*)A16, ends, E, K, threshold, flags);
+    int8_outlier_compact_grouped_kernel<<<E, kCompactThreads, 0, stream>>>(flags, K, cols, count);
+    const long long warps = (long long)M + (long long)E * N;
+    const long long want = (warps + 7) / 8;
+    const int grid = (int)(want < 132 * 16 ? want : 132 * 16);
+    if (dtype == 1)
+        int8_grouped_outlier_prep_kernel<__half><<<grid, 256, 0, stream>>>(
+            (const __half*)A, CA, CB, SCB, ends, cols, count, E, M, N, K, (__half*)subA, (__half*)subBT);
+    else
+        int8_grouped_outlier_prep_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(
+            (const __nv_bfloat16*)A, CA, CB, SCB, ends, cols, count, E, M, N, K, (__nv_bfloat16*)subA,
+            (__nv_bfloat16*)subBT);
+    BNB200_CHECK_LAUNCH("int8_grouped_outliers");
 }
 
 // q_col[rows, cols] + col_stats[cols] of A[rows, cols]; dtype: 1 fp16, 2 bf16 (false: dtype not served)

@@ -71,7 +71,112 @@ struct I8MultiParams : I8Params {
     // m % rows_per_out (scatter_row: each rank of a sequence-parallel layer receives its own tokens' partials)
     int rows_per_out;
 };
-template <bool kMulti> using I8ParamsOf = typename std::conditional<kMulti, I8MultiParams, I8Params>::type;
+// the parameters of a kGrouped instance: every expert of a mixture-of-experts layer in one launch.  CB / SCB / bias are
+// the E experts' [N, K] weights stacked ([E * N, K], [E * N], [E * N]); offs[E] the expert end rows, clamped on the
+// device; jcount / cols (kDevJ) the per-expert outlier counts [E] and ascending lists [E, K], subBT [E * N, JMAX]
+struct I8GroupedParams : I8Params {
+    const int* offs;
+    int E;
+};
+template <bool kMulti, bool kGrouped = false>
+using I8ParamsOf = typename std::conditional<
+    kMulti, I8MultiParams, typename std::conditional<kGrouped, I8GroupedParams, I8Params>::type>::type;
+
+// kGrouped: the group table past the outlier operands' shared memory: gend[e] = end_e, gtp[e] = the 128-row m-tiles of
+// experts 0..e-1 (gtp[E] = all of them), then the scan's per-warp totals
+constexpr int kI8Warps = kI8Threads / 32;
+constexpr int kI8GroupTabBytes = (2 * kMaxExperts + 1 + 2 * kI8Warps) * 4;
+
+// kGrouped: the group table, built by the whole CTA (every CTA builds the same one).  Thread t takes experts
+// [t * kPer, t * kPer + kPer): end_e = min(M, max(0, offs[0..e])) -- the clamp of the 4-bit grouped GEMM, as a prefix
+// maximum -- then the m-tile counts ceil((end_e - end_{e-1}) / 128) and their exclusive prefix sum, each scan over the
+// warp by shuffles and across the warps through shared memory.  Ends with a __syncthreads.
+__device__ __forceinline__ void i8_group_table(const int* __restrict__ offs, int E, int M, int* gend) {
+    constexpr int kPer = (kMaxExperts + kI8Threads - 1) / kI8Threads;
+    static_assert(kMaxExperts <= (kI8Threads - 1) * kPer, "the last thread must hold no expert");
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int* gtp = gend + kMaxExperts;
+    int* wtot = gtp + kMaxExperts + 1;  // [kI8Warps] maxima, then [kI8Warps] tile counts
+    const int e0 = threadIdx.x * kPer;
+    int v[kPer];
+    int run = 0;
+#pragma unroll
+    for (int i = 0; i < kPer; ++i) {
+        v[i] = e0 + i < E ? max(__ldg(offs + e0 + i), 0) : 0;
+        run = max(run, v[i]);
+    }
+    int inc = run;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const int o = __shfl_up_sync(0xffffffffu, inc, d);
+        if (lane >= d) inc = max(inc, o);
+    }
+    if (lane == 31) wtot[warp] = inc;
+    __syncthreads();
+    int r = __shfl_up_sync(0xffffffffu, inc, 1);
+    if (lane == 0) r = 0;
+    for (int w2 = 0; w2 < warp; ++w2) r = max(r, wtot[w2]);
+    int prev = min(r, M);
+    int cnt[kPer], tiles = 0;
+#pragma unroll
+    for (int i = 0; i < kPer; ++i) {
+        r = max(r, v[i]);
+        v[i] = min(r, M);  // end_e (experts past E: end_{E-1}, no rows)
+        cnt[i] = (v[i] - prev + kI8TileM - 1) / kI8TileM;
+        prev = v[i];
+        tiles += cnt[i];
+    }
+    int incs = tiles;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const int o = __shfl_up_sync(0xffffffffu, incs, d);
+        if (lane >= d) incs += o;
+    }
+    if (lane == 31) wtot[kI8Warps + warp] = incs;
+    __syncthreads();
+    int base = incs - tiles;
+    for (int w2 = 0; w2 < warp; ++w2) base += wtot[kI8Warps + w2];
+#pragma unroll
+    for (int i = 0; i < kPer; ++i) {
+        if (e0 + i < E) {
+            gend[e0 + i] = v[i];
+            gtp[e0 + i] = base;
+        }
+        base += cnt[i];
+    }
+    if (threadIdx.x == kI8Threads - 1) gtp[E] = base;  // the last thread's experts are past E: base is the total
+    __syncthreads();
+}
+
+// kGrouped: the unit's expert e (the last e with gtp[e] <= g for the CTA's m-tile g, which has m-tiles since g < gtp[E]),
+// its first row m0, its end row and its first row of the stacked weights.  Looked up where each role needs it, through
+// volatile reads, rather than held across the main loop: held, the values cost the device-count instances more spills.
+struct I8Unit {
+    int e, m0, m_end, wrow;
+};
+__device__ __forceinline__ I8Unit i8_unit(const int* gend_, int E, int N, int n_tiles) {
+    const volatile int* gend = gend_;
+    const volatile int* gtp = gend_ + kMaxExperts;
+    const int g = blockIdx.x / n_tiles;
+    int lo = 0;
+#pragma unroll
+    for (int step = kMaxExperts / 2; step >= 1; step >>= 1)
+        if (lo + step < E && gtp[lo + step] <= g) lo += step;
+    I8Unit u;
+    u.e = lo;
+    u.m0 = (lo > 0 ? gend[lo - 1] : 0) + (g - gtp[lo]) * kI8TileM;
+    u.m_end = gend[lo];
+    u.wrow = lo * N;
+    return u;
+}
+
+// kGrouped: rows [end_{E-1}, M) belong to no expert: +0, each CTA's 256 consumer threads storing a strided share
+__device__ __forceinline__ void i8_zero_tail(uint16_t* out, int m_tail, int M, int N, int ldc) {
+    const long long n_tail = (long long)(M - m_tail) * N;
+    for (long long i = (long long)blockIdx.x * kI8Consumers + threadIdx.x; i < n_tail;
+         i += (long long)gridDim.x * kI8Consumers)
+        out[(m_tail + i / N) * ldc + i % N] = 0;
+}
 
 // JMAX: capacity of the fused outlier term (0 = none): subA of the CTA's 128 tokens and subBT of its 128 features
 // are staged in shared memory after the main loop.
@@ -80,10 +185,16 @@ template <bool kMulti> using I8ParamsOf = typename std::conditional<kMulti, I8Mu
 // continue the same fp32 sum in column order.
 // kMulti: every output element goes to each of p.outs[0 .. p.n_outs) (a local buffer and the peers' mapped buffers of a
 // tensor-parallel layer) instead of p.out; the values are those of the single-destination instance.
-template <int EPI, int JMAX, bool kDevJ = false, bool kMulti = false>
+// kGrouped: every expert of a mixture-of-experts layer in one launch (I8GroupedParams).  A unit is a 128-row m-tile of
+// one expert and a 128-feature n-tile; blockIdx.x runs the units in (m-tile, n-tile) order, and the CTAs past the
+// device-known unit count only zero the tail rows.  Expert e's j-th m-tile starts at row end_{e-1} + 128 j; rows of it
+// past end_e are the next expert's, computed with the wrong weights and not stored.  Every stored element is the one the
+// plain (kDevJ) instance gives on that expert's rows alone.
+template <int EPI, int JMAX, bool kDevJ = false, bool kMulti = false, bool kGrouped = false>
 __global__ void __launch_bounds__(kI8Threads, 1)
     int8_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                        const I8ParamsOf<kMulti> p) {
+                        const I8ParamsOf<kMulti, kGrouped> p) {
+    static_assert(!(kGrouped && kMulti), "the grouped instances have one destination");
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     constexpr int kStages = I8Cfg<JMAX>::kStages;
@@ -97,7 +208,9 @@ __global__ void __launch_bounds__(kI8Threads, 1)
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     const int n0 = (blockIdx.x % p.n_tiles) * kI8TileN;
-    const int m0 = (blockIdx.x / p.n_tiles) * kI8TileM;
+    int m0 = (blockIdx.x / p.n_tiles) * kI8TileM;
+    // kGrouped: the unit's expert, its end row and its first row of the stacked weights (e * N)
+    int ge = 0, m_end = p.M, wrow = 0;
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < kStages; ++s) {
@@ -106,10 +219,24 @@ __global__ void __launch_bounds__(kI8Threads, 1)
         }
         ptx::fence_barrier_init();
     }
+    if constexpr (kGrouped) {
+        int* gend = reinterpret_cast<int*>(s_subb + kI8TileN * (JMAX / 8));
+        const int* gtp = gend + kMaxExperts;
+        i8_group_table(p.offs, p.E, p.M, gend);
+        if (blockIdx.x / p.n_tiles >= gtp[p.E]) {  // past the units
+            if (threadIdx.x < kI8Consumers) i8_zero_tail(reinterpret_cast<uint16_t*>(p.out), gend[p.E - 1], p.M, p.N, p.ldc);
+            return;
+        }
+    }
     __syncthreads();
 
     if (warp == kI8Consumers / 32) {
         // ================================================================== TMA producer
+        if constexpr (kGrouped) {
+            const I8Unit u = i8_unit(reinterpret_cast<const int*>(s_subb + kI8TileN * (JMAX / 8)), p.E, p.N, p.n_tiles);
+            m0 = u.m0;
+            wrow = u.wrow;
+        }
         if (ptx::elect_one()) {
             ptx::prefetch_tmap(&tmap_a);
             ptx::prefetch_tmap(&tmap_b);
@@ -120,7 +247,9 @@ __global__ void __launch_bounds__(kI8Threads, 1)
                 ptx::mbar_arrive_expect_tx(&full[s], kI8StageBytes);
                 // (rows past M / N and k columns past K are out of bounds for the tensor maps: TMA zero-fills them)
                 ptx::tma_load_2d(sa, &tmap_a, &full[s], i * kI8BK, m0);
-                ptx::tma_load_2d(sa + kI8TileM * kI8BK, &tmap_b, &full[s], i * kI8BK, n0);
+                // (kGrouped: rows of the expert's stacked weights; a tile reaching past its N features loads the next
+                // expert's rows, whose results are not stored)
+                ptx::tma_load_2d(sa + kI8TileM * kI8BK, &tmap_b, &full[s], i * kI8BK, wrow + n0);
             }
         }
         return;
@@ -154,6 +283,13 @@ __global__ void __launch_bounds__(kI8Threads, 1)
     ptx::wgmma_wait<0>();
 #pragma unroll
     for (int j = 0; j < 64; ++j) ptx::fence_operand(acc[j]);
+    if constexpr (kGrouped) {
+        const I8Unit u = i8_unit(reinterpret_cast<const int*>(s_subb + kI8TileN * (JMAX / 8)), p.E, p.N, p.n_tiles);
+        ge = u.e;
+        m0 = u.m0;
+        m_end = u.m_end;
+        wrow = u.wrow;
+    }
 
     // ====================================================================== epilogue
     // acc[4j + e]: token row rl + 8 * (e >= 2), feature column 8j + 2t + (e & 1)
@@ -162,7 +298,8 @@ __global__ void __launch_bounds__(kI8Threads, 1)
     float olr[kDevJ ? 64 : 1];   // kDevJ: the outlier term of this thread's outputs, (h, j, u) at 32 h + 2 j + u
     if constexpr (kDevJ) {
         static_assert(JMAX == 64, "the device-count instance stages 64 columns at a time");
-        J = __ldg(p.jcount);
+        J = __ldg(p.jcount + ge);  // (kGrouped: the unit's expert's count and list)
+        const int* cols = p.cols + (long long)ge * p.K;
 #pragma unroll
         for (int i = 0; i < 64; ++i) olr[i] = 0.f;
         // thread e stages row e & 127 of one of the two operands, as below
@@ -171,13 +308,14 @@ __global__ void __launch_bounds__(kI8Threads, 1)
         const bool is_b = e >= 128;
         const int gr = (is_b ? n0 : m0) + r;
         const bool ok = gr < (is_b ? p.N : p.M);
+        const int grow = gr + (is_b ? wrow : 0);  // the row of subBT / SCB / CB (kGrouped: of the stacked weights)
         uint4* dst = (is_b ? s_subb : s_suba) + r * (JMAX / 8);
         for (int c0 = 0; c0 < J; c0 += JMAX) {
             const int jc = min(J - c0, JMAX);
             const int jpad = (jc + 7) & ~7;
             if (c0 == 0) {
                 const uint16_t* src =
-                    reinterpret_cast<const uint16_t*>(is_b ? p.subBT : p.subA) + (long long)(ok ? gr : 0) * JMAX;
+                    reinterpret_cast<const uint16_t*>(is_b ? p.subBT : p.subA) + (long long)(ok ? grow : 0) * JMAX;
 #pragma unroll
                 for (int q = 0; q < JMAX / 8; ++q)
                     dst[q] = (ok && 8 * q < jpad) ? __ldg(reinterpret_cast<const uint4*>(src) + q) : make_uint4(0, 0, 0, 0);
@@ -185,14 +323,14 @@ __global__ void __launch_bounds__(kI8Threads, 1)
                 asm volatile("bar.sync 1, 256;" ::: "memory");  // every consumer is done with the previous chunk
                 // subA[m, j] = A[m, cols[j]]; subBT[n, j] = T((float(CB[n, cols[j]]) * SCB[n]) * (1/127)), as the prep
                 // kernel builds them
-                const float scb = ok && is_b ? __ldg(p.SCB + gr) : 0.f;
+                const float scb = ok && is_b ? __ldg(p.SCB + grow) : 0.f;
                 for (int q = 0; q < JMAX / 8; ++q) {
                     uint32_t w[4] = {0u, 0u, 0u, 0u};
 #pragma unroll
                     for (int x = 0; x < 8; ++x) {
                         const int jj = 8 * q + x;
                         if (ok && jj < jc) {
-                            const long long at = (long long)gr * p.K + __ldg(p.cols + c0 + jj);
+                            const long long at = (long long)grow * p.K + __ldg(cols + c0 + jj);
                             uint32_t bits;
                             if (is_b) {
                                 const float v = __fmul_rn(__fmul_rn((float)p.CB[at], scb), 7.874015718698502e-3f);
@@ -251,7 +389,7 @@ __global__ void __launch_bounds__(kI8Threads, 1)
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
         const int m = m0 + rl + 8 * h;
-        if (m >= p.M) continue;
+        if (m >= m_end) continue;  // (kGrouped: rows past the expert's end are the next expert's)
         float sca = 0.f;
         if (EPI != 0) sca = __ldg(p.SCA + m);
         // scattered rows: row m's one destination, found once for the column loop (a 128-token tile may span ranks)
@@ -318,11 +456,11 @@ __global__ void __launch_bounds__(kI8Threads, 1)
             for (int u = 0; u < 2; ++u) {
                 const int nn = n + u;
                 const int v = u ? v1 : v0;
-                const float scb = nn < p.N ? __ldg(p.SCB + nn) : 0.f;
+                const float scb = nn < p.N ? __ldg(p.SCB + wrow + nn) : 0.f;
                 float b = 0.f;
                 if (p.bias != nullptr && nn < p.N) {
-                    if (EPI == 1) b = __half2float(reinterpret_cast<const __half*>(p.bias)[nn]);
-                    else b = __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p.bias)[nn]);
+                    if (EPI == 1) b = __half2float(reinterpret_cast<const __half*>(p.bias)[wrow + nn]);
+                    else b = __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p.bias)[wrow + nn]);
                 }
                 f[u] = int8_epilogue_value<EPI>(v, sca, scb, b, p.bias != nullptr, add_ol, ol[u]);
             }
@@ -349,16 +487,21 @@ __global__ void __launch_bounds__(kI8Threads, 1)
             }
         }
     }
+    if constexpr (kGrouped) {
+        const int* gend = reinterpret_cast<const int*>(s_subb + kI8TileN * (JMAX / 8));
+        i8_zero_tail(reinterpret_cast<uint16_t*>(p.out), gend[p.E - 1], p.M, p.N, p.ldc);
+    }
 }
 
-template <int EPI, int JMAX = 0, bool kDevJ = false, bool kMulti = false>
-int launch_i8(const CUtensorMap& ta, const CUtensorMap& tb, I8ParamsOf<kMulti>& p, cudaStream_t stream) {
-    constexpr size_t smem_bytes =
-        1024 + size_t(I8Cfg<JMAX>::kStages) * kI8StageBytes + 256 + size_t(kI8TileM + kI8TileN) * JMAX * 2;
+template <int EPI, int JMAX = 0, bool kDevJ = false, bool kMulti = false, bool kGrouped = false>
+int launch_i8(const CUtensorMap& ta, const CUtensorMap& tb, I8ParamsOf<kMulti, kGrouped>& p, cudaStream_t stream) {
+    constexpr size_t smem_bytes = 1024 + size_t(I8Cfg<JMAX>::kStages) * kI8StageBytes + 256 +
+                                  size_t(kI8TileM + kI8TileN) * JMAX * 2 + (kGrouped ? kI8GroupTabBytes : 0);
+    static_assert(smem_bytes <= 227 * 1024, "shared memory");
     static bool attr_set[64] = {};  // the shared-memory opt-in is per device
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 1;
-    auto kern = int8_gemm_tc_kernel<EPI, JMAX, kDevJ, kMulti>;
+    auto kern = int8_gemm_tc_kernel<EPI, JMAX, kDevJ, kMulti, kGrouped>;
     p.kblocks = (p.K + kI8BK - 1) / kI8BK;
     if (!attr_set[dev]) {
         if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes) != cudaSuccess) {
@@ -368,7 +511,10 @@ int launch_i8(const CUtensorMap& ta, const CUtensorMap& tb, I8ParamsOf<kMulti>& 
         attr_set[dev] = true;
     }
     p.n_tiles = (p.N + kI8TileN - 1) / kI8TileN;
-    const int m_tiles = (p.M + kI8TileM - 1) / kI8TileM;
+    // kGrouped: the m-tiles are counted on the device; each expert adds at most one partial tile, so ceil(M / 128) + E
+    // bounds them and sizes the grid
+    int m_tiles = (p.M + kI8TileM - 1) / kI8TileM;
+    if constexpr (kGrouped) m_tiles += p.E;
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(p.n_tiles * m_tiles, 1, 1);
     cfg.blockDim = dim3(kI8Threads);
@@ -466,6 +612,55 @@ int launch_int8_gemm(const int8_t* acts, const int8_t* weights, void* out, const
     case 1: return launch_i8<1>(ta, tb, p, stream);
     default: return launch_i8<2>(ta, tb, p, stream);
     }
+}
+
+// The grouped int8 GEMM of a mixture-of-experts layer (epi 1 fp16 / 2 bf16): out[m, n] (row stride N) = the fused
+// epilogue of launch_int8_gemm with SCB / bias at e * N + n for the rows of expert e, end_{e-1} <= m < end_e, and +0 for
+// the rows past end_{E-1}.  CB [E * N, K] and SCB [E * N] are the experts' weights stacked; offs[E] the end rows
+// (int32, on the device), clamped as end_e = min(max(offs[e], end_{e-1}), M).  With count set (the outlier term): count[E]
+// and cols[E, K] the per-expert outlier counts and ascending lists, subA [M, 64] each row's own expert's first 64
+// outlier columns, subBT [E * N, 64] each expert's dequantised weight columns, A [M, K] the activations for the columns
+// past 64.  Returns 0, or 100 with nothing launched for what the instances do not serve; a failed launch returns 1 with
+// the error message set.
+int launch_int8_gemm_grouped(const int8_t* CA, const int8_t* CB, void* out, const float* SCA, const float* SCB,
+                             const void* bias, const int* offs, int E, int M, int N, int K, int epi, const void* A,
+                             const void* subA, const void* subBT, const int* cols, const int* count,
+                             cudaStream_t stream) {
+    if (epi != 1 && epi != 2) return 100;
+    if (E < 1 || E > kMaxExperts || N <= 0 || (long long)E * N > 0x7fffffffLL || K <= 0 || (K % 16) != 0) return 100;
+    if (count != nullptr && (cols == nullptr || A == nullptr || subA == nullptr || subBT == nullptr ||
+                             (reinterpret_cast<uintptr_t>(subA) & 15) != 0 ||
+                             (reinterpret_cast<uintptr_t>(subBT) & 15) != 0))
+        return 100;
+    if ((reinterpret_cast<uintptr_t>(CA) & 15) != 0 || (reinterpret_cast<uintptr_t>(CB) & 15) != 0) return 100;
+    if (M <= 0) return 0;
+    CUtensorMap ta, tb;
+    if (!encode_tmap_2d(&ta, CA, 1, 128, (uint64_t)M, (uint64_t)K, (uint64_t)K, kI8TileM, kI8BK)) return 100;
+    if (!encode_tmap_2d(&tb, CB, 1, 128, (uint64_t)E * N, (uint64_t)K, (uint64_t)K, kI8TileN, kI8BK)) return 100;
+    I8GroupedParams p{};
+    p.out = out;
+    p.SCA = SCA;
+    p.SCB = SCB;
+    p.bias = bias;
+    p.M = M;
+    p.N = N;
+    p.K = K;
+    p.ldc = N;
+    p.offs = offs;
+    p.E = E;
+    if (count != nullptr) {
+        p.subA = subA;
+        p.subBT = subBT;
+        p.jpad = 64;
+        p.jcount = count;
+        p.cols = cols;
+        p.A = A;
+        p.CB = CB;
+        return epi == 1 ? launch_i8<1, 64, true, false, true>(ta, tb, p, stream)
+                        : launch_i8<2, 64, true, false, true>(ta, tb, p, stream);
+    }
+    return epi == 1 ? launch_i8<1, 0, false, false, true>(ta, tb, p, stream)
+                    : launch_i8<2, 0, false, false, true>(ta, tb, p, stream);
 }
 
 } // namespace bnb200

@@ -8,6 +8,7 @@ from .embedding import (  # noqa: F401
 )
 from .modules import (  # noqa: F401
     GroupedLinear4bit,
+    GroupedLinear8bitLt,
     Int8Params,
     Linear4bit,
     Linear8bitLt,

@@ -19,7 +19,7 @@ import torch
 from torch import nn
 
 from .. import functional as F
-from ..autograd._functions import MatmulLtState, grouped_matmul_4bit, matmul, matmul_4bit
+from ..autograd._functions import MatmulLtState, grouped_matmul_4bit, grouped_matmul_8bit, matmul, matmul_4bit
 from ..functional import QuantState
 
 logger = logging.getLogger(__name__)
@@ -431,3 +431,78 @@ class Linear8bitLt(nn.Linear):
         if not self.state.has_fp16_weights and self.state.CB is not None:
             self.weight.data = self.state.CB
         return out
+
+
+class GroupedLinear8bitLt(nn.Module):
+    """The experts of a mixture-of-experts layer on LLM.int8() weights: ``num_experts`` linear maps ``in_features ->
+    out_features`` stored as one ``[E, N, K]`` expert tensor, quantised row-wise as one tensor on the first move to CUDA
+    (as ``Linear8bitLt`` quantises its weight, so expert e's codes and statistics are the ones a ``Linear8bitLt`` of that
+    expert holds), with an optional ``[E, N]`` bias.  ``forward(x, offs)`` takes the expert-sorted rows ``x [M, K]`` and
+    the int32 end row of each expert ``offs [E]`` on the device, and returns ``[M, N]``: every expert in one GEMM
+    launch (:func:`bitsandbytes_b200.grouped_matmul_8bit`), each with its own outlier columns when ``threshold > 0``.
+    The state dict has ``Linear8bitLt``'s keys: ``weight`` (the int8 codes), ``SCB`` and ``weight_format``.  Routing
+    stays with the model."""
+
+    def __init__(self, num_experts, in_features, out_features, bias=False, threshold=0.0, has_fp16_weights=False,
+                 device=None):
+        super().__init__()
+        if has_fp16_weights:
+            raise ValueError("GroupedLinear8bitLt: has_fp16_weights=True is not supported: the expert weights are "
+                             "frozen int8 codes")
+        self.num_experts, self.in_features, self.out_features = num_experts, in_features, out_features
+        self.threshold = threshold
+        w = torch.empty((num_experts, out_features, in_features), device=device)
+        nn.init.kaiming_uniform_(w.view(-1, in_features), a=5**0.5)  # each expert initialised as nn.Linear's weight
+        self.weight = Int8Params(w, requires_grad=False, has_fp16_weights=False)
+        if bias:
+            bound = 1 / in_features**0.5 if in_features > 0 else 0
+            self.bias = nn.Parameter(torch.empty((num_experts, out_features), device=device).uniform_(-bound, bound))
+        else:
+            self.register_parameter("bias", None)
+        self._register_load_state_dict_pre_hook(maybe_rearrange_weight)
+
+    def extra_repr(self) -> str:
+        return (f"num_experts={self.num_experts}, in_features={self.in_features}, out_features={self.out_features}, "
+                f"bias={self.bias is not None}, threshold={self.threshold}")
+
+    def _save_to_state_dict(self, destination, prefix, keep_vars):
+        super()._save_to_state_dict(destination, prefix, keep_vars)
+        scb = getattr(self.weight, "SCB", None)
+        if scb is not None:
+            destination[prefix + "SCB"] = scb if keep_vars else scb.detach()
+            destination[prefix + "weight_format"] = torch.tensor(0, dtype=torch.uint8)
+
+    def _load_from_state_dict(self, state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys,
+                              error_msgs):
+        w, scb = state_dict.get(prefix + "weight"), state_dict.get(prefix + "SCB")
+        if w is None or scb is None or w.dtype != torch.int8:
+            super()._load_from_state_dict(state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys,
+                                          error_msgs)
+            return
+        # quantised codes: they replace the weight whether or not it has been quantised yet (on CPU they move to the
+        # device with the module, as Int8Params does), so a checkpoint loads before or after .cuda()
+        own = (prefix + "weight", prefix + "SCB", prefix + "weight_format")
+        rest = {k: v for k, v in state_dict.items() if k not in own}
+        super()._load_from_state_dict(rest, prefix, local_metadata, strict, missing_keys, unexpected_keys, error_msgs)
+        for keys in (missing_keys, unexpected_keys):
+            keys[:] = [k for k in keys if k not in own]
+        shape = (self.num_experts, self.out_features, self.in_features)
+        if tuple(w.shape) != shape or tuple(scb.shape) != (shape[0] * shape[1],):
+            error_msgs.append(f"size mismatch for {prefix}weight / {prefix}SCB: expected int8 {list(shape)} and "
+                              f"[{shape[0] * shape[1]}], got {list(w.shape)} and {list(scb.shape)}")
+            return
+        dev = self.weight.device
+        CB = w.detach().to(dev, copy=True).contiguous()
+        self.weight = Int8Params(CB, requires_grad=False, has_fp16_weights=False, CB=CB,
+                                 SCB=scb.detach().to(device=dev, dtype=torch.float32, copy=True))
+
+    def forward(self, x: torch.Tensor, offs: torch.Tensor):
+        CB = self.weight.data
+        if CB.dtype != torch.int8:
+            raise RuntimeError("GroupedLinear8bitLt: the weight is not quantised yet: move the module to CUDA first")
+        scb = self.weight.SCB
+        if scb.device != CB.device:  # a module moved after loading codes on the CPU: the statistics follow the codes
+            scb = self.weight.SCB = scb.to(CB.device)
+        if self.bias is not None and self.bias.dtype != x.dtype:
+            self.bias.data = self.bias.data.to(x.dtype)
+        return grouped_matmul_8bit(x, CB, scb, offs, threshold=self.threshold, bias=self.bias)

@@ -292,6 +292,22 @@ void cbnb_b200_int8_outlier_prep_dev(const void* A, int8_t* CA, const int8_t* CB
  * cbnb_b200_int8_scaled_mm).  Returns 0 / 100. */
 int cbnb_b200_int8_mixed_mm_dev(const int8_t* CA, const int8_t* CB, const float* SCA, const float* SCB, const void* bias, const void* A, const void* subA, const void* subBT, const int* cols, const int* count, void* out, int M, int N, int K, int dtype, bnb_stream_t stream);
 
+/* Grouped LLM.int8() GEMM of a mixture-of-experts layer (no reference counterpart).  CB [E * N, K] int8 and SCB [E * N]
+ * are E experts' [N, K] weights quantised row-wise as one tensor; offs[E] (int32, on the device) the expert end rows,
+ * clamped on the device as end_e = min(max(offs[e], end_{e-1}), M).
+ * cbnb_b200_int8_grouped_outliers (threshold > 0): the per-expert outliers, from A (T[M, K]) and A16 (A as fp16, whose
+ * row codes and statistics are CA / SCA): ends[E], flags[E, K], each expert's ascending outlier columns cols[E, K] and
+ * count[E], subA [M, 64] from each row's own expert's list, subBT [E * N, 64] for the experts with rows, and CA zeroed
+ * in each row's expert's outlier columns when the expert has more than one row.  Returns 0 / 1 (bad arguments, message
+ * set).
+ * cbnb_b200_int8_grouped_mm: out[m, :] (row stride N) = cbnb_b200_int8_scaled_mm (count NULL) or
+ * cbnb_b200_int8_mixed_mm_dev (count, cols, subA, subBT and A from cbnb_b200_int8_grouped_outliers) on the rows of expert
+ * e alone, with CB / SCB / bias (T[E * N] or NULL) at e * N; rows past end_{E-1} are +0.  Returns 0; 1 for bad arguments
+ * (message set); 100 with no message for what is not served (K % 16 != 0, E > 1024); 100 with the message set when the
+ * launch fails.  dtype 1 = fp16, 2 = bf16. */
+int cbnb_b200_int8_grouped_outliers(const void* A, const void* A16, int8_t* CA, const int8_t* CB, const float* SCB, const int* offs, int E, float threshold, int* ends, int* flags, int* cols, int* count, void* subA, void* subBT, int M, int N, int K, int dtype, bnb_stream_t stream);
+int cbnb_b200_int8_grouped_mm(const int8_t* CA, const int8_t* CB, const float* SCA, const float* SCB, const void* bias, const int* offs, int E, const void* A, const void* subA, const void* subBT, const int* cols, const int* count, void* out, int M, int N, int K, int dtype, bnb_stream_t stream);
+
 /* Fused row quantisation + outlier-column detection without a host sync:
  * col_flags[c] = 1 if any |A[r,c]| >= threshold.  dtype 1 = fp16, 2 = bf16 (A is read as
  * that type; the reference kernel is fp16-only). */
